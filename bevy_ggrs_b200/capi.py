@@ -44,6 +44,8 @@ BGR_SESSION_NONE, BGR_SESSION_SYNCTEST, BGR_SESSION_P2P, BGR_SESSION_SPECTATOR =
 BGR_CFG_FORCE_STEPWISE = 1
 BGR_CFG_SHARDED = 2
 BGR_CFG_SKIP_UNCHANGED_PLANES = 4
+BGR_CFG_DESYNC_CAPTURE = 8
+BGR_DESYNC_NO_INDEX = 0xFFFFFFFF
 
 
 class bgr_request(C.Structure):
@@ -69,6 +71,21 @@ class bgr_config(C.Structure):
     _fields_ = [("abi_version", C.c_uint32), ("device", C.c_int32), ("max_entities", C.c_uint32),
                 ("max_depth", C.c_uint32), ("fps", C.c_uint32), ("flags", C.c_uint32),
                 ("order_base", C.c_uint64), ("stream", C.c_void_p)]
+
+
+class bgr_desync_column(C.Structure):
+    _fields_ = [("rows", C.c_uint32), ("rows_in_checksum", C.c_uint32), ("presence", C.c_uint32), ("reserved", C.c_uint32)]
+
+
+class bgr_desync_record(C.Structure):
+    _fields_ = [("row", C.c_uint32), ("column", C.c_uint32), ("word", C.c_uint32), ("first", C.c_uint32),
+                ("latest", C.c_uint32)]
+
+
+class bgr_desync_summary(C.Structure):
+    _fields_ = [("frame", C.c_int32), ("rows_first", C.c_uint32), ("rows_latest", C.c_uint32),
+                ("rows_differing", C.c_uint32), ("existence_differing", C.c_uint32), ("host_state_differs", C.c_uint32),
+                ("words_differing", C.c_uint64), ("elapsed_ns_first", C.c_uint64), ("elapsed_ns_latest", C.c_uint64)]
 
 
 u32p = C.POINTER(C.c_uint32)
@@ -110,6 +127,11 @@ PROTOTYPES = {
     "bgr_snapshot_frames": (C.c_int, [C.c_void_p, i32p, C.c_uint32, u32p]),
     "bgr_peek": (C.c_int, [C.c_void_p, C.c_int32, C.c_uint32, C.c_uint32, C.c_uint32, C.c_void_p, C.c_uint32,
                            C.c_void_p, i32p]),
+    "bgr_desync_frames": (C.c_int, [C.c_void_p, i32p, C.c_uint32, u32p]),
+    "bgr_desync_diff": (C.c_int, [C.c_void_p, C.c_int32, C.POINTER(bgr_desync_summary), C.POINTER(bgr_desync_column),
+                                  C.c_uint32, C.POINTER(bgr_desync_record), C.c_uint32, u32p, i32p]),
+    "bgr_peek_first": (C.c_int, [C.c_void_p, C.c_int32, C.c_uint32, C.c_uint32, C.c_uint32, C.c_void_p, C.c_uint32,
+                                 C.c_void_p, i32p]),
     "bgr_save_world": (C.c_int, [C.c_void_p, C.POINTER(bgr_checksum)]),
     "bgr_load_world": (C.c_int, [C.c_void_p]),
     "bgr_advance_world": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint32]),
@@ -150,6 +172,9 @@ PROTOTYPES = {
     "bgr_ring_rollback": (C.c_int, [C.c_void_p, C.c_int32, u32p]),
     "bgr_ring_get": (C.c_int, [C.c_void_p, u32p]),
     "bgr_ring_peek": (C.c_int, [C.c_void_p, C.c_int32, u32p, i32p]),
+    "bgr_ring_create_capture": (C.c_void_p, [C.c_uint32]),
+    "bgr_ring_first": (C.c_int, [C.c_void_p, C.c_int32, u32p, i32p]),
+    "bgr_ring_slots_in_use": (C.c_int, [C.c_void_p, u32p]),
 }
 
 _LIB: Optional[C.CDLL] = None

@@ -26,6 +26,7 @@
 #include "shard_group.hpp"
 #include "tma_copy.cuh"
 #include "generic_program.cuh"
+#include "desync_diff.cuh"
 #include "jit.hpp"
 
 using namespace bgr;
@@ -241,8 +242,17 @@ struct bgr_engine {
     uint32_t tma_stage_tiles = 0;  // one-tile stages of the TMA copy kernel (0: schema too wide for two stages of shared memory)
     unsigned int* d_tma_ticket = nullptr;
     int occ_cache[2][3][3][3] = {};
+    // desync diff scratch (BGR_CFG_DESYNC_CAPTURE), allocated by the first bgr_desync_diff
+    DiffColumn* d_diff_cols = nullptr;
+    unsigned int* d_diff_counts = nullptr;       // [n_cols][3] then the per-tile record counts
+    unsigned long long* d_diff_totals = nullptr;
+    unsigned int* d_diff_list = nullptr;         // [2 * tiles]
+    DiffRecord* d_diff_records = nullptr;
+    size_t diff_records_cap = 0;
 
     uint8_t* image(uint32_t idx) const { return arena + size_t(idx) * image_bytes; }
+    bool capture() const { return cfg.flags & BGR_CFG_DESYNC_CAPTURE; }
+    uint32_t n_slots() const { return capture() ? 2u * cfg.max_depth : cfg.max_depth; }  // frame slots behind the live image
     uint32_t image_off256(uint32_t idx) const { return uint32_t((size_t(idx) * image_bytes) >> 8); }
     uint32_t tiles_for(uint32_t rows) const { return (rows + kTileRows - 1) / kTileRows; }
     uint32_t grid_for(uint32_t n, uint32_t per_block) const {
@@ -1251,6 +1261,11 @@ BGR_API int bgr_engine_create(const bgr_config* cfg, bgr_engine** out) {
     if (cfg->abi_version != BGR_ABI_VERSION) return fail(BGR_ERR_INVALID_ARGUMENT, "ABI version mismatch");
     if (cfg->max_entities == 0 || cfg->fps == 0) return fail(BGR_ERR_INVALID_ARGUMENT, "max_entities and fps must be > 0");
     if (cfg->max_depth == 0 || cfg->max_depth > 64) return fail(BGR_ERR_INVALID_ARGUMENT, "max_depth must be in 1..64");
+    if (cfg->flags & BGR_CFG_DESYNC_CAPTURE) {
+        if (cfg->flags & BGR_CFG_SHARDED) return fail(BGR_ERR_UNSUPPORTED, "BGR_CFG_DESYNC_CAPTURE is not supported on a sharded engine");
+        if (cfg->max_depth > SlotRing::kMaxSlots / 2)
+            return fail(BGR_ERR_INVALID_ARGUMENT, "BGR_CFG_DESYNC_CAPTURE needs max_depth <= 32 (2 * max_depth frame slots)");
+    }
     int n_dev = 0;
     cudaError_t ce = cudaGetDeviceCount(&n_dev);
     if (ce != cudaSuccess || n_dev == 0)
@@ -1324,6 +1339,11 @@ BGR_API void bgr_engine_destroy(bgr_engine* e) {
     if (e->d_tile_done) cudaFree(e->d_tile_done);
     if (e->d_tile_cnt) cudaFree(e->d_tile_cnt);
     if (e->d_item_done) cudaFree(e->d_item_done);
+    if (e->d_diff_cols) cudaFree(e->d_diff_cols);
+    if (e->d_diff_counts) cudaFree(e->d_diff_counts);
+    if (e->d_diff_totals) cudaFree(e->d_diff_totals);
+    if (e->d_diff_list) cudaFree(e->d_diff_list);
+    if (e->d_diff_records) cudaFree(e->d_diff_records);
     for (auto& d : e->dl) {
         if (d.d_buf) cudaFree(d.d_buf);
         if (d.packed) cudaEventDestroy(d.packed);
@@ -1452,9 +1472,9 @@ BGR_API int bgr_build(bgr_engine* e) {
     e->n_tiles_cap = e->epad / kTileRows;
     e->tile_bytes = tile_bytes_of(e->words);
     e->image_bytes = (size_t(e->n_tiles_cap) * e->tile_bytes + 255u) & ~size_t(255);  // ops address images in 256-byte units
-    if ((e->image_bytes * (size_t(e->cfg.max_depth) + 1u)) >> 8 > 0xffffffffull)
+    if ((e->image_bytes * (size_t(e->n_slots()) + 1u)) >> 8 > 0xffffffffull)
         return fail(BGR_ERR_CAPACITY, "arena larger than 1 TB");
-    size_t total = e->image_bytes * (size_t(e->cfg.max_depth) + 1u);
+    size_t total = e->image_bytes * (size_t(e->n_slots()) + 1u);
     CUDA_TRY(cudaMalloc(&e->arena, total));
     CUDA_TRY(cudaMemsetAsync(e->arena, 0, total, e->stream));
     CUDA_TRY(cudaMalloc(&e->d_kill, e->epad));
@@ -1490,7 +1510,7 @@ BGR_API int bgr_build(bgr_engine* e) {
         CUDA_TRY(cudaHostGetDevicePointer(&e->d_out[i], e->h_out[i], 0));
         CUDA_TRY(cudaEventCreateWithFlags(&e->ev[i], cudaEventDisableTiming));
     }
-    e->st.ring.reset(e->cfg.max_depth);
+    e->st.ring.reset(e->n_slots(), e->capture());
     e->st.slot_rows.fill(0);
     e->st.slot_elapsed_ns.fill(0);
     e->st.slot_passive_ver.fill(0);
@@ -1721,6 +1741,138 @@ BGR_API int bgr_peek(bgr_engine* e, int32_t frame, uint32_t column, uint32_t fir
     if (rc != BGR_OK) return rc;
     // alive_dst[i] = the snapshot of `frame` holds this column for row first_row+i (the row existed and had the component)
     if (alive_dst) return read_alive_image(e, slot + 1, first_row, count, e->st.slot_rows[slot], alive_dst, e->cols[column].absent);
+    return BGR_OK;
+}
+
+// ---- desync capture (BGR_CFG_DESYNC_CAPTURE; ring.hpp keeps the witnesses, desync_diff.cuh compares) ----
+static int capture_args(bgr_engine* e) {
+    if (!e || !e->built) return fail(BGR_ERR_STATE, "engine not built");
+    if (!e->capture()) return fail(BGR_ERR_STATE, "the engine was not created with BGR_CFG_DESYNC_CAPTURE");
+    return drain(e);
+}
+
+BGR_API int bgr_desync_frames(bgr_engine* e, int32_t* frames_out, uint32_t cap, uint32_t* n_out) {
+    int rc = capture_args(e);
+    if (rc != BGR_OK) return rc;
+    std::vector<int32_t> f;
+    e->st.ring.desync_frames(&f);
+    for (uint32_t i = 0; i < f.size() && i < cap && frames_out; ++i) frames_out[i] = f[i];
+    if (n_out) *n_out = uint32_t(f.size());
+    return BGR_OK;
+}
+
+BGR_API int bgr_peek_first(bgr_engine* e, int32_t frame, uint32_t column, uint32_t first_row, uint32_t count,
+                           void* host_dst, uint32_t stride, uint8_t* alive_dst, int32_t* found) {
+    if (!found) return fail(BGR_ERR_INVALID_ARGUMENT, "null argument");
+    int rc = capture_args(e);
+    if (rc != BGR_OK) return rc;
+    uint32_t slot = 0;
+    if (!e->st.ring.first(frame, &slot)) { *found = 0; return BGR_OK; }
+    *found = 1;
+    rc = transfer_column(e, slot + 1, column, first_row, count, host_dst, stride, false);
+    if (rc != BGR_OK) return rc;
+    if (alive_dst) return read_alive_image(e, slot + 1, first_row, count, e->st.slot_rows[slot], alive_dst, e->cols[column].absent);
+    return BGR_OK;
+}
+
+BGR_API int bgr_desync_diff(bgr_engine* e, int32_t frame, bgr_desync_summary* summary, bgr_desync_column* cols,
+                            uint32_t cols_cap, bgr_desync_record* records, uint32_t records_cap, uint32_t* n_records,
+                            int32_t* found) {
+    static_assert(sizeof(DiffRecord) == sizeof(bgr_desync_record), "DiffRecord mirrors bgr_desync_record");
+    if (!summary || !found || (!cols && cols_cap) || (!records && records_cap))
+        return fail(BGR_ERR_INVALID_ARGUMENT, "null argument");
+    int rc = capture_args(e);
+    if (rc != BGR_OK) return rc;
+    if (n_records) *n_records = 0;
+    uint32_t sf = 0, sl = 0;
+    if (!e->st.ring.first(frame, &sf) || !e->st.ring.peek(frame, &sl)) { *found = 0; return BGR_OK; }
+    *found = 1;
+    const uint32_t n_cols = uint32_t(e->cols.size());
+    if (!e->d_diff_cols) {
+        std::vector<DiffColumn> dc(n_cols);
+        for (uint32_t c = 0; c < n_cols; ++c) {
+            const Column& k = e->cols[c];
+            const bool ck = k.hash_kind != BGR_HASH_NONE && k.hash_len > 0;
+            dc[c] = DiffColumn{k.first_plane, k.words, k.absent, ck ? k.hash_off : 0u, ck ? k.hash_off + k.hash_len : 0u};
+        }
+        CUDA_TRY(cudaMalloc(&e->d_diff_cols, sizeof(DiffColumn) * std::max(1u, n_cols)));
+        // on the engine's (non-blocking) stream: ordered before the pass-1 launch that reads the table
+        CUDA_TRY(cudaMemcpyAsync(e->d_diff_cols, dc.data(), sizeof(DiffColumn) * n_cols, cudaMemcpyHostToDevice, e->stream));
+        CUDA_TRY(cudaStreamSynchronize(e->stream));  // `dc` is a pageable host vector that goes out of scope below
+        CUDA_TRY(cudaMalloc(&e->d_diff_counts, sizeof(unsigned int) * (3u * n_cols + e->n_tiles_cap)));
+        CUDA_TRY(cudaMalloc(&e->d_diff_totals, sizeof(unsigned long long) * 3u));
+        CUDA_TRY(cudaMalloc(&e->d_diff_list, sizeof(unsigned int) * 2u * e->n_tiles_cap));
+    }
+    if (records_cap > e->diff_records_cap) {
+        if (e->d_diff_records) CUDA_TRY(cudaFree(e->d_diff_records));
+        e->d_diff_records = nullptr; e->diff_records_cap = 0;
+        CUDA_TRY(cudaMalloc(&e->d_diff_records, sizeof(DiffRecord) * records_cap));
+        e->diff_records_cap = records_cap;
+    }
+    DiffParams p{};
+    p.first = e->image(sf + 1);
+    p.latest = e->image(sl + 1);
+    p.words = e->words;
+    p.n_cols = n_cols;
+    p.rows_first = e->st.slot_rows[sf];
+    p.rows_latest = e->st.slot_rows[sl];
+    p.cols = e->d_diff_cols;
+    p.col_counts = e->d_diff_counts;
+    p.totals = e->d_diff_totals;
+    p.tile_records = e->d_diff_counts + 3u * n_cols;
+    p.cap = records_cap;
+    p.out = e->d_diff_records;
+    const uint32_t n_tiles = e->tiles_for(std::max(p.rows_first, p.rows_latest));
+    std::vector<unsigned int> counts(3u * n_cols + n_tiles, 0u);
+    unsigned long long totals[3] = {0, 0, 0};
+    if (n_tiles) {
+        CUDA_TRY(cudaMemsetAsync(e->d_diff_counts, 0, sizeof(unsigned int) * 3u * n_cols, e->stream));
+        CUDA_TRY(cudaMemsetAsync(e->d_diff_totals, 0, sizeof(unsigned long long) * 3u, e->stream));
+        k_desync_count<<<n_tiles, kDiffBlock, 0, e->stream>>>(p);
+        e->launches += 1;
+        CUDA_TRY(cudaGetLastError());
+        CUDA_TRY(cudaMemcpyAsync(counts.data(), e->d_diff_counts, sizeof(unsigned int) * counts.size(), cudaMemcpyDeviceToHost, e->stream));
+        CUDA_TRY(cudaMemcpyAsync(totals, e->d_diff_totals, sizeof totals, cudaMemcpyDeviceToHost, e->stream));
+        CUDA_TRY(cudaStreamSynchronize(e->stream));
+    }
+    // exclusive scan of the tile record counts: the tiles that hold one of the first records_cap records
+    std::vector<unsigned int> list;
+    uint64_t offset = 0;
+    for (uint32_t t = 0; t < n_tiles && offset < records_cap; ++t) {
+        const uint32_t n = counts[3u * n_cols + t];
+        if (n) { list.push_back(t); list.push_back(uint32_t(offset)); }
+        offset += n;
+    }
+    const uint32_t n_list = uint32_t(list.size() / 2);
+    const uint32_t n_out = uint32_t(std::min<uint64_t>(offset, records_cap));
+    if (n_list) {
+        std::vector<unsigned int> packed(2u * n_list);  // [tiles..., bases...]
+        for (uint32_t i = 0; i < n_list; ++i) { packed[i] = list[2 * i]; packed[n_list + i] = list[2 * i + 1]; }
+        CUDA_TRY(cudaMemcpyAsync(e->d_diff_list, packed.data(), sizeof(unsigned int) * packed.size(), cudaMemcpyHostToDevice, e->stream));
+        p.tile_list = e->d_diff_list;
+        p.n_list = n_list;
+        k_desync_records<<<n_list, kDiffBlock, 0, e->stream>>>(p);
+        e->launches += 1;
+        CUDA_TRY(cudaGetLastError());
+        CUDA_TRY(cudaMemcpyAsync(records, e->d_diff_records, sizeof(DiffRecord) * n_out, cudaMemcpyDeviceToHost, e->stream));
+        CUDA_TRY(cudaStreamSynchronize(e->stream));
+    }
+    if (n_records) *n_records = n_out;
+    std::memset(summary, 0, sizeof *summary);
+    summary->frame = frame;
+    summary->rows_first = p.rows_first;
+    summary->rows_latest = p.rows_latest;
+    summary->rows_differing = uint32_t(totals[0]);
+    summary->existence_differing = uint32_t(totals[1]);
+    summary->words_differing = totals[2];
+    summary->host_state_differs = (std::memcmp(&e->st.slot_rng[sf], &e->st.slot_rng[sl], sizeof(ParticleRng)) != 0 ? 1u : 0u) |
+                                  (e->st.slot_elapsed_ns[sf] != e->st.slot_elapsed_ns[sl] ? 2u : 0u);
+    summary->elapsed_ns_first = e->st.slot_elapsed_ns[sf];
+    summary->elapsed_ns_latest = e->st.slot_elapsed_ns[sl];
+    for (uint32_t c = 0; c < cols_cap; ++c) {
+        cols[c] = bgr_desync_column{0, 0, 0, 0};
+        if (c < n_cols) cols[c] = bgr_desync_column{counts[3 * c], counts[3 * c + 1], counts[3 * c + 2], 0};
+    }
     return BGR_OK;
 }
 
@@ -1967,6 +2119,7 @@ BGR_API int bgr_reset_session(bgr_engine* e) {
     e->st.confirmed = -1;         // ConfirmedFrameCount(-1)
     e->st.has_maxpred = true;     // MaxPredictionWindow(8)
     e->st.maxpred = 8;
+    e->st.ring.release_witnesses();  // a new session compares nothing against the old one's first images
     return BGR_OK;
 }
 
@@ -2044,6 +2197,18 @@ BGR_API int bgr_ring_peek(bgr_ring* r, int32_t frame, uint32_t* slot_out, int32_
     bool ok = r->r.peek(frame, &s);
     if (found) *found = ok ? 1 : 0;
     if (ok && slot_out) *slot_out = s;
+    return BGR_OK;
+}
+BGR_API bgr_ring* bgr_ring_create_capture(uint32_t n_slots) { auto* r = new bgr_ring(); r->r.reset(n_slots, true); return r; }
+BGR_API int bgr_ring_first(bgr_ring* r, int32_t frame, uint32_t* slot_out, int32_t* found) {
+    uint32_t s = 0;
+    bool ok = r->r.first(frame, &s);
+    if (found) *found = ok ? 1 : 0;
+    if (ok && slot_out) *slot_out = s;
+    return BGR_OK;
+}
+BGR_API int bgr_ring_slots_in_use(bgr_ring* r, uint32_t* n_out) {
+    if (n_out) *n_out = r->r.slots_in_use();
     return BGR_OK;
 }
 

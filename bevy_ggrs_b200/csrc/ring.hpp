@@ -13,6 +13,22 @@
 // hot path.  All per-type rings of the reference move in lock-step (every SaveWorld pushes
 // the same frame into each of them, every LoadWorld rolls each back to the same frame), so one
 // ring serves every registered column.
+//
+// Desync capture (BGR_CFG_DESYNC_CAPTURE, reset(n, true)): the ring also keeps, per frame, a WITNESS — the slot of the
+// frame's first push since its previous witness was released.  A witness slot is pinned: when the queue drops the
+// entry (rollback, or a push of an older / equal frame) the slot does not go back on the free list, so a re-save of
+// the frame lands in another slot and the first image survives for bgr_desync_diff.  The queue itself (get / peek /
+// frames) is exactly the plain ring's.  A witness is released when
+//   - confirm(c) runs with its frame < c (whether or not the frame is still queued),
+//   - the queue evicts its frame from the OLD end for depth,
+//   - release_witnesses() runs (bgr_reset_session),
+//   - a push finds no free slot: the witness recorded first is released, and so on until a slot is free.
+// Bound: a SyncTest of check distance d (d < max_prediction <= depth) needs at most 2(d+1) slots.  A re-save of frame
+// f inside a rollback confirms only f-d, so while tick `cur` re-saves frame cur-1 the queue holds cur-d-1 .. cur-1
+// (d+1 images) and the witnesses of those d+1 frames sit in other slots.  d+1 <= max_prediction <= max_depth, so the
+// engine's 2*max_depth slots always suffice (tests/test_desync_capture.py walks every d in 1..7, max_prediction in
+// d+1..8 and sees exactly 2(d+1) for d >= 2).  Deeper P2P rollbacks can exceed that; the shortage rule then trades
+// witnesses for slots, so capture never makes a push fail that the plain ring would have served.
 #pragma once
 #include <array>
 #include <cstdint>
@@ -30,10 +46,12 @@ public:
 
     explicit SlotRing(uint32_t n_slots = 0) { reset(n_slots); }
 
-    void reset(uint32_t n_slots) {
+    void reset(uint32_t n_slots, bool capture = false) {
         n_slots_ = n_slots > kMaxSlots ? kMaxSlots : n_slots;
+        capture_ = capture;
         entries_.n = 0;
         free_.n = 0;
+        witnesses_.n = 0;
         for (uint32_t s = n_slots_; s-- > 0;) free_.push_back(s);
         depth_ = 60;  // DEFAULT_FPS until sync_depth runs (mod.rs:112)
     }
@@ -52,16 +70,41 @@ public:
         // the final queue is identical and their slots become reusable for this push
         while (!entries_.empty() && entries_.size() + 1 > depth_) release_front();
         if (depth_ == 0) return kNoSlot - 1;  // pushed and immediately evicted: nothing is stored
+        while (free_.empty() && !witnesses_.empty()) release_witness(0);  // capture only: shortage rule
         if (free_.empty()) return kNoSlot;
         uint32_t s = free_.back();
         free_.pop_back();
         entries_.push_back({frame, s});
+        if (capture_ && find_witness(frame) == kNoSlot) witnesses_.push_back({frame, s});
         return s;
     }
 
     void confirm(int32_t confirmed_frame) {
         while (!entries_.empty() && entries_.front().frame < confirmed_frame) release_front();
+        for (uint32_t i = 0; i < witnesses_.size();) {
+            if (witnesses_[i].frame < confirmed_frame) release_witness(i);
+            else ++i;
+        }
     }
+
+    bool capture() const { return capture_; }
+    void release_witnesses() { while (!witnesses_.empty()) release_witness(0); }
+    // the slot of `frame`'s first-recorded image (capture rings only)
+    bool first(int32_t frame, uint32_t* slot) const {
+        uint32_t i = find_witness(frame);
+        if (i == kNoSlot) return false;
+        *slot = witnesses_[i].slot;
+        return true;
+    }
+    // queued frames whose first-recorded image is a different slot (re-saved since), newest first
+    void desync_frames(std::vector<int32_t>* out) const {
+        out->clear();
+        for (uint32_t i = entries_.size(); i-- > 0;) {
+            uint32_t w = find_witness(entries_[i].frame);
+            if (w != kNoSlot && witnesses_[w].slot != entries_[i].slot) out->push_back(entries_[i].frame);
+        }
+    }
+    uint32_t slots_in_use() const { return n_slots_ - free_.size(); }
 
     // false => the reference would panic; `error` gets the same text
     bool rollback(int32_t frame, std::string* error) {
@@ -126,14 +169,50 @@ private:
         void push_back(const T& v) { a[n++] = v; }
         void pop_back() { --n; }
         void pop_front() { for (uint32_t i = 1; i < n; ++i) a[i - 1] = a[i]; --n; }
+        void erase(uint32_t k) { for (uint32_t i = k + 1; i < n; ++i) a[i - 1] = a[i]; --n; }
     };
-    void release_back() { free_.push_back(entries_.back().slot); entries_.pop_back(); }
-    void release_front() { free_.push_back(entries_.front().slot); entries_.pop_front(); }
+    uint32_t find_witness(int32_t frame) const {
+        for (uint32_t i = 0; i < witnesses_.size(); ++i)
+            if (witnesses_[i].frame == frame) return i;
+        return kNoSlot;
+    }
+    bool pinned(uint32_t slot) const {
+        for (uint32_t i = 0; i < witnesses_.size(); ++i)
+            if (witnesses_[i].slot == slot) return true;
+        return false;
+    }
+    bool queued(uint32_t slot) const {
+        for (uint32_t i = 0; i < entries_.size(); ++i)
+            if (entries_[i].slot == slot) return true;
+        return false;
+    }
+    void release_witness(uint32_t i) {
+        const uint32_t s = witnesses_[i].slot;
+        witnesses_.erase(i);
+        if (!queued(s)) free_.push_back(s);
+    }
+    // dropping from the new end keeps the frame's witness (a SyncTest Load and its re-saves do exactly that)
+    void release_back() {
+        const uint32_t s = entries_.back().slot;
+        entries_.pop_back();
+        if (!pinned(s)) free_.push_back(s);
+    }
+    // dropping from the old end (depth, confirm) releases the frame's witness too
+    void release_front() {
+        const Entry e = entries_.front();
+        entries_.pop_front();
+        const uint32_t w = find_witness(e.frame);
+        if (w != kNoSlot && witnesses_[w].slot != e.slot) release_witness(w);
+        else if (w != kNoSlot) witnesses_.erase(w);  // the witness is this entry's own slot, freed below
+        if (!pinned(e.slot)) free_.push_back(e.slot);
+    }
 
     Small<Entry> entries_;  // oldest first; depth is small (<= 64), O(depth) per operation
     Small<uint32_t> free_;
+    Small<Entry> witnesses_;  // capture rings: (frame, slot of its first-recorded image), in the order recorded
     uint32_t n_slots_ = 0;
     uint32_t depth_ = 60;
+    bool capture_ = false;
 };
 
 }  // namespace bgr

@@ -12,6 +12,7 @@ import numpy as np
 
 from . import capi
 from .capi import BgrError
+from .desync import RECORD_DTYPE, DesyncColumn, DesyncReport
 
 
 class Engine:
@@ -25,6 +26,7 @@ class Engine:
         self._check(self._lib.bgr_engine_create(C.byref(cfg), C.byref(handle)))
         self._h = handle
         self.elem_bytes: List[int] = []
+        self.names: List[str] = []
         self.max_entities = max_entities
         self._pinned: List[C.c_void_p] = []
 
@@ -52,6 +54,7 @@ class Engine:
         col = C.c_uint32()
         self._check(self._lib.bgr_rollback_component(self._h, name.encode(), elem_bytes, strategy, C.byref(col)))
         self.elem_bytes.append(elem_bytes)
+        self.names.append(name)
         return col.value
 
     def checksum_component(self, col: int, byte_offset: int, byte_len: int, flags: int = 0) -> None:
@@ -175,6 +178,41 @@ class Engine:
         found = C.c_int32()
         self._check(self._lib.bgr_peek(self._h, frame, col, first_row, count, out.ctypes.data, eb,
                                        alive.ctypes.data, C.byref(found)))
+        return (out, alive) if found.value else None
+
+    # ---- desync capture (flags=BGR_CFG_DESYNC_CAPTURE) ----
+    def desync_frames(self) -> List[int]:
+        """Frames whose first-recorded snapshot is retained and that were saved again since, newest first."""
+        buf = (C.c_int32 * 128)()
+        n = C.c_uint32()
+        self._check(self._lib.bgr_desync_frames(self._h, buf, 128, C.byref(n)))
+        return [buf[i] for i in range(min(n.value, 128))]
+
+    def desync_diff(self, frame: int, max_records: int = 64) -> Optional[DesyncReport]:
+        """First-recorded vs current snapshot of ``frame`` (bgr_desync_diff); None if either is not held."""
+        s = capi.bgr_desync_summary()
+        cols = (capi.bgr_desync_column * max(1, len(self.elem_bytes)))()
+        recs = np.zeros(max_records, RECORD_DTYPE)
+        n, found = C.c_uint32(), C.c_int32()
+        self._check(self._lib.bgr_desync_diff(self._h, frame, C.byref(s), cols, len(self.elem_bytes),
+                                              recs.ctypes.data_as(C.POINTER(capi.bgr_desync_record)), max_records,
+                                              C.byref(n), C.byref(found)))
+        if not found.value:
+            return None
+        return DesyncReport(s.frame, s.rows_first, s.rows_latest, s.rows_differing, s.existence_differing,
+                            s.words_differing, s.host_state_differs, s.elapsed_ns_first, s.elapsed_ns_latest,
+                            {i: DesyncColumn(i, self.names[i], cols[i].rows, cols[i].rows_in_checksum, cols[i].presence)
+                             for i in range(len(self.elem_bytes))},
+                            recs[: n.value].copy())
+
+    def peek_first(self, frame: int, col: int, first_row: int, count: int) -> Optional[Tuple[np.ndarray, np.ndarray]]:
+        """``peek`` of the first-recorded snapshot of ``frame``."""
+        eb = self.elem_bytes[col]
+        out = np.zeros((count, eb), dtype=np.uint8)
+        alive = np.zeros(count, dtype=np.uint8)
+        found = C.c_int32()
+        self._check(self._lib.bgr_peek_first(self._h, frame, col, first_row, count, out.ctypes.data, eb,
+                                             alive.ctypes.data, C.byref(found)))
         return (out, alive) if found.value else None
 
     # ---- schedules ----

@@ -233,6 +233,33 @@ public:
         return std::vector<int32_t>(f, f + std::min<uint32_t>(n, 128));
     }
 
+    // ---- desync capture (App(..., BGR_CFG_DESYNC_CAPTURE)) ----
+    // Where a SyncTest re-simulation diverged: the frame's first-recorded image against its re-saved one, compared in HBM
+    // (bgr_desync_diff).  Call it from a SyncTestMismatch observer with one of ev.mismatched_frames.  found == false: the
+    // frame has no retained first image or no current snapshot.  An empty report for a mismatched frame means the
+    // difference is in state the engine does not hold (resources, host-side component tables).
+    struct DesyncReport {
+        bool found = false;
+        bgr_desync_summary summary{};
+        std::vector<bgr_desync_column> columns;   // by column index (registration order)
+        std::vector<std::string> column_names;    // typeid names, same index
+        std::vector<bgr_desync_record> records;   // the first max_records, ascending (row, column, word)
+    };
+    DesyncReport desync_report(ggrs::Frame frame, uint32_t max_records = 64) {
+        finish();
+        DesyncReport r;
+        r.columns.resize(pending_cols_.size());
+        r.records.resize(max_records);
+        uint32_t n = 0;
+        int32_t found = 0;
+        check(bgr_desync_diff(engine_, frame, &r.summary, r.columns.data(), uint32_t(r.columns.size()), r.records.data(),
+                              max_records, &n, &found));
+        r.found = found != 0;
+        r.records.resize(n);
+        for (auto& c : pending_cols_) r.column_names.push_back(c.name);
+        return r;
+    }
+
 private:
     template <class T> App& register_component(uint32_t strategy) {
         static_assert(std::is_trivially_copyable<T>::value, "only POD components cross the C ABI");

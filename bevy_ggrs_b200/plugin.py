@@ -226,6 +226,15 @@ class App:
         self._res_checksummed.append(type_name)
         return self
 
+    # ---- desync capture ----
+    def desync_report(self, frame: int, max_records: int = 64):
+        """Where the re-simulation of ``frame`` diverged from its first simulation: a ``DesyncReport`` of the frame's
+        first-recorded snapshot against its re-saved one, or None if the backend no longer holds both.  Meant for a
+        ``SyncTestMismatch`` observer (call it with one of ``ev.mismatched_frames``); the backend must have been created
+        with ``BGR_CFG_DESYNC_CAPTURE``.  Host-side resources and host component tables are not compared: an empty
+        report for a mismatched frame points at them."""
+        return self.world.desync_diff(frame, max_records)
+
     # ---- frame resources ----
     def rollback_frame_count(self) -> int:
         return self.world.rollback_frame_count()

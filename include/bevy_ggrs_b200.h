@@ -173,6 +173,14 @@ typedef struct bgr_config {
  * every observable result is unchanged; only redundant HBM stores are elided.  The reference clones every
  * registered component on every save (component_snapshot.rs:71-75), so the default keeps doing exactly that. */
 #define BGR_CFG_SKIP_UNCHANGED_PLANES 4u
+/* OPT-IN, off by default: keep the first-recorded image of every frame so a SyncTest mismatch can be inspected
+ * (bgr_desync_*, below).  bgr_build allocates 2*max_depth frame slots instead of max_depth; the ring hands a frame's
+ * first slot out again only once the frame is confirmed, evicted from the old end, or bgr_reset_session runs, or when
+ * a Save finds no free slot: then the first images recorded earliest are released until one is free, so capture never
+ * makes a Save fail.  A SyncTest never runs short (it needs at most 2*(check_distance+1) <= 2*max_depth slots); deep
+ * P2P rollbacks can.  Loads, checksums, bgr_peek, bgr_snapshot_frames and the kernels launched are unchanged.  Needs
+ * max_depth <= 32; not with BGR_CFG_SHARDED. */
+#define BGR_CFG_DESYNC_CAPTURE 8u
 
 typedef struct bgr_engine bgr_engine;
 
@@ -254,6 +262,46 @@ BGR_API int bgr_snapshot_frames(bgr_engine* e, int32_t* frames_out, uint32_t cap
 /* peek(frame) (:233-240): *found = 0 if no snapshot for `frame`; otherwise copies the rows. */
 BGR_API int bgr_peek(bgr_engine* e, int32_t frame, uint32_t column, uint32_t first_row, uint32_t count,
                      void* host_dst, uint32_t stride, uint8_t* alive_dst, int32_t* found);
+
+/* ---- desync capture (engines created with BGR_CFG_DESYNC_CAPTURE; BGR_ERR_STATE otherwise) ----------------------
+ * The reference can only say WHICH frames mismatched (SyncTestMismatch, lib.rs:131-137); docs/debugging-desyncs.md
+ * ("Known Limitations") notes the diverging snapshot cannot be inspected.  Here the first-recorded image of a frame
+ * ("first", what ggrs compared against) and its current ring image ("latest", the re-simulation) are compared in HBM
+ * with the keyed-map semantics of component_snapshot.rs:99-115:
+ *   - row r exists in an image iff r < that image's RollbackOrdered::len() and the entity was alive;
+ *   - existence difference: the row exists in exactly one image (record: column = word = 0xFFFFFFFF);
+ *   - presence difference: exists in both, an optional column's absent bit differs (record: word = 0xFFFFFFFF);
+ *   - word difference: exists in both, column present in both, a 4-byte word of the element differs.
+ * Existence / presence records carry the two per-row mask bytes (bit 0 alive, bit 1+k optional column k absent;
+ * 0 for a row that does not exist) in first / latest; word records carry the two words.  Records come in ascending
+ * (row, column, word) order; only the first records_cap are returned.  Like every entry point that reads the world,
+ * these wait for submitted vectors and leave their results queued for bgr_collect. */
+#define BGR_DESYNC_NO_INDEX 0xFFFFFFFFu
+typedef struct bgr_desync_column {
+    uint32_t rows;              /* rows with a word difference in this column */
+    uint32_t rows_in_checksum;  /* ... of which a differing word overlaps the column's checksummed byte range */
+    uint32_t presence;          /* rows with a presence difference in this column */
+    uint32_t reserved;
+} bgr_desync_column;
+typedef struct bgr_desync_record { uint32_t row, column, word, first, latest; } bgr_desync_record;
+typedef struct bgr_desync_summary {
+    int32_t frame;
+    uint32_t rows_first, rows_latest;                 /* RollbackOrdered::len() captured by each image */
+    uint32_t rows_differing, existence_differing;     /* rows with any difference; rows that exist in one image only */
+    uint32_t host_state_differs;                      /* bit 0 ParticleRng, bit 1 Time<GgrsTime> */
+    uint64_t words_differing;                         /* differing words over all rows and columns */
+    uint64_t elapsed_ns_first, elapsed_ns_latest;     /* Time<GgrsTime>::elapsed captured by each image */
+} bgr_desync_summary;
+/* frames that have a first-recorded image AND a later save into a different slot, newest first */
+BGR_API int bgr_desync_frames(bgr_engine* e, int32_t* frames_out, uint32_t cap, uint32_t* n_out);
+/* *found = 0 when `frame` lacks a retained first image or a current ring entry.  cols[c] for c < cols_cap;
+ * *n_records = records written (<= records_cap). */
+BGR_API int bgr_desync_diff(bgr_engine* e, int32_t frame, bgr_desync_summary* summary, bgr_desync_column* cols,
+                            uint32_t cols_cap, bgr_desync_record* records, uint32_t records_cap, uint32_t* n_records,
+                            int32_t* found);
+/* bgr_peek, but of the first-recorded image of `frame` */
+BGR_API int bgr_peek_first(bgr_engine* e, int32_t frame, uint32_t column, uint32_t first_row, uint32_t count,
+                           void* host_dst, uint32_t stride, uint8_t* alive_dst, int32_t* found);
 
 /* ---- the three schedules, one at a time (SnapshotPlugin-only users: benches/bench.rs:18-27,
  *      mod.rs:510-535 save_world / advance_frame / load_world helpers) -------------------- */
@@ -357,6 +405,10 @@ BGR_API int bgr_ring_confirm(bgr_ring* r, int32_t frame);
 BGR_API int bgr_ring_rollback(bgr_ring* r, int32_t frame, uint32_t* slot_out);
 BGR_API int bgr_ring_get(bgr_ring* r, uint32_t* slot_out);
 BGR_API int bgr_ring_peek(bgr_ring* r, int32_t frame, uint32_t* slot_out, int32_t* found);
+/* the same ring with desync capture (BGR_CFG_DESYNC_CAPTURE): first(frame) = slot of the frame's retained first image */
+BGR_API bgr_ring* bgr_ring_create_capture(uint32_t n_slots);
+BGR_API int bgr_ring_first(bgr_ring* r, int32_t frame, uint32_t* slot_out, int32_t* found);
+BGR_API int bgr_ring_slots_in_use(bgr_ring* r, uint32_t* n_out);  /* queued or pinned slots */
 
 #ifdef __cplusplus
 }

@@ -61,10 +61,11 @@ use bevy_ggrs::{
 // ------------------------------------------------------------------------------------------------------------------
 // engine handle + status -> panic
 // ------------------------------------------------------------------------------------------------------------------
-/// Where the rollback columns live.  Insert before `GgrsPlugin`; defaults: 1M entities, 9 frame slots, device 0.
+/// Where the rollback columns live.  Insert before `GgrsPlugin`; defaults: 1M entities, 9 frame slots, device 0, no
+/// desync capture (`desync_capture: true` keeps every frame's first snapshot for [`desync_report`]; max_depth <= 32).
 #[derive(Resource, Clone, Copy)]
-pub struct B200Config { pub max_entities: u32, pub max_depth: u32, pub device: i32 }
-impl Default for B200Config { fn default() -> Self { Self { max_entities: 1 << 20, max_depth: 9, device: 0 } } }
+pub struct B200Config { pub max_entities: u32, pub max_depth: u32, pub device: i32, pub desync_capture: bool }
+impl Default for B200Config { fn default() -> Self { Self { max_entities: 1 << 20, max_depth: 9, device: 0, desync_capture: false } } }
 
 /// The engine handle, a non-send resource (one caller thread, like the exclusive system that owns the World,
 /// schedule_systems.rs:19,170).
@@ -104,6 +105,24 @@ struct Columns { by_type: HashMap<TypeId, u32>, bytes: HashMap<TypeId, u32>, mir
 struct Rows { entity_of_row: Vec<Entity>, row_of: HashMap<Entity, u32>, uploaded: u32 }
 
 fn engine(world: &World) -> *mut sys::bgr_engine { world.non_send_resource::<B200Engine>().raw }
+
+/// Where the re-simulation of `frame` diverged from its first simulation (`B200Config { desync_capture: true, .. }`):
+/// call it from a `SyncTestMismatch` observer with one of `mismatched_frames`.  `None` when the engine no longer holds
+/// both snapshots of the frame.  Returns the summary, per-column counts (registration order) and the first
+/// `max_records` differences in (row, column, word) order; rows are RollbackOrdered indices.  A report without any
+/// difference means the mismatch came from state outside the engine (resources, non-POD components).
+pub fn desync_report(world: &World, frame: i32, max_records: u32)
+    -> Option<(sys::bgr_desync_summary, Vec<sys::bgr_desync_column>, Vec<sys::bgr_desync_record>)> {
+    let e = engine(world);
+    let n_cols = world.get_resource::<Columns>().map(|c| c.by_type.len()).unwrap_or(0);
+    let mut summary = sys::bgr_desync_summary::default();
+    let mut cols = vec![sys::bgr_desync_column::default(); n_cols];
+    let mut recs = vec![sys::bgr_desync_record::default(); max_records as usize];
+    let (mut n, mut found) = (0u32, 0i32);
+    check(unsafe { sys::bgr_desync_diff(e, frame, &mut summary, cols.as_mut_ptr(), n_cols as u32, recs.as_mut_ptr(), max_records, &mut n, &mut found) });
+    recs.truncate(n as usize);
+    (found != 0).then_some((summary, cols, recs))
+}
 
 // ------------------------------------------------------------------------------------------------------------------
 // RollbackApp — the reference's trait, same method names and signatures (rollback_app.rs:31-133, :135-248)
@@ -187,7 +206,7 @@ impl<C: Config<Input = u8>> Plugin for GgrsPlugin<C> {
         let cfg = app.world().get_resource::<B200Config>().copied().unwrap_or_default();
         let fps = app.world().get_resource::<RollbackFrameRate>().map(|r| **r as u32).unwrap_or(60);
         let c = sys::bgr_config { abi_version: sys::BGR_ABI_VERSION, device: cfg.device, max_entities: cfg.max_entities, max_depth: cfg.max_depth,
-                                  fps, flags: 0, order_base: 0, stream: core::ptr::null_mut() };
+                                  fps, flags: if cfg.desync_capture { sys::BGR_CFG_DESYNC_CAPTURE } else { 0 }, order_base: 0, stream: core::ptr::null_mut() };
         let mut raw = core::ptr::null_mut();
         check(unsafe { sys::bgr_engine_create(&c, &mut raw) });
         app.insert_non_send_resource(B200Engine { raw, built: false })

@@ -39,6 +39,12 @@ pub const BGR_SESSION_SPECTATOR: u32 = 3;
 pub const BGR_CFG_FORCE_STEPWISE: u32 = 1;
 pub const BGR_CFG_SHARDED: u32 = 2;
 pub const BGR_CFG_SKIP_UNCHANGED_PLANES: u32 = 4;
+pub const BGR_CFG_DESYNC_CAPTURE: u32 = 8;
+pub const BGR_DESYNC_NO_INDEX: u32 = 0xFFFFFFFF;
+
+// the desync capture structs (bgr_desync_column / _record / _summary) live in their own module
+mod desync;
+pub use desync::*;
 
 #[repr(C)]
 #[derive(Clone, Copy, Default)]
@@ -126,6 +132,9 @@ extern "C" {
     pub fn bgr_confirm(e: *mut bgr_engine, confirmed_frame: i32) -> c_int;
     pub fn bgr_snapshot_frames(e: *mut bgr_engine, frames_out: *mut i32, cap: u32, n_out: *mut u32) -> c_int;
     pub fn bgr_peek(e: *mut bgr_engine, frame: i32, column: u32, first_row: u32, count: u32, host_dst: *mut c_void, stride: u32, alive_dst: *mut u8, found: *mut i32) -> c_int;
+    pub fn bgr_desync_frames(e: *mut bgr_engine, frames_out: *mut i32, cap: u32, n_out: *mut u32) -> c_int;
+    pub fn bgr_desync_diff(e: *mut bgr_engine, frame: i32, summary: *mut bgr_desync_summary, cols: *mut bgr_desync_column, cols_cap: u32, records: *mut bgr_desync_record, records_cap: u32, n_records: *mut u32, found: *mut i32) -> c_int;
+    pub fn bgr_peek_first(e: *mut bgr_engine, frame: i32, column: u32, first_row: u32, count: u32, host_dst: *mut c_void, stride: u32, alive_dst: *mut u8, found: *mut i32) -> c_int;
     pub fn bgr_save_world(e: *mut bgr_engine, checksum_out: *mut bgr_checksum) -> c_int;
     pub fn bgr_load_world(e: *mut bgr_engine) -> c_int;
     pub fn bgr_advance_world(e: *mut bgr_engine, inputs: *const u8, status: *const u8, n_players: u32) -> c_int;
