@@ -46,6 +46,9 @@ BGR_CFG_SHARDED = 2
 BGR_CFG_SKIP_UNCHANGED_PLANES = 4
 BGR_CFG_DESYNC_CAPTURE = 8
 BGR_DESYNC_NO_INDEX = 0xFFFFFFFF
+# bgr_last_kernel: kind in bits 0-3
+BGR_KERNEL_NONE, BGR_KERNEL_STEPWISE_TMA, BGR_KERNEL_STEPWISE_FLAT, BGR_KERNEL_BUNDLE, \
+    BGR_KERNEL_GENERIC_INTERPRETER, BGR_KERNEL_GENERIC_NVRTC = range(6)
 
 
 class bgr_request(C.Structure):
@@ -151,6 +154,7 @@ PROTOTYPES = {
     "bgr_slot_bytes": (C.c_int, [C.c_void_p, u64p]),
     "bgr_last_path": (C.c_int, [C.c_void_p, u32p]),
     "bgr_generic_specialised": (C.c_int, [C.c_void_p, u32p]),
+    "bgr_last_kernel": (C.c_int, [C.c_void_p, u32p]),
     "bgr_synchronize": (C.c_int, [C.c_void_p]),
     "bgr_stream": (C.c_int, [C.c_void_p, C.POINTER(C.c_void_p)]),
     "bgr_trace_enable": (C.c_int, [C.c_void_p, C.c_uint32]),

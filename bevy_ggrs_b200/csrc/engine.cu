@@ -200,6 +200,7 @@ struct bgr_engine {
     uint64_t launches = 0;
     uint64_t prof[8] = {};          // host-side time of the hot loop: [0] calls, [1] compile ns, [2] launch ns, [3] wait ns, [4] fold ns
     bool last_fused = false;
+    uint32_t last_kernel = BGR_KERNEL_NONE;  // bgr_last_kernel: what the last request vector ran
     unsigned long long seq = 0;   // sequence number of the last submit (completion flag value)
     int tune_poll = 1;            // collect() spins on the host-mapped flag before falling back to the event
     int tune_tiledep = 1;         // consecutive fused launches overlap: per-tile dependencies instead of grid-level (PF_TILE_WAIT)
@@ -241,7 +242,7 @@ struct bgr_engine {
     int tune_tma = 1;          // stepwise Save/Load through the TMA-staged bulk-copy kernel
     uint32_t tma_stage_tiles = 0;  // one-tile stages of the TMA copy kernel (0: schema too wide for two stages of shared memory)
     unsigned int* d_tma_ticket = nullptr;
-    int occ_cache[2][3][3][3] = {};
+    int occ_cache[2][2][3][3][3] = {};  // [passive TMA][sub-tile items][VEC][MODE][launch-bounds tier]: blocks per SM
     // desync diff scratch (BGR_CFG_DESYNC_CAPTURE), allocated by the first bgr_desync_diff
     DiffColumn* d_diff_cols = nullptr;
     unsigned int* d_diff_counts = nullptr;       // [n_cols][3] then the per-tile record counts
@@ -422,14 +423,19 @@ int launch_particles(bgr_engine* e, const ProgramParams& pp, int vi, int si, int
     constexpr int BLOCK = SUB / VEC;
     constexpr uint32_t kSubs = kTileRows / SUB;
     constexpr int ui = kSubs > 1 ? 1 : 0;
-    const size_t smem = (pp.flags & PF_PASSIVE_TMA) ? size_t(2) * pp.passive_bytes : 0;
-    if (e->occ_cache[ui][vi][si][mi] == 0) {
+    const int ti = (pp.flags & PF_PASSIVE_TMA) ? 1 : 0;
+    const size_t smem = ti ? size_t(2) * pp.passive_bytes : 0;
+    // A variant runs with and without the passive double buffer (spawns and multi-Load vectors move passive planes
+    // per thread): the shared-memory opt-in and the occupancy are per (variant, buffer).  passive_bytes is fixed at
+    // bgr_build for a given variant, so one entry per buffer setting is exact.
+    int& occ = e->occ_cache[ti][ui][vi][si][mi];
+    if (occ == 0) {
         if (smem > 48 * 1024) CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem)));
         int nb = 0;
         CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, kern, BLOCK, smem));
-        e->occ_cache[ui][vi][si][mi] = std::max(1, nb);
+        occ = std::max(1, nb);
     }
-    int bps = e->occ_cache[ui][vi][si][mi];
+    int bps = occ;
     if (e->tune_bps > 0) bps = std::min(e->tune_bps, bps);
     uint32_t grid = std::max(1u, std::min((pp.n_tiles - pp.tile_begin) * kSubs, uint32_t(e->num_sms * bps)));
     if (e->tune_grid > 0) grid = std::min(grid, uint32_t(e->tune_grid));
@@ -444,6 +450,9 @@ int launch_particles(bgr_engine* e, const ProgramParams& pp, int vi, int si, int
     CUDA_TRY(cudaLaunchKernelEx(&lc, kern, pp));
     CUDA_TRY(cudaGetLastError());
     e->launches += 1;
+    const bool tma = ti && (kSubs == 1 ? pp.n_runs : pp.n_passive) > 0;  // the kernel's `use_tma`
+    e->last_kernel = BGR_KERNEL_BUNDLE | (uint32_t(VEC) << 4) | (uint32_t(MODE) << 8) | (uint32_t(mi) << 10) |
+                     (tma ? 1u << 12 : 0u) | (uint32_t(SUB) << 16);
     return BGR_OK;
 }
 
@@ -753,6 +762,7 @@ int run_stepwise(bgr_engine* e, const Program& pg, uint32_t buf) {
     k_publish<<<1, 128, 0, e->stream>>>(e->d_accum, e->d_out[buf], std::max(1u, pg.n_saves) * kAccStride, e->seq);
     e->launches += 1;
     CUDA_TRY(cudaGetLastError());
+    e->last_kernel = (e->tune_tma && e->tma_stage_tiles) ? BGR_KERNEL_STEPWISE_TMA : BGR_KERNEL_STEPWISE_FLAT;
     return BGR_OK;
 }
 
@@ -896,6 +906,7 @@ int run_generic(bgr_engine* e, const Program& pg, uint32_t buf) {
         CUDA_TRY(cudaLaunchKernelExC(&cfg, k.fn, args));
         CUDA_TRY(cudaGetLastError());
         e->launches += 1;
+        e->last_kernel = BGR_KERNEL_GENERIC_NVRTC | (uint32_t(k.item_rows) << 16);
         e->tiledep_chain = tiledep;
         e->tiledep_seq = uint32_t(e->seq); e->tiledep_tiles = n_items; e->jit_chain_kernel = k.fn;
         return BGR_OK;
@@ -919,6 +930,7 @@ int run_generic(bgr_engine* e, const Program& pg, uint32_t buf) {
     CUDA_TRY(cudaLaunchKernel(fn, dim3(grid), dim3(block), args, smem, e->stream));
     CUDA_TRY(cudaGetLastError());
     e->launches += 1;
+    e->last_kernel = BGR_KERNEL_GENERIC_INTERPRETER;
     return BGR_OK;
 }
 
@@ -2016,6 +2028,10 @@ BGR_API int bgr_generic_specialised(bgr_engine* e, uint32_t* specialised_out) {
 BGR_API int bgr_last_path(bgr_engine* e, uint32_t* fused_out) {
     if (!e || !fused_out) return fail(BGR_ERR_INVALID_ARGUMENT, "null argument");
     *fused_out = e->last_fused ? 1u : 0u; return BGR_OK;
+}
+BGR_API int bgr_last_kernel(bgr_engine* e, uint32_t* kernel_out) {
+    if (!e || !kernel_out) return fail(BGR_ERR_INVALID_ARGUMENT, "null argument");
+    *kernel_out = e->last_kernel; return BGR_OK;
 }
 BGR_API int bgr_synchronize(bgr_engine* e) {
     if (!e) return fail(BGR_ERR_INVALID_ARGUMENT, "null engine");

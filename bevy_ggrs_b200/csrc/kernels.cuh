@@ -689,7 +689,8 @@ __global__ void __launch_bounds__(SUB / VEC, MINB) k_particles_program(const __g
 #ifndef __CUDACC_RTC__  // the run-time specialisation (generic_program_jit.cuh) only needs the structs and helpers
 
 // flat copy of tiles [0, n_tiles) of an image (fallback when the TMA kernel cannot be used);
-// alive bytes of rows >= n_rows_src are forced to 0 (a Load that shrinks the world).
+// mask bytes of rows >= n_rows_src are forced to 0 (a Load that shrinks the world); the others are copied whole, with
+// the absent bits of the optional columns.
 __global__ void __launch_bounds__(256) k_copy_image(const uint8_t* __restrict__ src, uint8_t* __restrict__ dst,
                                                     uint32_t words, uint32_t n_tiles, uint32_t n_rows_src) {
     const uint32_t tb = tile_bytes_of(words);
@@ -702,7 +703,7 @@ __global__ void __launch_bounds__(256) k_copy_image(const uint8_t* __restrict__ 
             const uint32_t r0 = tile * kTileRows + (in_tile - words * kPlaneBytes);
             uint32_t* w = reinterpret_cast<uint32_t*>(&x);
 #pragma unroll
-            for (int k = 0; k < 4; ++k) w[k] &= rows_mask<4>(r0 + 4 * k, n_rows_src);
+            for (int k = 0; k < 4; ++k) w[k] &= rows_mask_full<4>(r0 + 4 * k, n_rows_src);
         }
         __stcs(reinterpret_cast<uint4*>(dst) + v, x);
     }

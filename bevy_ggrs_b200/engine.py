@@ -6,13 +6,35 @@ re-simulation all happen in the CUDA library.
 from __future__ import annotations
 
 import ctypes as C
-from typing import List, Optional, Sequence, Tuple
+from typing import List, NamedTuple, Optional, Sequence, Tuple
 
 import numpy as np
 
 from . import capi
 from .capi import BgrError
 from .desync import RECORD_DTYPE, DesyncColumn, DesyncReport
+
+
+_KERNEL_KINDS = {capi.BGR_KERNEL_NONE: "none", capi.BGR_KERNEL_STEPWISE_TMA: "stepwise_tma",
+                 capi.BGR_KERNEL_STEPWISE_FLAT: "stepwise_flat", capi.BGR_KERNEL_BUNDLE: "bundle",
+                 capi.BGR_KERNEL_GENERIC_INTERPRETER: "generic_interpreter", capi.BGR_KERNEL_GENERIC_NVRTC: "generic_nvrtc"}
+
+
+class LastKernel(NamedTuple):
+    """bgr_last_kernel decoded.  vec / mode / tier / passive_tma describe the bundle kernel (0 / False otherwise);
+    item_rows is set for the bundle and the NVRTC kernel.  tier: 0 unconstrained, 1 768 and 2 1024 threads per SM."""
+    kind: str
+    vec: int
+    mode: int
+    tier: int
+    passive_tma: bool
+    item_rows: int
+    raw: int
+
+    @staticmethod
+    def decode(v: int) -> "LastKernel":
+        return LastKernel(_KERNEL_KINDS.get(v & 0xF, f"unknown({v & 0xF})"), (v >> 4) & 0xF, (v >> 8) & 0x3,
+                          (v >> 10) & 0x3, bool((v >> 12) & 1), (v >> 16) & 0x3FF, v)
 
 
 class Engine:
@@ -284,6 +306,12 @@ class Engine:
         v = C.c_uint32()
         self._check(self._lib.bgr_generic_specialised(self._h, C.byref(v)))
         return bool(v.value)
+
+    def last_kernel(self) -> "LastKernel":
+        """What the last request vector executed (bgr_last_kernel), decoded."""
+        v = C.c_uint32()
+        self._check(self._lib.bgr_last_kernel(self._h, C.byref(v)))
+        return LastKernel.decode(v.value)
 
     def synchronize(self) -> None:
         self._check(self._lib.bgr_synchronize(self._h))

@@ -17,15 +17,20 @@ TRANSFORM_BYTES, VELOCITY_BYTES, TTL_BYTES = 40, 12, 8
 SLOT_BYTES_PER_ENTITY = TRANSFORM_BYTES + VELOCITY_BYTES + TTL_BYTES + 1  # + alive byte
 
 
-def register_particles(world, spawn_rate: int = 0, spawn_ttl: int = 300, rng_seed: int = 123):
+def register_particles(world, spawn_rate: int = 0, spawn_ttl: int = 300, rng_seed: int = 123, checksums=None):
     """Same registration sequence as the example's main() on any Engine-shaped backend.
     spawn_rate > 0 also registers spawn_particles.run_if(spawn_pressed) with ParticleRng(seed_from_u64(rng_seed))
-    (particles.rs:233-243; `--rate`, ttl = fps * 5)."""
+    (particles.rs:233-243; `--rate`, ttl = fps * 5).
+    checksums(world, transform, velocity) replaces the example's two checksum registrations (other setups of the
+    same world: one column, none, no finite assertion)."""
     t = world.rollback_component("Transform", TRANSFORM_BYTES, capi.BGR_STRATEGY_CLONE)
     v = world.rollback_component("Velocity", VELOCITY_BYTES, capi.BGR_STRATEGY_COPY)
     l = world.rollback_component("Ttl", TTL_BYTES, capi.BGR_STRATEGY_COPY)
-    world.checksum_component(v, 0, 12, capi.BGR_HASH_FLAG_ASSERT_FINITE_F32)   # checksum_component_with_hash::<Velocity>()
-    world.checksum_component(t, 0, 12, capi.BGR_HASH_FLAG_ASSERT_FINITE_F32)   # checksum_component::<Transform>(translation bits)
+    if checksums is not None:
+        checksums(world, t, v)
+    else:
+        world.checksum_component(v, 0, 12, capi.BGR_HASH_FLAG_ASSERT_FINITE_F32)   # checksum_component_with_hash::<Velocity>()
+        world.checksum_component(t, 0, 12, capi.BGR_HASH_FLAG_ASSERT_FINITE_F32)   # checksum_component::<Transform>(translation bits)
     if spawn_rate:
         world.add_system(capi.BGR_SYS_PARTICLES_SPAWN, [t, v, l],
                          [spawn_rate, spawn_ttl, rng_seed & 0xFFFFFFFF, (rng_seed >> 32) & 0xFFFFFFFF])

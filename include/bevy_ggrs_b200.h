@@ -380,6 +380,22 @@ BGR_API int bgr_last_path(bgr_engine* e, uint32_t* fused_out);   /* 1 if the las
  * csrc/generic_program_jit.cuh): every non-bundle request vector then runs on it; 0 = the interpreter kernel (same results).
  * Env BGR_TUNE_JIT: 0 never, 1 (default) engines created for >= 16384 entities, 2 always. */
 BGR_API int bgr_generic_specialised(bgr_engine* e, uint32_t* specialised_out);
+/* Which kernel the last request vector executed (0 before the first one).  Tuning knobs fall back quietly (an optional
+ * column forces VEC 2, BGR_TUNE_SUB=128 needs VEC 2 ...): this says what actually ran.
+ *   bits 0-3   kind: BGR_KERNEL_*
+ *   bits 4-7   bundle: rows per thread (VEC: 1, 2 or 4)
+ *   bits 8-9   bundle: MODE 0 (checksum flags tested at run time), 1 (Transform and Velocity both checksummed with
+ *              BGR_HASH_FLAG_ASSERT_FINITE_F32: specialised), 2 (per-entity presence of optional columns)
+ *   bits 10-11 bundle: launch-bounds tier, 0 unconstrained, 1 768 threads per SM, 2 1024 threads per SM
+ *   bit 12     bundle: passive planes moved by TMA bulk copies
+ *   bits 16-25 bundle and generic NVRTC: rows per work item (512 = a whole tile) */
+#define BGR_KERNEL_NONE 0u
+#define BGR_KERNEL_STEPWISE_TMA 1u       /* one kernel per request; Save / Load through the TMA-staged copy kernel */
+#define BGR_KERNEL_STEPWISE_FLAT 2u      /* one kernel per request; k_checksum_column + k_copy_image */
+#define BGR_KERNEL_BUNDLE 3u             /* the compiled particles kernel (k_particles_program) */
+#define BGR_KERNEL_GENERIC_INTERPRETER 4u
+#define BGR_KERNEL_GENERIC_NVRTC 5u
+BGR_API int bgr_last_kernel(bgr_engine* e, uint32_t* kernel_out);
 BGR_API int bgr_synchronize(bgr_engine* e);
 BGR_API int bgr_stream(bgr_engine* e, void** stream_out);        /* the cudaStream_t the engine launches on (timing events) */
 /* device-side launch trace: 4 x u64 per fused launch after the call, up to `capacity` launches (GPU globaltimer ns):

@@ -36,6 +36,13 @@ pub const BGR_SESSION_SYNCTEST: u32 = 1;
 pub const BGR_SESSION_P2P: u32 = 2;
 pub const BGR_SESSION_SPECTATOR: u32 = 3;
 
+pub const BGR_KERNEL_NONE: u32 = 0;
+pub const BGR_KERNEL_STEPWISE_TMA: u32 = 1;
+pub const BGR_KERNEL_STEPWISE_FLAT: u32 = 2;
+pub const BGR_KERNEL_BUNDLE: u32 = 3;
+pub const BGR_KERNEL_GENERIC_INTERPRETER: u32 = 4;
+pub const BGR_KERNEL_GENERIC_NVRTC: u32 = 5;
+
 pub const BGR_CFG_FORCE_STEPWISE: u32 = 1;
 pub const BGR_CFG_SHARDED: u32 = 2;
 pub const BGR_CFG_SKIP_UNCHANGED_PLANES: u32 = 4;
@@ -153,6 +160,7 @@ extern "C" {
     pub fn bgr_slot_bytes(e: *mut bgr_engine, bytes_out: *mut u64) -> c_int;
     pub fn bgr_last_path(e: *mut bgr_engine, fused_out: *mut u32) -> c_int;
     pub fn bgr_generic_specialised(e: *mut bgr_engine, specialised_out: *mut u32) -> c_int;
+    pub fn bgr_last_kernel(e: *mut bgr_engine, kernel_out: *mut u32) -> c_int;
     pub fn bgr_synchronize(e: *mut bgr_engine) -> c_int;
     pub fn bgr_stream(e: *mut bgr_engine, stream_out: *mut *mut c_void) -> c_int;
     pub fn bgr_trace_enable(e: *mut bgr_engine, capacity: u32) -> c_int;

@@ -19,7 +19,7 @@ def input_system(app):
 
 
 def make_particles_app(backend, n_entities, seed, session, ttl_lo, ttl_hi, noop_inputs=False, spawn_rate=0,
-                       spawn_ttl=300, startup_burst=False, z_fraction=0.0):
+                       spawn_ttl=300, startup_burst=False, z_fraction=0.0, checksums=None):
     app = App(backend)
     app.add_plugins(GgrsPlugin())
     app.insert_resource(RollbackFrameRate(60))
@@ -38,7 +38,7 @@ def make_particles_app(backend, n_entities, seed, session, ttl_lo, ttl_hi, noop_
         app.add_systems(ReadInputs, read)
     else:
         app.add_systems(ReadInputs, input_system)
-    cols = register_particles(backend, spawn_rate=spawn_rate, spawn_ttl=spawn_ttl)
+    cols = register_particles(backend, spawn_rate=spawn_rate, spawn_ttl=spawn_ttl, checksums=checksums)
     app.insert_resource(session)
     mism = []
     app.add_observer(SyncTestMismatch, lambda ev: mism.append(ev))
@@ -66,8 +66,9 @@ def compare_state(eng, orc, cols, n):
 
 def run_particles_synctest_pair(n_entities, check_distance, ticks, seed, max_prediction=None, ttl_lo=None,
                                 ttl_hi=None, flags=0, tune=None, spawn_rate=0, spawn_ttl=300, startup_burst=False,
-                                peek_check=False, z_fraction=0.0):
-    """SyncTest on the GPU engine and on the oracle with identical inputs; returns comparison facts."""
+                                peek_check=False, z_fraction=0.0, checksums=None):
+    """SyncTest on the GPU engine and on the oracle with identical inputs; returns comparison facts.
+    checksums(world, transform, velocity): the checksum registration (default: the example's, see register_particles)."""
     maxp = max_prediction or max(8, check_distance + 1)
     ttl_lo = ttl_lo if ttl_lo is not None else 300 + check_distance
     ttl_hi = ttl_hi if ttl_hi is not None else ttl_lo
@@ -76,10 +77,12 @@ def run_particles_synctest_pair(n_entities, check_distance, ticks, seed, max_pre
     orc = OracleWorld(fps=60)
     app_e, cols_e, mism_e = make_particles_app(eng, n_entities, seed, Session.SyncTest(
         SyncTestSession(2, check_distance, maxp, input_delay=2)), ttl_lo, ttl_hi, noop_inputs=True,
-        spawn_rate=spawn_rate, spawn_ttl=spawn_ttl, startup_burst=startup_burst, z_fraction=z_fraction)
+        spawn_rate=spawn_rate, spawn_ttl=spawn_ttl, startup_burst=startup_burst, z_fraction=z_fraction,
+        checksums=checksums)
     app_o, cols_o, mism_o = make_particles_app(orc, n_entities, seed, Session.SyncTest(
         SyncTestSession(2, check_distance, maxp, input_delay=2)), ttl_lo, ttl_hi, noop_inputs=True,
-        spawn_rate=spawn_rate, spawn_ttl=spawn_ttl, startup_burst=startup_burst, z_fraction=z_fraction)
+        spawn_rate=spawn_rate, spawn_ttl=spawn_ttl, startup_burst=startup_burst, z_fraction=z_fraction,
+        checksums=checksums)
     all_e, all_o = [], []
     launches0 = eng.launch_count()
     for _ in range(ticks):
@@ -89,6 +92,7 @@ def run_particles_synctest_pair(n_entities, check_distance, ticks, seed, max_pre
         all_o += app_o.last_checksums
     tick_launches = eng.launch_count() - launches0
     fused = eng.last_path_fused()
+    kernel = eng.last_kernel()
     peek_equal = True
     if peek_check:  # every live snapshot, every column: same bytes as the oracle's snapshot of that frame
         n_rows = eng.row_count()
@@ -108,6 +112,7 @@ def run_particles_synctest_pair(n_entities, check_distance, ticks, seed, max_pre
         "peek_equal": peek_equal,
         "mismatch_events": (len(mism_e), len(mism_o)),
         "fused": fused,
+        "kernel": kernel,
         "launches": tick_launches,
         "frames": (eng.rollback_frame_count(), orc.rollback_frame_count()),
         "active": (eng.active_count(), orc.active_count()),

@@ -34,6 +34,23 @@ def test_struct_layouts_match_the_header():
     assert C.sizeof(capi.bgr_config) == 40
 
 
+def test_last_kernel_kinds_agree_across_header_ctypes_and_rust():
+    """bgr_last_kernel's kind values are part of the ABI: the header's #defines, capi.py and the Rust constants agree,
+    and Engine.last_kernel() decodes the documented bit layout."""
+    from bevy_ggrs_b200.engine import LastKernel
+    hdr = open(os.path.join(ROOT, "include", "bevy_ggrs_b200.h")).read()
+    rs = open(os.path.join(ROOT, "rust_shim", "bevy_ggrs_b200_sys", "src", "lib.rs")).read()
+    in_hdr = {k: int(v) for k, v in re.findall(r"#define (BGR_KERNEL_\w+) (\d+)u", hdr)}
+    in_rs = {k: int(v) for k, v in re.findall(r"pub const (BGR_KERNEL_\w+): u32 = (\d+);", rs)}
+    assert len(in_hdr) == 6 and in_hdr == in_rs
+    assert all(getattr(capi, k) == v for k, v in in_hdr.items())
+    # bundle, VEC 4, MODE 1, 1024-thread tier, passive TMA, whole-tile items
+    raw = capi.BGR_KERNEL_BUNDLE | (4 << 4) | (1 << 8) | (2 << 10) | (1 << 12) | (512 << 16)
+    assert LastKernel.decode(raw) == LastKernel("bundle", 4, 1, 2, True, 512, raw)
+    assert LastKernel.decode(capi.BGR_KERNEL_GENERIC_NVRTC | (128 << 16)).item_rows == 128
+    assert LastKernel.decode(capi.BGR_KERNEL_STEPWISE_FLAT).kind == "stepwise_flat"
+
+
 def test_ggrs_time_delta_bits_matches_oracle(oracle_lib):
     lib = capi.load_library()
     for fps in (30, 60, 144):

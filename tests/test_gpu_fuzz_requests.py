@@ -3,7 +3,10 @@ compiled systems, random populations, random VALID request vectors (plain ticks,
 snapshots that exist, spectator-style catch-up runs), random host edits between vectors (remove / insert of optional
 components, spawns), and the occasional invalid rollback.  After every vector: checksums, frame resources and ring
 contents equal the oracle's; periodically every column, presence bit and the alive set.  Each seed runs on the default
-one-launch path and on the stepwise path."""
+one-launch path and on the stepwise path.  A second schema generator reaches the wide rows and long checksum ranges
+that pick other kernels: rows too wide for the NVRTC kernel (> 24 words), for the one-launch program and two TMA stages
+(> 49 words), a 1024-byte element, ranges up to the element's end, 6 checksummed and 7 optional columns, 8 and 9
+systems."""
 import numpy as np
 import pytest
 
@@ -85,7 +88,8 @@ def _compare_state(eng, orc, cols):
         assert np.array_equal(eng.read_component(c, 0, rows)[he], vo[he]), f"values of column {c}"
 
 
-def _drive(eng, orc, cols, sizes, optional, rng, flags, seed, n_vectors=40, input_hi=5, insert_value=None, allow_host_spawn=True):
+def _drive(eng, orc, cols, sizes, optional, rng, flags, seed, n_vectors=40, input_hi=5, insert_value=None, allow_host_spawn=True,
+           expect_kind=None):
     frame = 0  # RollbackFrameCount of both worlds
     for step in range(n_vectors):
         frames = orc.snapshot_frames()
@@ -114,7 +118,9 @@ def _drive(eng, orc, cols, sizes, optional, rng, flags, seed, n_vectors=40, inpu
         a, b = eng.handle_requests(NOSESS, reqs), orc.handle_requests(NOSESS, reqs)
         assert a == b, f"seed {seed} step {step}"
         assert eng.rollback_frame_count() == orc.rollback_frame_count() == frame
-        if flags == 0:
+        if expect_kind is not None:
+            assert eng.last_kernel().kind == expect_kind, f"seed {seed} step {step}"
+        elif flags == 0:
             assert eng.last_path_fused()
         # host edits between vectors
         rows = orc.row_count()
@@ -204,3 +210,170 @@ def test_random_request_vectors_on_the_particles_bundle_match_the_oracle(seed, f
         return np.array([int(r.integers(2, 20))], np.uint64).view(np.uint8)
     _drive(eng, orc, cols, sizes, optional, rng, flags, seed, n_vectors=32, input_hi=32, insert_value=insert_value, allow_host_spawn=False)
     eng.close(); orc.close()
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# wide rows and long checksum ranges
+# ---------------------------------------------------------------------------------------------------------------------
+WIDE_WORDS = [24, 25, 49, 50, 256]   # 256: one 1024-byte element
+RANGE_LENS = [0, 1, 3, 4, 8, 12, 16, 20, 31, 32, 33, 60, 64, 68]
+U32_SYSTEMS = [capi.BGR_SYS_U32_ADD, capi.BGR_SYS_U32_SATSUB_DESPAWN, capi.BGR_SYS_U32_STORE_CALL_COUNT]
+
+
+def _expected_kind(path, words, n_sys, nvrtc_ranges, generic_kernel):
+    """The kernel bgr_build / submit pick for this registration (engine.cu bgr_build, jit_specialise, run_stepwise)."""
+    tma_stages = words <= 49   # at least two one-tile stages in 200 KB of shared memory (BGR_TUNE_TMA_STAGES=2 keeps two)
+    if path == "generic" and words <= 49 and n_sys <= 8:
+        if generic_kernel != "interpreter" and words <= 24 and nvrtc_ranges:
+            return "generic_nvrtc"
+        return "generic_interpreter"
+    if path == "stepwise_flat":
+        return "stepwise_flat"
+    return "stepwise_tma" if tma_stages else "stepwise_flat"
+
+
+def _make_wide_worlds(rng, flags, words, aligned):
+    """Columns that add up to `words` words (sub-word tails included), up to 7 optional, up to 6 checksummed over
+    ranges of the lengths and offsets that change code paths, and 2, 8 or 9 u32 systems."""
+    n = int(rng.integers(1, 1400))
+    depth = int(rng.integers(2, 9))
+    if words == 256:
+        col_words = [256]
+    else:
+        n_cols = int(rng.integers(2, 9))
+        cuts = sorted(rng.choice(np.arange(1, words), size=n_cols - 1, replace=False).tolist())
+        col_words = [b - a for a, b in zip([0] + cuts, cuts + [words])]
+    sizes = [4 * w - (int(rng.integers(0, 4)) if (rng.random() < 0.3 and not aligned) else 0) for w in col_words]
+    n_opt = min(len(sizes), int(rng.choice([0, 2, 7])))
+    optional = [i < n_opt for i in range(len(sizes))]
+    rng.shuffle(optional)
+    worlds = [Engine(max_entities=n + 64, max_depth=depth + 1, flags=flags), OracleWorld()]
+    cols = []
+    for w in worlds:
+        cols = [w.rollback_component(f"W{i}", sizes[i], (capi.BGR_STRATEGY_COPY | OPT) if optional[i] else capi.BGR_STRATEGY_CLONE)
+                for i in range(len(sizes))]
+    cks, nvrtc_ranges = [], True
+    for i in rng.permutation(len(sizes))[:6]:
+        size = sizes[i]
+        if aligned:   # whole words, 4..64 bytes: the ranges the NVRTC kernel accepts (lanes wrap past 32 bytes)
+            ln = min(int(rng.choice([4, 8, 12, 16, 20, 32, 60, 64])), size - size % 4)
+            off = 4 * int(rng.integers(0, (size - ln) // 4 + 1))
+        else:
+            off = int(rng.choice([0, 1, 2, 3, 4 * int(rng.integers(0, max(1, size // 4)))]))
+            off = min(off, size)
+            ln = int(rng.choice(RANGE_LENS + [size - off]))
+            ln = min(ln, size - off)
+        nvrtc_ranges = nvrtc_ranges and (off % 4 == 0 and ln % 4 == 0 and 4 <= ln <= 64)
+        cks.append((int(i), off, ln))
+    for w in worlds:
+        for i, off, ln in cks:
+            w.checksum_component(cols[i], off, ln)
+    u32_cols = [i for i in range(len(sizes)) if sizes[i] >= 4]
+    systems = []
+    for _ in range(int(rng.choice([2, 8, 9]))):
+        i = int(rng.choice(u32_cols))
+        off = 4 * int(rng.integers(0, sizes[i] // 4))
+        kind = int(rng.choice(U32_SYSTEMS))
+        systems.append((kind, [cols[i]], [off] if kind == capi.BGR_SYS_U32_STORE_CALL_COUNT else [off, int(rng.integers(1, 4))]))
+    for w in worlds:
+        for sid, c, p in systems:
+            w.add_system(sid, c, p)
+        w.build()
+        w.set_depth(depth)
+    data = [rng.integers(0, 256, (n, s), dtype=np.uint8) for s in sizes]
+    for i, s in enumerate(sizes):   # small u32 words: SATSUB despawns inside the run
+        if s % 4 == 0:
+            data[i].view(np.uint32)[:] = rng.integers(1, 30, (n, s // 4), dtype=np.uint32)
+    removes = [(i, int(r)) for i in range(len(sizes)) if optional[i] for r in rng.choice(n, size=min(n, 6), replace=False)]
+    for w in worlds:
+        w.spawn(n)
+        for i in range(len(sizes)):
+            w.write_component(cols[i], 0, data[i])
+        for i, r in removes:
+            w.remove_component(cols[i], r)
+    return worlds[0], worlds[1], cols, sizes, optional, len(systems), nvrtc_ranges
+
+
+WIDE_PATHS = {"generic": ({}, 0), "stepwise_tma": ({}, capi.BGR_CFG_FORCE_STEPWISE),
+              "stepwise_flat": ({"BGR_TUNE_TMA": "0"}, capi.BGR_CFG_FORCE_STEPWISE),
+              "stepwise_tma_stages2": ({"BGR_TUNE_TMA_STAGES": "2"}, capi.BGR_CFG_FORCE_STEPWISE)}
+
+
+def _path_env(monkeypatch, path, generic_kernel):
+    if path != "generic" and generic_kernel != "interpreter":
+        pytest.skip("the stepwise path does not depend on the generic kernel: run once")
+    env, flags = WIDE_PATHS[path]
+    for k, v in env.items():
+        monkeypatch.setenv(k, v)
+    return flags
+
+
+@pytest.mark.parametrize("path", list(WIDE_PATHS))
+@pytest.mark.parametrize("seed", [0, 1])
+@pytest.mark.parametrize("words", WIDE_WORDS)
+def test_wide_rows_and_long_ranges_match_the_oracle(monkeypatch, generic_kernel, words, seed, path):
+    flags = _path_env(monkeypatch, path, generic_kernel)
+    rng = np.random.default_rng(9000 + 17 * words + seed)
+    aligned = seed == 0 and words <= 24    # seed 0 of the narrow class stays inside what the NVRTC kernel accepts
+    eng, orc, cols, sizes, optional, n_sys, nvrtc_ranges = _make_wide_worlds(rng, flags, words, aligned)
+    kind = _expected_kind(path, words, n_sys, nvrtc_ranges, generic_kernel)
+    _drive(eng, orc, cols, sizes, optional, rng, flags, seed, n_vectors=24, expect_kind=kind)
+    eng.close(); orc.close()
+
+
+@pytest.mark.parametrize("path", ["generic", "stepwise_tma", "stepwise_flat"])
+@pytest.mark.parametrize("elem,off,ln", [(96, 4, 64), (196, 8, 188), (1024, 0, 1024), (1024, 512, 508)])
+def test_finite_assertion_covers_the_whole_long_range(monkeypatch, generic_kernel, elem, off, ln, path):
+    """A finite-checked range that ends inside the element: inf in its last word raises BGR_ERR_NON_FINITE (the oracle
+    panics), inf in the word right after it does not.  Every kernel that hashes such a range: the one-launch program
+    (interpreter; NVRTC up to 64 bytes), the TMA copy kernel and k_checksum_column."""
+    flags = _path_env(monkeypatch, path, generic_kernel)
+    words = elem // 4
+    kind = _expected_kind(path, words, 0, ln <= 64, generic_kernel)
+    for word, raises in ((off + ln) // 4 - 1, True), ((off + ln) // 4, False):
+        if word >= words:
+            continue
+        eng, orc = Engine(max_entities=1200, max_depth=4, flags=flags), OracleWorld()
+        data = np.random.default_rng(elem + word).uniform(-9.0, 9.0, (1100, words)).astype(np.float32)
+        data[1037, word] = np.inf
+        res = []
+        for w in (eng, orc):
+            c = w.rollback_component("Wide", elem, capi.BGR_STRATEGY_COPY)
+            w.checksum_component(c, off, ln, capi.BGR_HASH_FLAG_ASSERT_FINITE_F32)
+            w.build()
+            w.spawn(1100)
+            w.write_component(c, 0, data)
+            try:
+                res.append(("ok", w.handle_requests(NOSESS, [Request(SAVE, 0), Request(ADVANCE, 0, [0]), Request(SAVE, 1)])))
+            except (BgrError, OracleError) as ex:
+                res.append(("raised", ex.status, str(ex)))
+        assert res[0] == res[1]
+        assert res[0][0] == ("raised" if raises else "ok")
+        if raises:
+            assert res[0][1] == capi.BGR_ERR_NON_FINITE
+        assert eng.last_kernel().kind == kind
+        eng.close(); orc.close()
+
+
+def test_a_1024_byte_column_round_trips(generic_kernel):
+    """write_component -> read_component (whole and a sub-range) and peek of a saved frame for a 1024-byte element
+    (256 word planes) next to a 3-byte one."""
+    n = 700
+    eng = Engine(max_entities=n, max_depth=4)
+    c = eng.rollback_component("Blob", 1024, capi.BGR_STRATEGY_CLONE)
+    small = eng.rollback_component("Small", 3, capi.BGR_STRATEGY_COPY)
+    eng.checksum_component(c, 0, 1024)
+    eng.build()
+    eng.spawn(n)
+    data = np.random.default_rng(5).integers(0, 256, (n, 1024), dtype=np.uint8)
+    eng.write_component(c, 0, data)
+    eng.write_component(small, 0, data[:, :3])
+    assert np.array_equal(eng.read_component(c, 0, n), data)
+    assert np.array_equal(eng.read_component(c, 300, 17), data[300:317])
+    eng.handle_requests(NOSESS, [Request(SAVE, 0)])
+    assert eng.last_kernel().kind == "stepwise_flat"
+    eng.write_component(c, 0, data[::-1].copy())
+    pe = eng.peek(0, c, 0, n)
+    assert pe is not None and pe[1].all() and np.array_equal(pe[0], data)
+    assert np.array_equal(eng.read_component(c, 0, n), data[::-1])
+    eng.close()

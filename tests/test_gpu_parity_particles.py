@@ -328,23 +328,6 @@ def test_both_work_item_sizes_match_the_oracle(monkeypatch, sub, n, d, spawn):
     assert r["ring"][0] == r["ring"][1] and r["active"][0] == r["active"][1]
 
 
-@pytest.mark.timeout(180)
-@pytest.mark.timeout(180)
-@pytest.mark.parametrize("grid,block", [("3", "128"), ("7", "256"), ("40", "64")])
-def test_generic_program_blocks_that_run_many_tiles(monkeypatch, generic_kernel, grid, block):
-    """The generic one-launch program with far fewer blocks than tiles (BGR_TUNE_GRID): every block claims tile after
-    tile from the global counter, reloads its shared-memory tile, and must wait for its own bulk stores before the
-    buffer is overwritten.  (Without the cap a world needs > 1.2M entities before a block sees a second tile.)"""
-    monkeypatch.setenv("BGR_TUNE_BUNDLE", "0")
-    monkeypatch.setenv("BGR_TUNE_GRID", grid)
-    monkeypatch.setenv("BGR_TUNE_GENERIC_BLOCK", block)
-    monkeypatch.setenv("BGR_TUNE_JIT_ROWS", {"64": "4", "128": "4", "256": "2"}[block])
-    r = run_particles_synctest_pair(60_000, 4, 10, seed=23, ttl_lo=3, ttl_hi=40, peek_check=True, z_fraction=0.2)
-    assert r["fused"] and r["launches"] == 10
-    assert r["checksums_equal"] and r["state_equal"] and r["peek_equal"]
-    assert r["active"][0] == r["active"][1] < 60_000
-
-
 @pytest.mark.parametrize("sub", ["128", "512"])
 def test_pipelined_overlap_with_both_work_item_sizes(monkeypatch, sub):
     """Tile dependencies count announcements per TILE: with 128-row items four blocks complete one tile together."""
