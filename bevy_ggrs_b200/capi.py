@@ -49,6 +49,9 @@ BGR_DESYNC_NO_INDEX = 0xFFFFFFFF
 # bgr_last_kernel: kind in bits 0-3
 BGR_KERNEL_NONE, BGR_KERNEL_STEPWISE_TMA, BGR_KERNEL_STEPWISE_FLAT, BGR_KERNEL_BUNDLE, \
     BGR_KERNEL_GENERIC_INTERPRETER, BGR_KERNEL_GENERIC_NVRTC = range(6)
+# ... and flags: the vector deferred its live-image write / started from a deferred live image's base slot
+BGR_KERNEL_DEFERRED_LIVE = 1 << 13
+BGR_KERNEL_FROM_DEFERRED = 1 << 14
 
 
 class bgr_request(C.Structure):

@@ -60,6 +60,22 @@ constexpr uint32_t kReqAdvanceNoBump = 100;  // bgr_advance_world: caller alread
 
 constexpr uint32_t kMaxSpawnVals = 1u << 16;  // particles spawned by one request vector
 
+constexpr uint32_t kMaxDeferredOps = 4;  // trailing ADVANCEs a deferred live image replays (SyncTest / P2P ticks: 1)
+
+// Deferred live image (BGR_TUNE_DEFER_LIVE).  A fused program that ends in `Save(f), Advance...` need not write image 0:
+// a Save stores the program's state verbatim and the kernels are bit-deterministic, so image 0 is exactly the base
+// slot's image with the trailing ADVANCEs replayed, on every tile the program would have written.  The next program
+// starts from the base slot instead (or with its own Load), and entry points that touch image 0 materialise it first.
+struct DeferredLive {
+    bool active = false;
+    bool passive = false;          // the eager program would also have written the passive planes (bundle)
+    uint32_t base_off256 = 0;      // the image the program's last stored Save wrote
+    uint32_t base_rows = 0;        // RollbackOrdered::len() at that Save
+    uint32_t max_rows = 0;         // image 0 is pending on tiles [0, max(1, tiles_for(max_rows)))
+    uint32_t n_ops = 0;
+    Op ops[kMaxDeferredOps];       // the ADVANCEs after the Save, verbatim
+};
+
 // Every host-side resource handle_requests / the schedules mutate.  A request vector is compiled
 // against a copy and committed only if the whole vector is valid.
 struct HostState {  // trivially copyable: copying it per call must not allocate
@@ -192,6 +208,10 @@ struct bgr_engine {
     unsigned long long* own_h_out[kBufs] = {};  // the engine's private result blocks while it is in a group
     unsigned long long* own_d_out[kBufs] = {};
     bool ticked = false;            // a request vector has been executed (the initial population is over)
+    DeferredLive deferred;          // committed by submit() together with `st`
+    bool live_touched = false;      // an entry point read or wrote image 0 since the last submit: the next one stays eager
+    int tune_defer_live = 1;        // 0: every fused program writes image 0 itself
+    unsigned long long* d_internal_out = nullptr;  // result block of internal launches (materialisation), [kMaxChains]
     // device-side launch trace (bgr_trace_enable): per launch [first block start, last block end] in globaltimer ns
     unsigned long long* d_trace = nullptr;
     uint32_t trace_cap = 0;
@@ -277,7 +297,11 @@ struct Program {
     bool has_load = false, has_advance = false, first_is_load = false, has_spawn = false;
     bool passive_to_slots = false;   // at least one SAVE must (re)write the passive planes
     bool passive_to_live = false;    // a LOAD changed the content of the live passive planes
+    bool defer_live = false;         // launch without the live-write flags (DeferredLive)
+    bool from_deferred = false;      // ops[0] is the LOAD of a deferred live image's base slot, followed by its ADVANCEs
+    bool internal = false;           // not a request vector: own result block, no trace row, no overlap with other launches
     std::vector<float2> spawn_vals;
+    bool writes_live_passive() const { return (has_load && passive_to_live) || has_spawn; }
 };
 
 int compile_requests(bgr_engine* e, HostState& s, const bgr_session_info* sess, const bgr_request* reqs, uint32_t n,
@@ -470,8 +494,8 @@ int run_fused(bgr_engine* e, const Program& pg, uint32_t buf, uint32_t* chains_o
     pp.live_rows = pg.live_rows;
     pp.flags = 0;
     if (!pg.first_is_load) pp.flags |= PF_READ_LIVE;
-    if (pg.has_load || pg.has_advance) pp.flags |= PF_WRITE_LIVE_ACTIVE;
-    if ((pg.has_load && pg.passive_to_live) || pg.has_spawn) pp.flags |= PF_WRITE_LIVE_PASSIVE;
+    if ((pg.has_load || pg.has_advance) && !pg.defer_live) pp.flags |= PF_WRITE_LIVE_ACTIVE;
+    if (pg.writes_live_passive() && !pg.defer_live) pp.flags |= PF_WRITE_LIVE_PASSIVE;
     const bool passive_needed = pg.passive_to_slots || (pp.flags & PF_WRITE_LIVE_PASSIVE) || pg.has_spawn;
     uint32_t n_loads = 0;
     for (uint32_t i = 0; i < pg.n_ops; ++i) n_loads += (pg.ops[i].kind == OP_LOAD);
@@ -527,7 +551,8 @@ int run_fused(bgr_engine* e, const Program& pg, uint32_t buf, uint32_t* chains_o
     // a synchronous caller collects before the next submit, so there is nothing to overlap with
     // ... and only on a stream the engine owns: on a caller's stream foreign work may sit between two submits and
     // become the programmatic-launch primary, which the per-tile flags know nothing about
-    const bool tiledep = e->tune_tiledep && chains == 1 && e->d_tile_done && e->own_stream && (e->tune_tiledep > 1 || !e->pending.empty());
+    const bool tiledep = e->tune_tiledep && chains == 1 && e->d_tile_done && e->own_stream && !pg.internal &&
+                         (e->tune_tiledep > 1 || !e->pending.empty());
     if (e->tiledep_chain && total_tiles != e->tiledep_tiles) {
         // The tile range changed (rows crossed a tile boundary): a tile outside the previous launch's range may still be
         // in use by an OLDER overlapping launch that nothing would make this one wait for.  Rare: drain the stream.
@@ -556,9 +581,9 @@ int run_fused(bgr_engine* e, const Program& pg, uint32_t buf, uint32_t* chains_o
         const uint32_t set = tiledep ? uint32_t(e->seq % bgr_engine::kBufs) : c;
         pp.accum = e->d_accum_c[set];
         pp.ticket = e->d_ticket_c[set];
-        pp.out = e->d_out[buf] + size_t(c) * kResultStride;
+        pp.out = (pg.internal ? e->d_internal_out : e->d_out[buf]) + size_t(c) * kResultStride;
         pp.trace = nullptr;
-        if (e->d_trace && c == 0 && e->seq - e->trace_first_seq < e->trace_cap) pp.trace = e->d_trace + (e->seq - e->trace_first_seq) * 4;
+        if (e->d_trace && c == 0 && !pg.internal && e->seq - e->trace_first_seq < e->trace_cap) pp.trace = e->d_trace + (e->seq - e->trace_first_seq) * 4;
         cudaStream_t stream = chains > 1 ? e->chain_stream[c] : e->stream;
         int rc = launch_fused_variant(e, pp, stream);
         if (rc != BGR_OK) return rc;
@@ -859,15 +884,15 @@ int run_generic(bgr_engine* e, const Program& pg, uint32_t buf) {
     gp.order_base = e->cfg.order_base;
     gp.accum = e->d_accum_c[0];
     gp.ticket = e->d_ticket_c[0];
-    gp.out = e->d_out[buf];
+    gp.out = pg.internal ? e->d_internal_out : e->d_out[buf];
     gp.seq = e->seq;
-    if (e->d_trace && e->seq - e->trace_first_seq < e->trace_cap) gp.trace = e->d_trace + (e->seq - e->trace_first_seq) * 4;
+    if (e->d_trace && !pg.internal && e->seq - e->trace_first_seq < e->trace_cap) gp.trace = e->d_trace + (e->seq - e->trace_first_seq) * 4;
     gp.words = e->words; gp.tile_bytes = e->tile_bytes;
     gp.n_ops = pg.n_ops; gp.n_saves = pg.n_saves;
     gp.n_tiles = std::max(1u, e->tiles_for(pg.max_rows));
     gp.live_rows = pg.live_rows;
     if (!pg.first_is_load) gp.flags |= PF_READ_LIVE;
-    if (pg.has_load || pg.has_advance) gp.flags |= PF_WRITE_LIVE_ACTIVE;
+    if ((pg.has_load || pg.has_advance) && !pg.defer_live) gp.flags |= PF_WRITE_LIVE_ACTIVE;
     fill_generic_specs(e, gp);
     std::memcpy(gp.ops, pg.ops, sizeof(Op) * pg.n_ops);
     if (e->jit.fn) {  // the registration's own register-resident kernel
@@ -879,7 +904,8 @@ int run_generic(bgr_engine* e, const Program& pg, uint32_t buf) {
         // Overlap of consecutive launches: only when request vectors are queued behind each other (a synchronous caller
         // collects before its next submit), only on a stream the engine owns, and only between launches of the SAME kernel
         // over the SAME items (the per-item flags mean nothing across partitions: drain instead — rare, rows crossed a tile).
-        const bool tiledep = e->tune_jit_tiledep && e->d_item_done && e->own_stream && (e->tune_jit_tiledep > 1 || !e->pending.empty());
+        const bool tiledep = e->tune_jit_tiledep && e->d_item_done && e->own_stream && !pg.internal &&
+                             (e->tune_jit_tiledep > 1 || !e->pending.empty());
         bool wait = false;
         if (prev_chain) {
             if (tiledep && e->jit_chain_kernel == k.fn && e->tiledep_tiles == n_items) wait = true;
@@ -935,6 +961,105 @@ int run_generic(bgr_engine* e, const Program& pg, uint32_t buf) {
 }
 
 
+bool use_bundle(const bgr_engine* e) {
+    return e->bundle_particles && e->tune_bundle && !(e->cfg.flags & BGR_CFG_FORCE_STEPWISE);
+}
+bool use_generic(const bgr_engine* e) {
+    return !use_bundle(e) && e->generic_ok && e->tune_generic && !(e->cfg.flags & BGR_CFG_FORCE_STEPWISE);
+}
+uint32_t program_tiles(const bgr_engine* e, uint32_t rows) { return std::max(1u, e->tiles_for(rows)); }
+
+// Writes the deferred live image: the internal program [LOAD(base), pending ADVANCEs] with the live-write flags over
+// the deferred tile range.  It publishes into the engine's own result block (queued submits keep theirs), takes no
+// trace row and leaves bgr_last_kernel alone; it is counted by bgr_launch_count.
+int materialize_live(bgr_engine* e) {
+    if (!e->deferred.active) return BGR_OK;
+    const DeferredLive d = e->deferred;
+    e->deferred.active = false;
+    Program pg;
+    Op& ld = pg.ops[0];
+    std::memset(&ld, 0, sizeof ld);
+    ld.kind = OP_LOAD; ld.image_off256 = d.base_off256; ld.n_rows = d.base_rows;
+    std::memcpy(pg.ops + 1, d.ops, sizeof(Op) * d.n_ops);
+    pg.n_ops = 1 + d.n_ops;
+    pg.max_rows = d.max_rows; pg.live_rows = d.base_rows;
+    pg.has_load = pg.first_is_load = true;
+    pg.has_advance = d.n_ops > 0;
+    pg.passive_to_live = d.passive;
+    pg.internal = true;
+    const uint32_t kernel = e->last_kernel;
+    uint32_t chains = 1;
+    const int rc = use_bundle(e) ? run_fused(e, pg, 0, &chains) : run_generic(e, pg, 0);
+    e->last_kernel = kernel;
+    return rc;
+}
+
+// Every entry point that reads or writes image 0 outside a program calls this (after drain(), where it drains).  The
+// next request vector then writes image 0 eagerly: a caller that reads the live world every tick pays at most one
+// materialisation instead of one per tick.
+int touch_live(bgr_engine* e) {
+    e->live_touched = true;
+    return materialize_live(e);
+}
+
+// The previous fused program deferred its live write.  A program that starts with its own Load reads nothing of image
+// 0 and rewrites it (the record is dropped); one that would read image 0 starts from the base slot instead:
+// [LOAD(base), pending ADVANCEs, its own ops].  Otherwise image 0 is written first: a Save of this program would
+// overwrite the base slot (shallow rings), the rewritten vector would not fit, or this program covers fewer tiles than
+// the deferred range (rows shrank through a Load), whose tiles it would otherwise leave stale.
+int consume_deferred(bgr_engine* e, Program& pg) {
+    const DeferredLive& d = e->deferred;
+    if (!d.active) return BGR_OK;
+    if (program_tiles(e, pg.max_rows) >= program_tiles(e, d.max_rows)) {
+        if (pg.first_is_load) {
+            if (d.passive) pg.passive_to_live = true;  // the live passive planes were not written either
+            return BGR_OK;
+        }
+        bool base_saved = false;
+        for (uint32_t i = 0; i < pg.n_ops; ++i)
+            base_saved = base_saved || (pg.ops[i].kind == OP_SAVE && !(pg.ops[i].flags & OPF_NO_STORE) &&
+                                        pg.ops[i].image_off256 == d.base_off256);
+        if (!base_saved && pg.n_ops + 1 + d.n_ops <= uint32_t(kMaxOps)) {
+            std::memmove(pg.ops + 1 + d.n_ops, pg.ops, sizeof(Op) * pg.n_ops);
+            Op& ld = pg.ops[0];
+            std::memset(&ld, 0, sizeof ld);
+            ld.kind = OP_LOAD; ld.image_off256 = d.base_off256; ld.n_rows = d.base_rows;
+            std::memcpy(pg.ops + 1, d.ops, sizeof(Op) * d.n_ops);
+            pg.n_ops += 1 + d.n_ops;
+            pg.has_load = pg.first_is_load = true;
+            pg.has_advance = pg.has_advance || d.n_ops > 0;
+            // the prepended LOAD rewrites the live passive planes exactly when the deferring program would have
+            pg.passive_to_live = pg.passive_to_live || d.passive;
+            pg.max_rows = std::max(pg.max_rows, d.base_rows);
+            pg.from_deferred = true;
+            return BGR_OK;
+        }
+    }
+    return materialize_live(e);
+}
+
+// A fused program defers its live write when its last stored Save is followed only by ADVANCEs that spawn nothing
+// (at most kMaxDeferredOps of them).  Returns the record submit() commits.
+DeferredLive plan_deferral(Program& pg) {
+    DeferredLive d;
+    if (!(pg.has_load || pg.has_advance)) return d;  // the program writes no live image
+    uint32_t i = pg.n_ops;
+    while (i > 0 && pg.ops[i - 1].kind == OP_ADVANCE && !(pg.ops[i - 1].flags & OPF_SPAWN)) --i;
+    const uint32_t n_tail = pg.n_ops - i;
+    if (i == 0 || n_tail > kMaxDeferredOps) return d;
+    const Op& sv = pg.ops[i - 1];
+    if (sv.kind != OP_SAVE || (sv.flags & OPF_NO_STORE)) return d;
+    d.active = true;
+    d.passive = pg.writes_live_passive();
+    d.base_off256 = sv.image_off256;
+    d.base_rows = sv.n_rows;
+    d.max_rows = pg.max_rows;
+    d.n_ops = n_tail;
+    std::memcpy(d.ops, pg.ops + i, sizeof(Op) * n_tail);
+    pg.defer_live = true;
+    return d;
+}
+
 int submit(bgr_engine* e, const bgr_session_info* sess, const bgr_request* reqs, uint32_t n) {
     NvtxRange span("HandleRequests");
     if (!e) return fail(BGR_ERR_INVALID_ARGUMENT, "null engine");
@@ -959,17 +1084,24 @@ int submit(bgr_engine* e, const bgr_session_info* sess, const bgr_request* reqs,
     if (!pg.spawn_vals.empty()) std::memcpy(e->h_spawn[buf], pg.spawn_vals.data(), pg.spawn_vals.size() * sizeof(float2));
     e->seq += 1;
     e->ticked = true;
-    const bool stepwise_forced = e->cfg.flags & BGR_CFG_FORCE_STEPWISE;
-    const bool bundle = e->bundle_particles && e->tune_bundle && !stepwise_forced;
-    const bool generic = !bundle && e->generic_ok && e->tune_generic && !stepwise_forced;
+    const bool bundle = use_bundle(e);
+    const bool generic = use_generic(e);
     const bool fused = bundle || generic;   // one launch for the whole request vector
+    rc = fused ? consume_deferred(e, pg) : materialize_live(e);
+    if (rc != BGR_OK) return rc;
+    DeferredLive next;
+    if (fused && e->tune_defer_live && !e->live_touched) next = plan_deferral(pg);
     uint32_t chains = 1;
     rc = bundle ? run_fused(e, pg, buf, &chains) : generic ? run_generic(e, pg, buf) : run_stepwise(e, pg, buf);
     if (rc != BGR_OK) return rc;
+    if (pg.defer_live) e->last_kernel |= BGR_KERNEL_DEFERRED_LIVE;
+    if (pg.from_deferred) e->last_kernel |= BGR_KERNEL_FROM_DEFERRED;
     // an event between two launches would serialise them; with host polling it is only a fallback, taken lazily
     if (!(e->tune_tiledep && e->tune_poll)) CUDA_TRY(cudaEventRecord(e->ev[buf], e->stream));
     e->last_fused = fused;
     e->st = s;
+    e->deferred = next;
+    e->live_touched = false;
     Pending pd;
     pd.buf = buf; pd.n_saves = pg.n_saves; pd.seq = e->seq; pd.chains = chains; pd.gseq = e->group ? e->gseq : 0;
     std::memcpy(pd.frames, pg.save_frames, sizeof(int32_t) * pg.n_saves);
@@ -1114,6 +1246,7 @@ int transfer_column(bgr_engine* e, uint32_t image_idx, uint32_t column, uint32_t
     if (uint64_t(first) + count > e->cfg.max_entities) return fail(BGR_ERR_CAPACITY, "row range exceeds max_entities");
     if (count == 0) return BGR_OK;
     int rc = drain(e);
+    if (rc == BGR_OK && image_idx == 0) rc = touch_live(e);
     if (rc != BGR_OK) return rc;
     const size_t bytes = size_t(count) * stride;
     rc = ensure_stage(e, bytes);
@@ -1142,6 +1275,7 @@ int read_alive_image(bgr_engine* e, uint32_t image_idx, uint32_t first, uint32_t
                      uint32_t need = 0) {
     if (count == 0) return BGR_OK;
     int rc = drain(e);
+    if (rc == BGR_OK && image_idx == 0) rc = touch_live(e);
     if (rc != BGR_OK) return rc;
     if (uint64_t(first) + count > e->cfg.max_entities) return fail(BGR_ERR_CAPACITY, "row range exceeds max_entities");
     rc = ensure_stage(e, count);
@@ -1169,6 +1303,8 @@ int download_begin(bgr_engine* e, uint32_t column, uint32_t off, uint32_t len, u
         if (!e->dl[i].busy) { slot = i; break; }
     }
     if (slot == BGR_MAX_DOWNLOADS) return fail(BGR_ERR_STATE, "too many downloads in flight (BGR_MAX_DOWNLOADS)");
+    int rc = touch_live(e);  // stream-ordered behind the queued submits, like the gather below
+    if (rc != BGR_OK) return rc;
     bgr_engine::Download& d = e->dl[slot];
     const size_t bytes = size_t(count) * len;
     if (!e->copy_stream) CUDA_TRY(cudaStreamCreateWithFlags(&e->copy_stream, cudaStreamNonBlocking));
@@ -1318,6 +1454,7 @@ BGR_API int bgr_engine_create(const bgr_config* cfg, bgr_engine** out) {
     e->tune_passive_early = env_int("BGR_TUNE_PASSIVE_EARLY", -1);
     e->tune_stagger_ns = env_int("BGR_TUNE_STAGGER_NS", 800);
     e->tune_bundle = env_int("BGR_TUNE_BUNDLE", 1);
+    e->tune_defer_live = env_int("BGR_TUNE_DEFER_LIVE", 1);
     e->n_chains = std::max(1, std::min(int(bgr_engine::kMaxChains), env_int("BGR_TUNE_CHAINS", 1)));
     if (e->tune_vec != 1 && e->tune_vec != 2 && e->tune_vec != 4) e->tune_vec = 2;
     e->st.confirmed = 0;
@@ -1346,6 +1483,7 @@ BGR_API void bgr_engine_destroy(bgr_engine* e) {
     if (e->d_stage) cudaFree(e->d_stage);
     if (e->d_accum) cudaFree(e->d_accum);
     if (e->d_ticket) cudaFree(e->d_ticket);
+    if (e->d_internal_out) cudaFree(e->d_internal_out);
     if (e->copy_stream) { cudaStreamSynchronize(e->copy_stream); cudaStreamDestroy(e->copy_stream); }
     if (e->d_tma_ticket) cudaFree(e->d_tma_ticket);
     if (e->d_tile_done) cudaFree(e->d_tile_done);
@@ -1515,6 +1653,7 @@ BGR_API int bgr_build(bgr_engine* e) {
         CUDA_TRY(cudaEventCreateWithFlags(&e->main_ev, cudaEventDisableTiming));
         e->main_dirty = true;  // the memsets above
     }
+    CUDA_TRY(cudaMalloc(&e->d_internal_out, sizeof(unsigned long long) * kResultStride * bgr_engine::kMaxChains));
     for (int i = 0; i < bgr_engine::kBufs; ++i) {
         const size_t out_bytes = sizeof(unsigned long long) * kResultStride * bgr_engine::kMaxChains;
         CUDA_TRY(cudaHostAlloc(&e->h_out[i], out_bytes, cudaHostAllocMapped));
@@ -1567,6 +1706,7 @@ BGR_API int bgr_run_startup_system(bgr_engine* e, uint32_t system) {
     if (system != BGR_SYS_PARTICLES_SPAWN || e->spawn_sys < 0)
         return fail(BGR_ERR_INVALID_ARGUMENT, "only a registered spawn_particles system can run at Startup");
     int rc = drain(e);
+    if (rc == BGR_OK) rc = touch_live(e);
     if (rc != BGR_OK) return rc;
     const SystemReg& sy = e->systems[size_t(e->spawn_sys)];
     const uint32_t rate = sy.params[0];
@@ -1590,6 +1730,7 @@ BGR_API int bgr_run_startup_system(bgr_engine* e, uint32_t system) {
 BGR_API int bgr_spawn(bgr_engine* e, uint32_t count, uint32_t* first_row_out) {
     if (!e || !e->built) return fail(BGR_ERR_STATE, "engine not built");
     int rc = drain(e);
+    if (rc == BGR_OK) rc = touch_live(e);
     if (rc != BGR_OK) return rc;
     if (uint64_t(e->st.n_rows) + count > e->cfg.max_entities) return fail(BGR_ERR_CAPACITY, "spawn exceeds max_entities");
     if (count && e->ticked && ((e->cfg.flags & BGR_CFG_SHARDED) || e->cfg.order_base != 0))
@@ -1611,6 +1752,7 @@ BGR_API int bgr_spawn(bgr_engine* e, uint32_t count, uint32_t* first_row_out) {
 BGR_API int bgr_despawn(bgr_engine* e, uint32_t row) {
     if (!e || !e->built) return fail(BGR_ERR_STATE, "engine not built");
     int rc = drain(e);
+    if (rc == BGR_OK) rc = touch_live(e);
     if (rc != BGR_OK) return rc;
     if (row >= e->st.n_rows) return fail(BGR_ERR_INVALID_ARGUMENT, "row out of range");
     k_set_alive<<<1, 1, 0, e->stream>>>(e->image(0), e->words, row, 0);
@@ -1654,7 +1796,8 @@ static int presence_args(bgr_engine* e, uint32_t column, uint32_t row) {
     if (column >= e->cols.size()) return fail(BGR_ERR_INVALID_ARGUMENT, "unknown column");
     if (!e->cols[column].absent) return fail(BGR_ERR_INVALID_ARGUMENT, "column was not registered with BGR_STRATEGY_OPTIONAL");
     if (row >= e->st.n_rows) return fail(BGR_ERR_INVALID_ARGUMENT, "row out of range");
-    return drain(e);
+    const int rc = drain(e);
+    return rc == BGR_OK ? touch_live(e) : rc;
 }
 BGR_API int bgr_remove_component(bgr_engine* e, uint32_t column, uint32_t row) {
     int rc = presence_args(e, column, row);
@@ -1722,14 +1865,20 @@ BGR_API int bgr_max_prediction_window(bgr_engine* e, uint32_t* out) {
     *out = e->st.has_maxpred ? e->st.maxpred : 0; return BGR_OK;
 }
 
+// Ring operations outside a program can hand the slot of a deferred live image's base to a later Save: the live image
+// is written first.
 BGR_API int bgr_set_depth(bgr_engine* e, uint32_t depth) {
     if (!e) return fail(BGR_ERR_INVALID_ARGUMENT, "null engine");
+    const int rc = materialize_live(e);
+    if (rc != BGR_OK) return rc;
     e->st.has_maxpred = true; e->st.maxpred = depth;  // MaxPredictionWindow: sync_depth applies it before every save
     e->st.ring.set_depth(depth);
     return BGR_OK;
 }
 BGR_API int bgr_confirm(bgr_engine* e, int32_t confirmed_frame) {
     if (!e) return fail(BGR_ERR_INVALID_ARGUMENT, "null engine");
+    const int rc = materialize_live(e);
+    if (rc != BGR_OK) return rc;
     e->st.confirmed = confirmed_frame;
     e->st.ring.confirm(confirmed_frame);
     return BGR_OK;
@@ -2131,6 +2280,8 @@ BGR_API int bgr_group_collect(bgr_group* h, uint64_t gseq, bgr_checksum* out, ui
 BGR_API int bgr_reset_session(bgr_engine* e) {
     if (!e) return fail(BGR_ERR_INVALID_ARGUMENT, "null engine");
     if (!e->pending.empty()) return fail(BGR_ERR_STATE, "collect every submitted request vector first");
+    const int rc = materialize_live(e);
+    if (rc != BGR_OK) return rc;
     e->st.frame_count = 0;        // RollbackFrameCount(0)
     e->st.confirmed = -1;         // ConfirmedFrameCount(-1)
     e->st.has_maxpred = true;     // MaxPredictionWindow(8)

@@ -22,7 +22,9 @@ _KERNEL_KINDS = {capi.BGR_KERNEL_NONE: "none", capi.BGR_KERNEL_STEPWISE_TMA: "st
 
 class LastKernel(NamedTuple):
     """bgr_last_kernel decoded.  vec / mode / tier / passive_tma describe the bundle kernel (0 / False otherwise);
-    item_rows is set for the bundle and the NVRTC kernel.  tier: 0 unconstrained, 1 768 and 2 1024 threads per SM."""
+    item_rows is set for the bundle and the NVRTC kernel.  tier: 0 unconstrained, 1 768 and 2 1024 threads per SM.
+    deferred_live: the vector did not write the live image (BGR_TUNE_DEFER_LIVE); from_deferred: it started from the
+    base slot of the previous vector's deferred live image."""
     kind: str
     vec: int
     mode: int
@@ -30,11 +32,14 @@ class LastKernel(NamedTuple):
     passive_tma: bool
     item_rows: int
     raw: int
+    deferred_live: bool = False
+    from_deferred: bool = False
 
     @staticmethod
     def decode(v: int) -> "LastKernel":
         return LastKernel(_KERNEL_KINDS.get(v & 0xF, f"unknown({v & 0xF})"), (v >> 4) & 0xF, (v >> 8) & 0x3,
-                          (v >> 10) & 0x3, bool((v >> 12) & 1), (v >> 16) & 0x3FF, v)
+                          (v >> 10) & 0x3, bool((v >> 12) & 1), (v >> 16) & 0x3FF, v,
+                          bool(v & capi.BGR_KERNEL_DEFERRED_LIVE), bool(v & capi.BGR_KERNEL_FROM_DEFERRED))
 
 
 class Engine:

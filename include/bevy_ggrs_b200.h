@@ -388,7 +388,13 @@ BGR_API int bgr_generic_specialised(bgr_engine* e, uint32_t* specialised_out);
  *              BGR_HASH_FLAG_ASSERT_FINITE_F32: specialised), 2 (per-entity presence of optional columns)
  *   bits 10-11 bundle: launch-bounds tier, 0 unconstrained, 1 768 threads per SM, 2 1024 threads per SM
  *   bit 12     bundle: passive planes moved by TMA bulk copies
+ *   bit 13     BGR_KERNEL_DEFERRED_LIVE: the vector ended in Save, Advance... and did not write the live image; it is
+ *              rebuilt from that Save's slot when something needs it (env BGR_TUNE_DEFER_LIVE, default 1)
+ *   bit 14     BGR_KERNEL_FROM_DEFERRED: the vector would have read a deferred live image and started from the base
+ *              slot instead (a Load of that slot and its pending Advances ran first, inside the same launch)
  *   bits 16-25 bundle and generic NVRTC: rows per work item (512 = a whole tile) */
+#define BGR_KERNEL_DEFERRED_LIVE (1u << 13)
+#define BGR_KERNEL_FROM_DEFERRED (1u << 14)
 #define BGR_KERNEL_NONE 0u
 #define BGR_KERNEL_STEPWISE_TMA 1u       /* one kernel per request; Save / Load through the TMA-staged copy kernel */
 #define BGR_KERNEL_STEPWISE_FLAT 2u      /* one kernel per request; k_checksum_column + k_copy_image */

@@ -42,6 +42,10 @@ pub const BGR_KERNEL_STEPWISE_FLAT: u32 = 2;
 pub const BGR_KERNEL_BUNDLE: u32 = 3;
 pub const BGR_KERNEL_GENERIC_INTERPRETER: u32 = 4;
 pub const BGR_KERNEL_GENERIC_NVRTC: u32 = 5;
+/// bgr_last_kernel flag: the request vector deferred its live-image write.
+pub const BGR_KERNEL_DEFERRED_LIVE: u32 = 1 << 13;
+/// bgr_last_kernel flag: the request vector started from a deferred live image's base slot.
+pub const BGR_KERNEL_FROM_DEFERRED: u32 = 1 << 14;
 
 pub const BGR_CFG_FORCE_STEPWISE: u32 = 1;
 pub const BGR_CFG_SHARDED: u32 = 2;
