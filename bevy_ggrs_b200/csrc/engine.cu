@@ -98,7 +98,6 @@ struct HostState {  // trivially copyable: copying it per call must not allocate
 
 struct Pending {
     uint32_t buf = 0;
-    uint32_t chains = 1;            // result blocks to wait for
     unsigned long long seq = 0;
     unsigned long long gseq = 0;    // shard group sequence number (0: not in a group)
     bool finished = false;          // the GPU work is known to be complete (drain() synchronised the stream)
@@ -166,19 +165,10 @@ struct bgr_engine {
     HostState st;
 
     static constexpr int kBufs = 8;  // result / spawn buffers = max un-collected submits (== PendingRing capacity)
-    static constexpr int kMaxChains = 8;
-    // Chains: the entity range is cut into n_chains contiguous tile ranges, each with its own stream, accumulators
-    // and result block.  Entities are independent, so chain A's kernel of tick i+1 only depends on chain A's kernel
-    // of tick i: with back-to-back submits the ramp / tail of one chain's kernel overlaps the other chain's kernel
-    // (the same entity-range sharding as across GPUs, inside one GPU; partials are XOR-folded on the host).
-    int n_chains = 1;
-    cudaStream_t chain_stream[kMaxChains] = {};
-    cudaEvent_t chain_ev[kMaxChains] = {};
-    cudaEvent_t main_ev = nullptr;
-    bool main_dirty = false;        // the main stream has un-synchronised work the chains must wait for
-    uint32_t last_total_tiles = 0, last_chains = 0;  // tile partition of the previous chained launch
-    unsigned long long* d_accum_c[kMaxChains] = {};
-    unsigned int* d_ticket_c[kMaxChains] = {};
+    // accumulator / ticket sets: one per in-flight request vector, so that overlapping launches (tile dependencies)
+    // never share one; set 0 serves every launch that overlaps nothing
+    unsigned long long* d_accum_set[kBufs] = {};
+    unsigned int* d_ticket_set[kBufs] = {};
     unsigned long long* d_accum = nullptr;
     unsigned int* d_ticket = nullptr;
     float2* h_spawn[kBufs] = {};  // host-mapped (vx, vy) of spawned particles
@@ -211,7 +201,7 @@ struct bgr_engine {
     DeferredLive deferred;          // committed by submit() together with `st`
     bool live_touched = false;      // an entry point read or wrote image 0 since the last submit: the next one stays eager
     int tune_defer_live = 1;        // 0: every fused program writes image 0 itself
-    unsigned long long* d_internal_out = nullptr;  // result block of internal launches (materialisation), [kMaxChains]
+    unsigned long long* d_internal_out = nullptr;  // result block of internal launches (materialisation)
     // device-side launch trace (bgr_trace_enable): per launch [first block start, last block end] in globaltimer ns
     unsigned long long* d_trace = nullptr;
     uint32_t trace_cap = 0;
@@ -230,7 +220,6 @@ struct bgr_engine {
     uint32_t tiledep_seq = 0, tiledep_tiles = 0;
     int tune_grid = 0;            // experiment / tests: cap the one-launch kernels' grid (0 = SMs x resident blocks)
     int tune_prefetch = 1;        // L2 prefetch of the next tile's active planes
-    int tune_pdl = 0;             // programmatic dependent launch between consecutive fused kernels (measured: +0.8 % at 1M, -14 % at 100k -> off)
     int tune_dynamic = 1;         // dynamic tile scheduling in the fused kernel (measured +5% over a static stride)
 
     // compiled bundle: particles (update_particles + despawn_particles)
@@ -253,16 +242,15 @@ struct bgr_engine {
     int tune_jit_item = 0;          // 0 auto (quarter tiles below 3 tiles per SM), 512 / 256 / 128 force the rows per work item
     int tune_generic_block = 0;     // 0 = 128; 64 / 256 / 512 force
     int tune_passive_early = -1;    // -1: early passive stores for single-wave grids (auto); 0 never; 1 always
-    int tune_sub = 0;               // 128: the 128-row work-item variant of the fused kernel (experiment; default: whole tiles)
     int tune_stagger_ns = 800;      // start-of-grid phase stagger between the resident blocks of an SM (synchronous launches; measured -1.3 %)
     int tune_generic = 1;
     int tune_bundle = 1;            // 0: never use the specialised particles kernel (A/B tests of the generic program)
     bool bundle_opt = false;        // a registered column is BGR_STRATEGY_OPTIONAL: the presence-aware kernel variant (MODE 2)
-    int tune_vec = 2, tune_minb = 2, tune_bps = 0, tune_passive_tma = 1;
+    int tune_bps = 0, tune_passive_tma = 1;
     int tune_tma = 1;          // stepwise Save/Load through the TMA-staged bulk-copy kernel
     uint32_t tma_stage_tiles = 0;  // one-tile stages of the TMA copy kernel (0: schema too wide for two stages of shared memory)
     unsigned int* d_tma_ticket = nullptr;
-    int occ_cache[2][2][3][3][3] = {};  // [passive TMA][sub-tile items][VEC][MODE][launch-bounds tier]: blocks per SM
+    int occ_cache[2][3] = {};  // [passive TMA][MODE]: blocks per SM of k_particles_program
     // desync diff scratch (BGR_CFG_DESYNC_CAPTURE), allocated by the first bgr_desync_diff
     DiffColumn* d_diff_cols = nullptr;
     unsigned int* d_diff_counts = nullptr;       // [n_cols][3] then the per-tile record counts
@@ -441,55 +429,56 @@ int compile_requests(bgr_engine* e, HostState& s, const bgr_session_info* sess, 
 // ---------------------------------------------------------------------------------------------
 // launch: fused bundle kernel
 // ---------------------------------------------------------------------------------------------
-template <int VEC, int MODE, int MINB, int SUB = int(kTileRows)>
-int launch_particles(bgr_engine* e, const ProgramParams& pp, int vi, int si, int mi, cudaStream_t stream) {
-    auto kern = k_particles_program<VEC, MODE, MINB, SUB>;
-    constexpr int BLOCK = SUB / VEC;
-    constexpr uint32_t kSubs = kTileRows / SUB;
-    constexpr int ui = kSubs > 1 ? 1 : 0;
+template <int MODE>
+int launch_particles(bgr_engine* e, const ProgramParams& pp) {
+    auto kern = k_particles_program<MODE>;
+    constexpr int kBlock = int(kTileRows) / 2;  // two rows per thread
     const int ti = (pp.flags & PF_PASSIVE_TMA) ? 1 : 0;
     const size_t smem = ti ? size_t(2) * pp.passive_bytes : 0;
-    // A variant runs with and without the passive double buffer (spawns and multi-Load vectors move passive planes
-    // per thread): the shared-memory opt-in and the occupancy are per (variant, buffer).  passive_bytes is fixed at
-    // bgr_build for a given variant, so one entry per buffer setting is exact.
-    int& occ = e->occ_cache[ti][ui][vi][si][mi];
+    // A mode runs with and without the passive double buffer (spawns and multi-Load vectors move passive planes per
+    // thread): the shared-memory opt-in and the occupancy are per (mode, buffer).  passive_bytes is fixed at bgr_build,
+    // so one entry per buffer setting is exact.
+    int& occ = e->occ_cache[ti][MODE];
     if (occ == 0) {
         if (smem > 48 * 1024) CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem)));
         int nb = 0;
-        CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, kern, BLOCK, smem));
+        CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, kern, kBlock, smem));
         occ = std::max(1, nb);
     }
     int bps = occ;
     if (e->tune_bps > 0) bps = std::min(e->tune_bps, bps);
-    uint32_t grid = std::max(1u, std::min((pp.n_tiles - pp.tile_begin) * kSubs, uint32_t(e->num_sms * bps)));
+    uint32_t grid = std::max(1u, std::min(pp.n_tiles, uint32_t(e->num_sms * bps)));
     if (e->tune_grid > 0) grid = std::min(grid, uint32_t(e->tune_grid));
-    if (kSubs > 1) grid = std::max(kSubs, grid / kSubs * kSubs);  // the first wave covers whole tiles (per-tile completion counts)
     cudaLaunchConfig_t lc{};
-    lc.gridDim = dim3(grid); lc.blockDim = dim3(BLOCK); lc.dynamicSmemBytes = smem; lc.stream = stream;
+    lc.gridDim = dim3(grid); lc.blockDim = dim3(kBlock); lc.dynamicSmemBytes = smem; lc.stream = e->stream;
     cudaLaunchAttribute attr[1];
     attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
     attr[0].val.programmaticStreamSerializationAllowed = 1;
-    const bool pdl = e->tune_pdl || (pp.flags & PF_TILE_WAIT);
-    lc.attrs = attr; lc.numAttrs = pdl ? 1 : 0;
+    lc.attrs = attr; lc.numAttrs = (pp.flags & PF_TILE_WAIT) ? 1 : 0;
     CUDA_TRY(cudaLaunchKernelEx(&lc, kern, pp));
     CUDA_TRY(cudaGetLastError());
     e->launches += 1;
-    const bool tma = ti && (kSubs == 1 ? pp.n_runs : pp.n_passive) > 0;  // the kernel's `use_tma`
-    e->last_kernel = BGR_KERNEL_BUNDLE | (uint32_t(VEC) << 4) | (uint32_t(MODE) << 8) | (uint32_t(mi) << 10) |
-                     (tma ? 1u << 12 : 0u) | (uint32_t(SUB) << 16);
+    const bool tma = ti && pp.n_runs > 0;  // the kernel's `use_tma`
+    // VEC 2, launch-bounds tier 1 (768 threads per SM), whole-tile work items
+    e->last_kernel = BGR_KERNEL_BUNDLE | (2u << 4) | (uint32_t(MODE) << 8) | (1u << 10) | (tma ? 1u << 12 : 0u) |
+                     (uint32_t(kTileRows) << 16);
     return BGR_OK;
 }
 
-int launch_fused_variant(bgr_engine* e, const ProgramParams& pp, cudaStream_t stream);
+int launch_fused_variant(bgr_engine* e, const ProgramParams& pp) {
+    if (e->bundle_opt) return launch_particles<2>(e, pp);         // per-entity presence
+    if (e->bundle_static_ck) return launch_particles<1>(e, pp);   // both columns checksummed with the finite assertion
+    return launch_particles<0>(e, pp);
+}
 
-int run_fused(bgr_engine* e, const Program& pg, uint32_t buf, uint32_t* chains_out) {
+int run_fused(bgr_engine* e, const Program& pg, uint32_t buf) {
     ProgramParams pp;
     std::memset(&pp, 0, sizeof pp);
     pp.seq = e->seq;
     pp.arena = e->arena;
     pp.order_base = e->cfg.order_base;
     pp.words = e->words; pp.tile_bytes = e->tile_bytes;
-    const uint32_t total_tiles = std::max(1u, e->tiles_for(pg.max_rows));  // at least one tile so a result block is published
+    pp.n_tiles = std::max(1u, e->tiles_for(pg.max_rows));  // at least one tile so a result block is published
     pp.n_ops = pg.n_ops; pp.n_saves = pg.n_saves;
     pp.live_rows = pg.live_rows;
     pp.flags = 0;
@@ -508,14 +497,8 @@ int run_fused(bgr_engine* e, const Program& pg, uint32_t buf, uint32_t* chains_o
         pp.spawn_ttl_lo = uint32_t(ttl); pp.spawn_ttl_hi = uint32_t(ttl >> 32);
     }
     if (!pg.has_spawn && simple && e->tune_passive_tma && !e->runs.empty() && 2u * e->passive_bytes <= 96u * 1024u) pp.flags |= PF_PASSIVE_TMA;
-    // Opt-in experiment (BGR_TUNE_SUB=128): cut every tile into 128-row work items handled by 64-thread blocks
-    // (kernels.cuh `SUB`).  Meant to balance small worlds (100k entities = 196 tiles on 132 SMs); the better balance is
-    // paid for with fewer warps per scheduler on the busy SMs and per-plane bulk copies, and the tick is
-    // issue-latency-bound on the hash, not imbalance-bound.  Kept for A/B runs.
-    const bool sub_items = e->tune_sub == 128;
-    if (sub_items && e->tune_vec == 2 && e->n_chains == 1) pp.flags |= PF_SUB_ITEMS;
     // one wave of blocks (every block runs one or two tiles): the tile's tail is the grid's tail
-    if (e->tune_passive_early == 1 || (e->tune_passive_early < 0 && total_tiles <= 3u * uint32_t(e->num_sms))) pp.flags |= PF_PASSIVE_EARLY;
+    if (e->tune_passive_early == 1 || (e->tune_passive_early < 0 && pp.n_tiles <= 3u * uint32_t(e->num_sms))) pp.flags |= PF_PASSIVE_EARLY;
     const Column& ct = e->cols[e->bt]; const Column& cv = e->cols[e->bv];
     if (ct.hash_kind != BGR_HASH_NONE) { pp.flags |= PF_CK_T; if (ct.hash_flags & BGR_HASH_FLAG_ASSERT_FINITE_F32) pp.flags |= PF_FIN_T; pp.ck_t_slot = uint32_t(ct.ck_slot); }
     if (cv.hash_kind != BGR_HASH_NONE) { pp.flags |= PF_CK_V; if (cv.hash_flags & BGR_HASH_FLAG_ASSERT_FINITE_F32) pp.flags |= PF_FIN_V; pp.ck_v_slot = uint32_t(cv.ck_slot); }
@@ -523,7 +506,7 @@ int run_fused(bgr_engine* e, const Program& pg, uint32_t buf, uint32_t* chains_o
     pp.l_off = e->cols[e->bl].first_plane * kPlaneBytes; pp.alive_off = e->words * kPlaneBytes;
     pp.need_t = ct.absent; pp.need_v = cv.absent; pp.need_tv = ct.absent | cv.absent; pp.need_l = e->cols[e->bl].absent;
     pp.n_runs = passive_needed ? uint32_t(e->runs.size()) : 0u;
-    pp.passive_bytes = (pp.flags & PF_SUB_ITEMS) ? uint32_t(e->passive.size()) * 128u * 4u : e->passive_bytes;
+    pp.passive_bytes = e->passive_bytes;
     for (size_t i = 0; i < e->runs.size(); ++i) pp.runs[i] = e->runs[i];
     pp.n_passive = passive_needed ? uint32_t(e->passive.size()) : 0u;
     for (size_t i = 0; i < e->passive.size(); ++i) {
@@ -534,26 +517,13 @@ int run_fused(bgr_engine* e, const Program& pg, uint32_t buf, uint32_t* chains_o
     }
     std::memcpy(pp.ops, pg.ops, sizeof(Op) * pg.n_ops);
 
-    // one launch per chain: contiguous tile ranges, own stream / accumulators / result block
-    const uint32_t chains = std::max(1u, std::min(uint32_t(e->n_chains), total_tiles));
-    *chains_out = chains;
-    // Chain c of this launch follows chain c of the previous one in stream order, which is all the ordering the data
-    // needs while both cover the same tiles.  A changed partition (rows spawned, first launch), stepwise work, or a
-    // caller-owned stream (whose earlier work we cannot see) makes every chain wait for everything before it.
-    if (chains != e->last_chains || total_tiles != e->last_total_tiles || !e->own_stream) e->main_dirty = true;
-    e->last_chains = chains; e->last_total_tiles = total_tiles;
-    if (chains > 1 && e->main_dirty) {
-        CUDA_TRY(cudaEventRecord(e->main_ev, e->stream));
-        for (uint32_t c = 0; c < chains; ++c) CUDA_TRY(cudaStreamWaitEvent(e->chain_stream[c], e->main_ev, 0));
-        e->main_dirty = false;
-    }
     // only worth it when request vectors are queued behind each other (bgr_submit_requests with others un-collected):
     // a synchronous caller collects before the next submit, so there is nothing to overlap with
     // ... and only on a stream the engine owns: on a caller's stream foreign work may sit between two submits and
     // become the programmatic-launch primary, which the per-tile flags know nothing about
-    const bool tiledep = e->tune_tiledep && chains == 1 && e->d_tile_done && e->own_stream && !pg.internal &&
+    const bool tiledep = e->tune_tiledep && e->d_tile_done && e->own_stream && !pg.internal &&
                          (e->tune_tiledep > 1 || !e->pending.empty());
-    if (e->tiledep_chain && total_tiles != e->tiledep_tiles) {
+    if (e->tiledep_chain && pp.n_tiles != e->tiledep_tiles) {
         // The tile range changed (rows crossed a tile boundary): a tile outside the previous launch's range may still be
         // in use by an OLDER overlapping launch that nothing would make this one wait for.  Rare: drain the stream.
         CUDA_TRY(cudaStreamSynchronize(e->stream));
@@ -568,65 +538,22 @@ int run_fused(bgr_engine* e, const Program& pg, uint32_t buf, uint32_t* chains_o
     }
     // start stagger: only launches that start on an idle GPU with at least two resident blocks per SM (overlapping
     // launches arrive dephased already)
-    if (e->tune_stagger_ns > 0 && !(pp.flags & PF_TILE_WAIT) && total_tiles / chains >= 2u * uint32_t(e->num_sms)) {
+    if (e->tune_stagger_ns > 0 && !(pp.flags & PF_TILE_WAIT) && pp.n_tiles >= 2u * uint32_t(e->num_sms)) {
         pp.stagger_ns = uint32_t(e->tune_stagger_ns); pp.stagger_div = uint32_t(e->num_sms);
     }
-    for (uint32_t c = 0; c < chains; ++c) {
-        pp.tile_begin = uint32_t(uint64_t(total_tiles) * c / chains);
-        pp.n_tiles = uint32_t(uint64_t(total_tiles) * (c + 1) / chains);
-        // overlapping launches (tile dependencies) must not share accumulators / tickets: rotate over kBufs sets — at
-        // most kBufs request vectors are un-collected, so a set is re-armed (before its launch's completion word is
-        // written) long before the launch kBufs later touches it
-        static_assert(bgr_engine::kMaxChains >= bgr_engine::kBufs, "one accumulator set per in-flight request vector");
-        const uint32_t set = tiledep ? uint32_t(e->seq % bgr_engine::kBufs) : c;
-        pp.accum = e->d_accum_c[set];
-        pp.ticket = e->d_ticket_c[set];
-        pp.out = (pg.internal ? e->d_internal_out : e->d_out[buf]) + size_t(c) * kResultStride;
-        pp.trace = nullptr;
-        if (e->d_trace && c == 0 && !pg.internal && e->seq - e->trace_first_seq < e->trace_cap) pp.trace = e->d_trace + (e->seq - e->trace_first_seq) * 4;
-        cudaStream_t stream = chains > 1 ? e->chain_stream[c] : e->stream;
-        int rc = launch_fused_variant(e, pp, stream);
-        if (rc != BGR_OK) return rc;
-        if (chains > 1) {  // everything later on the main stream (and external timing events) is ordered after the chains
-            CUDA_TRY(cudaEventRecord(e->chain_ev[c], stream));
-            CUDA_TRY(cudaStreamWaitEvent(e->stream, e->chain_ev[c], 0));
-        }
-    }
+    // overlapping launches (tile dependencies) must not share accumulators / tickets: rotate over kBufs sets — at most
+    // kBufs request vectors are un-collected, so a set is re-armed (before its launch's completion word is written) long
+    // before the launch kBufs later touches it
+    const uint32_t set = tiledep ? uint32_t(e->seq % bgr_engine::kBufs) : 0u;
+    pp.accum = e->d_accum_set[set];
+    pp.ticket = e->d_ticket_set[set];
+    pp.out = pg.internal ? e->d_internal_out : e->d_out[buf];
+    if (e->d_trace && !pg.internal && e->seq - e->trace_first_seq < e->trace_cap) pp.trace = e->d_trace + (e->seq - e->trace_first_seq) * 4;
+    int rc = launch_fused_variant(e, pp);
+    if (rc != BGR_OK) return rc;
     e->tiledep_chain = tiledep;
-    e->tiledep_seq = uint32_t(e->seq); e->tiledep_tiles = total_tiles;
+    e->tiledep_seq = uint32_t(e->seq); e->tiledep_tiles = pp.n_tiles;
     return BGR_OK;
-}
-
-int launch_fused_variant(bgr_engine* e, const ProgramParams& pp, cudaStream_t stream) {
-    const int v = e->bundle_opt ? 2 : e->tune_vec;
-    const bool st = e->bundle_static_ck && !e->bundle_opt;
-    if (pp.flags & PF_SUB_ITEMS) {  // small worlds: 128-row work items, 64-thread blocks, 768 threads per SM
-        constexpr int kSub = 128, kMinbSub = 768 / (kSub / 2);
-        if (e->bundle_opt) return launch_particles<2, 2, kMinbSub, kSub>(e, pp, 1, 2, 1, stream);
-        if (st) return launch_particles<2, 1, kMinbSub, kSub>(e, pp, 1, 1, 1, stream);
-        return launch_particles<2, 0, kMinbSub, kSub>(e, pp, 1, 0, 1, stream);
-    }
-    const int mb = e->tune_minb >= 8 ? 2 : (e->tune_minb >= 2 ? 1 : 0);  // launch-bounds tier: 1024 / 768 / unconstrained threads per SM
-    if (e->bundle_opt) {  // per-entity presence: one variant (2 rows per thread, 768 threads per SM)
-        constexpr int kMidOpt = 768 / int(kTileRows / 2);
-        return launch_particles<2, 2, kMidOpt>(e, pp, 1, 2, 1, stream);
-    }
-#define BGR_LAUNCH(VEC, VI)                                                                                \
-    if (v == VEC) {                                                                                        \
-        constexpr int kHi = (1024 / int(kTileRows / VEC)) > 32 ? 32 : (1024 / int(kTileRows / VEC));        \
-        constexpr int kMid = (768 / int(kTileRows / VEC)) < 1 ? 1 : (768 / int(kTileRows / VEC));           \
-        if (st && mb == 2) return launch_particles<VEC, 1, kHi>(e, pp, VI, 1, 2, stream);                          \
-        if (st && mb == 1) return launch_particles<VEC, 1, kMid>(e, pp, VI, 1, 1, stream);                         \
-        if (st) return launch_particles<VEC, 1, 1>(e, pp, VI, 1, 0, stream);                                       \
-        if (mb == 2) return launch_particles<VEC, 0, kHi>(e, pp, VI, 0, 2, stream);                                \
-        if (mb == 1) return launch_particles<VEC, 0, kMid>(e, pp, VI, 0, 1, stream);                               \
-        return launch_particles<VEC, 0, 1>(e, pp, VI, 0, 0, stream);                                               \
-    }
-    BGR_LAUNCH(1, 0)
-    BGR_LAUNCH(4, 2)
-    BGR_LAUNCH(2, 1)
-#undef BGR_LAUNCH
-    return fail(BGR_ERR_STATE, "bad BGR_TUNE_VEC");
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -665,7 +592,6 @@ int launch_tma(bgr_engine* e, const uint8_t* src, uint8_t* dst, uint32_t n_rows_
 // launch: stepwise path (generic schemas / systems)
 // ---------------------------------------------------------------------------------------------
 int run_stepwise(bgr_engine* e, const Program& pg, uint32_t buf) {
-    e->main_dirty = true;
     e->tiledep_chain = false;
     uint32_t live_rows = pg.live_rows;
     uint8_t* live = e->image(0);
@@ -875,15 +801,14 @@ void jit_specialise(bgr_engine* e) {
 // launch: generic one-launch program (any schema, compiled systems; generic_program.cuh)
 // ---------------------------------------------------------------------------------------------
 int run_generic(bgr_engine* e, const Program& pg, uint32_t buf) {
-    e->main_dirty = true;
     const bool prev_chain = e->tiledep_chain;  // the last operation on the stream was a signalling launch of the generated kernel
     e->tiledep_chain = false;
     GenericParams gp;
     std::memset(&gp, 0, sizeof gp);
     gp.arena = e->arena;
     gp.order_base = e->cfg.order_base;
-    gp.accum = e->d_accum_c[0];
-    gp.ticket = e->d_ticket_c[0];
+    gp.accum = e->d_accum_set[0];
+    gp.ticket = e->d_ticket_set[0];
     gp.out = pg.internal ? e->d_internal_out : e->d_out[buf];
     gp.seq = e->seq;
     if (e->d_trace && !pg.internal && e->seq - e->trace_first_seq < e->trace_cap) gp.trace = e->d_trace + (e->seq - e->trace_first_seq) * 4;
@@ -918,8 +843,8 @@ int run_generic(bgr_engine* e, const Program& pg, uint32_t buf) {
             if (wait) { gp.flags |= PF_TILE_WAIT; gp.wait_seq = e->tiledep_seq; gp.wait_items = n_items; }
             // overlapping launches must not share accumulators / tickets: one set per in-flight request vector (run_fused)
             const uint32_t set = uint32_t(e->seq % bgr_engine::kBufs);
-            gp.accum = e->d_accum_c[set];
-            gp.ticket = e->d_ticket_c[set];
+            gp.accum = e->d_accum_set[set];
+            gp.ticket = e->d_ticket_set[set];
         }
         void* args[] = {&gp};
         cudaLaunchConfig_t cfg;
@@ -988,8 +913,7 @@ int materialize_live(bgr_engine* e) {
     pg.passive_to_live = d.passive;
     pg.internal = true;
     const uint32_t kernel = e->last_kernel;
-    uint32_t chains = 1;
-    const int rc = use_bundle(e) ? run_fused(e, pg, 0, &chains) : run_generic(e, pg, 0);
+    const int rc = use_bundle(e) ? run_fused(e, pg, 0) : run_generic(e, pg, 0);
     e->last_kernel = kernel;
     return rc;
 }
@@ -1091,8 +1015,7 @@ int submit(bgr_engine* e, const bgr_session_info* sess, const bgr_request* reqs,
     if (rc != BGR_OK) return rc;
     DeferredLive next;
     if (fused && e->tune_defer_live && !e->live_touched) next = plan_deferral(pg);
-    uint32_t chains = 1;
-    rc = bundle ? run_fused(e, pg, buf, &chains) : generic ? run_generic(e, pg, buf) : run_stepwise(e, pg, buf);
+    rc = bundle ? run_fused(e, pg, buf) : generic ? run_generic(e, pg, buf) : run_stepwise(e, pg, buf);
     if (rc != BGR_OK) return rc;
     if (pg.defer_live) e->last_kernel |= BGR_KERNEL_DEFERRED_LIVE;
     if (pg.from_deferred) e->last_kernel |= BGR_KERNEL_FROM_DEFERRED;
@@ -1103,7 +1026,7 @@ int submit(bgr_engine* e, const bgr_session_info* sess, const bgr_request* reqs,
     e->deferred = next;
     e->live_touched = false;
     Pending pd;
-    pd.buf = buf; pd.n_saves = pg.n_saves; pd.seq = e->seq; pd.chains = chains; pd.gseq = e->group ? e->gseq : 0;
+    pd.buf = buf; pd.n_saves = pg.n_saves; pd.seq = e->seq; pd.gseq = e->group ? e->gseq : 0;
     std::memcpy(pd.frames, pg.save_frames, sizeof(int32_t) * pg.n_saves);
     std::memcpy(pd.totals, pg.save_totals, sizeof(uint32_t) * pg.n_saves);
     e->pending.push_back(pd);
@@ -1130,52 +1053,42 @@ int collect(bgr_engine* e, bgr_checksum* out, uint32_t cap, uint32_t* n_out) {
     Pending pd = e->pending.front();
     e->pending.pop_front();
     const uint64_t t_wait0 = host_ns();
-    // Completion: the last block of each chain's kernel publishes every result word as a self-validating pair
+    // Completion: the last block of the kernel publishes every result word as a self-validating pair
     // (v, v ^ result_tag(seq, i)) plus a completion pair; a word is accepted when its halves XOR to this launch's tag.
-    unsigned long long folded[kMaxSaves * kAccStride];
-    for (uint32_t i = 0; i < pd.n_saves * kAccStride; ++i) folded[i] = 0;
+    const volatile unsigned long long* blk = e->h_out[pd.buf];
     const uint32_t n_words = pd.n_saves * kAccStride;
-    for (uint32_t c = 0; c < pd.chains; ++c) {
-        const volatile unsigned long long* blk = &e->h_out[pd.buf][size_t(c) * kResultStride];
-        unsigned long long words[kMaxSaves * kAccStride];
-        uint32_t valid = 0;
-        bool seq_ok = false;
-        auto ready = [&]() {
-            if (!seq_ok) {
-                const unsigned long long a = blk[2 * kSeqIndex], b = blk[2 * kSeqIndex + 1];
-                if ((a ^ b) != result_tag(pd.seq, kSeqIndex)) return false;
-                seq_ok = true;
-            }
-            while (valid < n_words) {
-                const unsigned long long a = blk[2 * valid], b = blk[2 * valid + 1];
-                if ((a ^ b) != result_tag(pd.seq, valid)) return false;
-                words[valid++] = a;
-            }
-            return true;
-        };
-        bool done = false;
-        if (e->tune_poll && !pd.finished) {
-            for (int spin = 0; spin < 200000; ++spin) {
-                if (ready()) { done = true; break; }
-                __builtin_ia32_pause();
-            }
+    unsigned long long r[kMaxSaves * kAccStride];
+    uint32_t valid = 0;
+    bool seq_ok = false;
+    auto ready = [&]() {
+        if (!seq_ok) {
+            const unsigned long long a = blk[2 * kSeqIndex], b = blk[2 * kSeqIndex + 1];
+            if ((a ^ b) != result_tag(pd.seq, kSeqIndex)) return false;
+            seq_ok = true;
         }
-        if (!done) {  // the event / the stream is ordered after every chain
-            if (!pd.finished) {
-                if (e->tune_tiledep && e->tune_poll) CUDA_TRY(cudaStreamSynchronize(e->stream));
-                else CUDA_TRY(cudaEventSynchronize(e->ev[pd.buf]));
-            }
-            if (!ready()) return fail(BGR_ERR_CUDA, "request vector completed without publishing valid results");
+        while (valid < n_words) {
+            const unsigned long long a = blk[2 * valid], b = blk[2 * valid + 1];
+            if ((a ^ b) != result_tag(pd.seq, valid)) return false;
+            r[valid++] = a;
         }
-        // fold the chains' result blocks: XOR the column words, sum the live-row counts, OR the flags
-        for (uint32_t i = 0; i < n_words; ++i) {
-            const uint32_t w = i % kAccStride;
-            if (w == 6) folded[i] += words[i]; else if (w == 7) folded[i] |= words[i]; else folded[i] ^= words[i];
+        return true;
+    };
+    bool done = false;
+    if (e->tune_poll && !pd.finished) {
+        for (int spin = 0; spin < 200000; ++spin) {
+            if (ready()) { done = true; break; }
+            __builtin_ia32_pause();
         }
+    }
+    if (!done) {  // the event / the stream is ordered after the launch
+        if (!pd.finished) {
+            if (e->tune_tiledep && e->tune_poll) CUDA_TRY(cudaStreamSynchronize(e->stream));
+            else CUDA_TRY(cudaEventSynchronize(e->ev[pd.buf]));
+        }
+        if (!ready()) return fail(BGR_ERR_CUDA, "request vector completed without publishing valid results");
     }
     const uint64_t t_wait1 = host_ns();
     e->prof[3] += t_wait1 - t_wait0;
-    const unsigned long long* r = folded;
     e->last_partials.clear();
     bool nonfinite = false;
     // shard group: wait for every rank's block of this request vector and combine (XOR / sum / OR) across ranks
@@ -1220,7 +1133,7 @@ int collect(bgr_engine* e, bgr_checksum* out, uint32_t cap, uint32_t* n_out) {
 int drain(bgr_engine* e) {
     e->tiledep_chain = false;  // callers enqueue ordinary (fully ordered) work next
     if (e->pending.empty()) return BGR_OK;
-    CUDA_TRY(cudaStreamSynchronize(e->stream));  // every chain stream is joined into the main stream by an event
+    CUDA_TRY(cudaStreamSynchronize(e->stream));
     e->pending.for_each([](Pending& pd) { pd.finished = true; });
     return BGR_OK;
 }
@@ -1325,7 +1238,6 @@ int download_begin(bgr_engine* e, uint32_t column, uint32_t off, uint32_t len, u
                                                       reinterpret_cast<uint32_t*>(d.d_buf));
         e->launches += 1;
         CUDA_TRY(cudaGetLastError());
-        e->main_dirty = true;  // later chain launches overwrite the live image this kernel reads
         e->tiledep_chain = false;
         CUDA_TRY(cudaEventRecord(d.packed, e->stream));
         CUDA_TRY(cudaStreamWaitEvent(e->copy_stream, d.packed, 0));
@@ -1433,19 +1345,15 @@ BGR_API int bgr_engine_create(const bgr_config* cfg, bgr_engine** out) {
         if (se != cudaSuccess) { delete e; return fail(BGR_ERR_CUDA, cudaGetErrorString(se)); }
         e->own_stream = true;
     }
-    e->tune_vec = env_int("BGR_TUNE_VEC", 2);
-    e->tune_minb = env_int("BGR_TUNE_MINB", 2);
     e->tune_bps = env_int("BGR_TUNE_BPS", 0);
     e->tune_tma = env_int("BGR_TUNE_TMA", 1);
     e->tune_passive_tma = env_int("BGR_TUNE_PASSIVE_TMA", 1);
     e->tune_poll = env_int("BGR_TUNE_POLL", 1);
     e->tune_dynamic = env_int("BGR_TUNE_DYNAMIC", 1);
-    e->tune_pdl = env_int("BGR_TUNE_PDL", 0);
     e->tune_prefetch = env_int("BGR_TUNE_PREFETCH", 1);
     e->tune_grid = env_int("BGR_TUNE_GRID", 0);
     e->tune_tiledep = env_int("BGR_TUNE_TILEDEP", 1);
     e->tune_generic = env_int("BGR_TUNE_GENERIC", 1);
-    e->tune_sub = env_int("BGR_TUNE_SUB", 0);
     e->tune_generic_block = env_int("BGR_TUNE_GENERIC_BLOCK", 0);
     e->tune_jit = env_int("BGR_TUNE_JIT", 1);
     e->tune_jit_rows = env_int("BGR_TUNE_JIT_ROWS", 4);
@@ -1455,8 +1363,6 @@ BGR_API int bgr_engine_create(const bgr_config* cfg, bgr_engine** out) {
     e->tune_stagger_ns = env_int("BGR_TUNE_STAGGER_NS", 800);
     e->tune_bundle = env_int("BGR_TUNE_BUNDLE", 1);
     e->tune_defer_live = env_int("BGR_TUNE_DEFER_LIVE", 1);
-    e->n_chains = std::max(1, std::min(int(bgr_engine::kMaxChains), env_int("BGR_TUNE_CHAINS", 1)));
-    if (e->tune_vec != 1 && e->tune_vec != 2 && e->tune_vec != 4) e->tune_vec = 2;
     e->st.confirmed = 0;
     *out = e;
     return BGR_OK;
@@ -1499,11 +1405,6 @@ BGR_API void bgr_engine_destroy(bgr_engine* e) {
         if (d.packed) cudaEventDestroy(d.packed);
         if (d.done) cudaEventDestroy(d.done);
     }
-    for (int c = 0; c < bgr_engine::kMaxChains; ++c) {
-        if (e->chain_stream[c]) { cudaStreamSynchronize(e->chain_stream[c]); cudaStreamDestroy(e->chain_stream[c]); }
-        if (e->chain_ev[c]) cudaEventDestroy(e->chain_ev[c]);
-    }
-    if (e->main_ev) cudaEventDestroy(e->main_ev);
     if (e->own_stream && e->stream) cudaStreamDestroy(e->stream);
     delete e;
 }
@@ -1630,13 +1531,13 @@ BGR_API int bgr_build(bgr_engine* e) {
     CUDA_TRY(cudaMalloc(&e->d_kill, e->epad));
     CUDA_TRY(cudaMemsetAsync(e->d_kill, 0, e->epad, e->stream));
     const size_t acc_bytes = sizeof(unsigned long long) * kMaxSaves * kAccStride;
-    CUDA_TRY(cudaMalloc(&e->d_accum, acc_bytes * bgr_engine::kMaxChains));
-    CUDA_TRY(cudaMemsetAsync(e->d_accum, 0, acc_bytes * bgr_engine::kMaxChains, e->stream));
-    CUDA_TRY(cudaMalloc(&e->d_ticket, 4 * sizeof(unsigned int) * bgr_engine::kMaxChains));
-    CUDA_TRY(cudaMemsetAsync(e->d_ticket, 0, 4 * sizeof(unsigned int) * bgr_engine::kMaxChains, e->stream));
-    for (int c = 0; c < bgr_engine::kMaxChains; ++c) {
-        e->d_accum_c[c] = e->d_accum + size_t(c) * kMaxSaves * kAccStride;
-        e->d_ticket_c[c] = e->d_ticket + 4 * c;
+    CUDA_TRY(cudaMalloc(&e->d_accum, acc_bytes * bgr_engine::kBufs));
+    CUDA_TRY(cudaMemsetAsync(e->d_accum, 0, acc_bytes * bgr_engine::kBufs, e->stream));
+    CUDA_TRY(cudaMalloc(&e->d_ticket, 4 * sizeof(unsigned int) * bgr_engine::kBufs));
+    CUDA_TRY(cudaMemsetAsync(e->d_ticket, 0, 4 * sizeof(unsigned int) * bgr_engine::kBufs, e->stream));
+    for (int s = 0; s < bgr_engine::kBufs; ++s) {
+        e->d_accum_set[s] = e->d_accum + size_t(s) * kMaxSaves * kAccStride;
+        e->d_ticket_set[s] = e->d_ticket + 4 * s;
     }
     if (e->tune_tiledep) {
         const size_t nt = size_t(e->tiles_for(e->cfg.max_entities)) + 1;
@@ -1645,17 +1546,9 @@ BGR_API int bgr_build(bgr_engine* e) {
         CUDA_TRY(cudaMemsetAsync(e->d_tile_done, 0, nt * sizeof(unsigned int), e->stream));
         CUDA_TRY(cudaMemsetAsync(e->d_tile_cnt, 0, nt * sizeof(unsigned int), e->stream));
     }
-    if (e->n_chains > 1) {
-        for (int c = 0; c < e->n_chains; ++c) {
-            CUDA_TRY(cudaStreamCreateWithFlags(&e->chain_stream[c], cudaStreamNonBlocking));
-            CUDA_TRY(cudaEventCreateWithFlags(&e->chain_ev[c], cudaEventDisableTiming));
-        }
-        CUDA_TRY(cudaEventCreateWithFlags(&e->main_ev, cudaEventDisableTiming));
-        e->main_dirty = true;  // the memsets above
-    }
-    CUDA_TRY(cudaMalloc(&e->d_internal_out, sizeof(unsigned long long) * kResultStride * bgr_engine::kMaxChains));
+    CUDA_TRY(cudaMalloc(&e->d_internal_out, sizeof(unsigned long long) * kResultStride));
     for (int i = 0; i < bgr_engine::kBufs; ++i) {
-        const size_t out_bytes = sizeof(unsigned long long) * kResultStride * bgr_engine::kMaxChains;
+        const size_t out_bytes = sizeof(unsigned long long) * kResultStride;
         CUDA_TRY(cudaHostAlloc(&e->h_out[i], out_bytes, cudaHostAllocMapped));
         std::memset(e->h_out[i], 0, out_bytes);
         CUDA_TRY(cudaHostGetDevicePointer(&e->d_out[i], e->h_out[i], 0));
@@ -2196,13 +2089,12 @@ BGR_API int bgr_shard_group_join(bgr_engine* e, const char* name, uint32_t rank,
     if (!(e->cfg.flags & BGR_CFG_SHARDED)) return fail(BGR_ERR_STATE, "only a BGR_CFG_SHARDED engine can join a shard group");
     if (e->group) return fail(BGR_ERR_STATE, "engine is already in a shard group");
     if (!e->pending.empty()) return fail(BGR_ERR_STATE, "collect every submitted request vector before joining a shard group");
-    if (e->n_chains != 1) return fail(BGR_ERR_UNSUPPORTED, "BGR_TUNE_CHAINS > 1 cannot be combined with a shard group");
     CUDA_TRY(cudaSetDevice(e->cfg.device));
     CUDA_TRY(cudaStreamSynchronize(e->stream));
     auto* g = new ShardGroup();
     if (timeout_ms) g->timeout_ms = timeout_ms;
     std::string err;
-    const uint32_t block_words = uint32_t(kResultStride) * bgr_engine::kMaxChains;
+    const uint32_t block_words = uint32_t(kResultStride);
     static_assert(bgr_engine::kBufs == int(kGroupBufs) && kMaxSaves == int(kGroupMaxSaves) && kAccStride == int(kGroupAccStride),
                   "shard_group.hpp mirrors the engine's result block layout");
     if (!g->join(name, rank, world_size, block_words, e->seq, &err)) { delete g; return fail(BGR_ERR_STATE, err); }
@@ -2249,7 +2141,7 @@ BGR_API bgr_group* bgr_group_join(const char* name, uint32_t rank, uint32_t worl
     h->n_columns = n_columns;
     if (timeout_ms) h->g.timeout_ms = timeout_ms;
     std::string err;
-    if (!h->g.join(name, rank, world_size, uint32_t(kResultStride) * bgr_engine::kMaxChains, 0, &err)) { fail(BGR_ERR_STATE, err); delete h; return nullptr; }
+    if (!h->g.join(name, rank, world_size, uint32_t(kResultStride), 0, &err)) { fail(BGR_ERR_STATE, err); delete h; return nullptr; }
     return h;
 }
 BGR_API void bgr_group_leave(bgr_group* h) { delete h; }

@@ -44,7 +44,7 @@ constexpr int kMaxSaves = 40;
 constexpr int kMaxPassive = 64;   // word planes that no compiled system touches (per-thread fallback)
 constexpr int kMaxRuns = 8;       // runs of adjacent passive planes (TMA path)
 constexpr int kAccStride = 8;     // u64 per save: [0..5] column xors, [6] active rows, [7] flags
-// Result block (host-mapped, one per chain per buffer): kResultPairs PAIRS of u64.  Result word i is published as
+// Result block (host-mapped, one per buffer): kResultPairs PAIRS of u64.  Result word i is published as
 // (v, v ^ result_tag(seq, i)); pair kSeqIndex is the completion pair (v = seq).  The host accepts a word when the two
 // halves XOR to the tag of the sequence number it is waiting for: every word validates itself, so the GPU needs no
 // system-scope fence and no separate flag store behind the data (that round trip was 3.2 us of every synchronous call,
@@ -100,7 +100,6 @@ enum ProgFlags : uint32_t {
     PF_TILE_SIGNAL = 1024u,      // announce each block's FIRST tile in tile_done[] as soon as its stores are visible, and the
                                  // whole launch in *grid_done: what the next launch's first wave needs to start early
     PF_PASSIVE_EARLY = 8192u,    // single-wave grid: issue the passive planes' bulk stores at the top of a tile
-    PF_SUB_ITEMS = 4096u,        // host: launch the 128-row work-item variant (small worlds)
     PF_TILE_WAIT = 2048u,        // the previous launch on the stream was a PF_TILE_SIGNAL launch: start without waiting for
                                  // its grid (no griddepcontrol.wait) and wait per tile for tile_done[tile] or grid_done >=
                                  // wait_seq instead.  Tile i of tick k+1 only depends on tile i of tick k, so this grid's
@@ -119,7 +118,7 @@ struct ProgramParams {
     unsigned long long seq;     // sequence number of this launch: tags every published result pair (result_tag)
     unsigned long long* trace;  // nullptr, or this launch's row of the launch trace: [0] min block start, [1] max block end, [2] results published (globaltimer ns)
     uint32_t words, tile_bytes, n_ops, n_saves;
-    uint32_t tile_begin, n_tiles;  // this launch covers tiles [tile_begin, n_tiles) (one chain of the entity range)
+    uint32_t n_tiles;              // this launch covers tiles [0, n_tiles)
     unsigned int* tile_done;       // [tiles] sequence number of the last PF_TILE_SIGNAL launch that finished the tile
     unsigned int* tile_cnt;        // [tiles] warps of the current launch that finished the tile
     unsigned int* grid_done;       // sequence number of the last PF_TILE_SIGNAL launch that completed entirely
@@ -148,24 +147,16 @@ static_assert(sizeof(ProgramParams) <= 4000, "kernel parameter block must fit 4 
 // vector access helpers: VEC consecutive rows of one word plane = one 4*VEC byte access
 // ---------------------------------------------------------------------------------------------
 template <int VEC> __device__ __forceinline__ void vec_load(const uint8_t* p, uint32_t (&r)[VEC]);
-template <> __device__ __forceinline__ void vec_load<1>(const uint8_t* p, uint32_t (&r)[1]) { r[0] = __ldcs(reinterpret_cast<const uint32_t*>(p)); }
 template <> __device__ __forceinline__ void vec_load<2>(const uint8_t* p, uint32_t (&r)[2]) { uint2 v = __ldcs(reinterpret_cast<const uint2*>(p)); r[0] = v.x; r[1] = v.y; }
-template <> __device__ __forceinline__ void vec_load<4>(const uint8_t* p, uint32_t (&r)[4]) { uint4 v = __ldcs(reinterpret_cast<const uint4*>(p)); r[0] = v.x; r[1] = v.y; r[2] = v.z; r[3] = v.w; }
 
 template <int VEC> __device__ __forceinline__ void vec_store(uint8_t* p, const uint32_t (&r)[VEC]);
-template <> __device__ __forceinline__ void vec_store<1>(uint8_t* p, const uint32_t (&r)[1]) { __stcs(reinterpret_cast<uint32_t*>(p), r[0]); }
 template <> __device__ __forceinline__ void vec_store<2>(uint8_t* p, const uint32_t (&r)[2]) { __stcs(reinterpret_cast<uint2*>(p), make_uint2(r[0], r[1])); }
-template <> __device__ __forceinline__ void vec_store<4>(uint8_t* p, const uint32_t (&r)[4]) { __stcs(reinterpret_cast<uint4*>(p), make_uint4(r[0], r[1], r[2], r[3])); }
 
 // alive plane: VEC bytes packed little-endian into one register
 template <int VEC> __device__ __forceinline__ uint32_t alive_load(const uint8_t* p);
-template <> __device__ __forceinline__ uint32_t alive_load<1>(const uint8_t* p) { return __ldcs(p); }
 template <> __device__ __forceinline__ uint32_t alive_load<2>(const uint8_t* p) { return __ldcs(reinterpret_cast<const unsigned short*>(p)); }
-template <> __device__ __forceinline__ uint32_t alive_load<4>(const uint8_t* p) { return __ldcs(reinterpret_cast<const uint32_t*>(p)); }
 template <int VEC> __device__ __forceinline__ void alive_store(uint8_t* p, uint32_t a);
-template <> __device__ __forceinline__ void alive_store<1>(uint8_t* p, uint32_t a) { __stcs(p, (unsigned char)a); }
 template <> __device__ __forceinline__ void alive_store<2>(uint8_t* p, uint32_t a) { __stcs(reinterpret_cast<unsigned short*>(p), (unsigned short)a); }
-template <> __device__ __forceinline__ void alive_store<4>(uint8_t* p, uint32_t a) { __stcs(reinterpret_cast<uint32_t*>(p), a); }
 
 __device__ __forceinline__ unsigned long long globaltimer_ns() {
     unsigned long long t;
@@ -280,14 +271,12 @@ __device__ __forceinline__ void particle_step(uint32_t& tx, uint32_t& ty, uint32
 // byte carries absent bits (BGR_STRATEGY_OPTIONAL), every system and checksum applies the reference's query filter
 // (`Query<(&RollbackId, &T)>`, component_checksum.rs:73-77; `Query<(&mut Transform, &mut Velocity)>`, particles.rs:273)
 // per row, and Save / Load move the mask with the image (= the four-way match of component_snapshot.rs:99-115).
-// SUB: rows per work item.  SUB == kTileRows: one tile per block iteration (large worlds).  SUB < kTileRows: a tile is cut
-// into kTileRows / SUB row ranges handled by different (smaller) blocks — small worlds: 100k entities are 196 tiles on
-// 132 SMs, so half of the SMs carry two tiles and set the pace (issue-bound); 128-row items spread the
-// same rows as 5-6 items per SM.
-template <int VEC, int MODE, int MINB, int SUB = int(kTileRows)>
-__global__ void __launch_bounds__(SUB / VEC, MINB) k_particles_program(const __grid_constant__ ProgramParams p) {
-    constexpr int BLOCK = SUB / VEC;
-    constexpr uint32_t kSubs = kTileRows / SUB;
+// Two rows per thread, 256 threads per tile, three resident blocks (768 threads) per SM: DESIGN.md "What a synchronous
+// call costs" has the measurements against 1 and 4 rows per thread and the other launch-bounds tiers.
+template <int MODE>
+__global__ void __launch_bounds__(256, 3) k_particles_program(const __grid_constant__ ProgramParams p) {
+    constexpr int VEC = 2, BLOCK = 256;  // rows per thread, threads per block (__launch_bounds__)
+    static_assert(VEC * BLOCK == int(kTileRows), "a block iteration covers one tile");
     constexpr bool STATIC_CK = MODE == 1;
     constexpr bool OPT = MODE == 2;
     // STATIC_CK: both columns checksummed with the finite assertion (the stress test's registration) —
@@ -307,15 +296,10 @@ __global__ void __launch_bounds__(SUB / VEC, MINB) k_particles_program(const __g
     // into SM slots as this grid drains (hides launch latency and block ramp-up between back-to-back ticks) ...
     asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
     for (uint32_t i = tid; i < p.n_saves * kAccStride * 2; i += BLOCK) s_acc[i] = 0u;
-    const bool use_tma = (p.flags & PF_PASSIVE_TMA) && (kSubs == 1 ? p.n_runs : p.n_passive) > 0;
-    // the passive planes of one work item as bulk-copy chunks: whole runs of adjacent planes (full tiles), or this
-    // item's row range of every passive plane (sub-tiles); f(offset inside the tile, bytes)
-    auto for_each_passive_chunk = [&](uint32_t sub, auto&& f) {
-        if (kSubs == 1) {
-            for (uint32_t r = 0; r < p.n_runs; ++r) f(p.runs[r].off, p.runs[r].bytes);
-        } else {
-            for (uint32_t k = 0; k < p.n_passive; ++k) f(uint32_t(p.passive[k]) * kPlaneBytes + sub * uint32_t(SUB) * 4u, uint32_t(SUB) * 4u);
-        }
+    const bool use_tma = (p.flags & PF_PASSIVE_TMA) && p.n_runs > 0;
+    // the passive planes of a tile as bulk-copy chunks: whole runs of adjacent planes; f(offset inside the tile, bytes)
+    auto for_each_passive_chunk = [&](auto&& f) {
+        for (uint32_t r = 0; r < p.n_runs; ++r) f(p.runs[r].off, p.runs[r].bytes);
     };
     if (tid == 0 && use_tma) {
         mbar_init(&s_bar[0], 1);
@@ -359,18 +343,16 @@ __global__ void __launch_bounds__(SUB / VEC, MINB) k_particles_program(const __g
         fence_acq_rel_gpu();                      // every thread's stores are visible gpu-wide before its warp arrives
         __syncwarp();
         if (lane == 0) {
-            if (atomicAdd(&p.tile_cnt[t], 1u) == kTileRows / (32 * VEC) - 1) {  // last warp (of all the tile's items) to announce this tile
+            if (atomicAdd(&p.tile_cnt[t], 1u) == kTileRows / (32 * VEC) - 1) {  // last warp to announce this tile
                 p.tile_cnt[t] = 0u;
                 fence_acq_rel_gpu();
                 st_release_gpu(&p.tile_done[t], p.done_seq);
             }
         }
     };
-    const uint32_t n_items = p.n_tiles * kSubs;
-    for (uint32_t item = p.tile_begin * kSubs + blockIdx.x; item < n_items; ++it) {
-        if (dynamic && tid == 0) claimed = p.tile_begin * kSubs + gridDim.x + atomicAdd(&p.ticket[1], 1u);  // published after the loads below
-        const uint32_t tile = item / kSubs, sub = item % kSubs;
-        const uint32_t i0 = sub * uint32_t(SUB) + tid * VEC;  // first row of this thread inside the tile
+    for (uint32_t tile = blockIdx.x; tile < p.n_tiles; ++it) {
+        if (dynamic && tid == 0) claimed = gridDim.x + atomicAdd(&p.ticket[1], 1u);  // published after the loads below
+        const uint32_t i0 = tid * VEC;  // first row of this thread inside the tile
         if (tile_wait && tile < p.wait_tiles) {
             // the previous tick's kernel may still be running: this tile's images are complete once it has signalled
             if (lane == 0)
@@ -392,7 +374,7 @@ __global__ void __launch_bounds__(SUB / VEC, MINB) k_particles_program(const __g
             uint8_t* dst = s_passive + size_t(buf) * p.passive_bytes;
             mbar_arrive_expect_tx(&s_bar[buf], p.passive_bytes);
             uint32_t o = 0;
-            for_each_passive_chunk(sub, [&](uint32_t off, uint32_t bytes) {
+            for_each_passive_chunk([&](uint32_t off, uint32_t bytes) {
                 tma_load_1d(dst + o, src + off, bytes, &s_bar[buf]);
                 o += bytes;
             });
@@ -445,16 +427,15 @@ __global__ void __launch_bounds__(SUB / VEC, MINB) k_particles_program(const __g
             // the next tile's first touch is a dependent DRAM read at the top of the tile (20 % of all stall samples in
             // the round-1 profile): pull its active planes (8 word planes + alive = 132 lines) into L2 now
             const uint32_t nxt = __shfl_sync(0xffffffffu, claimed, 0);
-            if (nxt < n_items) {
-                const uint32_t nsub = nxt % kSubs;
-                const uint8_t* img = p.arena + ((p.flags & PF_READ_LIVE) ? size_t(0) : (size_t(p.ops[0].image_off256) << 8)) + size_t(nxt / kSubs) * p.tile_bytes;
-                constexpr uint32_t kLines = uint32_t(SUB) * 4u / 128u, kAliveLines = (uint32_t(SUB) + 127u) / 128u;  // per plane / alive range of one item
+            if (nxt < p.n_tiles) {
+                const uint8_t* img = p.arena + ((p.flags & PF_READ_LIVE) ? size_t(0) : (size_t(p.ops[0].image_off256) << 8)) + size_t(nxt) * p.tile_bytes;
+                constexpr uint32_t kLines = kPlaneBytes / 128u, kAliveLines = (kTileRows + 127u) / 128u;  // per plane / alive plane of a tile
                 for (uint32_t l = lane; l < 8u * kLines + kAliveLines; l += 32u) {
                     const uint32_t plane = l / kLines, line = l % kLines;
-                    const size_t off = plane < 3 ? p.t_off + size_t(plane) * kPlaneBytes + size_t(nsub) * SUB * 4u
-                                     : plane < 6 ? p.v_off + size_t(plane - 3) * kPlaneBytes + size_t(nsub) * SUB * 4u
-                                     : plane < 8 ? p.l_off + size_t(plane - 6) * kPlaneBytes + size_t(nsub) * SUB * 4u
-                                                 : size_t(p.alive_off) + size_t(nsub) * SUB;
+                    const size_t off = plane < 3 ? p.t_off + size_t(plane) * kPlaneBytes
+                                     : plane < 6 ? p.v_off + size_t(plane - 3) * kPlaneBytes
+                                     : plane < 8 ? p.l_off + size_t(plane - 6) * kPlaneBytes
+                                                 : size_t(p.alive_off);
                     asm volatile("prefetch.global.L2 [%0];" ::"l"(img + off + size_t(line) * 128u));
                 }
             }
@@ -472,12 +453,12 @@ __global__ void __launch_bounds__(SUB / VEC, MINB) k_particles_program(const __g
                 if (p.ops[i].kind != OP_SAVE || (p.ops[i].flags & (OPF_NO_STORE | OPF_SKIP_PASSIVE))) continue;
                 uint8_t* img = p.arena + (size_t(p.ops[i].image_off256) << 8) + tile_off;
                 uint32_t o = 0;
-                for_each_passive_chunk(sub, [&](uint32_t off, uint32_t bytes) { tma_store_1d(img + off, src + o, bytes); o += bytes; });
+                for_each_passive_chunk([&](uint32_t off, uint32_t bytes) { tma_store_1d(img + off, src + o, bytes); o += bytes; });
             }
             if (p.flags & PF_WRITE_LIVE_PASSIVE) {
                 uint8_t* img = p.arena + tile_off;
                 uint32_t o = 0;
-                for_each_passive_chunk(sub, [&](uint32_t off, uint32_t bytes) { tma_store_1d(img + off, src + o, bytes); o += bytes; });
+                for_each_passive_chunk([&](uint32_t off, uint32_t bytes) { tma_store_1d(img + off, src + o, bytes); o += bytes; });
             }
             tma_commit();
         };
@@ -643,11 +624,11 @@ __global__ void __launch_bounds__(SUB / VEC, MINB) k_particles_program(const __g
         if (dynamic) {
             const uint32_t slot = it % kRing, use = it / kRing;  // entry of iteration it + 1
             mbar_wait(&s_full[slot], use & 1u);
-            item = s_tile[slot];
+            tile = s_tile[slot];
             __syncwarp();
             if (lane == 0) mbar_arrive(&s_empty[slot]);
         } else {
-            item += gridDim.x;
+            tile += gridDim.x;
         }
     }
     if (use_tma && tid == 0) tma_wait_all();  // every bulk store has landed before the results are published

@@ -380,10 +380,10 @@ BGR_API int bgr_last_path(bgr_engine* e, uint32_t* fused_out);   /* 1 if the las
  * csrc/generic_program_jit.cuh): every non-bundle request vector then runs on it; 0 = the interpreter kernel (same results).
  * Env BGR_TUNE_JIT: 0 never, 1 (default) engines created for >= 16384 entities, 2 always. */
 BGR_API int bgr_generic_specialised(bgr_engine* e, uint32_t* specialised_out);
-/* Which kernel the last request vector executed (0 before the first one).  Tuning knobs fall back quietly (an optional
- * column forces VEC 2, BGR_TUNE_SUB=128 needs VEC 2 ...): this says what actually ran.
+/* Which kernel the last request vector executed (0 before the first one).  Tuning knobs fall back quietly: this says
+ * what actually ran.  The bundle currently always reports VEC 2, tier 1 and 512-row work items.
  *   bits 0-3   kind: BGR_KERNEL_*
- *   bits 4-7   bundle: rows per thread (VEC: 1, 2 or 4)
+ *   bits 4-7   bundle: rows per thread (VEC)
  *   bits 8-9   bundle: MODE 0 (checksum flags tested at run time), 1 (Transform and Velocity both checksummed with
  *              BGR_HASH_FLAG_ASSERT_FINITE_F32: specialised), 2 (per-entity presence of optional columns)
  *   bits 10-11 bundle: launch-bounds tier, 0 unconstrained, 1 768 threads per SM, 2 1024 threads per SM

@@ -62,12 +62,8 @@ def one(workload, env, K=300):
 
 def main():
     workloads = sys.argv[1:] or ["stress_1m_d8", "stress_100k_d8"]
-    variants = [{}]
-    for vec in (1, 2, 4):
-        for minb in (1, 2, 8):
-            variants.append({"BGR_TUNE_VEC": vec, "BGR_TUNE_MINB": minb})
-    variants += [{"BGR_TUNE_CHAINS": 2}, {"BGR_TUNE_CHAINS": 4}, {"BGR_TUNE_DYNAMIC": 0}, {"BGR_TUNE_PREFETCH": 0},
-                 {"BGR_TUNE_BPS": 2}, {"BGR_TUNE_BPS": 1}, {"BGR_TUNE_POLL": 0}]
+    variants = [{}, {"BGR_TUNE_DYNAMIC": 0}, {"BGR_TUNE_PREFETCH": 0}, {"BGR_TUNE_BPS": 2}, {"BGR_TUNE_BPS": 1},
+                {"BGR_TUNE_POLL": 0}]
     extra = os.environ.get("SWEEP_EXTRA")
     if extra:
         variants = [{}] + json.loads(extra)

@@ -1,9 +1,8 @@
 """-m gpu: every variant of the compiled particles kernel the engine can select, against the oracle.
 
-The bundle kernel (k_particles_program) is instantiated per rows-per-thread (BGR_TUNE_VEC), checksum mode (MODE 0: the
-checksum / finite flags are tested at run time; MODE 1: both columns checksummed with the finite assertion; MODE 2:
-optional columns), launch-bounds tier (BGR_TUNE_MINB) and work-item size, and a launch moves the passive planes by TMA
-bulk copies or per thread.  Each case asserts through Engine.last_kernel() that the variant it names is the one that
+The bundle kernel (k_particles_program) is instantiated per checksum mode (MODE 0: the checksum / finite flags are
+tested at run time; MODE 1: both columns checksummed with the finite assertion; MODE 2: optional columns), and a launch
+moves the passive planes by TMA bulk copies or per thread.  Each case asserts through Engine.last_kernel() that the variant it names is the one that
 ran, then compares checksums, live state, ring frames and snapshot bytes with the oracle."""
 import numpy as np
 import pytest
@@ -110,35 +109,20 @@ def test_non_finite_raises_exactly_when_the_oracle_panics(setup, column, flags):
 
 
 # ---------------------------------------------------------------------------------------------------------------------
-# the instantiation matrix: VEC x launch-bounds tier x MODE, single-wave and multi-wave grids
+# the instantiation matrix: MODE 0 and 1, single-wave and multi-wave grids
 # ---------------------------------------------------------------------------------------------------------------------
 @pytest.mark.parametrize("n", [SINGLE_WAVE, MULTI_WAVE])
 @pytest.mark.parametrize("mode", [0, 1])
-@pytest.mark.parametrize("minb", ["1", "2", "8"])
-@pytest.mark.parametrize("vec", ["1", "2", "4"])
-def test_every_vec_tier_mode_instantiation_matches_the_oracle(monkeypatch, vec, minb, mode, n):
-    monkeypatch.setenv("BGR_TUNE_VEC", vec)
-    monkeypatch.setenv("BGR_TUNE_MINB", minb)
+def test_every_vec_tier_mode_instantiation_matches_the_oracle(mode, n):
     big = n == MULTI_WAVE
-    r = run_particles_synctest_pair(n, 2 if big else 4, 6 if big else 12, seed=int(vec) * 10 + int(minb), ttl_lo=2,
+    r = run_particles_synctest_pair(n, 2 if big else 4, 6 if big else 12, seed=22, ttl_lo=2,
                                     ttl_hi=20, z_fraction=0.2, peek_check=not big,
                                     checksums=MODE1 if mode else MODE0_SETUPS["both_plain"])
     k = r["kernel"]
     assert r["fused"] and k.kind == "bundle"
-    assert (k.vec, k.mode, k.tier, k.item_rows) == (int(vec), mode, {"1": 0, "2": 1, "8": 2}[minb], 512)
+    assert (k.vec, k.mode, k.tier, k.item_rows) == (2, mode, 1, 512)
     assert k.passive_tma   # the example's layout: the Transform's 7 passive planes are one TMA run
     _assert_parity(r, peek=not big)
-
-
-@pytest.mark.parametrize("mode", [0, 1])
-def test_sub_tile_work_items_in_both_checksum_modes(monkeypatch, mode):
-    """BGR_TUNE_SUB=128: 128-row work items, 64-thread blocks, passive planes as per-plane bulk copies."""
-    monkeypatch.setenv("BGR_TUNE_SUB", "128")
-    r = run_particles_synctest_pair(2100, 4, 12, seed=61, ttl_lo=1, ttl_hi=20, spawn_rate=30, spawn_ttl=5,
-                                    peek_check=True, z_fraction=0.2, checksums=MODE1 if mode else MODE0_SETUPS["v_only"])
-    k = r["kernel"]
-    assert (k.kind, k.vec, k.mode, k.tier, k.item_rows) == ("bundle", 2, mode, 1, 128)
-    _assert_parity(r)
 
 
 # ---------------------------------------------------------------------------------------------------------------------
@@ -272,9 +256,8 @@ def test_passive_plane_limit(planes):
         assert all(k.kind == "stepwise_flat" for k in kernels)
 
 
-def test_optional_column_forces_vec2_mode2(monkeypatch):
-    """BGR_TUNE_VEC=4 is ignored by the presence-aware variant: it always runs 2 rows per thread."""
-    monkeypatch.setenv("BGR_TUNE_VEC", "4")
+def test_optional_column_runs_mode2():
+    """An optional column selects the presence-aware variant (MODE 2, 2 rows per thread)."""
     eng, orc, cols = _extra_pair(["T", "V", "L", ("Tag", 4, COPY | capi.BGR_STRATEGY_OPTIONAL)], 2000)
     info, vectors = _synctest_vectors(10, 3, 8)
     kernels = _run_vectors(eng, orc, cols, info, vectors)
@@ -299,10 +282,10 @@ def test_knob_matches_the_oracle(monkeypatch, knob, value, n):
     _assert_parity(r, peek=not big)
 
 
-@pytest.mark.parametrize("knob,value", [("BGR_TUNE_PDL", "1"), ("BGR_TUNE_POLL", "0")])
+@pytest.mark.parametrize("knob,value", [("BGR_TUNE_POLL", "0")])
 def test_knob_with_four_submits_in_flight(monkeypatch, knob, value):
-    """Programmatic dependent launch between consecutive fused kernels / collect() waiting on the event instead of
-    polling the result block, with four request vectors queued and spawns changing the tile range."""
+    """collect() waiting on the event instead of polling the result block, with four request vectors queued and spawns
+    changing the tile range."""
     monkeypatch.setenv(knob, value)
     eng, orc, cols = _extra_pair(["T", "V", "L"], 5000, spawn_rate=40, spawn_ttl=7, seed=9)
     info, vectors = _synctest_vectors(24, 3, 8, spawn_ticks=(1, 2, 11), input_delay=2)
