@@ -231,7 +231,7 @@ struct bgr_engine {
     bool bundle_static_ck = false;  // both columns checksummed with the finite assertion: fully specialised kernel
     // generic one-launch program (generic_program.cuh): any schema whose tile fits shared memory + the compiled systems
     bool generic_ok = false;
-    int generic_bps[4] = {0, 0, 0, 0};  // resident blocks per SM of k_generic_program<64 | 128 | 256 | 512> (occupancy query, cached)
+    int generic_bps = 0;            // resident blocks per SM of k_generic_program (occupancy query, cached)
     int tune_jit = 1;               // 0 never, 1 worlds of >= 16k entities, 2 always: NVRTC-specialised generic program (jit.hpp)
     int tune_jit_rows = 4;          // rows of a tile per thread in the specialised kernel (1, 2, 4)
     JitKernel jit;                  // fn == nullptr: the interpreter kernel runs.  Work item = a whole tile
@@ -240,7 +240,6 @@ struct bgr_engine {
     unsigned int* d_item_done = nullptr;   // [4 * tiles] GenericParams::item_done (quarter-tile work items at most)
     const void* jit_chain_kernel = nullptr;  // the signalling launch `tiledep_chain` refers to (its work-item partition must match)
     int tune_jit_item = 0;          // 0 auto (quarter tiles below 3 tiles per SM), 512 / 256 / 128 force the rows per work item
-    int tune_generic_block = 0;     // 0 = 128; 64 / 256 / 512 force
     int tune_passive_early = -1;    // -1: early passive stores for single-wave grids (auto); 0 never; 1 always
     int tune_stagger_ns = 800;      // start-of-grid phase stagger between the resident blocks of an SM (synchronous launches; measured -1.3 %)
     int tune_generic = 1;
@@ -863,22 +862,17 @@ int run_generic(bgr_engine* e, const Program& pg, uint32_t buf) {
         return BGR_OK;
     }
     const size_t smem = size_t((e->tile_bytes + 127u) & ~127u);
-    // rows of a tile per thread: 8 (64 threads per tile), 4 (128), 2 (256) or 1 (512).  More rows per thread = more
-    // independent hash chains interleaved in one warp
-    const int block = e->tune_generic_block == 64 || e->tune_generic_block == 256 || e->tune_generic_block == 512 ? e->tune_generic_block : 128;
-    const int vi = block == 64 ? 0 : block == 128 ? 1 : block == 256 ? 2 : 3;
-    const void* fn = vi == 0 ? (const void*)k_generic_program<64> : vi == 1 ? (const void*)k_generic_program<128>
-                   : vi == 2 ? (const void*)k_generic_program<256> : (const void*)k_generic_program<512>;
-    if (e->generic_bps[vi] == 0) {
+    const void* fn = (const void*)k_generic_program;
+    if (e->generic_bps == 0) {
         if (smem > 48 * 1024) CUDA_TRY(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem)));
         int nb = 0;
-        CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, fn, block, smem));
-        e->generic_bps[vi] = std::max(1, nb);
+        CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, fn, kGenericBlock, smem));
+        e->generic_bps = std::max(1, nb);
     }
-    uint32_t grid = std::max(1u, std::min(gp.n_tiles, uint32_t(e->num_sms * e->generic_bps[vi])));
+    uint32_t grid = std::max(1u, std::min(gp.n_tiles, uint32_t(e->num_sms * e->generic_bps)));
     if (e->tune_grid > 0) grid = std::min(grid, uint32_t(e->tune_grid));  // tests: several tiles per block on small worlds
     void* args[] = {&gp};
-    CUDA_TRY(cudaLaunchKernel(fn, dim3(grid), dim3(block), args, smem, e->stream));
+    CUDA_TRY(cudaLaunchKernel(fn, dim3(grid), dim3(kGenericBlock), args, smem, e->stream));
     CUDA_TRY(cudaGetLastError());
     e->launches += 1;
     e->last_kernel = BGR_KERNEL_GENERIC_INTERPRETER;
@@ -1354,7 +1348,6 @@ BGR_API int bgr_engine_create(const bgr_config* cfg, bgr_engine** out) {
     e->tune_grid = env_int("BGR_TUNE_GRID", 0);
     e->tune_tiledep = env_int("BGR_TUNE_TILEDEP", 1);
     e->tune_generic = env_int("BGR_TUNE_GENERIC", 1);
-    e->tune_generic_block = env_int("BGR_TUNE_GENERIC_BLOCK", 0);
     e->tune_jit = env_int("BGR_TUNE_JIT", 1);
     e->tune_jit_rows = env_int("BGR_TUNE_JIT_ROWS", 4);
     e->tune_jit_item = env_int("BGR_TUNE_JIT_ITEM", 0);

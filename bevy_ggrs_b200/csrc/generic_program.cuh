@@ -34,10 +34,11 @@
 namespace bgr {
 
 constexpr int kMaxGenericSys = 8;
-// threads per block: 64 / 128 / 256 / 512 = 8 / 4 / 2 / 1 rows of the tile per thread; 128 is the default (four independent
-// hash chains interleaved per thread).  This kernel is the INTERPRETER: it reads the
+// threads per block: 128 = 4 rows of the tile per thread, four independent hash chains interleaved per thread (DESIGN.md
+// has the measurements against 1, 2 and 8 rows).  This kernel is the INTERPRETER: it reads the
 // schema from its parameter block.  bgr_build also compiles the registration's own kernel with NVRTC when it can
 // (generic_program_jit.cuh, jit.hpp), and this one is then only the fallback.
+constexpr int kGenericBlock = 128;
 
 struct SysSpec {
     uint32_t id;      // bgr_system
@@ -124,7 +125,7 @@ __device__ __forceinline__ void hash_words_column(const uint32_t* col, const uin
     }
 }
 
-template <int kGenericBlock>
+#ifndef __CUDACC_RTC__  // the run-time specialisation only needs the structs and helpers: its cubin holds k_generic_jit alone
 __global__ void __launch_bounds__(kGenericBlock) k_generic_program(const __grid_constant__ GenericParams p) {
     constexpr int kRows = kTileRows / kGenericBlock;  // rows of a tile per thread
     extern __shared__ __align__(128) uint8_t s_buf[];  // one tile
@@ -370,5 +371,6 @@ __global__ void __launch_bounds__(kGenericBlock) k_generic_program(const __grid_
         }
     }
 }
+#endif  // !__CUDACC_RTC__
 
 }  // namespace bgr

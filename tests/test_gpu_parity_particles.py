@@ -268,15 +268,14 @@ def test_pipelined_submits_overlap_without_observable_change(monkeypatch, tilede
             assert np.array_equal(pe[1].astype(bool), m) and np.array_equal(pe[0][m], po[0][m])
 
 
-@pytest.mark.parametrize("block", ["64", "128", "256", "512"])
+@pytest.mark.parametrize("jit_rows", ["4", "2", "1"])
 @pytest.mark.parametrize("n,d,ticks", [(257, 3, 14), (10_000, 8, 12)])
-def test_particles_world_on_the_generic_program_matches_oracle(monkeypatch, generic_kernel, n, d, ticks, block):
+def test_particles_world_on_the_generic_program_matches_oracle(monkeypatch, generic_kernel, n, d, ticks, jit_rows):
     """BGR_TUNE_BUNDLE=0 takes the specialised particles kernel out: the same world runs on the generic one-launch
     program (shared-memory tile, systems and hashes driven by the registration) and must match the oracle bit for bit,
     including despawns inside the window and the passive Transform planes of every snapshot."""
     monkeypatch.setenv("BGR_TUNE_BUNDLE", "0")
-    monkeypatch.setenv("BGR_TUNE_GENERIC_BLOCK", block)   # interpreter: 8 / 4 (default) / 2 / 1 rows of a tile per thread
-    monkeypatch.setenv("BGR_TUNE_JIT_ROWS", {"64": "4", "128": "4", "256": "2", "512": "1"}[block])  # specialised kernel: 4 / 2 / 1
+    monkeypatch.setenv("BGR_TUNE_JIT_ROWS", jit_rows)  # specialised whole-tile kernel: 4 / 2 / 1 rows per thread
     r = run_particles_synctest_pair(n, d, ticks, seed=5, ttl_lo=3, ttl_hi=40, peek_check=True, z_fraction=0.3)
     assert r["fused"] and r["launches"] == ticks
     assert r["checksums_equal"] and r["state_equal"] and r["peek_equal"]
@@ -284,15 +283,14 @@ def test_particles_world_on_the_generic_program_matches_oracle(monkeypatch, gene
 
 
 @pytest.mark.timeout(180)
-@pytest.mark.parametrize("grid,block", [("3", "128"), ("7", "256"), ("40", "64")])
-def test_generic_program_blocks_that_run_many_tiles(monkeypatch, generic_kernel, grid, block):
+@pytest.mark.parametrize("grid,jit_rows", [("3", "4"), ("7", "2"), ("40", "4")])
+def test_generic_program_blocks_that_run_many_tiles(monkeypatch, generic_kernel, grid, jit_rows):
     """The generic one-launch program with far fewer blocks than tiles (BGR_TUNE_GRID): every block claims tile after
     tile from the global counter, reloads its shared-memory tile, and must wait for its own bulk stores before the
     buffer is overwritten.  (Without the cap a world needs > 1.2M entities before a block sees a second tile.)"""
     monkeypatch.setenv("BGR_TUNE_BUNDLE", "0")
     monkeypatch.setenv("BGR_TUNE_GRID", grid)
-    monkeypatch.setenv("BGR_TUNE_GENERIC_BLOCK", block)
-    monkeypatch.setenv("BGR_TUNE_JIT_ROWS", {"64": "4", "128": "4", "256": "2"}[block])
+    monkeypatch.setenv("BGR_TUNE_JIT_ROWS", jit_rows)
     r = run_particles_synctest_pair(60_000, 4, 10, seed=23, ttl_lo=3, ttl_hi=40, peek_check=True, z_fraction=0.2)
     assert r["fused"] and r["launches"] == 10
     assert r["checksums_equal"] and r["state_equal"] and r["peek_equal"]
