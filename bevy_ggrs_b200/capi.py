@@ -46,6 +46,10 @@ BGR_CFG_SHARDED = 2
 BGR_CFG_SKIP_UNCHANGED_PLANES = 4
 BGR_CFG_DESYNC_CAPTURE = 8
 BGR_DESYNC_NO_INDEX = 0xFFFFFFFF
+# P2P desync reports
+BGR_DIGEST_BLOCK_ROWS = 512
+BGR_FRAME_BLOB_MAGIC = 0x50424752
+BGR_FRAME_BLOB_VERSION = 1
 # bgr_last_kernel: kind in bits 0-3
 BGR_KERNEL_NONE, BGR_KERNEL_STEPWISE_TMA, BGR_KERNEL_STEPWISE_FLAT, BGR_KERNEL_BUNDLE, \
     BGR_KERNEL_GENERIC_INTERPRETER, BGR_KERNEL_GENERIC_NVRTC = range(6)
@@ -94,6 +98,18 @@ class bgr_desync_summary(C.Structure):
                 ("words_differing", C.c_uint64), ("elapsed_ns_first", C.c_uint64), ("elapsed_ns_latest", C.c_uint64)]
 
 
+class bgr_frame_digest_header(C.Structure):
+    _fields_ = [("layout", C.c_uint64), ("frame", C.c_int32), ("rows", C.c_uint32), ("n_blocks", C.c_uint32),
+                ("n_columns", C.c_uint32), ("active", C.c_uint64), ("elapsed_ns", C.c_uint64), ("rng", C.c_uint64 * 4),
+                ("root", C.c_uint64)]
+
+
+class bgr_frame_blob_header(C.Structure):
+    _fields_ = [("magic", C.c_uint32), ("version", C.c_uint32), ("layout", C.c_uint64), ("frame", C.c_int32),
+                ("rows", C.c_uint32), ("words", C.c_uint32), ("n_blocks", C.c_uint32), ("n_exported", C.c_uint32),
+                ("reserved", C.c_uint32), ("elapsed_ns", C.c_uint64), ("rng", C.c_uint64 * 4)]
+
+
 u32p = C.POINTER(C.c_uint32)
 i32p = C.POINTER(C.c_int32)
 u64p = C.POINTER(C.c_uint64)
@@ -138,6 +154,16 @@ PROTOTYPES = {
                                   C.c_uint32, C.POINTER(bgr_desync_record), C.c_uint32, u32p, i32p]),
     "bgr_peek_first": (C.c_int, [C.c_void_p, C.c_int32, C.c_uint32, C.c_uint32, C.c_uint32, C.c_void_p, C.c_uint32,
                                  C.c_void_p, i32p]),
+    "bgr_retain_confirmed": (C.c_int, [C.c_void_p, C.c_uint32, C.c_uint32]),
+    "bgr_retained_frames": (C.c_int, [C.c_void_p, i32p, C.c_uint32, u32p]),
+    "bgr_frame_digest": (C.c_int, [C.c_void_p, C.c_int32, C.POINTER(bgr_frame_digest_header), C.c_void_p, C.c_uint32, i32p]),
+    "bgr_digest_mismatch": (C.c_int, [C.POINTER(bgr_frame_digest_header), C.c_void_p, C.POINTER(bgr_frame_digest_header),
+                                      C.c_void_p, C.c_void_p, C.c_uint32, u32p, u32p]),
+    "bgr_frame_export": (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p, C.c_uint32, C.c_void_p, C.c_size_t,
+                                   C.POINTER(C.c_size_t), i32p]),
+    "bgr_desync_diff_remote": (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p, C.c_size_t, C.POINTER(bgr_desync_summary),
+                                         C.POINTER(bgr_desync_column), C.c_uint32, C.POINTER(bgr_desync_record),
+                                         C.c_uint32, u32p, i32p]),
     "bgr_save_world": (C.c_int, [C.c_void_p, C.POINTER(bgr_checksum)]),
     "bgr_load_world": (C.c_int, [C.c_void_p]),
     "bgr_advance_world": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint32]),
@@ -182,6 +208,8 @@ PROTOTYPES = {
     "bgr_ring_create_capture": (C.c_void_p, [C.c_uint32]),
     "bgr_ring_first": (C.c_int, [C.c_void_p, C.c_int32, u32p, i32p]),
     "bgr_ring_slots_in_use": (C.c_int, [C.c_void_p, u32p]),
+    "bgr_ring_set_retention": (C.c_int, [C.c_void_p, C.c_uint32, C.c_uint32]),
+    "bgr_ring_retained": (C.c_int, [C.c_void_p, i32p, C.c_uint32, u32p]),
 }
 
 _LIB: Optional[C.CDLL] = None

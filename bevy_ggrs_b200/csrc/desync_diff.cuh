@@ -12,6 +12,11 @@
 //           every row its output position, so records land in ascending (row, column, word) order whatever the
 //           scheduling: the output is deterministic.
 // Integer counts only: the result does not depend on the order the atomics land in.
+//
+// P2P remote diff (bgr_desync_diff_remote): `latest` is not an image but a staging buffer of tiles uploaded from a
+// peer's export blob.  `visit` then lists the tiles to compare, ascending: work position i (pass 1: block i; pass 2:
+// tile_list entries are positions) compares local tile visit[i] of `first` with the tile at position i of `latest`.
+// Without `visit` (SyncTest capture) position i is tile i of both images, as before.
 #pragma once
 #include "kernels.cuh"
 
@@ -33,15 +38,28 @@ struct DiffParams {
     unsigned int* col_counts;        // [n_cols][3]: rows with a word difference, ... inside the checksum, presence differences
     unsigned long long* totals;      // [0] rows with any difference, [1] existence differences, [2] differing words
     unsigned int* tile_records;      // [tiles] records of each tile (pass 1 output)
-    const unsigned int* tile_list;   // pass 2: [n_list] tile index, [n_list + i] its first record's output index
+    const unsigned int* tile_list;   // pass 2: [n_list] work position, [n_list + i] its first record's output index
     uint32_t n_list, cap;
     DiffRecord* out;                 // [cap]
+    const unsigned int* visit;       // optional: [positions] local tile of each work position (remote diff)
 };
 
-// the row's mask byte in an image: 0 unless the row exists there (stale bytes past the image's row count are not data)
-__device__ __forceinline__ uint32_t diff_mask(const uint8_t* img, uint32_t words, uint32_t row, uint32_t n_rows) {
-    const uint32_t m = row < n_rows ? uint32_t(img[alive_offset(words, row)]) : 0u;
+// the local tile and the two tile bases of work position `pos`
+struct DiffTiles { uint32_t tile; const uint8_t* first; const uint8_t* latest; };
+__device__ __forceinline__ DiffTiles diff_tiles(const DiffParams& p, uint32_t pos) {
+    const uint32_t tile = p.visit ? p.visit[pos] : pos;
+    const size_t tb = tile_bytes_of(p.words);
+    return DiffTiles{tile, p.first + size_t(tile) * tb, p.latest + size_t(p.visit ? pos : tile) * tb};
+}
+
+// the mask byte of row `row` (tile-local index row % kTileRows) from the base of its tile: 0 unless the row exists
+// there (stale bytes past the image's row count are not data)
+__device__ __forceinline__ uint32_t diff_mask_tile(const uint8_t* tile, uint32_t words, uint32_t row, uint32_t n_rows) {
+    const uint32_t m = row < n_rows ? uint32_t(tile[size_t(words) * kPlaneBytes + row % kTileRows]) : 0u;
     return (m & 1u) ? m : 0u;
+}
+__device__ __forceinline__ uint32_t diff_mask(const uint8_t* img, uint32_t words, uint32_t row, uint32_t n_rows) {
+    return diff_mask_tile(img + size_t(row / kTileRows) * tile_bytes_of(words), words, row, n_rows);
 }
 
 // Walks the records of one row in (column, word) order.  Every lane of a warp runs the same loop trip counts (the
@@ -50,9 +68,10 @@ __device__ __forceinline__ uint32_t diff_mask(const uint8_t* img, uint32_t words
 //   per_column(column, word_diff, ck_diff, presence)   after each column (not called for existence-only rows' columns
 //                                                      with any flag set: all false there)
 template <class OnRecord, class PerColumn>
-__device__ __forceinline__ void diff_row(const DiffParams& p, uint32_t row, OnRecord&& on_record, PerColumn&& per_column) {
-    const uint32_t mf = diff_mask(p.first, p.words, row, p.rows_first);
-    const uint32_t ml = diff_mask(p.latest, p.words, row, p.rows_latest);
+__device__ __forceinline__ void diff_row(const DiffParams& p, const DiffTiles& t, uint32_t row, OnRecord&& on_record,
+                                         PerColumn&& per_column) {
+    const uint32_t mf = diff_mask_tile(t.first, p.words, row, p.rows_first);
+    const uint32_t ml = diff_mask_tile(t.latest, p.words, row, p.rows_latest);
     const bool both = mf && ml;
     if ((mf != 0u) != (ml != 0u)) on_record(kDiffNone, kDiffNone, mf, ml);
     for (uint32_t c = 0; c < p.n_cols; ++c) {
@@ -61,12 +80,12 @@ __device__ __forceinline__ void diff_row(const DiffParams& p, uint32_t row, OnRe
         const bool presence = both && pf != pl;
         if (presence) on_record(c, kDiffNone, mf, ml);
         bool word_diff = false, ck_diff = false;
-        const size_t base = size_t(row / kTileRows) * tile_bytes_of(p.words) + size_t(row % kTileRows) * 4u;
+        const size_t base = size_t(row % kTileRows) * 4u;
         for (uint32_t w = 0; w < col.words; ++w) {
             if (pf && pl) {
                 const size_t off = base + size_t(col.first_plane + w) * kPlaneBytes;
-                const uint32_t a = __ldcs(reinterpret_cast<const uint32_t*>(p.first + off));
-                const uint32_t b = __ldcs(reinterpret_cast<const uint32_t*>(p.latest + off));
+                const uint32_t a = __ldcs(reinterpret_cast<const uint32_t*>(t.first + off));
+                const uint32_t b = __ldcs(reinterpret_cast<const uint32_t*>(t.latest + off));
                 if (a != b) {
                     on_record(c, w, a, b);
                     word_diff = true;
@@ -92,10 +111,11 @@ __global__ void __launch_bounds__(kDiffBlock) k_desync_count(const __grid_consta
     __shared__ uint32_t s_warp[kDiffBlock / 32u];
     const unsigned full = 0xffffffffu;
     const uint32_t lane = threadIdx.x & 31u;
-    const uint32_t row = blockIdx.x * kTileRows + threadIdx.x;
+    const DiffTiles t = diff_tiles(p, blockIdx.x);
+    const uint32_t row = t.tile * kTileRows + threadIdx.x;
     uint32_t n_rec = 0, n_words = 0;
     bool existence = false;
-    diff_row(p, row,
+    diff_row(p, t, row,
              [&](uint32_t c, uint32_t w, uint32_t, uint32_t) {
                  ++n_rec;
                  if (w != kDiffNone) ++n_words;
@@ -126,12 +146,12 @@ __global__ void __launch_bounds__(kDiffBlock) k_desync_count(const __grid_consta
 __global__ void __launch_bounds__(kDiffBlock) k_desync_records(const __grid_constant__ DiffParams p) {
     __shared__ uint32_t s_warp[kDiffBlock / 32u];
     const uint32_t lane = threadIdx.x & 31u, warp = threadIdx.x >> 5;
-    const uint32_t tile = p.tile_list[blockIdx.x];
+    const DiffTiles t = diff_tiles(p, p.tile_list[blockIdx.x]);
     const uint32_t base = p.tile_list[p.n_list + blockIdx.x];
-    const uint32_t row = tile * kTileRows + threadIdx.x;
+    const uint32_t row = t.tile * kTileRows + threadIdx.x;
     auto no_column = [](uint32_t, bool, bool, bool) {};
     uint32_t n_rec = 0;
-    diff_row(p, row, [&](uint32_t, uint32_t, uint32_t, uint32_t) { ++n_rec; }, no_column);
+    diff_row(p, t, row, [&](uint32_t, uint32_t, uint32_t, uint32_t) { ++n_rec; }, no_column);
     // exclusive scan of n_rec over the block (row order)
     uint32_t incl = n_rec;
     for (uint32_t o = 1; o < 32u; o <<= 1) {
@@ -144,7 +164,7 @@ __global__ void __launch_bounds__(kDiffBlock) k_desync_records(const __grid_cons
     for (uint32_t k = 0; k < warp; ++k) warp_base += s_warp[k];
     uint32_t pos = base + warp_base + incl - n_rec;
     if (n_rec == 0 || pos >= p.cap) return;  // no collective follows
-    diff_row(p, row,
+    diff_row(p, t, row,
              [&](uint32_t c, uint32_t w, uint32_t a, uint32_t b) {
                  if (pos < p.cap) p.out[pos] = DiffRecord{row, c, w, a, b};
                  ++pos;

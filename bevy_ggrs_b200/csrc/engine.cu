@@ -27,6 +27,7 @@
 #include "tma_copy.cuh"
 #include "generic_program.cuh"
 #include "desync_diff.cuh"
+#include "frame_digest.cuh"
 #include "jit.hpp"
 
 using namespace bgr;
@@ -257,10 +258,20 @@ struct bgr_engine {
     unsigned int* d_diff_list = nullptr;         // [2 * tiles]
     DiffRecord* d_diff_records = nullptr;
     size_t diff_records_cap = 0;
+    // P2P desync reports: retention of confirmed frames (bgr_retain_confirmed) and the digest / remote diff scratch,
+    // allocated by their first use
+    uint32_t retain_interval = 0, retain_count = 0;
+    DigestColumn* d_digest_cols = nullptr;
+    unsigned long long* d_digest_words = nullptr;  // [tiles][n_cols + 1]
+    unsigned int* d_digest_active = nullptr;       // [tiles]
+    uint8_t* d_remote = nullptr;                   // tiles uploaded from a peer's export blob
+    unsigned int* d_remote_visit = nullptr;        // [tiles] their local tile indices
+    uint32_t remote_cap_tiles = 0;
 
     uint8_t* image(uint32_t idx) const { return arena + size_t(idx) * image_bytes; }
     bool capture() const { return cfg.flags & BGR_CFG_DESYNC_CAPTURE; }
-    uint32_t n_slots() const { return capture() ? 2u * cfg.max_depth : cfg.max_depth; }  // frame slots behind the live image
+    // frame slots behind the live image
+    uint32_t n_slots() const { return (capture() ? 2u * cfg.max_depth : cfg.max_depth) + retain_count; }
     uint32_t image_off256(uint32_t idx) const { return uint32_t((size_t(idx) * image_bytes) >> 8); }
     uint32_t tiles_for(uint32_t rows) const { return (rows + kTileRows - 1) / kTileRows; }
     uint32_t grid_for(uint32_t n, uint32_t per_block) const {
@@ -1393,6 +1404,11 @@ BGR_API void bgr_engine_destroy(bgr_engine* e) {
     if (e->d_diff_totals) cudaFree(e->d_diff_totals);
     if (e->d_diff_list) cudaFree(e->d_diff_list);
     if (e->d_diff_records) cudaFree(e->d_diff_records);
+    if (e->d_digest_cols) cudaFree(e->d_digest_cols);
+    if (e->d_digest_words) cudaFree(e->d_digest_words);
+    if (e->d_digest_active) cudaFree(e->d_digest_active);
+    if (e->d_remote) cudaFree(e->d_remote);
+    if (e->d_remote_visit) cudaFree(e->d_remote_visit);
     for (auto& d : e->dl) {
         if (d.d_buf) cudaFree(d.d_buf);
         if (d.packed) cudaEventDestroy(d.packed);
@@ -1516,6 +1532,11 @@ BGR_API int bgr_build(bgr_engine* e) {
     e->n_tiles_cap = e->epad / kTileRows;
     e->tile_bytes = tile_bytes_of(e->words);
     e->image_bytes = (size_t(e->n_tiles_cap) * e->tile_bytes + 255u) & ~size_t(255);  // ops address images in 256-byte units
+    if (e->n_slots() > SlotRing::kMaxSlots)
+        return fail(BGR_ERR_INVALID_ARGUMENT, "bgr_retain_confirmed: " + std::to_string(e->n_slots() - e->retain_count) +
+                                                  " ring slots + " + std::to_string(e->retain_count) + " retained frames = " +
+                                                  std::to_string(e->n_slots()) + " frame slots, more than " +
+                                                  std::to_string(SlotRing::kMaxSlots));
     if ((e->image_bytes * (size_t(e->n_slots()) + 1u)) >> 8 > 0xffffffffull)
         return fail(BGR_ERR_CAPACITY, "arena larger than 1 TB");
     size_t total = e->image_bytes * (size_t(e->n_slots()) + 1u);
@@ -1548,6 +1569,7 @@ BGR_API int bgr_build(bgr_engine* e) {
         CUDA_TRY(cudaEventCreateWithFlags(&e->ev[i], cudaEventDisableTiming));
     }
     e->st.ring.reset(e->n_slots(), e->capture());
+    e->st.ring.set_retention(e->retain_interval, e->retain_count);
     e->st.slot_rows.fill(0);
     e->st.slot_elapsed_ns.fill(0);
     e->st.slot_passive_ver.fill(0);
@@ -1822,18 +1844,8 @@ BGR_API int bgr_peek_first(bgr_engine* e, int32_t frame, uint32_t column, uint32
     return BGR_OK;
 }
 
-BGR_API int bgr_desync_diff(bgr_engine* e, int32_t frame, bgr_desync_summary* summary, bgr_desync_column* cols,
-                            uint32_t cols_cap, bgr_desync_record* records, uint32_t records_cap, uint32_t* n_records,
-                            int32_t* found) {
-    static_assert(sizeof(DiffRecord) == sizeof(bgr_desync_record), "DiffRecord mirrors bgr_desync_record");
-    if (!summary || !found || (!cols && cols_cap) || (!records && records_cap))
-        return fail(BGR_ERR_INVALID_ARGUMENT, "null argument");
-    int rc = capture_args(e);
-    if (rc != BGR_OK) return rc;
-    if (n_records) *n_records = 0;
-    uint32_t sf = 0, sl = 0;
-    if (!e->st.ring.first(frame, &sf) || !e->st.ring.peek(frame, &sl)) { *found = 0; return BGR_OK; }
-    *found = 1;
+// the column table and counters of k_desync_*, allocated by the first diff; records grow with records_cap
+static int ensure_diff_scratch(bgr_engine* e, uint32_t records_cap) {
     const uint32_t n_cols = uint32_t(e->cols.size());
     if (!e->d_diff_cols) {
         std::vector<DiffColumn> dc(n_cols);
@@ -1856,36 +1868,40 @@ BGR_API int bgr_desync_diff(bgr_engine* e, int32_t frame, bgr_desync_summary* su
         CUDA_TRY(cudaMalloc(&e->d_diff_records, sizeof(DiffRecord) * records_cap));
         e->diff_records_cap = records_cap;
     }
-    DiffParams p{};
-    p.first = e->image(sf + 1);
-    p.latest = e->image(sl + 1);
+    return BGR_OK;
+}
+
+// Both passes of the diff over `n_pos` work positions (tiles, or the entries of p.visit); fills the summary's counts.
+static int run_diff(bgr_engine* e, DiffParams p, uint32_t n_pos, int32_t frame, bgr_desync_summary* summary,
+                    bgr_desync_column* cols, uint32_t cols_cap, bgr_desync_record* records, uint32_t records_cap,
+                    uint32_t* n_records) {
+    const uint32_t n_cols = uint32_t(e->cols.size());
+    int rc = ensure_diff_scratch(e, records_cap);
+    if (rc != BGR_OK) return rc;
     p.words = e->words;
     p.n_cols = n_cols;
-    p.rows_first = e->st.slot_rows[sf];
-    p.rows_latest = e->st.slot_rows[sl];
     p.cols = e->d_diff_cols;
     p.col_counts = e->d_diff_counts;
     p.totals = e->d_diff_totals;
     p.tile_records = e->d_diff_counts + 3u * n_cols;
     p.cap = records_cap;
     p.out = e->d_diff_records;
-    const uint32_t n_tiles = e->tiles_for(std::max(p.rows_first, p.rows_latest));
-    std::vector<unsigned int> counts(3u * n_cols + n_tiles, 0u);
+    std::vector<unsigned int> counts(3u * n_cols + n_pos, 0u);
     unsigned long long totals[3] = {0, 0, 0};
-    if (n_tiles) {
+    if (n_pos) {
         CUDA_TRY(cudaMemsetAsync(e->d_diff_counts, 0, sizeof(unsigned int) * 3u * n_cols, e->stream));
         CUDA_TRY(cudaMemsetAsync(e->d_diff_totals, 0, sizeof(unsigned long long) * 3u, e->stream));
-        k_desync_count<<<n_tiles, kDiffBlock, 0, e->stream>>>(p);
+        k_desync_count<<<n_pos, kDiffBlock, 0, e->stream>>>(p);
         e->launches += 1;
         CUDA_TRY(cudaGetLastError());
         CUDA_TRY(cudaMemcpyAsync(counts.data(), e->d_diff_counts, sizeof(unsigned int) * counts.size(), cudaMemcpyDeviceToHost, e->stream));
         CUDA_TRY(cudaMemcpyAsync(totals, e->d_diff_totals, sizeof totals, cudaMemcpyDeviceToHost, e->stream));
         CUDA_TRY(cudaStreamSynchronize(e->stream));
     }
-    // exclusive scan of the tile record counts: the tiles that hold one of the first records_cap records
+    // exclusive scan of the per-position record counts: the positions that hold one of the first records_cap records
     std::vector<unsigned int> list;
     uint64_t offset = 0;
-    for (uint32_t t = 0; t < n_tiles && offset < records_cap; ++t) {
+    for (uint32_t t = 0; t < n_pos && offset < records_cap; ++t) {
         const uint32_t n = counts[3u * n_cols + t];
         if (n) { list.push_back(t); list.push_back(uint32_t(offset)); }
         offset += n;
@@ -1893,7 +1909,7 @@ BGR_API int bgr_desync_diff(bgr_engine* e, int32_t frame, bgr_desync_summary* su
     const uint32_t n_list = uint32_t(list.size() / 2);
     const uint32_t n_out = uint32_t(std::min<uint64_t>(offset, records_cap));
     if (n_list) {
-        std::vector<unsigned int> packed(2u * n_list);  // [tiles..., bases...]
+        std::vector<unsigned int> packed(2u * n_list);  // [positions..., bases...]
         for (uint32_t i = 0; i < n_list; ++i) { packed[i] = list[2 * i]; packed[n_list + i] = list[2 * i + 1]; }
         CUDA_TRY(cudaMemcpyAsync(e->d_diff_list, packed.data(), sizeof(unsigned int) * packed.size(), cudaMemcpyHostToDevice, e->stream));
         p.tile_list = e->d_diff_list;
@@ -1912,14 +1928,289 @@ BGR_API int bgr_desync_diff(bgr_engine* e, int32_t frame, bgr_desync_summary* su
     summary->rows_differing = uint32_t(totals[0]);
     summary->existence_differing = uint32_t(totals[1]);
     summary->words_differing = totals[2];
-    summary->host_state_differs = (std::memcmp(&e->st.slot_rng[sf], &e->st.slot_rng[sl], sizeof(ParticleRng)) != 0 ? 1u : 0u) |
-                                  (e->st.slot_elapsed_ns[sf] != e->st.slot_elapsed_ns[sl] ? 2u : 0u);
-    summary->elapsed_ns_first = e->st.slot_elapsed_ns[sf];
-    summary->elapsed_ns_latest = e->st.slot_elapsed_ns[sl];
     for (uint32_t c = 0; c < cols_cap; ++c) {
         cols[c] = bgr_desync_column{0, 0, 0, 0};
         if (c < n_cols) cols[c] = bgr_desync_column{counts[3 * c], counts[3 * c + 1], counts[3 * c + 2], 0};
     }
+    return BGR_OK;
+}
+
+BGR_API int bgr_desync_diff(bgr_engine* e, int32_t frame, bgr_desync_summary* summary, bgr_desync_column* cols,
+                            uint32_t cols_cap, bgr_desync_record* records, uint32_t records_cap, uint32_t* n_records,
+                            int32_t* found) {
+    static_assert(sizeof(DiffRecord) == sizeof(bgr_desync_record), "DiffRecord mirrors bgr_desync_record");
+    if (!summary || !found || (!cols && cols_cap) || (!records && records_cap))
+        return fail(BGR_ERR_INVALID_ARGUMENT, "null argument");
+    int rc = capture_args(e);
+    if (rc != BGR_OK) return rc;
+    if (n_records) *n_records = 0;
+    uint32_t sf = 0, sl = 0;
+    if (!e->st.ring.first(frame, &sf) || !e->st.ring.peek(frame, &sl)) { *found = 0; return BGR_OK; }
+    *found = 1;
+    DiffParams p{};
+    p.first = e->image(sf + 1);
+    p.latest = e->image(sl + 1);
+    p.rows_first = e->st.slot_rows[sf];
+    p.rows_latest = e->st.slot_rows[sl];
+    rc = run_diff(e, p, e->tiles_for(std::max(p.rows_first, p.rows_latest)), frame, summary, cols, cols_cap, records,
+                  records_cap, n_records);
+    if (rc != BGR_OK) return rc;
+    summary->host_state_differs = (std::memcmp(&e->st.slot_rng[sf], &e->st.slot_rng[sl], sizeof(ParticleRng)) != 0 ? 1u : 0u) |
+                                  (e->st.slot_elapsed_ns[sf] != e->st.slot_elapsed_ns[sl] ? 2u : 0u);
+    summary->elapsed_ns_first = e->st.slot_elapsed_ns[sf];
+    summary->elapsed_ns_latest = e->st.slot_elapsed_ns[sl];
+    return BGR_OK;
+}
+
+// ---- P2P desync reports (ring.hpp retains confirmed frames, frame_digest.cuh digests, desync_diff.cuh compares) ----
+BGR_API int bgr_retain_confirmed(bgr_engine* e, uint32_t interval, uint32_t count) {
+    if (!e) return fail(BGR_ERR_INVALID_ARGUMENT, "null engine");
+    if (e->built) return fail(BGR_ERR_STATE, "bgr_retain_confirmed must be called before bgr_build");
+    if (e->cfg.flags & BGR_CFG_SHARDED) return fail(BGR_ERR_UNSUPPORTED, "bgr_retain_confirmed is not supported on a sharded engine");
+    if (interval == 0 || count == 0) return fail(BGR_ERR_INVALID_ARGUMENT, "bgr_retain_confirmed needs interval >= 1 and count >= 1");
+    e->retain_interval = interval;
+    e->retain_count = count;
+    return BGR_OK;
+}
+
+BGR_API int bgr_retained_frames(bgr_engine* e, int32_t* frames_out, uint32_t cap, uint32_t* n_out) {
+    if (!e) return fail(BGR_ERR_INVALID_ARGUMENT, "null engine");
+    std::vector<int32_t> f;
+    e->st.ring.retained_frames(&f);
+    for (uint32_t i = 0; i < f.size() && i < cap && frames_out; ++i) frames_out[i] = f[i];
+    if (n_out) *n_out = uint32_t(f.size());
+    return BGR_OK;
+}
+
+static int p2p_args(bgr_engine* e) {
+    if (!e || !e->built) return fail(BGR_ERR_STATE, "engine not built");
+    if (e->cfg.flags & BGR_CFG_SHARDED) return fail(BGR_ERR_UNSUPPORTED, "P2P desync reports are not supported on a sharded engine");
+    return drain(e);
+}
+
+// the slot of `frame`: a queued snapshot first, then a retained one
+static bool p2p_slot(const bgr_engine* e, int32_t frame, uint32_t* slot) {
+    return e->st.ring.peek(frame, slot) || e->st.ring.retained(frame, slot);
+}
+
+
+// what makes two engines' images comparable (registered systems deliberately excluded); order_base too, because every
+// digest word hashes the RollbackOrdered index order_base + row
+static uint64_t digest_layout(const bgr_engine* e) {
+    std::vector<uint32_t> v{BGR_DIGEST_BLOCK_ROWS, e->words, uint32_t(e->cols.size()), uint32_t(e->cfg.order_base),
+                            uint32_t(e->cfg.order_base >> 32)};
+    for (const Column& c : e->cols) {
+        const bool ck = c.hash_kind != BGR_HASH_NONE;
+        v.insert(v.end(), {c.elem_bytes, c.first_plane, c.words, c.absent ? 1u : 0u, ck ? 1u : 0u, ck ? c.hash_off : 0u,
+                           ck ? c.hash_len : 0u});
+    }
+    return bgr_seahash(v.data(), v.size() * sizeof(uint32_t));
+}
+
+BGR_API int bgr_frame_digest(bgr_engine* e, int32_t frame, bgr_frame_digest_header* header, uint64_t* words, uint32_t words_cap,
+                             int32_t* found) {
+    if (!header || !found || (!words && words_cap)) return fail(BGR_ERR_INVALID_ARGUMENT, "null argument");
+    int rc = p2p_args(e);
+    if (rc != BGR_OK) return rc;
+    uint32_t slot = 0;
+    if (!p2p_slot(e, frame, &slot)) { *found = 0; return BGR_OK; }
+    *found = 1;
+    const uint32_t n_cols = uint32_t(e->cols.size()), per = n_cols + 1u;
+    // dynamic shared memory: 16 warps x (n_cols + 1) words, next to the kernel's static s_warp[16] (48 KB in all)
+    const size_t smem = sizeof(unsigned long long) * (kTileRows / 32u) * per;
+    if (smem + sizeof(uint32_t) * (kTileRows / 32u) > 48u * 1024u)
+        return fail(BGR_ERR_UNSUPPORTED, "bgr_frame_digest supports at most 382 registered columns");
+    if (!e->d_digest_cols) {
+        std::vector<DigestColumn> dc(n_cols);
+        for (uint32_t c = 0; c < n_cols; ++c) dc[c] = DigestColumn{e->cols[c].first_plane, e->cols[c].elem_bytes, e->cols[c].absent};
+        CUDA_TRY(cudaMalloc(&e->d_digest_cols, sizeof(DigestColumn) * std::max(1u, n_cols)));
+        CUDA_TRY(cudaMemcpyAsync(e->d_digest_cols, dc.data(), sizeof(DigestColumn) * n_cols, cudaMemcpyHostToDevice, e->stream));
+        CUDA_TRY(cudaStreamSynchronize(e->stream));  // `dc` goes out of scope below
+        CUDA_TRY(cudaMalloc(&e->d_digest_words, sizeof(unsigned long long) * per * e->n_tiles_cap));
+        CUDA_TRY(cudaMalloc(&e->d_digest_active, sizeof(unsigned int) * e->n_tiles_cap));
+    }
+    const uint32_t rows = e->st.slot_rows[slot], n_blocks = e->tiles_for(rows);
+    std::vector<uint64_t> w(size_t(n_blocks) * per);
+    std::vector<unsigned int> active(n_blocks);
+    if (n_blocks) {
+        DigestParams p{};
+        p.img = e->image(slot + 1);
+        p.words = e->words;
+        p.n_cols = n_cols;
+        p.n_rows = rows;
+        p.order_base = e->cfg.order_base;
+        p.cols = e->d_digest_cols;
+        p.out = e->d_digest_words;
+        p.active = e->d_digest_active;
+        k_frame_digest<<<n_blocks, kTileRows, smem, e->stream>>>(p);
+        e->launches += 1;
+        CUDA_TRY(cudaGetLastError());
+        CUDA_TRY(cudaMemcpyAsync(w.data(), e->d_digest_words, sizeof(uint64_t) * w.size(), cudaMemcpyDeviceToHost, e->stream));
+        CUDA_TRY(cudaMemcpyAsync(active.data(), e->d_digest_active, sizeof(unsigned int) * n_blocks, cudaMemcpyDeviceToHost, e->stream));
+        CUDA_TRY(cudaStreamSynchronize(e->stream));
+    }
+    std::memset(header, 0, sizeof *header);
+    header->layout = digest_layout(e);
+    header->frame = frame;
+    header->rows = rows;
+    header->n_blocks = n_blocks;
+    header->n_columns = n_cols;
+    for (unsigned int a : active) header->active += a;
+    header->elapsed_ns = e->st.slot_elapsed_ns[slot];
+    static_assert(sizeof(ParticleRng) == sizeof(header->rng), "ParticleRng is four u64 words");
+    std::memcpy(header->rng, &e->st.slot_rng[slot], sizeof header->rng);
+    header->root = bgr_seahash(w.data(), w.size() * sizeof(uint64_t));
+    if (words) std::memcpy(words, w.data(), sizeof(uint64_t) * std::min<size_t>(words_cap, w.size()));
+    return BGR_OK;
+}
+
+BGR_API int bgr_digest_mismatch(const bgr_frame_digest_header* lh, const uint64_t* lw, const bgr_frame_digest_header* rh,
+                                const uint64_t* rw, uint32_t* blocks_out, uint32_t cap, uint32_t* n_out,
+                                uint32_t* host_state_differs) {
+    if (!lh || !rh || !n_out || (!blocks_out && cap) || (!lw && lh->n_blocks) || (!rw && rh->n_blocks))
+        return fail(BGR_ERR_INVALID_ARGUMENT, "null argument");
+    if (lh->layout != rh->layout)
+        return fail(BGR_ERR_INVALID_ARGUMENT, "the digests come from engines with different registrations (layout differs)");
+    if (lh->frame != rh->frame)
+        return fail(BGR_ERR_INVALID_ARGUMENT, "the digests are of different frames (" + std::to_string(lh->frame) + " and " +
+                                                  std::to_string(rh->frame) + ")");
+    if (lh->n_columns != rh->n_columns)
+        return fail(BGR_ERR_INVALID_ARGUMENT, "the digests have different column counts (" + std::to_string(lh->n_columns) +
+                                                  " and " + std::to_string(rh->n_columns) + ")");
+    const size_t per = size_t(lh->n_columns) + 1u;
+    const uint32_t common = std::min(lh->n_blocks, rh->n_blocks), most = std::max(lh->n_blocks, rh->n_blocks);
+    uint32_t n = 0;
+    for (uint32_t b = 0; b < most; ++b) {
+        const bool differs = b >= common || std::memcmp(lw + b * per, rw + b * per, per * sizeof(uint64_t)) != 0;
+        if (!differs) continue;
+        if (n < cap) blocks_out[n] = b;
+        ++n;
+    }
+    *n_out = n;
+    if (host_state_differs)
+        *host_state_differs = (std::memcmp(lh->rng, rh->rng, sizeof lh->rng) != 0 ? 1u : 0u) |
+                              (lh->elapsed_ns != rh->elapsed_ns ? 2u : 0u);
+    return BGR_OK;
+}
+
+static constexpr size_t kBlobBlockHeader = 8;  // u32 block index + u32 zero ahead of each tile
+
+BGR_API int bgr_frame_export(bgr_engine* e, int32_t frame, const uint32_t* blocks, uint32_t n_blocks, void* dst,
+                             size_t dst_cap, size_t* bytes, int32_t* found) {
+    if (!bytes || !found || (!blocks && n_blocks)) return fail(BGR_ERR_INVALID_ARGUMENT, "null argument");
+    int rc = p2p_args(e);
+    if (rc != BGR_OK) return rc;
+    uint32_t slot = 0;
+    if (!p2p_slot(e, frame, &slot)) { *found = 0; return BGR_OK; }
+    *found = 1;
+    const uint32_t rows = e->st.slot_rows[slot], total = e->tiles_for(rows);
+    for (uint32_t i = 0; i < n_blocks; ++i) {
+        if (blocks[i] >= total)
+            return fail(BGR_ERR_INVALID_ARGUMENT, "block " + std::to_string(blocks[i]) + " is past the frame's " +
+                                                      std::to_string(total) + " blocks");
+        if (i && blocks[i] <= blocks[i - 1]) return fail(BGR_ERR_INVALID_ARGUMENT, "the block list must be ascending without duplicates");
+    }
+    const size_t tb = e->tile_bytes;
+    const size_t need = sizeof(bgr_frame_blob_header) + size_t(n_blocks) * (kBlobBlockHeader + tb);
+    *bytes = need;
+    if (!dst) return BGR_OK;
+    if (dst_cap < need) return fail(BGR_ERR_CAPACITY, "the export needs " + std::to_string(need) + " bytes");
+    uint8_t* out = static_cast<uint8_t*>(dst);
+    bgr_frame_blob_header h{};
+    h.magic = BGR_FRAME_BLOB_MAGIC;
+    h.version = BGR_FRAME_BLOB_VERSION;
+    h.layout = digest_layout(e);
+    h.frame = frame;
+    h.rows = rows;
+    h.words = e->words;
+    h.n_blocks = total;
+    h.n_exported = n_blocks;
+    h.elapsed_ns = e->st.slot_elapsed_ns[slot];
+    std::memcpy(h.rng, &e->st.slot_rng[slot], sizeof h.rng);
+    std::memcpy(out, &h, sizeof h);
+    for (uint32_t i = 0; i < n_blocks; ++i) {
+        uint8_t* rec = out + sizeof h + size_t(i) * (kBlobBlockHeader + tb);
+        const uint32_t idx[2] = {blocks[i], 0u};
+        std::memcpy(rec, idx, sizeof idx);
+        CUDA_TRY(cudaMemcpyAsync(rec + kBlobBlockHeader, e->image(slot + 1) + size_t(blocks[i]) * tb, tb, cudaMemcpyDeviceToHost, e->stream));
+    }
+    CUDA_TRY(cudaStreamSynchronize(e->stream));
+    // rows >= rows of the last block hold whatever an older frame left there: zero their words and mask bytes
+    if (n_blocks && blocks[n_blocks - 1] == total - 1 && rows % kTileRows) {
+        uint8_t* tile = out + sizeof h + size_t(n_blocks - 1) * (kBlobBlockHeader + tb) + kBlobBlockHeader;
+        const uint32_t r0 = rows % kTileRows;
+        for (uint32_t w = 0; w < e->words; ++w) std::memset(tile + size_t(w) * kPlaneBytes + r0 * 4u, 0, (kTileRows - r0) * 4u);
+        std::memset(tile + size_t(e->words) * kPlaneBytes + r0, 0, kTileRows - r0);
+    }
+    return BGR_OK;
+}
+
+BGR_API int bgr_desync_diff_remote(bgr_engine* e, int32_t frame, const void* blob, size_t bytes,
+                                   bgr_desync_summary* summary, bgr_desync_column* cols, uint32_t cols_cap,
+                                   bgr_desync_record* records, uint32_t records_cap, uint32_t* n_records, int32_t* found) {
+    if (!summary || !found || !blob || (!cols && cols_cap) || (!records && records_cap))
+        return fail(BGR_ERR_INVALID_ARGUMENT, "null argument");
+    int rc = p2p_args(e);
+    if (rc != BGR_OK) return rc;
+    if (n_records) *n_records = 0;
+    // the blob comes from another machine: check every field before using it
+    const uint8_t* in = static_cast<const uint8_t*>(blob);
+    bgr_frame_blob_header h;
+    if (bytes < sizeof h) return fail(BGR_ERR_INVALID_ARGUMENT, "blob truncated: shorter than its header");
+    std::memcpy(&h, in, sizeof h);
+    if (h.magic != BGR_FRAME_BLOB_MAGIC) return fail(BGR_ERR_INVALID_ARGUMENT, "not a frame export blob (bad magic)");
+    if (h.version != BGR_FRAME_BLOB_VERSION)
+        return fail(BGR_ERR_INVALID_ARGUMENT, "unsupported blob format version " + std::to_string(h.version));
+    if (h.layout != digest_layout(e) || h.words != e->words)
+        return fail(BGR_ERR_INVALID_ARGUMENT, "the blob comes from an engine with a different registration (layout differs)");
+    if (h.frame != frame)
+        return fail(BGR_ERR_INVALID_ARGUMENT, "the blob holds frame " + std::to_string(h.frame) + ", not " + std::to_string(frame));
+    if (h.reserved != 0) return fail(BGR_ERR_INVALID_ARGUMENT, "blob header: reserved field is not zero");
+    if (h.n_blocks != e->tiles_for(h.rows) || h.n_blocks > e->n_tiles_cap || h.n_exported > h.n_blocks)
+        return fail(BGR_ERR_INVALID_ARGUMENT, "the blob's row and block counts are inconsistent or exceed this engine's capacity");
+    const size_t tb = e->tile_bytes, rec = kBlobBlockHeader + tb;
+    if (bytes != sizeof h + size_t(h.n_exported) * rec)
+        return fail(BGR_ERR_INVALID_ARGUMENT, "blob length " + std::to_string(bytes) + " does not match its " +
+                                                  std::to_string(h.n_exported) + " blocks (truncated or overlong)");
+    std::vector<unsigned int> visit(h.n_exported);
+    for (uint32_t i = 0; i < h.n_exported; ++i) {
+        uint32_t idx[2];
+        std::memcpy(idx, in + sizeof h + size_t(i) * rec, sizeof idx);
+        if (idx[1] != 0) return fail(BGR_ERR_INVALID_ARGUMENT, "blob block " + std::to_string(i) + ": reserved word is not zero");
+        if (idx[0] >= h.n_blocks)
+            return fail(BGR_ERR_INVALID_ARGUMENT, "blob block index " + std::to_string(idx[0]) + " >= its " +
+                                                      std::to_string(h.n_blocks) + " blocks");
+        if (i && idx[0] <= visit[i - 1]) return fail(BGR_ERR_INVALID_ARGUMENT, "blob block list is unsorted or has duplicates");
+        visit[i] = idx[0];
+    }
+    uint32_t slot = 0;
+    if (!p2p_slot(e, frame, &slot)) { *found = 0; return BGR_OK; }
+    *found = 1;
+    if (h.n_exported > e->remote_cap_tiles) {  // staging for the peer's tiles, grown on demand
+        if (e->d_remote) CUDA_TRY(cudaFree(e->d_remote));
+        if (e->d_remote_visit) CUDA_TRY(cudaFree(e->d_remote_visit));
+        e->d_remote = nullptr; e->d_remote_visit = nullptr; e->remote_cap_tiles = 0;
+        CUDA_TRY(cudaMalloc(&e->d_remote, tb * h.n_exported));
+        CUDA_TRY(cudaMalloc(&e->d_remote_visit, sizeof(unsigned int) * h.n_exported));
+        e->remote_cap_tiles = h.n_exported;
+    }
+    for (uint32_t i = 0; i < h.n_exported; ++i)
+        CUDA_TRY(cudaMemcpyAsync(e->d_remote + size_t(i) * tb, in + sizeof h + size_t(i) * rec + kBlobBlockHeader, tb,
+                                 cudaMemcpyHostToDevice, e->stream));
+    if (h.n_exported)
+        CUDA_TRY(cudaMemcpyAsync(e->d_remote_visit, visit.data(), sizeof(unsigned int) * h.n_exported, cudaMemcpyHostToDevice, e->stream));
+    DiffParams p{};
+    p.first = e->image(slot + 1);
+    p.latest = e->d_remote;
+    p.visit = e->d_remote_visit;
+    p.rows_first = e->st.slot_rows[slot];
+    p.rows_latest = h.rows;
+    rc = run_diff(e, p, h.n_exported, frame, summary, cols, cols_cap, records, records_cap, n_records);
+    if (rc != BGR_OK) return rc;
+    summary->host_state_differs = (std::memcmp(&e->st.slot_rng[slot], h.rng, sizeof h.rng) != 0 ? 1u : 0u) |
+                                  (e->st.slot_elapsed_ns[slot] != h.elapsed_ns ? 2u : 0u);
+    summary->elapsed_ns_first = e->st.slot_elapsed_ns[slot];
+    summary->elapsed_ns_latest = h.elapsed_ns;
     return BGR_OK;
 }
 
@@ -2172,6 +2463,7 @@ BGR_API int bgr_reset_session(bgr_engine* e) {
     e->st.has_maxpred = true;     // MaxPredictionWindow(8)
     e->st.maxpred = 8;
     e->st.ring.release_witnesses();  // a new session compares nothing against the old one's first images
+    e->st.ring.release_retained();   // ... and reports no desync of the old one's frames
     return BGR_OK;
 }
 
@@ -2261,6 +2553,18 @@ BGR_API int bgr_ring_first(bgr_ring* r, int32_t frame, uint32_t* slot_out, int32
 }
 BGR_API int bgr_ring_slots_in_use(bgr_ring* r, uint32_t* n_out) {
     if (n_out) *n_out = r->r.slots_in_use();
+    return BGR_OK;
+}
+BGR_API int bgr_ring_set_retention(bgr_ring* r, uint32_t interval, uint32_t count) {
+    if (count && interval == 0) return fail(BGR_ERR_INVALID_ARGUMENT, "retention needs interval >= 1");
+    r->r.set_retention(interval, count);
+    return BGR_OK;
+}
+BGR_API int bgr_ring_retained(bgr_ring* r, int32_t* frames_out, uint32_t cap, uint32_t* n_out) {
+    std::vector<int32_t> f;
+    r->r.retained_frames(&f);
+    for (uint32_t i = 0; i < f.size() && i < cap && frames_out; ++i) frames_out[i] = f[i];
+    if (n_out) *n_out = uint32_t(f.size());
     return BGR_OK;
 }
 

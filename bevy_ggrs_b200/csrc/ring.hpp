@@ -29,6 +29,22 @@
 // engine's 2*max_depth slots always suffice (tests/test_desync_capture.py walks every d in 1..7, max_prediction in
 // d+1..8 and sees exactly 2(d+1) for d >= 2).  Deeper P2P rollbacks can exceed that; the shortage rule then trades
 // witnesses for slots, so capture never makes a push fail that the plain ring would have served.
+//
+// Retention (bgr_retain_confirmed, set_retention(interval, count)): P2P desync detection compares the checksums of the
+// confirmed frames 0, interval, 2*interval, ... between peers, and the report arrives a round trip after confirm() has
+// dropped the frame.  So a frame f >= 0 with f % interval == 0 that leaves the queue from the OLD end (confirm, or the
+// depth eviction in push) keeps its slot as a RETAINED frame instead of freeing it.
+//   - Only the old end counts: a frame dropped from the new end (rollback, the re-save of an equal or older frame) was
+//     not final.
+//   - At most `count` frames are retained; the one retained first is released first.
+//   - A push of a retained frame's number releases the stale copy; release_retained() (bgr_reset_session) releases all.
+//   - The queue (get / peek / frames) is exactly the plain ring's, and a push never fails where the plain ring would
+//     succeed: the engine allocates `count` extra slots and at most `count` are ever retained.
+//   - slot_rows / slot_elapsed_ns / slot_rng are indexed by slot, so a retained frame keeps its row count, time and RNG.
+// A retained slot is never handed to a Save, so it is never written again until it is released.  That is why the
+// deferred live image (BGR_TUNE_DEFER_LIVE) may keep reading the base slot of the last Save even when that Save's own
+// frame gets retained (a depth-1 ring retains it at the next push): the bytes the deferred image is rebuilt from stay
+// as they were, exactly as if the slot had been freed and not yet reused.
 #pragma once
 #include <array>
 #include <cstdint>
@@ -52,6 +68,9 @@ public:
         entries_.n = 0;
         free_.n = 0;
         witnesses_.n = 0;
+        retained_.n = 0;
+        retain_interval_ = 0;
+        retain_count_ = 0;
         for (uint32_t s = n_slots_; s-- > 0;) free_.push_back(s);
         depth_ = 60;  // DEFAULT_FPS until sync_depth runs (mod.rs:112)
     }
@@ -64,6 +83,8 @@ public:
     // Returns the slot that now holds `frame`, or kNoSlot if more than n_slots snapshots would
     // have to be alive at once (configuration error, reported by the caller).
     uint32_t push(int32_t frame) {
+        for (uint32_t i = 0; i < retained_.size(); ++i)  // the stale retained copy of this frame
+            if (retained_[i].frame == frame) { release_retained_at(i); break; }
         // entries_ is oldest-first; the reference's "front" is our back()
         while (!entries_.empty() && !is_older(entries_.back().frame, frame)) release_back();
         // the entries that `while len > depth` would evict after the insert can go first:
@@ -105,6 +126,25 @@ public:
         }
     }
     uint32_t slots_in_use() const { return n_slots_ - free_.size(); }
+
+    // retention (see the header comment); count == 0 turns it off
+    void set_retention(uint32_t interval, uint32_t count) {
+        release_retained();
+        retain_interval_ = interval;
+        retain_count_ = count;
+    }
+    uint32_t retain_count() const { return retain_count_; }
+    void release_retained() { while (!retained_.empty()) release_retained_at(0); }
+    bool retained(int32_t frame, uint32_t* slot) const {
+        for (uint32_t i = 0; i < retained_.size(); ++i)
+            if (retained_[i].frame == frame) { *slot = retained_[i].slot; return true; }
+        return false;
+    }
+    // retained frames, the most recently retained first
+    void retained_frames(std::vector<int32_t>* out) const {
+        out->clear();
+        for (uint32_t i = retained_.size(); i-- > 0;) out->push_back(retained_[i].frame);
+    }
 
     // false => the reference would panic; `error` gets the same text
     bool rollback(int32_t frame, std::string* error) {
@@ -176,9 +216,11 @@ private:
             if (witnesses_[i].frame == frame) return i;
         return kNoSlot;
     }
-    bool pinned(uint32_t slot) const {
+    bool pinned(uint32_t slot) const {  // a witness or a retained frame holds the slot
         for (uint32_t i = 0; i < witnesses_.size(); ++i)
             if (witnesses_[i].slot == slot) return true;
+        for (uint32_t i = 0; i < retained_.size(); ++i)
+            if (retained_[i].slot == slot) return true;
         return false;
     }
     bool queued(uint32_t slot) const {
@@ -204,12 +246,24 @@ private:
         const uint32_t w = find_witness(e.frame);
         if (w != kNoSlot && witnesses_[w].slot != e.slot) release_witness(w);
         else if (w != kNoSlot) witnesses_.erase(w);  // the witness is this entry's own slot, freed below
+        if (retain_count_ && e.frame >= 0 && e.frame % int64_t(retain_interval_) == 0) {
+            retained_.push_back(e);
+            if (retained_.size() > retain_count_) release_retained_at(0);
+            return;
+        }
         if (!pinned(e.slot)) free_.push_back(e.slot);
+    }
+    void release_retained_at(uint32_t i) {
+        const uint32_t s = retained_[i].slot;
+        retained_.erase(i);
+        if (!queued(s) && !pinned(s)) free_.push_back(s);
     }
 
     Small<Entry> entries_;  // oldest first; depth is small (<= 64), O(depth) per operation
     Small<uint32_t> free_;
     Small<Entry> witnesses_;  // capture rings: (frame, slot of its first-recorded image), in the order recorded
+    Small<Entry> retained_;   // retention: (frame, slot) that left from the old end, in the order retained
+    uint32_t retain_interval_ = 0, retain_count_ = 0;
     uint32_t n_slots_ = 0;
     uint32_t depth_ = 60;
     bool capture_ = false;

@@ -242,6 +242,58 @@ class Engine:
                                              alive.ctypes.data, C.byref(found)))
         return (out, alive) if found.value else None
 
+    # ---- P2P desync reports ----
+    def retain_confirmed(self, interval: int, count: int) -> None:
+        """Before build: keep the last ``count`` confirmed frames that are multiples of ``interval``."""
+        self._check(self._lib.bgr_retain_confirmed(self._h, interval, count))
+
+    def retained_frames(self) -> List[int]:
+        """Retained frames, the most recently retained first."""
+        buf = (C.c_int32 * 64)()
+        n = C.c_uint32()
+        self._check(self._lib.bgr_retained_frames(self._h, buf, 64, C.byref(n)))
+        return [buf[i] for i in range(min(n.value, 64))]
+
+    def frame_digest(self, frame: int) -> Optional[Tuple["capi.bgr_frame_digest_header", np.ndarray]]:
+        """(header, words[n_blocks, n_columns + 1]) of a queued or retained frame; None if neither holds it."""
+        h = capi.bgr_frame_digest_header()
+        found = C.c_int32()
+        per = len(self.elem_bytes) + 1
+        words = np.zeros(-(-self.max_entities // capi.BGR_DIGEST_BLOCK_ROWS) * per, np.uint64)  # any frame fits: one call
+        self._check(self._lib.bgr_frame_digest(self._h, frame, C.byref(h), words.ctypes.data, words.size, C.byref(found)))
+        if not found.value:
+            return None
+        return h, words[: h.n_blocks * per].reshape(h.n_blocks, per).copy()
+
+    def export_blocks(self, frame: int, blocks: Sequence[int]) -> Optional[bytes]:
+        """The export blob of ``blocks`` of a queued or retained frame; None if neither holds it."""
+        ba = np.ascontiguousarray(blocks, dtype=np.uint32)
+        size, found = C.c_size_t(), C.c_int32()
+        self._check(self._lib.bgr_frame_export(self._h, frame, ba.ctypes.data, len(ba), None, 0, C.byref(size), C.byref(found)))
+        if not found.value:
+            return None
+        out = np.zeros(size.value, np.uint8)
+        self._check(self._lib.bgr_frame_export(self._h, frame, ba.ctypes.data, len(ba), out.ctypes.data, out.size,
+                                               C.byref(size), C.byref(found)))
+        return out.tobytes()
+
+    def diff_remote(self, frame: int, blob: bytes, max_records: int = 64) -> Optional[DesyncReport]:
+        """The local image of ``frame`` ("first") against a peer's exported blocks ("latest")."""
+        s = capi.bgr_desync_summary()
+        cols = (capi.bgr_desync_column * max(1, len(self.elem_bytes)))()
+        recs = np.zeros(max_records, RECORD_DTYPE)
+        n, found = C.c_uint32(), C.c_int32()
+        self._check(self._lib.bgr_desync_diff_remote(self._h, frame, blob, len(blob), C.byref(s), cols, len(self.elem_bytes),
+                                                     recs.ctypes.data_as(C.POINTER(capi.bgr_desync_record)), max_records,
+                                                     C.byref(n), C.byref(found)))
+        if not found.value:
+            return None
+        return DesyncReport(s.frame, s.rows_first, s.rows_latest, s.rows_differing, s.existence_differing,
+                            s.words_differing, s.host_state_differs, s.elapsed_ns_first, s.elapsed_ns_latest,
+                            {i: DesyncColumn(i, self.names[i], cols[i].rows, cols[i].rows_in_checksum, cols[i].presence)
+                             for i in range(len(self.elem_bytes))},
+                            recs[: n.value].copy())
+
     # ---- schedules ----
     def save_world(self) -> Tuple[int, int]:
         cs = capi.bgr_checksum()
@@ -363,6 +415,21 @@ def fold_partials(partial: "capi.bgr_partial") -> int:
     if st != capi.BGR_OK:
         raise BgrError(st, lib.bgr_last_error().decode())
     return (cs.hi << 64) | cs.lo
+
+
+def digest_mismatch(local, remote) -> Tuple[List[int], int]:
+    """(blocks that differ, host_state_differs bits) of two ``Engine.frame_digest`` results (bgr_digest_mismatch)."""
+    lib = capi.load_library()
+    (lh, lw), (rh, rw) = local, remote
+    lw, rw = np.ascontiguousarray(lw, np.uint64), np.ascontiguousarray(rw, np.uint64)
+    cap = max(lh.n_blocks, rh.n_blocks, 1)
+    out = np.zeros(cap, np.uint32)
+    n, host = C.c_uint32(), C.c_uint32()
+    st = lib.bgr_digest_mismatch(C.byref(lh), lw.ctypes.data, C.byref(rh), rw.ctypes.data, out.ctypes.data, cap,
+                                 C.byref(n), C.byref(host))
+    if st != capi.BGR_OK:
+        raise BgrError(st, lib.bgr_last_error().decode("utf-8", "replace"))
+    return [int(b) for b in out[: n.value]], host.value
 
 
 def ggrs_time_delta_bits(fps: int, frame: int) -> int:

@@ -260,6 +260,74 @@ public:
         return r;
     }
 
+    // ---- P2P desync reports (GgrsEvent::DesyncDetected: the frame is confirmed and the other image is remote) ----
+    // retain_confirmed before the first update keeps the confirmed multiples of the session's desync interval; the peers
+    // exchange frame_digest results over the game's own channel, digest_mismatch (bgr_digest_mismatch, the one reader
+    // of the format) names the blocks, the remote peer export_blocks them and the local peer diff_remote's the blob.
+    App& retain_confirmed(uint32_t interval, uint32_t count) {  // applied by the engine's build, like the registrations
+        if (engine_) throw Panic(BGR_ERR_STATE, "retain_confirmed must be called before the App is built");
+        retain_ = {interval, count};
+        return *this;
+    }
+    std::vector<int32_t> retained_frames() {
+        finish();
+        int32_t f[64]; uint32_t n = 0;
+        check(bgr_retained_frames(engine_, f, 64, &n));
+        return std::vector<int32_t>(f, f + std::min<uint32_t>(n, 64));
+    }
+    struct FrameDigest {
+        bool found = false;
+        bgr_frame_digest_header header{};
+        std::vector<uint64_t> words;  // header.n_blocks x (header.n_columns + 1)
+    };
+    FrameDigest frame_digest(ggrs::Frame frame) {
+        finish();
+        FrameDigest d;
+        d.words.resize(size_t((cfg_.max_entities + BGR_DIGEST_BLOCK_ROWS - 1) / BGR_DIGEST_BLOCK_ROWS) * (pending_cols_.size() + 1));
+        int32_t found = 0;
+        check(bgr_frame_digest(engine_, frame, &d.header, d.words.data(), uint32_t(d.words.size()), &found));
+        d.found = found != 0;
+        d.words.resize(d.found ? size_t(d.header.n_blocks) * (d.header.n_columns + 1) : 0);
+        return d;
+    }
+    // blocks whose digests differ, ascending; *host_state_differs: bit 0 ParticleRng, bit 1 Time<GgrsTime>
+    static std::vector<uint32_t> digest_mismatch(const FrameDigest& local, const FrameDigest& remote,
+                                                 uint32_t* host_state_differs = nullptr) {
+        std::vector<uint32_t> blocks(std::max<uint32_t>(1, std::max(local.header.n_blocks, remote.header.n_blocks)));
+        uint32_t n = 0, host = 0;
+        check(bgr_digest_mismatch(&local.header, local.words.data(), &remote.header, remote.words.data(), blocks.data(),
+                                  uint32_t(blocks.size()), &n, &host));
+        blocks.resize(std::min<size_t>(n, blocks.size()));
+        if (host_state_differs) *host_state_differs = host;
+        return blocks;
+    }
+    // the export blob of `blocks` (ascending) of a queued or retained frame; empty when neither holds it
+    std::vector<uint8_t> export_blocks(ggrs::Frame frame, const std::vector<uint32_t>& blocks) {
+        finish();
+        size_t bytes = 0;
+        int32_t found = 0;
+        check(bgr_frame_export(engine_, frame, blocks.data(), uint32_t(blocks.size()), nullptr, 0, &bytes, &found));
+        if (!found) return {};
+        std::vector<uint8_t> blob(bytes);
+        check(bgr_frame_export(engine_, frame, blocks.data(), uint32_t(blocks.size()), blob.data(), blob.size(), &bytes, &found));
+        return blob;
+    }
+    // the local image of `frame` ("first") against a peer's blob ("latest"): the records of desync_report
+    DesyncReport diff_remote(ggrs::Frame frame, const std::vector<uint8_t>& blob, uint32_t max_records = 64) {
+        finish();
+        DesyncReport r;
+        r.columns.resize(pending_cols_.size());
+        r.records.resize(max_records);
+        uint32_t n = 0;
+        int32_t found = 0;
+        check(bgr_desync_diff_remote(engine_, frame, blob.data(), blob.size(), &r.summary, r.columns.data(),
+                                     uint32_t(r.columns.size()), r.records.data(), max_records, &n, &found));
+        r.found = found != 0;
+        r.records.resize(n);
+        for (auto& c : pending_cols_) r.column_names.push_back(c.name);
+        return r;
+    }
+
 private:
     template <class T> App& register_component(uint32_t strategy) {
         static_assert(std::is_trivially_copyable<T>::value, "only POD components cross the C ABI");
@@ -276,6 +344,7 @@ private:
                                          ck.second.assert_finite ? BGR_HASH_FLAG_ASSERT_FINITE_F32 : 0u));
         for (auto& s : systems_)
             check(bgr_add_system(engine_, s.id, s.columns.data(), uint32_t(s.columns.size()), s.params.data(), uint32_t(s.params.size())));
+        if (retain_.second) check(bgr_retain_confirmed(engine_, retain_.first, retain_.second));
         check(bgr_build(engine_));
         for (auto& f : startup_) f(*this);
     }
@@ -452,6 +521,7 @@ private:
     ggrs::Frame res_frame_ = 0;
     bgr_config cfg_{};
     bgr_engine* engine_ = nullptr;
+    std::pair<uint32_t, uint32_t> retain_{0, 0};  // retain_confirmed(interval, count); count 0: off
     std::vector<PendingCol> pending_cols_;
     std::map<std::type_index, uint32_t> columns_;
     std::vector<std::pair<uint32_t, ByteRangeHasher>> checksums_;

@@ -235,6 +235,38 @@ class App:
         report for a mismatched frame points at them."""
         return self.world.desync_diff(frame, max_records)
 
+    # ---- P2P desync reports ----
+    # GgrsEvent::DesyncDetected { frame, .. } arrives after `frame` was confirmed: retain_confirmed (before the first
+    # update) keeps the confirmed multiples of the session's desync interval, frame_digest / digest_mismatch find the
+    # blocks two peers disagree on, and export_blocks / diff_remote show the rows.  Moving digests and blobs between
+    # the peers is the game's job (GGRS carries no application messages).
+    def retain_confirmed(self, interval: int, count: int) -> "App":
+        self.world.retain_confirmed(interval, count)
+        return self
+
+    def retained_frames(self):
+        return self.world.retained_frames()
+
+    def frame_digest(self, frame: int):
+        """(bgr_frame_digest_header, words[n_blocks, n_columns + 1]) of a queued or retained frame, or None."""
+        self._finish()
+        return self.world.frame_digest(frame)
+
+    @staticmethod
+    def digest_mismatch(local, remote):
+        """(blocks whose digests differ, host_state_differs bits); bgr_digest_mismatch interprets the format."""
+        from .engine import digest_mismatch
+        return digest_mismatch(local, remote)
+
+    def export_blocks(self, frame: int, blocks):
+        self._finish()
+        return self.world.export_blocks(frame, blocks)
+
+    def diff_remote(self, frame: int, blob: bytes, max_records: int = 64):
+        """A ``DesyncReport`` of the local image of ``frame`` ("first") against a peer's exported blocks ("latest")."""
+        self._finish()
+        return self.world.diff_remote(frame, blob, max_records)
+
     # ---- frame resources ----
     def rollback_frame_count(self) -> int:
         return self.world.rollback_frame_count()

@@ -218,8 +218,12 @@ class P2PTraceSession:
     otherwise uniform in 1..=max_prediction (clamped to the frames that exist)."""
 
     def __init__(self, num_players: int = 2, max_prediction: int = 8, input_delay: int = 2,
-                 seed: int = 0xB200, p_clean: float = 0.5):
+                 seed: int = 0xB200, p_clean: float = 0.5, desync_interval: Optional[int] = None):
         self._num_players = num_players
+        # DesyncDetection::On { interval }: the checksums of confirmed frames 0, interval, 2*interval, ... go to the peer
+        self._desync_interval = desync_interval
+        self._checksums: Dict[int, Optional[int]] = {}
+        self._reported: set = set()
         self._max_prediction = max_prediction
         self.current_frame = 0
         self._rng = Xoshiro256pp(seed)
@@ -244,7 +248,16 @@ class P2PTraceSession:
         self._local[handle] = value
 
     def save_cell(self, frame: int, checksum: Optional[int]) -> None:
-        pass
+        if self._desync_interval and frame >= 0 and frame % self._desync_interval == 0:
+            self._checksums[frame] = checksum  # a re-save after a rollback replaces the prediction's checksum
+
+    def checksum_reports(self) -> List[tuple]:
+        """The (frame, checksum) pairs GGRS would send to the peer now (desync_interval set): each multiple of the
+        interval once it is confirmed, with its latest checksum."""
+        out = [(f, c) for f, c in sorted(self._checksums.items())
+               if f not in self._reported and f <= self.confirmed_frame()]
+        self._reported.update(f for f, _ in out)
+        return out
 
     def _advance_request(self, predicted: bool) -> Request:
         ins = self._inputs.get(self.current_frame)

@@ -303,6 +303,97 @@ BGR_API int bgr_desync_diff(bgr_engine* e, int32_t frame, bgr_desync_summary* su
 BGR_API int bgr_peek_first(bgr_engine* e, int32_t frame, uint32_t column, uint32_t first_row, uint32_t count,
                            void* host_dst, uint32_t stride, uint8_t* alive_dst, int32_t* found);
 
+/* ---- P2P desync reports (any built engine without BGR_CFG_SHARDED) ---------------------------------------------
+ * Serves GGRS's `GgrsEvent::DesyncDetected { frame, local_checksum, remote_checksum, addr }`, raised by a P2P session
+ * with `DesyncDetection::On { interval }` when the checksums two peers computed for the confirmed frame
+ * 0, interval, 2*interval, ... differ (docs/debugging-desyncs.md:61-71).  The reference cannot inspect that frame: its
+ * snapshot was pruned when the frame was confirmed, and the other image lives on another machine ("Known
+ * Limitations", :73-76).  Here:
+ *   1. bgr_retain_confirmed keeps the last `count` frames f >= 0, f % interval == 0 after they leave the ring from the
+ *      old end (confirmed or evicted for depth), in `count` extra frame slots.  Loads, checksums, bgr_peek and
+ *      bgr_snapshot_frames are unchanged; bgr_launch_count can only be lower (a depth-1 ring no longer writes a
+ *      deferred live image early because the next Save reuses its base slot).  bgr_reset_session releases them.
+ *   2. bgr_frame_digest hashes a queued or retained frame per block of BGR_DIGEST_BLOCK_ROWS rows into n_columns + 1
+ *      u64 words (~62 KB at 1M rows of the stress schema).  The peers exchange digests over the game's own channel
+ *      (GGRS carries no application messages; the engine does no networking) and bgr_digest_mismatch lists the blocks
+ *      that differ.
+ *   3. The peer exports those blocks (bgr_frame_export, the tiles as stored, BGR_DIGEST_BLOCK_ROWS * (4*words + 1) B
+ *      each) and the local side diffs them against its own image (bgr_desync_diff_remote): the records and summary of
+ *      bgr_desync_diff, with "first" = the local image and "latest" = the remote one.
+ * Digest of block b, for C registered columns (word c < C per column, word C for existence and presence); rows r of
+ * the block with r < rows whose alive bit is set "exist":
+ *   word c = XOR over existing rows holding column c (absent bit clear) of
+ *            seahash_2xu64(order_base + r, seahash(element bytes [0, elem_bytes)))   (component_checksum.rs:81-90)
+ *   word C = XOR over existing rows of seahash_2xu64(order_base + r, mask byte)
+ * For a column whose checksummed range is the whole element, the XOR of its word over all blocks is the frame's
+ * per-column checksum partial (bgr_partial.xor_).  The digest is a wire format between peers: the block size is fixed
+ * here, not by the engine's tile size. */
+#define BGR_DIGEST_BLOCK_ROWS 512u
+typedef struct bgr_frame_digest_header {
+    uint64_t layout;       /* seahash fingerprint of what makes two images comparable: word planes per row and, per
+                              column, elem_bytes, first plane, words, optional or not and the checksummed byte range,
+                              and bgr_config.order_base (registered systems are not part of it) */
+    int32_t frame;
+    uint32_t rows;         /* RollbackOrdered::len() captured with the frame */
+    uint32_t n_blocks;     /* ceil(rows / BGR_DIGEST_BLOCK_ROWS) */
+    uint32_t n_columns;
+    uint64_t active;       /* alive rows */
+    uint64_t elapsed_ns;   /* Time<GgrsTime>::elapsed captured with the frame */
+    uint64_t rng[4];       /* ParticleRng state captured with the frame (zero without BGR_SYS_PARTICLES_SPAWN) */
+    uint64_t root;         /* seahash over the n_blocks * (n_columns + 1) words, in order */
+} bgr_frame_digest_header;
+/* Export blob: this header, then per exported block a u32 block index, a u32 zero and the block's tile bytes as
+ * stored (BGR_DIGEST_BLOCK_ROWS * (4 * words + 1) B: the word planes, then the mask bytes).  The bytes of rows >= rows
+ * are zeroed, so stale memory never leaves the machine.  `reserved` and the u32 after each block index are zero; a
+ * blob with anything else there is refused, so later versions can give them a meaning. */
+#define BGR_FRAME_BLOB_MAGIC 0x50424752u /* "RGBP" */
+#define BGR_FRAME_BLOB_VERSION 1u
+typedef struct bgr_frame_blob_header {
+    uint32_t magic;        /* BGR_FRAME_BLOB_MAGIC */
+    uint32_t version;      /* BGR_FRAME_BLOB_VERSION */
+    uint64_t layout;       /* bgr_frame_digest_header.layout */
+    int32_t frame;
+    uint32_t rows;
+    uint32_t words;        /* word planes per row */
+    uint32_t n_blocks;     /* blocks of the whole frame */
+    uint32_t n_exported;   /* blocks that follow, ascending */
+    uint32_t reserved;     /* 0 */
+    uint64_t elapsed_ns;
+    uint64_t rng[4];
+} bgr_frame_blob_header;
+/* Before bgr_build: retain `count` >= 1 confirmed frames that are multiples of `interval` >= 1.  bgr_build then
+ * allocates max_depth (2 * max_depth with BGR_CFG_DESYNC_CAPTURE) + count frame slots, at most 64.
+ * BGR_ERR_STATE after bgr_build, BGR_ERR_UNSUPPORTED on a BGR_CFG_SHARDED engine. */
+BGR_API int bgr_retain_confirmed(bgr_engine* e, uint32_t interval, uint32_t count);
+/* retained frames, the most recently retained first */
+BGR_API int bgr_retained_frames(bgr_engine* e, int32_t* frames_out, uint32_t cap, uint32_t* n_out);
+/* Digest of `frame`, looked up among the queued snapshots first, then the retained ones (*found = 0: neither).
+ * Writes the header and the first min(words_cap, n_blocks * (n_columns + 1)) words; a buffer of
+ * ceil(max_entities / BGR_DIGEST_BLOCK_ROWS) * (n_columns + 1) words always suffices.  Waits for submitted vectors and
+ * leaves their results queued, like bgr_desync_diff. */
+BGR_API int bgr_frame_digest(bgr_engine* e, int32_t frame, bgr_frame_digest_header* header, uint64_t* words, uint32_t words_cap,
+                             int32_t* found);
+/* Host only, the one place the digest format is interpreted.  Refuses (BGR_ERR_INVALID_ARGUMENT) digests of different
+ * layouts, frames or column counts.  Lists, ascending, the blocks whose words differ and the blocks only one side has
+ * (the first `cap`; *n_out = how many there are).  *host_state_differs: bit 0 rng, bit 1 elapsed_ns (the bits of
+ * bgr_desync_summary.host_state_differs), state the block words cannot show. */
+BGR_API int bgr_digest_mismatch(const bgr_frame_digest_header* local_header, const uint64_t* local_words,
+                                const bgr_frame_digest_header* remote_header, const uint64_t* remote_words, uint32_t* blocks_out,
+                                uint32_t cap, uint32_t* n_out, uint32_t* host_state_differs);
+/* Writes the blob of blocks[0..n_blocks) (ascending, each < the frame's block count) of `frame` (queued or retained;
+ * *found = 0: neither) to dst.  *bytes = the blob's size; dst == NULL only reports the size.  BGR_ERR_CAPACITY if
+ * dst_cap is smaller. */
+BGR_API int bgr_frame_export(bgr_engine* e, int32_t frame, const uint32_t* blocks, uint32_t n_blocks, void* dst,
+                             size_t dst_cap, size_t* bytes, int32_t* found);
+/* Diffs the blob's blocks against the same blocks of the local image of `frame` (queued or retained; *found = 0:
+ * neither) with the k_desync_* kernels of bgr_desync_diff: first = local, latest = remote; rows_latest, elapsed_ns_latest
+ * and host_state_differs come from the blob header.  Rows of blocks the blob does not carry are not compared.  The
+ * blob is input from another machine: a bad magic, version or layout, another frame, a truncated or overlong blob, a
+ * block index >= its n_blocks, or an unsorted or duplicate block list is refused with BGR_ERR_INVALID_ARGUMENT. */
+BGR_API int bgr_desync_diff_remote(bgr_engine* e, int32_t frame, const void* blob, size_t bytes,
+                                   bgr_desync_summary* summary, bgr_desync_column* cols, uint32_t cols_cap,
+                                   bgr_desync_record* records, uint32_t records_cap, uint32_t* n_records, int32_t* found);
+
 /* ---- the three schedules, one at a time (SnapshotPlugin-only users: benches/bench.rs:18-27,
  *      mod.rs:510-535 save_world / advance_frame / load_world helpers) -------------------- */
 BGR_API int bgr_save_world(bgr_engine* e, bgr_checksum* checksum_out);         /* world.run_schedule(SaveWorld) */
@@ -431,6 +522,9 @@ BGR_API int bgr_ring_peek(bgr_ring* r, int32_t frame, uint32_t* slot_out, int32_
 BGR_API bgr_ring* bgr_ring_create_capture(uint32_t n_slots);
 BGR_API int bgr_ring_first(bgr_ring* r, int32_t frame, uint32_t* slot_out, int32_t* found);
 BGR_API int bgr_ring_slots_in_use(bgr_ring* r, uint32_t* n_out);  /* queued or pinned slots */
+/* retention of confirmed frames on a standalone ring (bgr_retain_confirmed); count 0 turns it off */
+BGR_API int bgr_ring_set_retention(bgr_ring* r, uint32_t interval, uint32_t count);
+BGR_API int bgr_ring_retained(bgr_ring* r, int32_t* frames_out, uint32_t cap, uint32_t* n_out);  /* newest first */
 
 #ifdef __cplusplus
 }

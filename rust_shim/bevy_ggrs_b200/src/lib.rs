@@ -64,8 +64,10 @@ use bevy_ggrs::{
 /// Where the rollback columns live.  Insert before `GgrsPlugin`; defaults: 1M entities, 9 frame slots, device 0, no
 /// desync capture (`desync_capture: true` keeps every frame's first snapshot for [`desync_report`]; max_depth <= 32).
 #[derive(Resource, Clone, Copy)]
-pub struct B200Config { pub max_entities: u32, pub max_depth: u32, pub device: i32, pub desync_capture: bool }
-impl Default for B200Config { fn default() -> Self { Self { max_entities: 1 << 20, max_depth: 9, device: 0, desync_capture: false } } }
+/// `retain_confirmed: (interval, count)` keeps the last `count` confirmed frames that are multiples of `interval` (the
+/// session's `DesyncDetection::On { interval }`) for [`p2p_desync`]; count 0 keeps none.
+pub struct B200Config { pub max_entities: u32, pub max_depth: u32, pub device: i32, pub desync_capture: bool, pub retain_confirmed: (u32, u32) }
+impl Default for B200Config { fn default() -> Self { Self { max_entities: 1 << 20, max_depth: 9, device: 0, desync_capture: false, retain_confirmed: (0, 0) } } }
 
 /// The engine handle, a non-send resource (one caller thread, like the exclusive system that owns the World,
 /// schedule_systems.rs:19,170).
@@ -122,6 +124,75 @@ pub fn desync_report(world: &World, frame: i32, max_records: u32)
     check(unsafe { sys::bgr_desync_diff(e, frame, &mut summary, cols.as_mut_ptr(), n_cols as u32, recs.as_mut_ptr(), max_records, &mut n, &mut found) });
     recs.truncate(n as usize);
     (found != 0).then_some((summary, cols, recs))
+}
+
+/// P2P desync reports: what to do with `GgrsEvent::DesyncDetected { frame, .. }` (INTEGRATION.md, "Reacting to
+/// `DesyncDetected` between two peers").  The frame is
+/// confirmed by then, so the engine must retain it (`B200Config { retain_confirmed: (interval, count), .. }`); the peers
+/// exchange digests and blocks over the game's own channel (GGRS carries no application messages).
+pub mod p2p_desync {
+    use super::{check, engine, sys, Columns};
+    use bevy::prelude::World;
+
+    /// A frame digest: the header and `n_blocks x (n_columns + 1)` words (`bgr_frame_digest`).
+    #[derive(Clone, Debug)]
+    pub struct Digest { pub header: sys::bgr_frame_digest_header, pub words: Vec<u64> }
+
+    /// Frames retained after they were confirmed, the most recently retained first.
+    pub fn retained_frames(world: &World) -> Vec<i32> {
+        let mut f = [0i32; 64];
+        let mut n = 0u32;
+        check(unsafe { sys::bgr_retained_frames(engine(world), f.as_mut_ptr(), 64, &mut n) });
+        f[..(n as usize).min(64)].to_vec()
+    }
+
+    /// The digest of a queued or retained frame; `None` if the engine holds neither.
+    pub fn digest(world: &World, frame: i32, max_entities: u32) -> Option<Digest> {
+        let n_cols = world.get_resource::<Columns>().map(|c| c.by_type.len()).unwrap_or(0);
+        let per = n_cols + 1;
+        let mut words = vec![0u64; (max_entities as usize).div_ceil(sys::BGR_DIGEST_BLOCK_ROWS as usize) * per];
+        let mut header = sys::bgr_frame_digest_header::default();
+        let mut found = 0i32;
+        check(unsafe { sys::bgr_frame_digest(engine(world), frame, &mut header, words.as_mut_ptr(), words.len() as u32, &mut found) });
+        words.truncate(header.n_blocks as usize * per);
+        (found != 0).then_some(Digest { header, words })
+    }
+
+    /// The blocks whose digests differ, ascending, and the `host_state_differs` bits (bit 0 ParticleRng, bit 1 time).
+    /// Panics (like every engine call) when the digests are of different registrations, frames or column counts.
+    pub fn mismatched_blocks(local: &Digest, remote: &Digest) -> (Vec<u32>, u32) {
+        let mut blocks = vec![0u32; local.header.n_blocks.max(remote.header.n_blocks).max(1) as usize];
+        let (mut n, mut host) = (0u32, 0u32);
+        check(unsafe { sys::bgr_digest_mismatch(&local.header, local.words.as_ptr(), &remote.header, remote.words.as_ptr(),
+                                                blocks.as_mut_ptr(), blocks.len() as u32, &mut n, &mut host) });
+        blocks.truncate(n as usize);
+        (blocks, host)
+    }
+
+    /// The export blob of `blocks` (ascending) of a queued or retained frame; `None` if the engine holds neither.
+    pub fn export(world: &World, frame: i32, blocks: &[u32]) -> Option<Vec<u8>> {
+        let e = engine(world);
+        let (mut bytes, mut found) = (0usize, 0i32);
+        check(unsafe { sys::bgr_frame_export(e, frame, blocks.as_ptr(), blocks.len() as u32, core::ptr::null_mut(), 0, &mut bytes, &mut found) });
+        if found == 0 { return None; }
+        let mut blob = vec![0u8; bytes];
+        check(unsafe { sys::bgr_frame_export(e, frame, blocks.as_ptr(), blocks.len() as u32, blob.as_mut_ptr().cast(), blob.len(), &mut bytes, &mut found) });
+        Some(blob)
+    }
+
+    /// The local image of `frame` ("first") against a peer's blob ("latest"): what [`super::desync_report`] returns.
+    pub fn diff_remote(world: &World, frame: i32, blob: &[u8], max_records: u32)
+        -> Option<(sys::bgr_desync_summary, Vec<sys::bgr_desync_column>, Vec<sys::bgr_desync_record>)> {
+        let n_cols = world.get_resource::<Columns>().map(|c| c.by_type.len()).unwrap_or(0);
+        let mut summary = sys::bgr_desync_summary::default();
+        let mut cols = vec![sys::bgr_desync_column::default(); n_cols];
+        let mut recs = vec![sys::bgr_desync_record::default(); max_records as usize];
+        let (mut n, mut found) = (0u32, 0i32);
+        check(unsafe { sys::bgr_desync_diff_remote(engine(world), frame, blob.as_ptr().cast(), blob.len(), &mut summary, cols.as_mut_ptr(),
+                                                   n_cols as u32, recs.as_mut_ptr(), max_records, &mut n, &mut found) });
+        recs.truncate(n as usize);
+        (found != 0).then_some((summary, cols, recs))
+    }
 }
 
 // ------------------------------------------------------------------------------------------------------------------
@@ -209,6 +280,9 @@ impl<C: Config<Input = u8>> Plugin for GgrsPlugin<C> {
                                   fps, flags: if cfg.desync_capture { sys::BGR_CFG_DESYNC_CAPTURE } else { 0 }, order_base: 0, stream: core::ptr::null_mut() };
         let mut raw = core::ptr::null_mut();
         check(unsafe { sys::bgr_engine_create(&c, &mut raw) });
+        if cfg.retain_confirmed.1 > 0 {
+            check(unsafe { sys::bgr_retain_confirmed(raw, cfg.retain_confirmed.0, cfg.retain_confirmed.1) });
+        }
         app.insert_non_send_resource(B200Engine { raw, built: false })
             .init_resource::<Columns>()
             .init_resource::<Rows>()

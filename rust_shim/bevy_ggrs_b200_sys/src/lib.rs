@@ -56,6 +56,9 @@ pub const BGR_DESYNC_NO_INDEX: u32 = 0xFFFFFFFF;
 // the desync capture structs (bgr_desync_column / _record / _summary) live in their own module
 mod desync;
 pub use desync::*;
+// the P2P desync report structs (bgr_frame_digest_header / bgr_frame_blob_header) too
+mod p2p_desync;
+pub use p2p_desync::*;
 
 #[repr(C)]
 #[derive(Clone, Copy, Default)]
@@ -146,6 +149,12 @@ extern "C" {
     pub fn bgr_desync_frames(e: *mut bgr_engine, frames_out: *mut i32, cap: u32, n_out: *mut u32) -> c_int;
     pub fn bgr_desync_diff(e: *mut bgr_engine, frame: i32, summary: *mut bgr_desync_summary, cols: *mut bgr_desync_column, cols_cap: u32, records: *mut bgr_desync_record, records_cap: u32, n_records: *mut u32, found: *mut i32) -> c_int;
     pub fn bgr_peek_first(e: *mut bgr_engine, frame: i32, column: u32, first_row: u32, count: u32, host_dst: *mut c_void, stride: u32, alive_dst: *mut u8, found: *mut i32) -> c_int;
+    pub fn bgr_retain_confirmed(e: *mut bgr_engine, interval: u32, count: u32) -> c_int;
+    pub fn bgr_retained_frames(e: *mut bgr_engine, frames_out: *mut i32, cap: u32, n_out: *mut u32) -> c_int;
+    pub fn bgr_frame_digest(e: *mut bgr_engine, frame: i32, header: *mut bgr_frame_digest_header, words: *mut u64, words_cap: u32, found: *mut i32) -> c_int;
+    pub fn bgr_digest_mismatch(local_header: *const bgr_frame_digest_header, local_words: *const u64, remote_header: *const bgr_frame_digest_header, remote_words: *const u64, blocks_out: *mut u32, cap: u32, n_out: *mut u32, host_state_differs: *mut u32) -> c_int;
+    pub fn bgr_frame_export(e: *mut bgr_engine, frame: i32, blocks: *const u32, n_blocks: u32, dst: *mut c_void, dst_cap: usize, bytes: *mut usize, found: *mut i32) -> c_int;
+    pub fn bgr_desync_diff_remote(e: *mut bgr_engine, frame: i32, blob: *const c_void, bytes: usize, summary: *mut bgr_desync_summary, cols: *mut bgr_desync_column, cols_cap: u32, records: *mut bgr_desync_record, records_cap: u32, n_records: *mut u32, found: *mut i32) -> c_int;
     pub fn bgr_save_world(e: *mut bgr_engine, checksum_out: *mut bgr_checksum) -> c_int;
     pub fn bgr_load_world(e: *mut bgr_engine) -> c_int;
     pub fn bgr_advance_world(e: *mut bgr_engine, inputs: *const u8, status: *const u8, n_players: u32) -> c_int;

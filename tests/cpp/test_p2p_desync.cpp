@@ -1,0 +1,102 @@
+// P2P desync reports through the C++ host mirror (bevy_ggrs_b200/host/bevy_ggrs.hpp): two peers run the same game with
+// different rollback patterns; peer B's initial population differs in one Tag word of block 0 and one Score of
+// block 2.  Each keeps the confirmed multiples of the desync interval, the digests name exactly blocks 0 and 2, and
+// B's exported blocks diffed on A show exactly those two words.
+// Exit code 0 = passed.  Needs an H100 (tests/test_cpp_p2p_desync.py, -m gpu); `--no-gpu` only checks that the engine
+// refuses to start without a device.
+#include <cstdio>
+#include <set>
+#include <string>
+
+#include "../../bevy_ggrs_b200/host/bevy_ggrs.hpp"
+
+using namespace bevy_ggrs;
+
+static int g_failed = 0;
+#define EXPECT(cond)                                                                  \
+    do {                                                                              \
+        if (!(cond)) { std::printf("  FAILED %s:%d: %s\n", __FILE__, __LINE__, #cond); ++g_failed; } \
+    } while (0)
+
+struct Score { uint32_t v; };   // +1 per frame
+struct Tag { uint32_t a, b; };  // written once, no system
+
+static const uint32_t kRows = 1400;
+
+static void input_system(App& app) {
+    LocalInputs li;
+    for (auto h : app.local_players().handles) li.inputs[h] = 0;
+    app.insert_resource(li);
+}
+
+static void setup(App& app, int seed, bool edited) {
+    std::vector<int> depths;
+    for (int t = 0; t < 80; ++t) depths.push_back((t * seed + 3) % 4);
+    app.insert_resource(Session::P2P(ggrs::P2PTraceSession(2, 8, depths, /*confirm_lag=*/3)))
+        .add_plugins(GgrsPlugin<GgrsConfig<uint8_t>>{})
+        .add_systems(ReadInputs{}, input_system);
+    app.rollback_component_with_copy<Score>().checksum_component_with_hash<Score>();
+    app.rollback_component_with_copy<Tag>().checksum_component_with_hash<Tag>();
+    app.add_systems(GgrsSchedule{}, System{BGR_SYS_U32_ADD, {0}, {0, 1}});
+    app.retain_confirmed(5, 4);
+    app.add_systems(Startup{}, [edited](App& a) {
+        const uint32_t first = a.spawn(kRows);
+        std::vector<Score> s(kRows);
+        std::vector<Tag> t(kRows);
+        for (uint32_t i = 0; i < kRows; ++i) { s[i].v = i * 7u; t[i] = Tag{i, i ^ 0x5a5au}; }
+        if (edited) t[9].b ^= 1u;                                   // block 0
+        if (edited) s[2 * BGR_DIGEST_BLOCK_ROWS + 17].v += 1000u;    // block 2
+        a.write<Score>(first, s);
+        a.write<Tag>(first, t);
+    });
+}
+
+static void two_peers_find_and_diff_the_differing_blocks() {
+    std::printf("two_peers_find_and_diff_the_differing_blocks\n");
+    App a(kRows + 8, 8), b(kRows + 8, 8);
+    setup(a, 5, false);
+    setup(b, 3, true);
+    for (int i = 0; i < 60; ++i) { a.update(); b.update(); }
+    const auto ra = a.retained_frames(), rb = b.retained_frames();
+    EXPECT(ra.size() == 4 && ra == rb);
+    for (ggrs::Frame f : ra) {
+        App::FrameDigest da = a.frame_digest(f), db = b.frame_digest(f);
+        EXPECT(da.found && db.found && f % 5 == 0);
+        uint32_t host = 0;
+        const std::vector<uint32_t> blocks = App::digest_mismatch(da, db, &host);
+        EXPECT((blocks == std::vector<uint32_t>{0, 2}) && host == 0);
+        const std::vector<uint8_t> blob = b.export_blocks(f, blocks);
+        EXPECT(!blob.empty());
+        App::DesyncReport r = a.diff_remote(f, blob, 16);
+        EXPECT(r.found && r.summary.frame == f);
+        EXPECT(r.summary.rows_differing == 2 && r.summary.existence_differing == 0 && r.summary.words_differing == 2);
+        EXPECT(r.columns[a.col<Tag>()].rows == 1 && r.columns[a.col<Score>()].rows == 1);
+        EXPECT(r.records.size() == 2);
+        if (r.records.size() == 2) {
+            EXPECT(r.records[0].row == 9 && r.records[0].column == a.col<Tag>() && r.records[0].word == 1);
+            EXPECT(r.records[0].first == (9u ^ 0x5a5au) && r.records[0].latest == (9u ^ 0x5a5au ^ 1u));
+            EXPECT(r.records[1].row == 2 * BGR_DIGEST_BLOCK_ROWS + 17 && r.records[1].column == a.col<Score>());
+            EXPECT(r.records[1].word == 0 && r.records[1].latest == r.records[1].first + 1000u);
+        }
+    }
+    // a frame neither queued nor retained
+    EXPECT(!a.frame_digest(3).found && a.export_blocks(3, {0}).empty());
+}
+
+int main(int argc, char** argv) {
+    if (argc > 1 && std::string(argv[1]) == "--no-gpu") {
+        try {
+            App app(16, 8);
+            app.rollback_component_with_copy<Score>();
+            app.retain_confirmed(5, 2);
+            app.spawn(1);
+            std::printf("engine started: a GPU is present\n");
+        } catch (const Panic& p) {
+            std::printf("refused: %s\n", p.what());
+        }
+        return 0;
+    }
+    two_peers_find_and_diff_the_differing_blocks();
+    std::printf(g_failed ? "%d check(s) FAILED\n" : "p2p desync test passed\n", g_failed);
+    return g_failed ? 1 : 0;
+}
