@@ -265,8 +265,8 @@ struct bgr_engine {
     unsigned long long* d_digest_words = nullptr;  // [tiles][n_cols + 1]
     unsigned int* d_digest_active = nullptr;       // [tiles]
     uint8_t* d_remote = nullptr;                   // tiles uploaded from a peer's export blob
-    unsigned int* d_remote_visit = nullptr;        // [tiles] their local tile indices
-    uint32_t remote_cap_tiles = 0;
+    unsigned int* d_remote_visit = nullptr;        // [n_tiles_cap] the local tiles a remote diff visits
+    uint32_t remote_cap_tiles = 0;                 // tiles d_remote holds
 
     uint8_t* image(uint32_t idx) const { return arena + size_t(idx) * image_bytes; }
     bool capture() const { return cfg.flags & BGR_CFG_DESYNC_CAPTURE; }
@@ -2186,26 +2186,31 @@ BGR_API int bgr_desync_diff_remote(bgr_engine* e, int32_t frame, const void* blo
     uint32_t slot = 0;
     if (!p2p_slot(e, frame, &slot)) { *found = 0; return BGR_OK; }
     *found = 1;
+    // The local blocks at or past the peer's block count exist only here: every row of them is >= h.rows, so the peer
+    // has none of them and the blob cannot carry them.  They are visited after the exported blocks (positions
+    // n_exported.. of the list, whose staging address is never read: diff_mask_tile answers 0 for a row >= rows_latest
+    // before loading, and words are only loaded for rows that exist on both sides).  Ascending, at most n_tiles_cap.
+    for (uint32_t b = h.n_blocks; b < e->tiles_for(e->st.slot_rows[slot]); ++b) visit.push_back(b);
+    const uint32_t n_visit = uint32_t(visit.size());
+    if (!e->d_remote_visit) CUDA_TRY(cudaMalloc(&e->d_remote_visit, sizeof(unsigned int) * e->n_tiles_cap));
     if (h.n_exported > e->remote_cap_tiles) {  // staging for the peer's tiles, grown on demand
         if (e->d_remote) CUDA_TRY(cudaFree(e->d_remote));
-        if (e->d_remote_visit) CUDA_TRY(cudaFree(e->d_remote_visit));
-        e->d_remote = nullptr; e->d_remote_visit = nullptr; e->remote_cap_tiles = 0;
+        e->d_remote = nullptr; e->remote_cap_tiles = 0;
         CUDA_TRY(cudaMalloc(&e->d_remote, tb * h.n_exported));
-        CUDA_TRY(cudaMalloc(&e->d_remote_visit, sizeof(unsigned int) * h.n_exported));
         e->remote_cap_tiles = h.n_exported;
     }
     for (uint32_t i = 0; i < h.n_exported; ++i)
         CUDA_TRY(cudaMemcpyAsync(e->d_remote + size_t(i) * tb, in + sizeof h + size_t(i) * rec + kBlobBlockHeader, tb,
                                  cudaMemcpyHostToDevice, e->stream));
-    if (h.n_exported)
-        CUDA_TRY(cudaMemcpyAsync(e->d_remote_visit, visit.data(), sizeof(unsigned int) * h.n_exported, cudaMemcpyHostToDevice, e->stream));
+    if (n_visit)
+        CUDA_TRY(cudaMemcpyAsync(e->d_remote_visit, visit.data(), sizeof(unsigned int) * n_visit, cudaMemcpyHostToDevice, e->stream));
     DiffParams p{};
     p.first = e->image(slot + 1);
-    p.latest = e->d_remote;
+    p.latest = e->d_remote;  // null while nothing was ever exported to this engine: then no position reads it
     p.visit = e->d_remote_visit;
     p.rows_first = e->st.slot_rows[slot];
     p.rows_latest = h.rows;
-    rc = run_diff(e, p, h.n_exported, frame, summary, cols, cols_cap, records, records_cap, n_records);
+    rc = run_diff(e, p, n_visit, frame, summary, cols, cols_cap, records, records_cap, n_records);
     if (rc != BGR_OK) return rc;
     summary->host_state_differs = (std::memcmp(&e->st.slot_rng[slot], h.rng, sizeof h.rng) != 0 ? 1u : 0u) |
                                   (e->st.slot_elapsed_ns[slot] != h.elapsed_ns ? 2u : 0u);

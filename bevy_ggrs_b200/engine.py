@@ -278,7 +278,8 @@ class Engine:
         return out.tobytes()
 
     def diff_remote(self, frame: int, blob: bytes, max_records: int = 64) -> Optional[DesyncReport]:
-        """The local image of ``frame`` ("first") against a peer's exported blocks ("latest")."""
+        """The local image of ``frame`` ("first") against a peer's exported blocks ("latest"), plus the local blocks
+        past the peer's block count, whose rows only this side has."""
         s = capi.bgr_desync_summary()
         cols = (capi.bgr_desync_column * max(1, len(self.elem_bytes)))()
         recs = np.zeros(max_records, RECORD_DTYPE)

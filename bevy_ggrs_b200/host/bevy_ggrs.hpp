@@ -263,7 +263,8 @@ public:
     // ---- P2P desync reports (GgrsEvent::DesyncDetected: the frame is confirmed and the other image is remote) ----
     // retain_confirmed before the first update keeps the confirmed multiples of the session's desync interval; the peers
     // exchange frame_digest results over the game's own channel, digest_mismatch (bgr_digest_mismatch, the one reader
-    // of the format) names the blocks, the remote peer export_blocks them and the local peer diff_remote's the blob.
+    // of the format) names the blocks, the remote peer export_blocks those below its own header.n_blocks (possibly
+    // none) and the local peer diff_remote's the blob, which also compares the local blocks the remote frame lacks.
     App& retain_confirmed(uint32_t interval, uint32_t count) {  // applied by the engine's build, like the registrations
         if (engine_) throw Panic(BGR_ERR_STATE, "retain_confirmed must be called before the App is built");
         retain_ = {interval, count};

@@ -263,7 +263,8 @@ class App:
         return self.world.export_blocks(frame, blocks)
 
     def diff_remote(self, frame: int, blob: bytes, max_records: int = 64):
-        """A ``DesyncReport`` of the local image of ``frame`` ("first") against a peer's exported blocks ("latest")."""
+        """A ``DesyncReport`` of the local image of ``frame`` ("first") against a peer's exported blocks ("latest"),
+        plus the local blocks past the peer's block count, whose rows only this side has."""
         self._finish()
         return self.world.diff_remote(frame, blob, max_records)
 

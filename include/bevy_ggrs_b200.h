@@ -317,9 +317,10 @@ BGR_API int bgr_peek_first(bgr_engine* e, int32_t frame, uint32_t column, uint32
  *      u64 words (~62 KB at 1M rows of the stress schema).  The peers exchange digests over the game's own channel
  *      (GGRS carries no application messages; the engine does no networking) and bgr_digest_mismatch lists the blocks
  *      that differ.
- *   3. The peer exports those blocks (bgr_frame_export, the tiles as stored, BGR_DIGEST_BLOCK_ROWS * (4*words + 1) B
- *      each) and the local side diffs them against its own image (bgr_desync_diff_remote): the records and summary of
- *      bgr_desync_diff, with "first" = the local image and "latest" = the remote one.
+ *   3. The peer exports those of the blocks it has, the ones below its digest's n_blocks (bgr_frame_export, the tiles
+ *      as stored, BGR_DIGEST_BLOCK_ROWS * (4*words + 1) B each; possibly none), and the local side diffs them against
+ *      its own image (bgr_desync_diff_remote, which also compares the local blocks the peer's frame does not have): the
+ *      records and summary of bgr_desync_diff, with "first" = the local image and "latest" = the remote one.
  * Digest of block b, for C registered columns (word c < C per column, word C for existence and presence); rows r of
  * the block with r < rows whose alive bit is set "exist":
  *   word c = XOR over existing rows holding column c (absent bit clear) of
@@ -387,7 +388,9 @@ BGR_API int bgr_frame_export(bgr_engine* e, int32_t frame, const uint32_t* block
                              size_t dst_cap, size_t* bytes, int32_t* found);
 /* Diffs the blob's blocks against the same blocks of the local image of `frame` (queued or retained; *found = 0:
  * neither) with the k_desync_* kernels of bgr_desync_diff: first = local, latest = remote; rows_latest, elapsed_ns_latest
- * and host_state_differs come from the blob header.  Rows of blocks the blob does not carry are not compared.  The
+ * and host_state_differs come from the blob header.  The local blocks at or past the blob's n_blocks are compared too:
+ * the peer has none of their rows, so every existing row there is an existence difference, and the blob need not (and
+ * cannot: bgr_frame_export refuses them) carry them.  Rows of other blocks the blob does not carry are not compared.  The
  * blob is input from another machine: a bad magic, version or layout, another frame, a truncated or overlong blob, a
  * block index >= its n_blocks, or an unsorted or duplicate block list is refused with BGR_ERR_INVALID_ARGUMENT. */
 BGR_API int bgr_desync_diff_remote(bgr_engine* e, int32_t frame, const void* blob, size_t bytes,

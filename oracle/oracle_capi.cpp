@@ -181,6 +181,13 @@ static size_t row_of_order(World* w, uint64_t order) {
 ORC_API int orc_remove_component(World* w, uint32_t col, uint64_t order) {
     return guarded([&] { w->has.at(col).at(row_of_order(w, order)) = 0; });
 }
+// commands.entity(e).despawn() on the entity whose RollbackOrdered index is `order` (its index stays in RollbackOrdered)
+ORC_API int orc_despawn(World* w, uint64_t order) {
+    return guarded([&] {
+        std::vector<size_t> rows{row_of_order(w, order)};
+        w->apply_despawns(rows);
+    });
+}
 ORC_API int orc_insert_component(World* w, uint32_t col, uint64_t order, const void* value) {
     return guarded([&] {
         size_t r = row_of_order(w, order);

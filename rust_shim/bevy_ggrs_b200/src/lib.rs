@@ -159,6 +159,7 @@ pub mod p2p_desync {
     }
 
     /// The blocks whose digests differ, ascending, and the `host_state_differs` bits (bit 0 ParticleRng, bit 1 time).
+    /// Blocks only one side has are listed too; ask the peer to export only those below `remote.header.n_blocks`.
     /// Panics (like every engine call) when the digests are of different registrations, frames or column counts.
     pub fn mismatched_blocks(local: &Digest, remote: &Digest) -> (Vec<u32>, u32) {
         let mut blocks = vec![0u32; local.header.n_blocks.max(remote.header.n_blocks).max(1) as usize];
@@ -181,6 +182,7 @@ pub mod p2p_desync {
     }
 
     /// The local image of `frame` ("first") against a peer's blob ("latest"): what [`super::desync_report`] returns.
+    /// Compares the blob's blocks and the local blocks past the peer's block count, whose rows only this side has.
     pub fn diff_remote(world: &World, frame: i32, blob: &[u8], max_records: u32)
         -> Option<(sys::bgr_desync_summary, Vec<sys::bgr_desync_column>, Vec<sys::bgr_desync_record>)> {
         let n_cols = world.get_resource::<Columns>().map(|c| c.by_type.len()).unwrap_or(0);

@@ -78,6 +78,7 @@ def load_oracle() -> C.CDLL:
         "orc_read_alive": (C.c_int, [vp, u32, u32, vp]),
         "orc_remove_component": (C.c_int, [vp, u32, u64]),
         "orc_insert_component": (C.c_int, [vp, u32, u64, vp]),
+        "orc_despawn": (C.c_int, [vp, u64]),
         "orc_peek": (C.c_int, [vp, i32, u32, u32, u32, vp, u32, vp]),
         "orc_snapshot_frames": (C.c_int, [vp, C.POINTER(i32), u32]),
         "orc_read_resource": (C.c_int, [vp, u32, vp]),
@@ -173,6 +174,9 @@ class OracleWorld:
         first = C.c_uint32()
         self._check(self._lib.orc_spawn(self._h, count, C.byref(first)))
         return first.value
+
+    def despawn(self, row):
+        self._check(self._lib.orc_despawn(self._h, row))
 
     def row_count(self):
         return self._lib.orc_row_count(self._h)

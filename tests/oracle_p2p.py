@@ -88,12 +88,14 @@ class RetainOracleWorld(CaptureOracleWorld):
 
 def two_world_diff(a: RetainOracleWorld, b: RetainOracleWorld, frame: int, blocks, max_records: int) -> DesyncReport:
     """The keyed-map diff (component_snapshot.rs:99-115) of a's image of ``frame`` (first) against b's (latest), on the
-    rows of ``blocks`` only, in ascending (row, column, word) order."""
+    rows of ``blocks`` (b's exported blocks) and of a's blocks at or past b's block count (rows only a has), in
+    ascending (row, column, word) order."""
     sa, sb = a.image(frame), b.image(frame)
     n = max(sa["rows"], sb["rows"], max(blocks, default=-1) * BLOCK + BLOCK)
     sel = np.zeros(n, bool)
     for blk in blocks:
         sel[blk * BLOCK:(blk + 1) * BLOCK] = True
+    sel[-(-sb["rows"] // BLOCK) * BLOCK: -(-sa["rows"] // BLOCK) * BLOCK] = True
     ma, mb = a._masks(sa, n), b._masks(sb, n)
     both = (ma != 0) & (mb != 0) & sel
     existence = ((ma != 0) != (mb != 0)) & sel

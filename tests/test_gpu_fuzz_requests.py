@@ -15,6 +15,7 @@ from bevy_ggrs_b200.capi import BgrError
 from bevy_ggrs_b200.engine import Engine
 from bevy_ggrs_b200.session import ADVANCE, LOAD, SAVE, Request
 from oracle_backend import OracleError, OracleWorld
+from schema_util import WIDE_PATHS, expected_kind as _expected_kind, path_env as _path_env
 
 pytestmark = [pytest.mark.gpu, pytest.mark.timeout(300), pytest.mark.usefixtures("generic_kernel")]
 NOSESS = (capi.BGR_SESSION_NONE, 0, 0, 0)
@@ -220,18 +221,6 @@ RANGE_LENS = [0, 1, 3, 4, 8, 12, 16, 20, 31, 32, 33, 60, 64, 68]
 U32_SYSTEMS = [capi.BGR_SYS_U32_ADD, capi.BGR_SYS_U32_SATSUB_DESPAWN, capi.BGR_SYS_U32_STORE_CALL_COUNT]
 
 
-def _expected_kind(path, words, n_sys, nvrtc_ranges, generic_kernel):
-    """The kernel bgr_build / submit pick for this registration (engine.cu bgr_build, jit_specialise, run_stepwise)."""
-    tma_stages = words <= 49   # at least two one-tile stages in 200 KB of shared memory (BGR_TUNE_TMA_STAGES=2 keeps two)
-    if path == "generic" and words <= 49 and n_sys <= 8:
-        if generic_kernel != "interpreter" and words <= 24 and nvrtc_ranges:
-            return "generic_nvrtc"
-        return "generic_interpreter"
-    if path == "stepwise_flat":
-        return "stepwise_flat"
-    return "stepwise_tma" if tma_stages else "stepwise_flat"
-
-
 def _make_wide_worlds(rng, flags, words, aligned):
     """Columns that add up to `words` words (sub-word tails included), up to 7 optional, up to 6 checksummed over
     ranges of the lengths and offsets that change code paths, and 2, 8 or 9 u32 systems."""
@@ -292,20 +281,6 @@ def _make_wide_worlds(rng, flags, words, aligned):
         for i, r in removes:
             w.remove_component(cols[i], r)
     return worlds[0], worlds[1], cols, sizes, optional, len(systems), nvrtc_ranges
-
-
-WIDE_PATHS = {"generic": ({}, 0), "stepwise_tma": ({}, capi.BGR_CFG_FORCE_STEPWISE),
-              "stepwise_flat": ({"BGR_TUNE_TMA": "0"}, capi.BGR_CFG_FORCE_STEPWISE),
-              "stepwise_tma_stages2": ({"BGR_TUNE_TMA_STAGES": "2"}, capi.BGR_CFG_FORCE_STEPWISE)}
-
-
-def _path_env(monkeypatch, path, generic_kernel):
-    if path != "generic" and generic_kernel != "interpreter":
-        pytest.skip("the stepwise path does not depend on the generic kernel: run once")
-    env, flags = WIDE_PATHS[path]
-    for k, v in env.items():
-        monkeypatch.setenv(k, v)
-    return flags
 
 
 @pytest.mark.parametrize("path", list(WIDE_PATHS))

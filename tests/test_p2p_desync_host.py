@@ -257,3 +257,89 @@ def test_oracle_digest_folds_to_the_oracle_checksum_and_retains_by_the_rules():
         cs = capi.bgr_checksum()
         assert lib.bgr_fold_partials(C.byref(p), C.byref(cs)) == 0
         assert cs.lo == latest[f], f
+
+
+@pytest.mark.parametrize("seed,args,order_base", [
+    (0, dict(sizes=[1, 2, 3, 5, 7, 8, 12, 40], n_opt=7), 0),
+    (1, dict(words=24), (1 << 32) + 5),
+    (2, dict(words=50, n_opt=3), 17),
+    (3, dict(sizes=[1024, 3], n_opt=1), 0),
+])
+def test_oracle_digest_folds_on_random_schemas(seed, args, order_base):
+    """The restated digest on schema_util's random registrations (sub-word tails, up to seven optional columns, an
+    order_base above 2^32): for columns checksummed over their whole element, the words fold to the oracle's checksum."""
+    from bevy_ggrs_b200.session import P2PTraceSession
+    from oracle_p2p import RetainOracleWorld
+    from schema_util import random_schema
+    rng = np.random.default_rng(seed)
+    spec = random_schema(rng, ranges=("none", "whole"), **args)
+    n = int(rng.integers(500, 1100))
+    w = RetainOracleWorld(max_entities=n + 8, max_depth=8, order_base=order_base)
+    spec.register(w)
+    w.retain_confirmed(3, 3)
+    w.build()
+    w.spawn(n)
+    for i, d in enumerate(spec.values(rng, n)):
+        w.write_component(i, 0, d)
+    for i in (i for i, o in enumerate(spec.optional) if o):
+        for r in rng.choice(n, 9, replace=False):
+            w.remove_component(i, int(r))
+    sess, latest = P2PTraceSession(2, 8, seed=seed, p_clean=0.3), {}
+    for t in range(24):
+        if t % 6 == 5:
+            alive = np.flatnonzero(w.read_alive(0, n))
+            w.despawn(int(alive[len(alive) // 2]))
+        for h in range(2):
+            sess.add_local_input(h, 0)
+        for f, c in w.handle_requests(sess.info(), sess.advance_frame()):
+            latest[f] = c
+    assert len(w.retained_frames()) == 3
+    lib = capi.load_library()
+    frames = w.snapshot_frames() + w.retained_frames()
+    assert any(w.frame_digest(f)[1] < w.frame_digest(f)[0] for f in frames)   # despawned rows are in the frames
+    for f in frames:
+        rows, active, words = w.frame_digest(f)
+        p = capi.bgr_partial()
+        p.frame, p.n_columns, p.active, p.total = f, len(spec.cks), active, rows
+        x = np.bitwise_xor.reduce(words, axis=0)
+        for k, (i, _, _) in enumerate(spec.cks):
+            p.xor_[k] = int(x[i])
+        cs = capi.bgr_checksum()
+        assert lib.bgr_fold_partials(C.byref(p), C.byref(cs)) == 0
+        assert cs.lo == latest[f], f
+
+
+def test_two_world_diff_reports_the_local_only_rows_as_existence_records():
+    """A frame with more blocks locally than on the peer: the local blocks at or past the peer's block count are
+    diffed without the peer exporting them (it cannot), so every existing row there is an existence record."""
+    from bevy_ggrs_b200.desync import NO_INDEX
+    from bevy_ggrs_b200.session import SAVE, SESSION_NONE, Request
+    from oracle_p2p import RetainOracleWorld, two_world_diff
+
+    def world(rows):
+        w = RetainOracleWorld(max_entities=1100, max_depth=4)
+        w.rollback_component("A", 6)
+        w.rollback_component("B", 4, capi.BGR_STRATEGY_COPY | capi.BGR_STRATEGY_OPTIONAL)
+        w.checksum_component(0, 2, 4)
+        w.set_depth(2)
+        w.spawn(rows)
+        w.write_component(0, 0, np.arange(rows * 6, dtype=np.uint32).astype(np.uint8).reshape(rows, 6))
+        w.remove_component(1, 3)
+        return w
+    big, small = world(1030), world(512)          # 3 blocks against 1
+    big.despawn(1029)
+    big.remove_component(1, 600)
+    for w in (big, small):
+        w.handle_requests((SESSION_NONE, 0, 0, 0), [Request(SAVE, 0)])
+    for blocks in ([0], []):
+        rep = two_world_diff(big, small, 0, blocks, 10_000)
+        local_only = [r for r in range(512, 1029)]
+        assert rep.existence_differing == rep.rows_differing == len(local_only)
+        assert list(rep.records["row"]) == local_only
+        assert set(rep.records["column"]) == {NO_INDEX} and set(rep.records["word"]) == {NO_INDEX}
+        assert set(rep.records["latest"]) == {0} and set(rep.records["first"]) == {1, 1 | 2}   # row 600: B absent
+        assert rep.columns[1].presence == 0
+    # the other direction diffs only what the blob carries: the peer's rows past 512 are in blocks 1 and 2
+    assert two_world_diff(small, big, 0, [0], 10_000).rows_differing == 0
+    rep = two_world_diff(small, big, 0, [1, 2], 10_000)
+    assert rep.existence_differing == len(local_only) and set(rep.records["first"]) == {0}
