@@ -56,6 +56,8 @@ BGR_KERNEL_NONE, BGR_KERNEL_STEPWISE_TMA, BGR_KERNEL_STEPWISE_FLAT, BGR_KERNEL_B
 # ... and flags: the vector deferred its live-image write / started from a deferred live image's base slot
 BGR_KERNEL_DEFERRED_LIVE = 1 << 13
 BGR_KERNEL_FROM_DEFERRED = 1 << 14
+# ... and the bundle launch read or wrote passive planes
+BGR_KERNEL_PASSIVE_PLANES = 1 << 15
 
 
 class bgr_request(C.Structure):

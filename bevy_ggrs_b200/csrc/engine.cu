@@ -92,7 +92,27 @@ struct HostState {  // trivially copyable: copying it per call must not allocate
     uint32_t call_count = 0;                // un-rolled-back counter of BGR_SYS_U32_STORE_CALL_COUNT
     ParticleRng rng;                        // ParticleRng resource (particles.rs:128)
     std::array<ParticleRng, SlotRing::kMaxSlots> slot_rng{};  // its per-snapshot clones
-    // content versions of the passive planes (BGR_CFG_SKIP_UNCHANGED_PLANES): equal ids <=> identical bytes
+    // Content versions of the passive planes (those no registered system writes).  Every engine relies on:
+    //   slot_passive_ver[s] == live_passive_ver  =>  slot s holds the live image's passive bytes on every row below
+    //   the row count, dead rows included
+    // so a Save into such a slot stores no passive plane (OPF_SKIP_PASSIVE) and a Load from it rewrites none.  A version
+    // also fixes the row count: rows grow only through spawns (in a program, bgr_spawn, the startup system), which bump
+    // it, and a Load takes the slot's row count with its version, so a matching slot covers every row a later program
+    // touches.  Who writes image 0 or a slot, and why the invariant holds:
+    //   - compile_requests: a Save takes the live version; a Load makes the slot's version live; a spawn bumps
+    //     (newborn rows carry Transform::default()).
+    //   - deferred live image: the version is settled when the deferring program compiles.  The materialisation
+    //     launch, the prepended LOAD(base) and the early write restore exactly the bytes that version names
+    //     (DeferredLive::passive keeps the live passive write the eager program would have made).
+    //   - host writes of image 0 bump: transfer_column to the device (bgr_write_component, bgr_insert_component),
+    //     bgr_spawn, bgr_run_startup_system, bgr_remove_component.  bgr_despawn writes only the alive byte, an active
+    //     plane.  bgr_reset_session, bgr_set_depth and bgr_confirm move no bytes; slots keep bytes and versions.
+    //   - slots are written only by Saves; desync capture and retention hand a slot index out again with its
+    //     bytes, and the version is per slot index.
+    //   - the stepwise path, the interpreter and k_generic_jit ignore OPF_SKIP_PASSIVE and store whole images, which
+    //     keeps the invariant.  A sharded engine keeps its own versions.
+    //   - overlapping launches (PF_TILE_WAIT): elision only drops passive reads and stores, and a tick after a bump
+    //     stages the passive planes exactly as every tick did before, so no launch reads what an earlier one writes.
     uint64_t live_passive_ver = 1, ver_counter = 1;
     std::array<uint64_t, SlotRing::kMaxSlots> slot_passive_ver{};  // 0 = never written
 };
@@ -350,7 +370,7 @@ int compile_requests(bgr_engine* e, HostState& s, const bgr_session_info* sess, 
                 s.slot_rows[slot] = s.n_rows;
                 s.slot_elapsed_ns[slot] = s.elapsed_ns;
                 s.slot_rng[slot] = s.rng;
-                if ((e->cfg.flags & BGR_CFG_SKIP_UNCHANGED_PLANES) && s.slot_passive_ver[slot] == s.live_passive_ver)
+                if (s.slot_passive_ver[slot] == s.live_passive_ver)
                     op.flags |= OPF_SKIP_PASSIVE;
                 else
                     pg.passive_to_slots = true;
@@ -372,7 +392,7 @@ int compile_requests(bgr_engine* e, HostState& s, const bgr_session_info* sess, 
             s.n_rows = s.slot_rows[slot];
             s.elapsed_ns = s.slot_elapsed_ns[slot];
             s.rng = s.slot_rng[slot];
-            if (!(e->cfg.flags & BGR_CFG_SKIP_UNCHANGED_PLANES) || s.slot_passive_ver[slot] != s.live_passive_ver)
+            if (s.slot_passive_ver[slot] != s.live_passive_ver)
                 pg.passive_to_live = true;
             s.live_passive_ver = s.slot_passive_ver[slot];
             op.kind = OP_LOAD;
@@ -468,10 +488,12 @@ int launch_particles(bgr_engine* e, const ProgramParams& pp) {
     CUDA_TRY(cudaLaunchKernelEx(&lc, kern, pp));
     CUDA_TRY(cudaGetLastError());
     e->launches += 1;
-    const bool tma = ti && pp.n_runs > 0;  // the kernel's `use_tma`
+    // bit 12: the passive-TMA configuration (double buffer, its own opt-in and occupancy); whether this launch moved any
+    // passive plane at all is BGR_KERNEL_PASSIVE_PLANES: a steady-state tick whose slots already hold them moves none
+    const bool passive = pp.n_runs > 0 || pp.n_passive > 0;
     // VEC 2, launch-bounds tier 1 (768 threads per SM), whole-tile work items
-    e->last_kernel = BGR_KERNEL_BUNDLE | (2u << 4) | (uint32_t(MODE) << 8) | (1u << 10) | (tma ? 1u << 12 : 0u) |
-                     (uint32_t(kTileRows) << 16);
+    e->last_kernel = BGR_KERNEL_BUNDLE | (2u << 4) | (uint32_t(MODE) << 8) | (1u << 10) | (ti ? 1u << 12 : 0u) |
+                     (passive ? BGR_KERNEL_PASSIVE_PLANES : 0u) | (uint32_t(kTileRows) << 16);
     return BGR_OK;
 }
 

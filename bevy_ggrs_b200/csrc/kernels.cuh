@@ -73,7 +73,10 @@ enum OpKind : uint32_t { OP_SAVE = 0, OP_LOAD = 1, OP_ADVANCE = 2 };
 enum OpFlags : uint32_t {
     OPF_NO_STORE = 1u,  // SAVE with ring depth 0: checksum only
     OPF_SPAWN = 2u,     // ADVANCE: spawn_particles fired; rows [spawn_first, spawn_first+spawn_count) are born at the end of the frame
-    OPF_SKIP_PASSIVE = 4u,  // SAVE: the slot already holds the current content of the passive planes (BGR_CFG_SKIP_UNCHANGED_PLANES)
+    // SAVE: the slot already holds the current content of the passive planes (content versions, engine.cu HostState).
+    // Only this bundle kernel honours it; every other kernel stores whole images, which keeps the versions true.  A
+    // kernel that stores partial images must keep versions of its own.
+    OPF_SKIP_PASSIVE = 4u,
     // bits 8..11 of an ADVANCE op's flags: number of players (PlayerInputs<T>.len())
 };
 

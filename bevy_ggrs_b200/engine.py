@@ -24,7 +24,9 @@ class LastKernel(NamedTuple):
     """bgr_last_kernel decoded.  vec / mode / tier / passive_tma describe the bundle kernel (0 / False otherwise);
     item_rows is set for the bundle and the NVRTC kernel.  tier: 0 unconstrained, 1 768 and 2 1024 threads per SM.
     deferred_live: the vector did not write the live image (BGR_TUNE_DEFER_LIVE); from_deferred: it started from the
-    base slot of the previous vector's deferred live image."""
+    base slot of the previous vector's deferred live image.  passive_tma: the bundle ran in its passive-TMA
+    configuration; passive_planes: the bundle launch read or wrote passive planes at all (clear on ticks whose slots
+    already hold them)."""
     kind: str
     vec: int
     mode: int
@@ -34,12 +36,14 @@ class LastKernel(NamedTuple):
     raw: int
     deferred_live: bool = False
     from_deferred: bool = False
+    passive_planes: bool = False
 
     @staticmethod
     def decode(v: int) -> "LastKernel":
         return LastKernel(_KERNEL_KINDS.get(v & 0xF, f"unknown({v & 0xF})"), (v >> 4) & 0xF, (v >> 8) & 0x3,
                           (v >> 10) & 0x3, bool((v >> 12) & 1), (v >> 16) & 0x3FF, v,
-                          bool(v & capi.BGR_KERNEL_DEFERRED_LIVE), bool(v & capi.BGR_KERNEL_FROM_DEFERRED))
+                          bool(v & capi.BGR_KERNEL_DEFERRED_LIVE), bool(v & capi.BGR_KERNEL_FROM_DEFERRED),
+                          bool(v & capi.BGR_KERNEL_PASSIVE_PLANES))
 
 
 class Engine:

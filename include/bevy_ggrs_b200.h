@@ -166,12 +166,12 @@ typedef struct bgr_config {
 } bgr_config;
 #define BGR_CFG_FORCE_STEPWISE 1u  /* never use the fused one-launch program kernel (debug / A-B tests) */
 #define BGR_CFG_SHARDED 2u         /* handle_requests returns partials only; caller folds across shards */
-/* OPT-IN, off by default: do not rewrite word planes whose content is provably identical to what the target
- * image already holds.  The engine tracks a content version for the planes no registered system writes
- * (e.g. Transform.rotation/scale in the stress test): a Save into a slot that already holds the current version
- * skips those planes, and so does a Load.  Snapshots stay complete images (peek / load need no indirection) and
- * every observable result is unchanged; only redundant HBM stores are elided.  The reference clones every
- * registered component on every save (component_snapshot.rs:71-75), so the default keeps doing exactly that. */
+/* Accepted and ignored; kept so that code naming it still compiles.  Every engine now skips word planes whose content
+ * is provably identical to what the target image already holds: it tracks a content version for the planes no
+ * registered system writes (e.g. Transform.rotation/scale in the stress test), and a Save into a slot that already
+ * holds the current version stores none of them, nor does a Load from it.  Snapshots stay complete images (peek, load,
+ * desync capture and digests read the same bytes) and every observable result is what the reference's clone of every
+ * registered component on every save (component_snapshot.rs:71-75) gives; only redundant HBM traffic is elided. */
 #define BGR_CFG_SKIP_UNCHANGED_PLANES 4u
 /* OPT-IN, off by default: keep the first-recorded image of every frame so a SyncTest mismatch can be inspected
  * (bgr_desync_*, below).  bgr_build allocates 2*max_depth frame slots instead of max_depth; the ring hands a frame's
@@ -481,14 +481,19 @@ BGR_API int bgr_generic_specialised(bgr_engine* e, uint32_t* specialised_out);
  *   bits 8-9   bundle: MODE 0 (checksum flags tested at run time), 1 (Transform and Velocity both checksummed with
  *              BGR_HASH_FLAG_ASSERT_FINITE_F32: specialised), 2 (per-entity presence of optional columns)
  *   bits 10-11 bundle: launch-bounds tier, 0 unconstrained, 1 768 threads per SM, 2 1024 threads per SM
- *   bit 12     bundle: passive planes moved by TMA bulk copies
+ *   bit 12     bundle: launched in the passive-TMA configuration (shared-memory double buffer): passive planes the
+ *              launch moves go by TMA bulk copies; clear: they go per thread (spawns, several Loads, BGR_TUNE_PASSIVE_TMA=0)
  *   bit 13     BGR_KERNEL_DEFERRED_LIVE: the vector ended in Save, Advance... and did not write the live image; it is
  *              rebuilt from that Save's slot when something needs it (env BGR_TUNE_DEFER_LIVE, default 1)
  *   bit 14     BGR_KERNEL_FROM_DEFERRED: the vector would have read a deferred live image and started from the base
  *              slot instead (a Load of that slot and its pending Advances ran first, inside the same launch)
+ *   bit 15     BGR_KERNEL_PASSIVE_PLANES, bundle: the launch read or wrote passive planes.  Clear on a tick whose Saves
+ *              go into slots that already hold the live passive content and whose Load does not change it
+ *              (BGR_CFG_SKIP_UNCHANGED_PLANES above)
  *   bits 16-25 bundle and generic NVRTC: rows per work item (512 = a whole tile) */
 #define BGR_KERNEL_DEFERRED_LIVE (1u << 13)
 #define BGR_KERNEL_FROM_DEFERRED (1u << 14)
+#define BGR_KERNEL_PASSIVE_PLANES (1u << 15)
 #define BGR_KERNEL_NONE 0u
 #define BGR_KERNEL_STEPWISE_TMA 1u       /* one kernel per request; Save / Load through the TMA-staged copy kernel */
 #define BGR_KERNEL_STEPWISE_FLAT 2u      /* one kernel per request; k_checksum_column + k_copy_image */

@@ -46,6 +46,8 @@ pub const BGR_KERNEL_GENERIC_NVRTC: u32 = 5;
 pub const BGR_KERNEL_DEFERRED_LIVE: u32 = 1 << 13;
 /// bgr_last_kernel flag: the request vector started from a deferred live image's base slot.
 pub const BGR_KERNEL_FROM_DEFERRED: u32 = 1 << 14;
+/// bgr_last_kernel flag: the bundle launch read or wrote passive planes.
+pub const BGR_KERNEL_PASSIVE_PLANES: u32 = 1 << 15;
 
 pub const BGR_CFG_FORCE_STEPWISE: u32 = 1;
 pub const BGR_CFG_SHARDED: u32 = 2;

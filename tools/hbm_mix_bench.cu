@@ -3,9 +3,9 @@
 // reads 1 image and writes 9 (1 read : 9 writes).  This tool measures, with CUDA events:
 //   copy      1 read : 1 write   (plain 16-byte loads/stores)         == the driver's measurement shape
 //   fill      0 read : 1 write
-//   fanout    1 read : F writes  (plain stores)                       == the tick's mix for F = 9
+//   fanout    1 read : F writes  (plain stores)                       == the tick's mix: F = 8 Saves (live image deferred)
 //   fanout_tma 1 read : F writes (cp.async.bulk global->smem->global)
-// Output: one JSON line.  Not part of the product; evidence for the roofline discussion in DESIGN.md.
+// Usage: hbm_mix_bench [image_bytes] [F = 8 or 9].  Output: one JSON line.  Not part of the product; evidence for the roofline discussion in DESIGN.md.
 #include <cuda_runtime.h>
 #include <cstdint>
 #include <cstdio>
@@ -83,9 +83,8 @@ static double time_us(L launch, int iters) {
     return double(ms) * 1e3 / iters;
 }
 
-int main(int argc, char** argv) {
-    const size_t img = (argc > 1 ? size_t(atoll(argv[1])) : size_t(61) * 1000448);  // bytes of one image
-    const int F = 9;
+template <int F>
+static void run(size_t img) {
     const size_t n = img / 16, stride_v = (img / 16 + 63) & ~size_t(63);
     uint8_t *src, *dst;
     // large source ring so reads are not served by L2: rotate over 8 source images
@@ -107,8 +106,16 @@ int main(int argc, char** argv) {
     double t_tma = time_us([&] { k_fanout_tma<F><<<sms * 2, 32, 2 * chunk>>>(reinterpret_cast<const uint8_t*>(srcp()), reinterpret_cast<uint8_t*>(dstp()), n * 16, stride_v * 16, chunk); }, iters);
     CK(cudaGetLastError());
     printf("{\"image_bytes\": %zu, \"fanout\": %d, \"copy_1r1w\": {\"us\": %.2f, \"gbps\": %.0f}, \"fill_0r1w\": {\"us\": %.2f, \"gbps\": %.0f}, "
-           "\"fanout_1r9w_stg\": {\"us\": %.2f, \"gbps\": %.0f}, \"fanout_1r9w_tma\": {\"us\": %.2f, \"gbps\": %.0f}}\n",
+           "\"fanout_stg\": {\"us\": %.2f, \"gbps\": %.0f}, \"fanout_tma\": {\"us\": %.2f, \"gbps\": %.0f}}\n",
            n * 16, F, t_copy, 2.0 * n * 16 / t_copy / 1e3, t_fill, double(F) * n * 16 / t_fill / 1e3,
            t_fan, double(F + 1) * n * 16 / t_fan / 1e3, t_tma, double(F + 1) * n * 16 / t_tma / 1e3);
+}
+
+int main(int argc, char** argv) {
+    const size_t img = (argc > 1 ? size_t(atoll(argv[1])) : size_t(61) * 1000448);  // bytes of one image
+    const int F = argc > 2 ? atoi(argv[2]) : 9;
+    if (F == 8) run<8>(img);
+    else if (F == 9) run<9>(img);
+    else { fprintf(stderr, "fan-out must be 8 or 9\n"); return 2; }
     return 0;
 }
