@@ -11,6 +11,7 @@
 
 #include <algorithm>
 #include <array>
+#include <cmath>
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
@@ -414,6 +415,8 @@ int compile_requests(bgr_engine* e, HostState& s, const bgr_session_info* sess, 
             s.elapsed_ns = runtime;
             op.kind = OP_ADVANCE;
             op.dt_bits = f32_bits(duration_as_secs_f32(delta));
+            // move_cube_system's friction (box_game.rs:188-193) with the C library's powf, as the reference evaluates it
+            op.fr_bits = f32_bits(powf(0.0018f, duration_as_secs_f32(delta)));
             op.n_rows = s.n_rows;
             op.call_count = s.call_count;
             s.call_count += n_counter_systems;
@@ -717,7 +720,7 @@ int run_stepwise(bgr_engine* e, const Program& pg, uint32_t buf) {
                     unsigned long long packed = 0;
                     for (int k = 0; k < 8; ++k) packed |= (unsigned long long)(op.inputs[k]) << (8 * k);
                     k_sys_box_move<<<grid, 256, 0, e->stream>>>(live, e->words, e->cols[sy.cols[0]].first_plane, e->cols[sy.cols[1]].first_plane,
-                                                                 n, op.dt_bits, packed, (op.flags >> 8) & 0xFu, e->cfg.order_base, need);
+                                                                 n, op.dt_bits, op.fr_bits, packed, (op.flags >> 8) & 0xFu, e->cfg.order_base, need);
                     break;
                 }
                 default: return fail(BGR_ERR_UNSUPPORTED, "system has no GPU implementation yet");

@@ -280,7 +280,7 @@ __global__ void __launch_bounds__(kGenericBlock) k_generic_program(const __grid_
                                 float tx = t[0], ty = t[kTileRows], tz = t[2 * kTileRows], vx = v[0], vy = v[kTileRows], vz = v[2 * kTileRows];
                                 const unsigned long long handle = row0 + uint32_t(k * kGenericBlock);
                                 const uint32_t input = handle < n_players && handle < 8 ? op.inputs[handle] : 0u;
-                                box_move_step(tx, ty, tz, vx, vy, vz, dt, input);
+                                box_move_step(tx, ty, tz, vx, vy, vz, dt, __uint_as_float(op.fr_bits), input);
                                 t[0] = tx; t[kTileRows] = ty; t[2 * kTileRows] = tz; v[0] = vx; v[kTileRows] = vy; v[2 * kTileRows] = vz;
                             }
                         break;

@@ -90,13 +90,13 @@ __device__ __forceinline__ void jit_run_systems(JitRows& r, const Op& op, float 
                 if (on) { r.w[k][sy.plane0] = uint32_t(ttl); r.w[k][sy.plane0 + 1] = uint32_t(ttl >> 32); }
                 r.kill[k] = r.kill[k] || (on && ttl == 0);
             } else if constexpr (sy.id == BGR_SYS_BOX_MOVE) {
-                if (on) {  // two to four entities: a branch costs nothing and keeps powf off the other rows
+                if (on) {  // two to four entities: a branch costs nothing and keeps the step off the other rows
                     float tx = __uint_as_float(r.w[k][sy.plane0]), ty = __uint_as_float(r.w[k][sy.plane0 + 1]), tz = __uint_as_float(r.w[k][sy.plane0 + 2]);
                     float vx = __uint_as_float(r.w[k][sy.plane1]), vy = __uint_as_float(r.w[k][sy.plane1 + 1]), vz = __uint_as_float(r.w[k][sy.plane1 + 2]);
                     const unsigned long long handle = row0 + uint32_t(k * B);
                     const uint32_t n_players = (op.flags >> 8) & 0xFu;
                     const uint32_t input = handle < n_players && handle < 8 ? op.inputs[handle] : 0u;
-                    box_move_step(tx, ty, tz, vx, vy, vz, dt, input);
+                    box_move_step(tx, ty, tz, vx, vy, vz, dt, __uint_as_float(op.fr_bits), input);
                     r.w[k][sy.plane0] = __float_as_uint(tx); r.w[k][sy.plane0 + 1] = __float_as_uint(ty); r.w[k][sy.plane0 + 2] = __float_as_uint(tz);
                     r.w[k][sy.plane1] = __float_as_uint(vx); r.w[k][sy.plane1 + 1] = __float_as_uint(vy); r.w[k][sy.plane1 + 2] = __float_as_uint(vz);
                 }

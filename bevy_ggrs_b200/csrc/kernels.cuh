@@ -84,13 +84,14 @@ struct Op {
     uint32_t kind;
     uint32_t image_off256;  // LOAD/SAVE: byte offset of the image read / written, in 256-byte units.  ADVANCE+SPAWN: first spawned row
     uint32_t dt_bits;       // ADVANCE: Time<GgrsTime>::delta_secs as f32 bits (time.rs:63-76)
-    uint32_t n_rows;        // rows that exist while this op runs (RollbackOrdered::len())
+    uint32_t fr_bits;       // ADVANCE: 0.0018f.powf(dt) as f32 bits (box_game.rs:188-193), from the host's C library powf
+    uint32_t n_rows;       // rows that exist while this op runs (RollbackOrdered::len())
     uint32_t save_index;    // SAVE: which accumulator row.  ADVANCE+SPAWN: number of spawned rows
     uint32_t flags;
     uint32_t call_count;    // ADVANCE: value of the un-rolled-back host counter (test system).  ADVANCE+SPAWN: offset into spawn_vals
     uint8_t inputs[8];      // ADVANCE: PlayerInputs<T>.0[handle].0 for every handle (u8, BGR_MAX_PLAYERS)
 };
-static_assert(sizeof(Op) == 36, "Op layout");
+static_assert(sizeof(Op) == 40, "Op layout");
 
 enum ProgFlags : uint32_t {
     PF_READ_LIVE = 1u,           // program does not start with LOAD: initial state comes from image 0
@@ -885,17 +886,18 @@ __global__ void __launch_bounds__(256) k_sys_particles_spawn(uint8_t* img, uint3
 #endif  // !__CUDACC_RTC__
 
 // move_cube_system (box_game.rs:154-206), BASELINE config C1.  player handle == RollbackOrdered index.
-// `FRICTION.powf(dt)` is libm on the CPU and CUDA powf here: this is the one system of the path whose f32
-// results are only guaranteed within a tolerance (|d| <= 1e-5 * max(1, |x|), tested), not bit-exact.
-__device__ __forceinline__ void box_move_step(float& tx, float& ty, float& tz, float& vx, float& vy, float& vz, float dt, uint32_t input) {
-    const float ACCELERATION = 18.0f, MAX_SPEED = 3.0f, FRICTION = 0.0018f, PLANE_SIZE = 5.0f, CUBE_SIZE = 0.2f;
+// `fr` is `FRICTION.powf(dt)` (FRICTION = 0.0018), evaluated once per Advance by the host with the C library's powf,
+// the function the reference calls (Op::fr_bits).  A device powf is only good to about one ulp and rounds some frame
+// rates' factor the other way, so every result here is bit-exact with the CPU only because the factor comes from the host.
+__device__ __forceinline__ void box_move_step(float& tx, float& ty, float& tz, float& vx, float& vy, float& vz, float dt, float fr,
+                                              uint32_t input) {
+    const float ACCELERATION = 18.0f, MAX_SPEED = 3.0f, PLANE_SIZE = 5.0f, CUBE_SIZE = 0.2f;
     const bool up = input & 1u, down = input & 2u, left = input & 4u, right = input & 8u;
     const float a = __fmul_rn(ACCELERATION, dt);
     if (up && !down) vz = __fsub_rn(vz, a);
     if (!up && down) vz = __fadd_rn(vz, a);
     if (left && !right) vx = __fsub_rn(vx, a);
     if (!left && right) vx = __fadd_rn(vx, a);
-    const float fr = powf(FRICTION, dt);
     if (!up && !down) vz = __fmul_rn(vz, fr);
     if (!left && !right) vx = __fmul_rn(vx, fr);
     vy = __fmul_rn(vy, fr);
@@ -912,9 +914,9 @@ __device__ __forceinline__ void box_move_step(float& tx, float& ty, float& tz, f
 }
 #ifndef __CUDACC_RTC__
 __global__ void k_sys_box_move(uint8_t* img, uint32_t words, uint32_t t_plane, uint32_t v_plane, uint32_t n_rows,
-                               uint32_t dt_bits, unsigned long long inputs_packed, uint32_t n_players, unsigned long long order_base,
-                               uint32_t need) {
-    const float dt = __uint_as_float(dt_bits);
+                               uint32_t dt_bits, uint32_t fr_bits, unsigned long long inputs_packed, uint32_t n_players,
+                               unsigned long long order_base, uint32_t need) {
+    const float dt = __uint_as_float(dt_bits), fr = __uint_as_float(fr_bits);
     for (uint32_t r = blockIdx.x * blockDim.x + threadIdx.x; r < n_rows; r += gridDim.x * blockDim.x) {
         if (!row_matches(img[alive_offset(words, r)], need)) continue;
         float* t = reinterpret_cast<float*>(img + word_offset(words, r, t_plane));
@@ -923,7 +925,7 @@ __global__ void k_sys_box_move(uint8_t* img, uint32_t words, uint32_t t_plane, u
         float vx = v[0], vy = v[kTileRows], vz = v[2 * kTileRows];
         const unsigned long long handle = order_base + r;
         const uint32_t input = handle < n_players && handle < 8 ? uint32_t(inputs_packed >> (8 * uint32_t(handle))) & 0xffu : 0u;
-        box_move_step(tx, ty, tz, vx, vy, vz, dt, input);
+        box_move_step(tx, ty, tz, vx, vy, vz, dt, fr, input);
         t[0] = tx; t[kTileRows] = ty; t[2 * kTileRows] = tz;
         v[0] = vx; v[kTileRows] = vy; v[2 * kTileRows] = vz;
     }

@@ -592,6 +592,7 @@ struct World {
             uint32_t tc = s.cols[0], vc = s.cols[1];
             const float ACCELERATION = 18.0f, MAX_SPEED = 3.0f, FRICTION = 0.0018f, PLANE_SIZE = 5.0f, CUBE_SIZE = 0.2f;
             for (size_t r = 0; r < rows(); ++r) {
+                if (!has[tc][r] || !has[vc][r]) continue;  // Query<(&mut Transform, &mut Velocity, &Player)>
                 float* t = reinterpret_cast<float*>(&data[tc][r * 40]);
                 float* v = reinterpret_cast<float*>(&data[vc][r * 12]);
                 uint64_t handle = rollback_ordered.order_of(rollback_id[r]);

@@ -261,18 +261,14 @@ static void box_game_synctest_c1() {
     EXPECT(app.resource<FrameCount>().frame == 100);
     auto te = app.read<Transform>(0, 2);
     auto ve = app.read<Velocity>(0, 2);
-    bool within = true, moved = false;
+    bool equal = true, moved = false;
     for (int h = 0; h < 2; ++h) {
         size_t row = size_t(w.find_row(uint64_t(h)));
-        const float* to = reinterpret_cast<const float*>(&w.data[ot][row * 40]);
-        const float* vo = reinterpret_cast<const float*>(&w.data[ov][row * 12]);
-        for (int k = 0; k < 3; ++k) {
-            within = within && std::fabs(te[h].translation[k] - to[k]) <= 1e-5f * std::max(1.0f, std::fabs(to[k]));
-            within = within && std::fabs(ve[h].v[k] - vo[k]) <= 1e-5f * std::max(1.0f, std::fabs(vo[k]));
-            moved = moved || ve[h].v[k] != 0.0f;
-        }
+        equal = equal && std::memcmp(te[h].translation, &w.data[ot][row * 40], 12) == 0;
+        equal = equal && std::memcmp(ve[h].v, &w.data[ov][row * 12], 12) == 0;
+        for (int k = 0; k < 3; ++k) moved = moved || ve[h].v[k] != 0.0f;
     }
-    EXPECT(within);  // powf: the north_star's stated f32 tolerance
+    EXPECT(equal);  // bit-identical: the friction factor is the C library's powf on both sides
     EXPECT(moved);
 }
 

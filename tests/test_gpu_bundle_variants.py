@@ -71,14 +71,19 @@ def _outcome(w, reqs):
         return ("raised", ex.status, str(ex))
 
 
+# +inf, -inf, quiet NaNs of both signs, signalling NaNs (one with a payload): every encoding the hasher refuses
+NON_FINITE = [0x7F800000, 0xFF800000, 0x7FC00000, 0xFFC00000, 0x7F800001, 0xFFC01234]
+
+
+@pytest.mark.parametrize("pattern", NON_FINITE, ids=hex)
 @pytest.mark.parametrize("flags", [0, capi.BGR_CFG_FORCE_STEPWISE])
 @pytest.mark.parametrize("column", ["velocity", "transform"])
 @pytest.mark.parametrize("setup", list(MODE0_SETUPS) + ["mode1"])
-def test_non_finite_raises_exactly_when_the_oracle_panics(setup, column, flags):
-    """inf in the y of one live row's Velocity or Transform.translation.  The hasher's assertion fires only where the
-    column is checksummed with the finite flag (an inf velocity reaches the translation on the next Advance): the
-    engine raises BGR_ERR_NON_FINITE with the reference's text on exactly the vector where the oracle panics, and
-    returns the oracle's checksums on every vector before it."""
+def test_non_finite_raises_exactly_when_the_oracle_panics(setup, column, flags, pattern):
+    """A non-finite bit pattern in the y of one live row's Velocity or Transform.translation.  The hasher's assertion
+    fires only where the column is checksummed with the finite flag (a non-finite velocity reaches the translation on
+    the next Advance): the engine raises BGR_ERR_NON_FINITE with the reference's text on exactly the vector where the
+    oracle panics, and returns the oracle's checksums on every vector before it."""
     reg = MODE1 if setup == "mode1" else MODE0_SETUPS[setup]
     n = 700
     eng, orc = Engine(max_entities=n, max_depth=8, flags=flags), OracleWorld()
@@ -86,13 +91,18 @@ def test_non_finite_raises_exactly_when_the_oracle_panics(setup, column, flags):
         cols = register_particles(w, checksums=reg)
         w.build()
         tf, vel, ttl = synth_particles(n, 12, 50, 60)
-        (vel if column == "velocity" else tf)[517, 1] = np.inf
+        (vel if column == "velocity" else tf).view(np.uint32)[517, 1] = pattern
         populate(w, cols, tf, vel, ttl)
     outcomes = []
+    nan = (pattern & 0x7FFFFF) != 0
     for f in range(3):
         reqs = [Request(SAVE, f), Request(ADVANCE, 0, [0])]
         a, b = _outcome(eng, reqs), _outcome(orc, reqs)
-        assert a == b, (f, a, b)
+        if nan and f > 0 and a[0] == "ok":
+            # a NaN that went through an Advance: its payload is not specified, so neither is a checksum without the assertion
+            assert b[0] == "ok" and len(a[1]) == len(b[1]), (f, a, b)
+        else:
+            assert a == b, (f, a, b)
         k = eng.last_kernel()
         assert k.kind == ("stepwise_tma" if flags else "bundle") and (flags or k.mode == (1 if setup == "mode1" else 0))
         outcomes.append(a[0])

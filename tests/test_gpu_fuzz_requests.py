@@ -296,12 +296,14 @@ def test_wide_rows_and_long_ranges_match_the_oracle(monkeypatch, generic_kernel,
     eng.close(); orc.close()
 
 
+@pytest.mark.parametrize("pattern", [0x7F800000, 0xFF800000, 0xFFC00000, 0x7F800001], ids=hex)
 @pytest.mark.parametrize("path", ["generic", "stepwise_tma", "stepwise_flat"])
 @pytest.mark.parametrize("elem,off,ln", [(96, 4, 64), (196, 8, 188), (1024, 0, 1024), (1024, 512, 508)])
-def test_finite_assertion_covers_the_whole_long_range(monkeypatch, generic_kernel, elem, off, ln, path):
-    """A finite-checked range that ends inside the element: inf in its last word raises BGR_ERR_NON_FINITE (the oracle
-    panics), inf in the word right after it does not.  Every kernel that hashes such a range: the one-launch program
-    (interpreter; NVRTC up to 64 bytes), the TMA copy kernel and k_checksum_column."""
+def test_finite_assertion_covers_the_whole_long_range(monkeypatch, generic_kernel, elem, off, ln, path, pattern):
+    """A finite-checked range that ends inside the element: a non-finite bit pattern (+-inf, a quiet or a signalling
+    NaN) in its last word raises BGR_ERR_NON_FINITE (the oracle panics), the same pattern in the word right after it
+    does not.  Every kernel that hashes such a range: the one-launch program (interpreter; NVRTC up to 64 bytes), the
+    TMA copy kernel and k_checksum_column."""
     flags = _path_env(monkeypatch, path, generic_kernel)
     words = elem // 4
     kind = _expected_kind(path, words, 0, ln <= 64, generic_kernel)
@@ -310,7 +312,7 @@ def test_finite_assertion_covers_the_whole_long_range(monkeypatch, generic_kerne
             continue
         eng, orc = Engine(max_entities=1200, max_depth=4, flags=flags), OracleWorld()
         data = np.random.default_rng(elem + word).uniform(-9.0, 9.0, (1100, words)).astype(np.float32)
-        data[1037, word] = np.inf
+        data.view(np.uint32)[1037, word] = pattern
         res = []
         for w in (eng, orc):
             c = w.rollback_component("Wide", elem, capi.BGR_STRATEGY_COPY)
