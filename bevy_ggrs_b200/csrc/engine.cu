@@ -169,6 +169,11 @@ struct bgr_engine {
 
     std::vector<Column> cols;
     std::vector<SystemReg> systems;
+    // the registration as every kernel reads it, fixed at bgr_build (build_specs): one SysSpec per system in schedule
+    // order (and whether it can despawn), one HashSpec per checksummed column
+    std::vector<SysSpec> sys_specs;
+    std::vector<bool> sys_despawns;
+    std::vector<HashSpec> hash_specs;
     uint32_t n_ck = 0;
     bool built = false;
 
@@ -607,14 +612,10 @@ int launch_tma(bgr_engine* e, const uint8_t* src, uint8_t* dst, uint32_t n_rows_
     tp.n_rows_src = n_rows_src;
     tp.count_alive = save ? 1u : 0u;
     tp.store = store ? 1u : 0u;
-    if (save)
-        for (const Column& c : e->cols)
-            if (c.hash_kind != BGR_HASH_NONE) {
-                HashSpec& h = tp.hash[tp.n_hash++];
-                h.first_plane = c.first_plane; h.off = c.hash_off; h.len = c.hash_len;
-                h.finite = c.hash_flags & BGR_HASH_FLAG_ASSERT_FINITE_F32; h.slot = uint32_t(c.ck_slot);
-                h.absent = c.absent;
-            }
+    if (save) {
+        tp.n_hash = uint32_t(e->hash_specs.size());
+        std::copy(e->hash_specs.begin(), e->hash_specs.end(), tp.hash);
+    }
     uint32_t grid = std::max(1u, std::min(tp.n_tiles, uint32_t(e->num_sms)));
     size_t smem = size_t(tp.stages) * e->tile_bytes;
     k_image_tma<<<grid, kTmaBlock, smem, e->stream>>>(tp);
@@ -642,12 +643,10 @@ int run_stepwise(bgr_engine* e, const Program& pg, uint32_t buf) {
                 break;
             }
             bool counted = false;
-            for (const Column& c : e->cols) {
-                if (c.hash_kind == BGR_HASH_NONE) continue;
+            for (const HashSpec& h : e->hash_specs) {
                 k_checksum_column<<<e->grid_for(std::max(1u, op.n_rows), 256), 256, 0, e->stream>>>(
-                    live, e->words, c.first_plane, c.hash_off, c.hash_len,
-                    c.hash_flags & BGR_HASH_FLAG_ASSERT_FINITE_F32, op.n_rows, e->cfg.order_base, acc,
-                    uint32_t(c.ck_slot), counted ? 0u : 1u, 1u, c.absent);
+                    live, e->words, h.first_plane, h.off, h.len, h.finite, op.n_rows, e->cfg.order_base, acc,
+                    h.slot, counted ? 0u : 1u, 1u, h.absent);
                 counted = true;
                 e->launches += 1;
             }
@@ -680,52 +679,16 @@ int run_stepwise(bgr_engine* e, const Program& pg, uint32_t buf) {
         }
         case OP_ADVANCE: {
             bool any_despawn = false;
-            uint32_t counter = op.call_count;
             uint32_t n = op.n_rows;
             uint32_t grid = e->grid_for(std::max(1u, n), 256);
-            for (const SystemReg& sy : e->systems) {
-                if (n == 0) break;
-                uint32_t need = 0;  // the query matches entities that have every bound column
-                for (uint32_t c : sy.cols) need |= e->cols[c].absent;
-                switch (sy.id) {
-                case BGR_SYS_PARTICLES_UPDATE:
-                    k_sys_particles_update<<<grid, 256, 0, e->stream>>>(live, e->words, e->cols[sy.cols[0]].first_plane,
-                                                                          e->cols[sy.cols[1]].first_plane, n, op.dt_bits, need);
-                    break;
-                case BGR_SYS_PARTICLES_DESPAWN:
-                    k_sys_particles_despawn<<<grid, 256, 0, e->stream>>>(live, e->words, e->cols[sy.cols[0]].first_plane, n, e->d_kill, need);
-                    any_despawn = true;
-                    break;
-                case BGR_SYS_U32_ADD:
-                    k_sys_u32_add<<<grid, 256, 0, e->stream>>>(live, e->words, e->cols[sy.cols[0]].first_plane + sy.params[0] / 4, n, sy.params[1], need);
-                    break;
-                case BGR_SYS_U32_SATSUB_DESPAWN:
-                    k_sys_u32_satsub_despawn<<<grid, 256, 0, e->stream>>>(live, e->words, e->cols[sy.cols[0]].first_plane + sy.params[0] / 4, n, sy.params[1], e->d_kill, need);
-                    any_despawn = true;
-                    break;
-                case BGR_SYS_U32_STORE_CALL_COUNT:
-                    k_sys_u32_store<<<grid, 256, 0, e->stream>>>(live, e->words, e->cols[sy.cols[0]].first_plane + sy.params[0] / 4, n, counter++, need);
-                    break;
-                case BGR_SYS_PARTICLES_SPAWN:
-                    continue;  // Commands: applied after the schedule (below)
-                case BGR_SYS_DESPAWN_ON_INPUT: {
-                    const uint32_t player = sy.params[0], n_players = (op.flags >> 8) & 0xFu;
-                    const uint32_t input = player < n_players ? op.inputs[player] : 0u;
-                    if (input != sy.params[1]) continue;  // the run condition is host-known: no launch on other frames
-                    k_sys_despawn_having<<<grid, 256, 0, e->stream>>>(live, e->words, n, e->d_kill, need);
-                    any_despawn = true;
-                    break;
-                }
-                case BGR_SYS_BOX_MOVE: {
-                    unsigned long long packed = 0;
-                    for (int k = 0; k < 8; ++k) packed |= (unsigned long long)(op.inputs[k]) << (8 * k);
-                    k_sys_box_move<<<grid, 256, 0, e->stream>>>(live, e->words, e->cols[sy.cols[0]].first_plane, e->cols[sy.cols[1]].first_plane,
-                                                                 n, op.dt_bits, op.fr_bits, packed, (op.flags >> 8) & 0xFu, e->cfg.order_base, need);
-                    break;
-                }
-                default: return fail(BGR_ERR_UNSUPPORTED, "system has no GPU implementation yet");
-                }
+            for (size_t s = 0; s < e->sys_specs.size() && n > 0; ++s) {
+                const SysSpec& sy = e->sys_specs[s];
+                if (sy.id == BGR_SYS_PARTICLES_SPAWN) continue;  // Commands: applied after the schedule (below)
+                // despawn_on_input's run condition is host-known: no launch on frames whose input does not match
+                if (sy.id == BGR_SYS_DESPAWN_ON_INPUT && player_input(op, sy.param & 0xFFu) != (sy.param >> 8)) continue;
+                k_sys_rows<<<grid, 256, 0, e->stream>>>(live, e->words, n, sy, op, e->cfg.order_base, e->d_kill);
                 e->launches += 1;
+                any_despawn = any_despawn || e->sys_despawns[s];
             }
             if (any_despawn) {
                 k_apply_despawns<<<grid, 256, 0, e->stream>>>(live, e->words, n, e->d_kill);
@@ -753,34 +716,50 @@ int run_stepwise(bgr_engine* e, const Program& pg, uint32_t buf) {
 }
 
 
-// the registration as the generic program's spec tables (parameter block of the interpreter, prelude of the JIT kernel)
-void fill_generic_specs(const bgr_engine* e, GenericParams& gp) {
-    gp.n_hash = 0;
-    gp.n_sys = 0;
+// The registration as the kernels read it (bgr_engine::sys_specs / sys_despawns / hash_specs); called by bgr_build.  The
+// interpreter's parameter block, the generated kernel's prelude, the TMA Save and the stepwise path all use these tables.
+void build_specs(bgr_engine* e) {
+    e->hash_specs.clear();
+    e->sys_specs.clear();
+    e->sys_despawns.clear();
     for (const Column& c : e->cols)
         if (c.hash_kind != BGR_HASH_NONE) {
-            HashSpec& h = gp.hash[gp.n_hash++];
+            HashSpec h{};
             h.first_plane = c.first_plane; h.off = c.hash_off; h.len = c.hash_len;
             h.finite = c.hash_flags & BGR_HASH_FLAG_ASSERT_FINITE_F32; h.slot = uint32_t(c.ck_slot);
             h.absent = c.absent;
+            e->hash_specs.push_back(h);
         }
     uint32_t counter_index = 0;
     for (const SystemReg& sy : e->systems) {
-        SysSpec& sp = gp.sys[gp.n_sys++];
+        SysSpec sp{};
         sp.id = sy.id;
-        for (uint32_t c : sy.cols) sp.need |= e->cols[c].absent;
+        for (uint32_t c : sy.cols) sp.need |= e->cols[c].absent;  // the query matches entities that have every bound column
         sp.plane0 = e->cols[sy.cols[0]].first_plane;
+        bool despawns = false;
         switch (sy.id) {
-        case BGR_SYS_U32_ADD:
-        case BGR_SYS_U32_SATSUB_DESPAWN: sp.plane0 += sy.params[0] / 4; sp.param = sy.params[1]; break;
+        case BGR_SYS_U32_ADD: sp.plane0 += sy.params[0] / 4; sp.param = sy.params[1]; break;
+        case BGR_SYS_U32_SATSUB_DESPAWN: sp.plane0 += sy.params[0] / 4; sp.param = sy.params[1]; despawns = true; break;
         case BGR_SYS_U32_STORE_CALL_COUNT: sp.plane0 += sy.params[0] / 4; sp.param = counter_index++; break;
-        case BGR_SYS_DESPAWN_ON_INPUT: sp.param = sy.params[0] | (sy.params[1] << 8); break;
+        case BGR_SYS_DESPAWN_ON_INPUT: sp.param = sy.params[0] | (sy.params[1] << 8); despawns = true; break;
+        case BGR_SYS_PARTICLES_DESPAWN: despawns = true; break;
         case BGR_SYS_PARTICLES_UPDATE:
         case BGR_SYS_BOX_MOVE: sp.plane1 = e->cols[sy.cols[1]].first_plane; break;
         default: break;
         }
+        e->sys_specs.push_back(sp);
+        e->sys_despawns.push_back(despawns);
     }
 }
+
+// the system ids the generated kernel's sources switch on: NVRTC cannot parse the public header, the prelude defines them
+#define BGR_SYS_ID(name) {#name, name}
+constexpr std::pair<const char*, uint32_t> kSystemIds[] = {
+    BGR_SYS_ID(BGR_SYS_PARTICLES_UPDATE), BGR_SYS_ID(BGR_SYS_PARTICLES_DESPAWN), BGR_SYS_ID(BGR_SYS_BOX_MOVE),
+    BGR_SYS_ID(BGR_SYS_U32_ADD), BGR_SYS_ID(BGR_SYS_U32_SATSUB_DESPAWN), BGR_SYS_ID(BGR_SYS_U32_STORE_CALL_COUNT),
+    BGR_SYS_ID(BGR_SYS_PARTICLES_SPAWN), BGR_SYS_ID(BGR_SYS_DESPAWN_ON_INPUT),
+};
+#undef BGR_SYS_ID
 
 // NVRTC specialisation of the generic program for this registration (jit.hpp, generic_program_jit.cuh); called by bgr_build
 void jit_specialise(bgr_engine* e) {
@@ -789,37 +768,27 @@ void jit_specialise(bgr_engine* e) {
     if (!e->generic_ok || !e->tune_generic || e->tune_jit == 0 || (e->cfg.flags & BGR_CFG_FORCE_STEPWISE)) return;
     if (e->bundle_particles && e->tune_bundle) return;  // the bundle has its own kernel
     if (e->tune_jit == 1 && e->cfg.max_entities < 16384) return;  // small worlds: a tick is launch latency, not worth a compile
-    GenericParams gp;
-    std::memset(&gp, 0, sizeof gp);
-    fill_generic_specs(e, gp);
     if (e->words < 1 || e->words > 24) return;  // the row has to fit the register file
-    for (uint32_t c = 0; c < gp.n_hash; ++c)   // whole-word byte ranges only (every POD of u32 / f32 / u64 fields)
-        if (((gp.hash[c].off | gp.hash[c].len) & 3u) != 0u || gp.hash[c].len < 4 || gp.hash[c].len > 64) return;
+    for (const HashSpec& h : e->hash_specs)     // whole-word byte ranges only (every POD of u32 / f32 / u64 fields)
+        if (((h.off | h.len) & 3u) != 0u || h.len < 4 || h.len > 64) return;
     const int rows = e->tune_jit_rows == 1 || e->tune_jit_rows == 2 ? e->tune_jit_rows : 4;
     auto compile = [&](int item_rows, int rows, JitKernel* out) {
         const int threads = item_rows / rows;
         std::string pre;
         auto def = [&](const char* name, unsigned long long v) { pre += "#define " + std::string(name) + " " + std::to_string(v) + "\n"; };
-        def("BGR_SYS_PARTICLES_UPDATE", BGR_SYS_PARTICLES_UPDATE); def("BGR_SYS_PARTICLES_DESPAWN", BGR_SYS_PARTICLES_DESPAWN);
-        def("BGR_SYS_BOX_MOVE", BGR_SYS_BOX_MOVE); def("BGR_SYS_U32_ADD", BGR_SYS_U32_ADD);
-        def("BGR_SYS_U32_SATSUB_DESPAWN", BGR_SYS_U32_SATSUB_DESPAWN); def("BGR_SYS_U32_STORE_CALL_COUNT", BGR_SYS_U32_STORE_CALL_COUNT);
-        def("BGR_SYS_PARTICLES_SPAWN", BGR_SYS_PARTICLES_SPAWN); def("BGR_SYS_DESPAWN_ON_INPUT", BGR_SYS_DESPAWN_ON_INPUT);
+        for (const auto& id : kSystemIds) def(id.first, id.second);
         def("BGR_TILE_ROWS", kTileRows);
         def("BGR_JIT_WORDS", e->words); def("BGR_JIT_ROWS", rows); def("BGR_JIT_ITEM_ROWS", item_rows);
         // resident blocks the register allocation has to allow: ~512 threads per SM for narrow rows, ~256 for wide ones
         def("BGR_JIT_MINB", std::max(1, (e->words <= 8 ? 512 : 256) / threads));
-        def("BGR_JIT_NSYS", gp.n_sys); def("BGR_JIT_NHASH", gp.n_hash);
+        def("BGR_JIT_NSYS", e->sys_specs.size()); def("BGR_JIT_NHASH", e->hash_specs.size());
         auto u = [](uint32_t v) { return std::to_string(v) + "u"; };
         pre += "#define BGR_JIT_SYS_LIST ";
-        for (uint32_t i = 0; i < gp.n_sys; ++i) {
-            const SysSpec& y = gp.sys[i];
+        for (const SysSpec& y : e->sys_specs)
             pre += "{" + u(y.id) + "," + u(y.plane0) + "," + u(y.plane1) + "," + u(y.need) + "," + u(y.param) + "}, ";
-        }
         pre += "{0u,0u,0u,0u,0u}\n#define BGR_JIT_HASH_LIST ";
-        for (uint32_t i = 0; i < gp.n_hash; ++i) {
-            const HashSpec& h = gp.hash[i];
+        for (const HashSpec& h : e->hash_specs)
             pre += "{" + u(h.first_plane) + "," + u(h.off) + "," + u(h.len) + "," + u(h.finite) + "," + u(h.slot) + "," + u(h.absent) + "}, ";
-        }
         pre += "{0u,0u,0u,0u,0u,0u}\n";
         std::string why;
         if (!jit_generic_program(pre, threads, reinterpret_cast<const void*>(&bgr_abi_version), out, &why) && std::getenv("BGR_JIT_VERBOSE"))
@@ -853,7 +822,10 @@ int run_generic(bgr_engine* e, const Program& pg, uint32_t buf) {
     gp.live_rows = pg.live_rows;
     if (!pg.first_is_load) gp.flags |= PF_READ_LIVE;
     if ((pg.has_load || pg.has_advance) && !pg.defer_live) gp.flags |= PF_WRITE_LIVE_ACTIVE;
-    fill_generic_specs(e, gp);
+    gp.n_hash = uint32_t(e->hash_specs.size());
+    gp.n_sys = uint32_t(e->sys_specs.size());  // <= kMaxGenericSys: generic_ok
+    std::copy(e->hash_specs.begin(), e->hash_specs.end(), gp.hash);
+    std::copy(e->sys_specs.begin(), e->sys_specs.end(), gp.sys);
     std::memcpy(gp.ops, pg.ops, sizeof(Op) * pg.n_ops);
     if (e->jit.fn) {  // the registration's own register-resident kernel
         // few tiles per SM: with whole tiles some SMs carry twice the rows of others and set the kernel's duration
@@ -1603,15 +1575,11 @@ BGR_API int bgr_build(bgr_engine* e) {
             CUDA_TRY(cudaHostAlloc(&e->h_spawn[i], sizeof(float2) * kMaxSpawnVals, cudaHostAllocMapped));
             CUDA_TRY(cudaHostGetDevicePointer(&e->d_spawn[i], e->h_spawn[i], 0));
         }
+    build_specs(e);
     detect_bundles(e);
-    {   // generic one-launch program: every registered system has a shared-memory implementation, the tile fits twice per SM
-        bool ok = e->systems.size() <= size_t(kMaxGenericSys) && e->tile_bytes <= 100u * 1024u;  // at least two blocks per SM
-        for (const SystemReg& sy : e->systems)
-            ok = ok && (sy.id == BGR_SYS_U32_ADD || sy.id == BGR_SYS_U32_SATSUB_DESPAWN || sy.id == BGR_SYS_U32_STORE_CALL_COUNT ||
-                        sy.id == BGR_SYS_PARTICLES_UPDATE || sy.id == BGR_SYS_PARTICLES_DESPAWN || sy.id == BGR_SYS_BOX_MOVE ||
-                        sy.id == BGR_SYS_DESPAWN_ON_INPUT);
-        e->generic_ok = ok;
-    }
+    // generic one-launch program: every row system runs on its tile (run_system); spawning is a Command of the stepwise
+    // path; the parameter block holds kMaxGenericSys systems; the tile fits twice per SM
+    e->generic_ok = e->spawn_sys < 0 && e->sys_specs.size() <= size_t(kMaxGenericSys) && e->tile_bytes <= 100u * 1024u;
     jit_specialise(e);
     if (e->jit.fn && e->tune_jit_tiledep) {
         const size_t ni = size_t(e->tiles_for(e->cfg.max_entities)) * 4 + 4;

@@ -24,9 +24,6 @@
 #include <cstdint>
 #endif
 
-#ifndef __CUDACC_RTC__
-#include "../../include/bevy_ggrs_b200.h"
-#endif  // NVRTC: the engine's generated prelude defines the BGR_SYS_* ids (host function declarations cannot be parsed there)
 #include "kernels.cuh"
 #include "seahash.cuh"
 #include "tma_copy.cuh"
@@ -39,14 +36,6 @@ constexpr int kMaxGenericSys = 8;
 // schema from its parameter block.  bgr_build also compiles the registration's own kernel with NVRTC when it can
 // (generic_program_jit.cuh, jit.hpp), and this one is then only the fallback.
 constexpr int kGenericBlock = 128;
-
-struct SysSpec {
-    uint32_t id;      // bgr_system
-    uint32_t plane0;  // first word plane the system touches (column's first plane + byte_offset / 4)
-    uint32_t plane1;  // second bound column's first plane (Velocity for the Transform/Velocity systems)
-    uint32_t need;    // absent bits of the bound columns: the query matches a row iff row_matches(mask, need)
-    uint32_t param;   // k (U32_ADD / U32_SATSUB_DESPAWN) or the system's index among the call-count systems
-};
 
 struct GenericParams {
     uint8_t* arena;
@@ -204,89 +193,16 @@ __global__ void __launch_bounds__(kGenericBlock) k_generic_program(const __grid_
             const Op& op = p.ops[i];
             if (op.kind == OP_ADVANCE) {
                 before_write();
-                const float dt = __uint_as_float(op.dt_bits);
-                // systems outside, the thread's rows inside: a system's spec is decoded once for all of them.  A row still
-                // sees the schedule's systems in order, every system sees the entity's presence as it was before the frame,
-                // and despawn commands are applied after the last system.
+                // systems outside, the thread's rows inside (run_system): a system's spec is decoded once for all of them
                 uint32_t m[kRows];
                 bool kill[kRows];
 #pragma unroll
                 for (int k = 0; k < kRows; ++k) { m[k] = s_alive[tid + k * kGenericBlock]; kill[k] = false; }
+                auto word = [&](int k, uint32_t plane) -> uint32_t& { return tile_w[plane * uint32_t(kTileRows) + tid + k * kGenericBlock]; };
 #pragma unroll 1
                 for (uint32_t s = 0; s < p.n_sys; ++s) {
                     const SysSpec sy = p.sys[s];
-                    uint32_t* w0 = tile_w + sy.plane0 * uint32_t(kTileRows) + tid;
-                    switch (sy.id) {
-                    case BGR_SYS_U32_ADD:
-#pragma unroll
-                        for (int k = 0; k < kRows; ++k)
-                            if (row_matches(m[k], sy.need)) w0[k * kGenericBlock] += sy.param;
-                        break;
-                    case BGR_SYS_U32_SATSUB_DESPAWN:
-#pragma unroll
-                        for (int k = 0; k < kRows; ++k)
-                            if (row_matches(m[k], sy.need)) {
-                                uint32_t v = w0[k * kGenericBlock];
-                                v = v > sy.param ? v - sy.param : 0u;
-                                w0[k * kGenericBlock] = v;
-                                kill[k] = kill[k] || v == 0u;
-                            }
-                        break;
-                    case BGR_SYS_U32_STORE_CALL_COUNT:
-#pragma unroll
-                        for (int k = 0; k < kRows; ++k)
-                            if (row_matches(m[k], sy.need)) w0[k * kGenericBlock] = op.call_count + sy.param;
-                        break;
-                    case BGR_SYS_DESPAWN_ON_INPUT: {  // param = player handle | value << 8
-                        const uint32_t player = sy.param & 0xFFu, n_players = (op.flags >> 8) & 0xFu;
-                        const uint32_t input = player < n_players && player < 8 ? op.inputs[player] : 0u;
-                        const bool hit = input == (sy.param >> 8);
-#pragma unroll
-                        for (int k = 0; k < kRows; ++k) kill[k] = kill[k] || (hit && row_matches(m[k], sy.need));
-                        break;
-                    }
-                    case BGR_SYS_PARTICLES_UPDATE: {
-                        uint32_t* v0 = tile_w + sy.plane1 * uint32_t(kTileRows) + tid;
-#pragma unroll
-                        for (int k = 0; k < kRows; ++k)
-                            if (row_matches(m[k], sy.need)) {
-                                uint32_t* t = w0 + k * kGenericBlock;
-                                uint32_t* v = v0 + k * kGenericBlock;
-                                uint32_t tx = t[0], ty = t[kTileRows], tz = t[2 * kTileRows], vx = v[0], vy = v[kTileRows], vz = v[2 * kTileRows];
-                                particle_step(tx, ty, tz, vx, vy, vz, dt);
-                                t[0] = tx; t[kTileRows] = ty; t[2 * kTileRows] = tz; v[0] = vx; v[kTileRows] = vy; v[2 * kTileRows] = vz;
-                            }
-                        break;
-                    }
-                    case BGR_SYS_PARTICLES_DESPAWN:
-#pragma unroll
-                        for (int k = 0; k < kRows; ++k)
-                            if (row_matches(m[k], sy.need)) {
-                                uint32_t* t = w0 + k * kGenericBlock;
-                                uint64_t ttl = (uint64_t(t[kTileRows]) << 32) | t[0];
-                                ttl -= 1;
-                                t[0] = uint32_t(ttl); t[kTileRows] = uint32_t(ttl >> 32);
-                                kill[k] = kill[k] || ttl == 0;
-                            }
-                        break;
-                    case BGR_SYS_BOX_MOVE: {
-                        uint32_t* v0 = tile_w + sy.plane1 * uint32_t(kTileRows) + tid;
-                        const uint32_t n_players = (op.flags >> 8) & 0xFu;
-#pragma unroll
-                        for (int k = 0; k < kRows; ++k)
-                            if (row_matches(m[k], sy.need)) {
-                                float* t = reinterpret_cast<float*>(w0 + k * kGenericBlock);
-                                float* v = reinterpret_cast<float*>(v0 + k * kGenericBlock);
-                                float tx = t[0], ty = t[kTileRows], tz = t[2 * kTileRows], vx = v[0], vy = v[kTileRows], vz = v[2 * kTileRows];
-                                const unsigned long long handle = row0 + uint32_t(k * kGenericBlock);
-                                const uint32_t input = handle < n_players && handle < 8 ? op.inputs[handle] : 0u;
-                                box_move_step(tx, ty, tz, vx, vy, vz, dt, __uint_as_float(op.fr_bits), input);
-                                t[0] = tx; t[kTileRows] = ty; t[2 * kTileRows] = tz; v[0] = vx; v[kTileRows] = vy; v[2 * kTileRows] = vz;
-                            }
-                        break;
-                    }
-                    default: break;
-                    }
+                    run_system<kRows>(sy, word, m, kill, op, row0, kGenericBlock);
                 }
 #pragma unroll
                 for (int k = 0; k < kRows; ++k)

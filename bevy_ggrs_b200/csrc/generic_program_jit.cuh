@@ -55,54 +55,13 @@ struct JitRows {
     bool kill[kJitRows];
 };
 
-// the S-th registered system on the register copy; every system sees the entity's presence as it was before the frame
+// the S-th registered system on the register copy (run_system with a constexpr spec: plain register ops)
 template <int S>
-__device__ __forceinline__ void jit_run_systems(JitRows& r, const Op& op, float dt, unsigned long long row0, int B) {
+__device__ __forceinline__ void jit_run_systems(JitRows& r, const Op& op, unsigned long long row0, int B) {
     if constexpr (S < kJitNSys) {
         constexpr SysSpec sy = kJitSys[S];
-#pragma unroll
-        for (int k = 0; k < kJitRows; ++k) {
-            const bool on = row_matches(r.m[k], sy.need);
-            if constexpr (sy.id == BGR_SYS_U32_ADD) {
-                r.w[k][sy.plane0] += on ? sy.param : 0u;
-            } else if constexpr (sy.id == BGR_SYS_U32_SATSUB_DESPAWN) {
-                uint32_t v = r.w[k][sy.plane0];
-                v = v > sy.param ? v - sy.param : 0u;
-                r.w[k][sy.plane0] = on ? v : r.w[k][sy.plane0];
-                r.kill[k] = r.kill[k] || (on && v == 0u);
-            } else if constexpr (sy.id == BGR_SYS_U32_STORE_CALL_COUNT) {
-                r.w[k][sy.plane0] = on ? op.call_count + sy.param : r.w[k][sy.plane0];
-            } else if constexpr (sy.id == BGR_SYS_DESPAWN_ON_INPUT) {  // param = player handle | value << 8
-                const uint32_t player = sy.param & 0xFFu, n_players = (op.flags >> 8) & 0xFu;
-                const uint32_t input = player < n_players && player < 8 ? op.inputs[player] : 0u;
-                r.kill[k] = r.kill[k] || (on && input == (sy.param >> 8));
-            } else if constexpr (sy.id == BGR_SYS_PARTICLES_UPDATE) {
-                uint32_t tx = r.w[k][sy.plane0], ty = r.w[k][sy.plane0 + 1], tz = r.w[k][sy.plane0 + 2];
-                uint32_t vx = r.w[k][sy.plane1], vy = r.w[k][sy.plane1 + 1], vz = r.w[k][sy.plane1 + 2];
-                particle_step(tx, ty, tz, vx, vy, vz, dt);
-                if (on) {
-                    r.w[k][sy.plane0] = tx; r.w[k][sy.plane0 + 1] = ty; r.w[k][sy.plane0 + 2] = tz;
-                    r.w[k][sy.plane1] = vx; r.w[k][sy.plane1 + 1] = vy; r.w[k][sy.plane1 + 2] = vz;
-                }
-            } else if constexpr (sy.id == BGR_SYS_PARTICLES_DESPAWN) {
-                uint64_t ttl = (uint64_t(r.w[k][sy.plane0 + 1]) << 32) | r.w[k][sy.plane0];
-                ttl -= 1;
-                if (on) { r.w[k][sy.plane0] = uint32_t(ttl); r.w[k][sy.plane0 + 1] = uint32_t(ttl >> 32); }
-                r.kill[k] = r.kill[k] || (on && ttl == 0);
-            } else if constexpr (sy.id == BGR_SYS_BOX_MOVE) {
-                if (on) {  // two to four entities: a branch costs nothing and keeps the step off the other rows
-                    float tx = __uint_as_float(r.w[k][sy.plane0]), ty = __uint_as_float(r.w[k][sy.plane0 + 1]), tz = __uint_as_float(r.w[k][sy.plane0 + 2]);
-                    float vx = __uint_as_float(r.w[k][sy.plane1]), vy = __uint_as_float(r.w[k][sy.plane1 + 1]), vz = __uint_as_float(r.w[k][sy.plane1 + 2]);
-                    const unsigned long long handle = row0 + uint32_t(k * B);
-                    const uint32_t n_players = (op.flags >> 8) & 0xFu;
-                    const uint32_t input = handle < n_players && handle < 8 ? op.inputs[handle] : 0u;
-                    box_move_step(tx, ty, tz, vx, vy, vz, dt, __uint_as_float(op.fr_bits), input);
-                    r.w[k][sy.plane0] = __float_as_uint(tx); r.w[k][sy.plane0 + 1] = __float_as_uint(ty); r.w[k][sy.plane0 + 2] = __float_as_uint(tz);
-                    r.w[k][sy.plane1] = __float_as_uint(vx); r.w[k][sy.plane1 + 1] = __float_as_uint(vy); r.w[k][sy.plane1 + 2] = __float_as_uint(vz);
-                }
-            }
-        }
-        jit_run_systems<S + 1>(r, op, dt, row0, B);
+        run_system<kJitRows>(sy, [&](int k, uint32_t plane) -> uint32_t& { return r.w[k][plane]; }, r.m, r.kill, op, row0, uint32_t(B));
+        jit_run_systems<S + 1>(r, op, row0, B);
     }
 }
 
@@ -202,7 +161,7 @@ extern "C" __global__ void __launch_bounds__(BGR_JIT_ITEM_ROWS / BGR_JIT_ROWS, B
             if (op.kind == OP_ADVANCE) {
 #pragma unroll
                 for (int k = 0; k < kJitRows; ++k) r.kill[k] = false;
-                jit_run_systems<0>(r, op, __uint_as_float(op.dt_bits), row0, B);
+                jit_run_systems<0>(r, op, row0, B);
 #pragma unroll
                 for (int k = 0; k < kJitRows; ++k) r.m[k] = r.kill[k] ? 0u : r.m[k];  // despawn commands: after the last system
             } else if (op.kind == OP_SAVE) {

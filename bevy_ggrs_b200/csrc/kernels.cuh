@@ -30,6 +30,9 @@
 #include <cstdint>
 #endif
 
+#ifndef __CUDACC_RTC__
+#include "../../include/bevy_ggrs_b200.h"
+#endif  // NVRTC: the engine's generated prelude defines the BGR_SYS_* ids (host function declarations cannot be parsed there)
 #include "seahash.cuh"
 
 namespace bgr {
@@ -92,6 +95,16 @@ struct Op {
     uint8_t inputs[8];      // ADVANCE: PlayerInputs<T>.0[handle].0 for every handle (u8, BGR_MAX_PLAYERS)
 };
 static_assert(sizeof(Op) == 40, "Op layout");
+
+// One registered GgrsSchedule system as the kernels run it (run_system), fixed at bgr_build
+struct SysSpec {
+    uint32_t id;      // bgr_system
+    uint32_t plane0;  // first word plane the system touches (column's first plane + byte_offset / 4)
+    uint32_t plane1;  // second bound column's first plane (Velocity for the Transform/Velocity systems)
+    uint32_t need;    // absent bits of the bound columns: the query matches a row iff row_matches(mask, need)
+    uint32_t param;   // k (U32_ADD / U32_SATSUB_DESPAWN), the system's index among the call-count systems, or
+                      // player handle | value << 8 (DESPAWN_ON_INPUT)
+};
 
 enum ProgFlags : uint32_t {
     PF_READ_LIVE = 1u,           // program does not start with LOAD: initial state comes from image 0
@@ -250,6 +263,128 @@ __device__ __forceinline__ void particle_step(uint32_t& tx, uint32_t& ty, uint32
     float ftz = __fadd_rn(__uint_as_float(tz), __fmul_rn(fvz, dt));
     vx = __float_as_uint(fvx); vy = __float_as_uint(fvy); vz = __float_as_uint(fvz);
     tx = __float_as_uint(ftx); ty = __float_as_uint(fty); tz = __float_as_uint(ftz);
+}
+
+// move_cube_system (box_game.rs:154-206), BASELINE config C1.  player handle == RollbackOrdered index.
+// `fr` is `FRICTION.powf(dt)` (FRICTION = 0.0018), evaluated once per Advance by the host with the C library's powf,
+// the function the reference calls (Op::fr_bits).  A device powf is only good to about one ulp and rounds some frame
+// rates' factor the other way, so every result here is bit-exact with the CPU only because the factor comes from the host.
+__device__ __forceinline__ void box_move_step(float& tx, float& ty, float& tz, float& vx, float& vy, float& vz, float dt, float fr,
+                                              uint32_t input) {
+    const float ACCELERATION = 18.0f, MAX_SPEED = 3.0f, PLANE_SIZE = 5.0f, CUBE_SIZE = 0.2f;
+    const bool up = input & 1u, down = input & 2u, left = input & 4u, right = input & 8u;
+    const float a = __fmul_rn(ACCELERATION, dt);
+    if (up && !down) vz = __fsub_rn(vz, a);
+    if (!up && down) vz = __fadd_rn(vz, a);
+    if (left && !right) vx = __fsub_rn(vx, a);
+    if (!left && right) vx = __fadd_rn(vx, a);
+    if (!up && !down) vz = __fmul_rn(vz, fr);
+    if (!left && !right) vx = __fmul_rn(vx, fr);
+    vy = __fmul_rn(vy, fr);
+    // glam Vec3::clamp_length_max(MAX_SPEED)
+    const float len_sq = __fadd_rn(__fadd_rn(__fmul_rn(vx, vx), __fmul_rn(vy, vy)), __fmul_rn(vz, vz));
+    if (len_sq > __fmul_rn(MAX_SPEED, MAX_SPEED)) {
+        const float l = __fsqrt_rn(len_sq);
+        vx = __fmul_rn(MAX_SPEED, __fdiv_rn(vx, l)); vy = __fmul_rn(MAX_SPEED, __fdiv_rn(vy, l)); vz = __fmul_rn(MAX_SPEED, __fdiv_rn(vz, l));
+    }
+    tx = __fadd_rn(tx, __fmul_rn(vx, dt)); ty = __fadd_rn(ty, __fmul_rn(vy, dt)); tz = __fadd_rn(tz, __fmul_rn(vz, dt));
+    const float hw = __fmul_rn(__fsub_rn(PLANE_SIZE, CUBE_SIZE), 0.5f);
+    tx = tx < -hw ? -hw : (tx > hw ? hw : tx);
+    tz = tz < -hw ? -hw : (tz > hw ? hw : tz);
+}
+
+// PlayerInputs<T>.0[handle].0; 0 for a handle the frame has no input for.  (A u32 player handle is compared in 32 bits,
+// a u64 RollbackOrdered index in 64.)
+template <class Handle>
+__host__ __device__ __forceinline__ uint32_t player_input(const Op& op, Handle handle) {
+    const uint32_t n_players = (op.flags >> 8) & 0xFu;
+    return handle < n_players && handle < 8 ? op.inputs[handle] : 0u;
+}
+
+// =============================================================================================
+// THE per-row definition of every compiled GgrsSchedule system (include/bevy_ggrs_b200.h): one registered system
+// applied to the R rows a thread owns.  The interpreter (k_generic_program) runs it on its shared-memory tile, the
+// generated kernel (k_generic_jit) on its register copy with a constexpr spec (the switch folds away), the stepwise
+// path (k_sys_rows) on the live image with R = 1.
+//   word(k, plane) : reference to row k's word in `plane`
+//   m[k]           : row k's mask byte as it was before the frame (every system of a frame sees the same presence)
+//   kill[k]        : set when the system despawns row k; the caller applies it after the schedule's last system
+//                    (Commands are deferred to the end of GgrsSchedule)
+//   row0, row_step : row k's RollbackOrdered index is row0 + k * row_step
+// The switch sits outside the row loop (a system's spec is decoded once for all rows) and a word is written only on
+// rows the query matches.
+// =============================================================================================
+template <int R, class Word>
+__device__ __forceinline__ void run_system(const SysSpec& sy, Word&& word, const uint32_t (&m)[R], bool (&kill)[R], const Op& op,
+                                           unsigned long long row0, uint32_t row_step) {
+    const float dt = __uint_as_float(op.dt_bits);
+    switch (sy.id) {
+    case BGR_SYS_U32_ADD:  // x.0 += k   (tests/component_rollback.rs:25-29)
+#pragma unroll
+        for (int k = 0; k < R; ++k)
+            if (row_matches(m[k], sy.need)) word(k, sy.plane0) += sy.param;
+        break;
+    case BGR_SYS_U32_SATSUB_DESPAWN:  // h = h.saturating_sub(k); despawn at 0   (tests/synctest.rs:38-45)
+#pragma unroll
+        for (int k = 0; k < R; ++k) {
+            const bool on = row_matches(m[k], sy.need);
+            uint32_t v = word(k, sy.plane0);
+            v = v > sy.param ? v - sy.param : 0u;
+            if (on) word(k, sy.plane0) = v;
+            kill[k] = kill[k] || (on && v == 0u);
+        }
+        break;
+    case BGR_SYS_U32_STORE_CALL_COUNT:  // c.0 = count  (the deliberately non-deterministic system of tests/synctest.rs:92-97)
+#pragma unroll
+        for (int k = 0; k < R; ++k)
+            if (row_matches(m[k], sy.need)) word(k, sy.plane0) = op.call_count + sy.param;
+        break;
+    case BGR_SYS_DESPAWN_ON_INPUT: {  // commands.entity(e).despawn() for every entity that has the bound component (tests/hierarchy.rs:36-45)
+#pragma unroll
+        for (int k = 0; k < R; ++k) {
+            const bool on = row_matches(m[k], sy.need);
+            const uint32_t input = player_input(op, sy.param & 0xFFu);
+            kill[k] = kill[k] || (on && input == (sy.param >> 8));
+        }
+        break;
+    }
+    case BGR_SYS_PARTICLES_UPDATE:  // update_particles (particles.rs:272-280)
+#pragma unroll
+        for (int k = 0; k < R; ++k) {
+            const bool on = row_matches(m[k], sy.need);
+            uint32_t tx = word(k, sy.plane0), ty = word(k, sy.plane0 + 1), tz = word(k, sy.plane0 + 2);
+            uint32_t vx = word(k, sy.plane1), vy = word(k, sy.plane1 + 1), vz = word(k, sy.plane1 + 2);
+            particle_step(tx, ty, tz, vx, vy, vz, dt);
+            if (on) {
+                word(k, sy.plane0) = tx; word(k, sy.plane0 + 1) = ty; word(k, sy.plane0 + 2) = tz;
+                word(k, sy.plane1) = vx; word(k, sy.plane1 + 1) = vy; word(k, sy.plane1 + 2) = vz;
+            }
+        }
+        break;
+    case BGR_SYS_PARTICLES_DESPAWN:  // despawn_particles (particles.rs:282-289): ttl -= 1 (wrapping usize); despawn at 0
+#pragma unroll
+        for (int k = 0; k < R; ++k) {
+            const bool on = row_matches(m[k], sy.need);
+            uint64_t ttl = (uint64_t(word(k, sy.plane0 + 1)) << 32) | word(k, sy.plane0);
+            ttl -= 1;
+            if (on) { word(k, sy.plane0) = uint32_t(ttl); word(k, sy.plane0 + 1) = uint32_t(ttl >> 32); }
+            kill[k] = kill[k] || (on && ttl == 0);
+        }
+        break;
+    case BGR_SYS_BOX_MOVE:  // move_cube_system (box_game.rs:154-206)
+#pragma unroll
+        for (int k = 0; k < R; ++k)
+            if (row_matches(m[k], sy.need)) {  // two to four entities: a branch costs nothing and keeps the step off the other rows
+                float tx = __uint_as_float(word(k, sy.plane0)), ty = __uint_as_float(word(k, sy.plane0 + 1)), tz = __uint_as_float(word(k, sy.plane0 + 2));
+                float vx = __uint_as_float(word(k, sy.plane1)), vy = __uint_as_float(word(k, sy.plane1 + 1)), vz = __uint_as_float(word(k, sy.plane1 + 2));
+                const uint32_t input = player_input(op, row0 + uint32_t(k) * row_step);
+                box_move_step(tx, ty, tz, vx, vy, vz, dt, __uint_as_float(op.fr_bits), input);
+                word(k, sy.plane0) = __float_as_uint(tx); word(k, sy.plane0 + 1) = __float_as_uint(ty); word(k, sy.plane0 + 2) = __float_as_uint(tz);
+                word(k, sy.plane1) = __float_as_uint(vx); word(k, sy.plane1 + 1) = __float_as_uint(vy); word(k, sy.plane1 + 2) = __float_as_uint(vz);
+            }
+        break;
+    default: break;
+    }
 }
 
 // =============================================================================================
@@ -804,63 +939,22 @@ __global__ void __launch_bounds__(256) k_spawn_rows(uint8_t* img, uint32_t words
 __global__ void k_set_alive(uint8_t* img, uint32_t words, uint32_t row, uint8_t value) { img[alive_offset(words, row)] = value; }
 
 // ---- GgrsSchedule systems on the live image (stepwise path) ----
-__global__ void __launch_bounds__(256) k_sys_particles_update(uint8_t* img, uint32_t words, uint32_t t_plane,
-                                                              uint32_t v_plane, uint32_t n_rows, uint32_t dt_bits, uint32_t need) {
-    const float dt = __uint_as_float(dt_bits);
+// One registered system (run_system) over rows [0, n_rows), one row per thread.  `kill` receives the despawns;
+// k_apply_despawns applies them after every system of the schedule has run (Commands are deferred to the end of GgrsSchedule).
+// Eight resident blocks per SM (at most 32 registers): the grid (engine grid_for, 8 blocks per SM) is then one wave, as it
+// was with one small kernel per system.  Left to itself the union of all systems takes 37 registers, six blocks per SM,
+// and a 1M-entity stepwise tick was 8 % slower (H100 80GB HBM3, 400 W power limit).
+__global__ void __launch_bounds__(256, 8) k_sys_rows(uint8_t* img, uint32_t words, uint32_t n_rows, const SysSpec sy,
+                                                  const __grid_constant__ Op op,
+                                                  unsigned long long order_base, uint8_t* kill) {
     for (uint32_t r = blockIdx.x * blockDim.x + threadIdx.x; r < n_rows; r += gridDim.x * blockDim.x) {
-        if (!row_matches(img[alive_offset(words, r)], need)) continue;
-        uint32_t* t = reinterpret_cast<uint32_t*>(img + word_offset(words, r, t_plane));
-        uint32_t* v = reinterpret_cast<uint32_t*>(img + word_offset(words, r, v_plane));
-        uint32_t tx = t[0], ty = t[kTileRows], tz = t[2 * kTileRows], vx = v[0], vy = v[kTileRows], vz = v[2 * kTileRows];
-        particle_step(tx, ty, tz, vx, vy, vz, dt);
-        t[0] = tx; t[kTileRows] = ty; t[2 * kTileRows] = tz; v[0] = vx; v[kTileRows] = vy; v[2 * kTileRows] = vz;
+        const uint32_t m[1] = {img[alive_offset(words, r)]};
+        if (!row_matches(m[0], sy.need)) continue;  // no system touches a row its query does not match: read none of its words
+        bool despawn[1] = {false};
+        run_system<1>(sy, [&](int, uint32_t plane) -> uint32_t& { return *reinterpret_cast<uint32_t*>(img + word_offset(words, r, plane)); },
+                      m, despawn, op, order_base + r, 0u);
+        if (despawn[0]) kill[r] = 1;
     }
-}
-
-// `kill` receives the despawns; they are applied after every system of the schedule has run
-// (Commands are deferred to the end of GgrsSchedule).
-__global__ void __launch_bounds__(256) k_sys_particles_despawn(uint8_t* img, uint32_t words, uint32_t l_plane,
-                                                               uint32_t n_rows, uint8_t* kill, uint32_t need) {
-    for (uint32_t r = blockIdx.x * blockDim.x + threadIdx.x; r < n_rows; r += gridDim.x * blockDim.x) {
-        if (!row_matches(img[alive_offset(words, r)], need)) continue;
-        uint32_t* l = reinterpret_cast<uint32_t*>(img + word_offset(words, r, l_plane));
-        uint64_t ttl = (uint64_t(l[kTileRows]) << 32) | l[0];
-        ttl -= 1;
-        l[0] = uint32_t(ttl); l[kTileRows] = uint32_t(ttl >> 32);
-        if (ttl == 0) kill[r] = 1;
-    }
-}
-
-// x.0 += k   (tests/component_rollback.rs:25-29)
-__global__ void __launch_bounds__(256) k_sys_u32_add(uint8_t* img, uint32_t words, uint32_t plane, uint32_t n_rows, uint32_t k, uint32_t need) {
-    for (uint32_t r = blockIdx.x * blockDim.x + threadIdx.x; r < n_rows; r += gridDim.x * blockDim.x)
-        if (row_matches(img[alive_offset(words, r)], need)) *reinterpret_cast<uint32_t*>(img + word_offset(words, r, plane)) += k;
-}
-
-// h = h.saturating_sub(k); despawn at 0   (tests/synctest.rs:38-45)
-__global__ void __launch_bounds__(256) k_sys_u32_satsub_despawn(uint8_t* img, uint32_t words, uint32_t plane,
-                                                                uint32_t n_rows, uint32_t k, uint8_t* kill, uint32_t need) {
-    for (uint32_t r = blockIdx.x * blockDim.x + threadIdx.x; r < n_rows; r += gridDim.x * blockDim.x) {
-        if (!row_matches(img[alive_offset(words, r)], need)) continue;
-        uint32_t* x = reinterpret_cast<uint32_t*>(img + word_offset(words, r, plane));
-        uint32_t v = *x;
-        v = v > k ? v - k : 0u;
-        *x = v;
-        if (v == 0) kill[r] = 1;
-    }
-}
-
-// commands.entity(e).despawn() for every entity that has the bound component (tests/hierarchy.rs:36-45; launched only
-// on frames whose input matches)
-__global__ void __launch_bounds__(256) k_sys_despawn_having(const uint8_t* img, uint32_t words, uint32_t n_rows, uint8_t* kill, uint32_t need) {
-    for (uint32_t r = blockIdx.x * blockDim.x + threadIdx.x; r < n_rows; r += gridDim.x * blockDim.x)
-        if (row_matches(img[alive_offset(words, r)], need)) kill[r] = 1;
-}
-
-// c.0 = count  (the deliberately non-deterministic system of tests/synctest.rs:92-97)
-__global__ void __launch_bounds__(256) k_sys_u32_store(uint8_t* img, uint32_t words, uint32_t plane, uint32_t n_rows, uint32_t value, uint32_t need) {
-    for (uint32_t r = blockIdx.x * blockDim.x + threadIdx.x; r < n_rows; r += gridDim.x * blockDim.x)
-        if (row_matches(img[alive_offset(words, r)], need)) *reinterpret_cast<uint32_t*>(img + word_offset(words, r, plane)) = value;
 }
 
 // spawn_particles (particles.rs:258-270) on the live image: rows [first, first+count) become
@@ -880,54 +974,6 @@ __global__ void __launch_bounds__(256) k_sys_particles_spawn(uint8_t* img, uint3
         uint32_t* l = reinterpret_cast<uint32_t*>(img + word_offset(words, r, l_plane));
         l[0] = ttl_lo; l[kTileRows] = ttl_hi;
         img[alive_offset(words, r)] = 1;
-    }
-}
-
-#endif  // !__CUDACC_RTC__
-
-// move_cube_system (box_game.rs:154-206), BASELINE config C1.  player handle == RollbackOrdered index.
-// `fr` is `FRICTION.powf(dt)` (FRICTION = 0.0018), evaluated once per Advance by the host with the C library's powf,
-// the function the reference calls (Op::fr_bits).  A device powf is only good to about one ulp and rounds some frame
-// rates' factor the other way, so every result here is bit-exact with the CPU only because the factor comes from the host.
-__device__ __forceinline__ void box_move_step(float& tx, float& ty, float& tz, float& vx, float& vy, float& vz, float dt, float fr,
-                                              uint32_t input) {
-    const float ACCELERATION = 18.0f, MAX_SPEED = 3.0f, PLANE_SIZE = 5.0f, CUBE_SIZE = 0.2f;
-    const bool up = input & 1u, down = input & 2u, left = input & 4u, right = input & 8u;
-    const float a = __fmul_rn(ACCELERATION, dt);
-    if (up && !down) vz = __fsub_rn(vz, a);
-    if (!up && down) vz = __fadd_rn(vz, a);
-    if (left && !right) vx = __fsub_rn(vx, a);
-    if (!left && right) vx = __fadd_rn(vx, a);
-    if (!up && !down) vz = __fmul_rn(vz, fr);
-    if (!left && !right) vx = __fmul_rn(vx, fr);
-    vy = __fmul_rn(vy, fr);
-    // glam Vec3::clamp_length_max(MAX_SPEED)
-    const float len_sq = __fadd_rn(__fadd_rn(__fmul_rn(vx, vx), __fmul_rn(vy, vy)), __fmul_rn(vz, vz));
-    if (len_sq > __fmul_rn(MAX_SPEED, MAX_SPEED)) {
-        const float l = __fsqrt_rn(len_sq);
-        vx = __fmul_rn(MAX_SPEED, __fdiv_rn(vx, l)); vy = __fmul_rn(MAX_SPEED, __fdiv_rn(vy, l)); vz = __fmul_rn(MAX_SPEED, __fdiv_rn(vz, l));
-    }
-    tx = __fadd_rn(tx, __fmul_rn(vx, dt)); ty = __fadd_rn(ty, __fmul_rn(vy, dt)); tz = __fadd_rn(tz, __fmul_rn(vz, dt));
-    const float hw = __fmul_rn(__fsub_rn(PLANE_SIZE, CUBE_SIZE), 0.5f);
-    tx = tx < -hw ? -hw : (tx > hw ? hw : tx);
-    tz = tz < -hw ? -hw : (tz > hw ? hw : tz);
-}
-#ifndef __CUDACC_RTC__
-__global__ void k_sys_box_move(uint8_t* img, uint32_t words, uint32_t t_plane, uint32_t v_plane, uint32_t n_rows,
-                               uint32_t dt_bits, uint32_t fr_bits, unsigned long long inputs_packed, uint32_t n_players,
-                               unsigned long long order_base, uint32_t need) {
-    const float dt = __uint_as_float(dt_bits), fr = __uint_as_float(fr_bits);
-    for (uint32_t r = blockIdx.x * blockDim.x + threadIdx.x; r < n_rows; r += gridDim.x * blockDim.x) {
-        if (!row_matches(img[alive_offset(words, r)], need)) continue;
-        float* t = reinterpret_cast<float*>(img + word_offset(words, r, t_plane));
-        float* v = reinterpret_cast<float*>(img + word_offset(words, r, v_plane));
-        float tx = t[0], ty = t[kTileRows], tz = t[2 * kTileRows];
-        float vx = v[0], vy = v[kTileRows], vz = v[2 * kTileRows];
-        const unsigned long long handle = order_base + r;
-        const uint32_t input = handle < n_players && handle < 8 ? uint32_t(inputs_packed >> (8 * uint32_t(handle))) & 0xffu : 0u;
-        box_move_step(tx, ty, tz, vx, vy, vz, dt, fr, input);
-        t[0] = tx; t[kTileRows] = ty; t[2 * kTileRows] = tz;
-        v[0] = vx; v[kTileRows] = vy; v[2 * kTileRows] = vz;
     }
 }
 
