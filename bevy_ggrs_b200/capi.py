@@ -58,6 +58,8 @@ BGR_KERNEL_DEFERRED_LIVE = 1 << 13
 BGR_KERNEL_FROM_DEFERRED = 1 << 14
 # ... and the bundle launch read or wrote passive planes
 BGR_KERNEL_PASSIVE_PLANES = 1 << 15
+# ... and the bundle launch stored only the active planes whose content the target did not hold (grids of several waves)
+BGR_KERNEL_STABLE_PLANES = 1 << 26
 
 
 class bgr_request(C.Structure):

@@ -114,6 +114,26 @@ struct HostState {  // trivially copyable: copying it per call must not allocate
     //     keeps the invariant.  A sharded engine keeps its own versions.
     //   - overlapping launches (PF_TILE_WAIT): elision only drops passive reads and stores, and a tick after a bump
     //     stages the passive planes exactly as every tick did before, so no launch reads what an earlier one writes.
+    //
+    // Content stamps of the active planes (bgr_engine::d_stamps, engines that run the bundle kernel), the device-side
+    // counterpart for the planes the systems write, decided per warp segment because it depends on the values:
+    //   stamp[img][seg][q] == S != 0  =>  the bytes of active plane q of 64-row segment seg in image img are exactly
+    //   the content that stamp S names.  0 = unknown.
+    // Stamps are issued by the host, a fresh range per bundle launch (stamp_base + op index), and never reused: when
+    // the 32-bit range runs out the whole table is cleared on the stream and the range starts again.  Who writes:
+    //   - the bundle kernel keeps the invariant itself: a Load takes the source's stamps, a plane whose bits a frame
+    //     changed (or whose stamp is unknown) gets a fresh stamp at the next Save, a store writes the stamp with the bytes.
+    //     Its instance without stamps (single-wave grids, run_fused) stores whole active planes and writes no stamp: it
+    //     marks the table stale, and the next stamped launch clears the whole table first.
+    //   - every other writer of an image clears that image's stamps (clear_stamps): transfer_column to the device
+    //     (bgr_write_component, bgr_insert_component), bgr_spawn, bgr_run_startup_system, bgr_remove_component,
+    //     bgr_insert_component's presence bit, and bgr_despawn (the alive byte is an active plane).
+    //   - the deferred live image is materialised by the bundle kernel itself; while it is pending, image 0 keeps the
+    //     bytes and the stamps of its last write.
+    //   - the stepwise path (k_image_tma, k_copy_image), the interpreter and k_generic_jit only run on engines that do
+    //     not use the bundle (use_bundle is fixed at bgr_build); those have no stamp table.
+    //   - desync capture, retention, digests, export, bgr_reset_session and bgr_set_depth write no image bytes.  A
+    //     sharded engine keeps its own table.
     uint64_t live_passive_ver = 1, ver_counter = 1;
     std::array<uint64_t, SlotRing::kMaxSlots> slot_passive_ver{};  // 0 = never written
 };
@@ -255,6 +275,10 @@ struct bgr_engine {
     std::vector<uint16_t> passive;
     std::vector<PassiveRun> runs;
     uint32_t passive_bytes = 0;
+    uint32_t* d_stamps = nullptr;   // content stamps of the active planes (HostState): [images][segments][kActivePlanes]
+    uint32_t stamp_image = 0;       // words per image
+    uint32_t stamp_next = 1;        // first stamp of the next bundle launch
+    bool stamps_stale = false;      // a bundle launch without stamps wrote images since the table was last cleared
     bool bundle_static_ck = false;  // both columns checksummed with the finite assertion: fully specialised kernel
     // generic one-launch program (generic_program.cuh): any schema whose tile fits shared memory + the compiled systems
     bool generic_ok = false;
@@ -276,7 +300,7 @@ struct bgr_engine {
     int tune_tma = 1;          // stepwise Save/Load through the TMA-staged bulk-copy kernel
     uint32_t tma_stage_tiles = 0;  // one-tile stages of the TMA copy kernel (0: schema too wide for two stages of shared memory)
     unsigned int* d_tma_ticket = nullptr;
-    int occ_cache[2][3] = {};  // [passive TMA][MODE]: blocks per SM of k_particles_program
+    int occ_cache[2][3][2] = {};  // [passive TMA][MODE][STAMPS]: blocks per SM of k_particles_program
     // desync diff scratch (BGR_CFG_DESYNC_CAPTURE), allocated by the first bgr_desync_diff
     DiffColumn* d_diff_cols = nullptr;
     unsigned int* d_diff_counts = nullptr;       // [n_cols][3] then the per-tile record counts
@@ -308,6 +332,15 @@ struct bgr_engine {
 };
 
 namespace {
+
+// A write outside the bundle kernel: image `idx`'s content stamps become unknown (HostState).  Stream-ordered behind
+// every launch that could still write them.
+int clear_stamps(bgr_engine* e, uint32_t idx) {
+    if (!e->d_stamps) return BGR_OK;
+    CUDA_TRY(cudaMemsetAsync(e->d_stamps + size_t(idx) * e->stamp_image, 0, size_t(e->stamp_image) * sizeof(uint32_t), e->stream));
+    e->tiledep_chain = false;
+    return BGR_OK;
+}
 
 // ---------------------------------------------------------------------------------------------
 // compile: requests -> ops, mutating `s` exactly like handle_requests mutates the World
@@ -467,16 +500,16 @@ int compile_requests(bgr_engine* e, HostState& s, const bgr_session_info* sess, 
 // ---------------------------------------------------------------------------------------------
 // launch: fused bundle kernel
 // ---------------------------------------------------------------------------------------------
-template <int MODE>
+template <int MODE, bool STAMPS>
 int launch_particles(bgr_engine* e, const ProgramParams& pp) {
-    auto kern = k_particles_program<MODE>;
+    auto kern = k_particles_program<MODE, STAMPS>;
     constexpr int kBlock = int(kTileRows) / 2;  // two rows per thread
     const int ti = (pp.flags & PF_PASSIVE_TMA) ? 1 : 0;
     const size_t smem = ti ? size_t(2) * pp.passive_bytes : 0;
     // A mode runs with and without the passive double buffer (spawns and multi-Load vectors move passive planes per
     // thread): the shared-memory opt-in and the occupancy are per (mode, buffer).  passive_bytes is fixed at bgr_build,
     // so one entry per buffer setting is exact.
-    int& occ = e->occ_cache[ti][MODE];
+    int& occ = e->occ_cache[ti][MODE][STAMPS ? 1 : 0];
     if (occ == 0) {
         if (smem > 48 * 1024) CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem)));
         int nb = 0;
@@ -501,14 +534,15 @@ int launch_particles(bgr_engine* e, const ProgramParams& pp) {
     const bool passive = pp.n_runs > 0 || pp.n_passive > 0;
     // VEC 2, launch-bounds tier 1 (768 threads per SM), whole-tile work items
     e->last_kernel = BGR_KERNEL_BUNDLE | (2u << 4) | (uint32_t(MODE) << 8) | (1u << 10) | (ti ? 1u << 12 : 0u) |
-                     (passive ? BGR_KERNEL_PASSIVE_PLANES : 0u) | (uint32_t(kTileRows) << 16);
+                     (passive ? BGR_KERNEL_PASSIVE_PLANES : 0u) | (uint32_t(kTileRows) << 16) | (STAMPS ? BGR_KERNEL_STABLE_PLANES : 0u);
     return BGR_OK;
 }
 
+template <bool STAMPS>
 int launch_fused_variant(bgr_engine* e, const ProgramParams& pp) {
-    if (e->bundle_opt) return launch_particles<2>(e, pp);         // per-entity presence
-    if (e->bundle_static_ck) return launch_particles<1>(e, pp);   // both columns checksummed with the finite assertion
-    return launch_particles<0>(e, pp);
+    if (e->bundle_opt) return launch_particles<2, STAMPS>(e, pp);         // per-entity presence
+    if (e->bundle_static_ck) return launch_particles<1, STAMPS>(e, pp);   // both columns checksummed with the finite assertion
+    return launch_particles<0, STAMPS>(e, pp);
 }
 
 int run_fused(bgr_engine* e, const Program& pg, uint32_t buf) {
@@ -539,6 +573,10 @@ int run_fused(bgr_engine* e, const Program& pg, uint32_t buf) {
     if (!pg.has_spawn && simple && e->tune_passive_tma && !e->runs.empty() && 2u * e->passive_bytes <= 96u * 1024u) pp.flags |= PF_PASSIVE_TMA;
     // one wave of blocks (every block runs one or two tiles): the tile's tail is the grid's tail
     if (e->tune_passive_early == 1 || (e->tune_passive_early < 0 && pp.n_tiles <= 3u * uint32_t(e->num_sms))) pp.flags |= PF_PASSIVE_EARLY;
+    // Stable-plane elision pays where the grid is bandwidth-bound (several waves).  A single-wave grid is latency-bound:
+    // there the bit compares of every Advance and the stamp round trip of every Save only lengthen the critical path
+    // (100k entities: -9 % e2e), so it runs the instance without stamps.
+    const bool stamps = !(pp.flags & PF_PASSIVE_EARLY);
     const Column& ct = e->cols[e->bt]; const Column& cv = e->cols[e->bv];
     if (ct.hash_kind != BGR_HASH_NONE) { pp.flags |= PF_CK_T; if (ct.hash_flags & BGR_HASH_FLAG_ASSERT_FINITE_F32) pp.flags |= PF_FIN_T; pp.ck_t_slot = uint32_t(ct.ck_slot); }
     if (cv.hash_kind != BGR_HASH_NONE) { pp.flags |= PF_CK_V; if (cv.hash_flags & BGR_HASH_FLAG_ASSERT_FINITE_F32) pp.flags |= PF_FIN_V; pp.ck_v_slot = uint32_t(cv.ck_slot); }
@@ -556,6 +594,22 @@ int run_fused(bgr_engine* e, const Program& pg, uint32_t buf) {
         pp.passive_template[i] = (uint32_t(e->passive[i]) >= ct.first_plane && tw >= 6 && tw <= 9) ? 0x3f800000u : 0u;
     }
     std::memcpy(pp.ops, pg.ops, sizeof(Op) * pg.n_ops);
+    for (uint32_t i = 0; i < pg.n_ops; ++i)  // the stamp-table row of each image a LOAD / SAVE touches
+        if (pp.ops[i].kind != OP_ADVANCE) pp.ops[i].call_count = uint32_t((size_t(pp.ops[i].image_off256) << 8) / e->image_bytes);
+    // a fresh stamp range: one stamp per op and one for the live write.  The table is cleared when the range runs out,
+    // and before the first stamped launch after launches without stamps (they rewrote images behind the stamps' back;
+    // a world changes sides only when its row count crosses the one-wave size)
+    if (stamps && (e->stamps_stale || e->stamp_next > 0xFFFFFFFFu - uint32_t(kMaxOps + 1))) {
+        CUDA_TRY(cudaMemsetAsync(e->d_stamps, 0, size_t(e->stamp_image) * (e->n_slots() + 1u) * sizeof(uint32_t), e->stream));
+        e->tiledep_chain = false;
+        e->stamp_next = 1;
+        e->stamps_stale = false;
+    }
+    if (!stamps) e->stamps_stale = true;
+    pp.stamps = e->d_stamps;
+    pp.stamp_image = e->stamp_image;
+    pp.stamp_base = e->stamp_next;
+    if (stamps) e->stamp_next += pg.n_ops + 1;
 
     // only worth it when request vectors are queued behind each other (bgr_submit_requests with others un-collected):
     // a synchronous caller collects before the next submit, so there is nothing to overlap with
@@ -589,7 +643,7 @@ int run_fused(bgr_engine* e, const Program& pg, uint32_t buf) {
     pp.ticket = e->d_ticket_set[set];
     pp.out = pg.internal ? e->d_internal_out : e->d_out[buf];
     if (e->d_trace && !pg.internal && e->seq - e->trace_first_seq < e->trace_cap) pp.trace = e->d_trace + (e->seq - e->trace_first_seq) * 4;
-    int rc = launch_fused_variant(e, pp);
+    int rc = stamps ? launch_fused_variant<true>(e, pp) : launch_fused_variant<false>(e, pp);
     if (rc != BGR_OK) return rc;
     e->tiledep_chain = tiledep;
     e->tiledep_seq = uint32_t(e->seq); e->tiledep_tiles = pp.n_tiles;
@@ -1174,6 +1228,8 @@ int transfer_column(bgr_engine* e, uint32_t image_idx, uint32_t column, uint32_t
         k_scatter_column<<<grid, 256, 0, e->stream>>>(img, e->words, c.first_plane, c.words, c.elem_bytes, first, count, e->d_stage, stride);
         e->launches += 1;
         CUDA_TRY(cudaGetLastError());
+        rc = clear_stamps(e, image_idx);
+        if (rc != BGR_OK) return rc;
         CUDA_TRY(cudaStreamSynchronize(e->stream));
     } else {
         if (stride != c.elem_bytes) CUDA_TRY(cudaMemcpyAsync(e->d_stage, host, bytes, cudaMemcpyHostToDevice, e->stream));  // keep the caller's padding bytes
@@ -1386,6 +1442,7 @@ BGR_API void bgr_engine_destroy(bgr_engine* e) {
         if (e->ev[i]) cudaEventDestroy(e->ev[i]);
     }
     if (e->arena) cudaFree(e->arena);
+    if (e->d_stamps) cudaFree(e->d_stamps);
     if (e->d_kill) cudaFree(e->d_kill);
     if (e->d_stage) cudaFree(e->d_stage);
     if (e->d_accum) cudaFree(e->d_accum);
@@ -1577,6 +1634,12 @@ BGR_API int bgr_build(bgr_engine* e) {
         }
     build_specs(e);
     detect_bundles(e);
+    if (use_bundle(e)) {  // content stamps of the active planes: every image, every 64-row segment
+        e->stamp_image = e->n_tiles_cap * kSegsPerTile * kActivePlanes;
+        const size_t bytes = size_t(e->stamp_image) * (e->n_slots() + 1u) * sizeof(uint32_t);
+        CUDA_TRY(cudaMalloc(&e->d_stamps, bytes));
+        CUDA_TRY(cudaMemsetAsync(e->d_stamps, 0, bytes, e->stream));
+    }
     // generic one-launch program: every row system runs on its tile (run_system); spawning is a Command of the stepwise
     // path; the parameter block holds kMaxGenericSys systems; the tile fits twice per SM
     e->generic_ok = e->spawn_sys < 0 && e->sys_specs.size() <= size_t(kMaxGenericSys) && e->tile_bytes <= 100u * 1024u;
@@ -1622,6 +1685,8 @@ BGR_API int bgr_run_startup_system(bgr_engine* e, uint32_t system) {
         e->st.n_rows, rate, e->d_spawn[0], uint32_t(ttl), uint32_t(ttl >> 32));
     e->launches += 1;
     CUDA_TRY(cudaGetLastError());
+    rc = clear_stamps(e, 0);
+    if (rc != BGR_OK) return rc;
     CUDA_TRY(cudaStreamSynchronize(e->stream));
     e->st.n_rows += rate;
     e->st.live_passive_ver = ++e->st.ver_counter;
@@ -1642,6 +1707,8 @@ BGR_API int bgr_spawn(bgr_engine* e, uint32_t count, uint32_t* first_row_out) {
         k_spawn_rows<<<e->grid_for(count, 64), 256, 0, e->stream>>>(e->image(0), e->words, first, count);
         e->launches += 1;
         CUDA_TRY(cudaGetLastError());
+        rc = clear_stamps(e, 0);
+        if (rc != BGR_OK) return rc;
         CUDA_TRY(cudaStreamSynchronize(e->stream));
     }
     e->st.n_rows += count;
@@ -1659,6 +1726,8 @@ BGR_API int bgr_despawn(bgr_engine* e, uint32_t row) {
     k_set_alive<<<1, 1, 0, e->stream>>>(e->image(0), e->words, row, 0);
     e->launches += 1;
     CUDA_TRY(cudaGetLastError());
+    rc = clear_stamps(e, 0);
+    if (rc != BGR_OK) return rc;
     CUDA_TRY(cudaStreamSynchronize(e->stream));
     return BGR_OK;
 }
@@ -1706,6 +1775,8 @@ BGR_API int bgr_remove_component(bgr_engine* e, uint32_t column, uint32_t row) {
     k_set_absent<<<1, 1, 0, e->stream>>>(e->image(0), e->words, row, e->cols[column].absent, 1u);
     e->launches += 1;
     CUDA_TRY(cudaGetLastError());
+    rc = clear_stamps(e, 0);
+    if (rc != BGR_OK) return rc;
     CUDA_TRY(cudaStreamSynchronize(e->stream));
     e->st.live_passive_ver = ++e->st.ver_counter;
     return BGR_OK;
@@ -1719,6 +1790,8 @@ BGR_API int bgr_insert_component(bgr_engine* e, uint32_t column, uint32_t row, c
     k_set_absent<<<1, 1, 0, e->stream>>>(e->image(0), e->words, row, e->cols[column].absent, 0u);
     e->launches += 1;
     CUDA_TRY(cudaGetLastError());
+    rc = clear_stamps(e, 0);
+    if (rc != BGR_OK) return rc;
     CUDA_TRY(cudaStreamSynchronize(e->stream));
     return BGR_OK;
 }

@@ -91,8 +91,9 @@ struct Op {
     uint32_t n_rows;       // rows that exist while this op runs (RollbackOrdered::len())
     uint32_t save_index;    // SAVE: which accumulator row.  ADVANCE+SPAWN: number of spawned rows
     uint32_t flags;
-    uint32_t call_count;    // ADVANCE: value of the un-rolled-back host counter (test system).  ADVANCE+SPAWN: offset into spawn_vals
-    uint8_t inputs[8];      // ADVANCE: PlayerInputs<T>.0[handle].0 for every handle (u8, BGR_MAX_PLAYERS)
+    uint32_t call_count;    // ADVANCE: value of the un-rolled-back host counter (test system).  ADVANCE+SPAWN: offset into spawn_vals.
+                            // LOAD/SAVE in the bundle kernel: index of the image (its row of the content-stamp table)
+    uint8_t inputs[8];     // ADVANCE: PlayerInputs<T>.0[handle].0 for every handle (u8, BGR_MAX_PLAYERS)
 };
 static_assert(sizeof(Op) == 40, "Op layout");
 
@@ -125,6 +126,13 @@ enum ProgFlags : uint32_t {
 
 struct PassiveRun { uint32_t off, bytes; };  // inside a tile; adjacent passive planes form one run
 
+// Content stamps of the bundle kernel's active planes (translation x/y/z, velocity x/y/z, ttl lo/hi, alive: plane q in
+// that order), one u32 per (image, 64-row warp segment, plane); the invariant is in engine.cu HostState.
+constexpr uint32_t kActivePlanes = 9;
+constexpr uint32_t kAlivePlaneBit = 1u << 8;
+constexpr uint32_t kSegRows = 64;
+constexpr uint32_t kSegsPerTile = kTileRows / kSegRows;
+
 struct ProgramParams {
     uint8_t* arena;
     unsigned long long order_base;
@@ -153,6 +161,9 @@ struct ProgramParams {
     // all store): HBM idles while the ALUs work and vice versa until latency noise has dephased them.  Delaying the
     // second / third resident block of every SM by a fraction of one frame's time starts them out of phase.
     uint32_t stagger_ns, stagger_div;
+    uint32_t* stamps;               // [images][segments][kActivePlanes] content stamps (0 = unknown)
+    uint32_t stamp_image;           // words of one image's row of `stamps`
+    uint32_t stamp_base;            // this launch's fresh stamps: stamp_base + op index, stamp_base + n_ops for the live write
     PassiveRun runs[kMaxRuns];
     uint16_t passive[kMaxPassive];
     uint32_t passive_template[kMaxPassive];   // value of each passive word in a freshly spawned row (Transform::default())
@@ -395,8 +406,11 @@ __device__ __forceinline__ void run_system(const SysSpec& sy, Word&& word, const
 //       ADVANCE : update_particles + despawn_particles in registers (0 bytes)
 //       SAVE    : stream them into the frame's slot and fold the per-entity seahashes of the
 //                 checksummed columns: warp REDUX.XOR -> shared atomics -> one global atomic per
-//                 block per (save, column) -> last block publishes to host-mapped memory
-//       end     : write the live image once
+//                 block per (save, column) -> last block publishes to host-mapped memory.  A warp stores
+//                 only the planes of its 64-row segment whose content stamp the slot does not hold
+//                 already (ProgramParams::stamps): in a 2-D world z, velocity.x, ttl.hi and alive
+//                 keep their bits from frame to frame and are stored once per slot
+//       end     : write the live image once (same stamp rule)
 //   * passive planes (rotation, scale, any registered column no compiled system writes) never
 //     touch a register: one cp.async.bulk brings the tile's passive runs into shared memory and
 //     one cp.async.bulk per SAVE (and one for the live image) streams them out again.
@@ -412,7 +426,9 @@ __device__ __forceinline__ void run_system(const SysSpec& sy, Word&& word, const
 // per row, and Save / Load move the mask with the image (= the four-way match of component_snapshot.rs:99-115).
 // Two rows per thread, 256 threads per tile, three resident blocks (768 threads) per SM: DESIGN.md "What a synchronous
 // call costs" has the measurements against 1 and 4 rows per thread and the other launch-bounds tiers.
-template <int MODE>
+// STAMPS: stable-plane elision (content stamps, below).  It pays on bandwidth-bound grids of several waves; a single-wave
+// grid is latency-bound, and there the instance without it runs (engine.cu run_fused), which stores every active plane.
+template <int MODE, bool STAMPS>
 __global__ void __launch_bounds__(256, 3) k_particles_program(const __grid_constant__ ProgramParams p) {
     constexpr int VEC = 2, BLOCK = 256;  // rows per thread, threads per block (__launch_bounds__)
     static_assert(VEC * BLOCK == int(kTileRows), "a block iteration covers one tile");
@@ -428,9 +444,11 @@ __global__ void __launch_bounds__(256, 3) k_particles_program(const __grid_const
     __shared__ unsigned int s_acc[kMaxSaves * kAccStride * 2];  // 32-bit halves: native shared atomics, no CAS loop
     __shared__ __align__(8) uint64_t s_bar[2];
     __shared__ unsigned int s_last;
+    __shared__ unsigned int s_stored;  // bgr_trace_enable: 64-byte units of active planes this block stored
 
     const uint32_t tid = threadIdx.x, lane = tid & 31u;
     if (p.trace && tid == 0) atomicMin(&p.trace[0], globaltimer_ns());  // bgr_trace_enable: when did this launch's first block start
+    if (tid == 0) s_stored = 0u;
     // Programmatic dependent launch: let the NEXT request vector's kernel be launched and its blocks scheduled
     // into SM slots as this grid drains (hides launch latency and block ramp-up between back-to-back ticks) ...
     asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
@@ -477,9 +495,12 @@ __global__ void __launch_bounds__(256, 3) k_particles_program(const __grid_const
     uint32_t it = 0;
     // PF_TILE_SIGNAL: a fence per announced tile stalls the warp until its stores are acknowledged (8 % when every tile
     // was announced), so only the first tile of each block is — the tiles the next grid's first wave starts with
+    // The stamps of a tile's segments are read and written only by the warps that run that tile, so the next launch's
+    // stamp reads need exactly what its data reads need: the stamp stores are ordinary stores of those warps, behind the
+    // same fence as the tile's data (and behind the grid's __threadfence for tiles that only grid_done announces).
     auto signal_tile = [&](uint32_t t) {
         if (use_tma && tid == 0) tma_wait_all();  // that tile's bulk stores have landed (not just released their buffer)
-        fence_acq_rel_gpu();                      // every thread's stores are visible gpu-wide before its warp arrives
+        fence_acq_rel_gpu();                      // every thread's stores (data and stamps) are visible gpu-wide before its warp arrives
         __syncwarp();
         if (lane == 0) {
             if (atomicAdd(&p.tile_cnt[t], 1u) == kTileRows / (32 * VEC) - 1) {  // last warp to announce this tile
@@ -522,8 +543,15 @@ __global__ void __launch_bounds__(256, 3) k_particles_program(const __grid_const
         // ------------------------------ active words ------------------------------
         uint32_t tr[3][VEC], vl[3][VEC], tl[2][VEC];
         uint32_t alive = 0;
+        // Stable-plane elision.  Lane q < kActivePlanes holds `st`, the stamp of the content plane q of this warp's
+        // segment has in registers (0 = unknown); `dirty` collects the planes whose bits this thread changed since.  A
+        // Save gives every dirty or unknown plane a fresh stamp and stores only the planes whose stamp the target image
+        // does not already hold.
+        uint32_t st = 0, dirty = 0;
+        uint32_t* const seg_stamps = p.stamps + (size_t(tile) * kSegsPerTile + (tid >> 5)) * kActivePlanes + min(lane, kActivePlanes - 1u);
+        const bool stamp_lane = lane < kActivePlanes;
 
-        auto load_active = [&](const uint8_t* img, uint32_t n_rows) {
+        auto load_active = [&](const uint8_t* img, uint32_t n_rows, uint32_t img_idx) {
             const uint8_t* pt = img + p.t_off + woff;
             const uint8_t* pv = img + p.v_off + woff;
             const uint8_t* pl = img + p.l_off + woff;
@@ -533,23 +561,50 @@ __global__ void __launch_bounds__(256, 3) k_particles_program(const __grid_const
             for (int k = 0; k < 3; ++k) vec_load<VEC>(pv + k * kPlaneBytes, vl[k]);
 #pragma unroll
             for (int k = 0; k < 2; ++k) vec_load<VEC>(pl + k * kPlaneBytes, tl[k]);
-            alive = alive_load<VEC>(img + aoff) & (OPT ? rows_mask_full<VEC>(row0, n_rows) : rows_mask<VEC>(row0, n_rows));
+            const uint32_t raw = alive_load<VEC>(img + aoff);
+            alive = raw & (OPT ? rows_mask_full<VEC>(row0, n_rows) : rows_mask<VEC>(row0, n_rows));
+            if (STAMPS) {
+                dirty = alive != raw ? kAlivePlaneBit : 0u;  // the row count cleared alive bytes the image holds
+                st = stamp_lane ? __ldcg(seg_stamps + size_t(img_idx) * p.stamp_image) : 0u;
+            }
         };
-        auto store_active = [&](uint8_t* img) {
+        // first half of a stamped store into image img_idx: stamps the dirty planes with `fresh` and issues the read of
+        // the image's stamps, which store_active consumes later (the checksum of a Save hides part of its latency)
+        auto claim_stamps = [&](uint32_t img_idx, uint32_t fresh) -> uint32_t {
+            if (!STAMPS) return 0u;
+            const uint32_t d = __reduce_or_sync(0xffffffffu, dirty);
+            dirty = 0;
+            if (stamp_lane && (((d >> lane) & 1u) || st == 0u)) st = fresh;
+            return stamp_lane ? __ldcg(seg_stamps + size_t(img_idx) * p.stamp_image) : st;
+        };
+        // stores the planes whose stamp in image img_idx (`held`, from claim_stamps) differs and records the new stamps;
+        // without STAMPS every plane
+        auto store_active = [&](uint8_t* img, uint32_t img_idx, uint32_t held) {
+            uint32_t planes = (1u << kActivePlanes) - 1u;
+            if (STAMPS) {
+                const bool put = held != st;
+                planes = __ballot_sync(0xffffffffu, put);
+                if (put) __stcg(seg_stamps + size_t(img_idx) * p.stamp_image, st);
+            }
+            // a word plane-segment is 4 units of 64 B, the alive plane-segment 1
+            if (p.trace && lane == 0) atomicAdd(&s_stored, 4u * __popc(planes & 0xFFu) + (planes >> 8));
             uint8_t* pt = img + p.t_off + woff;
             uint8_t* pv = img + p.v_off + woff;
             uint8_t* pl = img + p.l_off + woff;
 #pragma unroll
-            for (int k = 0; k < 3; ++k) vec_store<VEC>(pt + k * kPlaneBytes, tr[k]);
+            for (int k = 0; k < 3; ++k)
+                if (planes & (1u << k)) vec_store<VEC>(pt + k * kPlaneBytes, tr[k]);
 #pragma unroll
-            for (int k = 0; k < 3; ++k) vec_store<VEC>(pv + k * kPlaneBytes, vl[k]);
+            for (int k = 0; k < 3; ++k)
+                if (planes & (8u << k)) vec_store<VEC>(pv + k * kPlaneBytes, vl[k]);
 #pragma unroll
-            for (int k = 0; k < 2; ++k) vec_store<VEC>(pl + k * kPlaneBytes, tl[k]);
-            alive_store<VEC>(img + aoff, alive);
+            for (int k = 0; k < 2; ++k)
+                if (planes & (64u << k)) vec_store<VEC>(pl + k * kPlaneBytes, tl[k]);
+            if (planes & kAlivePlaneBit) alive_store<VEC>(img + aoff, alive);
         };
 
-        if (p.flags & PF_READ_LIVE) load_active(p.arena, p.live_rows);
-        else load_active(p.arena + (size_t(p.ops[0].image_off256) << 8), p.ops[0].n_rows);  // ops[0] is a LOAD
+        if (p.flags & PF_READ_LIVE) load_active(p.arena, p.live_rows, 0u);
+        else load_active(p.arena + (size_t(p.ops[0].image_off256) << 8), p.ops[0].n_rows, p.ops[0].call_count);  // ops[0] is a LOAD
 
         // lane of the per-entity hash that only depends on the RollbackOrdered index
         uint64_t t0[VEC];
@@ -622,8 +677,17 @@ __global__ void __launch_bounds__(256, 3) k_particles_program(const __grid_const
             const uint32_t kind = p.ops[i].kind;
             if (kind == OP_ADVANCE) {
                 const float dt = __uint_as_float(p.ops[i].dt_bits);
+                const uint32_t alive_before = alive;
 #pragma unroll
                 for (int j = 0; j < VEC; ++j) {
+                    // bits, not values: -0.0 -> +0.0 and a changed NaN payload are changes
+                    const uint32_t o0 = tr[0][j], o1 = tr[1][j], o2 = tr[2][j], o3 = vl[0][j], o4 = vl[1][j], o5 = vl[2][j];
+                    const uint32_t o6 = tl[0][j], o7 = tl[1][j];
+                    auto note_changes = [&]() {
+                        dirty |= (tr[0][j] != o0 ? 1u : 0u) | (tr[1][j] != o1 ? 2u : 0u) | (tr[2][j] != o2 ? 4u : 0u) |
+                                 (vl[0][j] != o3 ? 8u : 0u) | (vl[1][j] != o4 ? 16u : 0u) | (vl[2][j] != o5 ? 32u : 0u) |
+                                 (tl[0][j] != o6 ? 64u : 0u) | (tl[1][j] != o7 ? 128u : 0u);
+                    };
                     if (OPT) {
                         // the queries only match entities that have the components (and exist)
                         const uint32_t m = (alive >> (8 * j)) & 0xFFu;
@@ -637,6 +701,7 @@ __global__ void __launch_bounds__(256, 3) k_particles_program(const __grid_const
                             tl[0][j] = lo; tl[1][j] = hi;
                             alive &= ((lo | hi) == 0u) ? ~(0xFFu << (8 * j)) : 0xFFFFFFFFu;
                         }
+                        if (STAMPS) note_changes();
                         continue;
                     }
                     particle_step(tr[0][j], tr[1][j], tr[2][j], vl[0][j], vl[1][j], vl[2][j], dt);
@@ -646,7 +711,9 @@ __global__ void __launch_bounds__(256, 3) k_particles_program(const __grid_const
                     lo -= 1u;
                     tl[0][j] = lo; tl[1][j] = hi;
                     alive &= ((lo | hi) == 0u) ? ~(0xFFu << (8 * j)) : 0xFFFFFFFFu;
+                    if (STAMPS) note_changes();
                 }
+                if (STAMPS && alive != alive_before) dirty |= kAlivePlaneBit;
                 if (p.ops[i].flags & OPF_SPAWN) {
                     // spawn_particles (particles.rs:258-270): Commands are applied after the schedule, so the
                     // newborn rows appear now, un-updated: Transform::default(), Velocity(vx, vy, 0), Ttl(ttl)
@@ -660,12 +727,15 @@ __global__ void __launch_bounds__(256, 3) k_particles_program(const __grid_const
                             vl[0][j] = __float_as_uint(v.x); vl[1][j] = __float_as_uint(v.y); vl[2][j] = 0u;
                             tl[0][j] = p.spawn_ttl_lo; tl[1][j] = p.spawn_ttl_hi;
                             alive = (alive & ~(0xFFu << (8 * j))) | (1u << (8 * j));  // exists, every component present
+                            dirty = (1u << kActivePlanes) - 1u;
                         }
                     }
                 }
             } else if (kind == OP_SAVE) {
                 uint8_t* img = p.arena + (size_t(p.ops[i].image_off256) << 8);
-                if (!(p.ops[i].flags & OPF_NO_STORE)) store_active(img);
+                const bool store = !(p.ops[i].flags & OPF_NO_STORE);
+                const uint32_t held = store ? claim_stamps(p.ops[i].call_count, p.stamp_base + i) : 0u;
+                if (store && !STAMPS) store_active(img, p.ops[i].call_count, held);  // nothing to wait for: issue the stores first
                 // ---- checksum partials (component_checksum.rs:81-90) ----
                 uint64_t hx_t = 0, hx_v = 0;
                 uint32_t bad = 0;
@@ -709,12 +779,13 @@ __global__ void __launch_bounds__(256, 3) k_particles_program(const __grid_const
                 pend[5] = (FINT || FINV) ? __reduce_or_sync(full, bad) : 0u;
                 pend_row = p.ops[i].save_index * kAccStride;
                 pend_valid = true;
+                if (store && STAMPS) store_active(img, p.ops[i].call_count, held);
             } else {  // OP_LOAD
-                load_active(p.arena + (size_t(p.ops[i].image_off256) << 8), p.ops[i].n_rows);
+                load_active(p.arena + (size_t(p.ops[i].image_off256) << 8), p.ops[i].n_rows, p.ops[i].call_count);
             }
         }
         flush_pending();
-        if (p.flags & PF_WRITE_LIVE_ACTIVE) store_active(p.arena);
+        if (p.flags & PF_WRITE_LIVE_ACTIVE) store_active(p.arena, 0u, claim_stamps(0u, p.stamp_base + p.n_ops));
 
         // ------------------------------ passive planes ------------------------------
         if (use_tma) {
@@ -783,6 +854,7 @@ __global__ void __launch_bounds__(256, 3) k_particles_program(const __grid_const
             else atomicXor(&p.accum[i], v);
         }
     }
+    if (p.trace && tid == 0 && s_stored) atomicAdd(&p.trace[3], (unsigned long long)s_stored);
     __threadfence();
     __syncthreads();
     if (p.trace && tid == 0) atomicMax(&p.trace[1], globaltimer_ns());  // ... and when did its last block finish its tiles

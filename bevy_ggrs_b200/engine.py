@@ -37,13 +37,14 @@ class LastKernel(NamedTuple):
     deferred_live: bool = False
     from_deferred: bool = False
     passive_planes: bool = False
+    stable_planes: bool = False
 
     @staticmethod
     def decode(v: int) -> "LastKernel":
         return LastKernel(_KERNEL_KINDS.get(v & 0xF, f"unknown({v & 0xF})"), (v >> 4) & 0xF, (v >> 8) & 0x3,
                           (v >> 10) & 0x3, bool((v >> 12) & 1), (v >> 16) & 0x3FF, v,
                           bool(v & capi.BGR_KERNEL_DEFERRED_LIVE), bool(v & capi.BGR_KERNEL_FROM_DEFERRED),
-                          bool(v & capi.BGR_KERNEL_PASSIVE_PLANES))
+                          bool(v & capi.BGR_KERNEL_PASSIVE_PLANES), bool(v & capi.BGR_KERNEL_STABLE_PLANES))
 
 
 class Engine:

@@ -490,10 +490,14 @@ BGR_API int bgr_generic_specialised(bgr_engine* e, uint32_t* specialised_out);
  *   bit 15     BGR_KERNEL_PASSIVE_PLANES, bundle: the launch read or wrote passive planes.  Clear on a tick whose Saves
  *              go into slots that already hold the live passive content and whose Load does not change it
  *              (BGR_CFG_SKIP_UNCHANGED_PLANES above)
- *   bits 16-25 bundle and generic NVRTC: rows per work item (512 = a whole tile) */
+ *   bits 16-25 bundle and generic NVRTC: rows per work item (512 = a whole tile)
+ *   bit 26     BGR_KERNEL_STABLE_PLANES, bundle: stable-plane elision.  Each warp stored only the active planes of its
+ *              64-row segment whose content the target image did not already hold (device-side content stamps).  Set on
+ *              grids of several waves; a single-wave (latency-bound) grid stores every active plane */
 #define BGR_KERNEL_DEFERRED_LIVE (1u << 13)
 #define BGR_KERNEL_FROM_DEFERRED (1u << 14)
 #define BGR_KERNEL_PASSIVE_PLANES (1u << 15)
+#define BGR_KERNEL_STABLE_PLANES (1u << 26)
 #define BGR_KERNEL_NONE 0u
 #define BGR_KERNEL_STEPWISE_TMA 1u       /* one kernel per request; Save / Load through the TMA-staged copy kernel */
 #define BGR_KERNEL_STEPWISE_FLAT 2u      /* one kernel per request; k_checksum_column + k_copy_image */
@@ -504,7 +508,9 @@ BGR_API int bgr_last_kernel(bgr_engine* e, uint32_t* kernel_out);
 BGR_API int bgr_synchronize(bgr_engine* e);
 BGR_API int bgr_stream(bgr_engine* e, void** stream_out);        /* the cudaStream_t the engine launches on (timing events) */
 /* device-side launch trace: 4 x u64 per fused launch after the call, up to `capacity` launches (GPU globaltimer ns):
- * [0] first block started, [1] last block finished its tiles, [2] results + completion word written, [3] reserved.
+ * [0] first block started, [1] last block finished its tiles, [2] results + completion word written, [3] bundle:
+ * 64-byte units of active planes the launch stored into slots and the live image (a word plane of 64 rows is 4 units,
+ * its alive plane 1).
  * bgr_trace_read copies the rows out (waits for the GPU).  capacity 0 disables. */
 BGR_API int bgr_trace_enable(bgr_engine* e, uint32_t capacity);
 BGR_API int bgr_trace_read(bgr_engine* e, uint64_t* rows_out, uint32_t cap_launches, uint32_t* n_out);

@@ -48,6 +48,8 @@ pub const BGR_KERNEL_DEFERRED_LIVE: u32 = 1 << 13;
 pub const BGR_KERNEL_FROM_DEFERRED: u32 = 1 << 14;
 /// bgr_last_kernel flag: the bundle launch read or wrote passive planes.
 pub const BGR_KERNEL_PASSIVE_PLANES: u32 = 1 << 15;
+/// bgr_last_kernel flag: the bundle launch stored only the active planes whose content the target did not hold.
+pub const BGR_KERNEL_STABLE_PLANES: u32 = 1 << 26;
 
 pub const BGR_CFG_FORCE_STEPWISE: u32 = 1;
 pub const BGR_CFG_SHARDED: u32 = 2;

@@ -8,8 +8,17 @@ active planes and bench.py's roofline figures are effective rates, not traffic. 
     bytes          = images touched x rows x (33 B active + 28 B passive when bgr_last_kernel reports passive planes)
 
 The passive planes are counted whenever the launch moved any (BGR_KERNEL_PASSIVE_PLANES), for every image touched: an
-upper bound on a tick after a version bump, where some Saves may still skip them.  In the same process it runs tools/hbm_mix_bench.cu's fan-out (1 read : 8 writes) over the
-active footprint, and prints the card's name and power limit.  One JSON line on stdout.
+upper bound on a tick after a version bump, where some Saves may still skip them.  tick_bytes() is that schema-level
+upper bound.  The bundle kernel also skips the active planes a slot already holds (content stamps,
+BGR_KERNEL_STABLE_PLANES); the launch trace counts the 64-byte units of active planes it stored (a word plane of a
+64-row segment is 4 units, its alive plane 1), and stored_bytes() turns that count into the bytes a tick actually moved:
+
+    stored bytes   = read image x rows x 33 B + stored units x 64 B + stamp traffic
+    stamp traffic  = (1 + Saves) x segments x 36 B read + one 4-byte stamp written per stored word plane-segment
+
+In the same process it runs tools/hbm_mix_bench.cu's fan-out (1 read : 8 writes) over the active footprint, and the
+same fan-out with the writes cut to the stored share, and prints the card's name and power limit.  One JSON line on
+stdout.
 
     python scripts/tick_bytes.py [--steps K] [--warmup W] [--entities N]
 """
@@ -29,6 +38,13 @@ sys.path.insert(0, ROOT)
 ACTIVE_BYTES = 12 + 12 + 8 + 1   # Transform.translation, Velocity, Ttl, alive byte: written by the tick's systems
 PASSIVE_BYTES = 16 + 12          # Transform.rotation, scale: no registered system writes them
 TILE_ROWS = 512
+SEG_ROWS = 64
+ACTIVE_PLANES = 9
+
+
+def stored_bytes(rows: int, n_saves: int, units: int) -> int:
+    segs = -(-rows // SEG_ROWS)
+    return rows * ACTIVE_BYTES + units * 64 + (1 + n_saves) * segs * ACTIVE_PLANES * 4 + units
 
 
 def images_touched(n_saves: int, deferred_live: bool) -> int:
@@ -45,13 +61,14 @@ def card():
     return q.stdout.strip().splitlines()[0] if q.returncode == 0 and q.stdout.strip() else None
 
 
-def fanout_ceiling(image_bytes: int, fan: int) -> dict:
+def fanout_ceiling(image_bytes: int, fan: int, write_bytes: int = 0) -> dict:
     nvcc = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
     with tempfile.TemporaryDirectory() as tmp:
         exe = os.path.join(tmp, "hbm_mix_bench")
         subprocess.run([nvcc, "-O3", "-gencode", "arch=compute_90a,code=sm_90a", "-o", exe,
                         os.path.join(ROOT, "tools", "hbm_mix_bench.cu")], check=True, capture_output=True)
-        r = subprocess.run([exe, str(image_bytes), str(fan)], check=True, capture_output=True, text=True)
+        r = subprocess.run([exe, str(image_bytes), str(fan)] + ([str(write_bytes)] if write_bytes else []),
+                           check=True, capture_output=True, text=True)
     return json.loads(r.stdout.strip().splitlines()[-1])
 
 
@@ -66,7 +83,7 @@ def main():
     n = args.entities or n
     K, W = args.steps, max(3, args.warmup)
     fill = max(d, maxp) + 2
-    ticks = bench.pregenerate_ticks(fill + W + 2 * K, d, maxp)
+    ticks = bench.pregenerate_ticks(fill + W + 2 * K + 2 * min(K, 256), d, maxp)
     steady_saves = len(ticks[-1][4])
     steady = tick_bytes(n, steady_saves, True, False)
     print(f"[tick_bytes] {n} entities, SyncTest d={d}: steady-state tick = {images_touched(steady_saves, True)} images x "
@@ -91,6 +108,13 @@ def main():
         k = eng.last_kernel()
         moved.append((tick_bytes(rows, len(t[4]), k.deferred_live, k.passive_planes), k.passive_planes))
 
+    def traced(leg_fn, tl, moved):
+        eng.trace_enable(len(tl))
+        leg_fn(tl, moved)
+        tr = eng.trace_read(len(tl))
+        eng.trace_enable(0)
+        return [(stored_bytes(rows, len(t[4]), int(r[3])), int(r[3]) * 64 // len(t[4])) for t, r in zip(tl, tr)]
+
     def pipelined(tl, moved):
         inflight = 0
         for t in tl:
@@ -105,6 +129,15 @@ def main():
 
     pipelined(take(fill + W), [])
     torch.cuda.synchronize()
+    # bytes actually stored, from the launch trace, in separate legs: the trace is off while the time is taken
+    stored_p = traced(pipelined, take(min(K, 256)), [])
+
+    def synchronous(tl, moved):
+        for t in tl:
+            submit(t, moved)
+            eng.collect()
+
+    stored_s = traced(synchronous, take(min(K, 256)), [])
     e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
     moved_p = []
     e0.record(stream)
@@ -121,17 +154,25 @@ def main():
     us_s = (time.perf_counter() - t0) * 1e6 / K
     eng.close()
 
-    fan = fanout_ceiling(ACTIVE_BYTES * (-(-n // TILE_ROWS) * TILE_ROWS), steady_saves)
+    image = ACTIVE_BYTES * (-(-n // TILE_ROWS) * TILE_ROWS)
+    fan = fanout_ceiling(image, steady_saves)
+    # the stored mix: each write carries the share of the image a steady-state Save stores
+    per_save = sorted(w for _, w in stored_p)[len(stored_p) // 2]   # data bytes one steady-state Save stores
+    fan_stored = fanout_ceiling(image, steady_saves, min(image, per_save) // 16 * 16)
 
-    def leg(us, moved):
+    def leg(us, moved, stored):
         b = sum(m for m, _ in moved) / len(moved)
+        s = sum(b for b, _ in stored) / len(stored)
         return {"us_per_tick": us, "frames_per_s": ticks[-1][2] / (us * 1e-6), "bytes_per_tick": b,
                 "ticks_with_passive_planes": sum(p for _, p in moved), "achieved_gbps": b / (us * 1e-6) / 1e9,
-                "frac_of_fanout_stg": b / (us * 1e-6) / 1e9 / fan["fanout_stg"]["gbps"]}
+                "frac_of_fanout_stg": b / (us * 1e-6) / 1e9 / fan["fanout_stg"]["gbps"],
+                "stored_bytes_per_tick": s, "stored_gbps": s / (us * 1e-6) / 1e9,
+                "frac_of_stored_mix_stg": s / (us * 1e-6) / 1e9 / fan_stored["fanout_stg"]["gbps"]}
 
     print(json.dumps({"card": card(), "torch_device": torch.cuda.get_device_name(0), "entities": n, "check_distance": d,
-                      "steps": K, "steady_state_bytes_per_tick": steady, "pipelined": leg(us_p, moved_p),
-                      "synchronous": leg(us_s, moved_s), "fanout_ceiling": fan}))
+                      "steps": K, "steady_state_bytes_per_tick": steady, "pipelined": leg(us_p, moved_p, stored_p),
+                      "synchronous": leg(us_s, moved_s, stored_s), "fanout_ceiling": fan,
+                      "stored_mix_ceiling": fan_stored}))
 
 
 if __name__ == "__main__":

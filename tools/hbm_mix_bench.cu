@@ -5,11 +5,14 @@
 //   fill      0 read : 1 write
 //   fanout    1 read : F writes  (plain stores)                       == the tick's mix: F = 8 Saves (live image deferred)
 //   fanout_tma 1 read : F writes (cp.async.bulk global->smem->global)
-// Usage: hbm_mix_bench [image_bytes] [F = 8 or 9].  Output: one JSON line.  Not part of the product; evidence for the roofline discussion in DESIGN.md.
+//   write_bytes (optional): fanout stores only the first write_bytes of each target, the mix of a tick whose Saves store
+//   part of the image (stable-plane elision: 33 B read : 8 x ~16 B written); copy, fill and fanout_tma stay whole-image.
+// Usage: hbm_mix_bench [image_bytes] [F = 8 or 9] [write_bytes].  Output: one JSON line.  Not part of the product; evidence for the roofline discussion in DESIGN.md.
 #include <cuda_runtime.h>
 #include <cstdint>
 #include <cstdio>
 #include <cstdlib>
+#include <algorithm>
 #include <vector>
 
 #define CK(x) do { cudaError_t e = (x); if (e != cudaSuccess) { printf("CUDA error %s at %d\n", cudaGetErrorString(e), __LINE__); exit(1); } } while (0)
@@ -24,12 +27,19 @@ __global__ void k_fill(uint4* __restrict__ dst, size_t n) {
         __stcs(dst + i, v);
 }
 template <int F>
-__global__ void k_fanout(const uint4* __restrict__ src, uint4* __restrict__ dst, size_t n, size_t stride) {
+__global__ void k_fanout(const uint4* __restrict__ src, uint4* __restrict__ dst, size_t n, size_t stride, size_t m,
+                         unsigned int* sink) {
+    unsigned int acc = 0;
     for (size_t i = size_t(blockIdx.x) * blockDim.x + threadIdx.x; i < n; i += size_t(gridDim.x) * blockDim.x) {
         uint4 v = __ldcs(src + i);
+        if (i < m) {
 #pragma unroll
-        for (int f = 0; f < F; ++f) __stcs(dst + f * stride + i, v);
+            for (int f = 0; f < F; ++f) __stcs(dst + f * stride + i, v);
+        } else {
+            acc ^= v.x ^ v.y ^ v.z ^ v.w;  // rows past write_bytes are read too: the load cannot sink into the branch
+        }
     }
+    if (acc == 0x9E3779B9u) *sink = acc;  // keeps the reads observable; practically never stores
 }
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return static_cast<uint32_t>(__cvta_generic_to_shared(p)); }
@@ -84,14 +94,16 @@ static double time_us(L launch, int iters) {
 }
 
 template <int F>
-static void run(size_t img) {
-    const size_t n = img / 16, stride_v = (img / 16 + 63) & ~size_t(63);
+static void run(size_t img, size_t write_bytes) {
+    const size_t n = img / 16, m = std::min(n, write_bytes / 16), stride_v = (img / 16 + 63) & ~size_t(63);
     uint8_t *src, *dst;
     // large source ring so reads are not served by L2: rotate over 8 source images
     const int NSRC = 8;
     CK(cudaMalloc(&src, stride_v * 16 * NSRC));
     CK(cudaMalloc(&dst, stride_v * 16 * (F + 1) * 2));
     CK(cudaMemset(src, 1, stride_v * 16 * NSRC));
+    unsigned int* sink;
+    CK(cudaMalloc(&sink, sizeof(unsigned int)));
     cudaDeviceProp prop; CK(cudaGetDeviceProperties(&prop, 0));
     const int sms = prop.multiProcessorCount;
     int it = 0;
@@ -100,22 +112,23 @@ static void run(size_t img) {
     const int iters = 50;
     double t_copy = time_us([&] { k_copy<<<sms * 8, 256>>>(srcp(), dstp(), n); }, iters);
     double t_fill = time_us([&] { k_fill<<<sms * 8, 256>>>(dstp(), n * F); }, iters);
-    double t_fan = time_us([&] { k_fanout<F><<<sms * 8, 256>>>(srcp(), dstp(), n, stride_v); }, iters);
+    double t_fan = time_us([&] { k_fanout<F><<<sms * 8, 256>>>(srcp(), dstp(), n, stride_v, m, sink); }, iters);
     const uint32_t chunk = 48 * 1024;
     CK(cudaFuncSetAttribute(k_fanout_tma<F>, cudaFuncAttributeMaxDynamicSharedMemorySize, int(2 * chunk)));
     double t_tma = time_us([&] { k_fanout_tma<F><<<sms * 2, 32, 2 * chunk>>>(reinterpret_cast<const uint8_t*>(srcp()), reinterpret_cast<uint8_t*>(dstp()), n * 16, stride_v * 16, chunk); }, iters);
     CK(cudaGetLastError());
-    printf("{\"image_bytes\": %zu, \"fanout\": %d, \"copy_1r1w\": {\"us\": %.2f, \"gbps\": %.0f}, \"fill_0r1w\": {\"us\": %.2f, \"gbps\": %.0f}, "
+    printf("{\"image_bytes\": %zu, \"write_bytes\": %zu, \"fanout\": %d, \"copy_1r1w\": {\"us\": %.2f, \"gbps\": %.0f}, \"fill_0r1w\": {\"us\": %.2f, \"gbps\": %.0f}, "
            "\"fanout_stg\": {\"us\": %.2f, \"gbps\": %.0f}, \"fanout_tma\": {\"us\": %.2f, \"gbps\": %.0f}}\n",
-           n * 16, F, t_copy, 2.0 * n * 16 / t_copy / 1e3, t_fill, double(F) * n * 16 / t_fill / 1e3,
-           t_fan, double(F + 1) * n * 16 / t_fan / 1e3, t_tma, double(F + 1) * n * 16 / t_tma / 1e3);
+           n * 16, m * 16, F, t_copy, 2.0 * n * 16 / t_copy / 1e3, t_fill, double(F) * n * 16 / t_fill / 1e3,
+           t_fan, (double(n) + double(F) * m) * 16 / t_fan / 1e3, t_tma, double(F + 1) * n * 16 / t_tma / 1e3);
 }
 
 int main(int argc, char** argv) {
     const size_t img = (argc > 1 ? size_t(atoll(argv[1])) : size_t(61) * 1000448);  // bytes of one image
     const int F = argc > 2 ? atoi(argv[2]) : 9;
-    if (F == 8) run<8>(img);
-    else if (F == 9) run<9>(img);
+    const size_t wb = argc > 3 ? size_t(atoll(argv[3])) : img;
+    if (F == 8) run<8>(img, wb);
+    else if (F == 9) run<9>(img, wb);
     else { fprintf(stderr, "fan-out must be 8 or 9\n"); return 2; }
     return 0;
 }
