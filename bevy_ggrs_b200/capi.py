@@ -60,6 +60,9 @@ BGR_KERNEL_FROM_DEFERRED = 1 << 14
 BGR_KERNEL_PASSIVE_PLANES = 1 << 15
 # ... and the bundle launch stored only the active planes whose content the target did not hold (grids of several waves)
 BGR_KERNEL_STABLE_PLANES = 1 << 26
+# change feed
+BGR_MAX_FEEDS = 8
+BGR_MAX_FEED_FIELDS = 8
 
 
 class bgr_request(C.Structure):
@@ -114,6 +117,14 @@ class bgr_frame_blob_header(C.Structure):
                 ("reserved", C.c_uint32), ("elapsed_ns", C.c_uint64), ("rng", C.c_uint64 * 4)]
 
 
+class bgr_feed_field(C.Structure):
+    _fields_ = [("column", C.c_uint32), ("byte_offset", C.c_uint32), ("byte_len", C.c_uint32)]
+
+
+class bgr_feed_info(C.Structure):
+    _fields_ = [("n_records", C.c_uint32), ("pending", C.c_uint32), ("rows", C.c_uint32), ("record_bytes", C.c_uint32)]
+
+
 u32p = C.POINTER(C.c_uint32)
 i32p = C.POINTER(C.c_int32)
 u64p = C.POINTER(C.c_uint64)
@@ -144,6 +155,10 @@ PROTOTYPES = {
     "bgr_host_free": (C.c_int, [C.c_void_p]),
     "bgr_download_begin": (C.c_int, [C.c_void_p, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, C.c_void_p, u32p]),
     "bgr_download_wait": (C.c_int, [C.c_void_p, C.c_uint32]),
+    "bgr_feed_create": (C.c_int, [C.c_void_p, C.POINTER(bgr_feed_field), C.c_uint32, u32p]),
+    "bgr_feed_reset": (C.c_int, [C.c_void_p, C.c_uint32]),
+    "bgr_feed_begin": (C.c_int, [C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, u32p]),
+    "bgr_feed_wait": (C.c_int, [C.c_void_p, C.c_uint32, C.POINTER(bgr_feed_info)]),
     "bgr_rollback_frame_count": (C.c_int, [C.c_void_p, i32p]),
     "bgr_set_rollback_frame_count": (C.c_int, [C.c_void_p, C.c_int32]),
     "bgr_confirmed_frame_count": (C.c_int, [C.c_void_p, i32p]),

@@ -28,6 +28,7 @@
 #include "tma_copy.cuh"
 #include "generic_program.cuh"
 #include "desync_diff.cuh"
+#include "change_feed.cuh"
 #include "frame_digest.cuh"
 #include "jit.hpp"
 
@@ -208,6 +209,19 @@ struct bgr_engine {
     Download dl[BGR_MAX_DOWNLOADS];
     cudaStream_t copy_stream = nullptr;
     uint32_t next_dl = 0;
+    // change feeds (bgr_feed_*, change_feed.cuh): reported state in HBM, both passes on the main stream, the records
+    // cross PCIe on copy_stream
+    struct Feed {
+        bool used = false, busy = false;
+        FeedParams p{};              // fields, rep, keep, rep_words, record_words and the scratch pointers
+        uint32_t bound = 0;          // no row at or past it has a reported state other than (0, zeros)
+        uint32_t ticket = 0;         // of the report in flight
+        uint32_t stage_records = 0;  // records p.out holds
+        unsigned int* h_info = nullptr;  // page-locked [4]: the info, copied behind the records
+        cudaEvent_t packed = nullptr, done = nullptr;
+    };
+    Feed feeds[BGR_MAX_FEEDS];
+    uint32_t feed_seq = 0;
 
     HostState st;
 
@@ -1316,6 +1330,145 @@ int download_wait(bgr_engine* e, uint32_t ticket) {
     return BGR_OK;
 }
 
+// ---- change feed (change_feed.cuh) ----
+int feed_create(bgr_engine* e, const bgr_feed_field* fields, uint32_t n_fields, uint32_t* feed_out) {
+    if (!e || !feed_out || (n_fields && !fields)) return fail(BGR_ERR_INVALID_ARGUMENT, "null argument");
+    if (!e->built) return fail(BGR_ERR_STATE, "bgr_feed_create before bgr_build");
+    if (n_fields > BGR_MAX_FEED_FIELDS) return fail(BGR_ERR_CAPACITY, "too many fields (BGR_MAX_FEED_FIELDS)");
+    uint32_t id = BGR_MAX_FEEDS;
+    for (uint32_t i = 0; i < BGR_MAX_FEEDS && id == BGR_MAX_FEEDS; ++i)
+        if (!e->feeds[i].used) id = i;
+    if (id == BGR_MAX_FEEDS) return fail(BGR_ERR_CAPACITY, "too many feeds (BGR_MAX_FEEDS)");
+    FeedParams p{};
+    p.keep = 1u;
+    for (uint32_t k = 0; k < n_fields; ++k) {
+        const bgr_feed_field& f = fields[k];
+        if (f.column >= e->cols.size()) return fail(BGR_ERR_INVALID_ARGUMENT, "unknown column");
+        const Column& c = e->cols[f.column];
+        if ((f.byte_offset & 3u) || (f.byte_len & 3u) || f.byte_len == 0 ||
+            uint64_t(f.byte_offset) + f.byte_len > uint64_t(c.words) * 4u)
+            return fail(BGR_ERR_INVALID_ARGUMENT, "field range must be 4-byte aligned and inside the element");
+        p.fields[k] = FeedField{c.first_plane + f.byte_offset / 4u, f.byte_len / 4u, c.absent, p.rep_words};
+        p.rep_words += f.byte_len / 4u;
+        p.keep |= c.absent;
+    }
+    p.n_fields = n_fields;
+    p.words = e->words;
+    p.record_words = 2u + p.rep_words;
+    bgr_engine::Feed& fd = e->feeds[id];
+    auto cleanup = [&]() {
+        cudaFree(fd.p.rep); cudaFree(fd.p.tile_count); cudaFree(fd.p.info);
+        if (fd.h_info) cudaFreeHost(fd.h_info);
+        if (fd.packed) cudaEventDestroy(fd.packed);
+        if (fd.done) cudaEventDestroy(fd.done);
+        fd = bgr_engine::Feed{};
+    };
+    fd.p = p;
+    const uint32_t tiles = e->n_tiles_cap;
+    cudaError_t ce = cudaMalloc(&fd.p.rep, size_t(tiles) * tile_bytes_of(p.rep_words));
+    if (ce == cudaSuccess) ce = cudaMalloc(&fd.p.tile_count, size_t(3) * tiles * sizeof(unsigned int));
+    if (ce == cudaSuccess) ce = cudaMalloc(&fd.p.info, 8 * sizeof(unsigned int));
+    if (ce == cudaSuccess) ce = cudaHostAlloc(&fd.h_info, 4 * sizeof(unsigned int), cudaHostAllocMapped);
+    if (ce == cudaSuccess) ce = cudaEventCreateWithFlags(&fd.packed, cudaEventDisableTiming);
+    if (ce == cudaSuccess) ce = cudaEventCreateWithFlags(&fd.done, cudaEventDisableTiming);
+    // the reported state starts as (0, zeros) on every row; ordered before any pass on the engine stream
+    if (ce == cudaSuccess) ce = cudaMemsetAsync(fd.p.rep, 0, size_t(tiles) * tile_bytes_of(p.rep_words), e->stream);
+    if (ce == cudaSuccess && !e->copy_stream) ce = cudaStreamCreateWithFlags(&e->copy_stream, cudaStreamNonBlocking);
+    if (ce != cudaSuccess) {
+        cleanup();
+        return fail(BGR_ERR_CUDA, std::string("bgr_feed_create: ") + cudaGetErrorString(ce));
+    }
+    fd.p.tile_off = fd.p.tile_count + tiles;
+    fd.p.tile_list = fd.p.tile_off + tiles;
+    fd.used = true;
+    e->tiledep_chain = false;
+    *feed_out = id;
+    return BGR_OK;
+}
+
+int feed_reset(bgr_engine* e, uint32_t feed) {
+    if (!e) return fail(BGR_ERR_INVALID_ARGUMENT, "null engine");
+    if (feed >= BGR_MAX_FEEDS || !e->feeds[feed].used) return fail(BGR_ERR_INVALID_ARGUMENT, "unknown feed");
+    bgr_engine::Feed& fd = e->feeds[feed];
+    // stream-ordered behind a report in flight, whose pass 2 is the last writer of the reported state
+    CUDA_TRY(cudaMemsetAsync(fd.p.rep, 0, size_t(e->tiles_for(fd.bound)) * tile_bytes_of(fd.p.rep_words), e->stream));
+    e->tiledep_chain = false;
+    fd.bound = 0;
+    return BGR_OK;
+}
+
+int feed_begin(bgr_engine* e, uint32_t feed, void* host, uint32_t cap, uint32_t* ticket_out) {
+    if (!e || !ticket_out || (cap && !host)) return fail(BGR_ERR_INVALID_ARGUMENT, "null argument");
+    if (!e->built) return fail(BGR_ERR_STATE, "engine not built");
+    if (feed >= BGR_MAX_FEEDS || !e->feeds[feed].used) return fail(BGR_ERR_INVALID_ARGUMENT, "unknown feed");
+    bgr_engine::Feed& fd = e->feeds[feed];
+    if (fd.busy) return fail(BGR_ERR_STATE, "a report of this feed is in flight");
+    uint32_t* host_dev = nullptr;
+    if (cap) {  // page-locked memory is mapped into the device address space (unified addressing)
+        cudaPointerAttributes a{};
+        if (cudaPointerGetAttributes(&a, host) != cudaSuccess || a.type != cudaMemoryTypeHost || !a.devicePointer) {
+            cudaGetLastError();
+            return fail(BGR_ERR_INVALID_ARGUMENT, "host_dst must come from bgr_host_alloc");
+        }
+        host_dev = static_cast<uint32_t*>(a.devicePointer);
+    }
+    // no report has more records than the rows it compares
+    const uint32_t cap_eff = std::min<uint64_t>(cap, uint64_t(e->n_tiles_cap) * kTileRows);
+    if (cap_eff > fd.stage_records) {  // grows to the largest cap and stays (no report of this feed is in flight)
+        if (fd.p.out) CUDA_TRY(cudaFree(fd.p.out));
+        fd.p.out = nullptr; fd.stage_records = 0;
+        CUDA_TRY(cudaMalloc(&fd.p.out, size_t(cap_eff) * fd.p.record_words * 4u));
+        fd.stage_records = cap_eff;
+    }
+    int rc = touch_live(e);  // stream-ordered behind the queued submits, like the passes below
+    if (rc != BGR_OK) return rc;
+    FeedParams p = fd.p;
+    p.img = e->image(0);
+    p.rows = e->st.n_rows;
+    p.n_tiles = e->tiles_for(std::max(p.rows, fd.bound));
+    p.cap = cap_eff;
+    if (p.n_tiles) {
+        k_feed_count<<<p.n_tiles, kFeedBlock, 0, e->stream>>>(p);
+        e->launches += 1;
+        CUDA_TRY(cudaGetLastError());
+    }
+    k_feed_scan<<<1, kFeedScanBlock, 0, e->stream>>>(p);
+    e->launches += 1;
+    CUDA_TRY(cudaGetLastError());
+    k_feed_records<<<std::max(1u, std::min(p.n_tiles, uint32_t(e->num_sms) * 4u)), kFeedBlock, 0, e->stream>>>(p);
+    e->launches += 1;
+    CUDA_TRY(cudaGetLastError());
+    e->tiledep_chain = false;
+    fd.bound = std::max(fd.bound, p.rows);
+    CUDA_TRY(cudaEventRecord(fd.packed, e->stream));
+    CUDA_TRY(cudaStreamWaitEvent(e->copy_stream, fd.packed, 0));
+    if (cap) {
+        k_feed_copy<<<std::max(1, e->num_sms), 256, 0, e->copy_stream>>>(p.out, p.info, host_dev);
+        e->launches += 1;
+        CUDA_TRY(cudaGetLastError());
+    }
+    CUDA_TRY(cudaMemcpyAsync(fd.h_info, p.info, 4 * sizeof(unsigned int), cudaMemcpyDeviceToHost, e->copy_stream));
+    CUDA_TRY(cudaEventRecord(fd.done, e->copy_stream));
+    fd.busy = true;
+    e->feed_seq = (e->feed_seq + 1u) & 0x0FFFFFFFu;
+    fd.ticket = feed + BGR_MAX_FEEDS * e->feed_seq;
+    *ticket_out = fd.ticket;
+    return BGR_OK;
+}
+
+int feed_wait(bgr_engine* e, uint32_t ticket, bgr_feed_info* info) {
+    if (!e) return fail(BGR_ERR_INVALID_ARGUMENT, "null engine");
+    bgr_engine::Feed& fd = e->feeds[ticket % BGR_MAX_FEEDS];
+    if (!fd.used || !fd.busy || fd.ticket != ticket) return fail(BGR_ERR_STATE, "no such feed report in flight");
+    CUDA_TRY(cudaEventSynchronize(fd.done));
+    fd.busy = false;
+    if (info) {
+        const volatile unsigned int* h = fd.h_info;
+        info->n_records = h[0]; info->pending = h[1]; info->rows = h[2]; info->record_bytes = h[3];
+    }
+    return BGR_OK;
+}
+
 void detect_bundles(bgr_engine* e) {
     e->bundle_particles = false;
     e->passive.clear();
@@ -1467,6 +1620,12 @@ BGR_API void bgr_engine_destroy(bgr_engine* e) {
         if (d.d_buf) cudaFree(d.d_buf);
         if (d.packed) cudaEventDestroy(d.packed);
         if (d.done) cudaEventDestroy(d.done);
+    }
+    for (auto& f : e->feeds) {
+        if (!f.used) continue;
+        cudaFree(f.p.rep); cudaFree(f.p.tile_count); cudaFree(f.p.info); cudaFree(f.p.out);
+        cudaFreeHost(f.h_info);
+        cudaEventDestroy(f.packed); cudaEventDestroy(f.done);
     }
     if (e->own_stream && e->stream) cudaStreamDestroy(e->stream);
     delete e;
@@ -1816,6 +1975,18 @@ BGR_API int bgr_download_begin(bgr_engine* e, uint32_t column, uint32_t byte_off
     return download_begin(e, column, byte_offset, byte_len, first_row, count, host_dst, ticket_out);
 }
 BGR_API int bgr_download_wait(bgr_engine* e, uint32_t ticket) { return download_wait(e, ticket); }
+BGR_API int bgr_feed_create(bgr_engine* e, const bgr_feed_field* fields, uint32_t n_fields, uint32_t* feed_out) {
+    return feed_create(e, fields, n_fields, feed_out);
+}
+BGR_API int bgr_feed_reset(bgr_engine* e, uint32_t feed) {
+    return feed_reset(e, feed);
+}
+BGR_API int bgr_feed_begin(bgr_engine* e, uint32_t feed, void* host_dst, uint32_t records_cap, uint32_t* ticket_out) {
+    return feed_begin(e, feed, host_dst, records_cap, ticket_out);
+}
+BGR_API int bgr_feed_wait(bgr_engine* e, uint32_t ticket, bgr_feed_info* info) {
+    return feed_wait(e, ticket, info);
+}
 
 BGR_API int bgr_read_alive(bgr_engine* e, uint32_t first_row, uint32_t count, uint8_t* host_dst) {
     if (!e || !e->built) return fail(BGR_ERR_STATE, "engine not built");

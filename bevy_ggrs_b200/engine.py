@@ -6,7 +6,7 @@ re-simulation all happen in the CUDA library.
 from __future__ import annotations
 
 import ctypes as C
-from typing import List, NamedTuple, Optional, Sequence, Tuple
+from typing import Dict, List, NamedTuple, Optional, Sequence, Tuple
 
 import numpy as np
 
@@ -47,6 +47,20 @@ class LastKernel(NamedTuple):
                           bool(v & capi.BGR_KERNEL_PASSIVE_PLANES), bool(v & capi.BGR_KERNEL_STABLE_PLANES))
 
 
+class FeedInfo(NamedTuple):
+    """bgr_feed_info: records written, differing rows left for the next report (cap), rows compared, bytes per record."""
+    n_records: int
+    pending: int
+    rows: int
+    record_bytes: int
+
+
+def feed_record_dtype(fields: Sequence[Tuple[int, int, int]]) -> np.dtype:
+    """A change-feed record: u32 row, u32 state (bit 0 exists, bit 1+k field k present), then field k's bytes as
+    ``f<k>``."""
+    return np.dtype([("row", "<u4"), ("state", "<u4")] + [(f"f{k}", np.uint8, (ln,)) for k, (_, _, ln) in enumerate(fields)])
+
+
 class Engine:
     def __init__(self, max_entities: int, max_depth: int = 9, fps: int = 60, device: int = 0, flags: int = 0,
                  order_base: int = 0, stream: Optional[int] = None):
@@ -61,6 +75,8 @@ class Engine:
         self.names: List[str] = []
         self.max_entities = max_entities
         self._pinned: List[C.c_void_p] = []
+        self._feed_dtypes: Dict[int, np.dtype] = {}
+        self._feed_tickets: Dict[int, Tuple[int, np.ndarray]] = {}
 
     # ---- plumbing ----
     def _check(self, status: int) -> None:
@@ -170,6 +186,45 @@ class Engine:
 
     def download_wait(self, ticket: int) -> None:
         self._check(self._lib.bgr_download_wait(self._h, ticket))
+
+    # ---- change feed (bgr_feed_*): the live rows whose existence, presence or tracked bytes changed ----
+    def feed_create(self, fields: Sequence[Tuple[int, int, int]]) -> int:
+        """A feed over ``fields`` = [(column, byte_offset, byte_len), ...]; its first report lists every existing row."""
+        fields = [tuple(int(x) for x in f) for f in fields]
+        arr = (capi.bgr_feed_field * max(1, len(fields)))(*[capi.bgr_feed_field(*f) for f in fields])
+        feed = C.c_uint32()
+        self._check(self._lib.bgr_feed_create(self._h, arr, len(fields), C.byref(feed)))
+        self._feed_dtypes[feed.value] = feed_record_dtype(fields)
+        return feed.value
+
+    def feed_reset(self, feed: int) -> None:
+        self._check(self._lib.bgr_feed_reset(self._h, feed))
+
+    def feed_record_dtype(self, feed: int) -> np.dtype:
+        return self._feed_dtypes[feed]
+
+    def feed_alloc(self, feed: int, cap: int) -> np.ndarray:
+        """Page-locked buffer for ``cap`` records of ``feed``; freed with the engine."""
+        return self.host_alloc(max(1, cap), self._feed_dtypes[feed].itemsize)
+
+    def feed_begin(self, feed: int, buf: np.ndarray, cap: int) -> int:
+        """Starts a report of at most ``cap`` records into ``buf`` (from feed_alloc); returns its ticket."""
+        assert buf.dtype == np.uint8 and buf.flags.c_contiguous and buf.size >= cap * self._feed_dtypes[feed].itemsize
+        t = C.c_uint32()
+        self._check(self._lib.bgr_feed_begin(self._h, feed, buf.ctypes.data, cap, C.byref(t)))
+        self._feed_tickets[t.value] = (feed, buf)
+        return t.value
+
+    def feed_wait(self, ticket: int) -> Tuple[np.ndarray, FeedInfo]:
+        """(records, info) of a report: a structured array (row, state, f0, f1, ...) copied out of the buffer."""
+        info = capi.bgr_feed_info()
+        self._check(self._lib.bgr_feed_wait(self._h, ticket, C.byref(info)))
+        feed, buf = self._feed_tickets.pop(ticket)
+        dt = self._feed_dtypes[feed]
+        assert info.record_bytes == dt.itemsize
+        recs = np.empty(info.n_records, dt)
+        C.memmove(recs.ctypes.data, buf.ctypes.data, info.n_records * dt.itemsize)  # only the records, not the buffer
+        return recs, FeedInfo(info.n_records, info.pending, info.rows, info.record_bytes)
 
     # ---- frame resources ----
     def rollback_frame_count(self) -> int:

@@ -25,6 +25,7 @@
 #include <optional>
 #include <stdexcept>
 #include <string>
+#include <type_traits>
 #include <typeindex>
 #include <typeinfo>
 #include <vector>
@@ -188,6 +189,44 @@ public:
         return ticket;
     }
     void download_wait(uint32_t ticket) { check(bgr_download_wait(engine_, ticket)); }
+    // change feed: only the rows whose existence, presence or tracked bytes changed since the last report
+    // (include/bevy_ggrs_b200.h "change feed"); `dst` from bgr_host_alloc, records_cap * record_bytes bytes
+    uint32_t feed_create(const std::vector<bgr_feed_field>& fields) {
+        uint32_t feed = 0;
+        check(bgr_feed_create(engine_, fields.data(), uint32_t(fields.size()), &feed));
+        return feed;
+    }
+    void feed_reset(uint32_t feed) { check(bgr_feed_reset(engine_, feed)); }
+    uint32_t feed_begin(uint32_t feed, void* dst, uint32_t records_cap) {
+        uint32_t ticket = 0;
+        check(bgr_feed_begin(engine_, feed, dst, records_cap, &ticket));
+        return ticket;
+    }
+    bgr_feed_info feed_wait(uint32_t ticket) {
+        bgr_feed_info info{};
+        check(bgr_feed_wait(engine_, ticket, &info));
+        return info;
+    }
+    // Applies the records of a feed whose field `field` is the whole of T to a row map: a record whose state has the
+    // field's bit inserts or updates the row's T, any other record (despawned, un-spawned, component removed) erases it.
+    // Rows that exist again after a rollback and rows spawned on the GPU come back as ordinary inserts.
+    template <class T, class Map>
+    static void apply_feed(const void* records, const bgr_feed_info& info, uint32_t field, uint32_t field_offset, Map& rows) {
+        static_assert(std::is_trivially_copyable<T>::value, "rollback components are POD");
+        const uint8_t* r = static_cast<const uint8_t*>(records);
+        for (uint32_t i = 0; i < info.n_records; ++i, r += info.record_bytes) {
+            uint32_t row = 0, state = 0;
+            std::memcpy(&row, r, 4);
+            std::memcpy(&state, r + 4, 4);
+            if (state & (2u << field)) {
+                T v;
+                std::memcpy(&v, r + 8 + field_offset, sizeof(T));
+                rows[row] = v;
+            } else {
+                rows.erase(row);
+            }
+        }
+    }
     // GgrsComponentSnapshots<T>::peek(frame) (mod.rs:233-240)
     template <class T> std::optional<std::vector<T>> peek(ggrs::Frame frame, uint32_t first_row, uint32_t count) {
         std::vector<T> v(count);

@@ -246,6 +246,41 @@ BGR_API int bgr_download_begin(bgr_engine* e, uint32_t column, uint32_t byte_off
                                uint32_t first_row, uint32_t count, void* host_dst, uint32_t* ticket_out);
 BGR_API int bgr_download_wait(bgr_engine* e, uint32_t ticket);
 
+/* ---- change feed: only the live rows that changed since the host was last told --------------------------------------
+ * A feed tracks up to BGR_MAX_FEED_FIELDS fields (bytes [byte_offset, byte_offset+byte_len) of `column`, both multiples
+ * of 4, inside the element) and keeps in HBM, per row, the state and field bytes it last reported; initially, and after
+ * bgr_feed_reset, every row is (state 0, zero bytes).  A report lists, in ascending row order, exactly the rows whose
+ * current (state, bytes) differs bit for bit from the reported one, and makes those the reported state.  A record is
+ * record_bytes = 8 + sum of byte_len bytes:
+ *   u32 row;
+ *   u32 state: bit 0 = the row exists (row < RollbackOrdered::len() and alive); bit 1+k = it exists and field k's column
+ *              is present (its absent bit is clear);
+ *   the bytes of every field in order, zero where the field is not present.
+ * Rows at or past the row count do not exist, whatever stale bytes image 0 holds there: rows a rollback un-spawned are
+ * reported with state 0.  When more than records_cap rows differ, the lowest records_cap are reported, `pending` counts
+ * the others and the next report picks them up: the records of capped reports concatenate to those of one uncapped
+ * report when nothing ran in between.
+ * bgr_feed_begin is ordered after every request vector submitted so far, materialises a deferred live image like
+ * bgr_download_begin, returns without waiting for the GPU and does not delay later submits: both passes run on the
+ * engine stream and only n_records * record_bytes cross PCIe, on a separate copy stream.  `host_dst` (records_cap *
+ * record_bytes bytes) must come from bgr_host_alloc and must not be read before bgr_feed_wait(ticket) returns.  One
+ * report per feed may be in flight (BGR_ERR_STATE otherwise).  Feeds are created after bgr_build (BGR_ERR_STATE before);
+ * a bad field is BGR_ERR_INVALID_ARGUMENT, too many feeds or fields BGR_ERR_CAPACITY; an unknown or already-waited
+ * ticket is BGR_ERR_STATE. */
+#define BGR_MAX_FEEDS 8u
+#define BGR_MAX_FEED_FIELDS 8u
+typedef struct bgr_feed_field { uint32_t column, byte_offset, byte_len; } bgr_feed_field;
+typedef struct bgr_feed_info {
+    uint32_t n_records;     /* records written, <= records_cap */
+    uint32_t pending;       /* rows that differed but were not reported because of the cap */
+    uint32_t rows;          /* RollbackOrdered::len() of the live world that was compared */
+    uint32_t record_bytes;  /* 8 + sum of byte_len */
+} bgr_feed_info;
+BGR_API int bgr_feed_create(bgr_engine* e, const bgr_feed_field* fields, uint32_t n_fields, uint32_t* feed_out);
+BGR_API int bgr_feed_reset(bgr_engine* e, uint32_t feed);  /* forget what was reported: the next report lists every existing row */
+BGR_API int bgr_feed_begin(bgr_engine* e, uint32_t feed, void* host_dst, uint32_t records_cap, uint32_t* ticket_out);
+BGR_API int bgr_feed_wait(bgr_engine* e, uint32_t ticket, bgr_feed_info* info);
+
 /* ---- frame resources (src/snapshot/mod.rs:66-77, lib.rs:116-117) ------------------------ */
 BGR_API int bgr_rollback_frame_count(bgr_engine* e, int32_t* out);
 BGR_API int bgr_set_rollback_frame_count(bgr_engine* e, int32_t frame);

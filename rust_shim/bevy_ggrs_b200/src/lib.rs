@@ -197,6 +197,61 @@ pub mod p2p_desync {
     }
 }
 
+/// Change feed: only the live rows whose existence, presence or tracked field bytes changed since the last report
+/// (`bgr_feed_*`; INTEGRATION.md "Per-tick mirror" applies the records to the ECS).
+pub mod change_feed {
+    use super::{check, engine, sys};
+    use bevy::prelude::World;
+
+    /// One record: the row, its state (bit 0 exists, bit 1+k field k present) and the bytes of every field, zero where
+    /// the field is not present.
+    pub struct Record<'a> { pub row: u32, pub state: u32, pub bytes: &'a [u8] }
+
+    /// A feed and its page-locked record buffer.  At most one report is in flight: `begin` then `wait`; `wait` before
+    /// dropping it, since the copy of a report in flight writes into the buffer.
+    pub struct ChangeFeed { id: u32, cap: u32, record_bytes: usize, buf: *mut u8, ticket: Option<u32>, info: sys::bgr_feed_info }
+
+    impl ChangeFeed {
+        /// A feed over `fields`, after the engine is built; its first report lists every existing row.
+        pub fn new(world: &World, fields: &[sys::bgr_feed_field], cap: u32) -> Self {
+            let mut id = 0u32;
+            check(unsafe { sys::bgr_feed_create(engine(world), fields.as_ptr(), fields.len() as u32, &mut id) });
+            let record_bytes = 8 + fields.iter().map(|f| f.byte_len as usize).sum::<usize>();
+            let mut buf = core::ptr::null_mut();
+            check(unsafe { sys::bgr_host_alloc(record_bytes * cap.max(1) as usize, &mut buf) });
+            ChangeFeed { id, cap, record_bytes, buf: buf.cast(), ticket: None, info: sys::bgr_feed_info::default() }
+        }
+
+        /// Forget what was reported: the next report lists every existing row.
+        pub fn reset(&mut self, world: &World) { check(unsafe { sys::bgr_feed_reset(engine(world), self.id) }); }
+
+        /// Starts a report ordered after the request vectors already submitted; returns at once.
+        pub fn begin(&mut self, world: &World) {
+            let mut t = 0u32;
+            check(unsafe { sys::bgr_feed_begin(engine(world), self.id, self.buf.cast(), self.cap, &mut t) });
+            self.ticket = Some(t);
+        }
+
+        /// Waits for the report in flight; returns its records, ascending by row, and how many rows the cap left over.
+        pub fn wait(&mut self, world: &World) -> (Vec<Record<'_>>, u32) {
+            if let Some(t) = self.ticket.take() {
+                check(unsafe { sys::bgr_feed_wait(engine(world), t, &mut self.info) });
+            }
+            let all = unsafe { core::slice::from_raw_parts(self.buf, self.info.n_records as usize * self.record_bytes) };
+            let recs = all.chunks_exact(self.record_bytes).map(|r| Record {
+                row: u32::from_le_bytes([r[0], r[1], r[2], r[3]]),
+                state: u32::from_le_bytes([r[4], r[5], r[6], r[7]]),
+                bytes: &r[8..],
+            }).collect();
+            (recs, self.info.pending)
+        }
+    }
+
+    impl Drop for ChangeFeed {
+        fn drop(&mut self) { unsafe { sys::bgr_host_free(self.buf.cast()); } }
+    }
+}
+
 // ------------------------------------------------------------------------------------------------------------------
 // RollbackApp — the reference's trait, same method names and signatures (rollback_app.rs:31-133, :135-248)
 // ------------------------------------------------------------------------------------------------------------------

@@ -63,6 +63,9 @@ pub use desync::*;
 // the P2P desync report structs (bgr_frame_digest_header / bgr_frame_blob_header) too
 mod p2p_desync;
 pub use p2p_desync::*;
+// the change feed structs (bgr_feed_field / bgr_feed_info) too
+mod change_feed;
+pub use change_feed::*;
 
 #[repr(C)]
 #[derive(Clone, Copy, Default)]
@@ -142,6 +145,10 @@ extern "C" {
     pub fn bgr_host_free(p: *mut c_void) -> c_int;
     pub fn bgr_download_begin(e: *mut bgr_engine, column: u32, byte_offset: u32, byte_len: u32, first_row: u32, count: u32, host_dst: *mut c_void, ticket_out: *mut u32) -> c_int;
     pub fn bgr_download_wait(e: *mut bgr_engine, ticket: u32) -> c_int;
+    pub fn bgr_feed_create(e: *mut bgr_engine, fields: *const bgr_feed_field, n_fields: u32, feed_out: *mut u32) -> c_int;
+    pub fn bgr_feed_reset(e: *mut bgr_engine, feed: u32) -> c_int;
+    pub fn bgr_feed_begin(e: *mut bgr_engine, feed: u32, host_dst: *mut c_void, records_cap: u32, ticket_out: *mut u32) -> c_int;
+    pub fn bgr_feed_wait(e: *mut bgr_engine, ticket: u32, info: *mut bgr_feed_info) -> c_int;
     pub fn bgr_rollback_frame_count(e: *mut bgr_engine, out: *mut i32) -> c_int;
     pub fn bgr_set_rollback_frame_count(e: *mut bgr_engine, frame: i32) -> c_int;
     pub fn bgr_confirmed_frame_count(e: *mut bgr_engine, out: *mut i32) -> c_int;
