@@ -45,6 +45,7 @@ BGR_CFG_FORCE_STEPWISE = 1
 BGR_CFG_SHARDED = 2
 BGR_CFG_SKIP_UNCHANGED_PLANES = 4
 BGR_CFG_DESYNC_CAPTURE = 8
+BGR_CFG_GROWABLE = 16
 BGR_DESYNC_NO_INDEX = 0xFFFFFFFF
 # P2P desync reports
 BGR_DIGEST_BLOCK_ROWS = 512
@@ -141,6 +142,8 @@ PROTOTYPES = {
     "bgr_add_system": (C.c_int, [C.c_void_p, C.c_uint32, u32p, C.c_uint32, u32p, C.c_uint32]),
     "bgr_build": (C.c_int, [C.c_void_p]),
     "bgr_run_startup_system": (C.c_int, [C.c_void_p, C.c_uint32]),
+    "bgr_reserve": (C.c_int, [C.c_void_p, C.c_uint32]),
+    "bgr_capacity": (C.c_int, [C.c_void_p, u32p, u32p]),
     "bgr_spawn": (C.c_int, [C.c_void_p, C.c_uint32, u32p]),
     "bgr_despawn": (C.c_int, [C.c_void_p, C.c_uint32]),
     "bgr_row_count": (C.c_int, [C.c_void_p, u32p]),

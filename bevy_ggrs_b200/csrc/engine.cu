@@ -31,6 +31,7 @@
 #include "change_feed.cuh"
 #include "frame_digest.cuh"
 #include "jit.hpp"
+#include "vmm_range.hpp"
 
 using namespace bgr;
 
@@ -115,6 +116,8 @@ struct HostState {  // trivially copyable: copying it per call must not allocate
     //     keeps the invariant.  A sharded engine keeps its own versions.
     //   - overlapping launches (PF_TILE_WAIT): elision only drops passive reads and stores, and a tick after a bump
     //     stages the passive planes exactly as every tick did before, so no launch reads what an earlier one writes.
+    //   - growth (BGR_CFG_GROWABLE, grow_to): maps new memory behind every image's bytes and zeroes it.  Every row it
+    //     writes is at or past every image's row count, so no version changes.
     //
     // Content stamps of the active planes (bgr_engine::d_stamps, engines that run the bundle kernel), the device-side
     // counterpart for the planes the systems write, decided per warp segment because it depends on the values:
@@ -135,6 +138,8 @@ struct HostState {  // trivially copyable: copying it per call must not allocate
     //     not use the bundle (use_bundle is fixed at bgr_build); those have no stamp table.
     //   - desync capture, retention, digests, export, bgr_reset_session and bgr_set_depth write no image bytes.  A
     //     sharded engine keeps its own table.
+    //   - growth maps the table's new segments behind every image's row and zeroes them (unknown); the stamps of the
+    //     segments that existed keep their positions and values, as the image bytes they name do.
     uint64_t live_passive_ver = 1, ver_counter = 1;
     std::array<uint64_t, SlotRing::kMaxSlots> slot_passive_ver{};  // 0 = never written
 };
@@ -219,6 +224,7 @@ struct bgr_engine {
         uint32_t stage_records = 0;  // records p.out holds
         unsigned int* h_info = nullptr;  // page-locked [4]: the info, copied behind the records
         cudaEvent_t packed = nullptr, done = nullptr;
+        StridedRange va_rep, va_count;   // growable engines: p.rep, and p.tile_count / tile_off / tile_list one stride each
     };
     Feed feeds[BGR_MAX_FEEDS];
     uint32_t feed_seq = 0;
@@ -331,9 +337,18 @@ struct bgr_engine {
     uint8_t* d_remote = nullptr;                   // tiles uploaded from a peer's export blob
     unsigned int* d_remote_visit = nullptr;        // [n_tiles_cap] the local tiles a remote diff visits
     uint32_t remote_cap_tiles = 0;                 // tiles d_remote holds
+    uint32_t diff_tiles = 0, digest_tiles = 0, visit_tiles = 0;  // tiles the scratch above was allocated for
+
+    // BGR_CFG_GROWABLE: cfg.max_entities, epad and n_tiles_cap are the current capacity, image_bytes (and stamp_image) the
+    // fixed stride of an image, sized for the ceiling.  Every buffer whose size follows the capacity and that a queued
+    // launch may use is a strided range (vmm_range.hpp) that grow_to maps further; none of their pointers ever changes.
+    uint32_t ceiling = 0;  // most rows the engine can hold (== the capacity without the flag)
+    StridedRange va_arena, va_stamps, va_kill, va_tile_done, va_tile_cnt, va_item_done;
 
     uint8_t* image(uint32_t idx) const { return arena + size_t(idx) * image_bytes; }
     bool capture() const { return cfg.flags & BGR_CFG_DESYNC_CAPTURE; }
+    bool growable() const { return cfg.flags & BGR_CFG_GROWABLE; }
+    uint32_t stamp_words() const { return n_tiles_cap * kSegsPerTile * kActivePlanes; }  // stamps of one image's rows
     // frame slots behind the live image
     uint32_t n_slots() const { return (capture() ? 2u * cfg.max_depth : cfg.max_depth) + retain_count; }
     uint32_t image_off256(uint32_t idx) const { return uint32_t((size_t(idx) * image_bytes) >> 8); }
@@ -351,7 +366,19 @@ namespace {
 // every launch that could still write them.
 int clear_stamps(bgr_engine* e, uint32_t idx) {
     if (!e->d_stamps) return BGR_OK;
-    CUDA_TRY(cudaMemsetAsync(e->d_stamps + size_t(idx) * e->stamp_image, 0, size_t(e->stamp_image) * sizeof(uint32_t), e->stream));
+    CUDA_TRY(cudaMemsetAsync(e->d_stamps + size_t(idx) * e->stamp_image, 0, size_t(e->stamp_words()) * sizeof(uint32_t), e->stream));
+    e->tiledep_chain = false;
+    return BGR_OK;
+}
+
+// The whole stamp table: one memset, or one per image row when the rows are strides of a growable engine.
+int clear_stamp_table(bgr_engine* e) {
+    const uint32_t images = e->n_slots() + 1u;
+    if (e->stamp_image == e->stamp_words())
+        CUDA_TRY(cudaMemsetAsync(e->d_stamps, 0, size_t(e->stamp_image) * images * sizeof(uint32_t), e->stream));
+    else
+        for (uint32_t i = 0; i < images; ++i)
+            CUDA_TRY(cudaMemsetAsync(e->d_stamps + size_t(i) * e->stamp_image, 0, size_t(e->stamp_words()) * sizeof(uint32_t), e->stream));
     e->tiledep_chain = false;
     return BGR_OK;
 }
@@ -365,6 +392,7 @@ struct Program {
     int32_t save_frames[kMaxSaves];
     uint32_t save_totals[kMaxSaves];
     uint32_t max_rows = 0, live_rows = 0;
+    uint64_t rows_needed = 0;        // BGR_CFG_GROWABLE: the capacity the spawns need, when more than the engine has
     bool has_load = false, has_advance = false, first_is_load = false, has_spawn = false;
     bool passive_to_slots = false;   // at least one SAVE must (re)write the passive planes
     bool passive_to_live = false;    // a LOAD changed the content of the live passive planes
@@ -481,8 +509,10 @@ int compile_requests(bgr_engine* e, HostState& s, const bgr_session_info* sess, 
                 if (pressed) {
                     const SystemReg& sy = e->systems[size_t(e->spawn_sys)];
                     const uint32_t rate = sy.params[0];
-                    if (uint64_t(s.n_rows) + rate > e->cfg.max_entities)
-                        return fail(BGR_ERR_CAPACITY, "spawn_particles exceeds max_entities");
+                    if (uint64_t(s.n_rows) + rate > e->cfg.max_entities) {
+                        if (!e->growable()) return fail(BGR_ERR_CAPACITY, "spawn_particles exceeds max_entities");
+                        pg.rows_needed = std::max(pg.rows_needed, uint64_t(s.n_rows) + rate);  // submit grows first
+                    }
                     if (pg.spawn_vals.size() + rate > kMaxSpawnVals)
                         return fail(BGR_ERR_CAPACITY, "too many particles spawned by one request vector");
                     op.flags |= OPF_SPAWN;
@@ -614,8 +644,8 @@ int run_fused(bgr_engine* e, const Program& pg, uint32_t buf) {
     // and before the first stamped launch after launches without stamps (they rewrote images behind the stamps' back;
     // a world changes sides only when its row count crosses the one-wave size)
     if (stamps && (e->stamps_stale || e->stamp_next > 0xFFFFFFFFu - uint32_t(kMaxOps + 1))) {
-        CUDA_TRY(cudaMemsetAsync(e->d_stamps, 0, size_t(e->stamp_image) * (e->n_slots() + 1u) * sizeof(uint32_t), e->stream));
-        e->tiledep_chain = false;
+        int rc = clear_stamp_table(e);
+        if (rc != BGR_OK) return rc;
         e->stamp_next = 1;
         e->stamps_stale = false;
     }
@@ -1054,6 +1084,69 @@ DeferredLive plan_deferral(Program& pg) {
     return d;
 }
 
+// BGR_CFG_GROWABLE: maps every capacity-sized range for `tiles` tiles and zeroes the new bytes on the stream, behind
+// every queued launch.  Either every range grows or none does.  host_ns spent mapping: [0] the arena, [1] the rest.
+int map_tiles(bgr_engine* e, uint64_t tiles, uint64_t* map_ns = nullptr) {
+    struct Step { StridedRange* r; size_t bytes; size_t old; };
+    std::vector<Step> steps;
+    auto add = [&](StridedRange& r, size_t bytes) { if (r.reserved()) steps.push_back({&r, bytes, r.mapped}); };
+    add(e->va_arena, tiles * e->tile_bytes);
+    add(e->va_stamps, tiles * kSegsPerTile * kActivePlanes * sizeof(uint32_t));
+    add(e->va_kill, tiles * kTileRows);
+    add(e->va_tile_done, (tiles + 1) * sizeof(unsigned int));
+    add(e->va_tile_cnt, (tiles + 1) * sizeof(unsigned int));
+    add(e->va_item_done, (4 * tiles + 4) * sizeof(unsigned int));
+    for (auto& fd : e->feeds)
+        if (fd.used) { add(fd.va_rep, tiles * tile_bytes_of(fd.p.rep_words)); add(fd.va_count, tiles * sizeof(unsigned int)); }
+    std::string err;
+    uint64_t t = host_ns();
+    for (size_t i = 0; i < steps.size(); ++i) {
+        if (!steps[i].r->map_to(steps[i].bytes, &err)) {
+            for (size_t k = 0; k < i; ++k) steps[k].r->shrink(steps[k].old);
+            return fail(BGR_ERR_CAPACITY, "growing to " + std::to_string(tiles * kTileRows) + " rows: " + err);
+        }
+        if (map_ns && i == 0) { const uint64_t u = host_ns(); map_ns[0] += u - t; t = u; }
+    }
+    if (map_ns) map_ns[1] += host_ns() - t;
+    for (const Step& s : steps) CUDA_TRY(s.r->zero_new(e->stream));
+    e->tiledep_chain = false;  // the next launch waits for the whole stream, the zeroing included
+    return BGR_OK;
+}
+
+// BGR_CFG_GROWABLE: capacity >= rows afterwards.  No byte moves, so compiled ops, queued launches, the deferred live
+// image, the slots with their passive versions and content stamps, and every feed's reported state stay valid.
+int grow_to(bgr_engine* e, uint64_t rows) {
+    if (rows <= e->cfg.max_entities) return BGR_OK;
+    if (rows > e->ceiling)
+        return fail(BGR_ERR_CAPACITY, std::to_string(rows) + " rows exceed the engine's ceiling of " + std::to_string(e->ceiling) +
+                                          " rows (BGR_CFG_GROWABLE)");
+    const uint64_t t0 = host_ns();
+    // max(rows needed, 2 x capacity) in whole tiles, plus the tiles the arena's mapping granularity pays for anyway
+    uint64_t tiles = (std::max<uint64_t>(rows, 2ull * e->cfg.max_entities) + kTileRows - 1) / kTileRows;
+    tiles = round_up(tiles * e->tile_bytes, e->va_arena.gran) / e->tile_bytes;
+    tiles = std::min<uint64_t>(tiles, e->ceiling / kTileRows);
+    uint64_t map_ns[2] = {0, 0};
+    int rc = map_tiles(e, tiles, map_ns);
+    if (rc != BGR_OK) return rc;
+    const bool verbose = std::getenv("BGR_GROW_VERBOSE") != nullptr;
+    const uint64_t t1 = host_ns();
+    if (verbose) CUDA_TRY(cudaStreamSynchronize(e->stream));  // the zeroing, timed (it is otherwise asynchronous)
+    const uint64_t t2 = host_ns();
+    const uint32_t old_cap = e->cfg.max_entities;
+    e->cfg.max_entities = uint32_t(tiles * kTileRows);
+    e->epad = e->cfg.max_entities;
+    e->n_tiles_cap = uint32_t(tiles);
+    // the registration's own kernel, compiled where bgr_build would have compiled it at this capacity
+    if (!e->jit.fn && e->tune_jit == 1 && old_cap < 16384 && e->cfg.max_entities >= 16384) jit_specialise(e);
+    const uint64_t t3 = host_ns();
+    if (verbose)
+        std::fprintf(stderr, "[bevy_ggrs_b200] grew %u -> %u rows: map arena %llu ns, map side tables %llu ns, zero %llu ns, "
+                             "jit %llu ns, total %llu ns\n", old_cap, e->cfg.max_entities, (unsigned long long)map_ns[0],
+                     (unsigned long long)map_ns[1], (unsigned long long)(t2 - t1), (unsigned long long)(t3 - t2),
+                     (unsigned long long)(t3 - t0));
+    return BGR_OK;
+}
+
 int submit(bgr_engine* e, const bgr_session_info* sess, const bgr_request* reqs, uint32_t n) {
     NvtxRange span("HandleRequests");
     if (!e) return fail(BGR_ERR_INVALID_ARGUMENT, "null engine");
@@ -1065,6 +1158,9 @@ int submit(bgr_engine* e, const bgr_session_info* sess, const bgr_request* reqs,
     Program pg;
     int rc = compile_requests(e, s, sess, reqs, n, pg);
     if (rc != BGR_OK) return rc;  // nothing executed, nothing committed
+    // the program does not depend on the capacity: growing behind the compile leaves it (and its ParticleRng draws) valid
+    if (pg.rows_needed) rc = grow_to(e, pg.rows_needed);
+    if (rc != BGR_OK) return rc;
     const uint64_t t_compiled = host_ns();
     uint32_t buf = e->next_buf;
     if (e->group) {
@@ -1357,7 +1453,9 @@ int feed_create(bgr_engine* e, const bgr_feed_field* fields, uint32_t n_fields, 
     p.record_words = 2u + p.rep_words;
     bgr_engine::Feed& fd = e->feeds[id];
     auto cleanup = [&]() {
-        cudaFree(fd.p.rep); cudaFree(fd.p.tile_count); cudaFree(fd.p.info);
+        if (fd.va_rep.reserved()) { cudaStreamSynchronize(e->stream); fd.va_rep.free(); fd.va_count.free(); }
+        else { cudaFree(fd.p.rep); cudaFree(fd.p.tile_count); }
+        cudaFree(fd.p.info);
         if (fd.h_info) cudaFreeHost(fd.h_info);
         if (fd.packed) cudaEventDestroy(fd.packed);
         if (fd.done) cudaEventDestroy(fd.done);
@@ -1365,8 +1463,26 @@ int feed_create(bgr_engine* e, const bgr_feed_field* fields, uint32_t n_fields, 
     };
     fd.p = p;
     const uint32_t tiles = e->n_tiles_cap;
-    cudaError_t ce = cudaMalloc(&fd.p.rep, size_t(tiles) * tile_bytes_of(p.rep_words));
-    if (ce == cudaSuccess) ce = cudaMalloc(&fd.p.tile_count, size_t(3) * tiles * sizeof(unsigned int));
+    cudaError_t ce = cudaSuccess;
+    size_t count_stride = tiles;  // words between tile_count, tile_off and tile_list
+    if (e->growable()) {  // reserved for the ceiling and grown with the engine (grow_to): the pointers never change
+        std::string err;
+        const uint64_t ceil_tiles = e->ceiling / kTileRows;
+        if (!fd.va_rep.reserve(e->cfg.device, 1, ceil_tiles * tile_bytes_of(p.rep_words), &err) ||
+            !fd.va_count.reserve(e->cfg.device, 3, ceil_tiles * sizeof(unsigned int), &err) ||
+            !fd.va_rep.map_to(size_t(tiles) * tile_bytes_of(p.rep_words), &err) || !fd.va_count.map_to(size_t(tiles) * sizeof(unsigned int), &err)) {
+            cleanup();
+            return fail(BGR_ERR_CUDA, "bgr_feed_create: " + err);
+        }
+        ce = fd.va_rep.zero_new(e->stream);
+        if (ce == cudaSuccess) ce = fd.va_count.zero_new(e->stream);
+        fd.p.rep = fd.va_rep.ptr();
+        fd.p.tile_count = fd.va_count.ptr<unsigned int>();
+        count_stride = fd.va_count.stride / sizeof(unsigned int);
+    } else {
+        ce = cudaMalloc(&fd.p.rep, size_t(tiles) * tile_bytes_of(p.rep_words));
+        if (ce == cudaSuccess) ce = cudaMalloc(&fd.p.tile_count, size_t(3) * tiles * sizeof(unsigned int));
+    }
     if (ce == cudaSuccess) ce = cudaMalloc(&fd.p.info, 8 * sizeof(unsigned int));
     if (ce == cudaSuccess) ce = cudaHostAlloc(&fd.h_info, 4 * sizeof(unsigned int), cudaHostAllocMapped);
     if (ce == cudaSuccess) ce = cudaEventCreateWithFlags(&fd.packed, cudaEventDisableTiming);
@@ -1378,8 +1494,8 @@ int feed_create(bgr_engine* e, const bgr_feed_field* fields, uint32_t n_fields, 
         cleanup();
         return fail(BGR_ERR_CUDA, std::string("bgr_feed_create: ") + cudaGetErrorString(ce));
     }
-    fd.p.tile_off = fd.p.tile_count + tiles;
-    fd.p.tile_list = fd.p.tile_off + tiles;
+    fd.p.tile_off = fd.p.tile_count + count_stride;
+    fd.p.tile_list = fd.p.tile_off + count_stride;
     fd.used = true;
     e->tiledep_chain = false;
     *feed_out = id;
@@ -1537,6 +1653,9 @@ BGR_API int bgr_engine_create(const bgr_config* cfg, bgr_engine** out) {
         if (cfg->max_depth > SlotRing::kMaxSlots / 2)
             return fail(BGR_ERR_INVALID_ARGUMENT, "BGR_CFG_DESYNC_CAPTURE needs max_depth <= 32 (2 * max_depth frame slots)");
     }
+    // a shard's rows are a fixed range of RollbackOrdered indices, and sharded engines do not spawn
+    if ((cfg->flags & BGR_CFG_GROWABLE) && ((cfg->flags & BGR_CFG_SHARDED) || cfg->order_base != 0))
+        return fail(BGR_ERR_UNSUPPORTED, "BGR_CFG_GROWABLE is not supported on a sharded engine (BGR_CFG_SHARDED / order_base != 0)");
     int n_dev = 0;
     cudaError_t ce = cudaGetDeviceCount(&n_dev);
     if (ce != cudaSuccess || n_dev == 0)
@@ -1589,6 +1708,13 @@ BGR_API void bgr_engine_destroy(bgr_engine* e) {
         e->group = nullptr;
     }
     if (e->d_trace) cudaFree(e->d_trace);
+    if (e->va_arena.reserved()) e->arena = nullptr;
+    if (e->va_stamps.reserved()) e->d_stamps = nullptr;
+    if (e->va_kill.reserved()) e->d_kill = nullptr;
+    if (e->va_tile_done.reserved()) e->d_tile_done = nullptr;
+    if (e->va_tile_cnt.reserved()) e->d_tile_cnt = nullptr;
+    if (e->va_item_done.reserved()) e->d_item_done = nullptr;
+    for (StridedRange* r : {&e->va_arena, &e->va_stamps, &e->va_kill, &e->va_tile_done, &e->va_tile_cnt, &e->va_item_done}) r->free();
     for (int i = 0; i < bgr_engine::kBufs; ++i) {
         if (e->h_out[i]) cudaFreeHost(e->h_out[i]);
         if (e->h_spawn[i]) cudaFreeHost(e->h_spawn[i]);
@@ -1623,7 +1749,9 @@ BGR_API void bgr_engine_destroy(bgr_engine* e) {
     }
     for (auto& f : e->feeds) {
         if (!f.used) continue;
-        cudaFree(f.p.rep); cudaFree(f.p.tile_count); cudaFree(f.p.info); cudaFree(f.p.out);
+        if (f.va_rep.reserved()) { f.va_rep.free(); f.va_count.free(); }
+        else { cudaFree(f.p.rep); cudaFree(f.p.tile_count); }
+        cudaFree(f.p.info); cudaFree(f.p.out);
         cudaFreeHost(f.h_info);
         cudaEventDestroy(f.packed); cudaEventDestroy(f.done);
     }
@@ -1752,11 +1880,34 @@ BGR_API int bgr_build(bgr_engine* e) {
                                                   std::to_string(SlotRing::kMaxSlots));
     if ((e->image_bytes * (size_t(e->n_slots()) + 1u)) >> 8 > 0xffffffffull)
         return fail(BGR_ERR_CAPACITY, "arena larger than 1 TB");
-    size_t total = e->image_bytes * (size_t(e->n_slots()) + 1u);
-    CUDA_TRY(cudaMalloc(&e->arena, total));
-    CUDA_TRY(cudaMemsetAsync(e->arena, 0, total, e->stream));
-    CUDA_TRY(cudaMalloc(&e->d_kill, e->epad));
-    CUDA_TRY(cudaMemsetAsync(e->d_kill, 0, e->epad, e->stream));
+    const uint32_t images = e->n_slots() + 1u;
+    e->ceiling = e->cfg.max_entities;
+    uint64_t ceil_tiles = e->n_tiles_cap;
+    std::string va_err;
+    if (e->growable()) {
+        // The ceiling: ops address images in 256-byte units with 32 bits, so all images together stay within 1 TB, and a
+        // row index is 32 bits.  Every image gets a stride of whole mapping granules sized for the ceiling.
+        const size_t gran = StridedRange::granularity(e->cfg.device, &va_err);
+        if (!gran) return fail(BGR_ERR_CUDA, va_err);
+        const uint64_t per_image = ((uint64_t(1) << 40) / images) / gran * gran;
+        ceil_tiles = std::min<uint64_t>(per_image / e->tile_bytes, 0xFFFFFFFFull / kTileRows);
+        if (ceil_tiles < e->n_tiles_cap)
+            return fail(BGR_ERR_CAPACITY, "max_entities exceeds the ceiling of a growable engine with this schema and slot count (" +
+                                              std::to_string(ceil_tiles * kTileRows) + " rows)");
+        e->ceiling = uint32_t(ceil_tiles * kTileRows);
+        if (!e->va_arena.reserve(e->cfg.device, images, ceil_tiles * e->tile_bytes, &va_err) ||
+            !e->va_kill.reserve(e->cfg.device, 1, ceil_tiles * kTileRows, &va_err))
+            return fail(BGR_ERR_CUDA, va_err);
+        e->image_bytes = e->va_arena.stride;
+        e->arena = e->va_arena.ptr();
+        e->d_kill = e->va_kill.ptr();
+    } else {
+        size_t total = e->image_bytes * (size_t(e->n_slots()) + 1u);
+        CUDA_TRY(cudaMalloc(&e->arena, total));
+        CUDA_TRY(cudaMemsetAsync(e->arena, 0, total, e->stream));
+        CUDA_TRY(cudaMalloc(&e->d_kill, e->epad));
+        CUDA_TRY(cudaMemsetAsync(e->d_kill, 0, e->epad, e->stream));
+    }
     const size_t acc_bytes = sizeof(unsigned long long) * kMaxSaves * kAccStride;
     CUDA_TRY(cudaMalloc(&e->d_accum, acc_bytes * bgr_engine::kBufs));
     CUDA_TRY(cudaMemsetAsync(e->d_accum, 0, acc_bytes * bgr_engine::kBufs, e->stream));
@@ -1766,7 +1917,13 @@ BGR_API int bgr_build(bgr_engine* e) {
         e->d_accum_set[s] = e->d_accum + size_t(s) * kMaxSaves * kAccStride;
         e->d_ticket_set[s] = e->d_ticket + 4 * s;
     }
-    if (e->tune_tiledep) {
+    if (e->tune_tiledep && e->growable()) {
+        if (!e->va_tile_done.reserve(e->cfg.device, 1, (ceil_tiles + 1) * sizeof(unsigned int), &va_err) ||
+            !e->va_tile_cnt.reserve(e->cfg.device, 1, (ceil_tiles + 1) * sizeof(unsigned int), &va_err))
+            return fail(BGR_ERR_CUDA, va_err);
+        e->d_tile_done = e->va_tile_done.ptr<unsigned int>();
+        e->d_tile_cnt = e->va_tile_cnt.ptr<unsigned int>();
+    } else if (e->tune_tiledep) {
         const size_t nt = size_t(e->tiles_for(e->cfg.max_entities)) + 1;
         CUDA_TRY(cudaMalloc(&e->d_tile_done, nt * sizeof(unsigned int)));
         CUDA_TRY(cudaMalloc(&e->d_tile_cnt, nt * sizeof(unsigned int)));
@@ -1793,7 +1950,12 @@ BGR_API int bgr_build(bgr_engine* e) {
         }
     build_specs(e);
     detect_bundles(e);
-    if (use_bundle(e)) {  // content stamps of the active planes: every image, every 64-row segment
+    if (use_bundle(e) && e->growable()) {  // one stride per image row of the table
+        if (!e->va_stamps.reserve(e->cfg.device, images, ceil_tiles * kSegsPerTile * kActivePlanes * sizeof(uint32_t), &va_err))
+            return fail(BGR_ERR_CUDA, va_err);
+        e->stamp_image = uint32_t(e->va_stamps.stride / sizeof(uint32_t));
+        e->d_stamps = e->va_stamps.ptr<uint32_t>();
+    } else if (use_bundle(e)) {  // content stamps of the active planes: every image, every 64-row segment
         e->stamp_image = e->n_tiles_cap * kSegsPerTile * kActivePlanes;
         const size_t bytes = size_t(e->stamp_image) * (e->n_slots() + 1u) * sizeof(uint32_t);
         CUDA_TRY(cudaMalloc(&e->d_stamps, bytes));
@@ -1803,7 +1965,11 @@ BGR_API int bgr_build(bgr_engine* e) {
     // path; the parameter block holds kMaxGenericSys systems; the tile fits twice per SM
     e->generic_ok = e->spawn_sys < 0 && e->sys_specs.size() <= size_t(kMaxGenericSys) && e->tile_bytes <= 100u * 1024u;
     jit_specialise(e);
-    if (e->jit.fn && e->tune_jit_tiledep) {
+    if (e->growable() && e->generic_ok && e->tune_jit_tiledep) {  // growth may compile the kernel later
+        if (!e->va_item_done.reserve(e->cfg.device, 1, (4 * ceil_tiles + 4) * sizeof(unsigned int), &va_err))
+            return fail(BGR_ERR_CUDA, va_err);
+        e->d_item_done = e->va_item_done.ptr<unsigned int>();
+    } else if (e->jit.fn && e->tune_jit_tiledep) {
         const size_t ni = size_t(e->tiles_for(e->cfg.max_entities)) * 4 + 4;
         CUDA_TRY(cudaMalloc(&e->d_item_done, ni * sizeof(unsigned int)));
         CUDA_TRY(cudaMemsetAsync(e->d_item_done, 0, ni * sizeof(unsigned int), e->stream));
@@ -1819,6 +1985,10 @@ BGR_API int bgr_build(bgr_engine* e) {
             CUDA_TRY(cudaMemsetAsync(e->d_tma_ticket, 0, 4 * sizeof(unsigned int), e->stream));
         }
     }
+    if (e->growable()) {
+        const int rc = map_tiles(e, e->n_tiles_cap);
+        if (rc != BGR_OK) return rc;
+    }
     CUDA_TRY(cudaStreamSynchronize(e->stream));
     e->built = true;
     return BGR_OK;
@@ -1833,7 +2003,11 @@ BGR_API int bgr_run_startup_system(bgr_engine* e, uint32_t system) {
     if (rc != BGR_OK) return rc;
     const SystemReg& sy = e->systems[size_t(e->spawn_sys)];
     const uint32_t rate = sy.params[0];
-    if (uint64_t(e->st.n_rows) + rate > e->cfg.max_entities) return fail(BGR_ERR_CAPACITY, "spawn_particles exceeds max_entities");
+    if (uint64_t(e->st.n_rows) + rate > e->cfg.max_entities) {
+        if (!e->growable()) return fail(BGR_ERR_CAPACITY, "spawn_particles exceeds max_entities");
+        rc = grow_to(e, uint64_t(e->st.n_rows) + rate);
+        if (rc != BGR_OK) return rc;
+    }
     for (uint32_t k = 0; k < rate; ++k) {
         e->h_spawn[0][k].x = e->st.rng.random_range(-200.0f, 200.0f);
         e->h_spawn[0][k].y = e->st.rng.random_range(-200.0f, 200.0f);
@@ -1857,10 +2031,12 @@ BGR_API int bgr_spawn(bgr_engine* e, uint32_t count, uint32_t* first_row_out) {
     int rc = drain(e);
     if (rc == BGR_OK) rc = touch_live(e);
     if (rc != BGR_OK) return rc;
-    if (uint64_t(e->st.n_rows) + count > e->cfg.max_entities) return fail(BGR_ERR_CAPACITY, "spawn exceeds max_entities");
+    if (uint64_t(e->st.n_rows) + count > e->cfg.max_entities && !e->growable()) return fail(BGR_ERR_CAPACITY, "spawn exceeds max_entities");
     if (count && e->ticked && ((e->cfg.flags & BGR_CFG_SHARDED) || e->cfg.order_base != 0))
         return fail(BGR_ERR_UNSUPPORTED, "bgr_spawn after the initial population is not supported on a sharded engine "
                                          "(the new rows' RollbackOrdered indices would collide with the next shard's range)");
+    rc = grow_to(e, uint64_t(e->st.n_rows) + count);
+    if (rc != BGR_OK) return rc;
     uint32_t first = e->st.n_rows;
     if (count) {
         k_spawn_rows<<<e->grid_for(count, 64), 256, 0, e->stream>>>(e->image(0), e->words, first, count);
@@ -1873,6 +2049,21 @@ BGR_API int bgr_spawn(bgr_engine* e, uint32_t count, uint32_t* first_row_out) {
     e->st.n_rows += count;
     e->st.live_passive_ver = ++e->st.ver_counter;
     if (first_row_out) *first_row_out = first;
+    return BGR_OK;
+}
+
+BGR_API int bgr_reserve(bgr_engine* e, uint32_t rows) {
+    if (!e || !e->built) return fail(BGR_ERR_STATE, "engine not built");
+    if (rows <= e->cfg.max_entities) return BGR_OK;
+    if (!e->growable()) return fail(BGR_ERR_UNSUPPORTED, "bgr_reserve past the capacity needs an engine created with BGR_CFG_GROWABLE");
+    return grow_to(e, rows);
+}
+
+BGR_API int bgr_capacity(bgr_engine* e, uint32_t* capacity_out, uint32_t* ceiling_out) {
+    if (!e || !capacity_out || !ceiling_out) return fail(BGR_ERR_INVALID_ARGUMENT, "null argument");
+    if (!e->built) return fail(BGR_ERR_STATE, "engine not built");
+    *capacity_out = e->cfg.max_entities;
+    *ceiling_out = e->ceiling;
     return BGR_OK;
 }
 
@@ -2095,9 +2286,15 @@ static int ensure_diff_scratch(bgr_engine* e, uint32_t records_cap) {
         // on the engine's (non-blocking) stream: ordered before the pass-1 launch that reads the table
         CUDA_TRY(cudaMemcpyAsync(e->d_diff_cols, dc.data(), sizeof(DiffColumn) * n_cols, cudaMemcpyHostToDevice, e->stream));
         CUDA_TRY(cudaStreamSynchronize(e->stream));  // `dc` is a pageable host vector that goes out of scope below
-        CUDA_TRY(cudaMalloc(&e->d_diff_counts, sizeof(unsigned int) * (3u * n_cols + e->n_tiles_cap)));
         CUDA_TRY(cudaMalloc(&e->d_diff_totals, sizeof(unsigned long long) * 3u));
+    }
+    if (e->diff_tiles < e->n_tiles_cap) {  // first use, or the capacity grew since (grow_to)
+        if (e->d_diff_counts) CUDA_TRY(cudaFree(e->d_diff_counts));
+        if (e->d_diff_list) CUDA_TRY(cudaFree(e->d_diff_list));
+        e->d_diff_counts = nullptr; e->d_diff_list = nullptr; e->diff_tiles = 0;
+        CUDA_TRY(cudaMalloc(&e->d_diff_counts, sizeof(unsigned int) * (3u * n_cols + e->n_tiles_cap)));
         CUDA_TRY(cudaMalloc(&e->d_diff_list, sizeof(unsigned int) * 2u * e->n_tiles_cap));
+        e->diff_tiles = e->n_tiles_cap;
     }
     if (records_cap > e->diff_records_cap) {
         if (e->d_diff_records) CUDA_TRY(cudaFree(e->d_diff_records));
@@ -2263,8 +2460,14 @@ BGR_API int bgr_frame_digest(bgr_engine* e, int32_t frame, bgr_frame_digest_head
         CUDA_TRY(cudaMalloc(&e->d_digest_cols, sizeof(DigestColumn) * std::max(1u, n_cols)));
         CUDA_TRY(cudaMemcpyAsync(e->d_digest_cols, dc.data(), sizeof(DigestColumn) * n_cols, cudaMemcpyHostToDevice, e->stream));
         CUDA_TRY(cudaStreamSynchronize(e->stream));  // `dc` goes out of scope below
+    }
+    if (e->digest_tiles < e->n_tiles_cap) {  // first use, or the capacity grew since (grow_to)
+        if (e->d_digest_words) CUDA_TRY(cudaFree(e->d_digest_words));
+        if (e->d_digest_active) CUDA_TRY(cudaFree(e->d_digest_active));
+        e->d_digest_words = nullptr; e->d_digest_active = nullptr; e->digest_tiles = 0;
         CUDA_TRY(cudaMalloc(&e->d_digest_words, sizeof(unsigned long long) * per * e->n_tiles_cap));
         CUDA_TRY(cudaMalloc(&e->d_digest_active, sizeof(unsigned int) * e->n_tiles_cap));
+        e->digest_tiles = e->n_tiles_cap;
     }
     const uint32_t rows = e->st.slot_rows[slot], n_blocks = e->tiles_for(rows);
     std::vector<uint64_t> w(size_t(n_blocks) * per);
@@ -2429,7 +2632,12 @@ BGR_API int bgr_desync_diff_remote(bgr_engine* e, int32_t frame, const void* blo
     // before loading, and words are only loaded for rows that exist on both sides).  Ascending, at most n_tiles_cap.
     for (uint32_t b = h.n_blocks; b < e->tiles_for(e->st.slot_rows[slot]); ++b) visit.push_back(b);
     const uint32_t n_visit = uint32_t(visit.size());
-    if (!e->d_remote_visit) CUDA_TRY(cudaMalloc(&e->d_remote_visit, sizeof(unsigned int) * e->n_tiles_cap));
+    if (e->visit_tiles < e->n_tiles_cap) {  // first use, or the capacity grew since (grow_to)
+        if (e->d_remote_visit) CUDA_TRY(cudaFree(e->d_remote_visit));
+        e->d_remote_visit = nullptr; e->visit_tiles = 0;
+        CUDA_TRY(cudaMalloc(&e->d_remote_visit, sizeof(unsigned int) * e->n_tiles_cap));
+        e->visit_tiles = e->n_tiles_cap;
+    }
     if (h.n_exported > e->remote_cap_tiles) {  // staging for the peer's tiles, grown on demand
         if (e->d_remote) CUDA_TRY(cudaFree(e->d_remote));
         e->d_remote = nullptr; e->remote_cap_tiles = 0;

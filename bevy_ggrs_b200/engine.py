@@ -119,6 +119,17 @@ class Engine:
     def run_startup_system(self, system: int) -> None:
         self._check(self._lib.bgr_run_startup_system(self._h, system))
 
+    # ---- capacity (flags=BGR_CFG_GROWABLE: row-creating calls grow it) ----
+    def reserve(self, rows: int) -> None:
+        """Capacity >= rows afterwards (BGR_CFG_GROWABLE engines; others only accept rows <= their capacity)."""
+        self._check(self._lib.bgr_reserve(self._h, rows))
+
+    def capacity(self) -> Tuple[int, int]:
+        """(rows held without growing, most rows the engine can ever hold)."""
+        cap, ceiling = C.c_uint32(), C.c_uint32()
+        self._check(self._lib.bgr_capacity(self._h, C.byref(cap), C.byref(ceiling)))
+        return cap.value, ceiling.value
+
     # ---- entities ----
     def spawn(self, count: int) -> int:
         first = C.c_uint32()
@@ -319,7 +330,7 @@ class Engine:
         h = capi.bgr_frame_digest_header()
         found = C.c_int32()
         per = len(self.elem_bytes) + 1
-        words = np.zeros(-(-self.max_entities // capi.BGR_DIGEST_BLOCK_ROWS) * per, np.uint64)  # any frame fits: one call
+        words = np.zeros(-(-self.capacity()[0] // capi.BGR_DIGEST_BLOCK_ROWS) * per, np.uint64)  # any frame fits: one call
         self._check(self._lib.bgr_frame_digest(self._h, frame, C.byref(h), words.ctypes.data, words.size, C.byref(found)))
         if not found.value:
             return None

@@ -164,6 +164,15 @@ public:
     // ---- World access ----
     const LocalPlayers& local_players() const { return local_players_; }
     uint32_t spawn(uint32_t count) { finish(); uint32_t first = 0; check(bgr_spawn(engine_, count, &first)); return first; }
+    // App(n, depth, device, BGR_CFG_GROWABLE): spawns grow the row capacity; reserve() grows it ahead of them
+    void reserve(uint32_t rows) { finish(); check(bgr_reserve(engine_, rows)); }
+    // {rows held without growing, most rows the engine can ever hold}
+    std::pair<uint32_t, uint32_t> capacity() {
+        finish();
+        uint32_t cap = 0, ceiling = 0;
+        check(bgr_capacity(engine_, &cap, &ceiling));
+        return {cap, ceiling};
+    }
     template <class T> void write(uint32_t first_row, const std::vector<T>& v) {
         finish();
         check(bgr_write_component(engine_, col<T>(), first_row, uint32_t(v.size()), v.data(), uint32_t(sizeof(T))));
@@ -323,7 +332,7 @@ public:
     FrameDigest frame_digest(ggrs::Frame frame) {
         finish();
         FrameDigest d;
-        d.words.resize(size_t((cfg_.max_entities + BGR_DIGEST_BLOCK_ROWS - 1) / BGR_DIGEST_BLOCK_ROWS) * (pending_cols_.size() + 1));
+        d.words.resize(size_t((capacity().first + BGR_DIGEST_BLOCK_ROWS - 1) / BGR_DIGEST_BLOCK_ROWS) * (pending_cols_.size() + 1));
         int32_t found = 0;
         check(bgr_frame_digest(engine_, frame, &d.header, d.words.data(), uint32_t(d.words.size()), &found));
         d.found = found != 0;

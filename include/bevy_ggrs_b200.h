@@ -157,7 +157,7 @@ typedef struct bgr_partial {
 typedef struct bgr_config {
     uint32_t abi_version;   /* BGR_ABI_VERSION */
     int32_t device;         /* CUDA ordinal */
-    uint32_t max_entities;  /* row capacity of this shard */
+    uint32_t max_entities;  /* row capacity of this shard; with BGR_CFG_GROWABLE the initial capacity (bgr_capacity) */
     uint32_t max_depth;     /* frame slots allocated in HBM; >= the largest MaxPredictionWindow used (+1 for SyncTest d == p-1 is not needed) */
     uint32_t fps;           /* RollbackFrameRate, time.rs:19-26 (default 60) */
     uint32_t flags;         /* BGR_CFG_* */
@@ -181,6 +181,16 @@ typedef struct bgr_config {
  * P2P rollbacks can.  Loads, checksums, bgr_peek, bgr_snapshot_frames and the kernels launched are unchanged.  Needs
  * max_depth <= 32; not with BGR_CFG_SHARDED. */
 #define BGR_CFG_DESYNC_CAPTURE 8u
+/* OPT-IN: max_entities is the initial capacity; row-creating calls grow it.  RollbackOrdered only ever appends
+ * (rollback.rs:66-83), so a spawning world grows for the whole session.  A request vector whose spawns do not fit,
+ * bgr_spawn, bgr_run_startup_system and bgr_reserve grow the capacity to max(rows needed, 2 x capacity), rounded up to
+ * whole 512-row tiles and to the memory mapping granularity and clamped to the ceiling.  bgr_build reserves virtual
+ * address space for the ceiling and maps memory for the capacity; growing maps more under every image and zeroes it, so
+ * no image moves, nothing in flight has to finish, and checksums, snapshots, feeds and desync reports are those of an
+ * engine created with the grown capacity.  Column writes never grow the capacity.  A call that needs more rows than
+ * the ceiling fails with BGR_ERR_CAPACITY and executes nothing.  Not with BGR_CFG_SHARDED or order_base != 0
+ * (BGR_ERR_UNSUPPORTED at bgr_engine_create). */
+#define BGR_CFG_GROWABLE 16u
 
 typedef struct bgr_engine bgr_engine;
 
@@ -205,6 +215,11 @@ BGR_API int bgr_build(bgr_engine* e);
 /* add_systems(Startup, system): run a registered GgrsSchedule system once, outside the rollback loop
  * (particles.rs:232 `add_systems(Startup, spawn_particles)` — the initial burst).  Only BGR_SYS_PARTICLES_SPAWN. */
 BGR_API int bgr_run_startup_system(bgr_engine* e, uint32_t system);
+/* Capacity >= rows on return (BGR_CFG_GROWABLE; after bgr_build).  At or below the capacity: no-op.  Above it on an
+ * engine without the flag: BGR_ERR_UNSUPPORTED; above the ceiling: BGR_ERR_CAPACITY, nothing changes. */
+BGR_API int bgr_reserve(bgr_engine* e, uint32_t rows);
+/* Rows the engine holds without growing, and the most it can ever hold (== capacity without BGR_CFG_GROWABLE). */
+BGR_API int bgr_capacity(bgr_engine* e, uint32_t* capacity_out, uint32_t* ceiling_out);
 
 /* ---- entity population (Rollback marker, src/snapshot/rollback.rs:23-94) ---------------- */
 /* `commands.spawn((..., Rollback))` x count: appends rows, RollbackOrdered index = order_base + row */

@@ -62,12 +62,14 @@ use bevy_ggrs::{
 // engine handle + status -> panic
 // ------------------------------------------------------------------------------------------------------------------
 /// Where the rollback columns live.  Insert before `GgrsPlugin`; defaults: 1M entities, 9 frame slots, device 0, no
-/// desync capture (`desync_capture: true` keeps every frame's first snapshot for [`desync_report`]; max_depth <= 32).
+/// desync capture (`desync_capture: true` keeps every frame's first snapshot for [`desync_report`]; max_depth <= 32), a
+/// fixed capacity (`growable: true` makes `max_entities` the initial capacity, which spawning grows, like
+/// `RollbackOrdered::push` without a bound).
 #[derive(Resource, Clone, Copy)]
 /// `retain_confirmed: (interval, count)` keeps the last `count` confirmed frames that are multiples of `interval` (the
 /// session's `DesyncDetection::On { interval }`) for [`p2p_desync`]; count 0 keeps none.
-pub struct B200Config { pub max_entities: u32, pub max_depth: u32, pub device: i32, pub desync_capture: bool, pub retain_confirmed: (u32, u32) }
-impl Default for B200Config { fn default() -> Self { Self { max_entities: 1 << 20, max_depth: 9, device: 0, desync_capture: false, retain_confirmed: (0, 0) } } }
+pub struct B200Config { pub max_entities: u32, pub max_depth: u32, pub device: i32, pub desync_capture: bool, pub retain_confirmed: (u32, u32), pub growable: bool }
+impl Default for B200Config { fn default() -> Self { Self { max_entities: 1 << 20, max_depth: 9, device: 0, desync_capture: false, retain_confirmed: (0, 0), growable: false } } }
 
 /// The engine handle, a non-send resource (one caller thread, like the exclusive system that owns the World,
 /// schedule_systems.rs:19,170).
@@ -334,7 +336,7 @@ impl<C: Config<Input = u8>> Plugin for GgrsPlugin<C> {
         let cfg = app.world().get_resource::<B200Config>().copied().unwrap_or_default();
         let fps = app.world().get_resource::<RollbackFrameRate>().map(|r| **r as u32).unwrap_or(60);
         let c = sys::bgr_config { abi_version: sys::BGR_ABI_VERSION, device: cfg.device, max_entities: cfg.max_entities, max_depth: cfg.max_depth,
-                                  fps, flags: if cfg.desync_capture { sys::BGR_CFG_DESYNC_CAPTURE } else { 0 }, order_base: 0, stream: core::ptr::null_mut() };
+                                  fps, flags: (if cfg.desync_capture { sys::BGR_CFG_DESYNC_CAPTURE } else { 0 }) | (if cfg.growable { sys::BGR_CFG_GROWABLE } else { 0 }), order_base: 0, stream: core::ptr::null_mut() };
         let mut raw = core::ptr::null_mut();
         check(unsafe { sys::bgr_engine_create(&c, &mut raw) });
         if cfg.retain_confirmed.1 > 0 {

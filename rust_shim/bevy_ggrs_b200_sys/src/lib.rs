@@ -55,6 +55,8 @@ pub const BGR_CFG_FORCE_STEPWISE: u32 = 1;
 pub const BGR_CFG_SHARDED: u32 = 2;
 pub const BGR_CFG_SKIP_UNCHANGED_PLANES: u32 = 4;
 pub const BGR_CFG_DESYNC_CAPTURE: u32 = 8;
+/// max_entities is the initial capacity; row-creating calls grow it (bgr_reserve / bgr_capacity)
+pub const BGR_CFG_GROWABLE: u32 = 16;
 pub const BGR_DESYNC_NO_INDEX: u32 = 0xFFFFFFFF;
 
 // the desync capture structs (bgr_desync_column / _record / _summary) live in their own module
@@ -131,6 +133,8 @@ extern "C" {
     pub fn bgr_add_system(e: *mut bgr_engine, system: u32, columns: *const u32, n_columns: u32, params: *const u32, n_params: u32) -> c_int;
     pub fn bgr_build(e: *mut bgr_engine) -> c_int;
     pub fn bgr_run_startup_system(e: *mut bgr_engine, system: u32) -> c_int;
+    pub fn bgr_reserve(e: *mut bgr_engine, rows: u32) -> c_int;
+    pub fn bgr_capacity(e: *mut bgr_engine, capacity_out: *mut u32, ceiling_out: *mut u32) -> c_int;
     pub fn bgr_spawn(e: *mut bgr_engine, count: u32, first_row_out: *mut u32) -> c_int;
     pub fn bgr_despawn(e: *mut bgr_engine, row: u32) -> c_int;
     pub fn bgr_row_count(e: *mut bgr_engine, rows_out: *mut u32) -> c_int;
