@@ -1692,6 +1692,9 @@ BGR_API int bgr_engine_create(const bgr_config* cfg, bgr_engine** out) {
     e->tune_stagger_ns = env_int("BGR_TUNE_STAGGER_NS", 800);
     e->tune_bundle = env_int("BGR_TUNE_BUNDLE", 1);
     e->tune_defer_live = env_int("BGR_TUNE_DEFER_LIVE", 1);
+    // tests: the first content stamp issued, so that the range rollover in run_fused is reached within a few launches
+    if (const char* v = std::getenv("BGR_TEST_STAMP_FIRST"); v && *v)
+        e->stamp_next = uint32_t(std::max(1ul, std::min(std::strtoul(v, nullptr, 0), 0xFFFFFFFFul)));
     e->st.confirmed = 0;
     *out = e;
     return BGR_OK;
