@@ -64,6 +64,8 @@ BGR_KERNEL_STABLE_PLANES = 1 << 26
 # change feed
 BGR_MAX_FEEDS = 8
 BGR_MAX_FEED_FIELDS = 8
+# host edits (bgr_edit.kind)
+BGR_EDIT_WRITE, BGR_EDIT_INSERT, BGR_EDIT_REMOVE, BGR_EDIT_DESPAWN, BGR_EDIT_SPAWN = range(5)
 
 
 class bgr_request(C.Structure):
@@ -126,6 +128,11 @@ class bgr_feed_info(C.Structure):
     _fields_ = [("n_records", C.c_uint32), ("pending", C.c_uint32), ("rows", C.c_uint32), ("record_bytes", C.c_uint32)]
 
 
+class bgr_edit(C.Structure):
+    _fields_ = [("kind", C.c_uint32), ("column", C.c_uint32), ("row", C.c_uint32), ("count", C.c_uint32),
+                ("byte_offset", C.c_uint32), ("byte_len", C.c_uint32), ("value_offset", C.c_uint32), ("reserved", C.c_uint32)]
+
+
 u32p = C.POINTER(C.c_uint32)
 i32p = C.POINTER(C.c_int32)
 u64p = C.POINTER(C.c_uint64)
@@ -154,6 +161,7 @@ PROTOTYPES = {
     "bgr_remove_component": (C.c_int, [C.c_void_p, C.c_uint32, C.c_uint32]),
     "bgr_insert_component": (C.c_int, [C.c_void_p, C.c_uint32, C.c_uint32, C.c_void_p]),
     "bgr_has_component": (C.c_int, [C.c_void_p, C.c_uint32, C.c_uint32, C.c_uint32, C.c_void_p]),
+    "bgr_apply_edits": (C.c_int, [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_size_t]),
     "bgr_host_alloc": (C.c_int, [C.c_size_t, C.POINTER(C.c_void_p)]),
     "bgr_host_free": (C.c_int, [C.c_void_p]),
     "bgr_download_begin": (C.c_int, [C.c_void_p, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, C.c_void_p, u32p]),

@@ -17,6 +17,7 @@
 #include <cstring>
 #include <deque>
 #include <string>
+#include <unordered_map>
 #include <vector>
 
 #include "../../include/bevy_ggrs_b200.h"
@@ -110,6 +111,10 @@ struct HostState {  // trivially copyable: copying it per call must not allocate
     //   - host writes of image 0 bump: transfer_column to the device (bgr_write_component, bgr_insert_component),
     //     bgr_spawn, bgr_run_startup_system, bgr_remove_component.  bgr_despawn writes only the alive byte, an active
     //     plane.  bgr_reset_session, bgr_set_depth and bgr_confirm move no bytes; slots keep bytes and versions.
+    //   - bgr_apply_edits (host edits) writes image 0 and bumps only when the batch changes passive bytes or row count:
+    //     a WRITE with a word on a passive plane, and every SPAWN, INSERT and REMOVE (what their single calls do).  A
+    //     DESPAWN writes the mask byte and a WRITE confined to active planes writes only active words: every slot's
+    //     passive bytes still equal the live image's, so a matching version stays true.
     //   - slots are written only by Saves; desync capture and retention hand a slot index out again with its
     //     bytes, and the version is per slot index.
     //   - the stepwise path, the interpreter and k_generic_jit ignore OPF_SKIP_PASSIVE and store whole images, which
@@ -132,6 +137,9 @@ struct HostState {  // trivially copyable: copying it per call must not allocate
     //   - every other writer of an image clears that image's stamps (clear_stamps): transfer_column to the device
     //     (bgr_write_component, bgr_insert_component), bgr_spawn, bgr_run_startup_system, bgr_remove_component,
     //     bgr_insert_component's presence bit, and bgr_despawn (the alive byte is an active plane).
+    //   - bgr_apply_edits clears only image 0's stamps of the (segment, plane) pairs its patch writes, in the same launch,
+    //     behind every queued vector: an active word's plane, the mask byte's plane (q = 8) for presence and despawn
+    //     records, every plane of the segments a spawn's rows fall in.  Every other stamp names bytes it did not touch.
     //   - the deferred live image is materialised by the bundle kernel itself; while it is pending, image 0 keeps the
     //     bytes and the stamps of its last write.
     //   - the stepwise path (k_image_tma, k_copy_image), the interpreter and k_generic_jit only run on engines that do
@@ -142,6 +150,23 @@ struct HostState {  // trivially copyable: copying it per call must not allocate
     //     segments that existed keep their positions and values, as the image bytes they name do.
     uint64_t live_passive_ver = 1, ver_counter = 1;
     std::array<uint64_t, SlotRing::kMaxSlots> slot_passive_ver{};  // 0 = never written
+};
+
+// The patch k_apply_edits applies (kernels.cuh EditPatch), folded on the host from a validated batch.  The engine keeps
+// one across calls: a batch of thousands of rows allocated (and page-faulted) a megabyte of fresh memory otherwise.
+struct EditFold {
+    struct Word { uint64_t key; uint32_t row, plane, value; };  // key: the word's offset in image 0 / 4
+    std::vector<Word> words, sorted;
+    std::vector<uint2> masks;                // (row, and | or << 8 | despawn << 16)
+    std::vector<uint32_t> stamps;
+    std::unordered_map<uint32_t, uint32_t> mask_of;  // row -> index into masks
+    bool bump = false;                       // the live passive version moves (HostState)
+    // per word plane, fixed at bgr_build and filled by the first batch: its content-stamp plane (kernels.cuh:
+    // translation, velocity, ttl; the mask byte is q = 8; -1 passive; empty without a stamp table) and whether it is
+    // a passive plane
+    std::vector<int8_t> stamp_q;
+    std::vector<uint8_t> passive;
+    void clear() { words.clear(); masks.clear(); stamps.clear(); mask_of.clear(); bump = false; }
 };
 
 struct Pending {
@@ -228,6 +253,12 @@ struct bgr_engine {
     };
     Feed feeds[BGR_MAX_FEEDS];
     uint32_t feed_seq = 0;
+    // host edits (bgr_apply_edits): page-locked patches the kernel reads in place, reused once their launch finished
+    struct EditStage { uint8_t* h = nullptr; size_t cap = 0; cudaEvent_t done = nullptr; bool busy = false; };
+    static constexpr int kEditBufs = 4;
+    EditStage edit_stage[kEditBufs];
+    uint32_t next_edit = 0;
+    EditFold edit_fold;
 
     HostState st;
 
@@ -1585,6 +1616,231 @@ int feed_wait(bgr_engine* e, uint32_t ticket, bgr_feed_info* info) {
     return BGR_OK;
 }
 
+// ---- host edits (bgr_apply_edits) ----
+int edit_fail(uint32_t i, int status, const std::string& text) { return fail(status, "edit " + std::to_string(i) + ": " + text); }
+
+// Checks the whole batch against the row count each record sees; returns the row count after it.
+int validate_edits(bgr_engine* e, const bgr_edit* edits, uint32_t n, size_t values_bytes, uint64_t* rows_out) {
+    uint64_t rows = e->st.n_rows;
+    for (uint32_t i = 0; i < n; ++i) {
+        const bgr_edit& d = edits[i];
+        const bool has_col = d.kind == BGR_EDIT_WRITE || d.kind == BGR_EDIT_INSERT || d.kind == BGR_EDIT_REMOVE;
+        if (d.kind > BGR_EDIT_SPAWN) return edit_fail(i, BGR_ERR_INVALID_ARGUMENT, "unknown edit kind");
+        if (has_col && d.column >= e->cols.size()) return edit_fail(i, BGR_ERR_INVALID_ARGUMENT, "unknown column");
+        const Column* c = has_col ? &e->cols[d.column] : nullptr;
+        if ((d.kind == BGR_EDIT_INSERT || d.kind == BGR_EDIT_REMOVE) && !c->absent)
+            return edit_fail(i, BGR_ERR_INVALID_ARGUMENT, "column was not registered with BGR_STRATEGY_OPTIONAL");
+        switch (d.kind) {
+        case BGR_EDIT_WRITE: {
+            const uint64_t end = uint64_t(d.byte_offset) + d.byte_len;
+            if ((d.byte_offset & 3u) || d.byte_len == 0 || end > c->elem_bytes || ((d.byte_len & 3u) && end != c->elem_bytes))
+                return edit_fail(i, BGR_ERR_INVALID_ARGUMENT, "field range must be 4-byte aligned and inside the element, "
+                                                              "its length a multiple of 4 or ending at the element's end");
+            if (uint64_t(d.row) + d.count > rows) return edit_fail(i, BGR_ERR_INVALID_ARGUMENT, "row range exceeds the spawned rows");
+            if (uint64_t(d.value_offset) + uint64_t(d.count) * d.byte_len > values_bytes)
+                return edit_fail(i, BGR_ERR_INVALID_ARGUMENT, "values range exceeds values_bytes");
+            break;
+        }
+        case BGR_EDIT_INSERT:
+            if (uint64_t(d.value_offset) + c->elem_bytes > values_bytes)
+                return edit_fail(i, BGR_ERR_INVALID_ARGUMENT, "values range exceeds values_bytes");
+            [[fallthrough]];
+        case BGR_EDIT_REMOVE:
+        case BGR_EDIT_DESPAWN:
+            if (d.row >= rows) return edit_fail(i, BGR_ERR_INVALID_ARGUMENT, "row out of range");
+            break;
+        case BGR_EDIT_SPAWN:
+            rows += d.count;
+            break;
+        }
+    }
+    const uint64_t spawned = rows - e->st.n_rows;
+    if (spawned) {
+        if (rows > e->cfg.max_entities && !e->growable()) return fail(BGR_ERR_CAPACITY, "spawn exceeds max_entities");
+        if (rows > 0xFFFFFFFFull) return fail(BGR_ERR_CAPACITY, "spawn exceeds the row index range");
+        if (e->ticked && ((e->cfg.flags & BGR_CFG_SHARDED) || e->cfg.order_base != 0))
+            return fail(BGR_ERR_UNSUPPORTED, "spawning after the initial population is not supported on a sharded engine "
+                                             "(the new rows' RollbackOrdered indices would collide with the next shard's range)");
+    }
+    *rows_out = rows;
+    return BGR_OK;
+}
+
+int fold_edits(bgr_engine* e, const bgr_edit* edits, uint32_t n, const uint8_t* values, EditFold& f) {
+    if (f.passive.size() != e->words) {
+        if (e->d_stamps) {
+            f.stamp_q.assign(e->words, -1);
+            for (uint32_t k = 0; k < 3; ++k) {
+                f.stamp_q[e->cols[e->bt].first_plane + k] = int8_t(k);
+                f.stamp_q[e->cols[e->bv].first_plane + k] = int8_t(3 + k);
+            }
+            for (uint32_t k = 0; k < 2; ++k) f.stamp_q[e->cols[e->bl].first_plane + k] = int8_t(6 + k);
+        }
+        f.passive.assign(e->words, 0);
+        for (uint16_t p : e->passive) f.passive[p] = 1;
+    }
+    const std::vector<int8_t>& stamp_q = f.stamp_q;
+    const std::vector<uint8_t>& passive = f.passive;
+    auto stamp = [&](uint32_t row, uint32_t q) { f.stamps.push_back((row / kSegRows) * kActivePlanes + q); };
+    auto word = [&](uint32_t row, uint32_t plane, uint32_t value) {
+        f.words.push_back({word_offset(e->words, row, plane) / 4u, row, plane, value});
+        if (passive[plane]) f.bump = true;
+    };
+    size_t n_words = 0;
+    for (uint32_t i = 0; i < n; ++i) {
+        const bgr_edit& d = edits[i];
+        if (d.kind == BGR_EDIT_WRITE) n_words += size_t(d.count) * ((d.byte_offset + d.byte_len + 3u) / 4u - d.byte_offset / 4u);
+        if (d.kind == BGR_EDIT_INSERT) n_words += e->cols[d.column].words;
+    }
+    f.words.reserve(n_words);
+    // little-endian word `w` of an element whose bytes [lo, hi) come from `src` (src[0] is byte lo); other bytes 0
+    auto pack = [](const uint8_t* src, uint32_t lo, uint32_t hi, uint32_t w) {
+        uint32_t v = 0;
+        if (4u * w + 4u <= hi) { std::memcpy(&v, src + (4u * w - lo), 4); return v; }  // a whole word (lo is aligned)
+        for (uint32_t b = std::max(4u * w, lo); b < std::min(4u * w + 4u, hi); ++b) v |= uint32_t(src[b - lo]) << (8 * (b - 4u * w));
+        return v;
+    };
+    auto mask = [&](uint32_t row) -> uint2& {
+        auto it = f.mask_of.emplace(row, uint32_t(f.masks.size()));
+        if (it.second) {
+            f.masks.push_back(make_uint2(row, 0xFFu));
+            if (!stamp_q.empty()) stamp(row, 8u);
+        }
+        return f.masks[it.first->second];
+    };
+    uint32_t rows = e->st.n_rows;
+    for (uint32_t i = 0; i < n; ++i) {
+        const bgr_edit& d = edits[i];
+        switch (d.kind) {
+        case BGR_EDIT_WRITE: {
+            const Column& c = e->cols[d.column];
+            const uint32_t w0 = d.byte_offset / 4u, w1 = (d.byte_offset + d.byte_len + 3u) / 4u;
+            for (uint32_t k = 0; k < d.count; ++k) {
+                const uint8_t* src = values + d.value_offset + size_t(k) * d.byte_len;
+                for (uint32_t w = w0; w < w1; ++w)
+                    word(d.row + k, c.first_plane + w, pack(src, d.byte_offset, d.byte_offset + d.byte_len, w));
+            }
+            break;
+        }
+        case BGR_EDIT_INSERT: {
+            const Column& c = e->cols[d.column];
+            for (uint32_t w = 0; w < c.words; ++w) word(d.row, c.first_plane + w, pack(values + d.value_offset, 0, c.elem_bytes, w));
+            uint2& m = mask(d.row);
+            if (!(m.y >> 16)) m.y = (m.y & ~c.absent) & ~(c.absent << 8);
+            f.bump = true;
+            break;
+        }
+        case BGR_EDIT_REMOVE: {
+            uint2& m = mask(d.row);
+            if (!(m.y >> 16)) m.y |= e->cols[d.column].absent << 8;
+            f.bump = true;
+            break;
+        }
+        case BGR_EDIT_DESPAWN:
+            mask(d.row).y = 1u << 16;
+            break;
+        case BGR_EDIT_SPAWN:
+            if (d.count) {
+                for (uint64_t s = rows / kSegRows; s <= (uint64_t(rows) + d.count - 1) / kSegRows && !stamp_q.empty(); ++s)
+                    for (uint32_t q = 0; q < kActivePlanes; ++q) f.stamps.push_back(uint32_t(s) * kActivePlanes + q);
+                rows += d.count;
+            }
+            f.bump = true;
+            break;
+        }
+    }
+    // in address order (a stable LSD radix sort: words of one address stay in record order), one store per word, the
+    // last record's
+    uint64_t max_key = 0;
+    for (const EditFold::Word& w : f.words) max_key = std::max(max_key, w.key);
+    std::vector<EditFold::Word>& tmp = f.sorted;
+    tmp.resize(f.words.size());
+    constexpr uint32_t kDigit = 12, kBins = 1u << kDigit;
+    uint32_t bins[kBins + 1];
+    for (uint32_t shift = 0; shift < 64 && (max_key >> shift); shift += kDigit) {
+        std::fill(bins, bins + kBins + 1, 0u);
+        for (const EditFold::Word& w : f.words) ++bins[((w.key >> shift) & (kBins - 1)) + 1];
+        for (uint32_t b = 1; b <= kBins; ++b) bins[b] += bins[b - 1];
+        for (const EditFold::Word& w : f.words) tmp[bins[(w.key >> shift) & (kBins - 1)]++] = w;
+        f.words.swap(tmp);
+    }
+    size_t out = 0;
+    for (size_t k = 0; k < f.words.size(); ++k)
+        if (k + 1 == f.words.size() || f.words[k + 1].key != f.words[k].key) f.words[out++] = f.words[k];
+    f.words.resize(out);
+    // the stamps the stores clear: sorted words of one (segment, plane) are adjacent.  A duplicate left elsewhere (a
+    // spawn's segments) zeroes the same stamp twice.
+    for (const EditFold::Word& w : f.words) {
+        if (stamp_q.empty() || stamp_q[w.plane] < 0) continue;
+        const uint32_t s = (w.row / kSegRows) * kActivePlanes + uint32_t(stamp_q[w.plane]);
+        if (f.stamps.empty() || f.stamps.back() != s) f.stamps.push_back(s);
+    }
+    if (f.words.size() + f.masks.size() + f.stamps.size() > 0x7FFFFFFFull) return fail(BGR_ERR_CAPACITY, "edit batch too large");
+    return BGR_OK;
+}
+
+int apply_edits(bgr_engine* e, const bgr_edit* edits, uint32_t n, const void* values, size_t values_bytes) {
+    if (!e) return fail(BGR_ERR_INVALID_ARGUMENT, "null engine");
+    if (!e->built) return fail(BGR_ERR_STATE, "engine not built");
+    if ((n && !edits) || (values_bytes && !values)) return fail(BGR_ERR_INVALID_ARGUMENT, "null argument");
+    if (n == 0) return BGR_OK;
+    uint64_t rows = 0;
+    int rc = validate_edits(e, edits, n, values_bytes, &rows);
+    if (rc != BGR_OK) return rc;
+    EditFold& f = e->edit_fold;
+    f.clear();
+    rc = fold_edits(e, edits, n, static_cast<const uint8_t*>(values), f);
+    if (rc != BGR_OK) return rc;
+    // the staging buffer: the next one of the ring, once the batch that last used it has finished
+    bgr_engine::EditStage& sg = e->edit_stage[e->next_edit];
+    const size_t bytes_w = f.words.size() * sizeof(uint4), bytes_m = f.masks.size() * sizeof(uint2);
+    const size_t bytes = bytes_w + bytes_m + f.stamps.size() * sizeof(uint32_t);
+    if (!sg.done) CUDA_TRY(cudaEventCreateWithFlags(&sg.done, cudaEventDisableTiming));
+    if (sg.busy) CUDA_TRY(cudaEventSynchronize(sg.done));
+    sg.busy = false;
+    // Grows to the largest batch and stays (16 B per stored word): freeing the smaller buffer synchronises the device.
+    // Even an empty patch gets a buffer, so that the kernel always has a mapped address to read from.
+    if (!sg.h || bytes > sg.cap) {
+        if (sg.h) CUDA_TRY(cudaFreeHost(sg.h));
+        sg.h = nullptr; sg.cap = 0;
+        const size_t cap = std::max<size_t>(bytes, 64u << 10);
+        CUDA_TRY(cudaHostAlloc(&sg.h, cap, cudaHostAllocMapped));
+        sg.cap = cap;
+    }
+    // nothing fails past the capacity: growing is the last step that can refuse
+    if (rows > e->st.n_rows) rc = grow_to(e, rows);
+    if (rc == BGR_OK) rc = touch_live(e);  // stream-ordered behind the queued submits, like the launches below
+    if (rc != BGR_OK) return rc;
+    uint4* hw = reinterpret_cast<uint4*>(sg.h);
+    for (size_t k = 0; k < f.words.size(); ++k) hw[k] = make_uint4(f.words[k].row, f.words[k].plane, f.words[k].value, 0u);
+    if (bytes_m) std::memcpy(sg.h + bytes_w, f.masks.data(), bytes_m);
+    if (!f.stamps.empty()) std::memcpy(sg.h + bytes_w + bytes_m, f.stamps.data(), f.stamps.size() * sizeof(uint32_t));
+    uint8_t* dev = nullptr;
+    CUDA_TRY(cudaHostGetDevicePointer(reinterpret_cast<void**>(&dev), sg.h, 0));
+    if (rows > e->st.n_rows) {
+        const uint32_t count = uint32_t(rows - e->st.n_rows);
+        k_spawn_rows<<<e->grid_for(count, 64), 256, 0, e->stream>>>(e->image(0), e->words, e->st.n_rows, count);
+        e->launches += 1;
+        CUDA_TRY(cudaGetLastError());
+    }
+    EditPatch p;
+    p.words = reinterpret_cast<const uint4*>(dev);
+    p.masks = reinterpret_cast<const uint2*>(dev + bytes_w);
+    p.stamps = reinterpret_cast<const uint32_t*>(dev + bytes_w + bytes_m);
+    p.n_words = uint32_t(f.words.size()); p.n_masks = uint32_t(f.masks.size()); p.n_stamps = uint32_t(f.stamps.size());
+    const uint32_t total = p.n_words + p.n_masks + p.n_stamps;
+    k_apply_edits<<<e->grid_for(total, 256), 256, 0, e->stream>>>(e->image(0), e->words, e->d_stamps, p);
+    e->launches += 1;
+    CUDA_TRY(cudaGetLastError());
+    CUDA_TRY(cudaEventRecord(sg.done, e->stream));
+    sg.busy = true;
+    e->next_edit = (e->next_edit + 1) % bgr_engine::kEditBufs;
+    e->tiledep_chain = false;
+    e->st.n_rows = uint32_t(rows);
+    if (f.bump) e->st.live_passive_ver = ++e->st.ver_counter;
+    return BGR_OK;
+}
+
 void detect_bundles(bgr_engine* e) {
     e->bundle_particles = false;
     e->passive.clear();
@@ -1749,6 +2005,10 @@ BGR_API void bgr_engine_destroy(bgr_engine* e) {
         if (d.d_buf) cudaFree(d.d_buf);
         if (d.packed) cudaEventDestroy(d.packed);
         if (d.done) cudaEventDestroy(d.done);
+    }
+    for (auto& s : e->edit_stage) {
+        if (s.h) cudaFreeHost(s.h);
+        if (s.done) cudaEventDestroy(s.done);
     }
     for (auto& f : e->feeds) {
         if (!f.used) continue;
@@ -2152,6 +2412,10 @@ BGR_API int bgr_has_component(bgr_engine* e, uint32_t column, uint32_t first_row
     if (!e || !e->built || !host_dst) return fail(BGR_ERR_STATE, "engine not built");
     if (column >= e->cols.size()) return fail(BGR_ERR_INVALID_ARGUMENT, "unknown column");
     return read_alive_image(e, 0, first_row, count, e->st.n_rows, host_dst, e->cols[column].absent);
+}
+
+BGR_API int bgr_apply_edits(bgr_engine* e, const bgr_edit* edits, uint32_t n, const void* values, size_t values_bytes) {
+    return apply_edits(e, edits, n, values, values_bytes);
 }
 
 BGR_API int bgr_host_alloc(size_t bytes, void** out) {

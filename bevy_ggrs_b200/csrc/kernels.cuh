@@ -1010,6 +1010,37 @@ __global__ void __launch_bounds__(256) k_spawn_rows(uint8_t* img, uint32_t words
 }
 __global__ void k_set_alive(uint8_t* img, uint32_t words, uint32_t row, uint8_t value) { img[alive_offset(words, row)] = value; }
 
+// A batch of host edits (bgr_apply_edits) folded by the host into one patch of image 0, read from page-locked memory:
+//   words:  (row, plane, value) stores, one per word, sorted by address so that neighbouring threads store neighbouring
+//           words of a plane;
+//   masks:  (row, and | or << 8 | despawn << 16) per row, the batch's presence records composed in order.  Like
+//           k_set_absent they only change a row that is alive here (a queued vector may have despawned it); a despawn
+//           clears the byte whatever it held;
+//   stamps: indices into image 0's content-stamp row whose stamps become unknown.
+// The three lists touch disjoint bytes, so one flat index space covers them in any order.
+struct EditPatch {
+    const uint4* words;
+    const uint2* masks;
+    const uint32_t* stamps;
+    uint32_t n_words, n_masks, n_stamps;
+};
+__global__ void __launch_bounds__(256) k_apply_edits(uint8_t* img, uint32_t words, uint32_t* stamps, const EditPatch p) {
+    const uint32_t n = p.n_words + p.n_masks + p.n_stamps;
+    for (uint32_t t = blockIdx.x * blockDim.x + threadIdx.x; t < n; t += gridDim.x * blockDim.x) {
+        if (t < p.n_words) {
+            const uint4 w = p.words[t];
+            *reinterpret_cast<uint32_t*>(img + word_offset(words, w.x, w.y)) = w.z;
+        } else if (t < p.n_words + p.n_masks) {
+            const uint2 m = p.masks[t - p.n_words];
+            uint8_t* a = img + alive_offset(words, m.x);
+            if (m.y >> 16) *a = 0;
+            else if (*a & 1u) *a = uint8_t((*a & m.y) | (m.y >> 8));
+        } else {
+            stamps[p.stamps[t - p.n_words - p.n_masks]] = 0u;
+        }
+    }
+}
+
 // ---- GgrsSchedule systems on the live image (stepwise path) ----
 // One registered system (run_system) over rows [0, n_rows), one row per thread.  `kill` receives the despawns;
 // k_apply_despawns applies them after every system of the schedule has run (Commands are deferred to the end of GgrsSchedule).

@@ -55,6 +55,9 @@ class FeedInfo(NamedTuple):
     record_bytes: int
 
 
+EDIT_DTYPE = np.dtype([(name, "<u4") for name, _ in capi.bgr_edit._fields_])   # one bgr_edit record
+
+
 def feed_record_dtype(fields: Sequence[Tuple[int, int, int]]) -> np.dtype:
     """A change-feed record: u32 row, u32 state (bit 0 exists, bit 1+k field k present), then field k's bytes as
     ``f<k>``."""
@@ -178,6 +181,15 @@ class Engine:
         out = np.zeros(count, dtype=np.uint8)
         self._check(self._lib.bgr_has_component(self._h, col, first_row, count, out.ctypes.data))
         return out
+
+    # ---- host edits (bgr_apply_edits) ----
+    def apply_edits(self, edits: np.ndarray, values: bytes = b"") -> None:
+        """One queued batch of live-world edits: ``edits`` is an ``EDIT_DTYPE`` array (kind, column, row, count,
+        byte_offset, byte_len, value_offset, reserved), ``values`` the bytes its WRITE / INSERT records point into.
+        Returns without waiting for the GPU; both buffers are free on return."""
+        e = np.ascontiguousarray(edits, dtype=EDIT_DTYPE)
+        v = np.frombuffer(bytes(values), dtype=np.uint8)
+        self._check(self._lib.bgr_apply_edits(self._h, e.ctypes.data, len(e), v.ctypes.data if v.size else None, v.size))
 
     # ---- asynchronous mirror download (bgr_download_begin / bgr_download_wait) ----
     def host_alloc(self, count: int, byte_len: int) -> np.ndarray:

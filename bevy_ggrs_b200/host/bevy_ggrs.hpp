@@ -190,6 +190,51 @@ public:
         check(bgr_has_component(engine_, col<T>(), first_row, count, v.data()));
         return v;
     }
+    // Host edits (bgr_apply_edits): what an Update system or Commands do to rollback entities between frames, recorded
+    // in order and sent as one queued batch by apply().  Equivalent to the single calls above in the same order.
+    class Edits {
+    public:
+        explicit Edits(const App& app) : app_(app) {}
+        template <class T> Edits& write(uint32_t first_row, const std::vector<T>& v) {
+            for (const T& x : v) values_.insert(values_.end(), reinterpret_cast<const uint8_t*>(&x), reinterpret_cast<const uint8_t*>(&x) + sizeof(T));
+            return add(BGR_EDIT_WRITE, app_.col<T>(), first_row, uint32_t(v.size()), 0, uint32_t(sizeof(T)), values_.size() - v.size() * sizeof(T));
+        }
+        // bytes [offset, offset + sizeof(F)) of T on `row`, e.g. write_field<Transform>(row, 0, translation)
+        template <class T, class F> Edits& write_field(uint32_t row, uint32_t offset, const F& field) {
+            const size_t at = push_bytes(&field, sizeof(F));
+            return add(BGR_EDIT_WRITE, app_.col<T>(), row, 1, offset, uint32_t(sizeof(F)), at);
+        }
+        template <class T> Edits& insert(uint32_t row, const T& value) {
+            const size_t at = push_bytes(&value, sizeof(T));
+            return add(BGR_EDIT_INSERT, app_.col<T>(), row, 0, 0, 0, at);
+        }
+        template <class T> Edits& remove(uint32_t row) { return add(BGR_EDIT_REMOVE, app_.col<T>(), row, 0, 0, 0, 0); }
+        Edits& despawn(uint32_t row) { return add(BGR_EDIT_DESPAWN, 0, row, 0, 0, 0, 0); }
+        Edits& spawn(uint32_t count) { return add(BGR_EDIT_SPAWN, 0, 0, count, 0, 0, 0); }
+        size_t size() const { return records_.size(); }
+
+    private:
+        friend class App;
+        size_t push_bytes(const void* p, size_t n) {
+            const size_t at = values_.size();
+            values_.insert(values_.end(), static_cast<const uint8_t*>(p), static_cast<const uint8_t*>(p) + n);
+            return at;
+        }
+        Edits& add(uint32_t kind, uint32_t column, uint32_t row, uint32_t count, uint32_t offset, uint32_t len, size_t at) {
+            records_.push_back(bgr_edit{kind, column, row, count, offset, len, uint32_t(at), 0u});
+            return *this;
+        }
+        const App& app_;
+        std::vector<bgr_edit> records_;
+        std::vector<uint8_t> values_;
+    };
+    // enqueues the batch behind the submitted request vectors and empties it; returns without waiting for the GPU
+    void apply(Edits& edits) {
+        finish();
+        check(bgr_apply_edits(engine_, edits.records_.data(), uint32_t(edits.records_.size()), edits.values_.data(), edits.values_.size()));
+        edits.records_.clear();
+        edits.values_.clear();
+    }
     // asynchronous host mirror of bytes [offset, offset+len) of every T in rows [first_row, first_row+count):
     // `dst` from bgr_host_alloc; readable after download_wait(ticket)
     template <class T> uint32_t download_begin(uint32_t offset, uint32_t len, uint32_t first_row, uint32_t count, void* dst) {

@@ -242,6 +242,54 @@ BGR_API int bgr_remove_component(bgr_engine* e, uint32_t column, uint32_t row);
 BGR_API int bgr_insert_component(bgr_engine* e, uint32_t column, uint32_t row, const void* value);
 BGR_API int bgr_has_component(bgr_engine* e, uint32_t column, uint32_t first_row, uint32_t count, uint8_t* host_dst);
 
+/* ---- host edits: a batch of live-world changes in one queued launch -----------------------------------------------
+ * What a game does to rollback entities outside GgrsSchedule (an Update system setting Transform.translation,
+ * commands.entity(e).despawn() / insert / remove, spawning with Rollback), applied to the live world as one batch.  A
+ * batch is observably identical to issuing its records in order through the single calls:
+ *   BGR_EDIT_WRITE   bytes [byte_offset, byte_offset+byte_len) of `column` on rows [row, row+count), a read-modify-write of
+ *                    each element through bgr_write_component.  Row k's bytes are values[value_offset + k*byte_len ...].
+ *                    byte_offset is a multiple of 4; byte_len > 0 is a multiple of 4 or ends at the element's end (the
+ *                    element's tail word is zero-padded, as bgr_write_component pads it).
+ *   BGR_EDIT_INSERT  bgr_insert_component(column, row, values + value_offset): the whole element, written whatever the
+ *                    row's state, then present if the row is alive.
+ *   BGR_EDIT_REMOVE  bgr_remove_component(column, row).
+ *   BGR_EDIT_DESPAWN bgr_despawn(row): later presence records of the row change nothing.
+ *   BGR_EDIT_SPAWN   bgr_spawn(count): appends `count` rows; later records of the batch may address them.
+ * Fields a kind does not name are ignored.  Later records win where records overlap.  Every row must be below the row
+ * count at that point of the batch (bgr_row_count, which counts the rows of queued request vectors, plus the batch's
+ * earlier spawns).  The whole batch is validated before anything runs: a bad kind, column, optional-ness, field range
+ * or value range (against values_bytes) is BGR_ERR_INVALID_ARGUMENT; spawns past max_entities are BGR_ERR_CAPACITY (or
+ * grow a BGR_CFG_GROWABLE engine, past its ceiling BGR_ERR_CAPACITY); spawning after the first request vector on a
+ * BGR_CFG_SHARDED engine or with order_base != 0 is BGR_ERR_UNSUPPORTED.  A refused batch changes nothing.
+ * The call is ordered behind every submitted request vector on the engine stream and does not wait for them: it copies
+ * the batch into the engine's own page-locked staging (the caller's buffers are free on return) and waits only when
+ * every staging buffer still belongs to an unfinished earlier batch.  Each of the 4 staging buffers grows to the
+ * largest patch it has held (16 bytes per stored word, plus 8 per row with presence records) and keeps that
+ * page-locked memory until bgr_engine_destroy; the call that grows one waits for the device, because releasing
+ * page-locked memory does.  Send a whole column with bgr_write_component instead.  Un-collected submits keep their
+ * results.  Unlike
+ * the single calls it keeps the skip records precise: only the content stamps of the (64-row segment, active plane)
+ * pairs it changes become unknown, and the passive-plane version moves only for spawns, presence changes and writes
+ * that touch a passive plane.  n == 0 does nothing. */
+typedef enum bgr_edit_kind {
+    BGR_EDIT_WRITE = 0,
+    BGR_EDIT_INSERT = 1,
+    BGR_EDIT_REMOVE = 2,
+    BGR_EDIT_DESPAWN = 3,
+    BGR_EDIT_SPAWN = 4
+} bgr_edit_kind;
+typedef struct bgr_edit {
+    uint32_t kind;          /* bgr_edit_kind */
+    uint32_t column;        /* WRITE, INSERT, REMOVE */
+    uint32_t row;           /* WRITE (first row), INSERT, REMOVE, DESPAWN */
+    uint32_t count;         /* WRITE: rows; SPAWN: rows appended */
+    uint32_t byte_offset;   /* WRITE */
+    uint32_t byte_len;      /* WRITE */
+    uint32_t value_offset;  /* WRITE, INSERT: into `values` */
+    uint32_t reserved;
+} bgr_edit;
+BGR_API int bgr_apply_edits(bgr_engine* e, const bgr_edit* edits, uint32_t n, const void* values, size_t values_bytes);
+
 /* ---- asynchronous mirror download: what the ECS side reads back every tick -----------------
  * In the reference the world lives in host memory and everything after GgrsSchedule (rendering via Transform,
  * examples/stress_tests/particles.rs:191-196; game logic outside the rollback schedule) reads it there.  With the

@@ -254,6 +254,64 @@ pub mod change_feed {
     }
 }
 
+/// Host edits: changes to rollback entities made outside `GgrsSchedule` (an `Update` system setting
+/// `transform.translation`, `commands.entity(e).despawn()` / `insert` / `remove`), sent to HBM as one queued batch
+/// (`bgr_apply_edits`, INTEGRATION.md §1).  Rows are RollbackOrdered indices.  The batch applies in record order.
+pub mod host_edits {
+    use super::{check, engine, sys, Columns, GpuColumn};
+    use bevy::prelude::World;
+    use core::any::TypeId;
+
+    #[derive(Default)]
+    pub struct Edits { records: Vec<sys::bgr_edit>, values: Vec<u8> }
+
+    fn column<T: GpuColumn>(world: &World) -> u32 {
+        *world.resource::<Columns>().by_type.get(&TypeId::of::<T>()).expect("component is not a rollback column in HBM")
+    }
+
+    impl Edits {
+        fn push(&mut self, kind: u32, column: u32, row: u32, count: u32, byte_offset: u32, bytes: &[u8]) {
+            self.records.push(sys::bgr_edit { kind, column, row, count, byte_offset, byte_len: (bytes.len() as u32) / count.max(1),
+                                              value_offset: self.values.len() as u32, reserved: 0 });
+            self.values.extend_from_slice(bytes);
+        }
+        /// The first `T::BYTES` bytes of `value` on `row`.
+        pub fn write<T: GpuColumn>(&mut self, world: &World, row: u32, value: &T) -> &mut Self {
+            let bytes = unsafe { core::slice::from_raw_parts((value as *const T).cast::<u8>(), T::BYTES as usize) };
+            self.push(sys::BGR_EDIT_WRITE, column::<T>(world), row, 1, 0, bytes);
+            self
+        }
+        /// Bytes [byte_offset, byte_offset + bytes.len()) of `T` on `row` (e.g. only `Transform::translation`).
+        pub fn write_field<T: GpuColumn>(&mut self, world: &World, row: u32, byte_offset: u32, bytes: &[u8]) -> &mut Self {
+            self.push(sys::BGR_EDIT_WRITE, column::<T>(world), row, 1, byte_offset, bytes);
+            self
+        }
+        /// `commands.entity(e).insert(value)` of an optional column.
+        pub fn insert<T: GpuColumn>(&mut self, world: &World, row: u32, value: &T) -> &mut Self {
+            let bytes = unsafe { core::slice::from_raw_parts((value as *const T).cast::<u8>(), T::BYTES as usize) };
+            self.push(sys::BGR_EDIT_INSERT, column::<T>(world), row, 0, 0, bytes);
+            self
+        }
+        /// `commands.entity(e).remove::<T>()` of an optional column.
+        pub fn remove<T: GpuColumn>(&mut self, world: &World, row: u32) -> &mut Self {
+            self.push(sys::BGR_EDIT_REMOVE, column::<T>(world), row, 0, 0, &[]);
+            self
+        }
+        /// `commands.entity(e).despawn()`.
+        pub fn despawn(&mut self, row: u32) -> &mut Self { self.push(sys::BGR_EDIT_DESPAWN, 0, row, 0, 0, &[]); self }
+        /// `count` new rows, appended after the rows that exist when the batch reaches this record.
+        pub fn spawn(&mut self, count: u32) -> &mut Self { self.push(sys::BGR_EDIT_SPAWN, 0, 0, count, 0, &[]); self }
+        pub fn is_empty(&self) -> bool { self.records.is_empty() }
+        /// Enqueues the batch behind the submitted request vectors and clears it; returns without waiting for the GPU.
+        pub fn apply(&mut self, world: &World) {
+            check(unsafe { sys::bgr_apply_edits(engine(world), self.records.as_ptr(), self.records.len() as u32,
+                                                self.values.as_ptr().cast(), self.values.len()) });
+            self.records.clear();
+            self.values.clear();
+        }
+    }
+}
+
 // ------------------------------------------------------------------------------------------------------------------
 // RollbackApp — the reference's trait, same method names and signatures (rollback_app.rs:31-133, :135-248)
 // ------------------------------------------------------------------------------------------------------------------

@@ -69,6 +69,9 @@ pub use p2p_desync::*;
 mod change_feed;
 pub use change_feed::*;
 
+mod host_edits;
+pub use host_edits::*;
+
 #[repr(C)]
 #[derive(Clone, Copy, Default)]
 pub struct bgr_request {
@@ -145,6 +148,7 @@ extern "C" {
     pub fn bgr_remove_component(e: *mut bgr_engine, column: u32, row: u32) -> c_int;
     pub fn bgr_insert_component(e: *mut bgr_engine, column: u32, row: u32, value: *const c_void) -> c_int;
     pub fn bgr_has_component(e: *mut bgr_engine, column: u32, first_row: u32, count: u32, host_dst: *mut u8) -> c_int;
+    pub fn bgr_apply_edits(e: *mut bgr_engine, edits: *const bgr_edit, n: u32, values: *const c_void, values_bytes: usize) -> c_int;
     pub fn bgr_host_alloc(bytes: usize, out: *mut *mut c_void) -> c_int;
     pub fn bgr_host_free(p: *mut c_void) -> c_int;
     pub fn bgr_download_begin(e: *mut bgr_engine, column: u32, byte_offset: u32, byte_len: u32, first_row: u32, count: u32, host_dst: *mut c_void, ticket_out: *mut u32) -> c_int;
