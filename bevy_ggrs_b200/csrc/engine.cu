@@ -33,6 +33,7 @@
 #include "frame_digest.cuh"
 #include "jit.hpp"
 #include "vmm_range.hpp"
+#include "device_memory.hpp"
 
 using namespace bgr;
 
@@ -124,7 +125,7 @@ struct HostState {  // trivially copyable: copying it per call must not allocate
     //   - growth (BGR_CFG_GROWABLE, grow_to): maps new memory behind every image's bytes and zeroes it.  Every row it
     //     writes is at or past every image's row count, so no version changes.
     //
-    // Content stamps of the active planes (bgr_engine::d_stamps, engines that run the bundle kernel), the device-side
+    // Content stamps of the active planes (bgr_engine::stamps, engines that run the bundle kernel), the device-side
     // counterpart for the planes the systems write, decided per warp segment because it depends on the values:
     //   stamp[img][seg][q] == S != 0  =>  the bytes of active plane q of 64-row segment seg in image img are exactly
     //   the content that stamp S names.  0 = unknown.
@@ -230,12 +231,11 @@ struct bgr_engine {
 
     uint32_t epad = 0, words = 0, tile_bytes = 0, n_tiles_cap = 0;
     size_t image_bytes = 0;
-    uint8_t* arena = nullptr;  // image 0 = live, image s+1 = slot s (tile-planar, kernels.cuh)
-    uint8_t* d_kill = nullptr;
-    uint8_t* d_stage = nullptr;  // device staging for ECS column <-> image transposition
-    size_t stage_cap = 0;
+    StridedRange arena;  // image 0 = live, image s+1 = slot s (tile-planar, kernels.cuh)
+    StridedRange kill;
+    DeviceBuffer<uint8_t> stage;  // device staging for ECS column <-> image transposition
     // asynchronous mirror downloads: packed on the main stream, copied D2H on copy_stream
-    struct Download { uint8_t* d_buf = nullptr; size_t cap = 0; cudaEvent_t packed = nullptr, done = nullptr; bool busy = false; };
+    struct Download { DeviceBuffer<uint8_t> buf; Event packed, done; bool busy = false; };
     Download dl[BGR_MAX_DOWNLOADS];
     cudaStream_t copy_stream = nullptr;
     uint32_t next_dl = 0;
@@ -243,18 +243,19 @@ struct bgr_engine {
     // cross PCIe on copy_stream
     struct Feed {
         bool used = false, busy = false;
-        FeedParams p{};              // fields, rep, keep, rep_words, record_words and the scratch pointers
+        FeedParams p{};              // fields, rep, keep, rep_words, record_words and views of the buffers below
         uint32_t bound = 0;          // no row at or past it has a reported state other than (0, zeros)
         uint32_t ticket = 0;         // of the report in flight
-        uint32_t stage_records = 0;  // records p.out holds
-        unsigned int* h_info = nullptr;  // page-locked [4]: the info, copied behind the records
-        cudaEvent_t packed = nullptr, done = nullptr;
-        StridedRange va_rep, va_count;   // growable engines: p.rep, and p.tile_count / tile_off / tile_list one stride each
+        StridedRange rep, count;     // p.rep, and p.tile_count / tile_off / tile_list one stride each
+        DeviceBuffer<unsigned int> info;
+        DeviceBuffer<uint32_t> out;  // the records of a report
+        MappedHostBuffer<unsigned int> h_info;  // [4]: the info, copied behind the records
+        Event packed, done;
     };
     Feed feeds[BGR_MAX_FEEDS];
     uint32_t feed_seq = 0;
     // host edits (bgr_apply_edits): page-locked patches the kernel reads in place, reused once their launch finished
-    struct EditStage { uint8_t* h = nullptr; size_t cap = 0; cudaEvent_t done = nullptr; bool busy = false; };
+    struct EditStage { MappedHostBuffer<uint8_t> h; Event done; bool busy = false; };
     static constexpr int kEditBufs = 4;
     EditStage edit_stage[kEditBufs];
     uint32_t next_edit = 0;
@@ -267,14 +268,15 @@ struct bgr_engine {
     // never share one; set 0 serves every launch that overlaps nothing
     unsigned long long* d_accum_set[kBufs] = {};
     unsigned int* d_ticket_set[kBufs] = {};
-    unsigned long long* d_accum = nullptr;
-    unsigned int* d_ticket = nullptr;
-    float2* h_spawn[kBufs] = {};  // host-mapped (vx, vy) of spawned particles
-    float2* d_spawn[kBufs] = {};
+    DeviceBuffer<unsigned long long> accum;
+    DeviceBuffer<unsigned int> ticket;
+    MappedHostBuffer<float2> spawn[kBufs];  // (vx, vy) of spawned particles
     int spawn_sys = -1;             // index of BGR_SYS_PARTICLES_SPAWN in `systems`, or -1
+    // result blocks: views of the engine's own (out_block) or, in a shard group, of the group's segment
+    MappedHostBuffer<unsigned long long> out_block[kBufs];
     unsigned long long* h_out[kBufs] = {};
     unsigned long long* d_out[kBufs] = {};
-    cudaEvent_t ev[kBufs] = {};
+    Event ev[kBufs];
     // un-collected request vectors, oldest first: a fixed ring (a std::deque allocated a chunk per push — the hot path
     // allocates nothing)
     struct PendingRing {
@@ -293,15 +295,13 @@ struct bgr_engine {
     // shard group (multi-GPU): result blocks live in a shared host segment every rank's GPU and CPU map
     ShardGroup* group = nullptr;
     unsigned long long gseq = 0;
-    unsigned long long* own_h_out[kBufs] = {};  // the engine's private result blocks while it is in a group
-    unsigned long long* own_d_out[kBufs] = {};
     bool ticked = false;            // a request vector has been executed (the initial population is over)
     DeferredLive deferred;          // committed by submit() together with `st`
     bool live_touched = false;      // an entry point read or wrote image 0 since the last submit: the next one stays eager
     int tune_defer_live = 1;        // 0: every fused program writes image 0 itself
-    unsigned long long* d_internal_out = nullptr;  // result block of internal launches (materialisation)
+    DeviceBuffer<unsigned long long> internal_out;  // result block of internal launches (materialisation)
     // device-side launch trace (bgr_trace_enable): per launch [first block start, last block end] in globaltimer ns
-    unsigned long long* d_trace = nullptr;
+    DeviceBuffer<unsigned long long> trace;
     uint32_t trace_cap = 0;
     unsigned long long trace_first_seq = 0;
 
@@ -312,8 +312,8 @@ struct bgr_engine {
     unsigned long long seq = 0;   // sequence number of the last submit (completion flag value)
     int tune_poll = 1;            // collect() spins on the host-mapped flag before falling back to the event
     int tune_tiledep = 1;         // consecutive fused launches overlap: per-tile dependencies instead of grid-level (PF_TILE_WAIT)
-    unsigned int* d_tile_done = nullptr;  // [tiles] see ProgramParams::tile_done
-    unsigned int* d_tile_cnt = nullptr;
+    StridedRange tile_done;       // [tiles + 1] see ProgramParams::tile_done
+    StridedRange tile_cnt;
     bool tiledep_chain = false;   // the last operation enqueued on the main stream was a PF_TILE_SIGNAL launch
     uint32_t tiledep_seq = 0, tiledep_tiles = 0;
     int tune_grid = 0;            // experiment / tests: cap the one-launch kernels' grid (0 = SMs x resident blocks)
@@ -326,8 +326,7 @@ struct bgr_engine {
     std::vector<uint16_t> passive;
     std::vector<PassiveRun> runs;
     uint32_t passive_bytes = 0;
-    uint32_t* d_stamps = nullptr;   // content stamps of the active planes (HostState): [images][segments][kActivePlanes]
-    uint32_t stamp_image = 0;       // words per image
+    StridedRange stamps;            // content stamps of the active planes (HostState): [images][segments][kActivePlanes]
     uint32_t stamp_next = 1;        // first stamp of the next bundle launch
     bool stamps_stale = false;      // a bundle launch without stamps wrote images since the table was last cleared
     bool bundle_static_ck = false;  // both columns checksummed with the finite assertion: fully specialised kernel
@@ -339,7 +338,7 @@ struct bgr_engine {
     JitKernel jit;                  // fn == nullptr: the interpreter kernel runs.  Work item = a whole tile
     JitKernel jit_small;            // the same kernel with quarter-tile work items: worlds of few tiles per SM (optional)
     int tune_jit_tiledep = 0;       // 1: consecutive launches of the generated kernel overlap through per-item dependencies (queued submits)
-    unsigned int* d_item_done = nullptr;   // [4 * tiles] GenericParams::item_done (quarter-tile work items at most)
+    StridedRange item_done;         // [4 * tiles + 4] GenericParams::item_done (quarter-tile work items at most)
     const void* jit_chain_kernel = nullptr;  // the signalling launch `tiledep_chain` refers to (its work-item partition must match)
     int tune_jit_item = 0;          // 0 auto (quarter tiles below 3 tiles per SM), 512 / 256 / 128 force the rows per work item
     int tune_passive_early = -1;    // -1: early passive stores for single-wave grids (auto); 0 never; 1 always
@@ -350,36 +349,34 @@ struct bgr_engine {
     int tune_bps = 0, tune_passive_tma = 1;
     int tune_tma = 1;          // stepwise Save/Load through the TMA-staged bulk-copy kernel
     uint32_t tma_stage_tiles = 0;  // one-tile stages of the TMA copy kernel (0: schema too wide for two stages of shared memory)
-    unsigned int* d_tma_ticket = nullptr;
+    DeviceBuffer<unsigned int> tma_ticket;
     int occ_cache[2][3][2] = {};  // [passive TMA][MODE][STAMPS]: blocks per SM of k_particles_program
     // desync diff scratch (BGR_CFG_DESYNC_CAPTURE), allocated by the first bgr_desync_diff
-    DiffColumn* d_diff_cols = nullptr;
-    unsigned int* d_diff_counts = nullptr;       // [n_cols][3] then the per-tile record counts
-    unsigned long long* d_diff_totals = nullptr;
-    unsigned int* d_diff_list = nullptr;         // [2 * tiles]
-    DiffRecord* d_diff_records = nullptr;
-    size_t diff_records_cap = 0;
+    DeviceBuffer<DiffColumn> diff_cols;
+    DeviceBuffer<unsigned int> diff_counts;      // [n_cols][3] then the per-tile record counts
+    DeviceBuffer<unsigned long long> diff_totals;
+    DeviceBuffer<unsigned int> diff_list;        // [2 * tiles]
+    DeviceBuffer<DiffRecord> diff_records;
     // P2P desync reports: retention of confirmed frames (bgr_retain_confirmed) and the digest / remote diff scratch,
     // allocated by their first use
     uint32_t retain_interval = 0, retain_count = 0;
-    DigestColumn* d_digest_cols = nullptr;
-    unsigned long long* d_digest_words = nullptr;  // [tiles][n_cols + 1]
-    unsigned int* d_digest_active = nullptr;       // [tiles]
-    uint8_t* d_remote = nullptr;                   // tiles uploaded from a peer's export blob
-    unsigned int* d_remote_visit = nullptr;        // [n_tiles_cap] the local tiles a remote diff visits
-    uint32_t remote_cap_tiles = 0;                 // tiles d_remote holds
-    uint32_t diff_tiles = 0, digest_tiles = 0, visit_tiles = 0;  // tiles the scratch above was allocated for
+    DeviceBuffer<DigestColumn> digest_cols;
+    DeviceBuffer<unsigned long long> digest_words;  // [tiles][n_cols + 1]
+    DeviceBuffer<unsigned int> digest_active;       // [tiles]
+    DeviceBuffer<uint8_t> remote;                   // tiles uploaded from a peer's export blob
+    DeviceBuffer<unsigned int> remote_visit;        // [n_tiles_cap] the local tiles a remote diff visits
 
-    // BGR_CFG_GROWABLE: cfg.max_entities, epad and n_tiles_cap are the current capacity, image_bytes (and stamp_image) the
-    // fixed stride of an image, sized for the ceiling.  Every buffer whose size follows the capacity and that a queued
-    // launch may use is a strided range (vmm_range.hpp) that grow_to maps further; none of their pointers ever changes.
+    // BGR_CFG_GROWABLE: cfg.max_entities, epad and n_tiles_cap are the current capacity, image_bytes (and stamp_image())
+    // the fixed stride of an image, sized for the ceiling.  Every buffer whose size follows the capacity and that a
+    // queued launch may use is a strided range (vmm_range.hpp, capacity_buffers) that grow_to maps further; none of their
+    // pointers ever changes.
     uint32_t ceiling = 0;  // most rows the engine can hold (== the capacity without the flag)
-    StridedRange va_arena, va_stamps, va_kill, va_tile_done, va_tile_cnt, va_item_done;
 
-    uint8_t* image(uint32_t idx) const { return arena + size_t(idx) * image_bytes; }
+    uint8_t* image(uint32_t idx) const { return arena.ptr() + size_t(idx) * image_bytes; }
     bool capture() const { return cfg.flags & BGR_CFG_DESYNC_CAPTURE; }
     bool growable() const { return cfg.flags & BGR_CFG_GROWABLE; }
     uint32_t stamp_words() const { return n_tiles_cap * kSegsPerTile * kActivePlanes; }  // stamps of one image's rows
+    uint32_t stamp_image() const { return uint32_t(stamps.stride / sizeof(uint32_t)); }  // words between two images' stamps
     // frame slots behind the live image
     uint32_t n_slots() const { return (capture() ? 2u * cfg.max_depth : cfg.max_depth) + retain_count; }
     uint32_t image_off256(uint32_t idx) const { return uint32_t((size_t(idx) * image_bytes) >> 8); }
@@ -396,20 +393,15 @@ namespace {
 // A write outside the bundle kernel: image `idx`'s content stamps become unknown (HostState).  Stream-ordered behind
 // every launch that could still write them.
 int clear_stamps(bgr_engine* e, uint32_t idx) {
-    if (!e->d_stamps) return BGR_OK;
-    CUDA_TRY(cudaMemsetAsync(e->d_stamps + size_t(idx) * e->stamp_image, 0, size_t(e->stamp_words()) * sizeof(uint32_t), e->stream));
+    if (e->stamps.empty()) return BGR_OK;
+    CUDA_TRY(cudaMemsetAsync(e->stamps.ptr<uint32_t>() + size_t(idx) * e->stamp_image(), 0, size_t(e->stamp_words()) * sizeof(uint32_t), e->stream));
     e->tiledep_chain = false;
     return BGR_OK;
 }
 
-// The whole stamp table: one memset, or one per image row when the rows are strides of a growable engine.
+// The whole stamp table: the stamps of every image's rows (one memset while the images' stamps are contiguous).
 int clear_stamp_table(bgr_engine* e) {
-    const uint32_t images = e->n_slots() + 1u;
-    if (e->stamp_image == e->stamp_words())
-        CUDA_TRY(cudaMemsetAsync(e->d_stamps, 0, size_t(e->stamp_image) * images * sizeof(uint32_t), e->stream));
-    else
-        for (uint32_t i = 0; i < images; ++i)
-            CUDA_TRY(cudaMemsetAsync(e->d_stamps + size_t(i) * e->stamp_image, 0, size_t(e->stamp_words()) * sizeof(uint32_t), e->stream));
+    CUDA_TRY(e->stamps.zero(0, size_t(e->stamp_words()) * sizeof(uint32_t), e->stream));
     e->tiledep_chain = false;
     return BGR_OK;
 }
@@ -624,7 +616,7 @@ int run_fused(bgr_engine* e, const Program& pg, uint32_t buf) {
     ProgramParams pp;
     std::memset(&pp, 0, sizeof pp);
     pp.seq = e->seq;
-    pp.arena = e->arena;
+    pp.arena = e->arena.ptr();
     pp.order_base = e->cfg.order_base;
     pp.words = e->words; pp.tile_bytes = e->tile_bytes;
     pp.n_tiles = std::max(1u, e->tiles_for(pg.max_rows));  // at least one tile so a result block is published
@@ -640,7 +632,7 @@ int run_fused(bgr_engine* e, const Program& pg, uint32_t buf) {
     const bool simple = n_loads == 0 || (n_loads == 1 && pg.first_is_load);
     if (e->tune_dynamic) pp.flags |= PF_DYNAMIC_TILES;
     if (e->tune_prefetch) pp.flags |= PF_PREFETCH_NEXT;
-    pp.spawn_vals = e->d_spawn[buf];
+    pp.spawn_vals = e->spawn[buf].dev();
     if (e->spawn_sys >= 0) {
         const uint64_t ttl = e->systems[size_t(e->spawn_sys)].params[1];
         pp.spawn_ttl_lo = uint32_t(ttl); pp.spawn_ttl_hi = uint32_t(ttl >> 32);
@@ -681,8 +673,8 @@ int run_fused(bgr_engine* e, const Program& pg, uint32_t buf) {
         e->stamps_stale = false;
     }
     if (!stamps) e->stamps_stale = true;
-    pp.stamps = e->d_stamps;
-    pp.stamp_image = e->stamp_image;
+    pp.stamps = e->stamps.ptr<uint32_t>();
+    pp.stamp_image = e->stamp_image();
     pp.stamp_base = e->stamp_next;
     if (stamps) e->stamp_next += pg.n_ops + 1;
 
@@ -690,7 +682,7 @@ int run_fused(bgr_engine* e, const Program& pg, uint32_t buf) {
     // a synchronous caller collects before the next submit, so there is nothing to overlap with
     // ... and only on a stream the engine owns: on a caller's stream foreign work may sit between two submits and
     // become the programmatic-launch primary, which the per-tile flags know nothing about
-    const bool tiledep = e->tune_tiledep && e->d_tile_done && e->own_stream && !pg.internal &&
+    const bool tiledep = e->tune_tiledep && !e->tile_done.empty() && e->own_stream && !pg.internal &&
                          (e->tune_tiledep > 1 || !e->pending.empty());
     if (e->tiledep_chain && pp.n_tiles != e->tiledep_tiles) {
         // The tile range changed (rows crossed a tile boundary): a tile outside the previous launch's range may still be
@@ -700,8 +692,8 @@ int run_fused(bgr_engine* e, const Program& pg, uint32_t buf) {
     }
     if (tiledep) {
         pp.flags |= PF_TILE_SIGNAL;
-        pp.grid_done = e->d_tile_done + e->tiles_for(e->cfg.max_entities);  // the extra word behind the per-tile flags
-        pp.tile_done = e->d_tile_done; pp.tile_cnt = e->d_tile_cnt;
+        pp.tile_done = e->tile_done.ptr<unsigned int>(); pp.tile_cnt = e->tile_cnt.ptr<unsigned int>();
+        pp.grid_done = pp.tile_done + e->tiles_for(e->cfg.max_entities);  // the extra word behind the per-tile flags
         pp.done_seq = uint32_t(e->seq);
         if (e->tiledep_chain) { pp.flags |= PF_TILE_WAIT; pp.wait_seq = e->tiledep_seq; pp.wait_tiles = e->tiledep_tiles; }
     }
@@ -716,8 +708,8 @@ int run_fused(bgr_engine* e, const Program& pg, uint32_t buf) {
     const uint32_t set = tiledep ? uint32_t(e->seq % bgr_engine::kBufs) : 0u;
     pp.accum = e->d_accum_set[set];
     pp.ticket = e->d_ticket_set[set];
-    pp.out = pg.internal ? e->d_internal_out : e->d_out[buf];
-    if (e->d_trace && !pg.internal && e->seq - e->trace_first_seq < e->trace_cap) pp.trace = e->d_trace + (e->seq - e->trace_first_seq) * 4;
+    pp.out = pg.internal ? e->internal_out.get() : e->d_out[buf];
+    if (e->trace.get() && !pg.internal && e->seq - e->trace_first_seq < e->trace_cap) pp.trace = e->trace.get() + (e->seq - e->trace_first_seq) * 4;
     int rc = stamps ? launch_fused_variant<true>(e, pp) : launch_fused_variant<false>(e, pp);
     if (rc != BGR_OK) return rc;
     e->tiledep_chain = tiledep;
@@ -736,7 +728,7 @@ int launch_tma(bgr_engine* e, const uint8_t* src, uint8_t* dst, uint32_t n_rows_
     tp.order_base = e->cfg.order_base;
     tp.accum = save ? acc : nullptr;
     tp.words = e->words; tp.tile_bytes = e->tile_bytes; tp.stages = e->tma_stage_tiles;
-    tp.ticket = e->d_tma_ticket;
+    tp.ticket = e->tma_ticket.get();
     tp.n_tiles = e->tiles_for(n_rows_copy);
     tp.n_rows_src = n_rows_src;
     tp.count_alive = save ? 1u : 0u;
@@ -765,9 +757,9 @@ int run_stepwise(bgr_engine* e, const Program& pg, uint32_t buf) {
         NvtxRange span(span_name(op.kind == OP_SAVE ? uint32_t(BGR_REQ_SAVE) : op.kind == OP_LOAD ? uint32_t(BGR_REQ_LOAD) : uint32_t(BGR_REQ_ADVANCE)));
         switch (op.kind) {
         case OP_SAVE: {
-            unsigned long long* acc = e->d_accum + size_t(op.save_index) * kAccStride;
+            unsigned long long* acc = e->accum.get() + size_t(op.save_index) * kAccStride;
             if (e->tune_tma && e->tma_stage_tiles) {
-                int rc = launch_tma(e, live, e->arena + (size_t(op.image_off256) << 8), op.n_rows, op.n_rows, true, acc, !(op.flags & OPF_NO_STORE));
+                int rc = launch_tma(e, live, e->arena.ptr() + (size_t(op.image_off256) << 8), op.n_rows, op.n_rows, true, acc, !(op.flags & OPF_NO_STORE));
                 if (rc != BGR_OK) return rc;
                 break;
             }
@@ -787,7 +779,7 @@ int run_stepwise(bgr_engine* e, const Program& pg, uint32_t buf) {
             if (!(op.flags & OPF_NO_STORE) && op.n_rows > 0) {
                 uint32_t nt = e->tiles_for(op.n_rows);
                 k_copy_image<<<e->grid_for(uint32_t(size_t(nt) * e->tile_bytes / 16u), 256), 256, 0, e->stream>>>(
-                    live, e->arena + (size_t(op.image_off256) << 8), e->words, nt, op.n_rows);
+                    live, e->arena.ptr() + (size_t(op.image_off256) << 8), e->words, nt, op.n_rows);
                 e->launches += 1;
             }
             break;
@@ -795,12 +787,12 @@ int run_stepwise(bgr_engine* e, const Program& pg, uint32_t buf) {
         case OP_LOAD: {
             uint32_t n_copy = std::max(op.n_rows, live_rows);
             if (n_copy > 0 && e->tune_tma && e->tma_stage_tiles) {
-                int rc = launch_tma(e, e->arena + (size_t(op.image_off256) << 8), live, op.n_rows, n_copy, false, nullptr, true);
+                int rc = launch_tma(e, e->arena.ptr() + (size_t(op.image_off256) << 8), live, op.n_rows, n_copy, false, nullptr, true);
                 if (rc != BGR_OK) return rc;
             } else if (n_copy > 0) {
                 uint32_t nt = e->tiles_for(n_copy);
                 k_copy_image<<<e->grid_for(uint32_t(size_t(nt) * e->tile_bytes / 16u), 256), 256, 0, e->stream>>>(
-                    e->arena + (size_t(op.image_off256) << 8), live, e->words, nt, op.n_rows);
+                    e->arena.ptr() + (size_t(op.image_off256) << 8), live, e->words, nt, op.n_rows);
                 e->launches += 1;
             }
             live_rows = op.n_rows;
@@ -815,12 +807,12 @@ int run_stepwise(bgr_engine* e, const Program& pg, uint32_t buf) {
                 if (sy.id == BGR_SYS_PARTICLES_SPAWN) continue;  // Commands: applied after the schedule (below)
                 // despawn_on_input's run condition is host-known: no launch on frames whose input does not match
                 if (sy.id == BGR_SYS_DESPAWN_ON_INPUT && player_input(op, sy.param & 0xFFu) != (sy.param >> 8)) continue;
-                k_sys_rows<<<grid, 256, 0, e->stream>>>(live, e->words, n, sy, op, e->cfg.order_base, e->d_kill);
+                k_sys_rows<<<grid, 256, 0, e->stream>>>(live, e->words, n, sy, op, e->cfg.order_base, e->kill.ptr());
                 e->launches += 1;
                 any_despawn = any_despawn || e->sys_despawns[s];
             }
             if (any_despawn) {
-                k_apply_despawns<<<grid, 256, 0, e->stream>>>(live, e->words, n, e->d_kill);
+                k_apply_despawns<<<grid, 256, 0, e->stream>>>(live, e->words, n, e->kill.ptr());
                 e->launches += 1;
             }
             break;
@@ -832,12 +824,12 @@ int run_stepwise(bgr_engine* e, const Program& pg, uint32_t buf) {
             const uint64_t ttl = sy.params[1];
             k_sys_particles_spawn<<<e->grid_for(op.save_index, 256), 256, 0, e->stream>>>(
                 live, e->words, e->cols[sy.cols[0]].first_plane, e->cols[sy.cols[1]].first_plane, e->cols[sy.cols[2]].first_plane,
-                op.image_off256, op.save_index, e->d_spawn[buf] + op.call_count, uint32_t(ttl), uint32_t(ttl >> 32));
+                op.image_off256, op.save_index, e->spawn[buf].dev() + op.call_count, uint32_t(ttl), uint32_t(ttl >> 32));
             e->launches += 1;
             live_rows = std::max(live_rows, op.image_off256 + op.save_index);
         }
     }
-    k_publish<<<1, 128, 0, e->stream>>>(e->d_accum, e->d_out[buf], std::max(1u, pg.n_saves) * kAccStride, e->seq);
+    k_publish<<<1, 128, 0, e->stream>>>(e->accum.get(), e->d_out[buf], std::max(1u, pg.n_saves) * kAccStride, e->seq);
     e->launches += 1;
     CUDA_TRY(cudaGetLastError());
     e->last_kernel = (e->tune_tma && e->tma_stage_tiles) ? BGR_KERNEL_STEPWISE_TMA : BGR_KERNEL_STEPWISE_FLAT;
@@ -938,13 +930,13 @@ int run_generic(bgr_engine* e, const Program& pg, uint32_t buf) {
     e->tiledep_chain = false;
     GenericParams gp;
     std::memset(&gp, 0, sizeof gp);
-    gp.arena = e->arena;
+    gp.arena = e->arena.ptr();
     gp.order_base = e->cfg.order_base;
     gp.accum = e->d_accum_set[0];
     gp.ticket = e->d_ticket_set[0];
-    gp.out = pg.internal ? e->d_internal_out : e->d_out[buf];
+    gp.out = pg.internal ? e->internal_out.get() : e->d_out[buf];
     gp.seq = e->seq;
-    if (e->d_trace && !pg.internal && e->seq - e->trace_first_seq < e->trace_cap) gp.trace = e->d_trace + (e->seq - e->trace_first_seq) * 4;
+    if (e->trace.get() && !pg.internal && e->seq - e->trace_first_seq < e->trace_cap) gp.trace = e->trace.get() + (e->seq - e->trace_first_seq) * 4;
     gp.words = e->words; gp.tile_bytes = e->tile_bytes;
     gp.n_ops = pg.n_ops; gp.n_saves = pg.n_saves;
     gp.n_tiles = std::max(1u, e->tiles_for(pg.max_rows));
@@ -965,7 +957,7 @@ int run_generic(bgr_engine* e, const Program& pg, uint32_t buf) {
         // Overlap of consecutive launches: only when request vectors are queued behind each other (a synchronous caller
         // collects before its next submit), only on a stream the engine owns, and only between launches of the SAME kernel
         // over the SAME items (the per-item flags mean nothing across partitions: drain instead — rare, rows crossed a tile).
-        const bool tiledep = e->tune_jit_tiledep && e->d_item_done && e->own_stream && !pg.internal &&
+        const bool tiledep = e->tune_jit_tiledep && !e->item_done.empty() && e->own_stream && !pg.internal &&
                              (e->tune_jit_tiledep > 1 || !e->pending.empty());
         bool wait = false;
         if (prev_chain) {
@@ -974,7 +966,7 @@ int run_generic(bgr_engine* e, const Program& pg, uint32_t buf) {
         }
         if (tiledep) {
             gp.flags |= PF_TILE_SIGNAL;
-            gp.item_done = e->d_item_done;
+            gp.item_done = e->item_done.ptr<unsigned int>();
             gp.done_seq = uint32_t(e->seq);
             if (wait) { gp.flags |= PF_TILE_WAIT; gp.wait_seq = e->tiledep_seq; gp.wait_items = n_items; }
             // overlapping launches must not share accumulators / tickets: one set per in-flight request vector (run_fused)
@@ -1115,20 +1107,53 @@ DeferredLive plan_deferral(Program& pg) {
     return d;
 }
 
-// BGR_CFG_GROWABLE: maps every capacity-sized range for `tiles` tiles and zeroes the new bytes on the stream, behind
-// every queued launch.  Either every range grows or none does.  host_ns spent mapping: [0] the arena, [1] the rest.
+// A buffer whose size follows the row capacity: `n` strides of bytes(tiles) each for a capacity of `tiles` tiles.
+struct CapacityBuffer {
+    StridedRange* range;
+    uint32_t n;
+    size_t per_tile, fixed, align;
+    bool wanted;  // bgr_build creates it
+    size_t bytes(uint64_t tiles) const { return round_up(tiles * per_tile + fixed, align); }
+};
+
+// The reported state of a feed (one stride) and its per-tile counters tile_count / tile_off / tile_list (three).
+std::array<CapacityBuffer, 2> feed_buffers(bgr_engine::Feed& fd) {
+    return {{{&fd.rep, 1, tile_bytes_of(fd.p.rep_words), 0, 1, true}, {&fd.count, 3, sizeof(unsigned int), 0, 1, true}}};
+}
+
+// Every capacity-sized buffer: the engine's own first (the arena leads), then those of its feeds.
+std::vector<CapacityBuffer> capacity_buffers(bgr_engine* e) {
+    const uint32_t images = e->n_slots() + 1u;
+    const size_t u32 = sizeof(unsigned int);
+    std::vector<CapacityBuffer> v = {
+        {&e->arena, images, e->tile_bytes, 0, 256, true},  // ops address images in 256-byte units
+        {&e->kill, 1, kTileRows, 0, 1, true},
+        {&e->tile_done, 1, u32, u32, 1, e->tune_tiledep != 0},  // one word per tile and the grid's word behind them
+        {&e->tile_cnt, 1, u32, u32, 1, e->tune_tiledep != 0},
+        {&e->stamps, images, kSegsPerTile * kActivePlanes * sizeof(uint32_t), 0, 1, use_bundle(e)},  // one stride per image
+        // quarter-tile work items at most; a growable engine may compile the generated kernel later (grow_to)
+        {&e->item_done, 1, 4 * u32, 4 * u32, 1, e->tune_jit_tiledep && (e->growable() ? e->generic_ok : e->jit.fn != nullptr)},
+    };
+    for (auto& fd : e->feeds)
+        if (fd.used)
+            for (const CapacityBuffer& b : feed_buffers(fd)) v.push_back(b);
+    return v;
+}
+
+// The one place that knows how capacity buffers are allocated: a growable engine reserves address space for the
+// ceiling and maps nothing yet (map_tiles maps); any other engine allocates the capacity with cudaMalloc.
+bool create_range(bgr_engine* e, const CapacityBuffer& b, std::string* err) {
+    if (e->growable()) return b.range->reserve(e->cfg.device, b.n, b.bytes(e->ceiling / kTileRows), err);
+    return b.range->allocate(b.n, b.bytes(e->n_tiles_cap), err);
+}
+
+// Maps every capacity buffer for `tiles` tiles and zeroes the new bytes on the stream, behind every queued launch.
+// Either every range grows or none does.  host_ns spent mapping: [0] the arena, [1] the rest.
 int map_tiles(bgr_engine* e, uint64_t tiles, uint64_t* map_ns = nullptr) {
     struct Step { StridedRange* r; size_t bytes; size_t old; };
     std::vector<Step> steps;
-    auto add = [&](StridedRange& r, size_t bytes) { if (r.reserved()) steps.push_back({&r, bytes, r.mapped}); };
-    add(e->va_arena, tiles * e->tile_bytes);
-    add(e->va_stamps, tiles * kSegsPerTile * kActivePlanes * sizeof(uint32_t));
-    add(e->va_kill, tiles * kTileRows);
-    add(e->va_tile_done, (tiles + 1) * sizeof(unsigned int));
-    add(e->va_tile_cnt, (tiles + 1) * sizeof(unsigned int));
-    add(e->va_item_done, (4 * tiles + 4) * sizeof(unsigned int));
-    for (auto& fd : e->feeds)
-        if (fd.used) { add(fd.va_rep, tiles * tile_bytes_of(fd.p.rep_words)); add(fd.va_count, tiles * sizeof(unsigned int)); }
+    for (const CapacityBuffer& b : capacity_buffers(e))
+        if (!b.range->empty()) steps.push_back({b.range, b.bytes(tiles), b.range->mapped});
     std::string err;
     uint64_t t = host_ns();
     for (size_t i = 0; i < steps.size(); ++i) {
@@ -1154,7 +1179,7 @@ int grow_to(bgr_engine* e, uint64_t rows) {
     const uint64_t t0 = host_ns();
     // max(rows needed, 2 x capacity) in whole tiles, plus the tiles the arena's mapping granularity pays for anyway
     uint64_t tiles = (std::max<uint64_t>(rows, 2ull * e->cfg.max_entities) + kTileRows - 1) / kTileRows;
-    tiles = round_up(tiles * e->tile_bytes, e->va_arena.gran) / e->tile_bytes;
+    tiles = round_up(tiles * e->tile_bytes, e->arena.gran) / e->tile_bytes;
     tiles = std::min<uint64_t>(tiles, e->ceiling / kTileRows);
     uint64_t map_ns[2] = {0, 0};
     int rc = map_tiles(e, tiles, map_ns);
@@ -1202,7 +1227,7 @@ int submit(bgr_engine* e, const bgr_session_info* sess, const bgr_request* reqs,
         buf = ShardGroup::buf_of(e->gseq);
         e->group->publish_meta(e->gseq, pg.n_saves, e->n_ck, pg.save_frames, pg.save_totals);
     }
-    if (!pg.spawn_vals.empty()) std::memcpy(e->h_spawn[buf], pg.spawn_vals.data(), pg.spawn_vals.size() * sizeof(float2));
+    if (!pg.spawn_vals.empty()) std::memcpy(e->spawn[buf].get(), pg.spawn_vals.data(), pg.spawn_vals.size() * sizeof(float2));
     e->seq += 1;
     e->ticked = true;
     const bool bundle = use_bundle(e);
@@ -1217,7 +1242,7 @@ int submit(bgr_engine* e, const bgr_session_info* sess, const bgr_request* reqs,
     if (pg.defer_live) e->last_kernel |= BGR_KERNEL_DEFERRED_LIVE;
     if (pg.from_deferred) e->last_kernel |= BGR_KERNEL_FROM_DEFERRED;
     // an event between two launches would serialise them; with host polling it is only a fallback, taken lazily
-    if (!(e->tune_tiledep && e->tune_poll)) CUDA_TRY(cudaEventRecord(e->ev[buf], e->stream));
+    if (!(e->tune_tiledep && e->tune_poll)) CUDA_TRY(cudaEventRecord(e->ev[buf].get(), e->stream));
     e->last_fused = fused;
     e->st = s;
     e->deferred = next;
@@ -1280,7 +1305,7 @@ int collect(bgr_engine* e, bgr_checksum* out, uint32_t cap, uint32_t* n_out) {
     if (!done) {  // the event / the stream is ordered after the launch
         if (!pd.finished) {
             if (e->tune_tiledep && e->tune_poll) CUDA_TRY(cudaStreamSynchronize(e->stream));
-            else CUDA_TRY(cudaEventSynchronize(e->ev[pd.buf]));
+            else CUDA_TRY(cudaEventSynchronize(e->ev[pd.buf].get()));
         }
         if (!ready()) return fail(BGR_ERR_CUDA, "request vector completed without publishing valid results");
     }
@@ -1335,16 +1360,6 @@ int drain(bgr_engine* e) {
     return BGR_OK;
 }
 
-int ensure_stage(bgr_engine* e, size_t bytes) {
-    if (bytes <= e->stage_cap) return BGR_OK;
-    if (e->d_stage) CUDA_TRY(cudaFree(e->d_stage));
-    e->d_stage = nullptr; e->stage_cap = 0;
-    size_t cap = std::max<size_t>(bytes, 1u << 20);
-    CUDA_TRY(cudaMalloc(&e->d_stage, cap));
-    e->stage_cap = cap;
-    return BGR_OK;
-}
-
 // ECS column (array of T, `stride` bytes apart) <-> tile-planar image: one H2D/D2H copy of the AoS
 // bytes + one transposition kernel (k_scatter_column / k_gather_column).
 int transfer_column(bgr_engine* e, uint32_t image_idx, uint32_t column, uint32_t first, uint32_t count, void* host,
@@ -1359,25 +1374,24 @@ int transfer_column(bgr_engine* e, uint32_t image_idx, uint32_t column, uint32_t
     if (rc == BGR_OK && image_idx == 0) rc = touch_live(e);
     if (rc != BGR_OK) return rc;
     const size_t bytes = size_t(count) * stride;
-    rc = ensure_stage(e, bytes);
-    if (rc != BGR_OK) return rc;
+    CUDA_TRY(e->stage.ensure(std::max<size_t>(bytes, 1u << 20)));
     uint8_t* img = e->image(image_idx);
     uint32_t grid = e->grid_for(uint32_t(std::min<size_t>(size_t(count) * c.words, 0x7fffffffu)), 256);
     if (to_device) {
         e->st.live_passive_ver = ++e->st.ver_counter;  // host wrote a column: live content is new
-        CUDA_TRY(cudaMemcpyAsync(e->d_stage, host, bytes, cudaMemcpyHostToDevice, e->stream));
-        k_scatter_column<<<grid, 256, 0, e->stream>>>(img, e->words, c.first_plane, c.words, c.elem_bytes, first, count, e->d_stage, stride);
+        CUDA_TRY(cudaMemcpyAsync(e->stage.get(), host, bytes, cudaMemcpyHostToDevice, e->stream));
+        k_scatter_column<<<grid, 256, 0, e->stream>>>(img, e->words, c.first_plane, c.words, c.elem_bytes, first, count, e->stage.get(), stride);
         e->launches += 1;
         CUDA_TRY(cudaGetLastError());
         rc = clear_stamps(e, image_idx);
         if (rc != BGR_OK) return rc;
         CUDA_TRY(cudaStreamSynchronize(e->stream));
     } else {
-        if (stride != c.elem_bytes) CUDA_TRY(cudaMemcpyAsync(e->d_stage, host, bytes, cudaMemcpyHostToDevice, e->stream));  // keep the caller's padding bytes
-        k_gather_column<<<grid, 256, 0, e->stream>>>(img, e->words, c.first_plane, c.words, c.elem_bytes, first, count, e->d_stage, stride);
+        if (stride != c.elem_bytes) CUDA_TRY(cudaMemcpyAsync(e->stage.get(), host, bytes, cudaMemcpyHostToDevice, e->stream));  // keep the caller's padding bytes
+        k_gather_column<<<grid, 256, 0, e->stream>>>(img, e->words, c.first_plane, c.words, c.elem_bytes, first, count, e->stage.get(), stride);
         e->launches += 1;
         CUDA_TRY(cudaGetLastError());
-        CUDA_TRY(cudaMemcpyAsync(host, e->d_stage, bytes, cudaMemcpyDeviceToHost, e->stream));
+        CUDA_TRY(cudaMemcpyAsync(host, e->stage.get(), bytes, cudaMemcpyDeviceToHost, e->stream));
         CUDA_TRY(cudaStreamSynchronize(e->stream));
     }
     return BGR_OK;
@@ -1390,12 +1404,11 @@ int read_alive_image(bgr_engine* e, uint32_t image_idx, uint32_t first, uint32_t
     if (rc == BGR_OK && image_idx == 0) rc = touch_live(e);
     if (rc != BGR_OK) return rc;
     if (uint64_t(first) + count > e->cfg.max_entities) return fail(BGR_ERR_CAPACITY, "row range exceeds max_entities");
-    rc = ensure_stage(e, count);
-    if (rc != BGR_OK) return rc;
-    k_gather_alive<<<e->grid_for(count, 256), 256, 0, e->stream>>>(e->image(image_idx), e->words, first, count, n_rows, e->d_stage, need);
+    CUDA_TRY(e->stage.ensure(std::max<size_t>(count, 1u << 20)));
+    k_gather_alive<<<e->grid_for(count, 256), 256, 0, e->stream>>>(e->image(image_idx), e->words, first, count, n_rows, e->stage.get(), need);
     e->launches += 1;
     CUDA_TRY(cudaGetLastError());
-    CUDA_TRY(cudaMemcpyAsync(dst, e->d_stage, count, cudaMemcpyDeviceToHost, e->stream));
+    CUDA_TRY(cudaMemcpyAsync(dst, e->stage.get(), count, cudaMemcpyDeviceToHost, e->stream));
     CUDA_TRY(cudaStreamSynchronize(e->stream));
     return BGR_OK;
 }
@@ -1420,29 +1433,22 @@ int download_begin(bgr_engine* e, uint32_t column, uint32_t off, uint32_t len, u
     bgr_engine::Download& d = e->dl[slot];
     const size_t bytes = size_t(count) * len;
     if (!e->copy_stream) CUDA_TRY(cudaStreamCreateWithFlags(&e->copy_stream, cudaStreamNonBlocking));
-    if (!d.packed) {
-        CUDA_TRY(cudaEventCreateWithFlags(&d.packed, cudaEventDisableTiming));
-        CUDA_TRY(cudaEventCreateWithFlags(&d.done, cudaEventDisableTiming));
-    }
-    if (bytes > d.cap) {  // grows to the largest request and stays (the slot is idle: its last copy was waited for)
-        if (d.d_buf) CUDA_TRY(cudaFree(d.d_buf));
-        d.d_buf = nullptr; d.cap = 0;
-        CUDA_TRY(cudaMalloc(&d.d_buf, bytes));
-        d.cap = bytes;
-    }
+    CUDA_TRY(d.packed.ensure());
+    CUDA_TRY(d.done.ensure());
+    CUDA_TRY(d.buf.ensure(bytes));  // the slot is idle: its last copy was waited for
     if (count) {
         const uint32_t n_words = len / 4u;
         const uint32_t grid = e->grid_for(uint32_t(std::min<size_t>(size_t(count) * n_words, 0x7fffffffu)), 256);
         k_gather_fields<<<grid, 256, 0, e->stream>>>(e->image(0), e->words, c.first_plane + off / 4u, n_words, first, count,
-                                                      reinterpret_cast<uint32_t*>(d.d_buf));
+                                                      reinterpret_cast<uint32_t*>(d.buf.get()));
         e->launches += 1;
         CUDA_TRY(cudaGetLastError());
         e->tiledep_chain = false;
-        CUDA_TRY(cudaEventRecord(d.packed, e->stream));
-        CUDA_TRY(cudaStreamWaitEvent(e->copy_stream, d.packed, 0));
-        CUDA_TRY(cudaMemcpyAsync(host, d.d_buf, bytes, cudaMemcpyDeviceToHost, e->copy_stream));
+        CUDA_TRY(cudaEventRecord(d.packed.get(), e->stream));
+        CUDA_TRY(cudaStreamWaitEvent(e->copy_stream, d.packed.get(), 0));
+        CUDA_TRY(cudaMemcpyAsync(host, d.buf.get(), bytes, cudaMemcpyDeviceToHost, e->copy_stream));
     }
-    CUDA_TRY(cudaEventRecord(d.done, e->copy_stream));
+    CUDA_TRY(cudaEventRecord(d.done.get(), e->copy_stream));
     d.busy = true;
     e->next_dl = (slot + 1) % BGR_MAX_DOWNLOADS;
     *ticket_out = slot;
@@ -1452,7 +1458,7 @@ int download_begin(bgr_engine* e, uint32_t column, uint32_t off, uint32_t len, u
 int download_wait(bgr_engine* e, uint32_t ticket) {
     if (!e) return fail(BGR_ERR_INVALID_ARGUMENT, "null engine");
     if (ticket >= BGR_MAX_DOWNLOADS || !e->dl[ticket].busy) return fail(BGR_ERR_STATE, "no such download in flight");
-    CUDA_TRY(cudaEventSynchronize(e->dl[ticket].done));
+    CUDA_TRY(cudaEventSynchronize(e->dl[ticket].done.get()));
     e->dl[ticket].busy = false;
     return BGR_OK;
 }
@@ -1483,48 +1489,29 @@ int feed_create(bgr_engine* e, const bgr_feed_field* fields, uint32_t n_fields, 
     p.words = e->words;
     p.record_words = 2u + p.rep_words;
     bgr_engine::Feed& fd = e->feeds[id];
-    auto cleanup = [&]() {
-        if (fd.va_rep.reserved()) { cudaStreamSynchronize(e->stream); fd.va_rep.free(); fd.va_count.free(); }
-        else { cudaFree(fd.p.rep); cudaFree(fd.p.tile_count); }
-        cudaFree(fd.p.info);
-        if (fd.h_info) cudaFreeHost(fd.h_info);
-        if (fd.packed) cudaEventDestroy(fd.packed);
-        if (fd.done) cudaEventDestroy(fd.done);
-        fd = bgr_engine::Feed{};
-    };
     fd.p = p;
-    const uint32_t tiles = e->n_tiles_cap;
-    cudaError_t ce = cudaSuccess;
-    size_t count_stride = tiles;  // words between tile_count, tile_off and tile_list
-    if (e->growable()) {  // reserved for the ceiling and grown with the engine (grow_to): the pointers never change
-        std::string err;
-        const uint64_t ceil_tiles = e->ceiling / kTileRows;
-        if (!fd.va_rep.reserve(e->cfg.device, 1, ceil_tiles * tile_bytes_of(p.rep_words), &err) ||
-            !fd.va_count.reserve(e->cfg.device, 3, ceil_tiles * sizeof(unsigned int), &err) ||
-            !fd.va_rep.map_to(size_t(tiles) * tile_bytes_of(p.rep_words), &err) || !fd.va_count.map_to(size_t(tiles) * sizeof(unsigned int), &err)) {
-            cleanup();
-            return fail(BGR_ERR_CUDA, "bgr_feed_create: " + err);
-        }
-        ce = fd.va_rep.zero_new(e->stream);
-        if (ce == cudaSuccess) ce = fd.va_count.zero_new(e->stream);
-        fd.p.rep = fd.va_rep.ptr();
-        fd.p.tile_count = fd.va_count.ptr<unsigned int>();
-        count_stride = fd.va_count.stride / sizeof(unsigned int);
-    } else {
-        ce = cudaMalloc(&fd.p.rep, size_t(tiles) * tile_bytes_of(p.rep_words));
-        if (ce == cudaSuccess) ce = cudaMalloc(&fd.p.tile_count, size_t(3) * tiles * sizeof(unsigned int));
-    }
-    if (ce == cudaSuccess) ce = cudaMalloc(&fd.p.info, 8 * sizeof(unsigned int));
-    if (ce == cudaSuccess) ce = cudaHostAlloc(&fd.h_info, 4 * sizeof(unsigned int), cudaHostAllocMapped);
-    if (ce == cudaSuccess) ce = cudaEventCreateWithFlags(&fd.packed, cudaEventDisableTiming);
-    if (ce == cudaSuccess) ce = cudaEventCreateWithFlags(&fd.done, cudaEventDisableTiming);
+    std::string err;
+    bool ok = true;
+    for (const CapacityBuffer& b : feed_buffers(fd))
+        ok = ok && create_range(e, b, &err) && b.range->map_to(b.bytes(e->n_tiles_cap), &err);
+    cudaError_t ce = ok ? cudaSuccess : cudaErrorMemoryAllocation;
     // the reported state starts as (0, zeros) on every row; ordered before any pass on the engine stream
-    if (ce == cudaSuccess) ce = cudaMemsetAsync(fd.p.rep, 0, size_t(tiles) * tile_bytes_of(p.rep_words), e->stream);
+    if (ce == cudaSuccess) ce = fd.rep.zero_new(e->stream);
+    if (ce == cudaSuccess) ce = fd.count.zero_new(e->stream);
+    if (ce == cudaSuccess) ce = fd.info.ensure(8);
+    if (ce == cudaSuccess) ce = fd.h_info.ensure(4);
+    if (ce == cudaSuccess) ce = fd.packed.ensure();
+    if (ce == cudaSuccess) ce = fd.done.ensure();
     if (ce == cudaSuccess && !e->copy_stream) ce = cudaStreamCreateWithFlags(&e->copy_stream, cudaStreamNonBlocking);
     if (ce != cudaSuccess) {
-        cleanup();
-        return fail(BGR_ERR_CUDA, std::string("bgr_feed_create: ") + cudaGetErrorString(ce));
+        cudaStreamSynchronize(e->stream);  // a memset may be queued on the ranges released here
+        fd = bgr_engine::Feed{};
+        return fail(BGR_ERR_CUDA, "bgr_feed_create: " + (ok ? std::string(cudaGetErrorString(ce)) : err));
     }
+    const size_t count_stride = fd.count.stride / sizeof(unsigned int);  // words between tile_count, tile_off and tile_list
+    fd.p.rep = fd.rep.ptr();
+    fd.p.tile_count = fd.count.ptr<unsigned int>();
+    fd.p.info = fd.info.get();
     fd.p.tile_off = fd.p.tile_count + count_stride;
     fd.p.tile_list = fd.p.tile_off + count_stride;
     fd.used = true;
@@ -1561,12 +1548,8 @@ int feed_begin(bgr_engine* e, uint32_t feed, void* host, uint32_t cap, uint32_t*
     }
     // no report has more records than the rows it compares
     const uint32_t cap_eff = std::min<uint64_t>(cap, uint64_t(e->n_tiles_cap) * kTileRows);
-    if (cap_eff > fd.stage_records) {  // grows to the largest cap and stays (no report of this feed is in flight)
-        if (fd.p.out) CUDA_TRY(cudaFree(fd.p.out));
-        fd.p.out = nullptr; fd.stage_records = 0;
-        CUDA_TRY(cudaMalloc(&fd.p.out, size_t(cap_eff) * fd.p.record_words * 4u));
-        fd.stage_records = cap_eff;
-    }
+    CUDA_TRY(fd.out.ensure(size_t(cap_eff) * fd.p.record_words));  // no report of this feed is in flight
+    fd.p.out = fd.out.get();
     int rc = touch_live(e);  // stream-ordered behind the queued submits, like the passes below
     if (rc != BGR_OK) return rc;
     FeedParams p = fd.p;
@@ -1587,15 +1570,15 @@ int feed_begin(bgr_engine* e, uint32_t feed, void* host, uint32_t cap, uint32_t*
     CUDA_TRY(cudaGetLastError());
     e->tiledep_chain = false;
     fd.bound = std::max(fd.bound, p.rows);
-    CUDA_TRY(cudaEventRecord(fd.packed, e->stream));
-    CUDA_TRY(cudaStreamWaitEvent(e->copy_stream, fd.packed, 0));
+    CUDA_TRY(cudaEventRecord(fd.packed.get(), e->stream));
+    CUDA_TRY(cudaStreamWaitEvent(e->copy_stream, fd.packed.get(), 0));
     if (cap) {
         k_feed_copy<<<std::max(1, e->num_sms), 256, 0, e->copy_stream>>>(p.out, p.info, host_dev);
         e->launches += 1;
         CUDA_TRY(cudaGetLastError());
     }
-    CUDA_TRY(cudaMemcpyAsync(fd.h_info, p.info, 4 * sizeof(unsigned int), cudaMemcpyDeviceToHost, e->copy_stream));
-    CUDA_TRY(cudaEventRecord(fd.done, e->copy_stream));
+    CUDA_TRY(cudaMemcpyAsync(fd.h_info.get(), p.info, 4 * sizeof(unsigned int), cudaMemcpyDeviceToHost, e->copy_stream));
+    CUDA_TRY(cudaEventRecord(fd.done.get(), e->copy_stream));
     fd.busy = true;
     e->feed_seq = (e->feed_seq + 1u) & 0x0FFFFFFFu;
     fd.ticket = feed + BGR_MAX_FEEDS * e->feed_seq;
@@ -1607,10 +1590,10 @@ int feed_wait(bgr_engine* e, uint32_t ticket, bgr_feed_info* info) {
     if (!e) return fail(BGR_ERR_INVALID_ARGUMENT, "null engine");
     bgr_engine::Feed& fd = e->feeds[ticket % BGR_MAX_FEEDS];
     if (!fd.used || !fd.busy || fd.ticket != ticket) return fail(BGR_ERR_STATE, "no such feed report in flight");
-    CUDA_TRY(cudaEventSynchronize(fd.done));
+    CUDA_TRY(cudaEventSynchronize(fd.done.get()));
     fd.busy = false;
     if (info) {
-        const volatile unsigned int* h = fd.h_info;
+        const volatile unsigned int* h = fd.h_info.get();
         info->n_records = h[0]; info->pending = h[1]; info->rows = h[2]; info->record_bytes = h[3];
     }
     return BGR_OK;
@@ -1668,7 +1651,7 @@ int validate_edits(bgr_engine* e, const bgr_edit* edits, uint32_t n, size_t valu
 
 int fold_edits(bgr_engine* e, const bgr_edit* edits, uint32_t n, const uint8_t* values, EditFold& f) {
     if (f.passive.size() != e->words) {
-        if (e->d_stamps) {
+        if (!e->stamps.empty()) {
             f.stamp_q.assign(e->words, -1);
             for (uint32_t k = 0; k < 3; ++k) {
                 f.stamp_q[e->cols[e->bt].first_plane + k] = int8_t(k);
@@ -1795,28 +1778,21 @@ int apply_edits(bgr_engine* e, const bgr_edit* edits, uint32_t n, const void* va
     bgr_engine::EditStage& sg = e->edit_stage[e->next_edit];
     const size_t bytes_w = f.words.size() * sizeof(uint4), bytes_m = f.masks.size() * sizeof(uint2);
     const size_t bytes = bytes_w + bytes_m + f.stamps.size() * sizeof(uint32_t);
-    if (!sg.done) CUDA_TRY(cudaEventCreateWithFlags(&sg.done, cudaEventDisableTiming));
-    if (sg.busy) CUDA_TRY(cudaEventSynchronize(sg.done));
+    CUDA_TRY(sg.done.ensure());
+    if (sg.busy) CUDA_TRY(cudaEventSynchronize(sg.done.get()));
     sg.busy = false;
     // Grows to the largest batch and stays (16 B per stored word): freeing the smaller buffer synchronises the device.
     // Even an empty patch gets a buffer, so that the kernel always has a mapped address to read from.
-    if (!sg.h || bytes > sg.cap) {
-        if (sg.h) CUDA_TRY(cudaFreeHost(sg.h));
-        sg.h = nullptr; sg.cap = 0;
-        const size_t cap = std::max<size_t>(bytes, 64u << 10);
-        CUDA_TRY(cudaHostAlloc(&sg.h, cap, cudaHostAllocMapped));
-        sg.cap = cap;
-    }
+    CUDA_TRY(sg.h.ensure(std::max<size_t>(bytes, 64u << 10)));
     // nothing fails past the capacity: growing is the last step that can refuse
     if (rows > e->st.n_rows) rc = grow_to(e, rows);
     if (rc == BGR_OK) rc = touch_live(e);  // stream-ordered behind the queued submits, like the launches below
     if (rc != BGR_OK) return rc;
-    uint4* hw = reinterpret_cast<uint4*>(sg.h);
+    uint4* hw = reinterpret_cast<uint4*>(sg.h.get());
     for (size_t k = 0; k < f.words.size(); ++k) hw[k] = make_uint4(f.words[k].row, f.words[k].plane, f.words[k].value, 0u);
-    if (bytes_m) std::memcpy(sg.h + bytes_w, f.masks.data(), bytes_m);
-    if (!f.stamps.empty()) std::memcpy(sg.h + bytes_w + bytes_m, f.stamps.data(), f.stamps.size() * sizeof(uint32_t));
-    uint8_t* dev = nullptr;
-    CUDA_TRY(cudaHostGetDevicePointer(reinterpret_cast<void**>(&dev), sg.h, 0));
+    if (bytes_m) std::memcpy(sg.h.get() + bytes_w, f.masks.data(), bytes_m);
+    if (!f.stamps.empty()) std::memcpy(sg.h.get() + bytes_w + bytes_m, f.stamps.data(), f.stamps.size() * sizeof(uint32_t));
+    const uint8_t* dev = sg.h.dev();
     if (rows > e->st.n_rows) {
         const uint32_t count = uint32_t(rows - e->st.n_rows);
         k_spawn_rows<<<e->grid_for(count, 64), 256, 0, e->stream>>>(e->image(0), e->words, e->st.n_rows, count);
@@ -1829,10 +1805,10 @@ int apply_edits(bgr_engine* e, const bgr_edit* edits, uint32_t n, const void* va
     p.stamps = reinterpret_cast<const uint32_t*>(dev + bytes_w + bytes_m);
     p.n_words = uint32_t(f.words.size()); p.n_masks = uint32_t(f.masks.size()); p.n_stamps = uint32_t(f.stamps.size());
     const uint32_t total = p.n_words + p.n_masks + p.n_stamps;
-    k_apply_edits<<<e->grid_for(total, 256), 256, 0, e->stream>>>(e->image(0), e->words, e->d_stamps, p);
+    k_apply_edits<<<e->grid_for(total, 256), 256, 0, e->stream>>>(e->image(0), e->words, e->stamps.ptr<uint32_t>(), p);
     e->launches += 1;
     CUDA_TRY(cudaGetLastError());
-    CUDA_TRY(cudaEventRecord(sg.done, e->stream));
+    CUDA_TRY(cudaEventRecord(sg.done.get(), e->stream));
     sg.busy = true;
     e->next_edit = (e->next_edit + 1) % bgr_engine::kEditBufs;
     e->tiledep_chain = false;
@@ -1887,6 +1863,20 @@ void detect_bundles(bgr_engine* e) {
     e->bundle_static_ck = ck_t && ck_v && fin_t && fin_v;
     e->bt = t; e->bv = v; e->bl = l;
     e->bundle_particles = true;
+}
+
+// Points the result views h_out / d_out at the engine's own blocks (outside a shard group).
+void use_own_blocks(bgr_engine* e) {
+    for (int b = 0; b < bgr_engine::kBufs; ++b) { e->h_out[b] = e->out_block[b].get(); e->d_out[b] = e->out_block[b].dev(); }
+}
+
+// Unregisters the group's segment and points the result views back at the engine's own blocks (the caller has
+// synchronised the stream).
+void leave_group(bgr_engine* e) {
+    cudaHostUnregister(e->group->blocks_base());
+    use_own_blocks(e);
+    delete e->group;
+    e->group = nullptr;
 }
 
 }  // namespace
@@ -1959,67 +1949,13 @@ BGR_API int bgr_engine_create(const bgr_config* cfg, bgr_engine** out) {
 BGR_API void bgr_engine_destroy(bgr_engine* e) {
     if (!e) return;
     cudaSetDevice(e->cfg.device);
+    // nothing is released while a stream that could still use it runs
     if (e->stream) cudaStreamSynchronize(e->stream);
-    if (e->group) {
-        cudaHostUnregister(e->group->blocks_base());
-        for (int b = 0; b < bgr_engine::kBufs; ++b) { e->h_out[b] = e->own_h_out[b]; e->d_out[b] = e->own_d_out[b]; }
-        delete e->group;
-        e->group = nullptr;
-    }
-    if (e->d_trace) cudaFree(e->d_trace);
-    if (e->va_arena.reserved()) e->arena = nullptr;
-    if (e->va_stamps.reserved()) e->d_stamps = nullptr;
-    if (e->va_kill.reserved()) e->d_kill = nullptr;
-    if (e->va_tile_done.reserved()) e->d_tile_done = nullptr;
-    if (e->va_tile_cnt.reserved()) e->d_tile_cnt = nullptr;
-    if (e->va_item_done.reserved()) e->d_item_done = nullptr;
-    for (StridedRange* r : {&e->va_arena, &e->va_stamps, &e->va_kill, &e->va_tile_done, &e->va_tile_cnt, &e->va_item_done}) r->free();
-    for (int i = 0; i < bgr_engine::kBufs; ++i) {
-        if (e->h_out[i]) cudaFreeHost(e->h_out[i]);
-        if (e->h_spawn[i]) cudaFreeHost(e->h_spawn[i]);
-        if (e->ev[i]) cudaEventDestroy(e->ev[i]);
-    }
-    if (e->arena) cudaFree(e->arena);
-    if (e->d_stamps) cudaFree(e->d_stamps);
-    if (e->d_kill) cudaFree(e->d_kill);
-    if (e->d_stage) cudaFree(e->d_stage);
-    if (e->d_accum) cudaFree(e->d_accum);
-    if (e->d_ticket) cudaFree(e->d_ticket);
-    if (e->d_internal_out) cudaFree(e->d_internal_out);
     if (e->copy_stream) { cudaStreamSynchronize(e->copy_stream); cudaStreamDestroy(e->copy_stream); }
-    if (e->d_tma_ticket) cudaFree(e->d_tma_ticket);
-    if (e->d_tile_done) cudaFree(e->d_tile_done);
-    if (e->d_tile_cnt) cudaFree(e->d_tile_cnt);
-    if (e->d_item_done) cudaFree(e->d_item_done);
-    if (e->d_diff_cols) cudaFree(e->d_diff_cols);
-    if (e->d_diff_counts) cudaFree(e->d_diff_counts);
-    if (e->d_diff_totals) cudaFree(e->d_diff_totals);
-    if (e->d_diff_list) cudaFree(e->d_diff_list);
-    if (e->d_diff_records) cudaFree(e->d_diff_records);
-    if (e->d_digest_cols) cudaFree(e->d_digest_cols);
-    if (e->d_digest_words) cudaFree(e->d_digest_words);
-    if (e->d_digest_active) cudaFree(e->d_digest_active);
-    if (e->d_remote) cudaFree(e->d_remote);
-    if (e->d_remote_visit) cudaFree(e->d_remote_visit);
-    for (auto& d : e->dl) {
-        if (d.d_buf) cudaFree(d.d_buf);
-        if (d.packed) cudaEventDestroy(d.packed);
-        if (d.done) cudaEventDestroy(d.done);
-    }
-    for (auto& s : e->edit_stage) {
-        if (s.h) cudaFreeHost(s.h);
-        if (s.done) cudaEventDestroy(s.done);
-    }
-    for (auto& f : e->feeds) {
-        if (!f.used) continue;
-        if (f.va_rep.reserved()) { f.va_rep.free(); f.va_count.free(); }
-        else { cudaFree(f.p.rep); cudaFree(f.p.tile_count); }
-        cudaFree(f.p.info); cudaFree(f.p.out);
-        cudaFreeHost(f.h_info);
-        cudaEventDestroy(f.packed); cudaEventDestroy(f.done);
-    }
-    if (e->own_stream && e->stream) cudaStreamDestroy(e->stream);
+    if (e->group) leave_group(e);
+    cudaStream_t own = e->own_stream ? e->stream : nullptr;
     delete e;
+    if (own) cudaStreamDestroy(own);
 }
 
 BGR_API int bgr_rollback_component(bgr_engine* e, const char* type_name, uint32_t elem_bytes, uint32_t strategy,
@@ -2143,100 +2079,49 @@ BGR_API int bgr_build(bgr_engine* e) {
                                                   std::to_string(SlotRing::kMaxSlots));
     if ((e->image_bytes * (size_t(e->n_slots()) + 1u)) >> 8 > 0xffffffffull)
         return fail(BGR_ERR_CAPACITY, "arena larger than 1 TB");
-    const uint32_t images = e->n_slots() + 1u;
     e->ceiling = e->cfg.max_entities;
-    uint64_t ceil_tiles = e->n_tiles_cap;
-    std::string va_err;
     if (e->growable()) {
         // The ceiling: ops address images in 256-byte units with 32 bits, so all images together stay within 1 TB, and a
         // row index is 32 bits.  Every image gets a stride of whole mapping granules sized for the ceiling.
-        const size_t gran = StridedRange::granularity(e->cfg.device, &va_err);
-        if (!gran) return fail(BGR_ERR_CUDA, va_err);
-        const uint64_t per_image = ((uint64_t(1) << 40) / images) / gran * gran;
-        ceil_tiles = std::min<uint64_t>(per_image / e->tile_bytes, 0xFFFFFFFFull / kTileRows);
+        std::string err;
+        const size_t gran = StridedRange::granularity(e->cfg.device, &err);
+        if (!gran) return fail(BGR_ERR_CUDA, err);
+        const uint64_t per_image = ((uint64_t(1) << 40) / (e->n_slots() + 1u)) / gran * gran;
+        const uint64_t ceil_tiles = std::min<uint64_t>(per_image / e->tile_bytes, 0xFFFFFFFFull / kTileRows);
         if (ceil_tiles < e->n_tiles_cap)
             return fail(BGR_ERR_CAPACITY, "max_entities exceeds the ceiling of a growable engine with this schema and slot count (" +
                                               std::to_string(ceil_tiles * kTileRows) + " rows)");
         e->ceiling = uint32_t(ceil_tiles * kTileRows);
-        if (!e->va_arena.reserve(e->cfg.device, images, ceil_tiles * e->tile_bytes, &va_err) ||
-            !e->va_kill.reserve(e->cfg.device, 1, ceil_tiles * kTileRows, &va_err))
-            return fail(BGR_ERR_CUDA, va_err);
-        e->image_bytes = e->va_arena.stride;
-        e->arena = e->va_arena.ptr();
-        e->d_kill = e->va_kill.ptr();
-    } else {
-        size_t total = e->image_bytes * (size_t(e->n_slots()) + 1u);
-        CUDA_TRY(cudaMalloc(&e->arena, total));
-        CUDA_TRY(cudaMemsetAsync(e->arena, 0, total, e->stream));
-        CUDA_TRY(cudaMalloc(&e->d_kill, e->epad));
-        CUDA_TRY(cudaMemsetAsync(e->d_kill, 0, e->epad, e->stream));
     }
     const size_t acc_bytes = sizeof(unsigned long long) * kMaxSaves * kAccStride;
-    CUDA_TRY(cudaMalloc(&e->d_accum, acc_bytes * bgr_engine::kBufs));
-    CUDA_TRY(cudaMemsetAsync(e->d_accum, 0, acc_bytes * bgr_engine::kBufs, e->stream));
-    CUDA_TRY(cudaMalloc(&e->d_ticket, 4 * sizeof(unsigned int) * bgr_engine::kBufs));
-    CUDA_TRY(cudaMemsetAsync(e->d_ticket, 0, 4 * sizeof(unsigned int) * bgr_engine::kBufs, e->stream));
+    CUDA_TRY(e->accum.ensure(kMaxSaves * kAccStride * bgr_engine::kBufs));
+    CUDA_TRY(cudaMemsetAsync(e->accum.get(), 0, acc_bytes * bgr_engine::kBufs, e->stream));
+    CUDA_TRY(e->ticket.ensure(4 * bgr_engine::kBufs));
+    CUDA_TRY(cudaMemsetAsync(e->ticket.get(), 0, 4 * sizeof(unsigned int) * bgr_engine::kBufs, e->stream));
     for (int s = 0; s < bgr_engine::kBufs; ++s) {
-        e->d_accum_set[s] = e->d_accum + size_t(s) * kMaxSaves * kAccStride;
-        e->d_ticket_set[s] = e->d_ticket + 4 * s;
+        e->d_accum_set[s] = e->accum.get() + size_t(s) * kMaxSaves * kAccStride;
+        e->d_ticket_set[s] = e->ticket.get() + 4 * s;
     }
-    if (e->tune_tiledep && e->growable()) {
-        if (!e->va_tile_done.reserve(e->cfg.device, 1, (ceil_tiles + 1) * sizeof(unsigned int), &va_err) ||
-            !e->va_tile_cnt.reserve(e->cfg.device, 1, (ceil_tiles + 1) * sizeof(unsigned int), &va_err))
-            return fail(BGR_ERR_CUDA, va_err);
-        e->d_tile_done = e->va_tile_done.ptr<unsigned int>();
-        e->d_tile_cnt = e->va_tile_cnt.ptr<unsigned int>();
-    } else if (e->tune_tiledep) {
-        const size_t nt = size_t(e->tiles_for(e->cfg.max_entities)) + 1;
-        CUDA_TRY(cudaMalloc(&e->d_tile_done, nt * sizeof(unsigned int)));
-        CUDA_TRY(cudaMalloc(&e->d_tile_cnt, nt * sizeof(unsigned int)));
-        CUDA_TRY(cudaMemsetAsync(e->d_tile_done, 0, nt * sizeof(unsigned int), e->stream));
-        CUDA_TRY(cudaMemsetAsync(e->d_tile_cnt, 0, nt * sizeof(unsigned int), e->stream));
-    }
-    CUDA_TRY(cudaMalloc(&e->d_internal_out, sizeof(unsigned long long) * kResultStride));
+    CUDA_TRY(e->internal_out.ensure(kResultStride));
     for (int i = 0; i < bgr_engine::kBufs; ++i) {
-        const size_t out_bytes = sizeof(unsigned long long) * kResultStride;
-        CUDA_TRY(cudaHostAlloc(&e->h_out[i], out_bytes, cudaHostAllocMapped));
-        std::memset(e->h_out[i], 0, out_bytes);
-        CUDA_TRY(cudaHostGetDevicePointer(&e->d_out[i], e->h_out[i], 0));
-        CUDA_TRY(cudaEventCreateWithFlags(&e->ev[i], cudaEventDisableTiming));
+        CUDA_TRY(e->out_block[i].ensure(kResultStride));
+        std::memset(e->out_block[i].get(), 0, sizeof(unsigned long long) * kResultStride);
+        CUDA_TRY(e->ev[i].ensure());
     }
+    use_own_blocks(e);
     e->st.ring.reset(e->n_slots(), e->capture());
     e->st.ring.set_retention(e->retain_interval, e->retain_count);
     e->st.slot_rows.fill(0);
     e->st.slot_elapsed_ns.fill(0);
     e->st.slot_passive_ver.fill(0);
     if (e->spawn_sys >= 0)
-        for (int i = 0; i < bgr_engine::kBufs; ++i) {
-            CUDA_TRY(cudaHostAlloc(&e->h_spawn[i], sizeof(float2) * kMaxSpawnVals, cudaHostAllocMapped));
-            CUDA_TRY(cudaHostGetDevicePointer(&e->d_spawn[i], e->h_spawn[i], 0));
-        }
+        for (int i = 0; i < bgr_engine::kBufs; ++i) CUDA_TRY(e->spawn[i].ensure(kMaxSpawnVals));
     build_specs(e);
     detect_bundles(e);
-    if (use_bundle(e) && e->growable()) {  // one stride per image row of the table
-        if (!e->va_stamps.reserve(e->cfg.device, images, ceil_tiles * kSegsPerTile * kActivePlanes * sizeof(uint32_t), &va_err))
-            return fail(BGR_ERR_CUDA, va_err);
-        e->stamp_image = uint32_t(e->va_stamps.stride / sizeof(uint32_t));
-        e->d_stamps = e->va_stamps.ptr<uint32_t>();
-    } else if (use_bundle(e)) {  // content stamps of the active planes: every image, every 64-row segment
-        e->stamp_image = e->n_tiles_cap * kSegsPerTile * kActivePlanes;
-        const size_t bytes = size_t(e->stamp_image) * (e->n_slots() + 1u) * sizeof(uint32_t);
-        CUDA_TRY(cudaMalloc(&e->d_stamps, bytes));
-        CUDA_TRY(cudaMemsetAsync(e->d_stamps, 0, bytes, e->stream));
-    }
     // generic one-launch program: every row system runs on its tile (run_system); spawning is a Command of the stepwise
     // path; the parameter block holds kMaxGenericSys systems; the tile fits twice per SM
     e->generic_ok = e->spawn_sys < 0 && e->sys_specs.size() <= size_t(kMaxGenericSys) && e->tile_bytes <= 100u * 1024u;
     jit_specialise(e);
-    if (e->growable() && e->generic_ok && e->tune_jit_tiledep) {  // growth may compile the kernel later
-        if (!e->va_item_done.reserve(e->cfg.device, 1, (4 * ceil_tiles + 4) * sizeof(unsigned int), &va_err))
-            return fail(BGR_ERR_CUDA, va_err);
-        e->d_item_done = e->va_item_done.ptr<unsigned int>();
-    } else if (e->jit.fn && e->tune_jit_tiledep) {
-        const size_t ni = size_t(e->tiles_for(e->cfg.max_entities)) * 4 + 4;
-        CUDA_TRY(cudaMalloc(&e->d_item_done, ni * sizeof(unsigned int)));
-        CUDA_TRY(cudaMemsetAsync(e->d_item_done, 0, ni * sizeof(unsigned int), e->stream));
-    }
     {   // TMA copy kernel: up to six one-tile stages in ~200 KB of shared memory, at least two
         uint32_t st = uint32_t(std::min<size_t>((200u * 1024u) / e->tile_bytes, size_t(kTmaMaxStages)));
         if (env_int("BGR_TUNE_TMA_STAGES", 0) > 0) st = std::min(st, uint32_t(env_int("BGR_TUNE_TMA_STAGES", 0)));
@@ -2244,14 +2129,16 @@ BGR_API int bgr_build(bgr_engine* e) {
         if (e->tma_stage_tiles) {
             size_t smem = size_t(e->tma_stage_tiles) * e->tile_bytes;
             CUDA_TRY(cudaFuncSetAttribute(k_image_tma, cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem)));
-            CUDA_TRY(cudaMalloc(&e->d_tma_ticket, 4 * sizeof(unsigned int)));
-            CUDA_TRY(cudaMemsetAsync(e->d_tma_ticket, 0, 4 * sizeof(unsigned int), e->stream));
+            CUDA_TRY(e->tma_ticket.ensure(4));
+            CUDA_TRY(cudaMemsetAsync(e->tma_ticket.get(), 0, 4 * sizeof(unsigned int), e->stream));
         }
     }
-    if (e->growable()) {
-        const int rc = map_tiles(e, e->n_tiles_cap);
-        if (rc != BGR_OK) return rc;
-    }
+    std::string err;
+    for (const CapacityBuffer& b : capacity_buffers(e))
+        if (b.wanted && !create_range(e, b, &err)) return fail(BGR_ERR_CUDA, err);
+    e->image_bytes = e->arena.stride;
+    const int rc = map_tiles(e, e->n_tiles_cap);  // maps the capacity and zeroes every capacity buffer
+    if (rc != BGR_OK) return rc;
     CUDA_TRY(cudaStreamSynchronize(e->stream));
     e->built = true;
     return BGR_OK;
@@ -2272,13 +2159,13 @@ BGR_API int bgr_run_startup_system(bgr_engine* e, uint32_t system) {
         if (rc != BGR_OK) return rc;
     }
     for (uint32_t k = 0; k < rate; ++k) {
-        e->h_spawn[0][k].x = e->st.rng.random_range(-200.0f, 200.0f);
-        e->h_spawn[0][k].y = e->st.rng.random_range(-200.0f, 200.0f);
+        e->spawn[0].get()[k].x = e->st.rng.random_range(-200.0f, 200.0f);
+        e->spawn[0].get()[k].y = e->st.rng.random_range(-200.0f, 200.0f);
     }
     const uint64_t ttl = sy.params[1];
     k_sys_particles_spawn<<<e->grid_for(rate, 256), 256, 0, e->stream>>>(
         e->image(0), e->words, e->cols[sy.cols[0]].first_plane, e->cols[sy.cols[1]].first_plane, e->cols[sy.cols[2]].first_plane,
-        e->st.n_rows, rate, e->d_spawn[0], uint32_t(ttl), uint32_t(ttl >> 32));
+        e->st.n_rows, rate, e->spawn[0].dev(), uint32_t(ttl), uint32_t(ttl >> 32));
     e->launches += 1;
     CUDA_TRY(cudaGetLastError());
     rc = clear_stamps(e, 0);
@@ -2542,33 +2429,22 @@ BGR_API int bgr_peek_first(bgr_engine* e, int32_t frame, uint32_t column, uint32
 // the column table and counters of k_desync_*, allocated by the first diff; records grow with records_cap
 static int ensure_diff_scratch(bgr_engine* e, uint32_t records_cap) {
     const uint32_t n_cols = uint32_t(e->cols.size());
-    if (!e->d_diff_cols) {
+    if (!e->diff_cols.get()) {
         std::vector<DiffColumn> dc(n_cols);
         for (uint32_t c = 0; c < n_cols; ++c) {
             const Column& k = e->cols[c];
             const bool ck = k.hash_kind != BGR_HASH_NONE && k.hash_len > 0;
             dc[c] = DiffColumn{k.first_plane, k.words, k.absent, ck ? k.hash_off : 0u, ck ? k.hash_off + k.hash_len : 0u};
         }
-        CUDA_TRY(cudaMalloc(&e->d_diff_cols, sizeof(DiffColumn) * std::max(1u, n_cols)));
+        CUDA_TRY(e->diff_cols.ensure(std::max(1u, n_cols)));
         // on the engine's (non-blocking) stream: ordered before the pass-1 launch that reads the table
-        CUDA_TRY(cudaMemcpyAsync(e->d_diff_cols, dc.data(), sizeof(DiffColumn) * n_cols, cudaMemcpyHostToDevice, e->stream));
+        CUDA_TRY(cudaMemcpyAsync(e->diff_cols.get(), dc.data(), sizeof(DiffColumn) * n_cols, cudaMemcpyHostToDevice, e->stream));
         CUDA_TRY(cudaStreamSynchronize(e->stream));  // `dc` is a pageable host vector that goes out of scope below
-        CUDA_TRY(cudaMalloc(&e->d_diff_totals, sizeof(unsigned long long) * 3u));
+        CUDA_TRY(e->diff_totals.ensure(3));
     }
-    if (e->diff_tiles < e->n_tiles_cap) {  // first use, or the capacity grew since (grow_to)
-        if (e->d_diff_counts) CUDA_TRY(cudaFree(e->d_diff_counts));
-        if (e->d_diff_list) CUDA_TRY(cudaFree(e->d_diff_list));
-        e->d_diff_counts = nullptr; e->d_diff_list = nullptr; e->diff_tiles = 0;
-        CUDA_TRY(cudaMalloc(&e->d_diff_counts, sizeof(unsigned int) * (3u * n_cols + e->n_tiles_cap)));
-        CUDA_TRY(cudaMalloc(&e->d_diff_list, sizeof(unsigned int) * 2u * e->n_tiles_cap));
-        e->diff_tiles = e->n_tiles_cap;
-    }
-    if (records_cap > e->diff_records_cap) {
-        if (e->d_diff_records) CUDA_TRY(cudaFree(e->d_diff_records));
-        e->d_diff_records = nullptr; e->diff_records_cap = 0;
-        CUDA_TRY(cudaMalloc(&e->d_diff_records, sizeof(DiffRecord) * records_cap));
-        e->diff_records_cap = records_cap;
-    }
+    CUDA_TRY(e->diff_counts.ensure(3u * n_cols + e->n_tiles_cap));
+    CUDA_TRY(e->diff_list.ensure(2u * e->n_tiles_cap));
+    CUDA_TRY(e->diff_records.ensure(records_cap));
     return BGR_OK;
 }
 
@@ -2581,22 +2457,22 @@ static int run_diff(bgr_engine* e, DiffParams p, uint32_t n_pos, int32_t frame, 
     if (rc != BGR_OK) return rc;
     p.words = e->words;
     p.n_cols = n_cols;
-    p.cols = e->d_diff_cols;
-    p.col_counts = e->d_diff_counts;
-    p.totals = e->d_diff_totals;
-    p.tile_records = e->d_diff_counts + 3u * n_cols;
+    p.cols = e->diff_cols.get();
+    p.col_counts = e->diff_counts.get();
+    p.totals = e->diff_totals.get();
+    p.tile_records = e->diff_counts.get() + 3u * n_cols;
     p.cap = records_cap;
-    p.out = e->d_diff_records;
+    p.out = e->diff_records.get();
     std::vector<unsigned int> counts(3u * n_cols + n_pos, 0u);
     unsigned long long totals[3] = {0, 0, 0};
     if (n_pos) {
-        CUDA_TRY(cudaMemsetAsync(e->d_diff_counts, 0, sizeof(unsigned int) * 3u * n_cols, e->stream));
-        CUDA_TRY(cudaMemsetAsync(e->d_diff_totals, 0, sizeof(unsigned long long) * 3u, e->stream));
+        CUDA_TRY(cudaMemsetAsync(e->diff_counts.get(), 0, sizeof(unsigned int) * 3u * n_cols, e->stream));
+        CUDA_TRY(cudaMemsetAsync(e->diff_totals.get(), 0, sizeof(unsigned long long) * 3u, e->stream));
         k_desync_count<<<n_pos, kDiffBlock, 0, e->stream>>>(p);
         e->launches += 1;
         CUDA_TRY(cudaGetLastError());
-        CUDA_TRY(cudaMemcpyAsync(counts.data(), e->d_diff_counts, sizeof(unsigned int) * counts.size(), cudaMemcpyDeviceToHost, e->stream));
-        CUDA_TRY(cudaMemcpyAsync(totals, e->d_diff_totals, sizeof totals, cudaMemcpyDeviceToHost, e->stream));
+        CUDA_TRY(cudaMemcpyAsync(counts.data(), e->diff_counts.get(), sizeof(unsigned int) * counts.size(), cudaMemcpyDeviceToHost, e->stream));
+        CUDA_TRY(cudaMemcpyAsync(totals, e->diff_totals.get(), sizeof totals, cudaMemcpyDeviceToHost, e->stream));
         CUDA_TRY(cudaStreamSynchronize(e->stream));
     }
     // exclusive scan of the per-position record counts: the positions that hold one of the first records_cap records
@@ -2612,13 +2488,13 @@ static int run_diff(bgr_engine* e, DiffParams p, uint32_t n_pos, int32_t frame, 
     if (n_list) {
         std::vector<unsigned int> packed(2u * n_list);  // [positions..., bases...]
         for (uint32_t i = 0; i < n_list; ++i) { packed[i] = list[2 * i]; packed[n_list + i] = list[2 * i + 1]; }
-        CUDA_TRY(cudaMemcpyAsync(e->d_diff_list, packed.data(), sizeof(unsigned int) * packed.size(), cudaMemcpyHostToDevice, e->stream));
-        p.tile_list = e->d_diff_list;
+        CUDA_TRY(cudaMemcpyAsync(e->diff_list.get(), packed.data(), sizeof(unsigned int) * packed.size(), cudaMemcpyHostToDevice, e->stream));
+        p.tile_list = e->diff_list.get();
         p.n_list = n_list;
         k_desync_records<<<n_list, kDiffBlock, 0, e->stream>>>(p);
         e->launches += 1;
         CUDA_TRY(cudaGetLastError());
-        CUDA_TRY(cudaMemcpyAsync(records, e->d_diff_records, sizeof(DiffRecord) * n_out, cudaMemcpyDeviceToHost, e->stream));
+        CUDA_TRY(cudaMemcpyAsync(records, e->diff_records.get(), sizeof(DiffRecord) * n_out, cudaMemcpyDeviceToHost, e->stream));
         CUDA_TRY(cudaStreamSynchronize(e->stream));
     }
     if (n_records) *n_records = n_out;
@@ -2721,21 +2597,15 @@ BGR_API int bgr_frame_digest(bgr_engine* e, int32_t frame, bgr_frame_digest_head
     const size_t smem = sizeof(unsigned long long) * (kTileRows / 32u) * per;
     if (smem + sizeof(uint32_t) * (kTileRows / 32u) > 48u * 1024u)
         return fail(BGR_ERR_UNSUPPORTED, "bgr_frame_digest supports at most 382 registered columns");
-    if (!e->d_digest_cols) {
+    if (!e->digest_cols.get()) {
         std::vector<DigestColumn> dc(n_cols);
         for (uint32_t c = 0; c < n_cols; ++c) dc[c] = DigestColumn{e->cols[c].first_plane, e->cols[c].elem_bytes, e->cols[c].absent};
-        CUDA_TRY(cudaMalloc(&e->d_digest_cols, sizeof(DigestColumn) * std::max(1u, n_cols)));
-        CUDA_TRY(cudaMemcpyAsync(e->d_digest_cols, dc.data(), sizeof(DigestColumn) * n_cols, cudaMemcpyHostToDevice, e->stream));
+        CUDA_TRY(e->digest_cols.ensure(std::max(1u, n_cols)));
+        CUDA_TRY(cudaMemcpyAsync(e->digest_cols.get(), dc.data(), sizeof(DigestColumn) * n_cols, cudaMemcpyHostToDevice, e->stream));
         CUDA_TRY(cudaStreamSynchronize(e->stream));  // `dc` goes out of scope below
     }
-    if (e->digest_tiles < e->n_tiles_cap) {  // first use, or the capacity grew since (grow_to)
-        if (e->d_digest_words) CUDA_TRY(cudaFree(e->d_digest_words));
-        if (e->d_digest_active) CUDA_TRY(cudaFree(e->d_digest_active));
-        e->d_digest_words = nullptr; e->d_digest_active = nullptr; e->digest_tiles = 0;
-        CUDA_TRY(cudaMalloc(&e->d_digest_words, sizeof(unsigned long long) * per * e->n_tiles_cap));
-        CUDA_TRY(cudaMalloc(&e->d_digest_active, sizeof(unsigned int) * e->n_tiles_cap));
-        e->digest_tiles = e->n_tiles_cap;
-    }
+    CUDA_TRY(e->digest_words.ensure(size_t(per) * e->n_tiles_cap));
+    CUDA_TRY(e->digest_active.ensure(e->n_tiles_cap));
     const uint32_t rows = e->st.slot_rows[slot], n_blocks = e->tiles_for(rows);
     std::vector<uint64_t> w(size_t(n_blocks) * per);
     std::vector<unsigned int> active(n_blocks);
@@ -2746,14 +2616,14 @@ BGR_API int bgr_frame_digest(bgr_engine* e, int32_t frame, bgr_frame_digest_head
         p.n_cols = n_cols;
         p.n_rows = rows;
         p.order_base = e->cfg.order_base;
-        p.cols = e->d_digest_cols;
-        p.out = e->d_digest_words;
-        p.active = e->d_digest_active;
+        p.cols = e->digest_cols.get();
+        p.out = e->digest_words.get();
+        p.active = e->digest_active.get();
         k_frame_digest<<<n_blocks, kTileRows, smem, e->stream>>>(p);
         e->launches += 1;
         CUDA_TRY(cudaGetLastError());
-        CUDA_TRY(cudaMemcpyAsync(w.data(), e->d_digest_words, sizeof(uint64_t) * w.size(), cudaMemcpyDeviceToHost, e->stream));
-        CUDA_TRY(cudaMemcpyAsync(active.data(), e->d_digest_active, sizeof(unsigned int) * n_blocks, cudaMemcpyDeviceToHost, e->stream));
+        CUDA_TRY(cudaMemcpyAsync(w.data(), e->digest_words.get(), sizeof(uint64_t) * w.size(), cudaMemcpyDeviceToHost, e->stream));
+        CUDA_TRY(cudaMemcpyAsync(active.data(), e->digest_active.get(), sizeof(unsigned int) * n_blocks, cudaMemcpyDeviceToHost, e->stream));
         CUDA_TRY(cudaStreamSynchronize(e->stream));
     }
     std::memset(header, 0, sizeof *header);
@@ -2899,27 +2769,17 @@ BGR_API int bgr_desync_diff_remote(bgr_engine* e, int32_t frame, const void* blo
     // before loading, and words are only loaded for rows that exist on both sides).  Ascending, at most n_tiles_cap.
     for (uint32_t b = h.n_blocks; b < e->tiles_for(e->st.slot_rows[slot]); ++b) visit.push_back(b);
     const uint32_t n_visit = uint32_t(visit.size());
-    if (e->visit_tiles < e->n_tiles_cap) {  // first use, or the capacity grew since (grow_to)
-        if (e->d_remote_visit) CUDA_TRY(cudaFree(e->d_remote_visit));
-        e->d_remote_visit = nullptr; e->visit_tiles = 0;
-        CUDA_TRY(cudaMalloc(&e->d_remote_visit, sizeof(unsigned int) * e->n_tiles_cap));
-        e->visit_tiles = e->n_tiles_cap;
-    }
-    if (h.n_exported > e->remote_cap_tiles) {  // staging for the peer's tiles, grown on demand
-        if (e->d_remote) CUDA_TRY(cudaFree(e->d_remote));
-        e->d_remote = nullptr; e->remote_cap_tiles = 0;
-        CUDA_TRY(cudaMalloc(&e->d_remote, tb * h.n_exported));
-        e->remote_cap_tiles = h.n_exported;
-    }
+    CUDA_TRY(e->remote_visit.ensure(e->n_tiles_cap));
+    CUDA_TRY(e->remote.ensure(tb * h.n_exported));  // staging for the peer's tiles
     for (uint32_t i = 0; i < h.n_exported; ++i)
-        CUDA_TRY(cudaMemcpyAsync(e->d_remote + size_t(i) * tb, in + sizeof h + size_t(i) * rec + kBlobBlockHeader, tb,
+        CUDA_TRY(cudaMemcpyAsync(e->remote.get() + size_t(i) * tb, in + sizeof h + size_t(i) * rec + kBlobBlockHeader, tb,
                                  cudaMemcpyHostToDevice, e->stream));
     if (n_visit)
-        CUDA_TRY(cudaMemcpyAsync(e->d_remote_visit, visit.data(), sizeof(unsigned int) * n_visit, cudaMemcpyHostToDevice, e->stream));
+        CUDA_TRY(cudaMemcpyAsync(e->remote_visit.get(), visit.data(), sizeof(unsigned int) * n_visit, cudaMemcpyHostToDevice, e->stream));
     DiffParams p{};
     p.first = e->image(slot + 1);
-    p.latest = e->d_remote;  // null while nothing was ever exported to this engine: then no position reads it
-    p.visit = e->d_remote_visit;
+    p.latest = e->remote.get();  // null while nothing was ever exported to this engine: then no position reads it
+    p.visit = e->remote_visit.get();
     p.rows_first = e->st.slot_rows[slot];
     p.rows_latest = h.rows;
     rc = run_diff(e, p, n_visit, frame, summary, cols, cols_cap, records, records_cap, n_records);
@@ -3103,12 +2963,11 @@ BGR_API int bgr_shard_group_join(bgr_engine* e, const char* name, uint32_t rank,
     cudaError_t ce = cudaHostRegister(g->blocks_base(), g->blocks_bytes(), cudaHostRegisterMapped | cudaHostRegisterPortable);
     if (ce != cudaSuccess) { delete g; return fail(BGR_ERR_CUDA, std::string("cudaHostRegister(shard group segment): ") + cudaGetErrorString(ce)); }
     for (int b = 0; b < bgr_engine::kBufs; ++b) {
-        e->own_h_out[b] = e->h_out[b]; e->own_d_out[b] = e->d_out[b];
         e->h_out[b] = reinterpret_cast<unsigned long long*>(g->block(rank, uint32_t(b)));
         void* dp = nullptr;
         ce = cudaHostGetDevicePointer(&dp, e->h_out[b], 0);
         if (ce != cudaSuccess) {
-            for (int k = 0; k <= b; ++k) { e->h_out[k] = e->own_h_out[k]; e->d_out[k] = e->own_d_out[k]; }
+            use_own_blocks(e);
             cudaHostUnregister(g->blocks_base());
             delete g;
             return fail(BGR_ERR_CUDA, std::string("cudaHostGetDevicePointer: ") + cudaGetErrorString(ce));
@@ -3127,10 +2986,7 @@ BGR_API int bgr_shard_group_leave(bgr_engine* e) {
     if (!e->pending.empty()) return fail(BGR_ERR_STATE, "collect every submitted request vector before leaving the shard group");
     cudaSetDevice(e->cfg.device);
     cudaStreamSynchronize(e->stream);
-    cudaHostUnregister(e->group->blocks_base());
-    for (int b = 0; b < bgr_engine::kBufs; ++b) { e->h_out[b] = e->own_h_out[b]; e->d_out[b] = e->own_d_out[b]; }
-    delete e->group;
-    e->group = nullptr;
+    leave_group(e);
     return BGR_OK;
 }
 
@@ -3203,24 +3059,25 @@ BGR_API int bgr_trace_enable(bgr_engine* e, uint32_t capacity) {
     if (!e || !e->built) return fail(BGR_ERR_STATE, "engine not built");
     int rc = drain(e);
     if (rc != BGR_OK) return rc;
-    if (e->d_trace) { CUDA_TRY(cudaFree(e->d_trace)); e->d_trace = nullptr; e->trace_cap = 0; }
+    e->trace = {};  // a new trace starts empty, at exactly its capacity
+    e->trace_cap = 0;
     if (capacity == 0) return BGR_OK;
     std::vector<unsigned long long> init(size_t(capacity) * 4, 0ULL);
     for (uint32_t i = 0; i < capacity; ++i) init[4 * i] = ~0ULL;
-    CUDA_TRY(cudaMalloc(&e->d_trace, init.size() * sizeof(unsigned long long)));
-    CUDA_TRY(cudaMemcpy(e->d_trace, init.data(), init.size() * sizeof(unsigned long long), cudaMemcpyHostToDevice));
+    CUDA_TRY(e->trace.ensure(init.size()));
+    CUDA_TRY(cudaMemcpy(e->trace.get(), init.data(), init.size() * sizeof(unsigned long long), cudaMemcpyHostToDevice));
     e->trace_cap = capacity;
     e->trace_first_seq = e->seq + 1;
     return BGR_OK;
 }
 BGR_API int bgr_trace_read(bgr_engine* e, uint64_t* start_end_ns_out, uint32_t cap, uint32_t* n_out) {
-    if (!e || !e->d_trace) return fail(BGR_ERR_STATE, "trace not enabled");
+    if (!e || !e->trace.get()) return fail(BGR_ERR_STATE, "trace not enabled");
     int rc = drain(e);
     if (rc != BGR_OK) return rc;
     CUDA_TRY(cudaStreamSynchronize(e->stream));
     const uint64_t done = e->seq + 1 > e->trace_first_seq ? e->seq + 1 - e->trace_first_seq : 0;
     const uint32_t n = uint32_t(std::min<uint64_t>(std::min<uint64_t>(done, e->trace_cap), cap));
-    if (n && start_end_ns_out) CUDA_TRY(cudaMemcpy(start_end_ns_out, e->d_trace, size_t(n) * 4 * sizeof(uint64_t), cudaMemcpyDeviceToHost));
+    if (n && start_end_ns_out) CUDA_TRY(cudaMemcpy(start_end_ns_out, e->trace.get(), size_t(n) * 4 * sizeof(uint64_t), cudaMemcpyDeviceToHost));
     if (n_out) *n_out = n;
     return BGR_OK;
 }

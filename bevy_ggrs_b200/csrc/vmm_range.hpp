@@ -1,9 +1,10 @@
-// Growable strided device ranges on the CUDA virtual memory management API (engines created with BGR_CFG_GROWABLE).
+// Strided device ranges: every buffer of an engine whose size follows its row capacity.
 //
-// One virtual range of `n` strides is reserved once; memory is mapped under a prefix of every stride, and growing maps
-// more under each stride behind what is there.  No byte moves and no address changes, so pointers handed to queued
-// launches stay valid while the range grows.  The driver entry points come through cudaGetDriverEntryPoint: the
-// library keeps static cudart as its only link-time dependency.
+// Engines created with BGR_CFG_GROWABLE reserve one virtual range of `n` strides once (the CUDA virtual memory
+// management API); memory is mapped under a prefix of every stride, and growing maps more under each stride behind what
+// is there.  No byte moves and no address changes, so pointers handed to queued launches stay valid while the range
+// grows.  Other engines allocate the `n` strides with one cudaMalloc, all of it mapped.  The driver entry points come
+// through cudaGetDriverEntryPoint: the library keeps static cudart as its only link-time dependency.
 #pragma once
 #include <cuda.h>
 #include <cudaTypedefs.h>
@@ -13,6 +14,7 @@
 #include <cstdint>
 #include <string>
 #include <type_traits>
+#include <utility>
 #include <vector>
 
 namespace bgr {
@@ -68,16 +70,36 @@ inline std::string vmm_error(const VmmApi* api, const char* what, CUresult r) {
 
 inline size_t round_up(size_t v, size_t to) { return (v + to - 1) / to * to; }
 
-// `n` strides of `stride` bytes at `base`; [0, mapped) of every stride is backed by memory.
+// `n` strides of `stride` bytes at `base`; [0, mapped) of every stride is backed by memory.  Owns that memory: it is
+// released when the range is destroyed, once the caller has synchronised every stream that used it.
 struct StridedRange {
     CUdeviceptr base = 0;
     size_t stride = 0, mapped = 0, zeroed = 0, gran = 0;
     uint32_t n = 0;
     int device = 0;
+    bool allocated = false;     // one cudaMalloc (allocate) rather than a reserved address range (reserve)
     std::vector<size_t> steps;  // mapped size after each growth step: every step is one mapping per stride
 
+    StridedRange() = default;
+    StridedRange(StridedRange&& o) noexcept { swap(o); }
+    StridedRange& operator=(StridedRange&& o) noexcept { StridedRange t(std::move(o)); swap(t); return *this; }
+    ~StridedRange() { free(); }
+
     template <class T = uint8_t> T* ptr() const { return reinterpret_cast<T*>(base); }
-    bool reserved() const { return base != 0; }
+    bool empty() const { return base == 0; }
+
+    // Allocates n contiguous strides of exactly `bytes` each, all mapped; map_to cannot grow them.
+    bool allocate(uint32_t n_strides, size_t bytes, std::string* err) {
+        void* p = nullptr;
+        const cudaError_t ce = cudaMalloc(&p, size_t(n_strides) * bytes);
+        if (ce != cudaSuccess) { *err = std::string("cudaMalloc: ") + cudaGetErrorString(ce); return false; }
+        base = reinterpret_cast<CUdeviceptr>(p);
+        n = n_strides;
+        stride = mapped = bytes;
+        gran = 1;
+        allocated = true;
+        return true;
+    }
 
     // Reserves n strides of at least `stride_min` bytes each (rounded up to the allocation granularity); maps nothing.
     bool reserve(int dev, uint32_t n_strides, size_t stride_min, std::string* err) {
@@ -141,11 +163,19 @@ struct StridedRange {
 
     // Zeroes what was mapped since the last call, on `stream` (ordered behind every launch that used the range).
     cudaError_t zero_new(cudaStream_t stream) {
-        for (uint32_t i = 0; i < n && zeroed < mapped; ++i) {
-            const cudaError_t ce = cudaMemsetAsync(reinterpret_cast<void*>(base + size_t(i) * stride + zeroed), 0, mapped - zeroed, stream);
+        const cudaError_t ce = zero(zeroed, mapped, stream);
+        if (ce == cudaSuccess) zeroed = mapped;
+        return ce;
+    }
+
+    // Zeroes [lo, hi) of every stride on `stream`: one memset when that is every stride whole.
+    cudaError_t zero(size_t lo, size_t hi, cudaStream_t stream) const {
+        if (lo >= hi) return cudaSuccess;
+        if (lo == 0 && hi == stride) return cudaMemsetAsync(ptr(), 0, stride * n, stream);
+        for (uint32_t i = 0; i < n; ++i) {
+            const cudaError_t ce = cudaMemsetAsync(ptr() + size_t(i) * stride + lo, 0, hi - lo, stream);
             if (ce != cudaSuccess) return ce;
         }
-        zeroed = mapped;
         return cudaSuccess;
     }
 
@@ -163,15 +193,27 @@ struct StridedRange {
         zeroed = std::min(zeroed, mapped);
     }
 
-    // Unmaps everything and frees the address range (the caller has synchronised every stream that used it).
+    // Releases the memory (the caller has synchronised every stream that used it); the range is empty afterwards.
     void free() {
-        if (!base) return;
-        shrink(0);
-        vmm_api(nullptr)->address_free(base, stride * n);
-        *this = StridedRange{};
+        if (allocated) cudaFree(ptr());
+        else if (base) {
+            shrink(0);
+            vmm_api(nullptr)->address_free(base, stride * n);
+        }
+        base = 0;
+        stride = mapped = zeroed = gran = 0;
+        n = 0;
+        allocated = false;
+        steps.clear();
     }
 
   private:
+    void swap(StridedRange& o) noexcept {
+        std::swap(base, o.base); std::swap(stride, o.stride); std::swap(mapped, o.mapped); std::swap(zeroed, o.zeroed);
+        std::swap(gran, o.gran); std::swap(n, o.n); std::swap(device, o.device); std::swap(allocated, o.allocated);
+        steps.swap(o.steps);
+    }
+
     static CUmemAllocationProp props(int dev) {
         CUmemAllocationProp prop{};
         prop.type = CU_MEM_ALLOCATION_TYPE_PINNED;
