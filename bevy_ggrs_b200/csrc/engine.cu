@@ -31,6 +31,7 @@
 #include "desync_diff.cuh"
 #include "change_feed.cuh"
 #include "frame_digest.cuh"
+#include "checkpoint.cuh"
 #include "jit.hpp"
 #include "vmm_range.hpp"
 #include "device_memory.hpp"
@@ -2584,14 +2585,10 @@ static uint64_t digest_layout(const bgr_engine* e) {
     return bgr_seahash(v.data(), v.size() * sizeof(uint32_t));
 }
 
-BGR_API int bgr_frame_digest(bgr_engine* e, int32_t frame, bgr_frame_digest_header* header, uint64_t* words, uint32_t words_cap,
-                             int32_t* found) {
-    if (!header || !found || (!words && words_cap)) return fail(BGR_ERR_INVALID_ARGUMENT, "null argument");
-    int rc = p2p_args(e);
-    if (rc != BGR_OK) return rc;
-    uint32_t slot = 0;
-    if (!p2p_slot(e, frame, &slot)) { *found = 0; return BGR_OK; }
-    *found = 1;
+// k_frame_digest over the first ceil(rows / 512) tiles of `img`: the block words ([n_blocks][n_columns + 1]), their root
+// and the alive rows
+static int digest_image(bgr_engine* e, const uint8_t* img, uint32_t rows, std::vector<uint64_t>* words, uint64_t* root,
+                        uint64_t* active_rows) {
     const uint32_t n_cols = uint32_t(e->cols.size()), per = n_cols + 1u;
     // dynamic shared memory: 16 warps x (n_cols + 1) words, next to the kernel's static s_warp[16] (48 KB in all)
     const size_t smem = sizeof(unsigned long long) * (kTileRows / 32u) * per;
@@ -2604,14 +2601,15 @@ BGR_API int bgr_frame_digest(bgr_engine* e, int32_t frame, bgr_frame_digest_head
         CUDA_TRY(cudaMemcpyAsync(e->digest_cols.get(), dc.data(), sizeof(DigestColumn) * n_cols, cudaMemcpyHostToDevice, e->stream));
         CUDA_TRY(cudaStreamSynchronize(e->stream));  // `dc` goes out of scope below
     }
-    CUDA_TRY(e->digest_words.ensure(size_t(per) * e->n_tiles_cap));
-    CUDA_TRY(e->digest_active.ensure(e->n_tiles_cap));
-    const uint32_t rows = e->st.slot_rows[slot], n_blocks = e->tiles_for(rows);
-    std::vector<uint64_t> w(size_t(n_blocks) * per);
+    const uint32_t n_blocks = e->tiles_for(rows);
+    CUDA_TRY(e->digest_words.ensure(size_t(per) * std::max(e->n_tiles_cap, n_blocks)));
+    CUDA_TRY(e->digest_active.ensure(std::max(e->n_tiles_cap, n_blocks)));
+    std::vector<uint64_t>& w = *words;
+    w.assign(size_t(n_blocks) * per, 0);
     std::vector<unsigned int> active(n_blocks);
     if (n_blocks) {
         DigestParams p{};
-        p.img = e->image(slot + 1);
+        p.img = img;
         p.words = e->words;
         p.n_cols = n_cols;
         p.n_rows = rows;
@@ -2626,17 +2624,36 @@ BGR_API int bgr_frame_digest(bgr_engine* e, int32_t frame, bgr_frame_digest_head
         CUDA_TRY(cudaMemcpyAsync(active.data(), e->digest_active.get(), sizeof(unsigned int) * n_blocks, cudaMemcpyDeviceToHost, e->stream));
         CUDA_TRY(cudaStreamSynchronize(e->stream));
     }
+    *active_rows = 0;
+    for (unsigned int a : active) *active_rows += a;
+    *root = bgr_seahash(w.data(), w.size() * sizeof(uint64_t));
+    return BGR_OK;
+}
+
+BGR_API int bgr_frame_digest(bgr_engine* e, int32_t frame, bgr_frame_digest_header* header, uint64_t* words, uint32_t words_cap,
+                             int32_t* found) {
+    if (!header || !found || (!words && words_cap)) return fail(BGR_ERR_INVALID_ARGUMENT, "null argument");
+    int rc = p2p_args(e);
+    if (rc != BGR_OK) return rc;
+    uint32_t slot = 0;
+    if (!p2p_slot(e, frame, &slot)) { *found = 0; return BGR_OK; }
+    *found = 1;
+    const uint32_t rows = e->st.slot_rows[slot];
+    std::vector<uint64_t> w;
+    uint64_t root = 0, active = 0;
+    rc = digest_image(e, e->image(slot + 1), rows, &w, &root, &active);
+    if (rc != BGR_OK) return rc;
     std::memset(header, 0, sizeof *header);
     header->layout = digest_layout(e);
     header->frame = frame;
     header->rows = rows;
-    header->n_blocks = n_blocks;
-    header->n_columns = n_cols;
-    for (unsigned int a : active) header->active += a;
+    header->n_blocks = e->tiles_for(rows);
+    header->n_columns = uint32_t(e->cols.size());
+    header->active = active;
     header->elapsed_ns = e->st.slot_elapsed_ns[slot];
     static_assert(sizeof(ParticleRng) == sizeof(header->rng), "ParticleRng is four u64 words");
     std::memcpy(header->rng, &e->st.slot_rng[slot], sizeof header->rng);
-    header->root = bgr_seahash(w.data(), w.size() * sizeof(uint64_t));
+    header->root = root;
     if (words) std::memcpy(words, w.data(), sizeof(uint64_t) * std::min<size_t>(words_cap, w.size()));
     return BGR_OK;
 }
@@ -2788,6 +2805,219 @@ BGR_API int bgr_desync_diff_remote(bgr_engine* e, int32_t frame, const void* blo
                                   (e->st.slot_elapsed_ns[slot] != h.elapsed_ns ? 2u : 0u);
     summary->elapsed_ns_first = e->st.slot_elapsed_ns[slot];
     summary->elapsed_ns_latest = h.elapsed_ns;
+    return BGR_OK;
+}
+
+// ---- world checkpoints (checkpoint.cuh encodes and decodes, k_frame_digest verifies a decoded world) ----
+static int checkpoint_args(bgr_engine* e) {
+    if (!e || !e->built) return fail(BGR_ERR_STATE, "engine not built");
+    if (e->cfg.flags & BGR_CFG_SHARDED) return fail(BGR_ERR_UNSUPPORTED, "world checkpoints are not supported on a sharded engine");
+    return BGR_OK;
+}
+
+// the absent bit of the column each word plane belongs to (0: not optional)
+static std::vector<uint32_t> plane_absent(const bgr_engine* e) {
+    std::vector<uint32_t> a(std::max(1u, e->words), 0u);
+    for (const Column& c : e->cols)
+        for (uint32_t w = 0; w < c.words; ++w) a[c.first_plane + w] = c.absent;
+    return a;
+}
+
+// bytes ahead of the payload: the header and the offsets
+static size_t checkpoint_prefix(uint32_t n_blocks) {
+    return sizeof(bgr_checkpoint_header) + sizeof(uint64_t) * (size_t(n_blocks) + 1u);
+}
+
+BGR_API int bgr_checkpoint_save(bgr_engine* e, int32_t frame, void* dst, size_t dst_cap, size_t* bytes, int32_t* found) {
+    if (!bytes || !found) return fail(BGR_ERR_INVALID_ARGUMENT, "null argument");
+    int rc = checkpoint_args(e);
+    if (rc == BGR_OK) rc = drain(e);
+    if (rc != BGR_OK) return rc;
+    uint32_t slot = 0;
+    if (!p2p_slot(e, frame, &slot)) { *found = 0; return BGR_OK; }
+    *found = 1;
+    const uint32_t rows = e->st.slot_rows[slot], n_blocks = e->tiles_for(rows);
+    if (!dst) {
+        *bytes = checkpoint_prefix(n_blocks) + size_t(n_blocks) * ckpt_max_block_words(e->words) * 4u;
+        return BGR_OK;
+    }
+    bgr_checkpoint_header h{};
+    h.magic = BGR_CHECKPOINT_MAGIC;
+    h.version = BGR_CHECKPOINT_VERSION;
+    h.layout = digest_layout(e);
+    h.frame = frame;
+    h.rows = rows;
+    h.words = e->words;
+    h.n_blocks = n_blocks;
+    h.n_columns = uint32_t(e->cols.size());
+    h.fps = e->cfg.fps;
+    h.elapsed_ns = e->st.slot_elapsed_ns[slot];
+    std::memcpy(h.rng, &e->st.slot_rng[slot], sizeof h.rng);
+    std::vector<uint64_t> digest_words;
+    rc = digest_image(e, e->image(slot + 1), rows, &digest_words, &h.digest_root, &h.active);
+    if (rc != BGR_OK) return rc;
+    std::vector<uint64_t> offsets(size_t(n_blocks) + 1u, 0);
+    const std::vector<uint32_t> absent = plane_absent(e);
+    DeviceBuffer<uint32_t> d_absent, d_payload;
+    DeviceBuffer<uint8_t> d_kinds;
+    DeviceBuffer<unsigned int> d_lens;
+    DeviceBuffer<unsigned long long> d_offsets;
+    CkptParams p{};
+    if (n_blocks) {
+        CUDA_TRY(d_absent.ensure(absent.size()));
+        CUDA_TRY(d_kinds.ensure(size_t(n_blocks) * (e->words + 1u)));
+        CUDA_TRY(d_lens.ensure(n_blocks));
+        CUDA_TRY(d_offsets.ensure(size_t(n_blocks) + 1u));
+        CUDA_TRY(cudaMemcpyAsync(d_absent.get(), absent.data(), sizeof(uint32_t) * absent.size(), cudaMemcpyHostToDevice, e->stream));
+        p.img = e->image(slot + 1);
+        p.words = e->words;
+        p.rows = rows;
+        p.plane_absent = d_absent.get();
+        p.kinds = d_kinds.get();
+        p.lens = d_lens.get();
+        p.offsets = d_offsets.get();
+        k_ckpt_measure<<<n_blocks, kTileRows, 0, e->stream>>>(p);
+        k_ckpt_scan<<<1, kCkptScanBlock, 0, e->stream>>>(d_lens.get(), n_blocks, d_offsets.get());
+        e->launches += 2;
+        CUDA_TRY(cudaGetLastError());
+        CUDA_TRY(cudaMemcpyAsync(offsets.data(), d_offsets.get(), sizeof(uint64_t) * offsets.size(), cudaMemcpyDeviceToHost, e->stream));
+        CUDA_TRY(cudaStreamSynchronize(e->stream));
+    }
+    h.payload_bytes = offsets[n_blocks];
+    const size_t prefix = checkpoint_prefix(n_blocks), need = prefix + h.payload_bytes;
+    *bytes = need;
+    if (dst_cap < need) return fail(BGR_ERR_CAPACITY, "the checkpoint needs " + std::to_string(need) + " bytes");
+    uint8_t* out = static_cast<uint8_t*>(dst);
+    if (n_blocks) {
+        CUDA_TRY(d_payload.ensure(h.payload_bytes / 4u));
+        p.payload = d_payload.get();
+        k_ckpt_pack<<<n_blocks, kTileRows, 0, e->stream>>>(p);
+        e->launches += 1;
+        CUDA_TRY(cudaGetLastError());
+        CUDA_TRY(cudaMemcpyAsync(out + prefix, d_payload.get(), h.payload_bytes, cudaMemcpyDeviceToHost, e->stream));
+        CUDA_TRY(cudaStreamSynchronize(e->stream));
+    }
+    std::memcpy(out, &h, sizeof h);
+    std::memcpy(out + sizeof h, offsets.data(), sizeof(uint64_t) * offsets.size());
+    return BGR_OK;
+}
+
+BGR_API int bgr_checkpoint_restore(bgr_engine* e, const void* blob, size_t bytes) {
+    int rc = checkpoint_args(e);
+    if (rc != BGR_OK) return rc;
+    if (!blob) return fail(BGR_ERR_INVALID_ARGUMENT, "null argument");
+    if (!e->pending.empty()) return fail(BGR_ERR_STATE, "collect every submitted request vector first");
+    if (e->st.ring.depth() == 0 || e->n_slots() == 0)
+        return fail(BGR_ERR_STATE, "the snapshot ring has depth 0: it cannot hold the restored frame");
+    // the blob is input from disk or another machine: check every field before using it
+    const uint8_t* in = static_cast<const uint8_t*>(blob);
+    bgr_checkpoint_header h;
+    if (bytes < sizeof h) return fail(BGR_ERR_INVALID_ARGUMENT, "checkpoint truncated: shorter than its header");
+    std::memcpy(&h, in, sizeof h);
+    if (h.magic != BGR_CHECKPOINT_MAGIC) return fail(BGR_ERR_INVALID_ARGUMENT, "not a world checkpoint (bad magic)");
+    if (h.version != BGR_CHECKPOINT_VERSION)
+        return fail(BGR_ERR_INVALID_ARGUMENT, "unsupported checkpoint format version " + std::to_string(h.version));
+    if (h.layout != digest_layout(e) || h.words != e->words || h.n_columns != e->cols.size())
+        return fail(BGR_ERR_INVALID_ARGUMENT, "the checkpoint comes from an engine with a different registration (layout differs)");
+    if (h.fps != e->cfg.fps)
+        return fail(BGR_ERR_INVALID_ARGUMENT, "the checkpoint was taken at " + std::to_string(h.fps) + " fps, this engine runs at " +
+                                                  std::to_string(e->cfg.fps));
+    if (h.n_blocks != e->tiles_for(h.rows))
+        return fail(BGR_ERR_INVALID_ARGUMENT, "checkpoint header: n_blocks does not match rows");
+    if (h.rows > e->ceiling)
+        return fail(BGR_ERR_CAPACITY, "the checkpoint holds " + std::to_string(h.rows) + " rows, more than this engine's " +
+                                          (e->growable() ? "ceiling of " : "capacity of ") + std::to_string(e->ceiling));
+    const uint32_t n_blocks = h.n_blocks;
+    const size_t prefix = checkpoint_prefix(n_blocks);
+    if (bytes < prefix) return fail(BGR_ERR_INVALID_ARGUMENT, "checkpoint truncated: shorter than its block offsets");
+    if (bytes - prefix != h.payload_bytes)
+        return fail(BGR_ERR_INVALID_ARGUMENT, "checkpoint length " + std::to_string(bytes) + " does not match its payload (truncated or overlong)");
+    std::vector<uint64_t> offsets(size_t(n_blocks) + 1u);
+    std::memcpy(offsets.data(), in + sizeof h, sizeof(uint64_t) * offsets.size());
+    // a block is at least its kind bytes and one u32 per vector (every vector CONST) and at most every vector RAW.  The
+    // lower bound also bounds the scratch image the decoding allocates by the blob's size: a tile of the image is at
+    // most tile_bytes / min_block times the smallest block (390x for the stress schema), and only a world that is
+    // constant in every tile gets there.
+    const uint64_t max_block = uint64_t(ckpt_max_block_words(e->words)) * 4u;
+    const uint64_t min_block = uint64_t(ckpt_kind_words(e->words) + e->words + 1u) * 4u;
+    if (offsets[0] != 0 || offsets[n_blocks] != h.payload_bytes)
+        return fail(BGR_ERR_INVALID_ARGUMENT, "checkpoint offsets do not span the payload");
+    for (uint32_t b = 0; b < n_blocks; ++b)
+        if (offsets[b + 1] < offsets[b] + min_block || offsets[b + 1] % 4u || offsets[b + 1] - offsets[b] > max_block)
+            return fail(BGR_ERR_INVALID_ARGUMENT, "checkpoint offset " + std::to_string(b + 1) + " is not ascending, aligned or within a block's size");
+    // decode into a scratch image and verify it with the frame digest before anything is committed
+    DeviceBuffer<uint8_t> scratch;
+    DeviceBuffer<uint32_t> d_payload, d_absent;
+    DeviceBuffer<unsigned long long> d_offsets;
+    DeviceBuffer<unsigned int> d_err;
+    const size_t tb = e->tile_bytes, image_bytes = size_t(n_blocks) * tb;
+    if (n_blocks) {
+        const size_t smem = sizeof(uint32_t) * (e->words + 1u);
+        if (smem + sizeof(uint32_t) * (kCkptMaskWords + 1u) > 48u * 1024u)
+            return fail(BGR_ERR_UNSUPPORTED, "bgr_checkpoint_restore supports at most 12000 word planes");
+        const std::vector<uint32_t> absent = plane_absent(e);
+        CUDA_TRY(scratch.ensure(image_bytes));
+        CUDA_TRY(d_payload.ensure(h.payload_bytes / 4u));
+        CUDA_TRY(d_absent.ensure(absent.size()));
+        CUDA_TRY(d_offsets.ensure(offsets.size()));
+        CUDA_TRY(d_err.ensure(1));
+        CUDA_TRY(cudaMemcpyAsync(d_payload.get(), in + prefix, h.payload_bytes, cudaMemcpyHostToDevice, e->stream));
+        CUDA_TRY(cudaMemcpyAsync(d_absent.get(), absent.data(), sizeof(uint32_t) * absent.size(), cudaMemcpyHostToDevice, e->stream));
+        CUDA_TRY(cudaMemcpyAsync(d_offsets.get(), offsets.data(), sizeof(uint64_t) * offsets.size(), cudaMemcpyHostToDevice, e->stream));
+        CUDA_TRY(cudaMemsetAsync(d_err.get(), 0xFF, sizeof(unsigned int), e->stream));
+        CkptParams p{};
+        p.img = scratch.get();
+        p.words = e->words;
+        p.rows = h.rows;
+        p.plane_absent = d_absent.get();
+        p.mask_bits = 1u;
+        for (const Column& c : e->cols) p.mask_bits |= c.absent;
+        p.offsets = d_offsets.get();
+        p.payload = d_payload.get();
+        p.err = d_err.get();
+        k_ckpt_unpack<<<n_blocks, kTileRows, smem, e->stream>>>(p);
+        e->launches += 1;
+        CUDA_TRY(cudaGetLastError());
+        unsigned int bad = 0;
+        CUDA_TRY(cudaMemcpyAsync(&bad, d_err.get(), sizeof bad, cudaMemcpyDeviceToHost, e->stream));
+        CUDA_TRY(cudaStreamSynchronize(e->stream));  // `absent` and `offsets` go out of scope or are reused below
+        if (bad != 0xFFFFFFFFu)
+            return fail(BGR_ERR_INVALID_ARGUMENT, "checkpoint block " + std::to_string(bad) +
+                                                      ": a bad kind byte or padding, its kinds and bitmaps imply another length than its "
+                                                      "offsets, or a row's mask byte has a bit this registration does not use");
+    }
+    std::vector<uint64_t> digest_words;
+    uint64_t root = 0, active = 0;
+    rc = digest_image(e, scratch.get(), h.rows, &digest_words, &root, &active);
+    if (rc != BGR_OK) return rc;
+    if (root != h.digest_root || active != h.active)
+        return fail(BGR_ERR_INVALID_ARGUMENT, "the decoded world's digest or active row count differs from the checkpoint header (corrupt payload)");
+    if (e->growable()) rc = grow_to(e, h.rows);
+    if (rc != BGR_OK) return rc;
+    // commit: image 0 and one slot hold the world, which the ring queues alone
+    e->deferred = DeferredLive{};  // image 0 is overwritten: nothing to materialise
+    HostState& s = e->st;
+    const uint32_t slot = s.ring.restart(h.frame);
+    if (n_blocks) {
+        CUDA_TRY(cudaMemcpyAsync(e->image(0), scratch.get(), image_bytes, cudaMemcpyDeviceToDevice, e->stream));
+        CUDA_TRY(cudaMemcpyAsync(e->image(slot + 1), scratch.get(), image_bytes, cudaMemcpyDeviceToDevice, e->stream));
+    }
+    rc = clear_stamps(e, 0);
+    if (rc == BGR_OK) rc = clear_stamps(e, slot + 1);
+    if (rc != BGR_OK) return rc;
+    e->tiledep_chain = false;
+    ParticleRng rng;
+    std::memcpy(&rng, h.rng, sizeof rng);
+    s.frame_count = h.frame;
+    s.elapsed_ns = h.elapsed_ns;
+    s.n_rows = h.rows;
+    s.rng = rng;
+    s.slot_rows[slot] = h.rows;
+    s.slot_elapsed_ns[slot] = h.elapsed_ns;
+    s.slot_rng[slot] = rng;
+    s.live_passive_ver = ++s.ver_counter;  // image 0 holds new content; the restored slot holds the same
+    s.slot_passive_ver[slot] = s.live_passive_ver;
+    CUDA_TRY(cudaStreamSynchronize(e->stream));  // before the scratch image is freed
     return BGR_OK;
 }
 

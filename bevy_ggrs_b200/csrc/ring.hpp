@@ -146,6 +146,17 @@ public:
         for (uint32_t i = retained_.size(); i-- > 0;) out->push_back(retained_[i].frame);
     }
 
+    // bgr_checkpoint_restore: forget every queued frame, witness and retained frame, then push `frame` alone.  Depth,
+    // capture and the retention setting stay.  Returns push()'s slot.
+    uint32_t restart(int32_t frame) {
+        entries_.n = 0;
+        witnesses_.n = 0;
+        retained_.n = 0;
+        free_.n = 0;
+        for (uint32_t s = n_slots_; s-- > 0;) free_.push_back(s);
+        return push(frame);
+    }
+
     // false => the reference would panic; `error` gets the same text
     bool rollback(int32_t frame, std::string* error) {
         for (;;) {

@@ -378,6 +378,22 @@ class Engine:
                              for i in range(len(self.elem_bytes))},
                             recs[: n.value].copy())
 
+    # ---- world checkpoints ----
+    def checkpoint(self, frame: int) -> Optional[bytes]:
+        """The checkpoint blob of a queued or retained frame (include/bevy_ggrs_b200.h "world checkpoints"); None if
+        neither holds it."""
+        size, found = C.c_size_t(), C.c_int32()
+        self._check(self._lib.bgr_checkpoint_save(self._h, frame, None, 0, C.byref(size), C.byref(found)))
+        if not found.value:
+            return None
+        out = np.empty(size.value, np.uint8)   # an upper bound: the call reports the exact size
+        self._check(self._lib.bgr_checkpoint_save(self._h, frame, out.ctypes.data, out.size, C.byref(size), C.byref(found)))
+        return out[: size.value].tobytes()
+
+    def restore(self, blob: bytes) -> None:
+        """Replace the world with a checkpoint's; the ring then holds the checkpoint's frame alone."""
+        self._check(self._lib.bgr_checkpoint_restore(self._h, blob, len(blob)))
+
     # ---- schedules ----
     def save_world(self) -> Tuple[int, int]:
         cs = capi.bgr_checksum()

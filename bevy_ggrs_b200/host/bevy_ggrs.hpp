@@ -144,7 +144,9 @@ public:
         static_assert(std::is_trivially_copyable<R>::value, "POD resources only");
         std::vector<uint8_t> b(sizeof(R));
         std::memcpy(b.data(), &initial, sizeof(R));
-        resources_[std::type_index(typeid(R))] = std::move(b);
+        const std::type_index t(typeid(R));
+        if (!resources_.count(t)) res_order_.push_back({t, uint32_t(sizeof(R))});
+        resources_[t] = std::move(b);
         return *this;
     }
     template <class R> App& rollback_resource_with_clone(const R& initial) { return rollback_resource_with_copy<R>(initial); }
@@ -422,7 +424,82 @@ public:
         return r;
     }
 
+    // ---- world checkpoints (bgr_checkpoint_save / bgr_checkpoint_restore; INTEGRATION.md "World checkpoints") ----
+    // The engine blob followed by the App's rollback resources of the frame: u32 count, then per resource in
+    // registration order u32 present, u32 len, the bytes, zero padding to a multiple of 4 (plugin.py writes the same).
+    // Refused while host-side component tables are registered (their values are not plain bytes) and, with resources
+    // registered, for a frame whose resource snapshot the App no longer holds (a retained frame).  Empty: the engine
+    // holds neither a queued nor a retained snapshot of the frame.
+    std::vector<uint8_t> checkpoint(ggrs::Frame frame) {
+        checkpoint_args();
+        auto rs = res_store_.find(frame);
+        if (!res_order_.empty() && rs == res_store_.end())
+            throw Panic(BGR_ERR_NO_SNAPSHOT, "the App holds no resource snapshot of frame " + std::to_string(frame));
+        size_t bytes = 0;
+        int32_t found = 0;
+        check(bgr_checkpoint_save(engine_, frame, nullptr, 0, &bytes, &found));
+        if (!found) return {};
+        std::vector<uint8_t> blob(bytes);  // an upper bound; the call reports the exact size
+        check(bgr_checkpoint_save(engine_, frame, blob.data(), blob.size(), &bytes, &found));
+        blob.resize(bytes);
+        auto put = [&blob](uint32_t v) { const uint8_t* p = reinterpret_cast<const uint8_t*>(&v); blob.insert(blob.end(), p, p + 4); };
+        put(uint32_t(res_order_.size()));
+        for (const auto& r : res_order_) {
+            auto it = rs->second.find(r.first);
+            const bool present = it != rs->second.end();
+            put(present ? 1u : 0u);
+            put(present ? uint32_t(it->second.size()) : 0u);
+            if (!present) continue;
+            blob.insert(blob.end(), it->second.begin(), it->second.end());
+            blob.resize(blob.size() + (4 - it->second.size() % 4) % 4, 0);
+        }
+        return blob;
+    }
+    // Replaces the world and the App's resources with a checkpoint's.  The resource section is checked before the
+    // engine restores, so a refused blob changes nothing.
+    void restore_checkpoint(const std::vector<uint8_t>& blob) {
+        checkpoint_args();
+        bgr_checkpoint_header h;
+        if (blob.size() < sizeof h) throw Panic(BGR_ERR_INVALID_ARGUMENT, "checkpoint truncated: shorter than its header");
+        std::memcpy(&h, blob.data(), sizeof h);
+        const uint64_t prefix = sizeof h + 8ull * (uint64_t(h.n_blocks) + 1);
+        if (h.payload_bytes > blob.size() || prefix + h.payload_bytes > blob.size())
+            throw Panic(BGR_ERR_INVALID_ARGUMENT, "checkpoint truncated: no resource section");
+        const size_t engine_bytes = size_t(prefix + h.payload_bytes);
+        size_t at = engine_bytes;
+        auto take = [&](size_t n) {
+            if (n > blob.size() - at) throw Panic(BGR_ERR_INVALID_ARGUMENT, "checkpoint truncated: its resource section is incomplete");
+            at += n;
+            return blob.data() + at - n;
+        };
+        auto get = [&]() { uint32_t v; std::memcpy(&v, take(4), 4); return v; };
+        if (get() != res_order_.size()) throw Panic(BGR_ERR_INVALID_ARGUMENT, "the checkpoint's resources are not the App's");
+        ResourceMap res;
+        for (const auto& r : res_order_) {
+            const uint32_t present = get(), n = get();
+            if (present > 1 || n != (present ? r.second : 0u))
+                throw Panic(BGR_ERR_INVALID_ARGUMENT, std::string("resource ") + r.first.name() + ": bad presence or length");
+            if (!present) continue;
+            const uint8_t* p = take(n);
+            res[r.first] = std::vector<uint8_t>(p, p + n);
+            const uint8_t* pad = take((4 - n % 4) % 4);
+            for (uint32_t i = 0; i < (4 - n % 4) % 4; ++i)
+                if (pad[i]) throw Panic(BGR_ERR_INVALID_ARGUMENT, std::string("resource ") + r.first.name() + ": non-zero padding");
+        }
+        if (at != blob.size()) throw Panic(BGR_ERR_INVALID_ARGUMENT, "checkpoint overlong: bytes follow its resource section");
+        check(bgr_checkpoint_restore(engine_, blob.data(), engine_bytes));
+        resources_ = res;
+        res_store_.clear();
+        if (!res_order_.empty()) res_store_[h.frame] = res;
+        res_frame_ = h.frame;
+    }
+
 private:
+    void checkpoint_args() {
+        finish();
+        if (!host_cols_.empty())
+            throw Panic(BGR_ERR_UNSUPPORTED, "an App with host-side component tables cannot be checkpointed: their values are not plain bytes");
+    }
     template <class T> App& register_component(uint32_t strategy) {
         static_assert(std::is_trivially_copyable<T>::value, "only POD components cross the C ABI");
         pending_cols_.push_back({std::type_index(typeid(T)), typeid(T).name(), uint32_t(sizeof(T)), strategy});
@@ -609,6 +686,7 @@ private:
     struct PendingCol { std::type_index type; std::string name; uint32_t bytes, strategy; };
     using ResourceMap = std::map<std::type_index, std::vector<uint8_t>>;
     ResourceMap resources_;
+    std::vector<std::pair<std::type_index, uint32_t>> res_order_;  // registered resources and their sizes, in order
     std::vector<std::type_index> res_checksummed_;
     std::vector<std::function<void(App&)>> res_systems_;
     std::map<ggrs::Frame, ResourceMap> res_store_;

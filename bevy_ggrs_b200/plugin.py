@@ -25,6 +25,7 @@ module is pure host logic: it never touches the GPU or the oracle itself.
 """
 from __future__ import annotations
 
+import struct
 from dataclasses import dataclass, field
 from typing import Callable, Dict, List, Optional, Sequence
 
@@ -267,6 +268,68 @@ class App:
         plus the local blocks past the peer's block count, whose rows only this side has."""
         self._finish()
         return self.world.diff_remote(frame, blob, max_records)
+
+    # ---- world checkpoints ----
+    # The engine blob (include/bevy_ggrs_b200.h "world checkpoints") followed by the App's rollback resources of the
+    # frame: u32 count, then per registered resource in registration order u32 present, u32 len, the bytes, zero
+    # padding to a multiple of 4 (INTEGRATION.md "World checkpoints"; bevy_ggrs.hpp writes the same section).
+    def _checkpoint_args(self) -> None:
+        self._finish()
+        if self.host_components.columns:
+            raise capi.BgrError(capi.BGR_ERR_UNSUPPORTED, "an App with host-side component tables cannot be checkpointed: "
+                                                          "their values are not plain bytes")
+
+    def checkpoint(self, frame: int) -> Optional[bytes]:
+        """The checkpoint of a queued or retained frame with the App's resources of that frame; None if the engine
+        holds neither.  Refused when the App no longer holds the frame's resource snapshot."""
+        self._checkpoint_args()
+        if self._res_registered and frame not in self._res_store:
+            raise capi.BgrError(capi.BGR_ERR_NO_SNAPSHOT, f"the App holds no resource snapshot of frame {frame}")
+        blob = self.world.checkpoint(frame)
+        if blob is None:
+            return None
+        snap = self._res_store.get(frame, {})
+        out = [blob, struct.pack("<I", len(self._res_registered))]
+        for name in self._res_registered:
+            v = snap.get(name)
+            out.append(struct.pack("<II", 0 if v is None else 1, 0 if v is None else len(v)))
+            if v is not None:
+                out.append(bytes(v) + bytes(-len(v) % 4))
+        return b"".join(out)
+
+    def restore_checkpoint(self, blob: bytes) -> None:
+        """Replaces the world and the App's resources with a checkpoint's.  The resource section is checked before the
+        engine restores, so a refused blob changes nothing."""
+        self._checkpoint_args()
+        if len(blob) < capi.C.sizeof(capi.bgr_checkpoint_header):
+            raise capi.BgrError(capi.BGR_ERR_INVALID_ARGUMENT, "checkpoint truncated: shorter than its header")
+        h = capi.bgr_checkpoint_header.from_buffer_copy(blob)
+        at = capi.C.sizeof(h) + 8 * (h.n_blocks + 1) + h.payload_bytes
+        res: Dict[str, Optional[bytes]] = {}
+
+        def take(n: int) -> bytes:
+            nonlocal at
+            if at + n > len(blob):
+                raise capi.BgrError(capi.BGR_ERR_INVALID_ARGUMENT, "checkpoint truncated: its resource section is incomplete")
+            at += n
+            return blob[at - n:at]
+        (count,) = struct.unpack("<I", take(4))
+        if count != len(self._res_registered):
+            raise capi.BgrError(capi.BGR_ERR_INVALID_ARGUMENT, f"the checkpoint holds {count} resources, the App registers "
+                                                               f"{len(self._res_registered)}")
+        for name in self._res_registered:
+            present, n = struct.unpack("<II", take(8))
+            if present > 1 or (not present and n):
+                raise capi.BgrError(capi.BGR_ERR_INVALID_ARGUMENT, f"resource {name}: bad presence or length")
+            res[name] = take(n) if present else None
+            if any(take(-n % 4)):
+                raise capi.BgrError(capi.BGR_ERR_INVALID_ARGUMENT, f"resource {name}: non-zero padding")
+        if at != len(blob):
+            raise capi.BgrError(capi.BGR_ERR_INVALID_ARGUMENT, "checkpoint overlong: bytes follow its resource section")
+        self.world.restore(blob[: capi.C.sizeof(h) + 8 * (h.n_blocks + 1) + h.payload_bytes])
+        self.resources = {n: bytearray(v) for n, v in res.items() if v is not None}
+        self._res_store = {h.frame: res} if self._res_registered else {}
+        self._res_frame = h.frame
 
     # ---- frame resources ----
     def rollback_frame_count(self) -> int:

@@ -495,6 +495,71 @@ BGR_API int bgr_desync_diff_remote(bgr_engine* e, int32_t frame, const void* blo
                                    bgr_desync_summary* summary, bgr_desync_column* cols, uint32_t cols_cap,
                                    bgr_desync_record* records, uint32_t records_cap, uint32_t* n_records, int32_t* found);
 
+/* ---- world checkpoints (any built engine without BGR_CFG_SHARDED) -----------------------------------------------
+ * A checkpoint is everything a match consists of at one saved frame: the image of every registered column, the row
+ * count, each optional column's presence, RollbackFrameCount, Time<GgrsTime> and ParticleRng.  Restoring it into an
+ * engine of the same registration layout (bgr_frame_digest_header.layout) and fps continues the match bit for bit, on
+ * any kernel and capacity.  The registered SYSTEMS are not part of the layout (as for digests): a world restored into
+ * an engine with other systems simulates with those systems.
+ * Blob: this header, then u64 offsets[n_blocks + 1], then payload_bytes of payload.  Offsets count bytes into the
+ * payload, start at 0, end at payload_bytes, never decrease and are multiples of 4; block b (rows [512b, 512b + 512))
+ * occupies payload bytes [offsets[b], offsets[b+1]) and holds words + 1 vectors: vectors 0 .. words-1 are the block's
+ * word planes (512 u32 each), vector `words` its mask bytes read as 128 little-endian u32.  A block starts with one kind
+ * byte per vector, zero-padded to a multiple of 4, followed by the vectors' bodies in order; for n elements:
+ *   BGR_CKPT_CONST  (0)  one u32: every element equals it;
+ *   BGR_CKPT_SPARSE (1)  n/32 u32 bitmap (bit i of word j set iff element 32j+i is non-zero), then the non-zero elements
+ *                        in ascending order;
+ *   BGR_CKPT_RAW    (2)  n u32.
+ * The encoded tile is canonical: a word of row r in a plane of column c is zero unless r < rows, the row's alive bit is
+ * set and c's absent bit is clear; a mask byte is zero unless the row exists.  The kind is CONST if all elements are
+ * equal, else SPARSE if nnz < n - n/32, else RAW.  So the blob is a pure function of the frame's content: two engines
+ * whose digests agree produce byte-identical checkpoints. */
+#define BGR_CHECKPOINT_MAGIC 0x43524742u /* "BGRC" */
+#define BGR_CHECKPOINT_VERSION 1u
+#define BGR_CKPT_CONST 0u
+#define BGR_CKPT_SPARSE 1u
+#define BGR_CKPT_RAW 2u
+typedef struct bgr_checkpoint_header {  /* 104 bytes, no padding */
+    uint32_t magic;          /* BGR_CHECKPOINT_MAGIC */
+    uint32_t version;        /* BGR_CHECKPOINT_VERSION */
+    uint64_t layout;         /* bgr_frame_digest_header.layout: same registration layout and order_base */
+    int32_t frame;
+    uint32_t rows;           /* RollbackOrdered::len() of the frame */
+    uint32_t words;          /* word planes per row */
+    uint32_t n_blocks;       /* ceil(rows / 512) */
+    uint32_t n_columns;
+    uint32_t fps;            /* bgr_config.fps: elapsed_ns is only continuable at the same rate */
+    uint64_t active;         /* existing rows */
+    uint64_t elapsed_ns;     /* Time<GgrsTime> of the frame */
+    uint64_t rng[4];         /* ParticleRng of the frame */
+    uint64_t digest_root;    /* bgr_frame_digest_header.root of the frame */
+    uint64_t payload_bytes;
+} bgr_checkpoint_header;
+/* Encodes `frame` (queued or retained; *found = 0: neither) on the GPU.  dst == NULL: *bytes = an upper bound (every
+ * vector RAW), nothing runs.  Otherwise the blob goes to dst (page-locked memory from bgr_host_alloc copies at the full
+ * PCIe rate); BGR_ERR_CAPACITY with *bytes = the exact size if dst_cap is smaller.  Waits for submitted vectors and
+ * leaves their results queued, like bgr_frame_export.  Device memory for the encoding is allocated and freed inside
+ * the call. */
+BGR_API int bgr_checkpoint_save(bgr_engine* e, int32_t frame, void* dst, size_t dst_cap, size_t* bytes, int32_t* found);
+/* Replaces the engine's world with the blob's.  The blob is untrusted input and is checked in full before anything
+ * changes: bad magic or version, another layout, fps or word count, n_blocks != ceil(rows / 512), a truncated or
+ * overlong blob, bad offsets, a kind byte > 2 or non-zero padding, a block whose kinds and bitmaps imply another length
+ * than its offsets give, and a decoded world whose digest root or active count differs from the header's are
+ * BGR_ERR_INVALID_ARGUMENT; rows past a fixed engine's capacity or a growable engine's ceiling BGR_ERR_CAPACITY;
+ * un-collected submits BGR_ERR_STATE (as bgr_reset_session); a sharded engine BGR_ERR_UNSUPPORTED.  A refused call
+ * changes nothing observable.  On success:
+ *   - image 0 holds the decoded world (canonical: see above); RollbackFrameCount = frame, and Time<GgrsTime>,
+ *     ParticleRng and the row count are the header's;
+ *   - the ring keeps its depth and retention setting, and its queue holds exactly one snapshot, of `frame`, holding the
+ *     same bytes, so a first Load(frame) works; with BGR_CFG_DESYNC_CAPTURE that slot is also the frame's first image;
+ *   - first images (witnesses) and retained frames are released; a pending deferred live image is dropped;
+ *   - a growable engine grows to `rows` (after the blob has been verified);
+ *   - ConfirmedFrameCount, MaxPredictionWindow, the call counter of BGR_SYS_U32_STORE_CALL_COUNT and every change
+ *     feed's reported state are left alone: the next feed report lists exactly the rows that differ from what it last
+ *     reported.
+ * Device memory for the decoding (a scratch image of the blob's rows) is allocated and freed inside the call. */
+BGR_API int bgr_checkpoint_restore(bgr_engine* e, const void* blob, size_t bytes);
+
 /* ---- the three schedules, one at a time (SnapshotPlugin-only users: benches/bench.rs:18-27,
  *      mod.rs:510-535 save_world / advance_frame / load_world helpers) -------------------- */
 BGR_API int bgr_save_world(bgr_engine* e, bgr_checksum* checksum_out);         /* world.run_schedule(SaveWorld) */

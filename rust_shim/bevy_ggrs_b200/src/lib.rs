@@ -199,6 +199,31 @@ pub mod p2p_desync {
     }
 }
 
+/// World checkpoints (`bgr_checkpoint_*`; INTEGRATION.md "World checkpoints"): the engine's world at a saved frame as a
+/// compact, canonical blob, and an engine restored from one.  Host-side rollback resources are not part of the blob.
+pub mod checkpoint {
+    use super::{check, engine, sys};
+    use bevy::prelude::World;
+
+    /// The checkpoint of a queued or retained frame; `None` if the engine holds neither.
+    pub fn save(world: &World, frame: i32) -> Option<Vec<u8>> {
+        let e = engine(world);
+        let (mut bytes, mut found) = (0usize, 0i32);
+        check(unsafe { sys::bgr_checkpoint_save(e, frame, core::ptr::null_mut(), 0, &mut bytes, &mut found) });
+        if found == 0 { return None; }
+        let mut blob = vec![0u8; bytes];  // an upper bound; the call reports the exact size
+        check(unsafe { sys::bgr_checkpoint_save(e, frame, blob.as_mut_ptr().cast(), blob.len(), &mut bytes, &mut found) });
+        blob.truncate(bytes);
+        Some(blob)
+    }
+
+    /// Replaces the engine's world with the blob's; panics (like every engine call) on a refused blob, which changes
+    /// nothing.
+    pub fn restore(world: &World, blob: &[u8]) {
+        check(unsafe { sys::bgr_checkpoint_restore(engine(world), blob.as_ptr().cast(), blob.len()) });
+    }
+}
+
 /// Change feed: only the live rows whose existence, presence or tracked field bytes changed since the last report
 /// (`bgr_feed_*`; INTEGRATION.md "Per-tick mirror" applies the records to the ECS).
 pub mod change_feed {

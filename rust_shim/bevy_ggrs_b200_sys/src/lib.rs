@@ -71,6 +71,9 @@ pub use change_feed::*;
 
 mod host_edits;
 pub use host_edits::*;
+// the world checkpoint header too
+mod checkpoint;
+pub use checkpoint::*;
 
 #[repr(C)]
 #[derive(Clone, Copy, Default)]
@@ -174,6 +177,8 @@ extern "C" {
     pub fn bgr_digest_mismatch(local_header: *const bgr_frame_digest_header, local_words: *const u64, remote_header: *const bgr_frame_digest_header, remote_words: *const u64, blocks_out: *mut u32, cap: u32, n_out: *mut u32, host_state_differs: *mut u32) -> c_int;
     pub fn bgr_frame_export(e: *mut bgr_engine, frame: i32, blocks: *const u32, n_blocks: u32, dst: *mut c_void, dst_cap: usize, bytes: *mut usize, found: *mut i32) -> c_int;
     pub fn bgr_desync_diff_remote(e: *mut bgr_engine, frame: i32, blob: *const c_void, bytes: usize, summary: *mut bgr_desync_summary, cols: *mut bgr_desync_column, cols_cap: u32, records: *mut bgr_desync_record, records_cap: u32, n_records: *mut u32, found: *mut i32) -> c_int;
+    pub fn bgr_checkpoint_save(e: *mut bgr_engine, frame: i32, dst: *mut c_void, dst_cap: usize, bytes: *mut usize, found: *mut i32) -> c_int;
+    pub fn bgr_checkpoint_restore(e: *mut bgr_engine, blob: *const c_void, bytes: usize) -> c_int;
     pub fn bgr_save_world(e: *mut bgr_engine, checksum_out: *mut bgr_checksum) -> c_int;
     pub fn bgr_load_world(e: *mut bgr_engine) -> c_int;
     pub fn bgr_advance_world(e: *mut bgr_engine, inputs: *const u8, status: *const u8, n_players: u32) -> c_int;
