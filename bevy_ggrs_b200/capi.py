@@ -65,6 +65,8 @@ BGR_KERNEL_FROM_DEFERRED = 1 << 14
 BGR_KERNEL_PASSIVE_PLANES = 1 << 15
 # ... and the bundle launch stored only the active planes whose content the target did not hold (grids of several waves)
 BGR_KERNEL_STABLE_PLANES = 1 << 26
+# ... and the bundle launch held at least one Save: its target slot already held the content (bgr_held_saves)
+BGR_KERNEL_HELD_SAVES = 1 << 27
 # change feed
 BGR_MAX_FEEDS = 8
 BGR_MAX_FEED_FIELDS = 8
@@ -227,6 +229,7 @@ PROTOTYPES = {
     "bgr_last_path": (C.c_int, [C.c_void_p, u32p]),
     "bgr_generic_specialised": (C.c_int, [C.c_void_p, u32p]),
     "bgr_last_kernel": (C.c_int, [C.c_void_p, u32p]),
+    "bgr_held_saves": (C.c_int, [C.c_void_p, C.c_void_p, C.c_uint32]),
     "bgr_synchronize": (C.c_int, [C.c_void_p]),
     "bgr_stream": (C.c_int, [C.c_void_p, C.POINTER(C.c_void_p)]),
     "bgr_trace_enable": (C.c_int, [C.c_void_p, C.c_uint32]),

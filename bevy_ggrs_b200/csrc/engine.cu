@@ -21,6 +21,7 @@
 #include <vector>
 
 #include "../../include/bevy_ggrs_b200.h"
+#include "content_ids.hpp"
 #include "kernels.cuh"
 #include "particle_rng.hpp"
 #include "ring.hpp"
@@ -150,9 +151,37 @@ struct HostState {  // trivially copyable: copying it per call must not allocate
     //     sharded engine keeps its own table.
     //   - growth maps the table's new segments behind every image's row and zeroes them (unknown); the stamps of the
     //     segments that existed keep their positions and values, as the image bytes they name do.
+    //
+    // Content ids (content_ids.hpp, engines that run the bundle kernel), which name whole images across launches:
+    //   cids.live / cids.slot[s].cid == X != 0  =>  the active planes and alive byte of image 0 / slot s, on every row
+    //   below its row count, are exactly the bytes derivation X produces, and the row count is X's
+    // A Save whose target slot already holds the registers' id (and row count) is held (OPF_HELD): the bundle kernel
+    // stores nothing of it and still checksums the registers.  In the steady state of a SyncTest the re-simulation
+    // from f-d repeats the last tick's Advances on the same content and gets back the same slots (SlotRing frees LIFO),
+    // so every re-save is held and only the new frame is stored.  Who writes an image, and why the invariant holds:
+    //   - derive_content_ids, on the final op list (after consume_deferred rewrote it, before the launch): a LOAD takes
+    //     the slot's record, an ADVANCE takes the id of a slot derived from the same content by an ADVANCE with the same
+    //     key (advance_key: every Op field the result depends on) or a fresh id, an ADVANCE that spawns a fresh id, a
+    //     SAVE gives the target the registers' record, the program's end gives it to image 0.  The derivation is exact:
+    //     equal ids mean equal derivations, never equal hashes.
+    //   - the deferred live image: cids.live names the image the deferring program would have written, and its record
+    //     (base slot's id, the last ADVANCE's key) is searched like a slot's (ContentIds::advance).  The prepended
+    //     [LOAD(base), pending ADVANCEs] derives that same id from the base slot; the materialisation holds no Save.
+    //   - every host write of an image goes through clear_stamps, which also gives the image a fresh id:
+    //     transfer_column to the device (bgr_write_component, bgr_insert_component), bgr_spawn, the startup system,
+    //     bgr_remove_component, bgr_insert_component's presence bit, bgr_despawn, and bgr_checkpoint_restore (image 0
+    //     and the restored slot).  bgr_apply_edits writes image 0 in its own launch and gives it a fresh id itself.
+    //   - growth, desync capture, retention, bgr_reset_session and bgr_set_depth move no bytes below a row count; ids
+    //     stay with their slot indices as the bytes do.
+    //   - every clear of the stamp table (range rollover, stamps_stale) forgets every id (cids.epoch), and the launch
+    //     that clears it stores its held Saves after all: a vector at a clear stores everything, as it did before.
+    //   - only the bundle kernel honours OPF_HELD; an engine that runs any other kernel derives no ids.  A sharded
+    //     engine keeps its own ids.
     uint64_t live_passive_ver = 1, ver_counter = 1;
     std::array<uint64_t, SlotRing::kMaxSlots> slot_passive_ver{};  // 0 = never written
+    ContentIds<SlotRing::kMaxSlots> cids;
 };
+static_assert(std::is_trivially_copyable<HostState>::value, "handle_requests copies HostState on every call");
 
 // The patch k_apply_edits applies (kernels.cuh EditPatch), folded on the host from a validated batch.  The engine keeps
 // one across calls: a batch of thousands of rows allocated (and page-faulted) a megabyte of fresh memory otherwise.
@@ -330,6 +359,13 @@ struct bgr_engine {
     StridedRange stamps;            // content stamps of the active planes (HostState): [images][segments][kActivePlanes]
     uint32_t stamp_next = 1;        // first stamp of the next bundle launch
     bool stamps_stale = false;      // a bundle launch without stamps wrote images since the table was last cleared
+    uint64_t stamp_epoch = 0;       // clears of the whole stamp table (HostState::cids forgets every id at one)
+    // held Saves (HostState content ids).  BGR_TUNE_HELD_SAVES: 0 store every Save, 1 hold (default), 2 hold and
+    // compare each held Save's target with the registers (mismatching words counted in held_check)
+    int tune_held_saves = 1;
+    uint32_t last_held = 0;         // held Saves of the last request vector
+    uint64_t held_total = 0;        // ... of every request vector
+    DeviceBuffer<unsigned long long> held_check;
     bool bundle_static_ck = false;  // both columns checksummed with the finite assertion: fully specialised kernel
     // generic one-launch program (generic_program.cuh): any schema whose tile fits shared memory + the compiled systems
     bool generic_ok = false;
@@ -351,7 +387,7 @@ struct bgr_engine {
     int tune_tma = 1;          // stepwise Save/Load through the TMA-staged bulk-copy kernel
     uint32_t tma_stage_tiles = 0;  // one-tile stages of the TMA copy kernel (0: schema too wide for two stages of shared memory)
     DeviceBuffer<unsigned int> tma_ticket;
-    int occ_cache[2][3][2] = {};  // [passive TMA][MODE][STAMPS]: blocks per SM of k_particles_program
+    int occ_cache[2][3][2][2] = {};  // [passive TMA][MODE][STAMPS][VERIFY]: blocks per SM of k_particles_program
     // desync diff scratch (BGR_CFG_DESYNC_CAPTURE), allocated by the first bgr_desync_diff
     DeviceBuffer<DiffColumn> diff_cols;
     DeviceBuffer<unsigned int> diff_counts;      // [n_cols][3] then the per-tile record counts
@@ -391,9 +427,12 @@ struct bgr_engine {
 
 namespace {
 
-// A write outside the bundle kernel: image `idx`'s content stamps become unknown (HostState).  Stream-ordered behind
-// every launch that could still write them.
+// A write outside the bundle kernel: image `idx`'s content stamps become unknown and its content id fresh (HostState).
+// Stream-ordered behind every launch that could still write them.
 int clear_stamps(bgr_engine* e, uint32_t idx) {
+    ContentIds<SlotRing::kMaxSlots>& c = e->st.cids;
+    if (idx == 0) c.live = c.fresh(e->st.n_rows);
+    else c.slot[idx - 1] = c.fresh(e->st.slot_rows[idx - 1]);
     if (e->stamps.empty()) return BGR_OK;
     CUDA_TRY(cudaMemsetAsync(e->stamps.ptr<uint32_t>() + size_t(idx) * e->stamp_image(), 0, size_t(e->stamp_words()) * sizeof(uint32_t), e->stream));
     e->tiledep_chain = false;
@@ -404,6 +443,7 @@ int clear_stamps(bgr_engine* e, uint32_t idx) {
 int clear_stamp_table(bgr_engine* e) {
     CUDA_TRY(e->stamps.zero(0, size_t(e->stamp_words()) * sizeof(uint32_t), e->stream));
     e->tiledep_chain = false;
+    e->stamp_epoch += 1;
     return BGR_OK;
 }
 
@@ -565,19 +605,51 @@ int compile_requests(bgr_engine* e, HostState& s, const bgr_session_info* sess, 
     return BGR_OK;
 }
 
+// The fields of an ADVANCE op its result depends on (content_ids.hpp).  A spawning ADVANCE also depends on the
+// spawned values: it never derives a known id.
+AdvanceKey advance_key(const Op& op) {
+    AdvanceKey k;
+    k.dt_bits = op.dt_bits; k.fr_bits = op.fr_bits; k.n_rows = op.n_rows; k.call_count = op.call_count;
+    k.n_players = (op.flags >> 8) & 0xFu;
+    std::memcpy(k.inputs, op.inputs, sizeof k.inputs);
+    return k;
+}
+
+// Content ids through the final op list of a bundle program (HostState), and OPF_HELD on every Save whose target slot
+// already holds the registers' content and row count (ContentIds::save).  A held Save must also skip the passive
+// planes: it then stores nothing at all.
+void derive_content_ids(bgr_engine* e, HostState& s, Program& pg) {
+    ContentIds<SlotRing::kMaxSlots>& c = s.cids;
+    c.sync_epoch(e->stamp_epoch);  // a clear of the stamp table since the last program forgets every id
+    auto slot_of = [&](const Op& op) { return uint32_t((size_t(op.image_off256) << 8) / e->image_bytes) - 1u; };
+    ContentRecord reg = c.live;  // the registers' content
+    for (uint32_t i = 0; i < pg.n_ops; ++i) {
+        Op& op = pg.ops[i];
+        if (op.kind == OP_LOAD) {
+            reg = c.slot[slot_of(op)];
+        } else if (op.kind == OP_ADVANCE) {
+            reg = (op.flags & OPF_SPAWN) ? c.fresh(op.n_rows + op.save_index) : c.advance(reg, advance_key(op));
+        } else if (!(op.flags & OPF_NO_STORE)) {
+            const bool may_hold = e->tune_held_saves && (op.flags & OPF_SKIP_PASSIVE);
+            if (c.save(slot_of(op), reg, op.n_rows, may_hold)) op.flags |= OPF_HELD;
+        }
+    }
+    c.live = reg;
+}
+
 // ---------------------------------------------------------------------------------------------
 // launch: fused bundle kernel
 // ---------------------------------------------------------------------------------------------
-template <int MODE, bool STAMPS>
+template <int MODE, bool STAMPS, bool VERIFY>
 int launch_particles(bgr_engine* e, const ProgramParams& pp) {
-    auto kern = k_particles_program<MODE, STAMPS>;
+    auto kern = k_particles_program<MODE, STAMPS, VERIFY>;
     constexpr int kBlock = int(kTileRows) / 2;  // two rows per thread
     const int ti = (pp.flags & PF_PASSIVE_TMA) ? 1 : 0;
     const size_t smem = ti ? size_t(2) * pp.passive_bytes : 0;
     // A mode runs with and without the passive double buffer (spawns and multi-Load vectors move passive planes per
     // thread): the shared-memory opt-in and the occupancy are per (mode, buffer).  passive_bytes is fixed at bgr_build,
     // so one entry per buffer setting is exact.
-    int& occ = e->occ_cache[ti][MODE][STAMPS ? 1 : 0];
+    int& occ = e->occ_cache[ti][MODE][STAMPS ? 1 : 0][VERIFY ? 1 : 0];
     if (occ == 0) {
         if (smem > 48 * 1024) CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem)));
         int nb = 0;
@@ -606,11 +678,11 @@ int launch_particles(bgr_engine* e, const ProgramParams& pp) {
     return BGR_OK;
 }
 
-template <bool STAMPS>
+template <bool STAMPS, bool VERIFY>
 int launch_fused_variant(bgr_engine* e, const ProgramParams& pp) {
-    if (e->bundle_opt) return launch_particles<2, STAMPS>(e, pp);         // per-entity presence
-    if (e->bundle_static_ck) return launch_particles<1, STAMPS>(e, pp);   // both columns checksummed with the finite assertion
-    return launch_particles<0, STAMPS>(e, pp);
+    if (e->bundle_opt) return launch_particles<2, STAMPS, VERIFY>(e, pp);         // per-entity presence
+    if (e->bundle_static_ck) return launch_particles<1, STAMPS, VERIFY>(e, pp);   // both columns checksummed with the finite assertion
+    return launch_particles<0, STAMPS, VERIFY>(e, pp);
 }
 
 int run_fused(bgr_engine* e, const Program& pg, uint32_t buf) {
@@ -672,7 +744,12 @@ int run_fused(bgr_engine* e, const Program& pg, uint32_t buf) {
         if (rc != BGR_OK) return rc;
         e->stamp_next = 1;
         e->stamps_stale = false;
+        // the clear forgets every content id (HostState): this launch stores its held Saves after all
+        for (uint32_t i = 0; i < pg.n_ops; ++i) pp.ops[i].flags &= ~uint32_t(OPF_HELD);
     }
+    uint32_t held = 0;
+    for (uint32_t i = 0; i < pg.n_ops; ++i) held += (pp.ops[i].flags & OPF_HELD) ? 1u : 0u;
+    if (held && e->tune_held_saves == 2) pp.held_check = e->held_check.get();
     if (!stamps) e->stamps_stale = true;
     pp.stamps = e->stamps.ptr<uint32_t>();
     pp.stamp_image = e->stamp_image();
@@ -711,8 +788,14 @@ int run_fused(bgr_engine* e, const Program& pg, uint32_t buf) {
     pp.ticket = e->d_ticket_set[set];
     pp.out = pg.internal ? e->internal_out.get() : e->d_out[buf];
     if (e->trace.get() && !pg.internal && e->seq - e->trace_first_seq < e->trace_cap) pp.trace = e->trace.get() + (e->seq - e->trace_first_seq) * 4;
-    int rc = stamps ? launch_fused_variant<true>(e, pp) : launch_fused_variant<false>(e, pp);
+    int rc = pp.held_check ? (stamps ? launch_fused_variant<true, true>(e, pp) : launch_fused_variant<false, true>(e, pp))
+                           : (stamps ? launch_fused_variant<true, false>(e, pp) : launch_fused_variant<false, false>(e, pp));
     if (rc != BGR_OK) return rc;
+    if (!pg.internal) {
+        e->last_held = held;
+        e->held_total += held;
+        if (held) e->last_kernel |= BGR_KERNEL_HELD_SAVES;
+    }
     e->tiledep_chain = tiledep;
     e->tiledep_seq = uint32_t(e->seq); e->tiledep_tiles = pp.n_tiles;
     return BGR_OK;
@@ -1236,6 +1319,7 @@ int submit(bgr_engine* e, const bgr_session_info* sess, const bgr_request* reqs,
     const bool fused = bundle || generic;   // one launch for the whole request vector
     rc = fused ? consume_deferred(e, pg) : materialize_live(e);
     if (rc != BGR_OK) return rc;
+    if (bundle) derive_content_ids(e, s, pg);
     DeferredLive next;
     if (fused && e->tune_defer_live && !e->live_touched) next = plan_deferral(pg);
     rc = bundle ? run_fused(e, pg, buf) : generic ? run_generic(e, pg, buf) : run_stepwise(e, pg, buf);
@@ -1815,6 +1899,7 @@ int apply_edits(bgr_engine* e, const bgr_edit* edits, uint32_t n, const void* va
     e->tiledep_chain = false;
     e->st.n_rows = uint32_t(rows);
     if (f.bump) e->st.live_passive_ver = ++e->st.ver_counter;
+    e->st.cids.live = e->st.cids.fresh(e->st.n_rows);
     return BGR_OK;
 }
 
@@ -1939,6 +2024,7 @@ BGR_API int bgr_engine_create(const bgr_config* cfg, bgr_engine** out) {
     e->tune_stagger_ns = env_int("BGR_TUNE_STAGGER_NS", 800);
     e->tune_bundle = env_int("BGR_TUNE_BUNDLE", 1);
     e->tune_defer_live = env_int("BGR_TUNE_DEFER_LIVE", 1);
+    e->tune_held_saves = env_int("BGR_TUNE_HELD_SAVES", 1);
     // tests: the first content stamp issued, so that the range rollover in run_fused is reached within a few launches
     if (const char* v = std::getenv("BGR_TEST_STAMP_FIRST"); v && *v)
         e->stamp_next = uint32_t(std::max(1ul, std::min(std::strtoul(v, nullptr, 0), 0xFFFFFFFFul)));
@@ -2134,6 +2220,10 @@ BGR_API int bgr_build(bgr_engine* e) {
             CUDA_TRY(cudaMemsetAsync(e->tma_ticket.get(), 0, 4 * sizeof(unsigned int), e->stream));
         }
     }
+    if (e->tune_held_saves == 2 && use_bundle(e)) {
+        CUDA_TRY(e->held_check.ensure(1));
+        CUDA_TRY(cudaMemsetAsync(e->held_check.get(), 0, sizeof(unsigned long long), e->stream));
+    }
     std::string err;
     for (const CapacityBuffer& b : capacity_buffers(e))
         if (b.wanted && !create_range(e, b, &err)) return fail(BGR_ERR_CUDA, err);
@@ -2169,10 +2259,10 @@ BGR_API int bgr_run_startup_system(bgr_engine* e, uint32_t system) {
         e->st.n_rows, rate, e->spawn[0].dev(), uint32_t(ttl), uint32_t(ttl >> 32));
     e->launches += 1;
     CUDA_TRY(cudaGetLastError());
+    e->st.n_rows += rate;  // before clear_stamps: the fresh content id carries the new row count
     rc = clear_stamps(e, 0);
     if (rc != BGR_OK) return rc;
     CUDA_TRY(cudaStreamSynchronize(e->stream));
-    e->st.n_rows += rate;
     e->st.live_passive_ver = ++e->st.ver_counter;
     return BGR_OK;
 }
@@ -2193,11 +2283,11 @@ BGR_API int bgr_spawn(bgr_engine* e, uint32_t count, uint32_t* first_row_out) {
         k_spawn_rows<<<e->grid_for(count, 64), 256, 0, e->stream>>>(e->image(0), e->words, first, count);
         e->launches += 1;
         CUDA_TRY(cudaGetLastError());
+        e->st.n_rows += count;  // before clear_stamps: the fresh content id carries the new row count
         rc = clear_stamps(e, 0);
         if (rc != BGR_OK) return rc;
         CUDA_TRY(cudaStreamSynchronize(e->stream));
     }
-    e->st.n_rows += count;
     e->st.live_passive_ver = ++e->st.ver_counter;
     if (first_row_out) *first_row_out = first;
     return BGR_OK;
@@ -3015,6 +3105,7 @@ BGR_API int bgr_checkpoint_restore(bgr_engine* e, const void* blob, size_t bytes
     s.slot_rows[slot] = h.rows;
     s.slot_elapsed_ns[slot] = h.elapsed_ns;
     s.slot_rng[slot] = rng;
+    s.cids.live = s.cids.slot[slot] = s.cids.fresh(h.rows);
     s.live_passive_ver = ++s.ver_counter;  // image 0 holds new content; the restored slot holds the same
     s.slot_passive_ver[slot] = s.live_passive_ver;
     CUDA_TRY(cudaStreamSynchronize(e->stream));  // before the scratch image is freed
@@ -3165,6 +3256,16 @@ BGR_API int bgr_last_path(bgr_engine* e, uint32_t* fused_out) {
 BGR_API int bgr_last_kernel(bgr_engine* e, uint32_t* kernel_out) {
     if (!e || !kernel_out) return fail(BGR_ERR_INVALID_ARGUMENT, "null argument");
     *kernel_out = e->last_kernel; return BGR_OK;
+}
+BGR_API int bgr_held_saves(bgr_engine* e, uint64_t* out, uint32_t cap) {
+    if (!e || !out) return fail(BGR_ERR_INVALID_ARGUMENT, "null argument");
+    uint64_t v[3] = {e->last_held, e->held_total, 0};
+    if (e->held_check.get()) {
+        CUDA_TRY(cudaMemcpyAsync(&v[2], e->held_check.get(), sizeof v[2], cudaMemcpyDeviceToHost, e->stream));
+        CUDA_TRY(cudaStreamSynchronize(e->stream));
+    }
+    for (uint32_t i = 0; i < cap && i < 3; ++i) out[i] = v[i];
+    return BGR_OK;
 }
 BGR_API int bgr_synchronize(bgr_engine* e) {
     if (!e) return fail(BGR_ERR_INVALID_ARGUMENT, "null engine");

@@ -80,6 +80,10 @@ enum OpFlags : uint32_t {
     // Only this bundle kernel honours it; every other kernel stores whole images, which keeps the versions true.  A
     // kernel that stores partial images must keep versions of its own.
     OPF_SKIP_PASSIVE = 4u,
+    // SAVE: the slot already holds the active planes and alive byte of the registers on every row below the row count
+    // (content ids, engine.cu HostState): no active store, no stamp.  The checksum is still computed from the
+    // registers.  Only this bundle kernel honours it, like OPF_SKIP_PASSIVE; it says nothing about passive planes.
+    OPF_HELD = 16u,
     // bits 8..11 of an ADVANCE op's flags: number of players (PlayerInputs<T>.len())
 };
 
@@ -164,6 +168,7 @@ struct ProgramParams {
     uint32_t* stamps;               // [images][segments][kActivePlanes] content stamps (0 = unknown)
     uint32_t stamp_image;           // words of one image's row of `stamps`
     uint32_t stamp_base;            // this launch's fresh stamps: stamp_base + op index, stamp_base + n_ops for the live write
+    unsigned long long* held_check;  // nullptr, or (BGR_TUNE_HELD_SAVES=2) where held Saves count the words the target lacks
     PassiveRun runs[kMaxRuns];
     uint16_t passive[kMaxPassive];
     uint32_t passive_template[kMaxPassive];   // value of each passive word in a freshly spawned row (Transform::default())
@@ -428,7 +433,9 @@ __device__ __forceinline__ void run_system(const SysSpec& sy, Word&& word, const
 // call costs" has the measurements against 1 and 4 rows per thread and the other launch-bounds tiers.
 // STAMPS: stable-plane elision (content stamps, below).  It pays on bandwidth-bound grids of several waves; a single-wave
 // grid is latency-bound, and there the instance without it runs (engine.cu run_fused), which stores every active plane.
-template <int MODE, bool STAMPS>
+// VERIFY: BGR_TUNE_HELD_SAVES=2, every held Save compares its target with the registers (check_held).  The instances
+// that run by default do not carry that code.
+template <int MODE, bool STAMPS, bool VERIFY>
 __global__ void __launch_bounds__(256, 3) k_particles_program(const __grid_constant__ ProgramParams p) {
     constexpr int VEC = 2, BLOCK = 256;  // rows per thread, threads per block (__launch_bounds__)
     static_assert(VEC * BLOCK == int(kTileRows), "a block iteration covers one tile");
@@ -602,6 +609,29 @@ __global__ void __launch_bounds__(256, 3) k_particles_program(const __grid_const
                 if (planes & (64u << k)) vec_store<VEC>(pl + k * kPlaneBytes, tl[k]);
             if (planes & kAlivePlaneBit) alive_store<VEC>(img + aoff, alive);
         };
+        // BGR_TUNE_HELD_SAVES=2: count the active words and alive bytes, on rows below the row count, in which a held
+        // Save's target differs from the registers
+        auto check_held = [&](const uint8_t* img, uint32_t n_rows) {
+            uint32_t r[8][VEC];
+            const uint8_t* pt = img + p.t_off + woff;
+            const uint8_t* pv = img + p.v_off + woff;
+            const uint8_t* pl = img + p.l_off + woff;
+#pragma unroll
+            for (int k = 0; k < 3; ++k) { vec_load<VEC>(pt + k * kPlaneBytes, r[k]); vec_load<VEC>(pv + k * kPlaneBytes, r[3 + k]); }
+#pragma unroll
+            for (int k = 0; k < 2; ++k) vec_load<VEC>(pl + k * kPlaneBytes, r[6 + k]);
+            const uint32_t a = alive_load<VEC>(img + aoff);
+            uint32_t bad = 0;
+#pragma unroll
+            for (int j = 0; j < VEC; ++j) {
+                if (row0 + j >= n_rows) continue;
+                bad += (r[0][j] != tr[0][j]) + (r[1][j] != tr[1][j]) + (r[2][j] != tr[2][j]) + (r[3][j] != vl[0][j]) +
+                       (r[4][j] != vl[1][j]) + (r[5][j] != vl[2][j]) + (r[6][j] != tl[0][j]) + (r[7][j] != tl[1][j]) +
+                       (((a ^ alive) >> (8 * j)) & 0xFFu ? 1u : 0u);
+            }
+            bad = __reduce_add_sync(0xffffffffu, bad);
+            if (lane == 0 && bad) atomicAdd(p.held_check, (unsigned long long)bad);
+        };
 
         if (p.flags & PF_READ_LIVE) load_active(p.arena, p.live_rows, 0u);
         else load_active(p.arena + (size_t(p.ops[0].image_off256) << 8), p.ops[0].n_rows, p.ops[0].call_count);  // ops[0] is a LOAD
@@ -733,9 +763,12 @@ __global__ void __launch_bounds__(256, 3) k_particles_program(const __grid_const
                 }
             } else if (kind == OP_SAVE) {
                 uint8_t* img = p.arena + (size_t(p.ops[i].image_off256) << 8);
-                const bool store = !(p.ops[i].flags & OPF_NO_STORE);
+                // a held Save stores nothing and claims no stamp: `dirty` keeps collecting until the next stored Save,
+                // and the target's stamps still name its bytes
+                const bool store = !(p.ops[i].flags & (OPF_NO_STORE | OPF_HELD));
                 const uint32_t held = store ? claim_stamps(p.ops[i].call_count, p.stamp_base + i) : 0u;
                 if (store && !STAMPS) store_active(img, p.ops[i].call_count, held);  // nothing to wait for: issue the stores first
+                if (VERIFY && (p.ops[i].flags & OPF_HELD)) check_held(img, p.ops[i].n_rows);
                 // ---- checksum partials (component_checksum.rs:81-90) ----
                 uint64_t hx_t = 0, hx_v = 0;
                 uint32_t bad = 0;

@@ -26,7 +26,7 @@ class LastKernel(NamedTuple):
     deferred_live: the vector did not write the live image (BGR_TUNE_DEFER_LIVE); from_deferred: it started from the
     base slot of the previous vector's deferred live image.  passive_tma: the bundle ran in its passive-TMA
     configuration; passive_planes: the bundle launch read or wrote passive planes at all (clear on ticks whose slots
-    already hold them)."""
+    already hold them); held_saves: at least one of its Saves stored nothing, its slot already holding that content."""
     kind: str
     vec: int
     mode: int
@@ -38,13 +38,15 @@ class LastKernel(NamedTuple):
     from_deferred: bool = False
     passive_planes: bool = False
     stable_planes: bool = False
+    held_saves: bool = False
 
     @staticmethod
     def decode(v: int) -> "LastKernel":
         return LastKernel(_KERNEL_KINDS.get(v & 0xF, f"unknown({v & 0xF})"), (v >> 4) & 0xF, (v >> 8) & 0x3,
                           (v >> 10) & 0x3, bool((v >> 12) & 1), (v >> 16) & 0x3FF, v,
                           bool(v & capi.BGR_KERNEL_DEFERRED_LIVE), bool(v & capi.BGR_KERNEL_FROM_DEFERRED),
-                          bool(v & capi.BGR_KERNEL_PASSIVE_PLANES), bool(v & capi.BGR_KERNEL_STABLE_PLANES))
+                          bool(v & capi.BGR_KERNEL_PASSIVE_PLANES), bool(v & capi.BGR_KERNEL_STABLE_PLANES),
+                          bool(v & capi.BGR_KERNEL_HELD_SAVES))
 
 
 class FeedInfo(NamedTuple):
@@ -469,6 +471,13 @@ class Engine:
         v = C.c_uint32()
         self._check(self._lib.bgr_last_kernel(self._h, C.byref(v)))
         return LastKernel.decode(v.value)
+
+    def held_saves(self) -> dict:
+        """bgr_held_saves: Saves of the last request vector and of all so far that stored nothing, and (env
+        BGR_TUNE_HELD_SAVES=2) the words in which a held Save's target differed from the registers (waits for the GPU)."""
+        out = (C.c_uint64 * 3)()
+        self._check(self._lib.bgr_held_saves(self._h, out, 3))
+        return {"last": out[0], "total": out[1], "mismatched_words": out[2]}
 
     def synchronize(self) -> None:
         self._check(self._lib.bgr_synchronize(self._h))

@@ -656,11 +656,15 @@ BGR_API int bgr_generic_specialised(bgr_engine* e, uint32_t* specialised_out);
  *   bits 16-25 bundle and generic NVRTC: rows per work item (512 = a whole tile)
  *   bit 26     BGR_KERNEL_STABLE_PLANES, bundle: stable-plane elision.  Each warp stored only the active planes of its
  *              64-row segment whose content the target image did not already hold (device-side content stamps).  Set on
- *              grids of several waves; a single-wave (latency-bound) grid stores every active plane */
+ *              grids of several waves; a single-wave (latency-bound) grid stores every active plane
+ *   bit 27     BGR_KERNEL_HELD_SAVES, bundle: at least one Save was held: its target slot already held the content and
+ *              row count it would have stored (host-side content ids), so it stored nothing and only checksummed
+ *              (bgr_held_saves; env BGR_TUNE_HELD_SAVES, default 1) */
 #define BGR_KERNEL_DEFERRED_LIVE (1u << 13)
 #define BGR_KERNEL_FROM_DEFERRED (1u << 14)
 #define BGR_KERNEL_PASSIVE_PLANES (1u << 15)
 #define BGR_KERNEL_STABLE_PLANES (1u << 26)
+#define BGR_KERNEL_HELD_SAVES (1u << 27)
 #define BGR_KERNEL_NONE 0u
 #define BGR_KERNEL_STEPWISE_TMA 1u       /* one kernel per request; Save / Load through the TMA-staged copy kernel */
 #define BGR_KERNEL_STEPWISE_FLAT 2u      /* one kernel per request; k_checksum_column + k_copy_image */
@@ -668,6 +672,11 @@ BGR_API int bgr_generic_specialised(bgr_engine* e, uint32_t* specialised_out);
 #define BGR_KERNEL_GENERIC_INTERPRETER 4u
 #define BGR_KERNEL_GENERIC_NVRTC 5u
 BGR_API int bgr_last_kernel(bgr_engine* e, uint32_t* kernel_out);
+/* Held Saves of the bundle kernel (bit 27 above): out[0] in the last request vector, [1] in every request vector so
+ * far, [2] with BGR_TUNE_HELD_SAVES=2 (verify) the active words and alive bytes, below the row count, in which a held
+ * Save's target differed from what the Save would have stored, counted on the GPU (waits for it; 0 otherwise).
+ * cap <= 3 */
+BGR_API int bgr_held_saves(bgr_engine* e, uint64_t* out, uint32_t cap);
 BGR_API int bgr_synchronize(bgr_engine* e);
 BGR_API int bgr_stream(bgr_engine* e, void** stream_out);        /* the cudaStream_t the engine launches on (timing events) */
 /* device-side launch trace: 4 x u64 per fused launch after the call, up to `capacity` launches (GPU globaltimer ns):

@@ -50,6 +50,8 @@ pub const BGR_KERNEL_FROM_DEFERRED: u32 = 1 << 14;
 pub const BGR_KERNEL_PASSIVE_PLANES: u32 = 1 << 15;
 /// bgr_last_kernel flag: the bundle launch stored only the active planes whose content the target did not hold.
 pub const BGR_KERNEL_STABLE_PLANES: u32 = 1 << 26;
+/// bgr_last_kernel flag: the bundle launch held at least one Save (its target slot already held that content).
+pub const BGR_KERNEL_HELD_SAVES: u32 = 1 << 27;
 
 pub const BGR_CFG_FORCE_STEPWISE: u32 = 1;
 pub const BGR_CFG_SHARDED: u32 = 2;
@@ -198,6 +200,7 @@ extern "C" {
     pub fn bgr_last_path(e: *mut bgr_engine, fused_out: *mut u32) -> c_int;
     pub fn bgr_generic_specialised(e: *mut bgr_engine, specialised_out: *mut u32) -> c_int;
     pub fn bgr_last_kernel(e: *mut bgr_engine, kernel_out: *mut u32) -> c_int;
+    pub fn bgr_held_saves(e: *mut bgr_engine, out: *mut u64, cap: u32) -> c_int;
     pub fn bgr_synchronize(e: *mut bgr_engine) -> c_int;
     pub fn bgr_stream(e: *mut bgr_engine, stream_out: *mut *mut c_void) -> c_int;
     pub fn bgr_trace_enable(e: *mut bgr_engine, capacity: u32) -> c_int;

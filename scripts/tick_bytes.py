@@ -16,6 +16,9 @@ BGR_KERNEL_STABLE_PLANES); the launch trace counts the 64-byte units of active p
     stored bytes   = read image x rows x 33 B + stored units x 64 B + stamp traffic
     stamp traffic  = (1 + Saves) x segments x 36 B read + one 4-byte stamp written per stored word plane-segment
 
+A held Save (its slot already holds the content, host-side content ids, bgr_held_saves) stores nothing and reads no
+stamps: held_stored_bytes() leaves its stamp reads out.  In the steady state 7 of the 8 Saves are held.
+
 In the same process it runs tools/hbm_mix_bench.cu's fan-out (1 read : 8 writes) over the active footprint, and the
 same fan-out with the writes cut to the stored share, and prints the card's name and power limit.  One JSON line on
 stdout.
@@ -45,6 +48,11 @@ ACTIVE_PLANES = 9
 def stored_bytes(rows: int, n_saves: int, units: int) -> int:
     segs = -(-rows // SEG_ROWS)
     return rows * ACTIVE_BYTES + units * 64 + (1 + n_saves) * segs * ACTIVE_PLANES * 4 + units
+
+
+def held_stored_bytes(rows: int, n_saves: int, n_held: int, units: int) -> int:
+    """stored_bytes() of a tick that held n_held of its Saves."""
+    return stored_bytes(rows, n_saves - n_held, units)
 
 
 def images_touched(n_saves: int, deferred_live: bool) -> int:
@@ -103,17 +111,22 @@ def main():
         pos[0] += k
         return out
 
+    held = []
+
     def submit(t, moved):
         eng.submit_prepared(t[3], t[0], t[1])
         k = eng.last_kernel()
         moved.append((tick_bytes(rows, len(t[4]), k.deferred_live, k.passive_planes), k.passive_planes))
+        held.append(eng.held_saves()["last"])
 
     def traced(leg_fn, tl, moved):
         eng.trace_enable(len(tl))
+        del held[:]
         leg_fn(tl, moved)
         tr = eng.trace_read(len(tl))
         eng.trace_enable(0)
-        return [(stored_bytes(rows, len(t[4]), int(r[3])), int(r[3]) * 64 // len(t[4])) for t, r in zip(tl, tr)]
+        return [(held_stored_bytes(rows, len(t[4]), h, int(r[3])), int(r[3]) * 64 // max(1, len(t[4]) - h), h)
+                for t, r, h in zip(tl, tr, held)]
 
     def pipelined(tl, moved):
         inflight = 0
@@ -157,16 +170,17 @@ def main():
     image = ACTIVE_BYTES * (-(-n // TILE_ROWS) * TILE_ROWS)
     fan = fanout_ceiling(image, steady_saves)
     # the stored mix: each write carries the share of the image a steady-state Save stores
-    per_save = sorted(w for _, w in stored_p)[len(stored_p) // 2]   # data bytes one steady-state Save stores
+    per_save = sorted(w for _, w, _ in stored_p)[len(stored_p) // 2]   # data bytes one stored steady-state Save stores
     fan_stored = fanout_ceiling(image, steady_saves, min(image, per_save) // 16 * 16)
 
     def leg(us, moved, stored):
         b = sum(m for m, _ in moved) / len(moved)
-        s = sum(b for b, _ in stored) / len(stored)
+        s = sum(b for b, _, _ in stored) / len(stored)
         return {"us_per_tick": us, "frames_per_s": ticks[-1][2] / (us * 1e-6), "bytes_per_tick": b,
                 "ticks_with_passive_planes": sum(p for _, p in moved), "achieved_gbps": b / (us * 1e-6) / 1e9,
                 "frac_of_fanout_stg": b / (us * 1e-6) / 1e9 / fan["fanout_stg"]["gbps"],
                 "stored_bytes_per_tick": s, "stored_gbps": s / (us * 1e-6) / 1e9,
+                "held_saves_per_tick": sum(h for _, _, h in stored) / len(stored),
                 "frac_of_stored_mix_stg": s / (us * 1e-6) / 1e9 / fan_stored["fanout_stg"]["gbps"]}
 
     print(json.dumps({"card": card(), "torch_device": torch.cuda.get_device_name(0), "entities": n, "check_distance": d,
