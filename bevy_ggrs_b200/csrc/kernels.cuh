@@ -200,6 +200,14 @@ __device__ __forceinline__ void publish_pair(unsigned long long* out, uint32_t i
     reinterpret_cast<ulonglong2*>(out)[i] = make_ulonglong2(v, v ^ result_tag(seq, i));  // one 16-byte store
 }
 __device__ __forceinline__ uint32_t f32_bits_nonfinite(uint32_t b) { return ((b & 0x7f800000u) == 0x7f800000u) ? 1u : 0u; }
+template <bool B> struct BoolConst { static constexpr bool value = B; };  // a compile-time flag passed to a generic lambda
+// f32_bits_nonfinite of any of three words, on the FP32 pipe: x * 0 is NaN exactly when x is an infinity or a NaN (and
+// +-0 otherwise), and a NaN addend carries through the fused multiply-adds.  Three FP32 instructions and one compare
+// instead of three masks and three compares on the integer pipes the checksum keeps busy.
+__device__ __forceinline__ uint32_t f32x3_bits_nonfinite(uint32_t a, uint32_t b, uint32_t c) {
+    const float z = __fmaf_rn(__uint_as_float(a), 0.0f, __fmaf_rn(__uint_as_float(b), 0.0f, __fmul_rn(__uint_as_float(c), 0.0f)));
+    return z != z ? 1u : 0u;
+}
 
 // mask with byte j = 0x01 for every row (row0 + j) < n_rows
 template <int VEC> __device__ __forceinline__ uint32_t rows_mask(uint32_t row0, uint32_t n_rows) {
@@ -436,7 +444,7 @@ __device__ __forceinline__ void run_system(const SysSpec& sy, Word&& word, const
 // VERIFY: BGR_TUNE_HELD_SAVES=2, every held Save compares its target with the registers (check_held).  The instances
 // that run by default do not carry that code.
 template <int MODE, bool STAMPS, bool VERIFY>
-__global__ void __launch_bounds__(256, 3) k_particles_program(const __grid_constant__ ProgramParams p) {
+__global__ void __launch_bounds__(256, 3) k_particles_program(const __grid_constant__ ProgramParams p) {  // budget: prologue
     constexpr int VEC = 2, BLOCK = 256;  // rows per thread, threads per block (__launch_bounds__)
     static_assert(VEC * BLOCK == int(kTileRows), "a block iteration covers one tile");
     constexpr bool STATIC_CK = MODE == 1;
@@ -517,7 +525,7 @@ __global__ void __launch_bounds__(256, 3) k_particles_program(const __grid_const
             }
         }
     };
-    for (uint32_t tile = blockIdx.x; tile < p.n_tiles; ++it) {
+    for (uint32_t tile = blockIdx.x; tile < p.n_tiles; ++it) {  // budget: tile_loop
         if (dynamic && tid == 0) claimed = gridDim.x + atomicAdd(&p.ticket[1], 1u);  // published after the loads below
         const uint32_t i0 = tid * VEC;  // first row of this thread inside the tile
         if (tile_wait && tile < p.wait_tiles) {
@@ -547,7 +555,7 @@ __global__ void __launch_bounds__(256, 3) k_particles_program(const __grid_const
             });
         }
 
-        // ------------------------------ active words ------------------------------
+        // ------------------------------ active words ------------------------------  budget: load
         uint32_t tr[3][VEC], vl[3][VEC], tl[2][VEC];
         uint32_t alive = 0;
         // Stable-plane elision.  Lane q < kActivePlanes holds `st`, the stamp of the content plane q of this warp's
@@ -641,6 +649,7 @@ __global__ void __launch_bounds__(256, 3) k_particles_program(const __grid_const
 #pragma unroll
         for (int j = 0; j < VEC; ++j) t0[j] = sea_order_lane(p.order_base + row0 + j);
 
+        // budget: tile_loop
         if (dynamic && tid == 0) {  // publish the tile of iteration it + 1 (ring entry `it`)
             const uint32_t slot = it % kRing, use = it / kRing;
             if (use > 0) mbar_wait(&s_empty[slot], (use - 1) & 1u);  // every warp has read the previous occupant
@@ -705,7 +714,7 @@ __global__ void __launch_bounds__(256, 3) k_particles_program(const __grid_const
 
         for (uint32_t i = (p.flags & PF_READ_LIVE) ? 0u : 1u; i < p.n_ops; ++i) {
             const uint32_t kind = p.ops[i].kind;
-            if (kind == OP_ADVANCE) {
+            if (kind == OP_ADVANCE) {  // budget: advance
                 const float dt = __uint_as_float(p.ops[i].dt_bits);
                 const uint32_t alive_before = alive;
 #pragma unroll
@@ -761,7 +770,7 @@ __global__ void __launch_bounds__(256, 3) k_particles_program(const __grid_const
                         }
                     }
                 }
-            } else if (kind == OP_SAVE) {
+            } else if (kind == OP_SAVE) {  // budget: save_store
                 uint8_t* img = p.arena + (size_t(p.ops[i].image_off256) << 8);
                 // a held Save stores nothing and claims no stamp: `dirty` keeps collecting until the next stored Save,
                 // and the target's stamps still name its bytes
@@ -769,7 +778,7 @@ __global__ void __launch_bounds__(256, 3) k_particles_program(const __grid_const
                 const uint32_t held = store ? claim_stamps(p.ops[i].call_count, p.stamp_base + i) : 0u;
                 if (store && !STAMPS) store_active(img, p.ops[i].call_count, held);  // nothing to wait for: issue the stores first
                 if (VERIFY && (p.ops[i].flags & OPF_HELD)) check_held(img, p.ops[i].n_rows);
-                // ---- checksum partials (component_checksum.rs:81-90) ----
+                // ---- checksum partials (component_checksum.rs:81-90) ----  budget: save_hash
                 uint64_t hx_t = 0, hx_v = 0;
                 uint32_t bad = 0;
                 // z == +0.0f for every row of the warp (a 2-D world): the tail lane of the 12-byte hash is a
@@ -782,26 +791,34 @@ __global__ void __launch_bounds__(256, 3) k_particles_program(const __grid_const
 #endif
                 const bool tz_zero = BGR_ZERO_TAIL && CKT && __all_sync(0xffffffffu, tz_any == 0u);
                 const bool vz_zero = BGR_ZERO_TAIL && CKV && __all_sync(0xffffffffu, vz_any == 0u);
+                // One warp-uniform branch around the whole block: when every checksummed column's z is +0.0f, the block has
+                // no branch inside and ptxas interleaves the four independent hash chains of the thread.  (A branch per row
+                // and column around a tail diffusion splits them into separate blocks, and the 1M tick gets slower.)
+                auto hash_rows = [&](auto zero_tails) {
+                    constexpr bool Z = decltype(zero_tails)::value;
 #pragma unroll
-                for (int j = 0; j < VEC; ++j) {
-                    const uint32_t m = (alive >> (8 * j)) & 0xFFu;
-                    const uint64_t live = (m & 1u) ? ~0ULL : 0ULL;
-                    const uint64_t live_t = OPT ? (row_matches(m, p.need_t) ? ~0ULL : 0ULL) : live;
-                    const uint64_t live_v = OPT ? (row_matches(m, p.need_v) ? ~0ULL : 0ULL) : live;
-                    if (CKT) {
-                        if (FINT) bad |= (f32_bits_nonfinite(tr[0][j]) | f32_bits_nonfinite(tr[1][j]) | f32_bits_nonfinite(tr[2][j])) & uint32_t(live_t);
-                        const uint64_t lane_t = tz_zero ? kSeaTailZero : sea_diffuse(kSeaB ^ uint64_t(tr[2][j]));
-                        uint64_t c = sea_hash_12_lane(uint64_t(tr[0][j]) | (uint64_t(tr[1][j]) << 32), lane_t);
-                        hx_t ^= sea_hash_entity(t0[j], c) & live_t;
+                    for (int j = 0; j < VEC; ++j) {
+                        const uint32_t m = (alive >> (8 * j)) & 0xFFu;
+                        const uint64_t live = (m & 1u) ? ~0ULL : 0ULL;
+                        const uint64_t live_t = OPT ? (row_matches(m, p.need_t) ? ~0ULL : 0ULL) : live;
+                        const uint64_t live_v = OPT ? (row_matches(m, p.need_v) ? ~0ULL : 0ULL) : live;
+                        if (CKT) {
+                            if (FINT) bad |= f32x3_bits_nonfinite(tr[0][j], tr[1][j], tr[2][j]) & uint32_t(live_t);
+                            const uint64_t lane_t = (Z || tz_zero) ? kSeaTailZero : sea_diffuse(kSeaB ^ uint64_t(tr[2][j]));
+                            uint64_t c = sea_hash_12_lane(uint64_t(tr[0][j]) | (uint64_t(tr[1][j]) << 32), lane_t);
+                            hx_t ^= sea_hash_entity(t0[j], c) & live_t;
+                        }
+                        if (CKV) {
+                            if (FINV) bad |= f32x3_bits_nonfinite(vl[0][j], vl[1][j], vl[2][j]) & uint32_t(live_v);
+                            const uint64_t lane_v = (Z || vz_zero) ? kSeaTailZero : sea_diffuse(kSeaB ^ uint64_t(vl[2][j]));
+                            uint64_t c = sea_hash_12_lane(uint64_t(vl[0][j]) | (uint64_t(vl[1][j]) << 32), lane_v);
+                            hx_v ^= sea_hash_entity(t0[j], c) & live_v;
+                        }
                     }
-                    if (CKV) {
-                        if (FINV) bad |= (f32_bits_nonfinite(vl[0][j]) | f32_bits_nonfinite(vl[1][j]) | f32_bits_nonfinite(vl[2][j])) & uint32_t(live_v);
-                        const uint64_t lane_v = vz_zero ? kSeaTailZero : sea_diffuse(kSeaB ^ uint64_t(vl[2][j]));
-                        uint64_t c = sea_hash_12_lane(uint64_t(vl[0][j]) | (uint64_t(vl[1][j]) << 32), lane_v);
-                        hx_v ^= sea_hash_entity(t0[j], c) & live_v;
-                    }
-                }
-                const uint32_t n_alive = __popc(alive & 0x01010101u);
+                };
+                if ((tz_zero || !CKT) && (vz_zero || !CKV)) hash_rows(BoolConst<true>{});
+                else hash_rows(BoolConst<false>{});
+                const uint32_t n_alive = __popc(alive & 0x01010101u);  // budget: save_fold
                 // warp-level fold (REDUX) now, shared-memory atomics at the NEXT save (or after the op
                 // loop): the REDUX latency is covered by the following ADVANCE instead of stalling lane 0
                 flush_pending();
@@ -812,15 +829,15 @@ __global__ void __launch_bounds__(256, 3) k_particles_program(const __grid_const
                 pend[5] = (FINT || FINV) ? __reduce_or_sync(full, bad) : 0u;
                 pend_row = p.ops[i].save_index * kAccStride;
                 pend_valid = true;
-                if (store && STAMPS) store_active(img, p.ops[i].call_count, held);
-            } else {  // OP_LOAD
+                if (store && STAMPS) store_active(img, p.ops[i].call_count, held);  // budget: save_store
+            } else {  // OP_LOAD  budget: load
                 load_active(p.arena + (size_t(p.ops[i].image_off256) << 8), p.ops[i].n_rows, p.ops[i].call_count);
             }
         }
-        flush_pending();
-        if (p.flags & PF_WRITE_LIVE_ACTIVE) store_active(p.arena, 0u, claim_stamps(0u, p.stamp_base + p.n_ops));
+        flush_pending();  // budget: save_fold
+        if (p.flags & PF_WRITE_LIVE_ACTIVE) store_active(p.arena, 0u, claim_stamps(0u, p.stamp_base + p.n_ops));  // budget: save_store
 
-        // ------------------------------ passive planes ------------------------------
+        // ------------------------------ passive planes ------------------------------  budget: tile_loop
         if (use_tma) {
             if (tid == 0 && !passive_early) issue_passive_stores();
         } else {
@@ -874,7 +891,7 @@ __global__ void __launch_bounds__(256, 3) k_particles_program(const __grid_const
             tile += gridDim.x;
         }
     }
-    if (use_tma && tid == 0) tma_wait_all();  // every bulk store has landed before the results are published
+    if (use_tma && tid == 0) tma_wait_all();  // every bulk store has landed before the results are published  budget: epilogue
 
     // ---- block partials -> global accumulators -> (last block) host-visible results ----
     __syncthreads();

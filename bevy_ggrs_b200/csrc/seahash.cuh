@@ -29,14 +29,40 @@ constexpr uint64_t kSeaC = 0x6fe2e5aaf078ebc9ULL;
 constexpr uint64_t kSeaD = 0x14f994a4c5259381ULL;
 constexpr uint64_t kSeaP = 0x6eed0e9da4d94a4fULL;
 
+// x * P (mod 2^64).  The device form is three instructions of the integer multiply-add pipe: the low product, then the
+// two cross products chained onto its high word as the addend.  Written as a u64 multiply, ptxas emits the low
+// product and the two cross products as three independent multiplies and a fourth instruction to add their high words.
+#if defined(__CUDA_ARCH__)
+__device__ __forceinline__ uint64_t sea_mul_p(uint64_t x) {
+    uint64_t r;
+    asm("{\n\t.reg .u32 l, h, wl, wh;\n\t"
+        "mov.b64 {l, h}, %1;\n\t"
+        "mul.wide.u32 %0, l, %2;\n\t"
+        "mov.b64 {wl, wh}, %0;\n\t"
+        "mad.lo.u32 wh, h, %2, wh;\n\t"
+        "mad.lo.u32 wh, l, %3, wh;\n\t"
+        "mov.b64 %0, {wl, wh};\n\t}"
+        : "=l"(r) : "l"(x), "n"(uint32_t(kSeaP)), "n"(uint32_t(kSeaP >> 32)));
+    return r;
+}
+#else
+inline constexpr uint64_t sea_mul_p(uint64_t x) { return x * kSeaP; }
+#endif
+
 // x *= P; x ^= (x >> 32) >> (x >> 60); x *= P
 // (x >> 32) >> (x >> 60) only involves the high word: hi >> (hi >> 28), a 32-bit value.
 BGR_HD uint64_t sea_diffuse(uint64_t x) {
+    x = sea_mul_p(x);
+    uint32_t hi = uint32_t(x >> 32);
+    x ^= uint64_t(hi >> (hi >> 28));
+    return sea_mul_p(x);
+}
+// the same in a constant expression (the device form above is inline PTX)
+BGR_HD uint64_t sea_diffuse_const(uint64_t x) {
     x *= kSeaP;
     uint32_t hi = uint32_t(x >> 32);
     x ^= uint64_t(hi >> (hi >> 28));
-    x *= kSeaP;
-    return x;
+    return x * kSeaP;
 }
 
 // seahash of exactly 8 bytes (one LE word)
@@ -52,7 +78,7 @@ BGR_HD uint64_t sea_hash_12(uint64_t w0, uint32_t tail) {
     return sea_diffuse(a ^ kSeaC ^ kSeaD ^ t ^ 12ULL);
 }
 // the tail lane when the last field is +0.0f (a 2-D game's z): a compile-time constant
-constexpr uint64_t kSeaTailZero = sea_diffuse(kSeaB);
+constexpr uint64_t kSeaTailZero = sea_diffuse_const(kSeaB);
 // same hash with the tail lane supplied by the caller (kSeaTailZero when the caller knows tail == 0)
 BGR_HD uint64_t sea_hash_12_lane(uint64_t w0, uint64_t tail_lane) {
     uint64_t t = sea_diffuse(kSeaA ^ w0);
