@@ -698,7 +698,7 @@ __global__ void __launch_bounds__(256, 3) k_particles_program(const __grid_const
         const bool passive_early = (p.flags & PF_PASSIVE_EARLY) != 0;
         if (use_tma && tid == 0 && passive_early) issue_passive_stores();
 
-        uint32_t pend[6] = {0, 0, 0, 0, 0, 0};
+        uint32_t pend[5] = {0, 0, 0, 0, 0};
         uint32_t pend_row = 0;
         bool pend_valid = false;
         auto flush_pending = [&]() {
@@ -706,8 +706,8 @@ __global__ void __launch_bounds__(256, 3) k_particles_program(const __grid_const
                 unsigned int* a = &s_acc[pend_row * 2];
                 if (CKT) { atomicXor(&a[2 * p.ck_t_slot], pend[0]); atomicXor(&a[2 * p.ck_t_slot + 1], pend[1]); }
                 if (CKV) { atomicXor(&a[2 * p.ck_v_slot], pend[2]); atomicXor(&a[2 * p.ck_v_slot + 1], pend[3]); }
-                atomicAdd(&a[12], pend[4]);
-                if (pend[5]) atomicOr(&a[14], 1u);
+                atomicAdd(&a[12], pend[4] & 0xFFFFu);
+                if (pend[4] >> 16) atomicOr(&a[14], 1u);
             }
             pend_valid = false;
         };
@@ -717,15 +717,18 @@ __global__ void __launch_bounds__(256, 3) k_particles_program(const __grid_const
             if (kind == OP_ADVANCE) {  // budget: advance
                 const float dt = __uint_as_float(p.ops[i].dt_bits);
                 const uint32_t alive_before = alive;
+                // bits, not values: -0.0 -> +0.0 and a changed NaN payload are changes.  chg[q] ORs the changed bits of
+                // plane q over the thread's rows (one LOP3 per row and plane); each plane is tested against zero once per
+                // Advance, not once per row.
+                uint32_t chg[8] = {0, 0, 0, 0, 0, 0, 0, 0};
 #pragma unroll
                 for (int j = 0; j < VEC; ++j) {
-                    // bits, not values: -0.0 -> +0.0 and a changed NaN payload are changes
                     const uint32_t o0 = tr[0][j], o1 = tr[1][j], o2 = tr[2][j], o3 = vl[0][j], o4 = vl[1][j], o5 = vl[2][j];
                     const uint32_t o6 = tl[0][j], o7 = tl[1][j];
                     auto note_changes = [&]() {
-                        dirty |= (tr[0][j] != o0 ? 1u : 0u) | (tr[1][j] != o1 ? 2u : 0u) | (tr[2][j] != o2 ? 4u : 0u) |
-                                 (vl[0][j] != o3 ? 8u : 0u) | (vl[1][j] != o4 ? 16u : 0u) | (vl[2][j] != o5 ? 32u : 0u) |
-                                 (tl[0][j] != o6 ? 64u : 0u) | (tl[1][j] != o7 ? 128u : 0u);
+                        chg[0] |= tr[0][j] ^ o0; chg[1] |= tr[1][j] ^ o1; chg[2] |= tr[2][j] ^ o2;
+                        chg[3] |= vl[0][j] ^ o3; chg[4] |= vl[1][j] ^ o4; chg[5] |= vl[2][j] ^ o5;
+                        chg[6] |= tl[0][j] ^ o6; chg[7] |= tl[1][j] ^ o7;
                     };
                     if (OPT) {
                         // the queries only match entities that have the components (and exist)
@@ -752,7 +755,11 @@ __global__ void __launch_bounds__(256, 3) k_particles_program(const __grid_const
                     alive &= ((lo | hi) == 0u) ? ~(0xFFu << (8 * j)) : 0xFFFFFFFFu;
                     if (STAMPS) note_changes();
                 }
-                if (STAMPS && alive != alive_before) dirty |= kAlivePlaneBit;
+                if (STAMPS) {
+#pragma unroll
+                    for (int q = 0; q < 8; ++q) dirty |= chg[q] != 0u ? 1u << q : 0u;
+                    if (alive != alive_before) dirty |= kAlivePlaneBit;
+                }
                 if (p.ops[i].flags & OPF_SPAWN) {
                     // spawn_particles (particles.rs:258-270): Commands are applied after the schedule, so the
                     // newborn rows appear now, un-updated: Transform::default(), Velocity(vx, vy, 0), Ttl(ttl)
@@ -825,8 +832,9 @@ __global__ void __launch_bounds__(256, 3) k_particles_program(const __grid_const
                 const unsigned full = 0xffffffffu;
                 if (CKT) { pend[0] = __reduce_xor_sync(full, uint32_t(hx_t)); pend[1] = __reduce_xor_sync(full, uint32_t(hx_t >> 32)); }
                 if (CKV) { pend[2] = __reduce_xor_sync(full, uint32_t(hx_v)); pend[3] = __reduce_xor_sync(full, uint32_t(hx_v >> 32)); }
-                pend[4] = __reduce_add_sync(full, n_alive);
-                pend[5] = (FINT || FINV) ? __reduce_or_sync(full, bad) : 0u;
+                // one REDUX for two counts: live rows (at most 32 * VEC) in the low half, lanes that saw a non-finite
+                // value in the high half
+                pend[4] = __reduce_add_sync(full, n_alive | (bad << 16));
                 pend_row = p.ops[i].save_index * kAccStride;
                 pend_valid = true;
                 if (store && STAMPS) store_active(img, p.ops[i].call_count, held);  // budget: save_store
