@@ -67,6 +67,8 @@ BGR_KERNEL_PASSIVE_PLANES = 1 << 15
 BGR_KERNEL_STABLE_PLANES = 1 << 26
 # ... and the bundle launch held at least one Save: its target slot already held the content (bgr_held_saves)
 BGR_KERNEL_HELD_SAVES = 1 << 27
+# ... and the vector ran inside a world batch's launch (bgr_batch_handle_requests)
+BGR_KERNEL_BATCHED = 1 << 28
 # change feed
 BGR_MAX_FEEDS = 8
 BGR_MAX_FEED_FIELDS = 8
@@ -220,6 +222,11 @@ PROTOTYPES = {
     "bgr_fold_partials": (C.c_int, [C.POINTER(bgr_partial), C.POINTER(bgr_checksum)]),
     "bgr_collect_partials": (C.c_int, [C.c_void_p, C.c_void_p, C.c_uint32, u32p]),
     "bgr_fold_partials_n": (C.c_int, [C.c_void_p, C.c_uint32, C.c_void_p]),
+    "bgr_batch_create": (C.c_int, [C.POINTER(C.c_void_p), C.c_uint32, C.POINTER(C.c_void_p)]),
+    "bgr_batch_destroy": (None, [C.c_void_p]),
+    "bgr_batch_specialised": (C.c_int, [C.c_void_p, u32p]),
+    "bgr_batch_handle_requests": (C.c_int, [C.c_void_p, u32p, C.c_uint32, C.POINTER(bgr_session_info), C.POINTER(bgr_request),
+                                            u32p, C.POINTER(bgr_checksum), C.c_uint32, u32p, i32p]),
     "bgr_seahash": (C.c_uint64, [C.c_void_p, C.c_uint64]),
     "bgr_ggrs_time_delta_bits": (C.c_uint32, [C.c_uint32, C.c_int32]),
     "bgr_particle_rng_stream": (C.c_int, [C.c_uint64, C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p, C.c_float, C.c_float]),

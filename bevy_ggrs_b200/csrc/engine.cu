@@ -966,6 +966,45 @@ constexpr std::pair<const char*, uint32_t> kSystemIds[] = {
 };
 #undef BGR_SYS_ID
 
+// Why the generated kernel cannot take this registration, or nullptr when it can
+const char* jit_unsupported(const bgr_engine* e) {
+    if (e->words < 1 || e->words > 24) return "the row has to fit the register file (1..24 words)";
+    for (const HashSpec& h : e->hash_specs)  // whole-word byte ranges only (every POD of u32 / f32 / u64 fields)
+        if (((h.off | h.len) & 3u) != 0u || h.len < 4 || h.len > 64) return "a checksummed byte range is not 1..16 whole words";
+    return nullptr;
+}
+
+// The generated kernel of this registration with `item_rows`-row work items and `rows` rows per thread: its prelude is
+// compiled by NVRTC, or fetched from jit.hpp's per-prelude cache.  False (and the reason in *why) when it cannot be.
+bool jit_compile(const bgr_engine* e, int item_rows, int rows, JitKernel* out, std::string* why) {
+    const int threads = item_rows / rows;
+    std::string pre;
+    auto def = [&](const char* name, unsigned long long v) { pre += "#define " + std::string(name) + " " + std::to_string(v) + "\n"; };
+    for (const auto& id : kSystemIds) def(id.first, id.second);
+    def("BGR_TILE_ROWS", kTileRows);
+    def("BGR_JIT_WORDS", e->words); def("BGR_JIT_ROWS", rows); def("BGR_JIT_ITEM_ROWS", item_rows);
+    // resident blocks the register allocation has to allow: ~512 threads per SM for narrow rows, ~256 for wide ones
+    def("BGR_JIT_MINB", std::max(1, (e->words <= 8 ? 512 : 256) / threads));
+    def("BGR_JIT_NSYS", e->sys_specs.size()); def("BGR_JIT_NHASH", e->hash_specs.size());
+    auto u = [](uint32_t v) { return std::to_string(v) + "u"; };
+    pre += "#define BGR_JIT_SYS_LIST ";
+    for (const SysSpec& y : e->sys_specs)
+        pre += "{" + u(y.id) + "," + u(y.plane0) + "," + u(y.plane1) + "," + u(y.need) + "," + u(y.param) + "}, ";
+    pre += "{0u,0u,0u,0u,0u}\n#define BGR_JIT_HASH_LIST ";
+    for (const HashSpec& h : e->hash_specs)
+        pre += "{" + u(h.first_plane) + "," + u(h.off) + "," + u(h.len) + "," + u(h.finite) + "," + u(h.slot) + "," + u(h.absent) + "}, ";
+    pre += "{0u,0u,0u,0u,0u,0u}\n";
+    const bool ok = jit_generic_program(pre, threads, reinterpret_cast<const void*>(&bgr_abi_version), out, why);
+    out->item_rows = item_rows;
+    return ok;
+}
+
+// rows per thread of the whole-tile instance (BGR_TUNE_JIT_ROWS), and the work item BGR_TUNE_JIT_ITEM forces (0: none)
+int jit_rows(const bgr_engine* e) { return e->tune_jit_rows == 1 || e->tune_jit_rows == 2 ? e->tune_jit_rows : 4; }
+int jit_forced_item(const bgr_engine* e) {
+    return e->tune_jit_item == 512 || e->tune_jit_item == 256 || e->tune_jit_item == 128 ? e->tune_jit_item : 0;
+}
+
 // NVRTC specialisation of the generic program for this registration (jit.hpp, generic_program_jit.cuh); called by bgr_build
 void jit_specialise(bgr_engine* e) {
     e->jit = JitKernel{};
@@ -973,35 +1012,14 @@ void jit_specialise(bgr_engine* e) {
     if (!e->generic_ok || !e->tune_generic || e->tune_jit == 0 || (e->cfg.flags & BGR_CFG_FORCE_STEPWISE)) return;
     if (e->bundle_particles && e->tune_bundle) return;  // the bundle has its own kernel
     if (e->tune_jit == 1 && e->cfg.max_entities < 16384) return;  // small worlds: a tick is launch latency, not worth a compile
-    if (e->words < 1 || e->words > 24) return;  // the row has to fit the register file
-    for (const HashSpec& h : e->hash_specs)     // whole-word byte ranges only (every POD of u32 / f32 / u64 fields)
-        if (((h.off | h.len) & 3u) != 0u || h.len < 4 || h.len > 64) return;
-    const int rows = e->tune_jit_rows == 1 || e->tune_jit_rows == 2 ? e->tune_jit_rows : 4;
+    if (jit_unsupported(e)) return;
     auto compile = [&](int item_rows, int rows, JitKernel* out) {
-        const int threads = item_rows / rows;
-        std::string pre;
-        auto def = [&](const char* name, unsigned long long v) { pre += "#define " + std::string(name) + " " + std::to_string(v) + "\n"; };
-        for (const auto& id : kSystemIds) def(id.first, id.second);
-        def("BGR_TILE_ROWS", kTileRows);
-        def("BGR_JIT_WORDS", e->words); def("BGR_JIT_ROWS", rows); def("BGR_JIT_ITEM_ROWS", item_rows);
-        // resident blocks the register allocation has to allow: ~512 threads per SM for narrow rows, ~256 for wide ones
-        def("BGR_JIT_MINB", std::max(1, (e->words <= 8 ? 512 : 256) / threads));
-        def("BGR_JIT_NSYS", e->sys_specs.size()); def("BGR_JIT_NHASH", e->hash_specs.size());
-        auto u = [](uint32_t v) { return std::to_string(v) + "u"; };
-        pre += "#define BGR_JIT_SYS_LIST ";
-        for (const SysSpec& y : e->sys_specs)
-            pre += "{" + u(y.id) + "," + u(y.plane0) + "," + u(y.plane1) + "," + u(y.need) + "," + u(y.param) + "}, ";
-        pre += "{0u,0u,0u,0u,0u}\n#define BGR_JIT_HASH_LIST ";
-        for (const HashSpec& h : e->hash_specs)
-            pre += "{" + u(h.first_plane) + "," + u(h.off) + "," + u(h.len) + "," + u(h.finite) + "," + u(h.slot) + "," + u(h.absent) + "}, ";
-        pre += "{0u,0u,0u,0u,0u,0u}\n";
         std::string why;
-        if (!jit_generic_program(pre, threads, reinterpret_cast<const void*>(&bgr_abi_version), out, &why) && std::getenv("BGR_JIT_VERBOSE"))
+        if (!jit_compile(e, item_rows, rows, out, &why) && std::getenv("BGR_JIT_VERBOSE"))
             std::fprintf(stderr, "[bevy_ggrs_b200] generic program not specialised, the interpreter kernel runs: %s\n", why.c_str());
-        out->item_rows = item_rows;
     };
-    const int forced = e->tune_jit_item == 512 || e->tune_jit_item == 256 || e->tune_jit_item == 128 ? e->tune_jit_item : 0;
-    compile(forced ? forced : int(kTileRows), std::min(rows, (forced ? forced : int(kTileRows)) / 32), &e->jit);  // a block is at least one warp
+    const int forced = jit_forced_item(e);
+    compile(forced ? forced : int(kTileRows), std::min(jit_rows(e), (forced ? forced : int(kTileRows)) / 32), &e->jit);  // a block is at least one warp
     // worlds of few tiles per SM: quarter-tile items, two rows per thread
     if (!forced && e->jit.fn) compile(128, 2, &e->jit_small);
 }
@@ -1009,24 +1027,43 @@ void jit_specialise(bgr_engine* e) {
 // ---------------------------------------------------------------------------------------------
 // launch: generic one-launch program (any schema, compiled systems; generic_program.cuh)
 // ---------------------------------------------------------------------------------------------
+// The launch record of one request vector on the generic program (ops and registration aside): what run_generic puts
+// into its parameter block and a world batch into its per-world record.  Sets no batch fields.
+JitWorld launch_record(const bgr_engine* e, const Program& pg, uint32_t buf) {
+    JitWorld w;
+    std::memset(&w, 0, sizeof w);
+    w.arena = e->arena.ptr();
+    w.order_base = e->cfg.order_base;
+    w.accum = e->d_accum_set[0];
+    w.ticket = e->d_ticket_set[0];
+    w.out = pg.internal ? e->internal_out.get() : e->d_out[buf];
+    w.seq = e->seq;
+    w.n_ops = pg.n_ops; w.n_saves = pg.n_saves;
+    w.n_tiles = std::max(1u, e->tiles_for(pg.max_rows));
+    w.live_rows = pg.live_rows;
+    if (!pg.first_is_load) w.flags |= PF_READ_LIVE;
+    if ((pg.has_load || pg.has_advance) && !pg.defer_live) w.flags |= PF_WRITE_LIVE_ACTIVE;
+    return w;
+}
+
 int run_generic(bgr_engine* e, const Program& pg, uint32_t buf) {
     const bool prev_chain = e->tiledep_chain;  // the last operation on the stream was a signalling launch of the generated kernel
     e->tiledep_chain = false;
+    const JitWorld w = launch_record(e, pg, buf);
     GenericParams gp;
     std::memset(&gp, 0, sizeof gp);
-    gp.arena = e->arena.ptr();
-    gp.order_base = e->cfg.order_base;
-    gp.accum = e->d_accum_set[0];
-    gp.ticket = e->d_ticket_set[0];
-    gp.out = pg.internal ? e->internal_out.get() : e->d_out[buf];
-    gp.seq = e->seq;
+    gp.arena = w.arena;
+    gp.order_base = w.order_base;
+    gp.accum = w.accum;
+    gp.ticket = w.ticket;
+    gp.out = w.out;
+    gp.seq = w.seq;
     if (e->trace.get() && !pg.internal && e->seq - e->trace_first_seq < e->trace_cap) gp.trace = e->trace.get() + (e->seq - e->trace_first_seq) * 4;
     gp.words = e->words; gp.tile_bytes = e->tile_bytes;
-    gp.n_ops = pg.n_ops; gp.n_saves = pg.n_saves;
-    gp.n_tiles = std::max(1u, e->tiles_for(pg.max_rows));
-    gp.live_rows = pg.live_rows;
-    if (!pg.first_is_load) gp.flags |= PF_READ_LIVE;
-    if ((pg.has_load || pg.has_advance) && !pg.defer_live) gp.flags |= PF_WRITE_LIVE_ACTIVE;
+    gp.n_ops = w.n_ops; gp.n_saves = w.n_saves;
+    gp.n_tiles = w.n_tiles;
+    gp.live_rows = w.live_rows;
+    gp.flags = w.flags;
     gp.n_hash = uint32_t(e->hash_specs.size());
     gp.n_sys = uint32_t(e->sys_specs.size());  // <= kMaxGenericSys: generic_ok
     std::copy(e->hash_specs.begin(), e->hash_specs.end(), gp.hash);
@@ -1287,21 +1324,74 @@ int grow_to(bgr_engine* e, uint64_t rows) {
     return BGR_OK;
 }
 
-int submit(bgr_engine* e, const bgr_session_info* sess, const bgr_request* reqs, uint32_t n) {
-    NvtxRange span("HandleRequests");
+// A request vector compiled against a copy of its engine's HostState: what submit() executes and commits
+struct Prepared {
+    HostState s;
+    Program pg;
+    DeferredLive next;        // the vector's own deferred live image (plan)
+    uint64_t t_begin = 0, t_compiled = 0;
+};
+
+// submit(), first half: validates the vector and compiles it against a copy of the HostState.  Executes and changes
+// nothing, so a batch prepares every world before any of them runs.
+int prepare(bgr_engine* e, const bgr_session_info* sess, const bgr_request* reqs, uint32_t n, Prepared& p) {
     if (!e) return fail(BGR_ERR_INVALID_ARGUMENT, "null engine");
     if (!e->built) return fail(BGR_ERR_STATE, "bgr_build has not been called");
     if (e->pending.size() >= size_t(bgr_engine::kBufs)) return fail(BGR_ERR_STATE, "too many un-collected submits");
     if (n && !reqs) return fail(BGR_ERR_INVALID_ARGUMENT, "null requests");
-    const uint64_t t_begin = host_ns();
-    HostState s = e->st;
-    Program pg;
-    int rc = compile_requests(e, s, sess, reqs, n, pg);
+    p.t_begin = host_ns();
+    p.s = e->st;
+    p.pg.~Program();
+    new (&p.pg) Program;
+    p.next = DeferredLive{};
+    return compile_requests(e, p.s, sess, reqs, n, p.pg);
+}
+
+// ... the vector takes its sequence number, consumes the previous vector's deferred live image (which may launch its
+// materialisation) and plans its own
+int plan(bgr_engine* e, Prepared& p) {
+    e->seq += 1;
+    e->ticked = true;
+    const bool bundle = use_bundle(e), fused = bundle || use_generic(e);  // one launch for the whole request vector
+    const int rc = fused ? consume_deferred(e, p.pg) : materialize_live(e);
+    if (rc != BGR_OK) return rc;
+    if (bundle) derive_content_ids(e, p.s, p.pg);
+    if (fused && e->tune_defer_live && !e->live_touched) p.next = plan_deferral(p.pg);
+    return BGR_OK;
+}
+
+// submit(), second half, behind the launch into result buffer `buf`: the last_kernel bits, the vector's pending
+// results, the state commit
+int commit(bgr_engine* e, const Prepared& p, uint32_t buf) {
+    const Program& pg = p.pg;
+    if (pg.defer_live) e->last_kernel |= BGR_KERNEL_DEFERRED_LIVE;
+    if (pg.from_deferred) e->last_kernel |= BGR_KERNEL_FROM_DEFERRED;
+    // an event between two launches would serialise them; with host polling it is only a fallback, taken lazily
+    if (!(e->tune_tiledep && e->tune_poll)) CUDA_TRY(cudaEventRecord(e->ev[buf].get(), e->stream));
+    e->last_fused = use_bundle(e) || use_generic(e);
+    e->st = p.s;
+    e->deferred = p.next;
+    e->live_touched = false;
+    Pending pd;
+    pd.buf = buf; pd.n_saves = pg.n_saves; pd.seq = e->seq; pd.gseq = e->group ? e->gseq : 0;
+    std::memcpy(pd.frames, pg.save_frames, sizeof(int32_t) * pg.n_saves);
+    std::memcpy(pd.totals, pg.save_totals, sizeof(uint32_t) * pg.n_saves);
+    e->pending.push_back(pd);
+    e->next_buf = (buf + 1) % bgr_engine::kBufs;
+    e->prof[0] += 1; e->prof[1] += p.t_compiled - p.t_begin; e->prof[2] += host_ns() - p.t_compiled;
+    return BGR_OK;
+}
+
+int submit(bgr_engine* e, const bgr_session_info* sess, const bgr_request* reqs, uint32_t n) {
+    NvtxRange span("HandleRequests");
+    Prepared p;
+    int rc = prepare(e, sess, reqs, n, p);
     if (rc != BGR_OK) return rc;  // nothing executed, nothing committed
+    const Program& pg = p.pg;
     // the program does not depend on the capacity: growing behind the compile leaves it (and its ParticleRng draws) valid
     if (pg.rows_needed) rc = grow_to(e, pg.rows_needed);
     if (rc != BGR_OK) return rc;
-    const uint64_t t_compiled = host_ns();
+    p.t_compiled = host_ns();
     uint32_t buf = e->next_buf;
     if (e->group) {
         // the buffer of this request vector was last used kBufs vectors ago: every peer must have folded that one
@@ -1312,34 +1402,11 @@ int submit(bgr_engine* e, const bgr_session_info* sess, const bgr_request* reqs,
         e->group->publish_meta(e->gseq, pg.n_saves, e->n_ck, pg.save_frames, pg.save_totals);
     }
     if (!pg.spawn_vals.empty()) std::memcpy(e->spawn[buf].get(), pg.spawn_vals.data(), pg.spawn_vals.size() * sizeof(float2));
-    e->seq += 1;
-    e->ticked = true;
-    const bool bundle = use_bundle(e);
-    const bool generic = use_generic(e);
-    const bool fused = bundle || generic;   // one launch for the whole request vector
-    rc = fused ? consume_deferred(e, pg) : materialize_live(e);
+    rc = plan(e, p);
     if (rc != BGR_OK) return rc;
-    if (bundle) derive_content_ids(e, s, pg);
-    DeferredLive next;
-    if (fused && e->tune_defer_live && !e->live_touched) next = plan_deferral(pg);
-    rc = bundle ? run_fused(e, pg, buf) : generic ? run_generic(e, pg, buf) : run_stepwise(e, pg, buf);
+    rc = use_bundle(e) ? run_fused(e, pg, buf) : use_generic(e) ? run_generic(e, pg, buf) : run_stepwise(e, pg, buf);
     if (rc != BGR_OK) return rc;
-    if (pg.defer_live) e->last_kernel |= BGR_KERNEL_DEFERRED_LIVE;
-    if (pg.from_deferred) e->last_kernel |= BGR_KERNEL_FROM_DEFERRED;
-    // an event between two launches would serialise them; with host polling it is only a fallback, taken lazily
-    if (!(e->tune_tiledep && e->tune_poll)) CUDA_TRY(cudaEventRecord(e->ev[buf].get(), e->stream));
-    e->last_fused = fused;
-    e->st = s;
-    e->deferred = next;
-    e->live_touched = false;
-    Pending pd;
-    pd.buf = buf; pd.n_saves = pg.n_saves; pd.seq = e->seq; pd.gseq = e->group ? e->gseq : 0;
-    std::memcpy(pd.frames, pg.save_frames, sizeof(int32_t) * pg.n_saves);
-    std::memcpy(pd.totals, pg.save_totals, sizeof(uint32_t) * pg.n_saves);
-    e->pending.push_back(pd);
-    e->next_buf = (buf + 1) % bgr_engine::kBufs;
-    e->prof[0] += 1; e->prof[1] += t_compiled - t_begin; e->prof[2] += host_ns() - t_compiled;
-    return BGR_OK;
+    return commit(e, p, buf);
 }
 
 void fold(const bgr_partial& p, bgr_checksum* out) {
@@ -3132,6 +3199,194 @@ BGR_API int bgr_handle_requests(bgr_engine* e, const bgr_session_info* session, 
     int rc = submit(e, session, requests, n_requests);
     if (rc != BGR_OK) return rc;
     return collect(e, checksums_out, checksums_cap, n_checksums_out);
+}
+
+// ---- world batches: the request vectors of many engines with one registration in one launch ----
+struct bgr_batch {
+    std::vector<bgr_engine*> engines;
+    cudaStream_t stream = nullptr;       // every member's
+    JitKernel k;                         // k.batch_fn == nullptr: a call runs its worlds one after another
+    std::vector<Prepared> prep;          // per member, reused by every call
+    std::vector<uint32_t> buf, listed;   // per member: its result buffer in this call, the last call that listed it
+    uint32_t calls = 0;
+    MappedHostBuffer<uint8_t> h_stage;   // a call's JitWorld records, then the listed worlds' ops
+    DeviceBuffer<uint8_t> d_stage;
+};
+
+static bool same_specs(const bgr_engine* a, const bgr_engine* b) {
+    return a->words == b->words && a->sys_specs.size() == b->sys_specs.size() && a->hash_specs.size() == b->hash_specs.size() &&
+           std::equal(a->sys_specs.begin(), a->sys_specs.end(), b->sys_specs.begin(),
+                      [](const SysSpec& x, const SysSpec& y) { return std::memcmp(&x, &y, sizeof x) == 0; }) &&
+           std::equal(a->hash_specs.begin(), a->hash_specs.end(), b->hash_specs.begin(),
+                      [](const HashSpec& x, const HashSpec& y) { return std::memcmp(&x, &y, sizeof x) == 0; });
+}
+
+// The batch's instance of the generated kernel: 128-row work items of two rows per thread unless BGR_TUNE_JIT_ITEM
+// forces a size, whatever the members' sizes.  False (and the reason in *why) when the calls run sequentially.
+static bool batch_specialise(bgr_batch* b, std::string* why) {
+    const bgr_engine* e = b->engines[0];
+    if (e->tune_jit == 0) { *why = "BGR_TUNE_JIT=0"; return false; }
+    if (const char* w = jit_unsupported(e)) { *why = w; return false; }
+    const int forced = jit_forced_item(e);
+    const int item_rows = forced ? forced : 128, rows = forced ? std::min(jit_rows(e), forced / 32) : 2;
+    if (!jit_compile(e, item_rows, rows, &b->k, why)) { b->k = JitKernel{}; return false; }
+    if (!b->k.batch_fn) { *why = "the compiled module has no k_generic_jit_batch"; b->k = JitKernel{}; return false; }
+    return true;
+}
+
+BGR_API int bgr_batch_create(bgr_engine* const* engines, uint32_t n, bgr_batch** out) {
+    if (!engines || n == 0 || !out) return fail(BGR_ERR_INVALID_ARGUMENT, "a batch needs at least one engine and an out pointer");
+    *out = nullptr;
+    for (uint32_t i = 0; i < n; ++i) {
+        const bgr_engine* e = engines[i];
+        const std::string who = "engine " + std::to_string(i) + ": ";
+        if (!e) return fail(BGR_ERR_INVALID_ARGUMENT, who + "null engine");
+        if (!e->built) return fail(BGR_ERR_INVALID_ARGUMENT, who + "bgr_build has not been called");
+        for (uint32_t j = 0; j < i; ++j)
+            if (engines[j] == e) return fail(BGR_ERR_INVALID_ARGUMENT, who + "the same engine as engine " + std::to_string(j));
+        if (e->cfg.device != engines[0]->cfg.device) return fail(BGR_ERR_INVALID_ARGUMENT, who + "on another device than engine 0");
+        if (!same_specs(e, engines[0]))
+            return fail(BGR_ERR_INVALID_ARGUMENT, who + "its registration (columns, systems, checksums) differs from engine 0's");
+        if (!e->cfg.stream || e->cfg.stream != engines[0]->cfg.stream)
+            return fail(BGR_ERR_INVALID_ARGUMENT, who + "every engine of a batch must be created with the same non-null bgr_config.stream");
+        if ((e->cfg.flags & BGR_CFG_SHARDED) || e->group)
+            return fail(BGR_ERR_UNSUPPORTED, who + "sharded engines (BGR_CFG_SHARDED, shard groups) cannot be batched");
+        if (!use_generic(e))
+            return fail(BGR_ERR_UNSUPPORTED, who + "only engines that run the generic one-launch program can be batched (not the particles "
+                                                   "bundle, BGR_CFG_FORCE_STEPWISE or a spawn system)");
+    }
+    CUDA_TRY(cudaSetDevice(engines[0]->cfg.device));
+    bgr_batch* b = new bgr_batch();
+    b->engines.assign(engines, engines + n);
+    b->stream = engines[0]->stream;
+    b->prep.resize(n);
+    b->buf.assign(n, 0);
+    b->listed.assign(n, 0);
+    std::string why;
+    if (batch_specialise(b, &why)) {
+        const size_t bytes = size_t(n) * (sizeof(JitWorld) + sizeof(Op) * kMaxOps);
+        cudaError_t ce = b->h_stage.ensure(bytes);
+        if (ce == cudaSuccess) ce = b->d_stage.ensure(bytes);
+        if (ce != cudaSuccess) { delete b; return fail(BGR_ERR_CUDA, std::string("batch staging: ") + cudaGetErrorString(ce)); }
+    } else if (std::getenv("BGR_JIT_VERBOSE")) {
+        std::fprintf(stderr, "[bevy_ggrs_b200] world batch not specialised, its worlds run one after another: %s\n", why.c_str());
+    }
+    *out = b;
+    return BGR_OK;
+}
+
+BGR_API void bgr_batch_destroy(bgr_batch* b) {
+    if (!b) return;
+    cudaStreamSynchronize(b->stream);
+    delete b;
+}
+
+BGR_API int bgr_batch_specialised(bgr_batch* b, uint32_t* specialised_out) {
+    if (!b || !specialised_out) return fail(BGR_ERR_INVALID_ARGUMENT, "null argument");
+    *specialised_out = b->k.batch_fn ? 1u : 0u;
+    return BGR_OK;
+}
+
+BGR_API int bgr_batch_handle_requests(bgr_batch* b, const uint32_t* worlds, uint32_t n_worlds, const bgr_session_info* sessions,
+                                      const bgr_request* requests, const uint32_t* n_requests, bgr_checksum* checksums_out,
+                                      uint32_t checksums_cap, uint32_t* n_checksums_out, int32_t* status_out) {
+    if (!b) return fail(BGR_ERR_INVALID_ARGUMENT, "null batch");
+    if (n_worlds && (!worlds || !n_requests || !n_checksums_out || !status_out)) return fail(BGR_ERR_INVALID_ARGUMENT, "null argument");
+    NvtxRange span("HandleRequests");
+    b->calls += 1;
+    for (uint32_t i = 0; i < n_worlds; ++i) { status_out[i] = BGR_OK; n_checksums_out[i] = 0; }
+    auto world_fail = [&](uint32_t i, int status) {
+        status_out[i] = status;
+        g_err = "world " + std::to_string(worlds[i]) + ": " + g_err;
+        return status;
+    };
+    auto session = [&](uint32_t i) { return sessions ? &sessions[i] : nullptr; };
+    // every world is validated and compiled before any executes
+    std::vector<size_t> req_off(n_worlds + 1, 0);
+    for (uint32_t i = 0; i < n_worlds; ++i) {
+        const uint32_t w = worlds[i];
+        if (w >= b->engines.size())
+            return world_fail(i, fail(BGR_ERR_INVALID_ARGUMENT, "no such world in a batch of " + std::to_string(b->engines.size())));
+        if (b->listed[w] == b->calls) return world_fail(i, fail(BGR_ERR_INVALID_ARGUMENT, "listed twice in one call"));
+        b->listed[w] = b->calls;
+        if (n_requests[i] > BGR_MAX_REQUESTS) return world_fail(i, fail(BGR_ERR_CAPACITY, "too many requests in one handle_requests call"));
+        bgr_engine* e = b->engines[w];
+        if (!e->pending.empty())
+            return world_fail(i, fail(BGR_ERR_STATE, "un-collected bgr_submit_requests pending: call bgr_collect first"));
+        req_off[i + 1] = req_off[i] + n_requests[i];
+        const int rc = prepare(e, session(i), requests ? requests + req_off[i] : nullptr, n_requests[i], b->prep[w]);
+        if (rc != BGR_OK) return world_fail(i, rc);
+    }
+    // results: each world's checksums behind the previous worlds', as far as checksums_cap reaches
+    int first = BGR_OK;
+    std::string first_err;
+    uint32_t out_off = 0;
+    auto collect_world = [&](uint32_t i, int rc, uint32_t n) {
+        n_checksums_out[i] = n;
+        out_off += std::min(n, checksums_cap - std::min(out_off, checksums_cap));
+        if (rc != BGR_OK) {
+            world_fail(i, rc);
+            if (first == BGR_OK) { first = rc; first_err = g_err; }
+        }
+    };
+    auto out_at = [&]() { return checksums_out && out_off < checksums_cap ? checksums_out + out_off : nullptr; };
+    auto cap_at = [&]() { return checksums_out && out_off < checksums_cap ? checksums_cap - out_off : 0u; };
+    if (!b->k.batch_fn) {  // the worlds' own submit path, in list order
+        for (uint32_t i = 0; i < n_worlds; ++i) {
+            uint32_t n = 0;
+            const int rc = bgr_handle_requests(b->engines[worlds[i]], session(i), requests ? requests + req_off[i] : nullptr, n_requests[i],
+                                               out_at(), cap_at(), &n);
+            collect_world(i, rc, n);
+        }
+        if (first != BGR_OK) g_err = first_err;
+        return first;
+    }
+    if (n_worlds == 0) return BGR_OK;
+    // one record per world and the worlds' ops in page-locked staging, one copy, one launch
+    uint8_t* h = b->h_stage.get();
+    JitWorld* recs = reinterpret_cast<JitWorld*>(h);
+    Op* ops = reinterpret_cast<Op*>(h + sizeof(JitWorld) * n_worlds);
+    const uint32_t subs = kTileRows / uint32_t(b->k.item_rows);
+    uint32_t items = 0, n_ops = 0;
+    for (uint32_t i = 0; i < n_worlds; ++i) {
+        const uint32_t w = worlds[i];
+        bgr_engine* e = b->engines[w];
+        Prepared& p = b->prep[w];
+        p.t_compiled = host_ns();
+        e->tiledep_chain = false;
+        b->buf[w] = e->next_buf;
+        const int rc = plan(e, p);  // a deferred live image this vector cannot start from is written here, before the launch
+        if (rc != BGR_OK) return world_fail(i, rc);
+        JitWorld r = launch_record(e, p.pg, b->buf[w]);
+        r.item0 = items;
+        r.ops_off = n_ops;
+        recs[i] = r;
+        std::memcpy(ops + n_ops, p.pg.ops, sizeof(Op) * p.pg.n_ops);
+        items += r.n_tiles * subs;
+        n_ops += p.pg.n_ops;
+    }
+    uint8_t* d = b->d_stage.get();
+    const JitWorld* d_recs = reinterpret_cast<const JitWorld*>(d);
+    const Op* d_ops = reinterpret_cast<const Op*>(d + sizeof(JitWorld) * n_worlds);
+    CUDA_TRY(cudaMemcpyAsync(d, h, sizeof(JitWorld) * n_worlds + sizeof(Op) * n_ops, cudaMemcpyHostToDevice, b->stream));
+    void* args[] = {&d_recs, &n_worlds, &d_ops};
+    CUDA_TRY(cudaLaunchKernel(b->k.batch_fn, dim3(items), dim3(b->k.threads), args, 0, b->stream));
+    CUDA_TRY(cudaGetLastError());
+    for (uint32_t i = 0; i < n_worlds; ++i) {
+        const uint32_t w = worlds[i];
+        bgr_engine* e = b->engines[w];
+        e->launches += 1;
+        e->last_kernel = BGR_KERNEL_GENERIC_NVRTC | (uint32_t(b->k.item_rows) << 16) | BGR_KERNEL_BATCHED;
+        const int rc = commit(e, b->prep[w], b->buf[w]);
+        if (rc != BGR_OK) return world_fail(i, rc);
+    }
+    for (uint32_t i = 0; i < n_worlds; ++i) {
+        uint32_t n = 0;
+        const int rc = collect(b->engines[worlds[i]], out_at(), cap_at(), &n);
+        collect_world(i, rc, n);
+    }
+    if (first != BGR_OK) g_err = first_err;
+    return first;
 }
 
 BGR_API int bgr_save_world(bgr_engine* e, bgr_checksum* checksum_out) {

@@ -56,6 +56,23 @@ struct GenericParams {
 };
 static_assert(sizeof(GenericParams) <= 4000, "kernel parameter block must fit 4 KB");
 
+// One request vector of one engine on the generated kernel, without its ops and registration: the per-world record of
+// a batched launch (k_generic_jit_batch, generic_program_jit.cuh), copied to the device with the worlds' ops behind the
+// records.  run_generic builds the same record for its own GenericParams.
+struct JitWorld {
+    uint8_t* arena;
+    unsigned long long order_base;
+    unsigned long long* accum;
+    unsigned int* ticket;
+    unsigned long long* out;
+    unsigned long long seq;
+    uint32_t n_ops, n_saves, n_tiles, live_rows, flags;
+    uint32_t item0;    // batched launch: the world's first block (sum of the item counts of the worlds before it)
+    uint32_t ops_off;  // batched launch: index of the world's first op in the launch's op array
+    uint32_t pad;
+};
+static_assert(sizeof(JitWorld) == 80, "JitWorld layout");
+
 // seahash of bytes [off, off+len) of one row's element whose words are `col[w * kTileRows]` (a column of the shared tile)
 // (__noinline__: inlined per checksummed column and per row the interpreter grew to 11k instructions — 176 KB of code,
 // more than the SM's instruction cache — and ran 2.7x slower per frame than the specialised bundle kernel)
@@ -114,7 +131,7 @@ __device__ __forceinline__ void hash_words_column(const uint32_t* col, const uin
     }
 }
 
-#ifndef __CUDACC_RTC__  // the run-time specialisation only needs the structs and helpers: its cubin holds k_generic_jit alone
+#ifndef __CUDACC_RTC__  // the run-time specialisation only needs the structs and helpers: its cubin holds its own entry points alone
 __global__ void __launch_bounds__(kGenericBlock) k_generic_program(const __grid_constant__ GenericParams p) {
     constexpr int kRows = kTileRows / kGenericBlock;  // rows of a tile per thread
     extern __shared__ __align__(128) uint8_t s_buf[];  // one tile

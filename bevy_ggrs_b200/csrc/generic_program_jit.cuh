@@ -91,6 +91,108 @@ __device__ __forceinline__ void jit_hash_columns(const JitRows& r, unsigned int*
     }
 }
 
+// One work item of a request vector: the rows' first read from `first_img`, the vector's ops (LOAD, ADVANCE, SAVE with its
+// hash into the save's shared accumulators `s_acc`) and the live store.  The one definition of what an op does on the
+// generated kernel: k_generic_jit and k_generic_jit_batch both run it.  `op_at(i)` is op i of the vector.
+template <class OpAt>
+__device__ __forceinline__ void jit_run_item(uint8_t* arena, unsigned long long order_base, uint32_t flags, uint32_t n_ops, OpAt op_at,
+                                             const uint8_t* first_img, uint32_t first_rows, uint32_t item, unsigned int* s_acc,
+                                             uint32_t tid, uint32_t lane) {
+    constexpr int B = kJitItemRows / kJitRows;  // threads per work item
+    constexpr uint32_t kTileBytes = kTileRows * (4u * kJitWords + 1u);
+    constexpr uint32_t kAliveOff = uint32_t(kJitWords) * kPlaneBytes;  // the mask bytes follow the word planes inside a tile
+    const uint32_t tile = item / uint32_t(kJitSubs), sub_row0 = (item % uint32_t(kJitSubs)) * uint32_t(kJitItemRows) + tid;  // first row of the thread inside the tile
+    const size_t tile_off = size_t(tile) * kTileBytes;
+    const unsigned long long row0 = order_base + size_t(tile) * kTileRows + sub_row0;
+
+    JitRows r;
+    auto load = [&](const uint8_t* img, uint32_t n_rows_src) {
+        const uint8_t* t = img + tile_off;
+#pragma unroll
+        for (int k = 0; k < kJitRows; ++k) {
+            const uint32_t row = sub_row0 + k * B;
+#pragma unroll
+            for (int j = 0; j < kJitWords; ++j) r.w[k][j] = __ldcg(reinterpret_cast<const uint32_t*>(t + size_t(j) * kPlaneBytes + size_t(row) * 4u));
+            const uint32_t mm = __ldcg(t + kAliveOff + row);  // .cg: L2 only — overlapping grids share an SM's L1 without a kernel boundary in between
+            r.m[k] = (tile * kTileRows + row < n_rows_src) ? mm : 0u;  // rows the image never contained come back dead
+        }
+    };
+    auto store = [&](uint8_t* img) {
+        uint8_t* t = img + tile_off;
+#pragma unroll
+        for (int k = 0; k < kJitRows; ++k) {
+            const uint32_t row = sub_row0 + k * B;
+#pragma unroll
+            for (int j = 0; j < kJitWords; ++j) *reinterpret_cast<uint32_t*>(t + size_t(j) * kPlaneBytes + size_t(row) * 4u) = r.w[k][j];
+            t[kAliveOff + row] = uint8_t(r.m[k]);
+        }
+    };
+    load(first_img, first_rows);
+#pragma unroll
+    for (int k = 0; k < kJitRows; ++k) r.t0[k] = sea_order_lane(row0 + uint32_t(k * B));
+
+    for (uint32_t i = (flags & PF_READ_LIVE) ? 0u : 1u; i < n_ops; ++i) {
+        const Op& op = op_at(i);
+        if (op.kind == OP_ADVANCE) {
+#pragma unroll
+            for (int k = 0; k < kJitRows; ++k) r.kill[k] = false;
+            jit_run_systems<0>(r, op, row0, B);
+#pragma unroll
+            for (int k = 0; k < kJitRows; ++k) r.m[k] = r.kill[k] ? 0u : r.m[k];  // despawn commands: after the last system
+        } else if (op.kind == OP_SAVE) {
+            if (!(op.flags & OPF_NO_STORE)) store(arena + (size_t(op.image_off256) << 8));
+            uint32_t n_alive = 0, bad = 0;
+#pragma unroll
+            for (int k = 0; k < kJitRows; ++k) n_alive += r.m[k] & 1u;
+            unsigned int* a = &s_acc[op.save_index * kAccStride * 2];
+            jit_hash_columns<0>(r, a, lane, bad);
+            const unsigned full = 0xffffffffu;
+            const uint32_t cnt = __reduce_add_sync(full, n_alive);
+            const uint32_t anybad = __reduce_or_sync(full, bad);
+            if (lane == 0) { atomicAdd(&a[12], cnt); if (anybad) atomicOr(&a[14], 1u); }
+        } else {  // OP_LOAD
+            load(arena + (size_t(op.image_off256) << 8), op.n_rows);
+        }
+    }
+    if (flags & PF_WRITE_LIVE_ACTIVE) store(arena);
+}
+
+// The end of a block: its shared accumulators folded into the vector's `accum`; the block that completes the vector's
+// `n_blocks`-th ticket then publishes the results as self-validating pairs plus the completion pair (k_particles_program's
+// protocol) and re-arms the ticket for the vector's next launch.
+__device__ __forceinline__ void jit_fold_publish(unsigned long long* accum, unsigned int* ticket, unsigned long long* out,
+                                                 unsigned long long seq, uint32_t n_saves, uint32_t n_blocks, const unsigned int* s_acc,
+                                                 unsigned int& s_last, unsigned long long* trace, uint32_t tid) {
+    constexpr int B = kJitItemRows / kJitRows;
+    __syncthreads();
+    for (uint32_t i = tid; i < n_saves * kAccStride; i += B) {
+        unsigned long long v = (unsigned long long)s_acc[2 * i] | ((unsigned long long)s_acc[2 * i + 1] << 32);
+        const uint32_t c = i % kAccStride;
+        if (v) {
+            if (c == 6) atomicAdd(&accum[i], v);
+            else if (c == 7) atomicOr(&accum[i], v);
+            else atomicXor(&accum[i], v);
+        }
+    }
+    __threadfence();
+    __syncthreads();
+    if (trace && tid == 0) atomicMax(&trace[1], globaltimer_ns());
+    if (tid == 0) s_last = (atomicAdd(ticket, 1u) == n_blocks - 1u);
+    __syncthreads();
+    if (s_last) {
+        __threadfence();
+        for (uint32_t i = tid; i < n_saves * kAccStride; i += B)
+            publish_pair(out, i, atomicExch(&accum[i], 0ULL), seq);
+        if (tid == 0) publish_pair(out, kSeqIndex, seq, seq);
+        __syncthreads();
+        if (tid == 0) {
+            ticket[0] = 0u;
+            ticket[1] = 0u;
+            if (trace) trace[2] = globaltimer_ns();
+        }
+    }
+}
+
 extern "C" __global__ void __launch_bounds__(BGR_JIT_ITEM_ROWS / BGR_JIT_ROWS, BGR_JIT_MINB) k_generic_jit(const __grid_constant__ GenericParams p) {
     constexpr int B = kJitItemRows / kJitRows;  // threads per work item
     __shared__ unsigned int s_acc[kMaxSaves * kAccStride * 2];
@@ -113,8 +215,6 @@ extern "C" __global__ void __launch_bounds__(BGR_JIT_ITEM_ROWS / BGR_JIT_ROWS, B
 
     const uint8_t* first_img = p.arena + ((p.flags & PF_READ_LIVE) ? size_t(0) : (size_t(p.ops[0].image_off256) << 8));
     const uint32_t first_rows = (p.flags & PF_READ_LIVE) ? p.live_rows : p.ops[0].n_rows;
-    constexpr uint32_t kTileBytes = kTileRows * (4u * kJitWords + 1u);
-    constexpr uint32_t kAliveOff = uint32_t(kJitWords) * kPlaneBytes;  // the mask bytes follow the word planes inside a tile
 
     const uint32_t n_items = p.n_tiles * uint32_t(kJitSubs);
     for (uint32_t item = blockIdx.x; item < n_items;) {
@@ -126,60 +226,8 @@ extern "C" __global__ void __launch_bounds__(BGR_JIT_ITEM_ROWS / BGR_JIT_ROWS, B
         }
         __syncthreads();
         const uint32_t next_item = s_next;
-        const uint32_t tile = item / uint32_t(kJitSubs), sub_row0 = (item % uint32_t(kJitSubs)) * uint32_t(kJitItemRows) + tid;  // first row of the thread inside the tile
-        const size_t tile_off = size_t(tile) * kTileBytes;
-        const unsigned long long row0 = p.order_base + size_t(tile) * kTileRows + sub_row0;
-
-        JitRows r;
-        auto load = [&](const uint8_t* img, uint32_t n_rows_src) {
-            const uint8_t* t = img + tile_off;
-#pragma unroll
-            for (int k = 0; k < kJitRows; ++k) {
-                const uint32_t row = sub_row0 + k * B;
-#pragma unroll
-                for (int j = 0; j < kJitWords; ++j) r.w[k][j] = __ldcg(reinterpret_cast<const uint32_t*>(t + size_t(j) * kPlaneBytes + size_t(row) * 4u));
-                const uint32_t mm = __ldcg(t + kAliveOff + row);  // .cg: L2 only — overlapping grids share an SM's L1 without a kernel boundary in between
-                r.m[k] = (tile * kTileRows + row < n_rows_src) ? mm : 0u;  // rows the image never contained come back dead
-            }
-        };
-        auto store = [&](uint8_t* img) {
-            uint8_t* t = img + tile_off;
-#pragma unroll
-            for (int k = 0; k < kJitRows; ++k) {
-                const uint32_t row = sub_row0 + k * B;
-#pragma unroll
-                for (int j = 0; j < kJitWords; ++j) *reinterpret_cast<uint32_t*>(t + size_t(j) * kPlaneBytes + size_t(row) * 4u) = r.w[k][j];
-                t[kAliveOff + row] = uint8_t(r.m[k]);
-            }
-        };
-        load(first_img, first_rows);
-#pragma unroll
-        for (int k = 0; k < kJitRows; ++k) r.t0[k] = sea_order_lane(row0 + uint32_t(k * B));
-
-        for (uint32_t i = (p.flags & PF_READ_LIVE) ? 0u : 1u; i < p.n_ops; ++i) {
-            const Op& op = p.ops[i];
-            if (op.kind == OP_ADVANCE) {
-#pragma unroll
-                for (int k = 0; k < kJitRows; ++k) r.kill[k] = false;
-                jit_run_systems<0>(r, op, row0, B);
-#pragma unroll
-                for (int k = 0; k < kJitRows; ++k) r.m[k] = r.kill[k] ? 0u : r.m[k];  // despawn commands: after the last system
-            } else if (op.kind == OP_SAVE) {
-                if (!(op.flags & OPF_NO_STORE)) store(p.arena + (size_t(op.image_off256) << 8));
-                uint32_t n_alive = 0, bad = 0;
-#pragma unroll
-                for (int k = 0; k < kJitRows; ++k) n_alive += r.m[k] & 1u;
-                unsigned int* a = &s_acc[op.save_index * kAccStride * 2];
-                jit_hash_columns<0>(r, a, lane, bad);
-                const unsigned full = 0xffffffffu;
-                const uint32_t cnt = __reduce_add_sync(full, n_alive);
-                const uint32_t anybad = __reduce_or_sync(full, bad);
-                if (lane == 0) { atomicAdd(&a[12], cnt); if (anybad) atomicOr(&a[14], 1u); }
-            } else {  // OP_LOAD
-                load(p.arena + (size_t(op.image_off256) << 8), op.n_rows);
-            }
-        }
-        if (p.flags & PF_WRITE_LIVE_ACTIVE) store(p.arena);
+        jit_run_item(p.arena, p.order_base, p.flags, p.n_ops, [&](uint32_t i) -> const Op& { return p.ops[i]; }, first_img, first_rows,
+                     item, s_acc, tid, lane);
         if (signal_items) {  // every thread's stores of this item are visible at gpu scope, then one release store announces it
             __threadfence();
             __syncthreads();
@@ -187,35 +235,37 @@ extern "C" __global__ void __launch_bounds__(BGR_JIT_ITEM_ROWS / BGR_JIT_ROWS, B
         }
         item = next_item;
     }
+    jit_fold_publish(p.accum, p.ticket, p.out, p.seq, p.n_saves, gridDim.x, s_acc, s_last, p.trace, tid);
+}
 
-    // ---- block partials -> global accumulators -> (last block) host-visible results: k_particles_program's protocol ----
-    __syncthreads();
-    for (uint32_t i = tid; i < p.n_saves * kAccStride; i += B) {
-        unsigned long long v = (unsigned long long)s_acc[2 * i] | ((unsigned long long)s_acc[2 * i + 1] << 32);
-        const uint32_t c = i % kAccStride;
-        if (v) {
-            if (c == 6) atomicAdd(&p.accum[i], v);
-            else if (c == 7) atomicOr(&p.accum[i], v);
-            else atomicXor(&p.accum[i], v);
-        }
+// The request vectors of many engines with this registration in ONE launch (bgr_batch_handle_requests).  Block b runs
+// one work item of one world: the world whose first block (JitWorld::item0, a prefix of the worlds' item counts) is the
+// last one <= b.  Each world keeps k_generic_jit's completion protocol on its own accumulators, ticket and result block,
+// with its item count in place of gridDim.x.  No dynamic claiming, no overlap of consecutive launches (PF_TILE_SIGNAL /
+// PF_TILE_WAIT) and no trace rows.
+extern "C" __global__ void __launch_bounds__(BGR_JIT_ITEM_ROWS / BGR_JIT_ROWS, BGR_JIT_MINB)
+    k_generic_jit_batch(const JitWorld* __restrict__ worlds, uint32_t n_worlds, const Op* __restrict__ ops) {
+    constexpr int B = kJitItemRows / kJitRows;
+    __shared__ unsigned int s_acc[kMaxSaves * kAccStride * 2];
+    __shared__ unsigned int s_last;
+    const uint32_t tid = threadIdx.x, lane = tid & 31u;
+
+    uint32_t lo = 0, hi = n_worlds;
+    while (hi - lo > 1u) {
+        const uint32_t mid = (lo + hi) / 2u;
+        if (worlds[mid].item0 <= blockIdx.x) lo = mid;
+        else hi = mid;
     }
-    __threadfence();
+    const JitWorld w = worlds[lo];
+    for (uint32_t i = tid; i < w.n_saves * kAccStride * 2; i += B) s_acc[i] = 0u;
     __syncthreads();
-    if (p.trace && tid == 0) atomicMax(&p.trace[1], globaltimer_ns());
-    if (tid == 0) s_last = (atomicAdd(p.ticket, 1u) == gridDim.x - 1u);
-    __syncthreads();
-    if (s_last) {
-        __threadfence();
-        for (uint32_t i = tid; i < p.n_saves * kAccStride; i += B)
-            publish_pair(p.out, i, atomicExch(&p.accum[i], 0ULL), p.seq);
-        if (tid == 0) publish_pair(p.out, kSeqIndex, p.seq, p.seq);
-        __syncthreads();
-        if (tid == 0) {
-            p.ticket[0] = 0u;
-            p.ticket[1] = 0u;
-            if (p.trace) p.trace[2] = globaltimer_ns();
-        }
-    }
+
+    const Op* wops = ops + w.ops_off;
+    const uint8_t* first_img = w.arena + ((w.flags & PF_READ_LIVE) ? size_t(0) : (size_t(wops[0].image_off256) << 8));
+    const uint32_t first_rows = (w.flags & PF_READ_LIVE) ? w.live_rows : wops[0].n_rows;
+    jit_run_item(w.arena, w.order_base, w.flags, w.n_ops, [&](uint32_t i) -> const Op& { return wops[i]; }, first_img, first_rows,
+                 blockIdx.x - w.item0, s_acc, tid, lane);
+    jit_fold_publish(w.accum, w.ticket, w.out, w.seq, w.n_saves, w.n_tiles * uint32_t(kJitSubs), s_acc, s_last, nullptr, tid);
 }
 
 }  // namespace bgr

@@ -40,6 +40,11 @@ class LastKernel(NamedTuple):
     stable_planes: bool = False
     held_saves: bool = False
 
+    @property
+    def batched(self) -> bool:
+        """The vector ran inside a world batch's launch (BGR_KERNEL_BATCHED, EngineBatch)."""
+        return bool(self.raw & capi.BGR_KERNEL_BATCHED)
+
     @staticmethod
     def decode(v: int) -> "LastKernel":
         return LastKernel(_KERNEL_KINDS.get(v & 0xF, f"unknown({v & 0xF})"), (v >> 4) & 0xF, (v >> 8) & 0x3,
@@ -515,6 +520,65 @@ class Engine:
 
     def shard_group_leave(self) -> None:
         self._check(self._lib.bgr_shard_group_leave(self._h))
+
+
+class EngineBatch:
+    """A world batch (bgr_batch_*): engines with one registration on one shared stream whose request vectors run in one
+    kernel launch.  Holds its engines, so none is destroyed while the batch exists."""
+
+    def __init__(self, engines: Sequence[Engine]):
+        self._lib = capi.load_library()
+        self._h = None
+        self.engines = list(engines)
+        arr = (C.c_void_p * max(1, len(self.engines)))(*[e._h for e in self.engines])
+        h = C.c_void_p()
+        self._check(self._lib.bgr_batch_create(arr, len(self.engines), C.byref(h)))
+        self._h = h
+
+    def _check(self, status: int) -> None:
+        if status != capi.BGR_OK:
+            raise BgrError(status, self._lib.bgr_last_error().decode("utf-8", "replace"))
+
+    def close(self) -> None:
+        if self._h is not None:
+            self._lib.bgr_batch_destroy(self._h)
+            self._h = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    def specialised(self) -> bool:
+        """True if calls run as one launch; False: each world's own handle_requests runs in turn (same results)."""
+        v = C.c_uint32()
+        self._check(self._lib.bgr_batch_specialised(self._h, C.byref(v)))
+        return bool(v.value)
+
+    def handle_requests(self, calls) -> List[Tuple[int, List[Tuple[int, int]]]]:
+        """``calls`` = [(world, session_info, requests), ...]: the listed worlds' vectors in one synchronous call.
+        Returns [(status, [(frame, checksum), ...]), ...] in the same order; a world's status is what its own
+        handle_requests would have returned (BGR_ERR_NON_FINITE ...).  A call refused before anything executed (bad
+        index, unsaved frame, pending submits ...) raises BgrError and changes no world."""
+        calls = [(w, si, list(r)) for w, si, r in calls]
+        n = len(calls)
+        worlds = (C.c_uint32 * max(1, n))(*[w for w, _, _ in calls])
+        sessions = (capi.bgr_session_info * max(1, n))(*[capi.make_session_info(si) for _, si, _ in calls])
+        reqs = capi.make_requests([q for _, _, r in calls for q in r])
+        n_req = (C.c_uint32 * max(1, n))(*[len(r) for _, _, r in calls])
+        cap = sum(1 for _, _, r in calls for q in r if q.kind == capi.BGR_REQ_SAVE)
+        out = (capi.bgr_checksum * max(1, cap))()
+        n_cs = (C.c_uint32 * max(1, n))()
+        status = (C.c_int32 * max(1, n))()
+        rc = self._lib.bgr_batch_handle_requests(self._h, worlds, n, sessions, reqs, n_req, out, cap, n_cs, status)
+        if rc not in (capi.BGR_OK, capi.BGR_ERR_NON_FINITE):
+            self._check(rc)
+        res, k = [], 0
+        for i in range(n):
+            res.append((status[i], [(out[k + j].frame, (out[k + j].hi << 64) | out[k + j].lo) for j in range(n_cs[i])]))
+            k += n_cs[i]
+        return res
 
 
 def fold_partials(partial: "capi.bgr_partial") -> int:

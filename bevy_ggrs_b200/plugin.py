@@ -346,6 +346,12 @@ class App:
             for s in self._startup:
                 s(self)
 
+    def finish(self) -> "App":
+        """``App::finish``: builds the engine and runs Startup once (the first update does it otherwise).  An
+        ``EngineBatch`` takes built engines."""
+        self._finish()
+        return self
+
     def update(self) -> None:
         self._finish()
         # bevy Time<Real>: the first update has zero delta, later ones the manual duration
@@ -375,6 +381,15 @@ class App:
             self._tick()
 
     def _tick(self) -> None:
+        requests = self._advance_session()
+        if requests is None:
+            return
+        self.handle_requests(requests)
+        self.ticks += 1
+
+    def _advance_session(self) -> Optional[List[Request]]:
+        """ReadInputs and the session's advance_frame of one tick: its request vector, or None when the session
+        skipped the tick (a SyncTest mismatch has fired the observers)."""
         sess = self._session
         inner = sess.inner
         self.local_players = LocalPlayers(list(range(inner.num_players())))
@@ -387,21 +402,24 @@ class App:
         for handle, value in self._local_inputs.inputs.items():
             inner.add_local_input(handle, value)
         try:
-            requests = inner.advance_frame()
+            return inner.advance_frame()
         except MismatchedChecksum as e:  # :104-115
             ev = SyncTestMismatch(e.current_frame, e.mismatched_frames)
             for obs in self._observers:
                 obs(ev)
-            return
+            return None
         except GgrsError:
-            return
-        self.handle_requests(requests)
-        self.ticks += 1
+            return None
 
     # ---- handle_requests (schedule_systems.rs:170-289) ----
     def handle_requests(self, requests: Sequence[Request]) -> None:
         inner = self._session.inner
-        checksums = self.world.handle_requests(inner.info(), requests)
+        self._host_requests(requests, self.world.handle_requests(inner.info(), requests))
+
+    def _host_requests(self, requests: Sequence[Request], checksums) -> None:
+        """The host half of handle_requests, given the engine's checksums of the vector: resources XORed into the
+        checksums, host-side component tables, and the session's cells."""
+        inner = self._session.inner
         if self._res_registered:
             checksums = self._handle_resource_requests(requests, checksums)
         if self.host_components.columns:
@@ -446,3 +464,29 @@ class App:
         alive = set(self.world.snapshot_frames())
         self._res_store = {f: v for f, v in self._res_store.items() if f in alive}
         return out
+
+
+def step_batch(apps: Sequence[App], batch) -> None:
+    """Exactly one GGRS tick of every App, like ``App.step()`` on each in turn, with ONE engine call for all of them:
+    ``batch`` is an ``EngineBatch`` over the Apps' engines (built: ``App.finish``).  Every App runs ReadInputs and its
+    session's advance_frame (an App whose SyncTest mismatches fires its own observers and skips the tick), the batch runs
+    the vectors, and each App runs the host half of handle_requests with its checksums.  A world whose call failed after
+    executing (BGR_ERR_NON_FINITE) raises once every other App has finished its tick."""
+    index = {id(e): i for i, e in enumerate(batch.engines)}
+    ticking = []
+    for app in apps:
+        app._finish()
+        requests = app._advance_session()
+        if requests is not None:
+            ticking.append((app, requests))
+    results = batch.handle_requests([(index[id(app.world)], app._session.inner.info(), requests) for app, requests in ticking])
+    failed = None
+    for (app, requests), (status, checksums) in zip(ticking, results):
+        if status != capi.BGR_OK:
+            failed = failed or capi.BgrError(status, "Hashing is not stable for NaN f32 values." if status == capi.BGR_ERR_NON_FINITE
+                                             else f"bgr_batch_handle_requests status {status}")
+            continue
+        app._host_requests(requests, checksums)
+        app.ticks += 1
+    if failed is not None:
+        raise failed

@@ -593,6 +593,34 @@ BGR_API int bgr_fold_partials(const bgr_partial* combined, bgr_checksum* out);
 BGR_API int bgr_collect_partials(bgr_engine* e, bgr_partial* partials_out, uint32_t cap, uint32_t* n_out);
 BGR_API int bgr_fold_partials_n(const bgr_partial* combined, uint32_t n, bgr_checksum* out);
 
+/* ---- world batches: the request vectors of many engines in ONE kernel launch ---------------------------------------
+ * A batch is a fixed set of built engines ("worlds") with an identical registration (the same columns, presence flags,
+ * checksums and systems in the same order), created on one device with the same non-null bgr_config.stream, that run
+ * the generic one-launch program (not the particles bundle, BGR_CFG_FORCE_STEPWISE or a spawn system) and are not
+ * sharded.  Capacity, max_depth, fps, row count, session kind, frame, BGR_CFG_DESYNC_CAPTURE, BGR_CFG_GROWABLE and
+ * order_base may differ.  bgr_batch_create checks all of this and names the first engine that fails.  Destroy a batch
+ * before any of its engines; between calls every per-engine entry point stays usable on the members. */
+typedef struct bgr_batch bgr_batch;
+BGR_API int bgr_batch_create(bgr_engine* const* engines, uint32_t n, bgr_batch** out);
+BGR_API void bgr_batch_destroy(bgr_batch* b);
+/* 1: calls run as ONE launch of the registration's generated kernel (k_generic_jit_batch).  0 without NVRTC, with
+ * BGR_TUNE_JIT=0, or for a registration the generated kernel does not take (more than 24 words per row, checksummed
+ * byte ranges that are not whole words): calls then run each world's own bgr_handle_requests in list order, with the
+ * same results (BGR_JIT_VERBOSE=1 prints why). */
+BGR_API int bgr_batch_specialised(bgr_batch* b, uint32_t* specialised_out);
+/* Synchronous: what bgr_handle_requests on worlds[0], worlds[1], ... in that order would do, in one launch.  World
+ * worlds[i] runs the n_requests[i] requests that follow the previous worlds' in `requests` under sessions[i] (sessions
+ * NULL: no session).  Every world is validated and its vector compiled first (indices in range and distinct,
+ * n_requests[i] <= BGR_MAX_REQUESTS, no un-collected bgr_submit_requests): if any fails, nothing executes in any world,
+ * the call returns that status, status_out marks that world and bgr_last_error() starts with "world <index>: ".
+ * Otherwise every world executes, status_out[i] is what its own call would have returned (BGR_ERR_NON_FINITE ...) and
+ * the call returns the first non-OK one.  World i's checksums follow the previous worlds' in checksums_out, as far as
+ * checksums_cap reaches; n_checksums_out[i] is its count.  Worlds not listed are untouched.  Each listed world's
+ * bgr_launch_count grows by one and its bgr_last_kernel carries BGR_KERNEL_BATCHED. */
+BGR_API int bgr_batch_handle_requests(bgr_batch* b, const uint32_t* worlds, uint32_t n_worlds, const bgr_session_info* sessions,
+                                      const bgr_request* requests, const uint32_t* n_requests, bgr_checksum* checksums_out,
+                                      uint32_t checksums_cap, uint32_t* n_checksums_out, int32_t* status_out);
+
 /* ---- shard group: the cross-shard step inside the engine (multi-GPU, one process per GPU, one node) -----------------
  * Entity-range shards never exchange state (SURVEY.md §8e: systems read no other entity, box_game.rs:162-169; the
  * checksum is an XOR over entities, component_checksum.rs:88-89).  The only exchange is 64 bytes of partials per
@@ -659,12 +687,14 @@ BGR_API int bgr_generic_specialised(bgr_engine* e, uint32_t* specialised_out);
  *              grids of several waves; a single-wave (latency-bound) grid stores every active plane
  *   bit 27     BGR_KERNEL_HELD_SAVES, bundle: at least one Save was held: its target slot already held the content and
  *              row count it would have stored (host-side content ids), so it stored nothing and only checksummed
- *              (bgr_held_saves; env BGR_TUNE_HELD_SAVES, default 1) */
+ *              (bgr_held_saves; env BGR_TUNE_HELD_SAVES, default 1)
+ *   bit 28     BGR_KERNEL_BATCHED, generic NVRTC: the vector ran inside a world batch's launch (bgr_batch_handle_requests) */
 #define BGR_KERNEL_DEFERRED_LIVE (1u << 13)
 #define BGR_KERNEL_FROM_DEFERRED (1u << 14)
 #define BGR_KERNEL_PASSIVE_PLANES (1u << 15)
 #define BGR_KERNEL_STABLE_PLANES (1u << 26)
 #define BGR_KERNEL_HELD_SAVES (1u << 27)
+#define BGR_KERNEL_BATCHED (1u << 28)
 #define BGR_KERNEL_NONE 0u
 #define BGR_KERNEL_STEPWISE_TMA 1u       /* one kernel per request; Save / Load through the TMA-staged copy kernel */
 #define BGR_KERNEL_STEPWISE_FLAT 2u      /* one kernel per request; k_checksum_column + k_copy_image */

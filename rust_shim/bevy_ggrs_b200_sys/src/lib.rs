@@ -52,6 +52,8 @@ pub const BGR_KERNEL_PASSIVE_PLANES: u32 = 1 << 15;
 pub const BGR_KERNEL_STABLE_PLANES: u32 = 1 << 26;
 /// bgr_last_kernel flag: the bundle launch held at least one Save (its target slot already held that content).
 pub const BGR_KERNEL_HELD_SAVES: u32 = 1 << 27;
+/// bgr_last_kernel flag: the request vector ran inside a world batch's launch (bgr_batch_handle_requests).
+pub const BGR_KERNEL_BATCHED: u32 = 1 << 28;
 
 pub const BGR_CFG_FORCE_STEPWISE: u32 = 1;
 pub const BGR_CFG_SHARDED: u32 = 2;
@@ -76,6 +78,9 @@ pub use host_edits::*;
 // the world checkpoint header too
 mod checkpoint;
 pub use checkpoint::*;
+// world batches: a safe owner of a bgr_batch
+mod batch;
+pub use batch::*;
 
 #[repr(C)]
 #[derive(Clone, Copy, Default)]
@@ -130,6 +135,7 @@ pub struct bgr_config {
 pub enum bgr_engine {}
 #[allow(non_camel_case_types)]
 pub enum bgr_group {}
+pub enum bgr_batch {}
 
 extern "C" {
     pub fn bgr_abi_version() -> u32;
@@ -191,6 +197,10 @@ extern "C" {
     pub fn bgr_fold_partials(combined: *const bgr_partial, out: *mut bgr_checksum) -> c_int;
     pub fn bgr_collect_partials(e: *mut bgr_engine, partials_out: *mut bgr_partial, cap: u32, n_out: *mut u32) -> c_int;
     pub fn bgr_fold_partials_n(combined: *const bgr_partial, n: u32, out: *mut bgr_checksum) -> c_int;
+    pub fn bgr_batch_create(engines: *const *mut bgr_engine, n: u32, out: *mut *mut bgr_batch) -> c_int;
+    pub fn bgr_batch_destroy(b: *mut bgr_batch);
+    pub fn bgr_batch_specialised(b: *mut bgr_batch, specialised_out: *mut u32) -> c_int;
+    pub fn bgr_batch_handle_requests(b: *mut bgr_batch, worlds: *const u32, n_worlds: u32, sessions: *const bgr_session_info, requests: *const bgr_request, n_requests: *const u32, checksums_out: *mut bgr_checksum, checksums_cap: u32, n_checksums_out: *mut u32, status_out: *mut i32) -> c_int;
     pub fn bgr_seahash(bytes: *const c_void, len: u64) -> u64;
     pub fn bgr_ggrs_time_delta_bits(fps: u32, frame: i32) -> u32;
     pub fn bgr_particle_rng_stream(seed: u64, state4_or_null: *const u64, n: u32, next_u64_out: *mut u64, range_out: *mut f32, low: f32, high: f32) -> c_int;
