@@ -21,6 +21,9 @@ The host bookkeeping behind the skipped work (passive-plane versions, content st
 these interleavings exercise; a stale record does not fault, it skips a store, so only a comparison finds it.  Each run
 counts what it reached (``Interleaving.tally``) so that a test can assert that it reached it.
 
+``Fleet`` runs several such worlds with one registration as the members of one world batch (``EngineBatch``): batched
+calls over random subsets of them, refused batched calls, and each member's own actions in between.
+
 ``REPLAY_ENV`` ("<configuration>:<seed>") restricts a test module to one configuration and seed.
 
 TEST INFRASTRUCTURE: nothing in the product package imports this file.
@@ -113,6 +116,9 @@ class Config:
     steps: int = 60
     digests: int = 1_000_000            # frame digests per run (the oracle's digest is a Python loop)
     grow_margin: int = 4096             # rows the sequence may add (the twin's capacity past the initial rows)
+    fps: int = 60                       # bgr_config.fps: Time<GgrsTime>'s dt reaches the systems through each Advance
+    order_base: int = 0                 # bgr_config.order_base: the RollbackOrdered index of row 0 (no spawns past the
+                                        # first vector then, so the generator draws none)
 
 
 class FlagsOracle(RetainOracleWorld):
@@ -155,8 +161,8 @@ class CheckFailed(AssertionError):
 
 
 class Interleaving:
-    """One configuration and seed.  ``new_engine(role, max_entities, flags, env)`` makes the engine ("engine") and its
-    twin ("twin"); the oracle is made here."""
+    """One configuration and seed.  ``new_engine(role, max_entities, flags, env, fps=, order_base=)`` makes the engine
+    ("engine") and its twin ("twin"); the oracle is made here."""
 
     def __init__(self, cfg: Config, seed: int, new_engine, stamp_first: Optional[int] = None):
         self.cfg, self.seed = cfg, seed
@@ -173,9 +179,10 @@ class Interleaving:
         self.stamp_next = stamp_first
         if stamp_first is not None:
             env["BGR_TEST_STAMP_FIRST"] = str(stamp_first)
-        self.eng = new_engine("engine", eng_cap, cfg.flags, env)
-        self.twin = new_engine("twin", self.twin_cap, cfg.flags & ~capi.BGR_CFG_GROWABLE, {**cfg.env, **TWIN_ENV})
-        self.orc = FlagsOracle(max_entities=self.twin_cap, max_depth=9)
+        world_cfg = dict(fps=cfg.fps, order_base=cfg.order_base)
+        self.eng = new_engine("engine", eng_cap, cfg.flags, env, **world_cfg)
+        self.twin = new_engine("twin", self.twin_cap, cfg.flags & ~capi.BGR_CFG_GROWABLE, {**cfg.env, **TWIN_ENV}, **world_cfg)
+        self.orc = FlagsOracle(max_entities=self.twin_cap, max_depth=9, **world_cfg)
         for x in (self.eng, self.twin, self.orc):
             w.register(x, cfg.retain)
             x.set_depth(8)   # a ring of at most 8 frames fits max_depth = 9 (twice that with desync capture)
@@ -189,7 +196,10 @@ class Interleaving:
         self.deferred_tail: Optional[int] = None   # trailing Advances of the engine's deferred live image, if any
         self.max_rows = w.n
         self.log: List[str] = []
+        self.tag = ""                      # prefix of this world's log lines (a Fleet member's index)
         self.step = -1
+        self.between_submits: Optional[Callable[[], None]] = None   # a Fleet's batched step, run between queued submits
+        self.last_way: Optional[str] = None   # "solo" / "batched": how the last vector ran
         self.tally: Counter = Counter()
         self.digests_left = cfg.digests
         self.last_cap = self.eng.capacity()[0]
@@ -206,7 +216,7 @@ class Interleaving:
 
     # ------------------------------------------------------------------ failure context
     def note(self, text: str) -> None:
-        self.log.append(f"{self.step}: {text}")
+        self.log.append(f"{self.step}: {self.tag}{text}")
 
     def fail(self, what: str) -> None:
         raise CheckFailed(what)
@@ -329,13 +339,19 @@ class Interleaving:
         self.max_rows = max(self.max_rows, self.orc.row_count())
         return out
 
-    def _kernel_after(self, reqs, launches_before: int, rows_before: int) -> None:
-        """Tally of one launched vector (last_kernel, launch_count) and the content-stamp mirror."""
+    def _kernel_after(self, reqs, launches_before: int, rows_before: int, batched: bool = False) -> None:
+        """Tally of one launched vector (last_kernel, launch_count) and the content-stamp mirror.  ``batched``: the
+        vector ran in a world batch's call (Fleet)."""
         k = self.eng.last_kernel()
         row = self.launched
         self.launched += 1
         if self.cfg.kind is not None:
             self.check(k.kind == self.cfg.kind, f"the vector ran {k.kind}, not {self.cfg.kind}")
+        way = "batched" if batched else "solo"
+        if self.last_way is not None and self.last_way != way:
+            self.tally[f"{way}_after_{self.last_way}"] += 1
+        self.last_way = way
+        self.tally[f"{way}_{k.kind}"] += 1
         extra = self.eng.launch_count() - launches_before - 1    # a materialisation runs before the vector
         if extra > 0 and k.kind in ("bundle", "generic_interpreter", "generic_nvrtc"):   # one launch per fused vector
             self.tally["materialisations"] += extra
@@ -489,6 +505,10 @@ class Interleaving:
             if chained and rows > rows_before and -(-rows // TILE) != -(-rows_before // TILE):
                 self.tally["queued_tile_crossings"] += 1
             chained = True
+            if i < k - 1 and self.between_submits is not None and self.rng.random() < 0.3:
+                self.note("  (other worlds' batched call, this world's submits in flight on the shared stream)")
+                self.between_submits()
+                chained = False
             if i < k - 1 and not self.rollover_due():   # nothing but a plain tick may launch at the rollover
                 r = self.rng.random()
                 chained = r >= 0.65
@@ -536,7 +556,7 @@ class Interleaving:
 
     def act_host_write(self) -> None:
         w, rng, rows = self.world, self.rng, self.orc.row_count()
-        opts = ["band", "band", "despawn", "presence", "spawn"]
+        opts = ["band", "band", "despawn", "presence"] + (["spawn"] if self.cfg.order_base == 0 else [])
         if w.spawn_rate:
             opts.append("startup")
         if self.growable:
@@ -864,3 +884,166 @@ class Interleaving:
             self.check(tuple(info) == tuple(einfo) and recs.tobytes() == expect.tobytes(), "the final feed report differs")
             replica.apply(recs)
             self.check(replica.matches(model, world), "the replica does not match the model at the end")
+
+
+# ---------------------------------------------------------------------------------------------------- world batches
+@dataclass
+class FleetConfig:
+    """A world batch's configuration.  ``registration(rng)`` draws the registration once per fleet and returns
+    ``make(rng, member)``, the maker of each member's World (its rows and data, drawn from the member's own generator).  ``members``: one Config
+    per member for its flags, retention, fps, order_base and grow margin (their name, world, env and kind are set here)."""
+    name: str
+    registration: Callable[[np.random.Generator], Callable[[np.random.Generator, int], World]]
+    members: List[Config]
+    env: Dict[str, str] = field(default_factory=dict)
+    steps: int = 80
+
+
+class Fleet:
+    """K ``Interleaving`` members whose engines share one stream and one ``EngineBatch``, each with its own oracle, twin
+    and feed models.  A step is a batched call over a random non-empty subset of the members in random order (each
+    member draws its own vector), sometimes with one world's vector refused, or one member's ordinary action
+    (``Interleaving.one_step``: its solo and queued vectors, host writes, reads and feeds land between batched calls).
+    While a member holds un-collected submits, a batched call over the other members may run on the shared stream.
+
+    ``new_engine(member, role, max_entities, flags, env, fps=, order_base=)`` makes member ``member``'s engine (on the
+    shared stream) and twin; ``new_batch(engines)`` makes the batch."""
+
+    def __init__(self, fcfg: FleetConfig, seed: int, new_engine, new_batch):
+        self.fcfg, self.seed = fcfg, seed
+        self.rng = np.random.default_rng(104729 * seed + sum(map(ord, fcfg.name)))
+        make = fcfg.registration(self.rng)
+        self.log: List[str] = []
+        self.step = -1
+        self.tally: Counter = Counter()
+        self.members: List[Interleaving] = []
+        self.batch = None
+        try:
+            for i, mc in enumerate(fcfg.members):
+                cfg = Config(**{**mc.__dict__, "name": f"{fcfg.name}/{i}", "world": lambda rng, _i=i: make(rng, _i), "env": {**fcfg.env, **mc.env},
+                                "kind": None, "stamped": False})
+                m = Interleaving(cfg, seed, lambda role, *a, _i=i, **kw: new_engine(_i, role, *a, **kw))
+                m.log, m.tag = self.log, f"w{i} "
+                m.between_submits = lambda _i=i: self.act_batch(exclude=_i)
+                self.members.append(m)
+            self.batch = new_batch([m.eng for m in self.members])
+        except BaseException:
+            self.close()
+            raise
+        self.specialised = self.batch.specialised()
+
+    def note(self, text: str) -> None:
+        self.log.append(f"{self.step}: {text}")
+
+    def totals(self) -> Counter:
+        """The fleet's tally and every member's, added up."""
+        t = Counter(self.tally)
+        for m in self.members:
+            t.update(m.tally)
+        return t
+
+    def run(self, steps: Optional[int] = None) -> Counter:
+        steps = self.fcfg.steps if steps is None else steps
+        for self.step in range(steps + 1):
+            for m in self.members:
+                m.step = self.step
+            try:
+                if self.step == steps:
+                    self.note("final: full comparison of every member")
+                    for m in self.members:
+                        m.compare_everything()
+                else:
+                    self.one_step()
+                    for m in self.members:
+                        m.compare_host_state()
+            except Exception as ex:
+                tail = "\n".join("  " + a for a in self.log)
+                raise CheckFailed(f"fleet {self.fcfg.name} seed {self.seed} step {self.step}: "
+                                  f"{type(ex).__name__}: {ex}\naction log:\n{tail}") from ex
+        return self.totals()
+
+    def close(self) -> None:
+        if self.batch is not None:
+            self.batch.close()   # before any of its engines
+            self.batch = None
+        for m in self.members:
+            m.close()
+
+    def one_step(self) -> None:
+        if self.rng.random() < 0.45:
+            return self.act_batch()
+        self.members[int(self.rng.integers(0, len(self.members)))].one_step()
+
+    def act_batch(self, exclude: Optional[int] = None) -> None:
+        """A batched call over a random subset (``exclude``: a member with submits in flight, never listed)."""
+        avail = [i for i in range(len(self.members)) if i != exclude]
+        if not avail:
+            return
+        k = int(self.rng.integers(1, len(avail) + 1))
+        worlds = [avail[int(j)] for j in self.rng.permutation(len(avail))[:k]]
+        calls = []
+        for i in worlds:
+            m = self.members[i]
+            shape, info, reqs = m.pick_vector(m.random_shape())
+            calls.append((i, shape, info, reqs))
+        if self.rng.random() < 0.08:
+            return self.act_batch_refused(calls, exclude)
+        self.note(f"batched call over worlds {worlds}" + (f" (w{exclude} has submits in flight)" if exclude is not None else ""))
+        expected = []
+        for i, shape, info, reqs in calls:   # the oracle of every listed world, before the call
+            m = self.members[i]
+            m.note(f"batched {shape}: {list(reqs)} session {info}")
+            rows_before = m.orc.row_count()
+            expected.append((m._oracle_vector(info, reqs), m.eng.launch_count(), rows_before))
+        res = self.batch.handle_requests([(i, info, reqs) for i, _, info, reqs in calls])
+        self.check(len(res) == len(calls), f"{len(res)} results for {len(calls)} worlds")
+        for (i, shape, info, reqs), (status, got), (expect, before, rows_before) in zip(calls, res, expected):
+            m = self.members[i]
+            m.check(status == capi.BGR_OK, f"world {i}: batched status {status}")
+            m.check(got == expect, f"world {i}: batched checksums {got} != oracle {expect}")
+            lk = m.eng.last_kernel()
+            if self.specialised:
+                m.check(lk.batched and lk.kind == "generic_nvrtc", f"world {i}: a batched vector ran {lk}")
+            else:
+                m.check(not lk.batched, f"world {i}: an unspecialised batch reported a batched launch")
+            m.check(m.twin.handle_requests(info, reqs) == expect, f"world {i}: the twin's checksums differ from the oracle's")
+            m._kernel_after(reqs, before, rows_before, batched=True)
+            m.tally["vectors"] += 1
+            m.tally["vectors_batched"] += 1
+        self.tally["batched_calls"] += 1
+        self.tally["batched_worlds"] += len(calls)
+        if exclude is not None:
+            self.tally["batch_with_queued_member"] += 1
+
+    def act_batch_refused(self, calls, exclude: Optional[int]) -> None:
+        """One listed world loads a frame it does not hold: the call is refused, names that world and changes nothing
+        anywhere (no oracle is advanced)."""
+        j = int(self.rng.integers(0, len(calls)))
+        bad = calls[j][0]
+        f = self.members[bad].frame()
+        calls[j] = (bad, "invalid", NOSESS, [Request(LOAD, f + 1000)])
+        self.note(f"batched call over worlds {[c[0] for c in calls]}, w{bad} loads frame {f + 1000}: refused")
+        state = lambda: [(m.eng.launch_count(), m.eng.snapshot_frames(), m.eng.rollback_frame_count(), m.eng.row_count(),
+                          m.eng.confirmed_frame_count()) for m in self.members]
+        before = state()
+        try:
+            self.batch.handle_requests([(i, info, reqs) for i, _, info, reqs in calls])
+        except BgrError as ex:
+            self.check(ex.status == capi.BGR_ERR_NO_SNAPSHOT, f"the refused batched call returned {ex.status}")
+            self.check(str(ex).startswith(f"world {bad}: "), f"the refusal does not name world {bad}: {ex}")
+        else:
+            self.fail(f"a batched call in which world {bad} loads an unsaved frame was accepted")
+        after = state()
+        self.check(after == before, f"a refused batched call changed {before} to {after}")
+        for m in self.members:
+            m.compare_host_state()
+        self.tally["batch_refusals"] += 1
+        if exclude is not None:
+            self.tally["batch_with_queued_member"] += 1
+
+    def check(self, cond: bool, what: str) -> None:
+        if not cond:
+            self.fail(what)
+
+    def fail(self, what: str) -> None:
+        raise CheckFailed(what)

@@ -112,11 +112,11 @@ def _env(values):
 
 
 def new_engine(name):
-    def make(role, max_entities, flags, env):
+    def make(role, max_entities, flags, env, fps=60, order_base=0):
         if name in STEPWISE:
             flags |= capi.BGR_CFG_FORCE_STEPWISE
         with _env(env):   # read once, at bgr_engine_create
-            return Engine(max_entities=max_entities, max_depth=9, flags=flags)
+            return Engine(max_entities=max_entities, max_depth=9, fps=fps, flags=flags, order_base=order_base)
     return make
 
 
