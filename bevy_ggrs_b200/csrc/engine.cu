@@ -388,6 +388,7 @@ struct bgr_engine {
     uint32_t tma_stage_tiles = 0;  // one-tile stages of the TMA copy kernel (0: schema too wide for two stages of shared memory)
     DeviceBuffer<unsigned int> tma_ticket;
     int occ_cache[2][3][2][2] = {};  // [passive TMA][MODE][STAMPS][VERIFY]: blocks per SM of k_particles_program
+    int snap_fits = -1;              // -1 unknown; 0: the stamp-point snapshot would cost the passive-TMA launches a block per SM
     // desync diff scratch (BGR_CFG_DESYNC_CAPTURE), allocated by the first bgr_desync_diff
     DeviceBuffer<DiffColumn> diff_cols;
     DeviceBuffer<unsigned int> diff_counts;      // [n_cols][3] then the per-tile record counts
@@ -645,10 +646,10 @@ int launch_particles(bgr_engine* e, const ProgramParams& pp) {
     auto kern = k_particles_program<MODE, STAMPS, VERIFY>;
     constexpr int kBlock = int(kTileRows) / 2;  // two rows per thread
     const int ti = (pp.flags & PF_PASSIVE_TMA) ? 1 : 0;
-    const size_t smem = ti ? size_t(2) * pp.passive_bytes : 0;
+    const size_t smem = (ti ? size_t(2) * pp.passive_bytes : 0) + (STAMPS ? kSnapBytes : 0);
     // A mode runs with and without the passive double buffer (spawns and multi-Load vectors move passive planes per
     // thread): the shared-memory opt-in and the occupancy are per (mode, buffer).  passive_bytes is fixed at bgr_build,
-    // so one entry per buffer setting is exact.
+    // so one entry per buffer setting is exact.  The stamped instances also hold the stamp-point snapshot.
     int& occ = e->occ_cache[ti][MODE][STAMPS ? 1 : 0][VERIFY ? 1 : 0];
     if (occ == 0) {
         if (smem > 48 * 1024) CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem)));
@@ -675,6 +676,34 @@ int launch_particles(bgr_engine* e, const ProgramParams& pp) {
     // VEC 2, launch-bounds tier 1 (768 threads per SM), whole-tile work items
     e->last_kernel = BGR_KERNEL_BUNDLE | (2u << 4) | (uint32_t(MODE) << 8) | (1u << 10) | (ti ? 1u << 12 : 0u) |
                      (passive ? BGR_KERNEL_PASSIVE_PLANES : 0u) | (uint32_t(kTileRows) << 16) | (STAMPS ? BGR_KERNEL_STABLE_PLANES : 0u);
+    return BGR_OK;
+}
+
+// The stamped instances add the stamp-point snapshot (kSnapBytes) to the passive double buffer.  With more than about
+// 13 passive planes that costs the passive-TMA launches a resident block per SM; such a registration runs the instance
+// without stamps instead.  Launches without the double buffer (17 KB of shared memory) always keep three blocks.
+template <int MODE>
+int snapshot_fits_mode(bgr_engine* e, bool& fits) {
+    fits = true;
+    if (e->runs.empty() || 2u * e->passive_bytes > 96u * 1024u) return BGR_OK;  // never the passive-TMA configuration
+    auto kern = k_particles_program<MODE, true, false>;
+    const size_t buf = size_t(2) * e->passive_bytes, with = buf + kSnapBytes;
+    if (with > 48 * 1024) CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, int(with)));
+    int nb_without = 0, nb_with = 0;
+    CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb_without, kern, int(kTileRows) / 2, buf));
+    CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb_with, kern, int(kTileRows) / 2, with));
+    fits = nb_with >= nb_without;
+    return BGR_OK;
+}
+
+int snapshot_fits(bgr_engine* e, bool& fits) {
+    if (e->snap_fits < 0) {
+        const int rc = e->bundle_opt ? snapshot_fits_mode<2>(e, fits) : e->bundle_static_ck ? snapshot_fits_mode<1>(e, fits)
+                                                                                             : snapshot_fits_mode<0>(e, fits);
+        if (rc != BGR_OK) return rc;
+        e->snap_fits = fits ? 1 : 0;
+    }
+    fits = e->snap_fits == 1;
     return BGR_OK;
 }
 
@@ -714,9 +743,11 @@ int run_fused(bgr_engine* e, const Program& pg, uint32_t buf) {
     // one wave of blocks (every block runs one or two tiles): the tile's tail is the grid's tail
     if (e->tune_passive_early == 1 || (e->tune_passive_early < 0 && pp.n_tiles <= 3u * uint32_t(e->num_sms))) pp.flags |= PF_PASSIVE_EARLY;
     // Stable-plane elision pays where the grid is bandwidth-bound (several waves).  A single-wave grid is latency-bound:
-    // there the bit compares of every Advance and the stamp round trip of every Save only lengthen the critical path
+    // there the change tracking and the stamp round trip of every stored Save only lengthen the critical path
     // (100k entities: -9 % e2e), so it runs the instance without stamps.
-    const bool stamps = !(pp.flags & PF_PASSIVE_EARLY);
+    bool snap_fits = true;
+    if (int rc = snapshot_fits(e, snap_fits); rc != BGR_OK) return rc;
+    const bool stamps = !(pp.flags & PF_PASSIVE_EARLY) && snap_fits;
     const Column& ct = e->cols[e->bt]; const Column& cv = e->cols[e->bv];
     if (ct.hash_kind != BGR_HASH_NONE) { pp.flags |= PF_CK_T; if (ct.hash_flags & BGR_HASH_FLAG_ASSERT_FINITE_F32) pp.flags |= PF_FIN_T; pp.ck_t_slot = uint32_t(ct.ck_slot); }
     if (cv.hash_kind != BGR_HASH_NONE) { pp.flags |= PF_CK_V; if (cv.hash_flags & BGR_HASH_FLAG_ASSERT_FINITE_F32) pp.flags |= PF_FIN_V; pp.ck_v_slot = uint32_t(cv.ck_slot); }

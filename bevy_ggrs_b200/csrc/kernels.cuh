@@ -136,6 +136,9 @@ constexpr uint32_t kActivePlanes = 9;
 constexpr uint32_t kAlivePlaneBit = 1u << 8;
 constexpr uint32_t kSegRows = 64;
 constexpr uint32_t kSegsPerTile = kTileRows / kSegRows;
+// The stamped instances keep the active words and alive bytes of the last stamp point in shared memory, one snapshot per
+// thread laid out [word group][thread]: four uint4 groups (two planes of its two rows each) and one alive word.
+constexpr uint32_t kSnapBytes = (4u * 16u + 4u) * (kTileRows / 2u);
 
 struct ProgramParams {
     uint8_t* arena;
@@ -455,7 +458,9 @@ __global__ void __launch_bounds__(256, 3) k_particles_program(const __grid_const
     const bool CKV = STATIC_CK ? true : (p.flags & PF_CK_V) != 0;
     const bool FINT = STATIC_CK ? true : (p.flags & PF_FIN_T) != 0;
     const bool FINV = STATIC_CK ? true : (p.flags & PF_FIN_V) != 0;
-    extern __shared__ __align__(128) uint8_t s_passive[];  // 2 x passive_bytes (double buffer)
+    extern __shared__ __align__(128) uint8_t s_dyn[];  // STAMPS: the stamp-point snapshot (kSnapBytes); then 2 x passive_bytes (double buffer)
+    uint8_t* const s_passive = s_dyn + (STAMPS ? kSnapBytes : 0u);
+    uint4* const s_snap = reinterpret_cast<uint4*>(s_dyn);
     __shared__ unsigned int s_acc[kMaxSaves * kAccStride * 2];  // 32-bit halves: native shared atomics, no CAS loop
     __shared__ __align__(8) uint64_t s_bar[2];
     __shared__ unsigned int s_last;
@@ -559,12 +564,21 @@ __global__ void __launch_bounds__(256, 3) k_particles_program(const __grid_const
         uint32_t tr[3][VEC], vl[3][VEC], tl[2][VEC];
         uint32_t alive = 0;
         // Stable-plane elision.  Lane q < kActivePlanes holds `st`, the stamp of the content plane q of this warp's
-        // segment has in registers (0 = unknown); `dirty` collects the planes whose bits this thread changed since.  A
-        // Save gives every dirty or unknown plane a fresh stamp and stores only the planes whose stamp the target image
-        // does not already hold.
+        // segment had at the last stamp point (a Load or read of the live image, a stored Save, the live write; 0 =
+        // unknown).  Each thread keeps its words and alive bytes of that point in s_snap.  A stored Save compares the
+        // registers with the snapshot once, gives every plane that differs (or is unknown) a fresh stamp and stores only
+        // the planes whose stamp the target image does not already hold.  `dirty` is only the spawn bit: a spawning
+        // Advance marks every plane.
         uint32_t st = 0, dirty = 0;
         uint32_t* const seg_stamps = p.stamps + (size_t(tile) * kSegsPerTile + (tid >> 5)) * kActivePlanes + min(lane, kActivePlanes - 1u);
         const bool stamp_lane = lane < kActivePlanes;
+        auto put_snapshot = [&](uint32_t a) {
+            s_snap[0 * BLOCK + tid] = make_uint4(tr[0][0], tr[0][1], tr[1][0], tr[1][1]);
+            s_snap[1 * BLOCK + tid] = make_uint4(tr[2][0], tr[2][1], vl[0][0], vl[0][1]);
+            s_snap[2 * BLOCK + tid] = make_uint4(vl[1][0], vl[1][1], vl[2][0], vl[2][1]);
+            s_snap[3 * BLOCK + tid] = make_uint4(tl[0][0], tl[0][1], tl[1][0], tl[1][1]);
+            reinterpret_cast<uint32_t*>(s_snap + 4 * BLOCK)[tid] = a;
+        };
 
         auto load_active = [&](const uint8_t* img, uint32_t n_rows, uint32_t img_idx) {
             const uint8_t* pt = img + p.t_off + woff;
@@ -579,16 +593,33 @@ __global__ void __launch_bounds__(256, 3) k_particles_program(const __grid_const
             const uint32_t raw = alive_load<VEC>(img + aoff);
             alive = raw & (OPT ? rows_mask_full<VEC>(row0, n_rows) : rows_mask<VEC>(row0, n_rows));
             if (STAMPS) {
-                dirty = alive != raw ? kAlivePlaneBit : 0u;  // the row count cleared alive bytes the image holds
+                // the image's bytes: where the row count cleared alive bytes the image holds, the alive plane differs
+                put_snapshot(raw);
+                dirty = 0;
                 st = stamp_lane ? __ldcg(seg_stamps + size_t(img_idx) * p.stamp_image) : 0u;
             }
         };
-        // first half of a stamped store into image img_idx: stamps the dirty planes with `fresh` and issues the read of
-        // the image's stamps, which store_active consumes later (the checksum of a Save hides part of its latency)
+        // first half of a stamped store into image img_idx: stamps the planes whose bits differ from the snapshot with
+        // `fresh`, takes the registers as the new snapshot and issues the read of the image's stamps, which store_active
+        // consumes later (the checksum of a Save hides part of its latency)
         auto claim_stamps = [&](uint32_t img_idx, uint32_t fresh) -> uint32_t {
             if (!STAMPS) return 0u;
-            const uint32_t d = __reduce_or_sync(0xffffffffu, dirty);
+            // bits, not values: -0.0 -> +0.0 and a changed NaN payload are changes
+            const uint4 s0 = s_snap[0 * BLOCK + tid], s1 = s_snap[1 * BLOCK + tid];
+            const uint4 s2 = s_snap[2 * BLOCK + tid], s3 = s_snap[3 * BLOCK + tid];
+            const uint32_t sa = reinterpret_cast<const uint32_t*>(s_snap + 4 * BLOCK)[tid];
+            uint32_t d = dirty;
+            auto note = [&](uint32_t q, uint32_t a0, uint32_t a1, uint32_t b0, uint32_t b1) {
+                d |= ((a0 ^ b0) | (a1 ^ b1)) != 0u ? 1u << q : 0u;
+            };
+            note(0, tr[0][0], tr[0][1], s0.x, s0.y); note(1, tr[1][0], tr[1][1], s0.z, s0.w);
+            note(2, tr[2][0], tr[2][1], s1.x, s1.y); note(3, vl[0][0], vl[0][1], s1.z, s1.w);
+            note(4, vl[1][0], vl[1][1], s2.x, s2.y); note(5, vl[2][0], vl[2][1], s2.z, s2.w);
+            note(6, tl[0][0], tl[0][1], s3.x, s3.y); note(7, tl[1][0], tl[1][1], s3.z, s3.w);
+            if (alive != sa) d |= kAlivePlaneBit;
+            d = __reduce_or_sync(0xffffffffu, d);
             dirty = 0;
+            if (d) put_snapshot(alive);  // else the registers equal it already
             if (stamp_lane && (((d >> lane) & 1u) || st == 0u)) st = fresh;
             return stamp_lane ? __ldcg(seg_stamps + size_t(img_idx) * p.stamp_image) : st;
         };
@@ -716,20 +747,8 @@ __global__ void __launch_bounds__(256, 3) k_particles_program(const __grid_const
             const uint32_t kind = p.ops[i].kind;
             if (kind == OP_ADVANCE) {  // budget: advance
                 const float dt = __uint_as_float(p.ops[i].dt_bits);
-                const uint32_t alive_before = alive;
-                // bits, not values: -0.0 -> +0.0 and a changed NaN payload are changes.  chg[q] ORs the changed bits of
-                // plane q over the thread's rows (one LOP3 per row and plane); each plane is tested against zero once per
-                // Advance, not once per row.
-                uint32_t chg[8] = {0, 0, 0, 0, 0, 0, 0, 0};
 #pragma unroll
                 for (int j = 0; j < VEC; ++j) {
-                    const uint32_t o0 = tr[0][j], o1 = tr[1][j], o2 = tr[2][j], o3 = vl[0][j], o4 = vl[1][j], o5 = vl[2][j];
-                    const uint32_t o6 = tl[0][j], o7 = tl[1][j];
-                    auto note_changes = [&]() {
-                        chg[0] |= tr[0][j] ^ o0; chg[1] |= tr[1][j] ^ o1; chg[2] |= tr[2][j] ^ o2;
-                        chg[3] |= vl[0][j] ^ o3; chg[4] |= vl[1][j] ^ o4; chg[5] |= vl[2][j] ^ o5;
-                        chg[6] |= tl[0][j] ^ o6; chg[7] |= tl[1][j] ^ o7;
-                    };
                     if (OPT) {
                         // the queries only match entities that have the components (and exist)
                         const uint32_t m = (alive >> (8 * j)) & 0xFFu;
@@ -743,7 +762,6 @@ __global__ void __launch_bounds__(256, 3) k_particles_program(const __grid_const
                             tl[0][j] = lo; tl[1][j] = hi;
                             alive &= ((lo | hi) == 0u) ? ~(0xFFu << (8 * j)) : 0xFFFFFFFFu;
                         }
-                        if (STAMPS) note_changes();
                         continue;
                     }
                     particle_step(tr[0][j], tr[1][j], tr[2][j], vl[0][j], vl[1][j], vl[2][j], dt);
@@ -753,12 +771,6 @@ __global__ void __launch_bounds__(256, 3) k_particles_program(const __grid_const
                     lo -= 1u;
                     tl[0][j] = lo; tl[1][j] = hi;
                     alive &= ((lo | hi) == 0u) ? ~(0xFFu << (8 * j)) : 0xFFFFFFFFu;
-                    if (STAMPS) note_changes();
-                }
-                if (STAMPS) {
-#pragma unroll
-                    for (int q = 0; q < 8; ++q) dirty |= chg[q] != 0u ? 1u << q : 0u;
-                    if (alive != alive_before) dirty |= kAlivePlaneBit;
                 }
                 if (p.ops[i].flags & OPF_SPAWN) {
                     // spawn_particles (particles.rs:258-270): Commands are applied after the schedule, so the
@@ -779,11 +791,11 @@ __global__ void __launch_bounds__(256, 3) k_particles_program(const __grid_const
                 }
             } else if (kind == OP_SAVE) {  // budget: save_store
                 uint8_t* img = p.arena + (size_t(p.ops[i].image_off256) << 8);
-                // a held Save stores nothing and claims no stamp: `dirty` keeps collecting until the next stored Save,
+                // a held Save stores nothing and claims no stamp: the snapshot and `st` stay at the last stamp point,
                 // and the target's stamps still name its bytes
                 const bool store = !(p.ops[i].flags & (OPF_NO_STORE | OPF_HELD));
-                const uint32_t held = store ? claim_stamps(p.ops[i].call_count, p.stamp_base + i) : 0u;
-                if (store && !STAMPS) store_active(img, p.ops[i].call_count, held);  // nothing to wait for: issue the stores first
+                const uint32_t held = store ? claim_stamps(p.ops[i].call_count, p.stamp_base + i) : 0u;  // budget: save_track
+                if (store && !STAMPS) store_active(img, p.ops[i].call_count, held);  // nothing to wait for: issue the stores first  budget: save_store
                 if (VERIFY && (p.ops[i].flags & OPF_HELD)) check_held(img, p.ops[i].n_rows);
                 // ---- checksum partials (component_checksum.rs:81-90) ----  budget: save_hash
                 uint64_t hx_t = 0, hx_v = 0;

@@ -35,7 +35,7 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 CSRC = os.path.join(ROOT, "bevy_ggrs_b200", "csrc")
 KERNELS = os.path.join(CSRC, "kernels.cuh")
 KERNEL = "k_particles_program"
-REGIONS = ["prologue", "tile_loop", "load", "advance", "save_store", "save_hash", "save_fold", "epilogue"]
+REGIONS = ["prologue", "tile_loop", "load", "advance", "save_track", "save_store", "save_hash", "save_fold", "epilogue"]
 PIPES = ["imad", "alu", "fp32", "other"]
 ALU = {"LOP3", "LOP", "SHF", "SHL", "SHR", "IADD3", "IADD", "ISETP", "SEL", "PLOP3", "LEA", "VIADD", "VIADDMNMX",
        "VIMNMX", "IMNMX", "IABS", "PRMT", "MOV", "P2R", "R2P", "POPC", "FLO", "BMSK", "BREV", "ICMP", "ISCADD", "SGXT"}
