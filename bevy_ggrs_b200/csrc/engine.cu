@@ -935,11 +935,9 @@ int run_stepwise(bgr_engine* e, const Program& pg, uint32_t buf) {
         default: break;
         }
         if (op.kind == OP_ADVANCE && (op.flags & OPF_SPAWN)) {
-            const SystemReg& sy = e->systems[size_t(e->spawn_sys)];
-            const uint64_t ttl = sy.params[1];
             k_sys_particles_spawn<<<e->grid_for(op.save_index, 256), 256, 0, e->stream>>>(
-                live, e->words, e->cols[sy.cols[0]].first_plane, e->cols[sy.cols[1]].first_plane, e->cols[sy.cols[2]].first_plane,
-                op.image_off256, op.save_index, e->spawn[buf].dev() + op.call_count, uint32_t(ttl), uint32_t(ttl >> 32));
+                live, e->words, e->sys_specs[size_t(e->spawn_sys)], op.image_off256, op.save_index, e->spawn[buf].dev() + op.call_count,
+                e->systems[size_t(e->spawn_sys)].params[1]);
             e->launches += 1;
             live_rows = std::max(live_rows, op.image_off256 + op.save_index);
         }
@@ -981,6 +979,9 @@ void build_specs(bgr_engine* e) {
         case BGR_SYS_PARTICLES_DESPAWN: despawns = true; break;
         case BGR_SYS_PARTICLES_UPDATE:
         case BGR_SYS_BOX_MOVE: sp.plane1 = e->cols[sy.cols[1]].first_plane; break;
+        // Transform, Velocity and Ttl: what spawn_row writes.  The spec is part of the registration (a batch compares it);
+        // rate, ttl and seed are not, and reach the kernels through the ops and parameter blocks.
+        case BGR_SYS_PARTICLES_SPAWN: sp.plane1 = e->cols[sy.cols[1]].first_plane; sp.param = e->cols[sy.cols[2]].first_plane; break;
         default: break;
         }
         e->sys_specs.push_back(sp);
@@ -1072,6 +1073,8 @@ JitWorld launch_record(const bgr_engine* e, const Program& pg, uint32_t buf) {
     w.n_ops = pg.n_ops; w.n_saves = pg.n_saves;
     w.n_tiles = std::max(1u, e->tiles_for(pg.max_rows));
     w.live_rows = pg.live_rows;
+    w.spawn_vals = e->spawn[buf].dev();  // compile_requests' draws, copied in by submit / the batch
+    if (e->spawn_sys >= 0) w.spawn_ttl = e->systems[size_t(e->spawn_sys)].params[1];
     if (!pg.first_is_load) w.flags |= PF_READ_LIVE;
     if ((pg.has_load || pg.has_advance) && !pg.defer_live) w.flags |= PF_WRITE_LIVE_ACTIVE;
     return w;
@@ -1089,6 +1092,8 @@ int run_generic(bgr_engine* e, const Program& pg, uint32_t buf) {
     gp.ticket = w.ticket;
     gp.out = w.out;
     gp.seq = w.seq;
+    gp.spawn_vals = w.spawn_vals;
+    gp.spawn_ttl = w.spawn_ttl;
     if (e->trace.get() && !pg.internal && e->seq - e->trace_first_seq < e->trace_cap) gp.trace = e->trace.get() + (e->seq - e->trace_first_seq) * 4;
     gp.words = e->words; gp.tile_bytes = e->tile_bytes;
     gp.n_ops = w.n_ops; gp.n_saves = w.n_saves;
@@ -2303,9 +2308,9 @@ BGR_API int bgr_build(bgr_engine* e) {
         for (int i = 0; i < bgr_engine::kBufs; ++i) CUDA_TRY(e->spawn[i].ensure(kMaxSpawnVals));
     build_specs(e);
     detect_bundles(e);
-    // generic one-launch program: every row system runs on its tile (run_system); spawning is a Command of the stepwise
-    // path; the parameter block holds kMaxGenericSys systems; the tile fits twice per SM
-    e->generic_ok = e->spawn_sys < 0 && e->sys_specs.size() <= size_t(kMaxGenericSys) && e->tile_bytes <= 100u * 1024u;
+    // generic one-launch program: every row system runs on its tile (run_system) and spawned rows are written after the
+    // frame's despawns (spawn_row); the parameter block holds kMaxGenericSys systems; the tile fits twice per SM
+    e->generic_ok = e->sys_specs.size() <= size_t(kMaxGenericSys) && e->tile_bytes <= 100u * 1024u;
     jit_specialise(e);
     {   // TMA copy kernel: up to six one-tile stages in ~200 KB of shared memory, at least two
         uint32_t st = uint32_t(std::min<size_t>((200u * 1024u) / e->tile_bytes, size_t(kTmaMaxStages)));
@@ -2352,9 +2357,8 @@ BGR_API int bgr_run_startup_system(bgr_engine* e, uint32_t system) {
         e->spawn[0].get()[k].y = e->st.rng.random_range(-200.0f, 200.0f);
     }
     const uint64_t ttl = sy.params[1];
-    k_sys_particles_spawn<<<e->grid_for(rate, 256), 256, 0, e->stream>>>(
-        e->image(0), e->words, e->cols[sy.cols[0]].first_plane, e->cols[sy.cols[1]].first_plane, e->cols[sy.cols[2]].first_plane,
-        e->st.n_rows, rate, e->spawn[0].dev(), uint32_t(ttl), uint32_t(ttl >> 32));
+    k_sys_particles_spawn<<<e->grid_for(rate, 256), 256, 0, e->stream>>>(e->image(0), e->words, e->sys_specs[size_t(e->spawn_sys)],
+                                                                         e->st.n_rows, rate, e->spawn[0].dev(), ttl);
     e->launches += 1;
     CUDA_TRY(cudaGetLastError());
     e->st.n_rows += rate;  // before clear_stamps: the fresh content id carries the new row count
@@ -3284,7 +3288,7 @@ BGR_API int bgr_batch_create(bgr_engine* const* engines, uint32_t n, bgr_batch**
             return fail(BGR_ERR_UNSUPPORTED, who + "sharded engines (BGR_CFG_SHARDED, shard groups) cannot be batched");
         if (!use_generic(e))
             return fail(BGR_ERR_UNSUPPORTED, who + "only engines that run the generic one-launch program can be batched (not the particles "
-                                                   "bundle, BGR_CFG_FORCE_STEPWISE or a spawn system)");
+                                                   "bundle or BGR_CFG_FORCE_STEPWISE)");
     }
     CUDA_TRY(cudaSetDevice(engines[0]->cfg.device));
     bgr_batch* b = new bgr_batch();
@@ -3373,6 +3377,27 @@ BGR_API int bgr_batch_handle_requests(bgr_batch* b, const uint32_t* worlds, uint
         return first;
     }
     if (n_worlds == 0) return BGR_OK;
+    // spawning worlds: growable members take the capacity their spawns need (a program does not depend on the capacity,
+    // submit), and each world's ParticleRng draws go to its result buffer's spawn values.  A vector past a member's
+    // ceiling is refused before any member grows.
+    for (uint32_t i = 0; i < n_worlds; ++i) {
+        const bgr_engine* e = b->engines[worlds[i]];
+        const uint64_t rows = b->prep[worlds[i]].pg.rows_needed;
+        if (rows > e->ceiling)
+            return world_fail(i, fail(BGR_ERR_CAPACITY, std::to_string(rows) + " rows exceed the engine's ceiling of " +
+                                                            std::to_string(e->ceiling) + " rows (BGR_CFG_GROWABLE)"));
+    }
+    for (uint32_t i = 0; i < n_worlds; ++i) {
+        const uint32_t w = worlds[i];
+        bgr_engine* e = b->engines[w];
+        const Program& pg = b->prep[w].pg;
+        if (pg.rows_needed) {
+            const int rc = grow_to(e, pg.rows_needed);
+            if (rc != BGR_OK) return world_fail(i, rc);
+        }
+        b->buf[w] = e->next_buf;
+        if (!pg.spawn_vals.empty()) std::memcpy(e->spawn[b->buf[w]].get(), pg.spawn_vals.data(), pg.spawn_vals.size() * sizeof(float2));
+    }
     // one record per world and the worlds' ops in page-locked staging, one copy, one launch
     uint8_t* h = b->h_stage.get();
     JitWorld* recs = reinterpret_cast<JitWorld*>(h);
@@ -3385,7 +3410,6 @@ BGR_API int bgr_batch_handle_requests(bgr_batch* b, const uint32_t* worlds, uint
         Prepared& p = b->prep[w];
         p.t_compiled = host_ns();
         e->tiledep_chain = false;
-        b->buf[w] = e->next_buf;
         const int rc = plan(e, p);  // a deferred live image this vector cannot start from is written here, before the launch
         if (rc != BGR_OK) return world_fail(i, rc);
         JitWorld r = launch_record(e, p.pg, b->buf[w]);

@@ -4,7 +4,8 @@
 //
 //     cp.async.bulk  slot/live image --> shared tile              (LOAD, or the program's first read)
 //     ADVANCE : every registered system updates its rows of the shared tile in place (a thread owns its rows for the
-//               whole program, so no barrier separates systems; despawn commands are applied after the last system)
+//               whole program, so no barrier separates systems; despawn commands are applied after the last system,
+//               then spawn_particles' newborn rows are written: a row is not updated in the frame it is born)
 //     SAVE    : cp.async.bulk shared tile --> the frame's slot, while all threads hash the checksummed byte ranges
 //               of their rows out of the same tile (component_checksum.rs:67-108) and count live rows
 //     end     : cp.async.bulk shared tile --> live image
@@ -45,6 +46,8 @@ struct GenericParams {
     unsigned int* ticket;       // [0] block-completion ticket, [1] dynamic tile counter
     unsigned long long seq;
     unsigned long long* trace;
+    const float2* spawn_vals;      // (vx, vy) of every row an OPF_SPAWN ADVANCE spawns (host-mapped; the op's call_count indexes it)
+    unsigned long long spawn_ttl;  // Ttl of a spawned row (spawn_particles' param)
     uint32_t words, tile_bytes, n_ops, n_saves, n_tiles, live_rows, flags, n_hash, n_sys;
     // overlap of consecutive launches (generated kernel only; the protocol of k_particles_program's PF_TILE_SIGNAL / PF_TILE_WAIT
     // per WORK ITEM): item_done[i] = sequence number of the last signalling launch whose stores of item i are visible
@@ -66,12 +69,14 @@ struct JitWorld {
     unsigned int* ticket;
     unsigned long long* out;
     unsigned long long seq;
+    const float2* spawn_vals;
+    unsigned long long spawn_ttl;
     uint32_t n_ops, n_saves, n_tiles, live_rows, flags;
     uint32_t item0;    // batched launch: the world's first block (sum of the item counts of the worlds before it)
     uint32_t ops_off;  // batched launch: index of the world's first op in the launch's op array
     uint32_t pad;
 };
-static_assert(sizeof(JitWorld) == 80, "JitWorld layout");
+static_assert(sizeof(JitWorld) == 96, "JitWorld layout");
 
 // seahash of bytes [off, off+len) of one row's element whose words are `col[w * kTileRows]` (a column of the shared tile)
 // (__noinline__: inlined per checksummed column and per row the interpreter grew to 11k instructions — 176 KB of code,
@@ -224,6 +229,19 @@ __global__ void __launch_bounds__(kGenericBlock) k_generic_program(const __grid_
 #pragma unroll
                 for (int k = 0; k < kRows; ++k)
                     if (kill[k]) s_alive[tid + k * kGenericBlock] = 0;
+                if (op.flags & OPF_SPAWN) {  // spawn_particles' Commands: rows [first, first + count) are born after the despawns
+                    uint32_t s = 0;
+                    while (p.sys[s].id != BGR_SYS_PARTICLES_SPAWN) ++s;  // OPF_SPAWN: the registration has the system (compile_requests)
+                    const SysSpec sy = p.sys[s];
+#pragma unroll
+                    for (int k = 0; k < kRows; ++k) {
+                        const uint32_t born = tile * kTileRows + tid + k * kGenericBlock - op.image_off256;  // index among the spawned rows
+                        if (born < op.save_index) {
+                            spawn_row(sy, word, k, p.words, p.spawn_vals[op.call_count + born], p.spawn_ttl);
+                            s_alive[tid + k * kGenericBlock] = 1;
+                        }
+                    }
+                }
             } else if (op.kind == OP_SAVE) {
                 // the bulk store streams the tile to the frame's slot while the threads hash their rows out of it
                 if (!(op.flags & OPF_NO_STORE)) store_tile(p.arena + (size_t(op.image_off256) << 8), tile);

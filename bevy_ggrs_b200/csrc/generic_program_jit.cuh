@@ -7,7 +7,8 @@
 // the particles bundle:
 //
 //     LOAD / first read : coalesced ld.global of the row's words, plane by plane, from the slot / live image
-//     ADVANCE           : the registered systems update the register copy (indices are constants: plain register ops)
+//     ADVANCE           : the registered systems update the register copy (indices are constants: plain register ops),
+//                         then the despawns, then spawn_particles' newborn rows (kernels.cuh spawn_row)
 //     SAVE              : coalesced st.global of the words to the frame's slot + the per-entity seahash of every
 //                         checksummed column, folded warp-REDUX -> shared atomics like the interpreter
 //     end               : st.global to the live image
@@ -35,6 +36,14 @@ constexpr int kJitNSys = BGR_JIT_NSYS;
 constexpr int kJitNHash = BGR_JIT_NHASH;
 constexpr SysSpec kJitSys[kJitNSys + 1] = {BGR_JIT_SYS_LIST};      // {id, plane0, plane1, need, param}, ... + one dummy
 constexpr HashSpec kJitHash[kJitNHash + 1] = {BGR_JIT_HASH_LIST};  // {first_plane, off, len, finite, slot, absent}, ... + one dummy
+
+// index of spawn_particles in kJitSys, or -1: a registration without it compiles no spawn code at all
+__host__ __device__ constexpr int jit_spawn_index() {
+    for (int s = 0; s < kJitNSys; ++s)
+        if (kJitSys[s].id == BGR_SYS_PARTICLES_SPAWN) return s;
+    return -1;
+}
+constexpr int kJitSpawn = jit_spawn_index();
 
 // seahash of the NWORDS whole words at planes [F, F + NWORDS) of a row: the stream form of seahash.cuh with the lane
 // rotation done by renaming (word pair q goes to lane q % 4, the odd tail word to the next lane)
@@ -94,10 +103,11 @@ __device__ __forceinline__ void jit_hash_columns(const JitRows& r, unsigned int*
 // One work item of a request vector: the rows' first read from `first_img`, the vector's ops (LOAD, ADVANCE, SAVE with its
 // hash into the save's shared accumulators `s_acc`) and the live store.  The one definition of what an op does on the
 // generated kernel: k_generic_jit and k_generic_jit_batch both run it.  `op_at(i)` is op i of the vector.
+// `spawn_vals` / `spawn_ttl`: what an OPF_SPAWN ADVANCE writes into its newborn rows (GenericParams).
 template <class OpAt>
 __device__ __forceinline__ void jit_run_item(uint8_t* arena, unsigned long long order_base, uint32_t flags, uint32_t n_ops, OpAt op_at,
                                              const uint8_t* first_img, uint32_t first_rows, uint32_t item, unsigned int* s_acc,
-                                             uint32_t tid, uint32_t lane) {
+                                             uint32_t tid, uint32_t lane, const float2* spawn_vals, unsigned long long spawn_ttl) {
     constexpr int B = kJitItemRows / kJitRows;  // threads per work item
     constexpr uint32_t kTileBytes = kTileRows * (4u * kJitWords + 1u);
     constexpr uint32_t kAliveOff = uint32_t(kJitWords) * kPlaneBytes;  // the mask bytes follow the word planes inside a tile
@@ -139,6 +149,20 @@ __device__ __forceinline__ void jit_run_item(uint8_t* arena, unsigned long long 
             jit_run_systems<0>(r, op, row0, B);
 #pragma unroll
             for (int k = 0; k < kJitRows; ++k) r.m[k] = r.kill[k] ? 0u : r.m[k];  // despawn commands: after the last system
+            if constexpr (kJitSpawn >= 0) {
+                if (op.flags & OPF_SPAWN) {  // spawn_particles' Commands: rows [first, first + count) are born after the despawns
+                    constexpr SysSpec sy = kJitSys[kJitSpawn];
+#pragma unroll
+                    for (int k = 0; k < kJitRows; ++k) {
+                        const uint32_t born = tile * kTileRows + sub_row0 + k * B - op.image_off256;  // index among the spawned rows
+                        if (born < op.save_index) {
+                            spawn_row(sy, [&](int kk, uint32_t plane) -> uint32_t& { return r.w[kk][plane]; }, k, kJitWords,
+                                      spawn_vals[op.call_count + born], spawn_ttl);
+                            r.m[k] = 1u;
+                        }
+                    }
+                }
+            }
         } else if (op.kind == OP_SAVE) {
             if (!(op.flags & OPF_NO_STORE)) store(arena + (size_t(op.image_off256) << 8));
             uint32_t n_alive = 0, bad = 0;
@@ -227,7 +251,7 @@ extern "C" __global__ void __launch_bounds__(BGR_JIT_ITEM_ROWS / BGR_JIT_ROWS, B
         __syncthreads();
         const uint32_t next_item = s_next;
         jit_run_item(p.arena, p.order_base, p.flags, p.n_ops, [&](uint32_t i) -> const Op& { return p.ops[i]; }, first_img, first_rows,
-                     item, s_acc, tid, lane);
+                     item, s_acc, tid, lane, p.spawn_vals, p.spawn_ttl);
         if (signal_items) {  // every thread's stores of this item are visible at gpu scope, then one release store announces it
             __threadfence();
             __syncthreads();
@@ -264,7 +288,7 @@ extern "C" __global__ void __launch_bounds__(BGR_JIT_ITEM_ROWS / BGR_JIT_ROWS, B
     const uint8_t* first_img = w.arena + ((w.flags & PF_READ_LIVE) ? size_t(0) : (size_t(wops[0].image_off256) << 8));
     const uint32_t first_rows = (w.flags & PF_READ_LIVE) ? w.live_rows : wops[0].n_rows;
     jit_run_item(w.arena, w.order_base, w.flags, w.n_ops, [&](uint32_t i) -> const Op& { return wops[i]; }, first_img, first_rows,
-                 blockIdx.x - w.item0, s_acc, tid, lane);
+                 blockIdx.x - w.item0, s_acc, tid, lane, w.spawn_vals, w.spawn_ttl);
     jit_fold_publish(w.accum, w.ticket, w.out, w.seq, w.n_saves, w.n_tiles * uint32_t(kJitSubs), s_acc, s_last, nullptr, tid);
 }
 

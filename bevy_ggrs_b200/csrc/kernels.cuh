@@ -414,6 +414,21 @@ __device__ __forceinline__ void run_system(const SysSpec& sy, Word&& word, const
     }
 }
 
+// THE definition of a row born to spawn_particles (particles.rs:258-270): row k's words become every registered word
+// zero, then Transform::default() (rotation.w and scale 1), Velocity(vx, vy, 0) and Ttl(ttl).  `sy` is the spawn
+// system's spec: plane0 = Transform, plane1 = Velocity, param = Ttl (build_specs).  The caller sets the row's mask byte
+// to 1: alive, every optional column present.  The stepwise path (k_sys_particles_spawn), the interpreter and the
+// generated kernel write newborn rows through it; the bundle kernel keeps its own register layout.
+template <class Word>
+__device__ __forceinline__ void spawn_row(const SysSpec& sy, Word&& word, int k, uint32_t words, float2 v, unsigned long long ttl) {
+#pragma unroll
+    for (uint32_t j = 0; j < words; ++j) word(k, j) = 0u;
+    word(k, sy.plane0 + 6) = 0x3f800000u;  // rotation.w = 1
+    word(k, sy.plane0 + 7) = 0x3f800000u; word(k, sy.plane0 + 8) = 0x3f800000u; word(k, sy.plane0 + 9) = 0x3f800000u;  // scale = 1
+    word(k, sy.plane1) = __float_as_uint(v.x); word(k, sy.plane1 + 1) = __float_as_uint(v.y);
+    word(k, sy.param) = uint32_t(ttl); word(k, sy.param + 1) = uint32_t(ttl >> 32);
+}
+
 // =============================================================================================
 // THE fused kernel: interprets the whole request vector (Load / Advance / Save ...) for the
 // particles bundle.  One launch per handle_requests; one tile (512 rows) per block iteration.
@@ -1130,22 +1145,14 @@ __global__ void __launch_bounds__(256, 8) k_sys_rows(uint8_t* img, uint32_t word
     }
 }
 
-// spawn_particles (particles.rs:258-270) on the live image: rows [first, first+count) become
-// Transform::default(), Velocity(vx, vy, 0), Ttl(ttl), alive; every other registered word is zero.
-__global__ void __launch_bounds__(256) k_sys_particles_spawn(uint8_t* img, uint32_t words, uint32_t t_plane, uint32_t v_plane,
-                                                             uint32_t l_plane, uint32_t first, uint32_t count,
-                                                             const float2* __restrict__ vals, uint32_t ttl_lo, uint32_t ttl_hi) {
+// spawn_particles (particles.rs:258-270) on the live image: rows [first, first+count) become spawn_row's newborn rows
+// (`sy` the spawn system's spec), alive.
+__global__ void __launch_bounds__(256) k_sys_particles_spawn(uint8_t* img, uint32_t words, const SysSpec sy, uint32_t first, uint32_t count,
+                                                             const float2* __restrict__ vals, unsigned long long ttl) {
     for (uint32_t k = blockIdx.x * blockDim.x + threadIdx.x; k < count; k += gridDim.x * blockDim.x) {
         const uint32_t r = first + k;
-        for (uint32_t w = 0; w < words; ++w) *reinterpret_cast<uint32_t*>(img + word_offset(words, r, w)) = 0u;
-        uint32_t* t = reinterpret_cast<uint32_t*>(img + word_offset(words, r, t_plane));
-        t[6 * kTileRows] = 0x3f800000u;                                                          // rotation.w = 1
-        t[7 * kTileRows] = 0x3f800000u; t[8 * kTileRows] = 0x3f800000u; t[9 * kTileRows] = 0x3f800000u;  // scale = 1
-        uint32_t* v = reinterpret_cast<uint32_t*>(img + word_offset(words, r, v_plane));
-        const float2 xy = vals[k];
-        v[0] = __float_as_uint(xy.x); v[kTileRows] = __float_as_uint(xy.y);
-        uint32_t* l = reinterpret_cast<uint32_t*>(img + word_offset(words, r, l_plane));
-        l[0] = ttl_lo; l[kTileRows] = ttl_hi;
+        spawn_row(sy, [&](int, uint32_t plane) -> uint32_t& { return *reinterpret_cast<uint32_t*>(img + word_offset(words, r, plane)); },
+                  0, words, vals[k], ttl);
         img[alive_offset(words, r)] = 1;
     }
 }

@@ -98,7 +98,9 @@ typedef enum bgr_system {
      * (1 << 4) set, appends `rate` rows: Transform::default(), Velocity(random_range(-200..200) x2, 0), Ttl(ttl),
      * Rollback.  Draws from the ParticleRng resource (Xoshiro256PlusPlus::seed_from_u64(seed)), which the engine
      * keeps host-side and rolls back with every snapshot (rollback_resource_with_clone::<ParticleRng>, :200).
-     * Commands are deferred: the new rows exist from the end of the frame on and are not updated in it.
+     * Commands are deferred: the new rows exist from the end of the frame on and are not updated in it.  Every other
+     * registered word of a new row is zero and every optional column is present.  A spawning world ticks in one launch
+     * (the particles bundle, or the generic one-launch program for any other registration) and can be batched.
      * cols = {Transform(40B), Velocity(12B), Ttl(8B)}; params = {rate, ttl, seed_lo, seed_hi} */
     BGR_SYS_PARTICLES_SPAWN = 7,
     /* `if inputs[player].0 == value { commands.entity(e).despawn() }` for every entity that has component C — the
@@ -568,9 +570,10 @@ BGR_API int bgr_advance_world(bgr_engine* e, const uint8_t* inputs, const uint8_
                               uint32_t n_players);                             /* world.run_schedule(AdvanceWorld); caller bumps the frame count */
 
 /* ---- THE HOT LOOP: handle_requests (src/schedule_systems.rs:170-289) ------------------- */
-/* Executes the whole request vector; one fused kernel launch when the registered systems
- * match a compiled bundle, otherwise one launch per request.  Writes one bgr_checksum per
- * SaveGameState, in request order, host-visible on return. */
+/* Executes the whole request vector in one kernel launch: the particles bundle's kernel when the registered systems
+ * match it, otherwise the generic one-launch program (spawning worlds included).  Only BGR_CFG_FORCE_STEPWISE and
+ * registrations the generic program does not take (more than 8 systems, a 512-row tile over 100 KB) run one launch
+ * per request and per system.  Writes one bgr_checksum per SaveGameState, in request order, host-visible on return. */
 BGR_API int bgr_handle_requests(bgr_engine* e, const bgr_session_info* session,
                                 const bgr_request* requests, uint32_t n_requests,
                                 bgr_checksum* checksums_out, uint32_t checksums_cap, uint32_t* n_checksums_out);
@@ -596,10 +599,12 @@ BGR_API int bgr_fold_partials_n(const bgr_partial* combined, uint32_t n, bgr_che
 /* ---- world batches: the request vectors of many engines in ONE kernel launch ---------------------------------------
  * A batch is a fixed set of built engines ("worlds") with an identical registration (the same columns, presence flags,
  * checksums and systems in the same order), created on one device with the same non-null bgr_config.stream, that run
- * the generic one-launch program (not the particles bundle, BGR_CFG_FORCE_STEPWISE or a spawn system) and are not
- * sharded.  Capacity, max_depth, fps, row count, session kind, frame, BGR_CFG_DESYNC_CAPTURE, BGR_CFG_GROWABLE and
- * order_base may differ.  bgr_batch_create checks all of this and names the first engine that fails.  Destroy a batch
- * before any of its engines; between calls every per-engine entry point stays usable on the members. */
+ * the generic one-launch program (not the particles bundle or BGR_CFG_FORCE_STEPWISE) and are not sharded.
+ * Capacity, max_depth, fps, row count, session kind, frame, BGR_CFG_DESYNC_CAPTURE, BGR_CFG_GROWABLE and order_base
+ * may differ, and so may a BGR_SYS_PARTICLES_SPAWN system's rate, ttl and seed (its columns may not).  A spawn past a
+ * member's max_entities (or, BGR_CFG_GROWABLE, its ceiling) refuses the whole call; a growable member grows first.
+ * bgr_batch_create checks all of this and names the first engine that fails.  Destroy a batch before any of its
+ * engines; between calls every per-engine entry point stays usable on the members. */
 typedef struct bgr_batch bgr_batch;
 BGR_API int bgr_batch_create(bgr_engine* const* engines, uint32_t n, bgr_batch** out);
 BGR_API void bgr_batch_destroy(bgr_batch* b);
