@@ -69,6 +69,10 @@ BGR_KERNEL_STABLE_PLANES = 1 << 26
 BGR_KERNEL_HELD_SAVES = 1 << 27
 # ... and the vector ran inside a world batch's launch (bgr_batch_handle_requests)
 BGR_KERNEL_BATCHED = 1 << 28
+# ... and the last replay ran on the generated kernel's replay entry point (bgr_replay / bgr_batch_replay)
+BGR_KERNEL_REPLAY = 1 << 29
+# replays
+BGR_MAX_REPLAY_FRAMES = 1 << 24
 # change feed
 BGR_MAX_FEEDS = 8
 BGR_MAX_FEED_FIELDS = 8
@@ -133,6 +137,11 @@ class bgr_checkpoint_header(C.Structure):
                 ("rows", C.c_uint32), ("words", C.c_uint32), ("n_blocks", C.c_uint32), ("n_columns", C.c_uint32),
                 ("fps", C.c_uint32), ("active", C.c_uint64), ("elapsed_ns", C.c_uint64), ("rng", C.c_uint64 * 4),
                 ("digest_root", C.c_uint64), ("payload_bytes", C.c_uint64)]
+
+
+class bgr_replay(C.Structure):
+    _fields_ = [("n_frames", C.c_uint32), ("n_players", C.c_uint32), ("checksum_interval", C.c_uint32),
+                ("reserved", C.c_uint32), ("inputs", C.c_void_p)]
 
 
 class bgr_feed_field(C.Structure):
@@ -227,6 +236,9 @@ PROTOTYPES = {
     "bgr_batch_specialised": (C.c_int, [C.c_void_p, u32p]),
     "bgr_batch_handle_requests": (C.c_int, [C.c_void_p, u32p, C.c_uint32, C.POINTER(bgr_session_info), C.POINTER(bgr_request),
                                             u32p, C.POINTER(bgr_checksum), C.c_uint32, u32p, i32p]),
+    "bgr_replay": (C.c_int, [C.c_void_p, C.POINTER(bgr_replay), C.POINTER(bgr_checksum), C.c_uint32, u32p]),
+    "bgr_batch_replay": (C.c_int, [C.c_void_p, u32p, C.c_uint32, C.POINTER(bgr_replay), C.POINTER(bgr_checksum), C.c_uint32,
+                                   u32p, i32p]),
     "bgr_seahash": (C.c_uint64, [C.c_void_p, C.c_uint64]),
     "bgr_ggrs_time_delta_bits": (C.c_uint32, [C.c_uint32, C.c_int32]),
     "bgr_particle_rng_stream": (C.c_int, [C.c_uint64, C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p, C.c_float, C.c_float]),

@@ -16,6 +16,7 @@
 #include <cstdlib>
 #include <cstring>
 #include <deque>
+#include <memory>
 #include <string>
 #include <unordered_map>
 #include <vector>
@@ -67,6 +68,10 @@ struct SystemReg {
 constexpr uint32_t kReqAdvanceNoBump = 100;  // bgr_advance_world: caller already bumped RollbackFrameCount
 
 constexpr uint32_t kMaxSpawnVals = 1u << 16;  // particles spawned by one request vector
+
+// checksum points one replay launch accumulates (64 MB of accumulators); BGR_TUNE_REPLAY_POINTS lowers it (tests of logs
+// that take several launches)
+constexpr uint32_t kReplayLaunchPoints = 1u << 20;
 
 constexpr uint32_t kMaxDeferredOps = 4;  // trailing ADVANCEs a deferred live image replays (SyncTest / P2P ticks: 1)
 
@@ -376,6 +381,12 @@ struct bgr_engine {
     JitKernel jit_small;            // the same kernel with quarter-tile work items: worlds of few tiles per SM (optional)
     int tune_jit_tiledep = 0;       // 1: consecutive launches of the generated kernel overlap through per-item dependencies (queued submits)
     StridedRange item_done;         // [4 * tiles + 4] GenericParams::item_done (quarter-tile work items at most)
+    // replays (bgr_replay): the generated kernel of an engine that has none (compiled by its first replay; whole tiles and
+    // 128-row items), and the device copies of a call's logs, spawn tables, records and checksum accumulators
+    JitKernel replay_jit, replay_jit_small;
+    uint32_t tune_replay_points = 0;  // checksum points per replay launch (kReplayLaunchPoints unless BGR_TUNE_REPLAY_POINTS)
+    DeviceBuffer<uint8_t> replay_stage;
+    DeviceBuffer<unsigned long long> replay_acc;
     const void* jit_chain_kernel = nullptr;  // the signalling launch `tiledep_chain` refers to (its work-item partition must match)
     int tune_jit_item = 0;          // 0 auto (quarter tiles below 3 tiles per SM), 512 / 256 / 128 force the rows per work item
     int tune_passive_early = -1;    // -1: early passive stores for single-wave grids (auto); 0 never; 1 always
@@ -1418,11 +1429,9 @@ int commit(bgr_engine* e, const Prepared& p, uint32_t buf) {
     return BGR_OK;
 }
 
-int submit(bgr_engine* e, const bgr_session_info* sess, const bgr_request* reqs, uint32_t n) {
-    NvtxRange span("HandleRequests");
-    Prepared p;
-    int rc = prepare(e, sess, reqs, n, p);
-    if (rc != BGR_OK) return rc;  // nothing executed, nothing committed
+// submit() after prepare(): grows, launches the vector and commits it
+int execute(bgr_engine* e, Prepared& p) {
+    int rc = BGR_OK;
     const Program& pg = p.pg;
     // the program does not depend on the capacity: growing behind the compile leaves it (and its ParticleRng draws) valid
     if (pg.rows_needed) rc = grow_to(e, pg.rows_needed);
@@ -1445,6 +1454,14 @@ int submit(bgr_engine* e, const bgr_session_info* sess, const bgr_request* reqs,
     return commit(e, p, buf);
 }
 
+int submit(bgr_engine* e, const bgr_session_info* sess, const bgr_request* reqs, uint32_t n) {
+    NvtxRange span("HandleRequests");
+    Prepared p;
+    const int rc = prepare(e, sess, reqs, n, p);
+    if (rc != BGR_OK) return rc;  // nothing executed, nothing committed
+    return execute(e, p);
+}
+
 void fold(const bgr_partial& p, bgr_checksum* out) {
     // EntityChecksumPlugin::update (entity_checksum.rs:35-43)
     uint64_t x = sea_hash_2xu64(p.active, p.total);
@@ -1457,7 +1474,8 @@ void fold(const bgr_partial& p, bgr_checksum* out) {
     out->hi = 0;
 }
 
-int collect(bgr_engine* e, bgr_checksum* out, uint32_t cap, uint32_t* n_out) {
+// `bad_frame`: where the first Save whose finite assertion failed goes (left alone when none did)
+int collect(bgr_engine* e, bgr_checksum* out, uint32_t cap, uint32_t* n_out, int32_t* bad_frame = nullptr) {
     if (!e) return fail(BGR_ERR_INVALID_ARGUMENT, "null engine");
     if (e->pending.empty()) return fail(BGR_ERR_STATE, "nothing to collect");
     Pending pd = e->pending.front();
@@ -1519,6 +1537,7 @@ int collect(bgr_engine* e, bgr_checksum* out, uint32_t cap, uint32_t* n_out) {
         p.active = r[k * kAccStride + 6];
         p.total = pd.totals[k];
         for (uint32_t c = 0; c < e->n_ck; ++c) p.xor_[c] = r[k * kAccStride + c];
+        if ((r[k * kAccStride + 7] & 1ULL) && !nonfinite && bad_frame) *bad_frame = pd.frames[k];
         if (r[k * kAccStride + 7] & 1ULL) nonfinite = true;
         e->last_partials.push_back(p);
     }
@@ -2122,6 +2141,7 @@ BGR_API int bgr_engine_create(const bgr_config* cfg, bgr_engine** out) {
     e->tune_jit = env_int("BGR_TUNE_JIT", 1);
     e->tune_jit_rows = env_int("BGR_TUNE_JIT_ROWS", 4);
     e->tune_jit_item = env_int("BGR_TUNE_JIT_ITEM", 0);
+    e->tune_replay_points = uint32_t(std::max(1, env_int("BGR_TUNE_REPLAY_POINTS", int(kReplayLaunchPoints))));
     e->tune_jit_tiledep = env_int("BGR_TUNE_JIT_TILEDEP", 0);
     e->tune_passive_early = env_int("BGR_TUNE_PASSIVE_EARLY", -1);
     e->tune_stagger_ns = env_int("BGR_TUNE_STAGGER_NS", 800);
@@ -3440,6 +3460,427 @@ BGR_API int bgr_batch_handle_requests(bgr_batch* b, const uint32_t* worlds, uint
         const int rc = collect(b->engines[worlds[i]], out_at(), cap_at(), &n);
         collect_world(i, rc, n);
     }
+    if (first != BGR_OK) g_err = first_err;
+    return first;
+}
+
+// ---- replays: a recorded input log run through a world, checksummed at an interval, without snapshots ----
+namespace {
+
+
+// One world's replay, validated and planned against its engine's HostState: nothing has executed yet
+struct ReplayJob {
+    bgr_engine* e = nullptr;
+    const struct bgr_replay* r = nullptr;
+    ReplayClock c{};
+    std::vector<uint32_t> prefix;    // [n + 1]: spawn frames before each frame; empty without spawn_particles
+    std::vector<float2> spawn_vals;  // the log's ParticleRng draws, in frame order (what compile_requests draws)
+    ParticleRng rng;                 // ParticleRng after the log
+    uint64_t rows_end = 0, elapsed_end = 0;
+    uint32_t n_points = 0;
+    std::vector<bgr_checksum> sums;
+    bool bad = false;                // a checksum frame failed its finite assertion; the first is bad_frame
+    int32_t bad_frame = 0;
+};
+
+uint64_t ggrs_runtime_ns(const bgr_engine* e, int64_t frame) { return uint64_t(frame) * 1000000000ULL / uint64_t(e->cfg.fps); }
+// checksum frames f0 + j with j in [a, b): the first one (~0: none) and how many
+uint64_t first_point(const ReplayJob& job, uint32_t a, uint32_t b) { return replay_first_point(job.c.f0, job.r->checksum_interval, a, b); }
+uint32_t points_in(const ReplayJob& job, uint32_t a, uint32_t b) { return replay_points_in(job.c.f0, job.r->checksum_interval, a, b); }
+// spawn frames before frame j, and RollbackOrdered::len() there
+uint32_t prefix_at(const ReplayJob& job, uint32_t j) { return job.prefix.empty() ? 0u : job.prefix[j]; }
+uint32_t rows_at(const ReplayJob& job, uint32_t j) { return job.c.rows0 + job.c.rate * prefix_at(job, j); }
+
+// Validates a replay and computes everything the replay changes on the host, without executing or changing anything
+int replay_plan(bgr_engine* e, const struct bgr_replay* r, ReplayJob& job) {
+    if (!e) return fail(BGR_ERR_INVALID_ARGUMENT, "null engine");
+    if (!e->built) return fail(BGR_ERR_STATE, "bgr_build has not been called");
+    if (!r) return fail(BGR_ERR_INVALID_ARGUMENT, "null replay");
+    if ((e->cfg.flags & BGR_CFG_SHARDED) || e->group) return fail(BGR_ERR_UNSUPPORTED, "replays do not run on sharded engines");
+    if (!e->pending.empty()) return fail(BGR_ERR_STATE, "bgr_replay with un-collected bgr_submit_requests pending: call bgr_collect first");
+    if (r->reserved) return fail(BGR_ERR_INVALID_ARGUMENT, "bgr_replay.reserved must be 0");
+    if (r->n_players > BGR_MAX_PLAYERS) return fail(BGR_ERR_INVALID_ARGUMENT, "n_players > BGR_MAX_PLAYERS");
+    if (r->n_frames > BGR_MAX_REPLAY_FRAMES) return fail(BGR_ERR_INVALID_ARGUMENT, "n_frames > BGR_MAX_REPLAY_FRAMES");
+    if (r->n_frames && r->n_players && !r->inputs) return fail(BGR_ERR_INVALID_ARGUMENT, "null input log");
+    const HostState& s = e->st;
+    if (s.frame_count < 0) return fail(BGR_ERR_STATE, "a replay starts at RollbackFrameCount >= 0");
+    if (int64_t(s.frame_count) + r->n_frames > int64_t(INT32_MAX)) return fail(BGR_ERR_INVALID_ARGUMENT, "RollbackFrameCount + n_frames overflows i32");
+    const uint32_t n = r->n_frames;
+    // GgrsTimePlugin::update of the first step (compile_requests)
+    if (n && ggrs_runtime_ns(e, int64_t(s.frame_count) + 1) < s.elapsed_ns)
+        return fail(BGR_ERR_STATE, "tried to move Time<GgrsTime> backwards (RollbackFrameCount went back without LoadWorld)");
+    job = ReplayJob{};
+    job.e = e; job.r = r;
+    uint32_t n_counter = 0;
+    for (const SystemReg& sy : e->systems) n_counter += (sy.id == BGR_SYS_U32_STORE_CALL_COUNT);
+    const bool spawn = e->spawn_sys >= 0;
+    job.c = replay_clock(s.frame_count, e->cfg.fps, n ? s.elapsed_ns : 0u, r->n_players, s.call_count, n_counter, spawn,
+                         spawn ? e->systems[size_t(e->spawn_sys)].params[0] : 0u, s.n_rows);
+    const ReplayClock& c = job.c;
+    job.rng = s.rng;
+    job.rows_end = s.n_rows;
+    if (spawn) {  // spawn_particles.run_if(spawn_pressed)
+        job.prefix.assign(size_t(n) + 1, 0u);
+        uint32_t spawns = 0;
+        for (uint32_t j = 0; j < n; ++j) {
+            job.prefix[j] = spawns;
+            bool pressed = false;
+            for (uint32_t k = 0; k < r->n_players; ++k) pressed = pressed || (r->inputs[size_t(j) * r->n_players + k] & BGR_INPUT_SPAWN);
+            spawns += pressed ? 1u : 0u;
+        }
+        job.prefix[n] = spawns;
+        if (spawns && c.rate > kMaxSpawnVals) return fail(BGR_ERR_CAPACITY, "too many particles spawned by one request vector");
+        job.rows_end = uint64_t(s.n_rows) + uint64_t(c.rate) * spawns;
+        if (job.rows_end > e->cfg.max_entities) {
+            if (!e->growable()) return fail(BGR_ERR_CAPACITY, "spawn_particles exceeds max_entities");
+            if (job.rows_end > e->ceiling)
+                return fail(BGR_ERR_CAPACITY, std::to_string(job.rows_end) + " rows exceed the engine's ceiling of " +
+                                                  std::to_string(e->ceiling) + " rows (BGR_CFG_GROWABLE)");
+        }
+        job.spawn_vals.reserve(size_t(c.rate) * spawns);
+        for (uint32_t i = 0; i < spawns; ++i)
+            for (uint32_t k = 0; k < c.rate; ++k) {  // particles.rs:262-268, in frame order
+                float2 v;
+                v.x = job.rng.random_range(-200.0f, 200.0f);
+                v.y = job.rng.random_range(-200.0f, 200.0f);
+                job.spawn_vals.push_back(v);
+            }
+    }
+    job.elapsed_end = n ? ggrs_runtime_ns(e, int64_t(c.f0) + n) : s.elapsed_ns;
+    job.n_points = points_in(job, 0, n);
+    return BGR_OK;
+}
+
+// The replay in chunks through the engine's own kernel: each chunk is one request vector of at most kMaxOps ops,
+// kMaxSaves Saves and kMaxSpawnVals spawned rows, compiled by compile_requests, whose checksum points are Saves that
+// store nothing (OPF_NO_STORE) and push nothing onto the ring
+int replay_chunked(ReplayJob& job) {
+    bgr_engine* e = job.e;
+    const struct bgr_replay* r = job.r;
+    const uint32_t n = r->n_frames, k = r->checksum_interval;
+    std::vector<bgr_request> reqs(kMaxOps);
+    Prepared p;
+    Program adv;
+    for (uint32_t j = 0; j < n;) {
+        uint32_t b = j, ops = 0, saves = 0, spawned = 0;
+        while (b < n) {
+            const uint32_t pt = (k && (int64_t(job.c.f0) + b) % k == 0) ? 1u : 0u;
+            const uint32_t sp = prefix_at(job, b + 1) != prefix_at(job, b) ? job.c.rate : 0u;
+            if (ops + pt + 1 > uint32_t(kMaxOps) || saves + pt > uint32_t(kMaxSaves) || spawned + sp > kMaxSpawnVals) break;
+            ops += pt + 1; saves += pt; spawned += sp;
+            ++b;
+        }
+        for (uint32_t i = 0; i < b - j; ++i) {
+            bgr_request& rq = reqs[i];
+            std::memset(&rq, 0, sizeof rq);
+            rq.kind = BGR_REQ_ADVANCE;
+            rq.n_players = r->n_players;
+            for (uint32_t h = 0; h < r->n_players; ++h) rq.inputs[h] = r->inputs[size_t(j + i) * r->n_players + h];
+        }
+        p.t_begin = host_ns();
+        p.s = e->st;
+        p.next = DeferredLive{};
+        adv.~Program();
+        new (&adv) Program;
+        int rc = compile_requests(e, p.s, nullptr, reqs.data(), b - j, adv);
+        if (rc != BGR_OK) return rc;
+        p.pg.~Program();
+        new (&p.pg) Program;
+        Program& pg = p.pg;
+        pg.live_rows = adv.live_rows; pg.max_rows = adv.max_rows; pg.rows_needed = adv.rows_needed;
+        pg.has_advance = adv.has_advance; pg.has_spawn = adv.has_spawn;
+        pg.spawn_vals = std::move(adv.spawn_vals);
+        for (uint32_t i = 0; i < b - j; ++i) {
+            const int64_t frame = int64_t(job.c.f0) + j + i;
+            if (k && frame % k == 0) {  // SaveGameState{frame}: the checksum only
+                Op& sv = pg.ops[pg.n_ops++];
+                std::memset(&sv, 0, sizeof sv);
+                sv.kind = OP_SAVE; sv.flags = OPF_NO_STORE;
+                sv.n_rows = adv.ops[i].n_rows;
+                sv.save_index = pg.n_saves;
+                pg.save_frames[pg.n_saves] = int32_t(frame);
+                pg.save_totals[pg.n_saves] = sv.n_rows;
+                ++pg.n_saves;
+            }
+            pg.ops[pg.n_ops++] = adv.ops[i];
+        }
+        rc = execute(e, p);
+        if (rc != BGR_OK) return rc;
+        bgr_checksum sums[kMaxSaves];
+        uint32_t got = 0;
+        int32_t bad_frame = 0;
+        rc = collect(e, sums, kMaxSaves, &got, &bad_frame);
+        if (rc == BGR_ERR_NON_FINITE) {
+            if (!job.bad) { job.bad = true; job.bad_frame = bad_frame; }
+        } else if (rc != BGR_OK) {
+            return rc;
+        }
+        job.sums.insert(job.sums.end(), sums, sums + got);
+        j = b;
+    }
+    return BGR_OK;
+}
+
+// The generated kernel's replay entry point for an engine whose rows end up in `tiles` tiles: its own kernel when bgr_build
+// compiled one (the instance run_generic picks), else one compiled now.  nullptr: the replay runs in chunks.
+const JitKernel* replay_kernel(bgr_engine* e, uint32_t tiles) {
+    // the registrations jit_specialise takes: an engine that ticks on the stepwise path (more than kMaxGenericSys
+    // systems, a tile over the generic program's limit) replays through it too
+    if (!e->generic_ok || e->tune_jit == 0 || !e->tune_generic || (e->cfg.flags & BGR_CFG_FORCE_STEPWISE) || jit_unsupported(e))
+        return nullptr;
+    const bool few = tiles < 3u * uint32_t(e->num_sms);  // few tiles per SM: 128-row work items (run_generic)
+    if (e->jit.fn) {
+        const JitKernel& k = (e->jit_small.fn && few) ? e->jit_small : e->jit;
+        return k.replay_fn ? &k : nullptr;
+    }
+    const int forced = jit_forced_item(e);
+    JitKernel& k = (few && !forced) ? e->replay_jit_small : e->replay_jit;
+    if (!k.fn) {
+        const int item = forced ? forced : few ? 128 : int(kTileRows);
+        const int rows = forced ? std::min(jit_rows(e), forced / 32) : few ? 2 : jit_rows(e);
+        std::string why;
+        if (!jit_compile(e, item, rows, &k, &why)) {
+            k = JitKernel{};
+            if (std::getenv("BGR_JIT_VERBOSE"))
+                std::fprintf(stderr, "[bevy_ggrs_b200] replay kernel not compiled, the replay runs in chunks: %s\n", why.c_str());
+            return nullptr;
+        }
+    }
+    return k.replay_fn ? &k : nullptr;
+}
+
+size_t align16(size_t v) { return (v + 15u) & ~size_t(15); }
+
+// The replays of `jobs` (every one with frames to run) on the replay entry point of `k`: the logs, spawn tables and spawn
+// values go to the device once, then each launch runs every unfinished world through its next frames, as many as keep
+// the launch's checksum points within kReplayLaunchPoints (one launch for everything but very long logs at short
+// intervals), and its checksum points come back with one copy.  Synchronous.
+int replay_launch(const JitKernel& k, const std::vector<ReplayJob*>& jobs, uint32_t kernel_bits) {
+    bgr_engine* e0 = jobs[0]->e;
+    cudaStream_t stream = e0->stream;
+    const size_t rec_bytes = align16(sizeof(ReplayWorld) * jobs.size());
+    std::vector<size_t> in_off(jobs.size()), pre_off(jobs.size()), val_off(jobs.size());
+    size_t bytes = rec_bytes;
+    for (size_t i = 0; i < jobs.size(); ++i) {
+        const ReplayJob& j = *jobs[i];
+        in_off[i] = bytes; bytes = align16(bytes + size_t(j.r->n_frames) * j.r->n_players);
+        pre_off[i] = bytes; bytes = align16(bytes + j.prefix.size() * sizeof(uint32_t));
+        val_off[i] = bytes; bytes = align16(bytes + j.spawn_vals.size() * sizeof(float2));
+    }
+    CUDA_TRY(e0->replay_stage.ensure(bytes));
+    uint8_t* d = e0->replay_stage.get();
+    // one copy: a copy per world from pageable memory cost more host time than a world's whole replay kernel (the
+    // staging is not zeroed: alignment padding is never read)
+    std::unique_ptr<uint8_t[]> h(new uint8_t[bytes - rec_bytes]);
+    for (size_t i = 0; i < jobs.size(); ++i) {
+        const ReplayJob& j = *jobs[i];
+        if (j.r->n_players) std::memcpy(&h[in_off[i] - rec_bytes], j.r->inputs, size_t(j.r->n_frames) * j.r->n_players);
+        if (!j.prefix.empty()) std::memcpy(&h[pre_off[i] - rec_bytes], j.prefix.data(), j.prefix.size() * sizeof(uint32_t));
+        if (!j.spawn_vals.empty()) std::memcpy(&h[val_off[i] - rec_bytes], j.spawn_vals.data(), j.spawn_vals.size() * sizeof(float2));
+    }
+    CUDA_TRY(cudaMemcpyAsync(d + rec_bytes, h.get(), bytes - rec_bytes, cudaMemcpyHostToDevice, stream));
+    for (ReplayJob* j : jobs) {  // image 0 is read: a pending deferred live image is written first
+        int rc = materialize_live(j->e);
+        if (rc != BGR_OK) return rc;
+        j->e->tiledep_chain = false;
+    }
+    const uint32_t subs = kTileRows / uint32_t(k.item_rows);
+    std::vector<uint32_t> cur(jobs.size(), 0u), seg_end(jobs.size()), seg_points(jobs.size());
+    std::vector<ReplayWorld> recs;
+    std::vector<size_t> rec_job, acc_off;
+    std::vector<unsigned long long> acc;
+    for (;;) {
+        recs.clear(); rec_job.clear(); acc_off.clear();
+        uint32_t active = 0;
+        for (size_t i = 0; i < jobs.size(); ++i) active += cur[i] < jobs[i]->r->n_frames ? 1u : 0u;
+        if (!active) break;
+        const uint32_t budget = std::max(1u, e0->tune_replay_points / active);
+        uint32_t items = 0;
+        size_t points = 0;
+        for (size_t i = 0; i < jobs.size(); ++i) {
+            const ReplayJob& job = *jobs[i];
+            bgr_engine* e = job.e;
+            const uint32_t n = job.r->n_frames, a = cur[i], kk = job.r->checksum_interval;
+            if (a >= n) continue;
+            uint32_t b = n;
+            const uint64_t f = first_point(job, a, n);
+            if (f != ~0ULL && f + uint64_t(budget) * kk < n) b = uint32_t(f + uint64_t(budget) * kk);  // `budget` points
+            seg_end[i] = b;
+            seg_points[i] = points_in(job, a, b);
+            ReplayWorld w;
+            std::memset(&w, 0, sizeof w);
+            w.arena = e->arena.ptr();
+            w.order_base = e->cfg.order_base;
+            w.inputs = d + in_off[i];
+            w.prefix = job.prefix.empty() ? nullptr : reinterpret_cast<const uint32_t*>(d + pre_off[i]);
+            w.spawn_vals = reinterpret_cast<const float2*>(d + val_off[i]);
+            if (e->spawn_sys >= 0) w.spawn_ttl = e->systems[size_t(e->spawn_sys)].params[1];
+            w.next_point = first_point(job, a, b);
+            w.c = job.c;
+            w.interval = kk;
+            w.j0 = a; w.j1 = b;
+            w.live_rows = rows_at(job, a);
+            w.n_tiles = std::max(1u, e->tiles_for(rows_at(job, b)));
+            w.item0 = items;
+            items += w.n_tiles * subs;
+            acc_off.push_back(points);  // w.acc, once the buffer is sized (below)
+            points += seg_points[i];
+            recs.push_back(w);
+            rec_job.push_back(i);
+        }
+        CUDA_TRY(e0->replay_acc.ensure(std::max<size_t>(1, points) * kAccStride));
+        for (size_t ri = 0; ri < recs.size(); ++ri) recs[ri].acc = e0->replay_acc.get() + acc_off[ri] * kAccStride;
+        if (points) CUDA_TRY(cudaMemsetAsync(e0->replay_acc.get(), 0, points * kAccStride * sizeof(unsigned long long), stream));
+        CUDA_TRY(cudaMemcpyAsync(d, recs.data(), sizeof(ReplayWorld) * recs.size(), cudaMemcpyHostToDevice, stream));
+        const ReplayWorld* d_recs = reinterpret_cast<const ReplayWorld*>(d);
+        uint32_t n_recs = uint32_t(recs.size());
+        void* args[] = {&d_recs, &n_recs};
+        CUDA_TRY(cudaLaunchKernel(k.replay_fn, dim3(items), dim3(k.threads), args, 0, stream));
+        CUDA_TRY(cudaGetLastError());
+        acc.resize(points * kAccStride);
+        if (points) CUDA_TRY(cudaMemcpyAsync(acc.data(), e0->replay_acc.get(), points * kAccStride * sizeof(unsigned long long), cudaMemcpyDeviceToHost, stream));
+        CUDA_TRY(cudaStreamSynchronize(stream));
+        // each checksum point through the fold bgr_handle_requests uses
+        size_t off = 0;
+        for (size_t ri = 0; ri < recs.size(); ++ri) {
+            const size_t i = rec_job[ri];
+            ReplayJob& job = *jobs[i];
+            job.e->launches += 1;
+            const uint64_t f = first_point(job, cur[i], seg_end[i]);
+            for (uint32_t q = 0; q < seg_points[i]; ++q, ++off) {
+                const unsigned long long* a = &acc[off * kAccStride];
+                const uint32_t j = uint32_t(f + uint64_t(q) * job.r->checksum_interval);
+                bgr_partial part;
+                std::memset(&part, 0, sizeof part);
+                part.frame = int32_t(int64_t(job.c.f0) + j);
+                part.n_columns = job.e->n_ck;
+                part.active = a[6];
+                part.total = rows_at(job, j);
+                for (uint32_t col = 0; col < job.e->n_ck; ++col) part.xor_[col] = a[col];
+                if ((a[7] & 1ULL) && !job.bad) { job.bad = true; job.bad_frame = part.frame; }
+                bgr_checksum cs;
+                fold(part, &cs);
+                job.sums.push_back(cs);
+            }
+            cur[i] = seg_end[i];
+        }
+    }
+    for (ReplayJob* j : jobs) j->e->last_kernel = BGR_KERNEL_GENERIC_NVRTC | (uint32_t(k.item_rows) << 16) | kernel_bits;
+    return BGR_OK;
+}
+
+// After the replay ran on the generated kernel: the engine's host state moves to the end of the log.  Image 0 was written
+// outside the bundle kernel's bookkeeping, like a host write: a fresh passive version, a fresh content id, unknown stamps.
+int replay_commit(ReplayJob& job) {
+    bgr_engine* e = job.e;
+    HostState& s = e->st;
+    const uint32_t n = job.r->n_frames;
+    s.frame_count = job.c.f0 + int32_t(n);
+    s.elapsed_ns = job.elapsed_end;
+    s.call_count = job.c.call0 + job.c.n_counter * n;
+    s.n_rows = uint32_t(job.rows_end);
+    s.rng = job.rng;
+    s.live_passive_ver = ++s.ver_counter;
+    e->ticked = true;
+    return clear_stamps(e, 0);
+}
+
+// Grows every growable engine its replay needs (each was checked against its ceiling when planned)
+int replay_grow(const std::vector<ReplayJob*>& jobs) {
+    for (ReplayJob* j : jobs)
+        if (j->rows_end > j->e->cfg.max_entities) {
+            const int rc = grow_to(j->e, j->rows_end);
+            if (rc != BGR_OK) return rc;
+        }
+    return BGR_OK;
+}
+
+// A planned replay of one engine: on the generated kernel when there is one, else in chunks
+int replay_run(ReplayJob& job) {
+    std::vector<ReplayJob*> one{&job};
+    int rc = replay_grow(one);
+    if (rc != BGR_OK || job.r->n_frames == 0) return rc;
+    const JitKernel* k = replay_kernel(job.e, std::max(1u, job.e->tiles_for(uint32_t(job.rows_end))));
+    if (!k) return replay_chunked(job);
+    rc = replay_launch(*k, one, BGR_KERNEL_REPLAY);
+    if (rc != BGR_OK) return rc;
+    return replay_commit(job);
+}
+
+// The checksums of a finished replay to caller memory and its status
+int replay_results(const ReplayJob& job, bgr_checksum* out, uint32_t cap, uint32_t* n_out) {
+    if (n_out) *n_out = uint32_t(job.sums.size());
+    if (out) std::copy(job.sums.begin(), job.sums.begin() + std::min<size_t>(cap, job.sums.size()), out);
+    if (job.bad)
+        return fail(BGR_ERR_NON_FINITE, "Hashing is not stable for NaN f32 values (first at the checksum of frame " +
+                                            std::to_string(job.bad_frame) + ")");
+    return BGR_OK;
+}
+
+}  // namespace
+
+BGR_API int bgr_replay(bgr_engine* e, const struct bgr_replay* r, bgr_checksum* checksums_out, uint32_t cap, uint32_t* n_out) {
+    if (n_out) *n_out = 0;
+    NvtxRange span("Replay");
+    ReplayJob job;
+    int rc = replay_plan(e, r, job);
+    if (rc != BGR_OK) return rc;  // nothing executed, nothing changed
+    rc = replay_run(job);
+    if (rc != BGR_OK) return rc;
+    return replay_results(job, checksums_out, cap, n_out);
+}
+
+BGR_API int bgr_batch_replay(bgr_batch* b, const uint32_t* worlds, uint32_t n_worlds, const struct bgr_replay* replays,
+                             bgr_checksum* checksums_out, uint32_t cap, uint32_t* n_checksums_out, int32_t* status_out) {
+    if (!b) return fail(BGR_ERR_INVALID_ARGUMENT, "null batch");
+    if (n_worlds && (!worlds || !replays || !n_checksums_out || !status_out)) return fail(BGR_ERR_INVALID_ARGUMENT, "null argument");
+    NvtxRange span("Replay");
+    b->calls += 1;
+    for (uint32_t i = 0; i < n_worlds; ++i) { status_out[i] = BGR_OK; n_checksums_out[i] = 0; }
+    auto world_fail = [&](uint32_t i, int status) {
+        status_out[i] = status;
+        g_err = "world " + std::to_string(worlds[i]) + ": " + g_err;
+        return status;
+    };
+    // every world is validated and planned before any executes
+    std::vector<ReplayJob> jobs(n_worlds);
+    for (uint32_t i = 0; i < n_worlds; ++i) {
+        const uint32_t w = worlds[i];
+        if (w >= b->engines.size())
+            return world_fail(i, fail(BGR_ERR_INVALID_ARGUMENT, "no such world in a batch of " + std::to_string(b->engines.size())));
+        if (b->listed[w] == b->calls) return world_fail(i, fail(BGR_ERR_INVALID_ARGUMENT, "listed twice in one call"));
+        b->listed[w] = b->calls;
+        const int rc = replay_plan(b->engines[w], &replays[i], jobs[i]);
+        if (rc != BGR_OK) return world_fail(i, rc);
+    }
+    int first = BGR_OK;
+    std::string first_err;
+    uint32_t out_off = 0;
+    auto results = [&](uint32_t i, int rc) {
+        uint32_t n = 0;
+        bgr_checksum* out = checksums_out && out_off < cap ? checksums_out + out_off : nullptr;
+        if (rc == BGR_OK) rc = replay_results(jobs[i], out, out ? cap - out_off : 0u, &n);
+        n_checksums_out[i] = n;
+        out_off += std::min(n, cap - std::min(out_off, cap));
+        if (rc != BGR_OK) {
+            world_fail(i, rc);
+            if (first == BGR_OK) { first = rc; first_err = g_err; }
+        }
+    };
+    if (!b->k.replay_fn) {  // each world's own replay, in list order
+        for (uint32_t i = 0; i < n_worlds; ++i) results(i, replay_run(jobs[i]));
+        if (first != BGR_OK) g_err = first_err;
+        return first;
+    }
+    std::vector<ReplayJob*> run;
+    for (ReplayJob& j : jobs)
+        if (j.r->n_frames) run.push_back(&j);
+    int rc = replay_grow(run);
+    if (rc == BGR_OK && !run.empty()) rc = replay_launch(b->k, run, BGR_KERNEL_REPLAY | BGR_KERNEL_BATCHED);
+    for (ReplayJob* j : run)
+        if (rc == BGR_OK) rc = replay_commit(*j);
+    if (rc != BGR_OK) return rc;
+    for (uint32_t i = 0; i < n_worlds; ++i) results(i, BGR_OK);
     if (first != BGR_OK) g_err = first_err;
     return first;
 }

@@ -22,7 +22,9 @@
 #include "rtc_prelude.cuh"
 #else
 #include <cuda_runtime.h>
+#include <cmath>
 #include <cstdint>
+#include <cstring>
 #endif
 
 #include "kernels.cuh"
@@ -77,6 +79,111 @@ struct JitWorld {
     uint32_t pad;
 };
 static_assert(sizeof(JitWorld) == 96, "JitWorld layout");
+
+// ---- replays (bgr_replay): the ADVANCE op of frame j of an input log, derived from the frame index ----
+// What compile_requests builds for AdvanceFrame j of the stream, field by field, from values fixed before the log starts.
+// The host evaluates everything that needs the C library (powf) once; the rest is integer arithmetic.
+struct ReplayClock {
+    int32_t f0;               // RollbackFrameCount before frame 0
+    uint32_t fps;
+    uint32_t n_players;       // PlayerInputs<T>.len() of every frame
+    uint32_t dt0, fr0;        // the first step's (dt_bits, fr_bits): Time<GgrsTime> may have been set by a restore
+    uint32_t dt[2], fr[2];    // every later step lasts floor(1e9 / fps) ns ([0]) or one more ([1])
+    uint32_t call0;           // BGR_SYS_U32_STORE_CALL_COUNT counter before frame 0
+    uint32_t n_counter;       // counter systems: the counter grows by this per frame
+    uint32_t spawn;           // 1: the registration has spawn_particles (an INPUT_SPAWN frame sets OPF_SPAWN)
+    uint32_t rate;            // its rows per spawn frame
+    uint32_t rows0;           // RollbackOrdered::len() before frame 0
+};
+static_assert(sizeof(ReplayClock) == 56, "ReplayClock layout (the engine and the NVRTC module must agree)");
+
+#ifndef __CUDACC_RTC__
+// The clock of a log that starts at RollbackFrameCount f0 with Time<GgrsTime> at `elapsed_ns` (the caller has checked
+// that the first step does not move it backwards): each step's (dt_bits, fr_bits) as compile_requests evaluates them,
+// Duration::as_secs_f32 and the C library's powf (move_cube_system's friction, box_game.rs:188-193).  Host only.
+inline ReplayClock replay_clock(int32_t f0, uint32_t fps, uint64_t elapsed_ns, uint32_t n_players, uint32_t call0,
+                                uint32_t n_counter, bool spawn, uint32_t rate, uint32_t rows0) {
+    auto step = [](uint64_t ns, uint32_t* dt, uint32_t* fr) {
+        const float secs = float(ns / 1000000000ULL) + float(uint32_t(ns % 1000000000ULL)) / 1000000000.0f;
+        const float f = powf(0.0018f, secs);
+        std::memcpy(dt, &secs, 4);
+        std::memcpy(fr, &f, 4);
+    };
+    ReplayClock c;
+    std::memset(&c, 0, sizeof c);
+    c.f0 = f0; c.fps = fps; c.n_players = n_players; c.call0 = call0; c.n_counter = n_counter;
+    c.spawn = spawn ? 1u : 0u; c.rate = spawn ? rate : 0u; c.rows0 = rows0;
+    step(uint64_t(int64_t(f0) + 1) * 1000000000ULL / fps - elapsed_ns, &c.dt0, &c.fr0);
+    const uint64_t base = 1000000000ULL / fps;
+    step(base, &c.dt[0], &c.fr[0]);
+    step(base + 1, &c.dt[1], &c.fr[1]);
+    return c;
+}
+#endif
+
+// Checksum frames of a log that starts at f0, with interval k: the first frame index j in [a, b) with (f0 + j) % k == 0
+// (~0: none), and how many there are
+__host__ __device__ inline unsigned long long replay_first_point(int32_t f0, uint32_t k, uint32_t a, uint32_t b) {
+    if (!k) return ~0ULL;
+    const unsigned long long rem = (unsigned long long)(int64_t(f0) + a) % k;
+    const unsigned long long j = (unsigned long long)a + (rem ? k - rem : 0u);
+    return j < b ? j : ~0ULL;
+}
+__host__ __device__ inline uint32_t replay_points_in(int32_t f0, uint32_t k, uint32_t a, uint32_t b) {
+    const unsigned long long f = replay_first_point(f0, k, a, b);
+    return f == ~0ULL ? 0u : uint32_t((b - 1u - f) / k + 1u);
+}
+
+// `in`: the frame's n_players input bytes; `prefix`: the spawn frames before frame j
+__host__ __device__ inline Op replay_op(const ReplayClock& c, uint32_t j, const uint8_t* in, uint32_t prefix) {
+    Op op;
+    op.kind = OP_ADVANCE;
+    op.image_off256 = 0; op.save_index = 0;
+    if (j == 0) {
+        op.dt_bits = c.dt0; op.fr_bits = c.fr0;
+    } else {  // GgrsTimePlugin::update: advance_to(frame * 1e9 / fps), from frame f0 + j to f0 + j + 1
+        const unsigned long long f = (unsigned long long)(c.f0 + int32_t(j)), ns = 1000000000ULL;
+        const bool longer = (f + 1ULL) * ns / c.fps - f * ns / c.fps != ns / c.fps;
+        op.dt_bits = longer ? c.dt[1] : c.dt[0];  // selects, not an index: the clock stays in registers
+        op.fr_bits = longer ? c.fr[1] : c.fr[0];
+    }
+    op.n_rows = c.rows0 + c.rate * prefix;
+    op.call_count = c.call0 + c.n_counter * j;
+    op.flags = (c.n_players & 0xFu) << 8;
+    uint32_t pressed = 0;
+    for (uint32_t k = 0; k < 8u; ++k) {
+        const uint8_t v = k < c.n_players ? in[k] : uint8_t(0);
+        op.inputs[k] = v;
+        pressed |= v & 0x10u;  // BGR_INPUT_SPAWN
+    }
+    if (c.spawn && pressed) {  // spawn_particles' rows: first row, count, offset into the log's spawn values
+        op.flags |= OPF_SPAWN;
+        op.image_off256 = op.n_rows;
+        op.save_index = c.rate;
+        op.call_count = c.rate * prefix;
+    }
+    return op;
+}
+
+// One world's frames [j0, j1) of a replay on the generated kernel (k_generic_jit_replay, generic_program_jit.cuh).
+// Rows come from and go back to the live image.  The block's checksum points go to acc[point][kAccStride], point 0
+// being the first checksum frame at or after j0.
+struct ReplayWorld {
+    uint8_t* arena;
+    unsigned long long order_base;
+    unsigned long long* acc;
+    const uint8_t* inputs;         // the whole log, frame-major (n_players bytes per frame)
+    const uint32_t* prefix;        // [n_frames + 1] spawn frames before each frame; nullptr without spawn_particles (all 0)
+    const float2* spawn_vals;      // (vx, vy) of every row the log spawns, in frame order
+    unsigned long long spawn_ttl;
+    unsigned long long next_point; // first checksum frame >= j0 (>= j1: none)
+    ReplayClock c;
+    uint32_t interval;             // checksum_interval (0: none)
+    uint32_t j0, j1;
+    uint32_t n_tiles, live_rows;   // tiles of the rows at j1; rows of the live image at j0
+    uint32_t item0;                // first block of the world
+};
+static_assert(sizeof(ReplayWorld) == 144, "ReplayWorld layout (the engine and the NVRTC module must agree)");
 
 // seahash of bytes [off, off+len) of one row's element whose words are `col[w * kTileRows]` (a column of the shared tile)
 // (__noinline__: inlined per checksummed column and per row the interpreter grew to 11k instructions — 176 KB of code,

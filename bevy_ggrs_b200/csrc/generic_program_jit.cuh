@@ -100,23 +100,24 @@ __device__ __forceinline__ void jit_hash_columns(const JitRows& r, unsigned int*
     }
 }
 
-// One work item of a request vector: the rows' first read from `first_img`, the vector's ops (LOAD, ADVANCE, SAVE with its
-// hash into the save's shared accumulators `s_acc`) and the live store.  The one definition of what an op does on the
-// generated kernel: k_generic_jit and k_generic_jit_batch both run it.  `op_at(i)` is op i of the vector.
-// `spawn_vals` / `spawn_ttl`: what an OPF_SPAWN ADVANCE writes into its newborn rows (GenericParams).
-template <class OpAt>
-__device__ __forceinline__ void jit_run_item(uint8_t* arena, unsigned long long order_base, uint32_t flags, uint32_t n_ops, OpAt op_at,
-                                             const uint8_t* first_img, uint32_t first_rows, uint32_t item, unsigned int* s_acc,
-                                             uint32_t tid, uint32_t lane, const float2* spawn_vals, unsigned long long spawn_ttl) {
-    constexpr int B = kJitItemRows / kJitRows;  // threads per work item
-    constexpr uint32_t kTileBytes = kTileRows * (4u * kJitWords + 1u);
-    constexpr uint32_t kAliveOff = uint32_t(kJitWords) * kPlaneBytes;  // the mask bytes follow the word planes inside a tile
-    const uint32_t tile = item / uint32_t(kJitSubs), sub_row0 = (item % uint32_t(kJitSubs)) * uint32_t(kJitItemRows) + tid;  // first row of the thread inside the tile
-    const size_t tile_off = size_t(tile) * kTileBytes;
-    const unsigned long long row0 = order_base + size_t(tile) * kTileRows + sub_row0;
+// A work item's rows: which tile and which rows of it the thread owns.  load / store move the register copy from / to an
+// image; advance and checksum are the one definition of what an ADVANCE and a SAVE do on the generated kernel, which
+// k_generic_jit, k_generic_jit_batch and k_generic_jit_replay all run.
+struct JitItem {
+    static constexpr int B = kJitItemRows / kJitRows;  // threads per work item
+    static constexpr uint32_t kTileBytes = kTileRows * (4u * kJitWords + 1u);
+    static constexpr uint32_t kAliveOff = uint32_t(kJitWords) * kPlaneBytes;  // the mask bytes follow the word planes inside a tile
+    uint32_t tile, sub_row0;  // first row of the thread inside the tile
+    size_t tile_off;
+    unsigned long long row0;
 
-    JitRows r;
-    auto load = [&](const uint8_t* img, uint32_t n_rows_src) {
+    __device__ __forceinline__ JitItem(unsigned long long order_base, uint32_t item, uint32_t tid) {
+        tile = item / uint32_t(kJitSubs);
+        sub_row0 = (item % uint32_t(kJitSubs)) * uint32_t(kJitItemRows) + tid;
+        tile_off = size_t(tile) * kTileBytes;
+        row0 = order_base + size_t(tile) * kTileRows + sub_row0;
+    }
+    __device__ __forceinline__ void load(JitRows& r, const uint8_t* img, uint32_t n_rows_src) const {
         const uint8_t* t = img + tile_off;
 #pragma unroll
         for (int k = 0; k < kJitRows; ++k) {
@@ -126,8 +127,8 @@ __device__ __forceinline__ void jit_run_item(uint8_t* arena, unsigned long long 
             const uint32_t mm = __ldcg(t + kAliveOff + row);  // .cg: L2 only — overlapping grids share an SM's L1 without a kernel boundary in between
             r.m[k] = (tile * kTileRows + row < n_rows_src) ? mm : 0u;  // rows the image never contained come back dead
         }
-    };
-    auto store = [&](uint8_t* img) {
+    }
+    __device__ __forceinline__ void store(const JitRows& r, uint8_t* img) const {
         uint8_t* t = img + tile_off;
 #pragma unroll
         for (int k = 0; k < kJitRows; ++k) {
@@ -136,49 +137,85 @@ __device__ __forceinline__ void jit_run_item(uint8_t* arena, unsigned long long 
             for (int j = 0; j < kJitWords; ++j) *reinterpret_cast<uint32_t*>(t + size_t(j) * kPlaneBytes + size_t(row) * 4u) = r.w[k][j];
             t[kAliveOff + row] = uint8_t(r.m[k]);
         }
-    };
-    load(first_img, first_rows);
+    }
+    __device__ __forceinline__ void order_lanes(JitRows& r) const {
 #pragma unroll
-    for (int k = 0; k < kJitRows; ++k) r.t0[k] = sea_order_lane(row0 + uint32_t(k * B));
-
-    for (uint32_t i = (flags & PF_READ_LIVE) ? 0u : 1u; i < n_ops; ++i) {
-        const Op& op = op_at(i);
-        if (op.kind == OP_ADVANCE) {
+        for (int k = 0; k < kJitRows; ++k) r.t0[k] = sea_order_lane(row0 + uint32_t(k * B));
+    }
+    // `spawn_vals` / `spawn_ttl`: what an OPF_SPAWN ADVANCE writes into its newborn rows (GenericParams)
+    template <int SPAWN = kJitSpawn>  // a template, so that a registration without spawn_particles discards the spawn code
+    __device__ __forceinline__ void advance(JitRows& r, const Op& op, const float2* spawn_vals, unsigned long long spawn_ttl) const {
 #pragma unroll
-            for (int k = 0; k < kJitRows; ++k) r.kill[k] = false;
-            jit_run_systems<0>(r, op, row0, B);
+        for (int k = 0; k < kJitRows; ++k) r.kill[k] = false;
+        jit_run_systems<0>(r, op, row0, B);
 #pragma unroll
-            for (int k = 0; k < kJitRows; ++k) r.m[k] = r.kill[k] ? 0u : r.m[k];  // despawn commands: after the last system
-            if constexpr (kJitSpawn >= 0) {
-                if (op.flags & OPF_SPAWN) {  // spawn_particles' Commands: rows [first, first + count) are born after the despawns
-                    constexpr SysSpec sy = kJitSys[kJitSpawn];
+        for (int k = 0; k < kJitRows; ++k) r.m[k] = r.kill[k] ? 0u : r.m[k];  // despawn commands: after the last system
+        if constexpr (SPAWN >= 0) {
+            if (op.flags & OPF_SPAWN) {  // spawn_particles' Commands: rows [first, first + count) are born after the despawns
+                constexpr SysSpec sy = kJitSys[SPAWN];
 #pragma unroll
-                    for (int k = 0; k < kJitRows; ++k) {
-                        const uint32_t born = tile * kTileRows + sub_row0 + k * B - op.image_off256;  // index among the spawned rows
-                        if (born < op.save_index) {
-                            spawn_row(sy, [&](int kk, uint32_t plane) -> uint32_t& { return r.w[kk][plane]; }, k, kJitWords,
-                                      spawn_vals[op.call_count + born], spawn_ttl);
-                            r.m[k] = 1u;
-                        }
+                for (int k = 0; k < kJitRows; ++k) {
+                    const uint32_t born = tile * kTileRows + sub_row0 + k * B - op.image_off256;  // index among the spawned rows
+                    if (born < op.save_index) {
+                        spawn_row(sy, [&](int kk, uint32_t plane) -> uint32_t& { return r.w[kk][plane]; }, k, kJitWords,
+                                  spawn_vals[op.call_count + born], spawn_ttl);
+                        r.m[k] = 1u;
                     }
                 }
             }
-        } else if (op.kind == OP_SAVE) {
-            if (!(op.flags & OPF_NO_STORE)) store(arena + (size_t(op.image_off256) << 8));
-            uint32_t n_alive = 0, bad = 0;
-#pragma unroll
-            for (int k = 0; k < kJitRows; ++k) n_alive += r.m[k] & 1u;
-            unsigned int* a = &s_acc[op.save_index * kAccStride * 2];
-            jit_hash_columns<0>(r, a, lane, bad);
-            const unsigned full = 0xffffffffu;
-            const uint32_t cnt = __reduce_add_sync(full, n_alive);
-            const uint32_t anybad = __reduce_or_sync(full, bad);
-            if (lane == 0) { atomicAdd(&a[12], cnt); if (anybad) atomicOr(&a[14], 1u); }
-        } else {  // OP_LOAD
-            load(arena + (size_t(op.image_off256) << 8), op.n_rows);
         }
     }
-    if (flags & PF_WRITE_LIVE_ACTIVE) store(arena);
+    // a SAVE's checksum of the register copy into the shared accumulators `a` of its save (kAccStride pairs of u32)
+    __device__ __forceinline__ static void checksum(const JitRows& r, unsigned int* a, uint32_t lane) {
+        uint32_t n_alive = 0, bad = 0;
+#pragma unroll
+        for (int k = 0; k < kJitRows; ++k) n_alive += r.m[k] & 1u;
+        jit_hash_columns<0>(r, a, lane, bad);
+        const unsigned full = 0xffffffffu;
+        const uint32_t cnt = __reduce_add_sync(full, n_alive);
+        const uint32_t anybad = __reduce_or_sync(full, bad);
+        if (lane == 0) { atomicAdd(&a[12], cnt); if (anybad) atomicOr(&a[14], 1u); }
+    }
+};
+
+// One work item of a request vector: the rows' first read from `first_img`, the vector's ops (LOAD, ADVANCE, SAVE with its
+// hash into the save's shared accumulators `s_acc`) and the live store.  k_generic_jit and k_generic_jit_batch both run
+// it.  `op_at(i)` is op i of the vector.
+template <class OpAt>
+__device__ __forceinline__ void jit_run_item(uint8_t* arena, unsigned long long order_base, uint32_t flags, uint32_t n_ops, OpAt op_at,
+                                             const uint8_t* first_img, uint32_t first_rows, uint32_t item, unsigned int* s_acc,
+                                             uint32_t tid, uint32_t lane, const float2* spawn_vals, unsigned long long spawn_ttl) {
+    const JitItem it(order_base, item, tid);
+    JitRows r;
+    it.load(r, first_img, first_rows);
+    it.order_lanes(r);
+    for (uint32_t i = (flags & PF_READ_LIVE) ? 0u : 1u; i < n_ops; ++i) {
+        const Op& op = op_at(i);
+        if (op.kind == OP_ADVANCE) {
+            it.advance(r, op, spawn_vals, spawn_ttl);
+        } else if (op.kind == OP_SAVE) {
+            if (!(op.flags & OPF_NO_STORE)) it.store(r, arena + (size_t(op.image_off256) << 8));
+            JitItem::checksum(r, &s_acc[op.save_index * kAccStride * 2], lane);
+        } else {  // OP_LOAD
+            it.load(r, arena + (size_t(op.image_off256) << 8), op.n_rows);
+        }
+    }
+    if (flags & PF_WRITE_LIVE_ACTIVE) it.store(r, arena);
+}
+
+// Shared accumulators of `n_saves` saves folded into global ones: XOR for the column words, add for the active rows,
+// OR for the flags
+__device__ __forceinline__ void jit_fold_acc(unsigned long long* accum, const unsigned int* s_acc, uint32_t n_saves, uint32_t tid) {
+    constexpr int B = kJitItemRows / kJitRows;
+    for (uint32_t i = tid; i < n_saves * kAccStride; i += B) {
+        unsigned long long v = (unsigned long long)s_acc[2 * i] | ((unsigned long long)s_acc[2 * i + 1] << 32);
+        const uint32_t c = i % kAccStride;
+        if (v) {
+            if (c == 6) atomicAdd(&accum[i], v);
+            else if (c == 7) atomicOr(&accum[i], v);
+            else atomicXor(&accum[i], v);
+        }
+    }
 }
 
 // The end of a block: its shared accumulators folded into the vector's `accum`; the block that completes the vector's
@@ -189,15 +226,7 @@ __device__ __forceinline__ void jit_fold_publish(unsigned long long* accum, unsi
                                                  unsigned int& s_last, unsigned long long* trace, uint32_t tid) {
     constexpr int B = kJitItemRows / kJitRows;
     __syncthreads();
-    for (uint32_t i = tid; i < n_saves * kAccStride; i += B) {
-        unsigned long long v = (unsigned long long)s_acc[2 * i] | ((unsigned long long)s_acc[2 * i + 1] << 32);
-        const uint32_t c = i % kAccStride;
-        if (v) {
-            if (c == 6) atomicAdd(&accum[i], v);
-            else if (c == 7) atomicOr(&accum[i], v);
-            else atomicXor(&accum[i], v);
-        }
-    }
+    jit_fold_acc(accum, s_acc, n_saves, tid);
     __threadfence();
     __syncthreads();
     if (trace && tid == 0) atomicMax(&trace[1], globaltimer_ns());
@@ -290,6 +319,74 @@ extern "C" __global__ void __launch_bounds__(BGR_JIT_ITEM_ROWS / BGR_JIT_ROWS, B
     jit_run_item(w.arena, w.order_base, w.flags, w.n_ops, [&](uint32_t i) -> const Op& { return wops[i]; }, first_img, first_rows,
                  blockIdx.x - w.item0, s_acc, tid, lane, w.spawn_vals, w.spawn_ttl);
     jit_fold_publish(w.accum, w.ticket, w.out, w.seq, w.n_saves, w.n_tiles * uint32_t(kJitSubs), s_acc, s_last, nullptr, tid);
+}
+
+// A recorded input log through many worlds in ONE launch (bgr_replay, bgr_batch_replay).  Block b runs one work item of
+// one world (the binary search of k_generic_jit_batch) through every frame [j0, j1) of the world's log: its rows are
+// read from the live image once, stay in registers, and are written back once.  Each frame's ADVANCE op is derived
+// on the device (replay_op) from the frame index, the input bytes and the spawn prefix, which the block stages into
+// shared memory kReplayChunk frames at a time.  A checksum frame hashes the registers into a window of kReplayWindow
+// shared accumulators; a full window (and the last one) is folded into the world's acc[point][kAccStride] with one
+// global atomic per non-zero word.  No barrier runs on frames that are neither checksum points nor chunk starts.
+constexpr uint32_t kReplayChunk = 256;  // frames of the log per staging step
+constexpr uint32_t kReplayWindow = 32;  // checksum points per shared window
+
+extern "C" __global__ void __launch_bounds__(BGR_JIT_ITEM_ROWS / BGR_JIT_ROWS, BGR_JIT_MINB)
+    k_generic_jit_replay(const ReplayWorld* __restrict__ worlds, uint32_t n_worlds) {
+    constexpr int B = kJitItemRows / kJitRows;
+    __shared__ unsigned int s_acc[kReplayWindow * kAccStride * 2];
+    __shared__ uint8_t s_in[kReplayChunk * 8];
+    __shared__ uint32_t s_pre[kReplayChunk];
+    __shared__ Op s_op[B];
+    const uint32_t tid = threadIdx.x, lane = tid & 31u;
+
+    uint32_t lo = 0, hi = n_worlds;
+    while (hi - lo > 1u) {
+        const uint32_t mid = (lo + hi) / 2u;
+        if (worlds[mid].item0 <= blockIdx.x) lo = mid;
+        else hi = mid;
+    }
+    const ReplayWorld& w = worlds[lo];
+    const ReplayClock c = w.c;
+    const uint32_t j1 = w.j1, np = c.n_players, interval = w.interval;
+    for (uint32_t i = tid; i < kReplayWindow * kAccStride * 2; i += B) s_acc[i] = 0u;
+
+    const JitItem it(w.order_base, blockIdx.x - w.item0, tid);
+    JitRows r;
+    it.load(r, w.arena, w.live_rows);
+    it.order_lanes(r);
+
+    unsigned long long next_point = w.next_point;
+    uint32_t point = 0, win0 = 0;  // checksum points seen, first point of the shared window
+    auto flush = [&](uint32_t n) {
+        __syncthreads();
+        jit_fold_acc(w.acc + size_t(win0) * kAccStride, s_acc, n, tid);
+        __syncthreads();
+        for (uint32_t i = tid; i < n * kAccStride * 2; i += B) s_acc[i] = 0u;
+        __syncthreads();
+    };
+    for (uint32_t j = w.j0, chunk0 = w.j0; j < j1; ++j) {
+        if (j == chunk0 || j - chunk0 == kReplayChunk) {  // the log's next kReplayChunk frames into shared memory
+            chunk0 = j;
+            const uint32_t n = min(kReplayChunk, j1 - j);
+            __syncthreads();  // every thread is done with the previous chunk (and the accumulators are zeroed)
+            for (uint32_t i = tid; i < n * np; i += B) s_in[i] = w.inputs[size_t(j) * np + i];
+            for (uint32_t i = tid; i < n; i += B) s_pre[i] = w.prefix ? w.prefix[j + i] : 0u;
+            __syncthreads();
+        }
+        const uint32_t q = j - chunk0;
+        if (j == next_point) {  // SaveGameState{f0 + j} with no store: the checksum of the registers
+            if (point - win0 == kReplayWindow) { flush(kReplayWindow); win0 = point; }
+            JitItem::checksum(r, &s_acc[(point - win0) * kAccStride * 2], lane);
+            point += 1;
+            next_point += interval;
+        }
+        Op& op = s_op[tid];  // the thread's own copy: box_move indexes its inputs by row, which would put a local one on the stack
+        op = replay_op(c, j, &s_in[q * np], s_pre[q]);
+        it.advance(r, op, w.spawn_vals, w.spawn_ttl);
+    }
+    if (point > win0) flush(point - win0);
+    it.store(r, w.arena);
 }
 
 }  // namespace bgr

@@ -45,6 +45,11 @@ class LastKernel(NamedTuple):
         """The vector ran inside a world batch's launch (BGR_KERNEL_BATCHED, EngineBatch)."""
         return bool(self.raw & capi.BGR_KERNEL_BATCHED)
 
+    @property
+    def replay(self) -> bool:
+        """The last replay ran on the generated kernel's replay entry point (BGR_KERNEL_REPLAY), not in chunks."""
+        return bool(self.raw & capi.BGR_KERNEL_REPLAY)
+
     @staticmethod
     def decode(v: int) -> "LastKernel":
         return LastKernel(_KERNEL_KINDS.get(v & 0xF, f"unknown({v & 0xF})"), (v >> 4) & 0xF, (v >> 8) & 0x3,
@@ -427,6 +432,19 @@ class Engine:
                                                   capi.BGR_MAX_REQUESTS, C.byref(n)))
         return [(out[i].frame, (out[i].hi << 64) | out[i].lo) for i in range(n.value)]
 
+    def replay(self, inputs: np.ndarray, checksum_interval: int = 0) -> List[Tuple[int, int]]:
+        """Run a recorded input log, ``inputs[n_frames, n_players]`` (uint8), from the current frame f0 in one call:
+        what ``[Save(f) if checksum_interval and f % checksum_interval == 0] + [Advance(inputs[j])]`` for every frame
+        f = f0 + j would do, without pushing snapshots.  Returns [(frame, checksum), ...] of the checksum frames in
+        order.  A non-finite value at a checksum frame raises BgrError(BGR_ERR_NON_FINITE) after the whole log ran."""
+        log = _replay_log(inputs)
+        r = capi.bgr_replay(log.shape[0], log.shape[1], checksum_interval, 0, log.ctypes.data if log.size else None)
+        cap = _replay_points(self.rollback_frame_count(), log.shape[0], checksum_interval)
+        out = (capi.bgr_checksum * max(1, cap))()
+        n = C.c_uint32()
+        self._check(self._lib.bgr_replay(self._h, C.byref(r), out, cap, C.byref(n)))
+        return _checksum_list(out, 0, n.value)
+
     def submit_requests(self, session_info: Sequence[int], requests) -> None:
         reqs = list(requests)
         arr = capi.make_requests(reqs)
@@ -579,6 +597,55 @@ class EngineBatch:
             res.append((status[i], [(out[k + j].frame, (out[k + j].hi << 64) | out[k + j].lo) for j in range(n_cs[i])]))
             k += n_cs[i]
         return res
+
+
+    def replay(self, calls) -> List[Tuple[int, List[Tuple[int, int]]]]:
+        """``calls`` = [(world, inputs[n_frames, n_players] uint8, checksum_interval), ...]: Engine.replay of every
+        listed world in one synchronous call (one launch when the batch is specialised).  Returns [(status, [(frame,
+        checksum), ...]), ...] in the same order.  A call refused before anything executed raises BgrError and changes
+        no world."""
+        calls = [(w, _replay_log(x), k) for w, x, k in calls]
+        n = len(calls)
+        worlds = (C.c_uint32 * max(1, n))(*[w for w, _, _ in calls])
+        reps = (capi.bgr_replay * max(1, n))(*[capi.bgr_replay(x.shape[0], x.shape[1], k, 0, x.ctypes.data if x.size else None)
+                                               for _, x, k in calls])
+        cap = 0
+        for w, x, k in calls:
+            if 0 <= w < len(self.engines):
+                cap += _replay_points(self.engines[w].rollback_frame_count(), x.shape[0], k)
+        out = (capi.bgr_checksum * max(1, cap))()
+        n_cs = (C.c_uint32 * max(1, n))()
+        status = (C.c_int32 * max(1, n))()
+        rc = self._lib.bgr_batch_replay(self._h, worlds, n, reps, out, cap, n_cs, status)
+        if rc not in (capi.BGR_OK, capi.BGR_ERR_NON_FINITE):
+            self._check(rc)
+        res, k = [], 0
+        for i in range(n):
+            res.append((status[i], _checksum_list(out, k, k + n_cs[i])))
+            k += n_cs[i]
+        return res
+
+
+def _replay_log(inputs) -> np.ndarray:
+    log = np.ascontiguousarray(inputs, dtype=np.uint8)
+    if log.ndim != 2:
+        raise ValueError("a replay log is a [n_frames, n_players] array")
+    return log
+
+
+def _checksum_list(out, a: int, b: int) -> List[Tuple[int, int]]:
+    """[(frame, checksum)] of bgr_checksum array elements [a, b), through numpy: a replay returns thousands."""
+    if b <= a:
+        return []
+    arr = np.ctypeslib.as_array(out)[a:b]
+    return [(f, (h << 64) | lo) for f, lo, h in zip(arr["frame"].tolist(), arr["lo"].tolist(), arr["hi"].tolist())]
+
+
+def _replay_points(f0: int, n: int, k: int) -> int:
+    """Checksum frames f0 + j, j < n, with (f0 + j) % k == 0 (the size of a replay's result)."""
+    if k <= 0 or n <= 0 or f0 < 0:
+        return 0
+    return (f0 + n + k - 1) // k - (f0 + k - 1) // k
 
 
 def fold_partials(partial: "capi.bgr_partial") -> int:

@@ -455,6 +455,34 @@ public:
         }
         return blob;
     }
+    // ---- replays (bgr_replay; INTEGRATION.md "Replays") ----
+    // A recorded input log (inputs[j * n_players + h], n_players per frame) run from the current frame in one call; the
+    // checksums of the frames f with f % checksum_interval == 0, before they are advanced, in order.  The engine's
+    // world only: refused while rollback resources or host-side component tables are registered, whose per-frame
+    // schedules the engine does not run.
+    std::vector<std::pair<ggrs::Frame, unsigned __int128>> replay(const std::vector<uint8_t>& inputs, uint32_t n_players,
+                                                                  uint32_t checksum_interval) {
+        finish();
+        if (!res_order_.empty() || !host_cols_.empty())
+            throw Panic(BGR_ERR_UNSUPPORTED, "replay runs the engine's world only: the App has rollback resources or host-side components");
+        if (n_players ? inputs.size() % n_players != 0 : !inputs.empty())
+            throw Panic(BGR_ERR_INVALID_ARGUMENT, "the input log is not a whole number of frames of n_players bytes");
+        struct bgr_replay r;
+        std::memset(&r, 0, sizeof r);
+        r.n_players = n_players;
+        r.n_frames = n_players ? uint32_t(inputs.size() / n_players) : 0u;
+        r.checksum_interval = checksum_interval;
+        r.inputs = inputs.data();
+        const int64_t f0 = rollback_frame_count(), n = r.n_frames, k = checksum_interval;
+        const size_t cap = k && f0 >= 0 ? size_t((f0 + n + k - 1) / k - (f0 + k - 1) / k) : 0u;
+        std::vector<bgr_checksum> cs(std::max<size_t>(cap, 1));
+        uint32_t got = 0;
+        check(bgr_replay(engine_, &r, cs.data(), uint32_t(cap), &got));
+        std::vector<std::pair<ggrs::Frame, unsigned __int128>> out;
+        for (uint32_t i = 0; i < got && i < cap; ++i) out.emplace_back(cs[i].frame, (static_cast<unsigned __int128>(cs[i].hi) << 64) | cs[i].lo);
+        return out;
+    }
+
     // Replaces the world and the App's resources with a checkpoint's.  The resource section is checked before the
     // engine restores, so a refused blob changes nothing.
     void restore_checkpoint(const std::vector<uint8_t>& blob) {

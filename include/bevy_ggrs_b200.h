@@ -626,6 +626,44 @@ BGR_API int bgr_batch_handle_requests(bgr_batch* b, const uint32_t* worlds, uint
                                       const bgr_request* requests, const uint32_t* n_requests, bgr_checksum* checksums_out,
                                       uint32_t checksums_cap, uint32_t* n_checksums_out, int32_t* status_out);
 
+/* ---- replays: a recorded input log run through a world in one launch ---------------------------------------------
+ * For an engine at RollbackFrameCount f0 >= 0, bgr_replay(n frames, inputs, checksum_interval k) does what this
+ * request stream would do through bgr_handle_requests (no session):
+ *     for j in 0 .. n-1:  if k > 0 and (f0 + j) % k == 0: SaveGameState{f0 + j};   AdvanceFrame{inputs[j*n_players ..]}
+ * with three differences: no snapshot is pushed (the ring, its depth, confirmed frame, retained frames and desync
+ * witnesses are left alone, so a Load of a frame from before the replay still works); frame f0 + n is not checksummed
+ * (replay(a) then replay(b) equals replay(a ++ b)); and there is no BGR_MAX_REQUESTS limit.  The live world, the row
+ * count, RollbackFrameCount (= f0 + n), Time<GgrsTime>, ParticleRng, the BGR_SYS_U32_STORE_CALL_COUNT counter and the
+ * checksums (one per checksum frame, in frame order) equal the stream's.  A non-finite finite-asserted value at a
+ * checksum frame is BGR_ERR_NON_FINITE after the whole replay has run; bgr_last_error() names the first such frame.
+ * Refusals change nothing: n_players > BGR_MAX_PLAYERS, n_frames > BGR_MAX_REPLAY_FRAMES, reserved != 0, a null log
+ * with n_frames > 0, or f0 + n past INT32_MAX: BGR_ERR_INVALID_ARGUMENT; un-collected submits, f0 < 0 or a first step
+ * that would move Time<GgrsTime> backwards: BGR_ERR_STATE; BGR_CFG_SHARDED: BGR_ERR_UNSUPPORTED; spawns past a fixed
+ * engine's max_entities or a growable engine's ceiling: BGR_ERR_CAPACITY (a growable engine otherwise grows first).
+ * Synchronous.  *n_out = the number of checksum frames; the first `cap` of them go to checksums_out.
+ * Runs on the registration's generated kernel (k_generic_jit_replay, bgr_last_kernel carries BGR_KERNEL_REPLAY; an
+ * engine without one compiles it at its first replay) unless BGR_TUNE_JIT=0, BGR_CFG_FORCE_STEPWISE or a registration
+ * the generated kernel does not take: then in chunks of at most BGR_MAX_REQUESTS ops through the engine's own kernel,
+ * with the same results.  Replay serves spectator catch-up, replay seeking and match verification; it does not
+ * replace bgr_handle_requests for a live session. */
+#define BGR_MAX_REPLAY_FRAMES (1u << 24)
+/* a struct tag without a typedef: the call below has the same name, so the type is spelled `struct bgr_replay` */
+struct bgr_replay {
+    uint32_t n_frames;           /* AdvanceFrame requests */
+    uint32_t n_players;          /* PlayerInputs<T>.len() of every frame, <= BGR_MAX_PLAYERS */
+    uint32_t checksum_interval;  /* 0: no checksums; k: frames f0+j with (f0+j) % k == 0, before advancing them */
+    uint32_t reserved;           /* 0 */
+    const uint8_t* inputs;       /* n_frames * n_players bytes, frame-major */
+};
+BGR_API int bgr_replay(bgr_engine* e, const struct bgr_replay* r, bgr_checksum* checksums_out, uint32_t cap, uint32_t* n_out);
+/* bgr_replay of replays[i] on worlds[i], in the conventions of bgr_batch_handle_requests: every listed world is validated
+ * and planned first, and if any fails nothing executes anywhere (status_out marks it, bgr_last_error() starts with
+ * "world <index>: ").  World i's checksums follow the previous worlds' in checksums_out as far as cap reaches;
+ * n_checksums_out[i] is its count.  A specialised batch (bgr_batch_specialised) runs every world in one launch of its
+ * generated kernel; otherwise each world's bgr_replay runs in list order. */
+BGR_API int bgr_batch_replay(bgr_batch* b, const uint32_t* worlds, uint32_t n_worlds, const struct bgr_replay* replays,
+                             bgr_checksum* checksums_out, uint32_t cap, uint32_t* n_checksums_out, int32_t* status_out);
+
 /* ---- shard group: the cross-shard step inside the engine (multi-GPU, one process per GPU, one node) -----------------
  * Entity-range shards never exchange state (SURVEY.md §8e: systems read no other entity, box_game.rs:162-169; the
  * checksum is an XOR over entities, component_checksum.rs:88-89).  The only exchange is 64 bytes of partials per
@@ -693,13 +731,16 @@ BGR_API int bgr_generic_specialised(bgr_engine* e, uint32_t* specialised_out);
  *   bit 27     BGR_KERNEL_HELD_SAVES, bundle: at least one Save was held: its target slot already held the content and
  *              row count it would have stored (host-side content ids), so it stored nothing and only checksummed
  *              (bgr_held_saves; env BGR_TUNE_HELD_SAVES, default 1)
- *   bit 28     BGR_KERNEL_BATCHED, generic NVRTC: the vector ran inside a world batch's launch (bgr_batch_handle_requests) */
+ *   bit 28     BGR_KERNEL_BATCHED, generic NVRTC: the vector ran inside a world batch's launch (bgr_batch_handle_requests)
+ *   bit 29     BGR_KERNEL_REPLAY, generic NVRTC: the last bgr_replay / bgr_batch_replay ran on the generated kernel's replay
+ *              entry point (k_generic_jit_replay); clear when it ran in chunks through the engine's own kernel */
 #define BGR_KERNEL_DEFERRED_LIVE (1u << 13)
 #define BGR_KERNEL_FROM_DEFERRED (1u << 14)
 #define BGR_KERNEL_PASSIVE_PLANES (1u << 15)
 #define BGR_KERNEL_STABLE_PLANES (1u << 26)
 #define BGR_KERNEL_HELD_SAVES (1u << 27)
 #define BGR_KERNEL_BATCHED (1u << 28)
+#define BGR_KERNEL_REPLAY (1u << 29)
 #define BGR_KERNEL_NONE 0u
 #define BGR_KERNEL_STEPWISE_TMA 1u       /* one kernel per request; Save / Load through the TMA-staged copy kernel */
 #define BGR_KERNEL_STEPWISE_FLAT 2u      /* one kernel per request; k_checksum_column + k_copy_image */

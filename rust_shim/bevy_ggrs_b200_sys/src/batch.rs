@@ -13,7 +13,7 @@ pub struct BatchCall<'a> {
 
 /// Owns a `bgr_batch`; the engines it was created from must outlive it (dropping it destroys the batch first).
 pub struct Batch {
-    raw: *mut bgr_batch,
+    pub(crate) raw: *mut bgr_batch,
 }
 
 impl Batch {

@@ -9,6 +9,7 @@ pub const BGR_MAX_REQUESTS: usize = 80;
 pub const BGR_MAX_CHECKSUM_COLUMNS: usize = 6;
 
 pub const BGR_OK: c_int = 0;
+pub const BGR_ERR_INVALID_ARGUMENT: c_int = 1;
 pub const BGR_ERR_NO_SNAPSHOT: c_int = 4;
 pub const BGR_ERR_NON_FINITE: c_int = 6;
 
@@ -54,6 +55,8 @@ pub const BGR_KERNEL_STABLE_PLANES: u32 = 1 << 26;
 pub const BGR_KERNEL_HELD_SAVES: u32 = 1 << 27;
 /// bgr_last_kernel flag: the request vector ran inside a world batch's launch (bgr_batch_handle_requests).
 pub const BGR_KERNEL_BATCHED: u32 = 1 << 28;
+/// bgr_last_kernel flag: the last replay ran on the generated kernel's replay entry point (bgr_replay / bgr_batch_replay).
+pub const BGR_KERNEL_REPLAY: u32 = 1 << 29;
 
 pub const BGR_CFG_FORCE_STEPWISE: u32 = 1;
 pub const BGR_CFG_SHARDED: u32 = 2;
@@ -81,6 +84,9 @@ pub use checkpoint::*;
 // world batches: a safe owner of a bgr_batch
 mod batch;
 pub use batch::*;
+// replays: the bgr_replay record and safe calls over an input log
+mod replay;
+pub use replay::*;
 
 #[repr(C)]
 #[derive(Clone, Copy, Default)]
@@ -201,6 +207,8 @@ extern "C" {
     pub fn bgr_batch_destroy(b: *mut bgr_batch);
     pub fn bgr_batch_specialised(b: *mut bgr_batch, specialised_out: *mut u32) -> c_int;
     pub fn bgr_batch_handle_requests(b: *mut bgr_batch, worlds: *const u32, n_worlds: u32, sessions: *const bgr_session_info, requests: *const bgr_request, n_requests: *const u32, checksums_out: *mut bgr_checksum, checksums_cap: u32, n_checksums_out: *mut u32, status_out: *mut i32) -> c_int;
+    pub fn bgr_replay(e: *mut bgr_engine, r: *const bgr_replay, checksums_out: *mut bgr_checksum, cap: u32, n_out: *mut u32) -> c_int;
+    pub fn bgr_batch_replay(b: *mut bgr_batch, worlds: *const u32, n_worlds: u32, replays: *const bgr_replay, checksums_out: *mut bgr_checksum, cap: u32, n_checksums_out: *mut u32, status_out: *mut i32) -> c_int;
     pub fn bgr_seahash(bytes: *const c_void, len: u64) -> u64;
     pub fn bgr_ggrs_time_delta_bits(fps: u32, frame: i32) -> u32;
     pub fn bgr_particle_rng_stream(seed: u64, state4_or_null: *const u64, n: u32, next_u64_out: *mut u64, range_out: *mut f32, low: f32, high: f32) -> c_int;
