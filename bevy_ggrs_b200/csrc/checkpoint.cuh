@@ -44,6 +44,7 @@ struct CkptParams {
     const uint8_t* img;                  // save: the source slot's image; restore: the scratch image written
     uint32_t words, rows;
     const uint32_t* plane_absent;        // [words] the absent bit of the column each plane belongs to (0: not optional)
+    const uint32_t* plane_pad;           // restore: [words] the bits of a plane's word past its column's element bytes
     uint32_t mask_bits;                  // restore: the bits a mask byte may hold (alive and the registered absent bits)
     uint8_t* kinds;                      // save: [tiles][words + 1]
     unsigned int* lens;                  // save: [tiles] bytes of each block
@@ -227,10 +228,13 @@ __global__ void __launch_bounds__(kTileRows) k_ckpt_unpack(const __grid_constant
         return;
     }
     tb[size_t(p.words) * kPlaneBytes + threadIdx.x] = uint8_t(m);
+    uint32_t stray = 0;   // bits past a sub-word element's end: no digest covers them, so they are refused here
     for (uint32_t v = 0; v < p.words; ++v) {
-        const uint32_t x = element(v);
-        *reinterpret_cast<uint32_t*>(tb + size_t(v) * kPlaneBytes + threadIdx.x * 4u) = (m && !(m & p.plane_absent[v])) ? x : 0u;
+        const uint32_t x = (m && !(m & p.plane_absent[v])) ? element(v) : 0u;
+        stray |= x & p.plane_pad[v];
+        *reinterpret_cast<uint32_t*>(tb + size_t(v) * kPlaneBytes + threadIdx.x * 4u) = x;
     }
+    if (__syncthreads_or(stray != 0u) && threadIdx.x == 0) atomicMin(p.err, tile);
 }
 
 }  // namespace bgr

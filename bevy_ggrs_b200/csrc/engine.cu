@@ -3035,6 +3035,14 @@ static std::vector<uint32_t> plane_absent(const bgr_engine* e) {
     return a;
 }
 
+// the bits of each plane's word that lie past its column's element bytes (the last word of a sub-word element)
+static std::vector<uint32_t> plane_pad(const bgr_engine* e) {
+    std::vector<uint32_t> a(std::max(1u, e->words), 0u);
+    for (const Column& c : e->cols)
+        if (c.elem_bytes % 4u) a[c.first_plane + c.words - 1u] = ~0u << (8u * (c.elem_bytes % 4u));
+    return a;
+}
+
 // bytes ahead of the payload: the header and the offsets
 static size_t checkpoint_prefix(uint32_t n_blocks) {
     return sizeof(bgr_checkpoint_header) + sizeof(uint64_t) * (size_t(n_blocks) + 1u);
@@ -3159,7 +3167,7 @@ BGR_API int bgr_checkpoint_restore(bgr_engine* e, const void* blob, size_t bytes
             return fail(BGR_ERR_INVALID_ARGUMENT, "checkpoint offset " + std::to_string(b + 1) + " is not ascending, aligned or within a block's size");
     // decode into a scratch image and verify it with the frame digest before anything is committed
     DeviceBuffer<uint8_t> scratch;
-    DeviceBuffer<uint32_t> d_payload, d_absent;
+    DeviceBuffer<uint32_t> d_payload, d_absent, d_pad;
     DeviceBuffer<unsigned long long> d_offsets;
     DeviceBuffer<unsigned int> d_err;
     const size_t tb = e->tile_bytes, image_bytes = size_t(n_blocks) * tb;
@@ -3167,14 +3175,16 @@ BGR_API int bgr_checkpoint_restore(bgr_engine* e, const void* blob, size_t bytes
         const size_t smem = sizeof(uint32_t) * (e->words + 1u);
         if (smem + sizeof(uint32_t) * (kCkptMaskWords + 1u) > 48u * 1024u)
             return fail(BGR_ERR_UNSUPPORTED, "bgr_checkpoint_restore supports at most 12000 word planes");
-        const std::vector<uint32_t> absent = plane_absent(e);
+        const std::vector<uint32_t> absent = plane_absent(e), pad = plane_pad(e);
         CUDA_TRY(scratch.ensure(image_bytes));
         CUDA_TRY(d_payload.ensure(h.payload_bytes / 4u));
         CUDA_TRY(d_absent.ensure(absent.size()));
+        CUDA_TRY(d_pad.ensure(pad.size()));
         CUDA_TRY(d_offsets.ensure(offsets.size()));
         CUDA_TRY(d_err.ensure(1));
         CUDA_TRY(cudaMemcpyAsync(d_payload.get(), in + prefix, h.payload_bytes, cudaMemcpyHostToDevice, e->stream));
         CUDA_TRY(cudaMemcpyAsync(d_absent.get(), absent.data(), sizeof(uint32_t) * absent.size(), cudaMemcpyHostToDevice, e->stream));
+        CUDA_TRY(cudaMemcpyAsync(d_pad.get(), pad.data(), sizeof(uint32_t) * pad.size(), cudaMemcpyHostToDevice, e->stream));
         CUDA_TRY(cudaMemcpyAsync(d_offsets.get(), offsets.data(), sizeof(uint64_t) * offsets.size(), cudaMemcpyHostToDevice, e->stream));
         CUDA_TRY(cudaMemsetAsync(d_err.get(), 0xFF, sizeof(unsigned int), e->stream));
         CkptParams p{};
@@ -3182,6 +3192,7 @@ BGR_API int bgr_checkpoint_restore(bgr_engine* e, const void* blob, size_t bytes
         p.words = e->words;
         p.rows = h.rows;
         p.plane_absent = d_absent.get();
+        p.plane_pad = d_pad.get();
         p.mask_bits = 1u;
         for (const Column& c : e->cols) p.mask_bits |= c.absent;
         p.offsets = d_offsets.get();
@@ -3196,7 +3207,8 @@ BGR_API int bgr_checkpoint_restore(bgr_engine* e, const void* blob, size_t bytes
         if (bad != 0xFFFFFFFFu)
             return fail(BGR_ERR_INVALID_ARGUMENT, "checkpoint block " + std::to_string(bad) +
                                                       ": a bad kind byte or padding, its kinds and bitmaps imply another length than its "
-                                                      "offsets, or a row's mask byte has a bit this registration does not use");
+                                                      "offsets, a row's mask byte has a bit this registration does not use, or a word has "
+                                                      "bits past its column's element bytes");
     }
     std::vector<uint64_t> digest_words;
     uint64_t root = 0, active = 0;

@@ -546,10 +546,10 @@ BGR_API int bgr_checkpoint_save(bgr_engine* e, int32_t frame, void* dst, size_t 
 /* Replaces the engine's world with the blob's.  The blob is untrusted input and is checked in full before anything
  * changes: bad magic or version, another layout, fps or word count, n_blocks != ceil(rows / 512), a truncated or
  * overlong blob, bad offsets, a kind byte > 2 or non-zero padding, a block whose kinds and bitmaps imply another length
- * than its offsets give, and a decoded world whose digest root or active count differs from the header's are
- * BGR_ERR_INVALID_ARGUMENT; rows past a fixed engine's capacity or a growable engine's ceiling BGR_ERR_CAPACITY;
- * un-collected submits BGR_ERR_STATE (as bgr_reset_session); a sharded engine BGR_ERR_UNSUPPORTED.  A refused call
- * changes nothing observable.  On success:
+ * than its offsets give, a present word with bits set past its column's element bytes (no digest covers them), and a
+ * decoded world whose digest root or active count differs from the header's are BGR_ERR_INVALID_ARGUMENT; rows past a
+ * fixed engine's capacity or a growable engine's ceiling BGR_ERR_CAPACITY; un-collected submits BGR_ERR_STATE (as
+ * bgr_reset_session); a sharded engine BGR_ERR_UNSUPPORTED.  A refused call changes nothing observable.  On success:
  *   - image 0 holds the decoded world (canonical: see above); RollbackFrameCount = frame, and Time<GgrsTime>,
  *     ParticleRng and the row count are the header's;
  *   - the ring keeps its depth and retention setting, and its queue holds exactly one snapshot, of `frame`, holding the

@@ -31,6 +31,8 @@ struct GgrsSnapshots {
     size_t depth = 60;
 
     GgrsSnapshots& set_depth(size_t d) { depth = d; return *this; }
+    // every stored frame dropped, the depth kept (a checkpoint restore starts the ring again)
+    GgrsSnapshots& clear() { snapshots.clear(); frames.clear(); return *this; }
 
     static uint32_t abs_diff(int32_t a, int32_t b) {
         int64_t x = int64_t(a) - int64_t(b);

@@ -236,6 +236,15 @@ ORC_API uint32_t orc_last_dt_bits(World* w) { uint32_t b; std::memcpy(&b, &w->gg
 ORC_API int orc_save_world(World* w, bgr_checksum* out) {
     return guarded([&] { w->save_world(); if (out) *out = bgr_checksum{w->rollback_frame_count, 1u, w->checksum_lo, 0}; });
 }
+// SaveWorld's Checksum half alone: the checksum of the current frame, no snapshot pushed (a replay's checksum frames)
+ORC_API int orc_checksum_world(World* w, bgr_checksum* out) {
+    return guarded([&] { w->checksum_world(); if (out) *out = bgr_checksum{w->rollback_frame_count, 1u, w->checksum_lo, 0}; });
+}
+// World::restore: `mask` one byte per row, `absent_bit` one per column, `cols[c]` rows * elem_bytes of column c
+ORC_API int orc_restore(World* w, int32_t frame, uint32_t rows, const uint8_t* mask, const uint32_t* absent_bit,
+                        const uint8_t* const* cols, uint64_t elapsed_ns, const uint64_t* rng) {
+    return guarded([&] { w->restore(frame, rows, mask, absent_bit, cols, elapsed_ns, rng); });
+}
 ORC_API int orc_load_world(World* w) { return guarded([&] { w->load_world(); }); }
 ORC_API int orc_advance_world(World* w, const uint8_t* inputs, uint32_t n_players) {
     return guarded([&] {

@@ -359,6 +359,12 @@ struct World {
         entity_snaps.push(rollback_frame_count, std::move(t));
     }
     void save_world() {
+        checksum_world();
+        snapshot_world();
+    }
+    // SaveWorldSystems::Checksum and ChecksumPlugin::update: the frame checksum without storing anything (what a
+    // replay computes at its checksum frames)
+    void checksum_world() {
         // --- SaveWorldSystems::Checksum: per-type systems, parallel-eligible ---
         std::vector<std::function<void()>> tasks;
         for (size_t c = 0; c < columns.size(); ++c)
@@ -377,8 +383,10 @@ struct World {
         for (size_t i = 0; i < resources.size(); ++i)
             if (resources[i].checksum) x ^= res_parts[i];
         checksum_lo = x;
+    }
+    void snapshot_world() {
         // --- SaveWorldSystems::Snapshot: per-type save systems ---
-        tasks.clear();
+        std::vector<std::function<void()>> tasks;
         for (size_t c = 0; c < columns.size(); ++c) tasks.push_back([this, c] { component_save(c); });
         tasks.push_back([this] { entity_save(); });
         tasks.push_back([this] {  // ResourceSnapshotPlugin<CloneStrategy<RollbackOrdered>> (mod.rs:339)
@@ -499,6 +507,45 @@ struct World {
             if (s) { res_data[i] = *s; res_present[i] = 1; } else { res_present[i] = 0; }
         }
     }
+    // A world checkpoint restored (bgr_checkpoint_restore): row r of the checkpoint gets RollbackOrdered index r, it
+    // exists iff bit 0 of its mask byte is set, and column c is present on it unless mask & absent_bit[c].
+    // RollbackFrameCount, Time<GgrsTime> and ParticleRng become the checkpoint's; every GgrsSnapshots is cleared and then
+    // holds that frame's one snapshot.  The call counter, ConfirmedFrameCount and MaxPredictionWindow are left alone.
+    void restore(int32_t frame, uint32_t n, const uint8_t* mask, const uint32_t* absent_bit,
+                 const uint8_t* const* col_bytes, uint64_t elapsed_ns, const uint64_t rng[4]) {
+        rollback_id.clear();
+        entity.clear();
+        for (auto& d : data) d.clear();
+        for (auto& h : has) h.clear();
+        rollback_ordered = RollbackOrdered{};
+        pending_spawns.clear();
+        for (uint32_t r = 0; r < n; ++r) {
+            const uint64_t id = next_entity++;
+            rollback_ordered.push(id);
+            if (!(mask[r] & 1u)) continue;
+            rollback_id.push_back(id);
+            entity.push_back(id);
+            for (size_t c = 0; c < columns.size(); ++c) {
+                const uint32_t eb = columns[c].elem_bytes;
+                const uint8_t* v = col_bytes[c] + size_t(r) * eb;
+                data[c].insert(data[c].end(), v, v + eb);
+                has[c].push_back((mask[r] & absent_bit[c]) ? 0 : 1);
+            }
+        }
+        rollback_frame_count = frame;
+        ggrs_time = GgrsTimeState{};
+        ggrs_time.elapsed_ns = elapsed_ns;
+        if (has_particle_rng)
+            for (int i = 0; i < 4; ++i) particle_rng.s[i] = rng[i];
+        for (auto& s : comp_snaps) s.clear();
+        entity_snaps.clear();
+        ordered_snaps.clear();
+        time_snaps.clear();
+        rng_snaps.clear();
+        for (auto& s : res_snaps) s.clear();
+        snapshot_world();
+    }
+
     // despawn commands applied at a flush point; Bevy tables swap_remove, so process rows descending
     void apply_despawns(std::vector<size_t>& rows_to_kill) {
         std::sort(rows_to_kill.begin(), rows_to_kill.end());

@@ -15,14 +15,18 @@ What is compared:
     every first image: the twin's;
   - feed records and FeedInfo: the FeedModel's on the oracle's world, and a Replica that applies them must match it;
   - desync diffs, digests, retained frames: the oracle's; export blobs: the twin's, and ``diff_remote`` of the engine's
-    blob on the twin finds nothing.
+    blob on the twin finds nothing;
+  - with ``Config.checkpoints``: checkpoint blobs, byte for byte the twin's and the oracle's (``checkpoint_of``), and
+    restores of kept blobs into all three worlds (``FlagsOracle.restore``), refused with submits pending or a corrupt
+    payload; with ``Config.input_replays``: input-log replays, their checksums the oracle's (``FlagsOracle.replay``).
 
 The host bookkeeping behind the skipped work (passive-plane versions, content stamps, the deferred live image) is what
 these interleavings exercise; a stale record does not fault, it skips a store, so only a comparison finds it.  Each run
 counts what it reached (``Interleaving.tally``) so that a test can assert that it reached it.
 
 ``Fleet`` runs several such worlds with one registration as the members of one world batch (``EngineBatch``): batched
-calls over random subsets of them, refused batched calls, and each member's own actions in between.
+calls over random subsets of them, refused batched calls, and each member's own actions in between; with
+``FleetConfig.match_state`` also batched replays (and refused ones) and restores of one member's checkpoint into another.
 
 ``REPLAY_ENV`` ("<configuration>:<seed>") restricts a test module to one configuration and seed.
 
@@ -40,8 +44,9 @@ import numpy as np
 from bevy_ggrs_b200 import capi
 from bevy_ggrs_b200.capi import BgrError
 from bevy_ggrs_b200.session import ADVANCE, LOAD, SAVE, P2PTraceSession, Request, SyncTestSession
+import checkpoint_codec as cc
 from change_feed_model import FeedModel, Replica, world_of
-from oracle_backend import OracleWorld
+from oracle_backend import OracleError, OracleWorld
 from oracle_desync import _is_older
 from oracle_p2p import BLOCK, RetainOracleWorld
 
@@ -119,6 +124,11 @@ class Config:
     fps: int = 60                       # bgr_config.fps: Time<GgrsTime>'s dt reaches the systems through each Advance
     order_base: int = 0                 # bgr_config.order_base: the RollbackOrdered index of row 0 (no spawns past the
                                         # first vector then, so the generator draws none)
+    checkpoints: bool = False           # draw checkpoint saves and restores (off: the action log of a seed is unchanged)
+    input_replays: bool = False         # draw input-log replays (bgr_replay)
+    max_log: int = 300                  # frames of the longest input log a replay draws (the oracle advances each one)
+    oracle_blobs: int = 1_000_000       # checkpoints restated by the oracle per run (a Python loop over every row); only
+                                        # those are kept for restores
 
 
 class FlagsOracle(RetainOracleWorld):
@@ -150,6 +160,65 @@ class FlagsOracle(RetainOracleWorld):
             self._first.setdefault(frame, snap)
             self._latest[frame] = snap
         return out
+
+    def replay(self, log, k: int) -> List[Tuple[int, int]]:
+        """bgr_replay restated: for frame f0 + j, the checksum alone (no snapshot) if k and (f0 + j) % k == 0, then an
+        Advance with log[j] outside any session (neither the depth nor the confirmed frame moves).  A non-finite value
+        at a checksum frame raises BGR_ERR_NON_FINITE after the whole log ran, naming the first such frame."""
+        log = np.asarray(log, np.uint8)
+        f0, out, bad = self.rollback_frame_count(), [], None
+        for j in range(log.shape[0]):
+            if k and (f0 + j) % k == 0:
+                try:
+                    out.append(self.checksum_world())
+                except OracleError as ex:
+                    if ex.status != capi.BGR_ERR_NON_FINITE:
+                        raise
+                    bad = f0 + j if bad is None else bad
+            OracleWorld.handle_requests(self, NOSESS, [Request(ADVANCE, 0, [int(v) for v in log[j]])])
+        if bad is not None:
+            raise OracleError(capi.BGR_ERR_NON_FINITE, f"non-finite value at the checksum of frame {bad}")
+        return out
+
+    def restore(self, blob: bytes) -> None:
+        """bgr_checkpoint_restore restated from the numpy decoder (checkpoint_codec.decode): the table, RollbackOrdered,
+        Time and ParticleRng of the blob, one snapshot of its frame, which is also the frame's first image; retained
+        frames and every other first image are released."""
+        h, planes, mask = cc.decode(blob)
+        rows, words = h["rows"], planes.shape[1]
+        per_row = np.ascontiguousarray(planes.transpose(0, 2, 1)).reshape(-1, words)[:rows]
+        cols, w0 = [], 0
+        for eb in self.elem_bytes:
+            cw = (eb + 3) // 4
+            cols.append(np.ascontiguousarray(per_row[:, w0:w0 + cw]).view(np.uint8).reshape(rows, 4 * cw)[:, :eb])
+            w0 += cw
+        self.restore_world(h["frame"], mask.reshape(-1)[:rows], self.absent_bit, cols, h["elapsed_ns"], h["rng"])
+        snap = self._snapshot(h["frame"])
+        self._first, self._latest, self._retained = {h["frame"]: snap}, {h["frame"]: snap}, []
+
+    def checkpoint_of(self, frame: int, layout: int, rng: Sequence[int]) -> Optional[bytes]:
+        """The checkpoint blob of a held frame from the oracle alone: the canonical image of its snapshot, its rows,
+        existing rows, Time and the seahash of its digest words; ``layout`` and ``rng`` (ParticleRng, which the
+        snapshots do not hold) come from the caller."""
+        snap = self.image(frame)
+        if snap is None:
+            return None
+        rows = snap["rows"]
+        n_blocks = -(-rows // BLOCK)
+        words = sum(c[0].shape[1] for c in snap["cols"])
+        planes = np.zeros((n_blocks * BLOCK, words), np.uint32)
+        w0 = 0
+        for padded, _, _ in snap["cols"]:
+            planes[:rows, w0:w0 + padded.shape[1]] = padded
+            w0 += padded.shape[1]
+        planes = np.ascontiguousarray(planes.reshape(n_blocks, BLOCK, words).transpose(0, 2, 1))
+        mask = self._masks(snap, n_blocks * BLOCK).astype(np.uint8).reshape(n_blocks, BLOCK)
+        absent = np.concatenate([[b] * ((eb + 3) // 4) for b, eb in zip(self.absent_bit, self.elem_bytes)]).astype(np.uint32)
+        planes, mask = cc.canonical(planes, mask, rows, absent)
+        _, active, digest = RetainOracleWorld.frame_digest(self, frame)
+        root = self._seahash(np.ascontiguousarray(digest, "<u8").tobytes())
+        return cc.encode(planes, mask, layout=layout, frame=frame, rows=rows, n_columns=len(self.elem_bytes), fps=self.fps,
+                         active=active, elapsed_ns=snap["elapsed"], rng=tuple(rng), digest_root=root)
 
 
 def _inputs_spawn(rng, rate: int) -> int:
@@ -202,6 +271,7 @@ class Interleaving:
         self.last_way: Optional[str] = None   # "solo" / "batched": how the last vector ran
         self.tally: Counter = Counter()
         self.digests_left = cfg.digests
+        self.oracle_blobs_left = cfg.oracle_blobs
         self.last_cap = self.eng.capacity()[0]
         self.tally["stamp_rollovers"] = 0
         self.witnesses, self.retained = set(), set()
@@ -211,6 +281,8 @@ class Interleaving:
         self.rollover_launch: Optional[Tuple[int, int, int, bool]] = None   # (trace row, all units, Saves' units, exact)
         self.rollover_pending = False   # the range rolled over at a materialisation: the next vector is checked
         self.was_stamped = None                            # the last vector ran with stamps (None: none yet)
+        self.blobs: List[Tuple[int, int, bytes]] = []      # (step, rows, blob) of the last checkpoints taken
+        self.before_replay: set = set()                    # held frames saved before the last replay, not saved since
         if cfg.stamped:
             self.eng.trace_enable(TRACE_CAP)
 
@@ -249,6 +321,8 @@ class Interleaving:
     def one_step(self) -> None:
         if self.rollover_due():   # the launch the stamp range rolls over at is a plain tick (pick_vector)
             return self.act_vector()
+        if (self.cfg.checkpoints or self.cfg.input_replays) and self.rng.random() < 0.2:
+            return self.act_match_state()
         r = self.rng.random()
         actions = [(0.30, self.act_vector), (0.14, self.act_queued), (0.22, self.act_host_write), (0.22, self.act_read),
                    (0.07, self.act_frame_state), (0.05, self.act_vector_long)]
@@ -335,6 +409,9 @@ class Interleaving:
 
     # ------------------------------------------------------------------ request vectors
     def _oracle_vector(self, info, reqs) -> List[Tuple[int, int]]:
+        if reqs and reqs[0].kind == LOAD and reqs[0].frame in self.before_replay:
+            self.tally["loads_across_replay"] += 1
+        self.before_replay -= {q.frame for q in reqs if q.kind == SAVE}
         out = self.orc.handle_requests(info, reqs)
         self.max_rows = max(self.max_rows, self.orc.row_count())
         return out
@@ -522,6 +599,8 @@ class Interleaving:
                     self.act_read()
                 elif r < 0.65:
                     self.act_host_write()
+                if self.cfg.checkpoints and self.rng.random() < 0.15:
+                    self.act_checkpoint()
         while self.pending:
             n = int(self.rng.integers(1, len(self.pending) + 1))
             self.note(f"  collect {n} of {len(self.pending)}")
@@ -535,8 +614,13 @@ class Interleaving:
     def try_refused(self) -> None:
         self.note("  handle_requests / reset_session with vectors pending: refused")
         before = (self.eng.snapshot_frames(), self.eng.rollback_frame_count(), self.eng.confirmed_frame_count())
-        for call in (lambda: self.eng.handle_requests(NOSESS, [Request(SAVE, self.frame()), Request(ADVANCE, 0, [0])]),
-                     self.eng.reset_session):
+        calls = [lambda: self.eng.handle_requests(NOSESS, [Request(SAVE, self.frame()), Request(ADVANCE, 0, [0])]),
+                 self.eng.reset_session]
+        if self.cfg.checkpoints and self.blobs:
+            calls.append(lambda: self.eng.restore(self.blobs[-1][2]))
+        if self.cfg.input_replays:
+            calls.append(lambda: self.eng.replay(np.zeros((3, 1), np.uint8), 1))
+        for call in calls:
             try:
                 call()
             except BgrError as ex:
@@ -546,6 +630,201 @@ class Interleaving:
         after = (self.eng.snapshot_frames(), self.eng.rollback_frame_count(), self.eng.confirmed_frame_count())
         self.check(after == before, "a refused call changed the frame state")
         self.tally["refusals"] += 1
+        self.tally["restore_refusals"] += bool(self.cfg.checkpoints and self.blobs)
+
+    # ------------------------------------------------------------------ checkpoints and replays
+    def act_match_state(self) -> None:
+        """One of the entry points that write or read a whole match: a checkpoint, a restore or an input-log replay."""
+        acts = ([self.act_checkpoint, self.act_restore] if self.cfg.checkpoints else []) + \
+               ([self.act_input_replay] if self.cfg.input_replays else [])
+        acts[int(self.rng.integers(0, len(acts)))]()
+
+    def _held(self) -> List[int]:
+        return sorted(set(self.orc.snapshot_frames()) | set(self.orc.retained_frames()))
+
+    def act_checkpoint(self) -> None:
+        """The checkpoint of a queued, a retained or an unheld frame (past the ring, or below it: evicted or confirmed
+        away) on the engine and the twin: byte for byte the same, and the oracle's own blob of that frame (within the
+        oracle-blob budget).  Only blobs the oracle restated are kept for act_restore."""
+        rng, queued, ret = self.rng, self.orc.snapshot_frames(), self.orc.retained_frames()
+        held = self._held()
+        below = [g for g in range(max(0, min(held, default=0) - 16), min(held, default=0)) if g not in held]
+        r = rng.random()
+        if r < 0.08 and below:
+            f = int(rng.choice(below))
+        elif r < 0.15 or not queued:
+            f = max(held + [self.frame()]) + 1 + int(rng.integers(0, 4))
+        elif ret and r < 0.4:
+            f = int(rng.choice(ret))
+        else:
+            f = int(rng.choice(queued))
+        held = f in held
+        self.note(f"{'  ' if self.pending else ''}checkpoint of frame {f}{'' if held else ' (no image holds it)'}"
+                  f"{' (vectors in flight)' if self.pending else ''}")
+        blob, tblob = self.eng.checkpoint(f), self.twin.checkpoint(f)
+        if not held:
+            self.check(blob is None and tblob is None, f"a checkpoint of frame {f}, which no image holds, was written")
+            self.tally["checkpoint_none"] += 1
+            self.tally["checkpoint_none_below"] += f < self.frame()
+            return
+        self.check(blob is not None and tblob is not None, f"no checkpoint of the held frame {f}")
+        self.check(blob == tblob, f"the checkpoint of frame {f} differs from the twin's ({self._blob_diff(blob, tblob)})")
+        self.tally["checkpoints"] += 1
+        self.tally["checkpoints_in_flight"] += bool(self.pending)
+        if self.oracle_blobs_left <= 0:
+            return
+        self.oracle_blobs_left -= 1
+        h = cc.unpack_header(tblob)   # ParticleRng and the layout fingerprint: the oracle's snapshots hold neither
+        expect = self.orc.checkpoint_of(f, h["layout"], h["rng"])
+        self.check(blob == expect, f"the checkpoint of frame {f} differs from the oracle's ({self._blob_diff(blob, expect)})")
+        self.tally["checkpoints_oracle"] += 1
+        self.blobs.append((self.step, h["rows"], expect))
+        del self.blobs[:-3]
+
+    def _blob_diff(self, a: bytes, b: bytes) -> str:
+        ha, hb = cc.unpack_header(a), cc.unpack_header(b)
+        fields = [k for k in cc.HEADER_FIELDS if ha[k] != hb[k]]
+        if fields:
+            return "header fields " + ", ".join(f"{k} {ha[k]} != {hb[k]}" for k in fields)
+        _, pa, ma = cc.decode(a)
+        _, pb, mb = cc.decode(b)
+        blk, plane, row = np.nonzero(pa != pb)
+        mrow = np.nonzero(ma != mb)
+        return f"payload: planes differ at (block, plane, row) {list(zip(blk, plane, row))[:4]}, masks at {list(zip(*mrow))[:4]}"
+
+    def _frame_state(self, x) -> tuple:
+        return (x.snapshot_frames(), x.rollback_frame_count(), x.confirmed_frame_count(), x.row_count(), x.capacity()[0])
+
+    def act_restore(self) -> None:
+        """Restores a kept checkpoint (the oracle's own blob, which the engine's equalled) into the engine, the twin and
+        the oracle, preferring one whose row count differs from the current one (taken before spawns, growth or host
+        writes); sometimes first a copy with one payload bit flipped, which must be refused without changing anything."""
+        if not self.blobs:
+            return self.act_checkpoint()
+        rng, rows = self.rng, self.orc.row_count()
+        older = [b for b in self.blobs if b[1] != rows]
+        pool = older if older and rng.random() < 0.8 else self.blobs
+        step, brows, blob = pool[int(rng.integers(0, len(pool)))]
+        frame = cc.unpack_header(blob)["frame"]
+        if rng.random() < 0.3:
+            self.try_corrupt_restore(blob)
+        self.note(f"restore the checkpoint of frame {frame} taken at step {step} ({brows} rows, {rows} now)")
+        self.restore_all(blob)
+        self.tally["restores"] += 1
+        self.tally["restores_older_rows"] += brows != rows
+
+    def restore_all(self, blob: bytes) -> None:
+        """``blob`` (one the oracle wrote) restored into the engine, the twin and the oracle, then compared."""
+        self.eng.restore(blob)
+        self.twin.restore(blob)
+        self.orc.restore(blob)
+        # the restore drops a pending deferred live image (image 0 is overwritten): no materialisation, no stamps taken
+        self.deferred_tail = None
+        self.witnesses, self.retained = set(self.orc._first), set(self.orc.retained_frames())
+        self.before_replay = set()
+        self.max_rows = max(self.max_rows, self.orc.row_count())
+        self.note_growth()
+        self.compare_live(0, self.orc.row_count())   # image 0 and the restored slot: the blob's world
+        self.act_peek([cc.unpack_header(blob)["frame"]])
+
+    def try_corrupt_restore(self, blob: bytes) -> None:
+        """A payload bit flipped where the decoded content changes (the decoder canonicalises, so a bit of a row that
+        does not exist may not): BGR_ERR_INVALID_ARGUMENT, and nothing changes."""
+        h, planes, mask = cc.decode(blob)
+        ref = cc.canonical(planes, mask, h["rows"], self.absent_planes())
+        prefix = cc.HEADER.size + 8 * (h["n_blocks"] + 1)
+        if len(blob) <= prefix:
+            return
+        for _ in range(8):
+            pos = prefix + int(self.rng.integers(0, len(blob) - prefix))
+            bad = bytearray(blob)
+            bad[pos] ^= 1 << int(self.rng.integers(0, 8))
+            bad = bytes(bad)
+            try:
+                h2, p2, m2 = cc.decode(bad)
+            except cc.CodecError:
+                break
+            got = cc.canonical(p2, m2, h2["rows"], self.absent_planes())
+            if not (np.array_equal(got[0], ref[0]) and np.array_equal(got[1], ref[1])):
+                break
+        else:
+            return
+        self.note(f"restore a checkpoint with payload byte {pos - prefix} corrupted: refused")
+        before = self._frame_state(self.eng)
+        try:
+            self.eng.restore(bad)
+        except BgrError as ex:
+            self.check(ex.status == capi.BGR_ERR_INVALID_ARGUMENT, f"a corrupt checkpoint was refused with {ex.status}")
+        else:
+            self.fail("a checkpoint with a corrupt payload was restored")
+        self.check(self._frame_state(self.eng) == before, "a refused restore changed the frame state")
+        self.tally["restore_refusals"] += 1
+
+    def absent_planes(self) -> np.ndarray:
+        return cc.plane_absent(self.world.sizes, self.world.optional)
+
+    def act_input_replay(self) -> None:
+        """An input log of 1..120 frames (on small worlds sometimes 81..300, past one chunk of the fallback), 1..4
+        players, checksum interval 0, 1, 2..12 or past the log, spawn bits while the rows fit, on the engine, the twin
+        and the oracle; on a fixed engine sometimes a spawning log past its capacity, which is refused."""
+        rng, w, f0, rows = self.rng, self.world, self.frame(), self.orc.row_count()
+        n = int(rng.integers(1, min(120, self.cfg.max_log) + 1))
+        if rows < 5000 and self.cfg.max_log >= 300 and rng.random() < 0.25:
+            n = int(rng.integers(81, 301))
+        k = [0, 1, int(rng.integers(2, 13)), f0 + n + int(rng.integers(1, 50))][int(rng.integers(0, 4))]
+        players = int(rng.integers(1, 5))
+        log = rng.integers(0, 16, (n, players), dtype=np.uint8)
+        rate = w.spawn_rate if self.cfg.order_base == 0 else 0
+        if rate and not self.growable and rng.random() < 0.15:
+            return self.replay_past_capacity(players)
+        spawns = 0
+        if rate and rng.random() < 0.6:
+            room = max(0, self.room() - 100) // rate
+            frames = rng.permutation(n)[:min(n, room, int(rng.integers(1, 40)))]
+            log[frames, rng.integers(0, players, len(frames))] |= capi.BGR_INPUT_SPAWN
+            spawns = len(frames)
+        self._touch()   # the replay materialises a pending deferred live image first
+        held = set(self._held())
+        expect = self.orc.replay(log, k)
+        self.note(f"input log of {n} frames x {players} players from frame {f0}, checksum interval {k}, {spawns} spawning "
+                  f"({len(expect)} checksums)")
+        self.max_rows = max(self.max_rows, self.orc.row_count())
+        got = self.eng.replay(log, k)
+        self.check(got == expect, f"replay checksums differ from the oracle's at "
+                                  f"{[e[0] for e, g in zip(expect, got) if e != g][:4]} ({len(got)} vs {len(expect)})")
+        self.check(self.twin.replay(log, k) == expect, "the twin's replay checksums differ from the oracle's")
+        lk = self.eng.last_kernel()
+        if self.cfg.kind is not None and n:
+            fast = self.cfg.kind in ("bundle", "generic_nvrtc")
+            self.check(lk.replay == fast, f"the replay ran {'on the replay kernel' if lk.replay else 'in chunks'} on {self.cfg.kind}")
+        self.before_replay = held
+        self.note_growth()
+        queued = [g for g in self.orc.snapshot_frames() if g in held]
+        if queued and self.rng.random() < 0.5 and not self.rollover_due():   # back to a frame saved before the replay
+            g = int(self.rng.choice(queued))
+            inp = [int(v) for v in self.rng.integers(0, 16, 2)]
+            self.run_vector(NOSESS, [Request(LOAD, g), Request(ADVANCE, 0, inp[:1]), Request(SAVE, g + 1),
+                                     Request(ADVANCE, 0, inp[1:])], "load_across_replay")
+        self.tally["input_replays"] += 1
+        self.tally["input_replays_fast"] += lk.replay
+        self.tally["input_replays_chunked"] += (not lk.replay) and n > MAX_REQUESTS
+        self.tally["input_replays_spawning"] += spawns > 0
+
+    def replay_past_capacity(self, players: int) -> None:
+        """Every frame spawning until the rows pass the fixed engine's capacity: BGR_ERR_CAPACITY, nothing runs."""
+        rate, rows, cap = self.world.spawn_rate, self.orc.row_count(), self.eng.capacity()[0]
+        n = (cap - rows) // rate + 2
+        log = np.full((n, players), capi.BGR_INPUT_SPAWN, np.uint8)
+        self.note(f"input log of {n} spawning frames from {rows} rows, past the capacity {cap}: refused")
+        before = self._frame_state(self.eng) + (self.eng.launch_count(),)
+        try:
+            self.eng.replay(log, 1)
+        except BgrError as ex:
+            self.check(ex.status == capi.BGR_ERR_CAPACITY, f"a replay past the capacity returned {ex.status}")
+        else:
+            self.fail("a replay that spawns past a fixed engine's capacity was accepted")
+        self.check(self._frame_state(self.eng) + (self.eng.launch_count(),) == before, "a refused replay changed the engine")
+        self.tally["replay_refusals"] += 1
 
     # ------------------------------------------------------------------ host writers
     def all3(self, fn) -> None:
@@ -897,6 +1176,7 @@ class FleetConfig:
     members: List[Config]
     env: Dict[str, str] = field(default_factory=dict)
     steps: int = 80
+    match_state: bool = False   # draw batched replays and restores of one member's checkpoint into another
 
 
 class Fleet:
@@ -924,7 +1204,7 @@ class Fleet:
                                 "kind": None, "stamped": False})
                 m = Interleaving(cfg, seed, lambda role, *a, _i=i, **kw: new_engine(_i, role, *a, **kw))
                 m.log, m.tag = self.log, f"w{i} "
-                m.between_submits = lambda _i=i: self.act_batch(exclude=_i)
+                m.between_submits = lambda _i=i: self.act_between(_i)
                 self.members.append(m)
             self.batch = new_batch([m.eng for m in self.members])
         except BaseException:
@@ -970,9 +1250,123 @@ class Fleet:
             m.close()
 
     def one_step(self) -> None:
+        if self.fcfg.match_state and self.rng.random() < 0.15:
+            return self.act_batch_replay() if self.rng.random() < 0.5 else self.act_cross_restore()
         if self.rng.random() < 0.45:
             return self.act_batch()
         self.members[int(self.rng.integers(0, len(self.members)))].one_step()
+
+    def act_between(self, exclude: int) -> None:
+        """Another worlds' batched call while member ``exclude`` has submits in flight on the shared stream."""
+        if self.fcfg.match_state and self.rng.random() < 0.3:
+            return self.act_batch_replay(exclude)
+        return self.act_batch(exclude)
+
+    def act_batch_replay(self, exclude: Optional[int] = None) -> None:
+        """bgr_batch_replay over a random subset, each listed world with its own input log (1..60 frames, 1..4 players,
+        checksum interval 0, 1 or 2..12): every world's checksums are its oracle's and its twin's.  Sometimes one
+        world's log has 9 players: the call is refused, names that world and changes nothing anywhere."""
+        rng = self.rng
+        avail = [i for i in range(len(self.members)) if i != exclude]
+        if not avail:
+            return
+        k = int(rng.integers(1, len(avail) + 1))
+        worlds = [avail[int(j)] for j in rng.permutation(len(avail))[:k]]
+        calls = []
+        for i in worlds:
+            n, players = int(rng.integers(1, 61)), int(rng.integers(1, 5))
+            calls.append((i, rng.integers(0, 16, (n, players), dtype=np.uint8), [0, 1, int(rng.integers(2, 13))][int(rng.integers(0, 3))]))
+        if rng.random() < 0.15:
+            return self.act_batch_replay_refused(calls, exclude)
+        self.note(f"batched replay over worlds {worlds}" + (f" (w{exclude} has submits in flight)" if exclude is not None else ""))
+        expected = []
+        for i, log, kk in calls:
+            m = self.members[i]
+            m.note(f"batched input log of {len(log)} frames x {log.shape[1]} players, checksum interval {kk}")
+            m._touch()
+            held = set(m._held())
+            expected.append((m.orc.replay(log, kk), held))
+            m.max_rows = max(m.max_rows, m.orc.row_count())
+        res = self.batch.replay(calls)
+        self.check(len(res) == len(calls), f"{len(res)} results for {len(calls)} worlds")
+        for (i, log, kk), (status, got), (expect, held) in zip(calls, res, expected):
+            m = self.members[i]
+            m.check(status == capi.BGR_OK, f"world {i}: batched replay status {status}")
+            m.check(got == expect, f"world {i}: batched replay checksums differ from the oracle's ({len(got)} vs {len(expect)})")
+            m.check(m.twin.replay(log, kk) == expect, f"world {i}: the twin's replay checksums differ from the oracle's")
+            lk = m.eng.last_kernel()
+            if self.specialised:
+                m.check(lk.replay and lk.batched, f"world {i}: a specialised batch's replay ran {lk}")
+            else:
+                m.check(not lk.batched, f"world {i}: an unspecialised batch reported a batched replay")
+            m.before_replay = held
+            m.note_growth()
+            m.tally["input_replays"] += 1
+            m.tally["input_replays_batched"] += 1
+        self.tally["batch_replays"] += 1
+        if exclude is not None:
+            self.tally["batch_replays_with_queued_member"] += 1
+
+    def act_batch_replay_refused(self, calls, exclude: Optional[int]) -> None:
+        j = int(self.rng.integers(0, len(calls)))
+        bad, log, kk = calls[j]
+        calls[j] = (bad, np.zeros((len(log), capi.BGR_MAX_PLAYERS + 1), np.uint8), kk)
+        self.note(f"batched replay over worlds {[c[0] for c in calls]}, w{bad} with {capi.BGR_MAX_PLAYERS + 1} players: refused")
+        state = lambda: [(m.eng.launch_count(), m.eng.snapshot_frames(), m.eng.rollback_frame_count(), m.eng.row_count(),
+                          m.eng.confirmed_frame_count()) for m in self.members]
+        before = state()
+        try:
+            self.batch.replay(calls)
+        except BgrError as ex:
+            self.check(ex.status == capi.BGR_ERR_INVALID_ARGUMENT, f"the refused batched replay returned {ex.status}")
+            self.check(str(ex).startswith(f"world {bad}: "), f"the refusal does not name world {bad}: {ex}")
+        else:
+            self.fail(f"a batched replay in which world {bad} has {capi.BGR_MAX_PLAYERS + 1} players was accepted")
+        self.check(state() == before, "a refused batched replay changed a world")
+        self.tally["batch_replay_refusals"] += 1
+
+    def act_cross_restore(self) -> None:
+        """Member i's checkpoint restored into member j.  The same fps and order_base: j, its twin and its oracle take
+        i's world (a growable j grows to its rows); otherwise the engine refuses it (another layout or fps) and j is
+        unchanged."""
+        rng = self.rng
+        key = lambda x: (self.members[x].cfg.fps, self.members[x].cfg.order_base)
+        paired = [i for i in range(len(self.members)) if any(key(x) == key(i) for x in range(len(self.members)) if x != i)]
+        i = int(rng.choice(paired if paired and rng.random() < 0.75 else range(len(self.members))))
+        a = self.members[i]
+        if not a.blobs:
+            a.act_checkpoint()
+        if not a.blobs:
+            return self.note(f"(w{i} holds no checkpoint to restore into another world)")
+        step, rows, blob = a.blobs[int(rng.integers(0, len(a.blobs)))]
+        others = [x for x in range(len(self.members)) if x != i]
+        same = [x for x in others if key(x) == key(i)]
+        grows = [x for x in same if self.members[x].growable and self.members[x].eng.capacity()[0] < rows]
+        r = rng.random()
+        j = int(rng.choice(grows if grows and r < 0.4 else same if same and r < 0.75 else others))
+        b = self.members[j]
+        frame = cc.unpack_header(blob)["frame"]
+        same = (a.cfg.fps, a.cfg.order_base) == (b.cfg.fps, b.cfg.order_base)
+        if same and rows > b.twin_cap - 8:
+            return self.note(f"(w{i}'s checkpoint of {rows} rows does not fit w{j})")
+        self.note(f"restore w{i}'s checkpoint of frame {frame} ({rows} rows) into w{j} ({b.orc.row_count()} rows)"
+                  + ("" if same else ": another fps or order_base, refused"))
+        if not same:
+            before = b._frame_state(b.eng)
+            try:
+                b.eng.restore(blob)
+            except BgrError as ex:
+                b.check(ex.status == capi.BGR_ERR_INVALID_ARGUMENT, f"a restore from another layout or fps returned {ex.status}")
+            else:
+                b.fail(f"w{i}'s checkpoint (fps {a.cfg.fps}, order_base {a.cfg.order_base}) was restored into w{j} "
+                       f"(fps {b.cfg.fps}, order_base {b.cfg.order_base})")
+            b.check(b._frame_state(b.eng) == before, "a refused restore changed the frame state")
+            self.tally["cross_restore_refusals"] += 1
+            return
+        cap = b.eng.capacity()[0]
+        b.restore_all(blob)
+        self.tally["cross_restores"] += 1
+        self.tally["cross_restores_grown"] += b.eng.capacity()[0] > cap
 
     def act_batch(self, exclude: Optional[int] = None) -> None:
         """A batched call over a random subset (``exclude``: a member with submits in flight, never listed)."""

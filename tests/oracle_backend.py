@@ -89,6 +89,8 @@ def load_oracle() -> C.CDLL:
         "orc_reset_session": (None, [vp]),
         "orc_last_dt_bits": (u32, [vp]),
         "orc_save_world": (C.c_int, [vp, C.POINTER(capi.bgr_checksum)]),
+        "orc_checksum_world": (C.c_int, [vp, C.POINTER(capi.bgr_checksum)]),
+        "orc_restore": (C.c_int, [vp, i32, u32, vp, u32p, C.POINTER(vp), u64, u64p]),
         "orc_load_world": (C.c_int, [vp]),
         "orc_advance_world": (C.c_int, [vp, vp, u32]),
         "orc_last_partial": (C.c_int, [vp, C.POINTER(capi.bgr_partial)]),
@@ -246,6 +248,25 @@ class OracleWorld:
         cs = capi.bgr_checksum()
         self._check(self._lib.orc_save_world(self._h, C.byref(cs)))
         return cs.frame, (cs.hi << 64) | cs.lo
+
+    def checksum_world(self):
+        """The Checksum half of SaveWorld: (frame, checksum) of the current world, no snapshot pushed."""
+        cs = capi.bgr_checksum()
+        self._check(self._lib.orc_checksum_world(self._h, C.byref(cs)))
+        return cs.frame, (cs.hi << 64) | cs.lo
+
+    def restore_world(self, frame, mask, absent_bits, columns, elapsed_ns, rng):
+        """Replaces the world with a checkpoint's content (World::restore): ``mask`` one byte per row, ``absent_bits``
+        each column's mask bit (0: required), ``columns[c]`` [rows, elem_bytes] u8."""
+        rows = len(mask)
+        mask = np.ascontiguousarray(mask, np.uint8)
+        absent = np.ascontiguousarray(absent_bits, np.uint32)
+        cols = [np.ascontiguousarray(c, np.uint8).reshape(rows, eb) for c, eb in zip(columns, self.elem_bytes)]
+        ptrs = (C.c_void_p * max(1, len(cols)))(*[c.ctypes.data for c in cols])
+        words = np.ascontiguousarray(rng, np.uint64)
+        self._check(self._lib.orc_restore(self._h, frame, rows, mask.ctypes.data,
+                                          absent.ctypes.data_as(C.POINTER(C.c_uint32)), ptrs, elapsed_ns,
+                                          words.ctypes.data_as(C.POINTER(C.c_uint64))))
 
     def load_world(self):
         self._check(self._lib.orc_load_world(self._h))

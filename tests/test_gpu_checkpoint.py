@@ -386,3 +386,45 @@ def test_app_checkpoint_carries_its_resources_into_a_second_app():
         with pytest.raises(BgrError) as ei:
             call()
         assert ei.value.status == capi.BGR_ERR_UNSUPPORTED
+
+
+def test_restore_refuses_bits_past_a_sub_word_element():
+    """A column of 5 bytes holds 3 bytes of its second word that no element byte covers: the frame digest hashes the 5
+    bytes only, so a blob that sets any of them passes the digest check.  The decoder refuses it (it would otherwise
+    land in image 0, and the next checkpoint of an engine whose digests agree with the writer's would differ)."""
+    def make():
+        e = Engine(max_entities=1200, max_depth=9)
+        a = e.rollback_component("Odd", 5, capi.BGR_STRATEGY_COPY)
+        b = e.rollback_component("Score", 4, capi.BGR_STRATEGY_COPY | OPT)
+        e.checksum_component(a, 0, 5)
+        e.add_system(capi.BGR_SYS_U32_ADD, [b], [0, 1])
+        e.build()
+        e.set_depth(8)
+        e.spawn(1000)
+        rng = np.random.default_rng(3)
+        e.write_component(a, 0, rng.integers(0, 256, (1000, 5), dtype=np.uint8))
+        e.write_component(b, 0, rng.integers(0, 99, 1000, dtype=np.uint32))
+        e.remove_component(b, 17)
+        return e
+    eng, other = make(), make()
+    for _ in range(3):
+        f = eng.rollback_frame_count()
+        for x in (eng, other):
+            x.handle_requests((capi.BGR_SESSION_NONE, 0, 0, 0), [Request(SAVE, f), Request(ADVANCE, 0, [0])])
+    f = eng.snapshot_frames()[0]
+    blob = eng.checkpoint(f)
+    h, planes, mask = cc.decode(blob)
+    header = {k: h[k] for k in ("layout", "frame", "rows", "n_columns", "fps", "active", "elapsed_ns", "rng", "digest_root")}
+    for pad_bit in (8 * 5 % 32, 31):   # the lowest and the highest bit past byte 5 of word plane 1
+        bad_planes = planes.copy()
+        bad_planes[1, 1, 700 - 512] |= np.uint32(1 << pad_bit)   # row 700: exists, Odd present
+        bad = cc.encode(bad_planes, mask, **header)
+        before = (other.snapshot_frames(), other.rollback_frame_count(), other.read_component(0, 0, 1000).copy())
+        with pytest.raises(BgrError) as ei:
+            other.restore(bad)
+        assert ei.value.status == capi.BGR_ERR_INVALID_ARGUMENT, str(ei.value)
+        after = (other.snapshot_frames(), other.rollback_frame_count(), other.read_component(0, 0, 1000))
+        assert before[:2] == after[:2] and np.array_equal(before[2], after[2])
+    other.restore(blob)   # the blob as written restores, and checkpoints back to itself
+    assert other.checkpoint(f) == blob
+    eng.close(); other.close()
