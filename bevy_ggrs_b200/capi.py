@@ -144,6 +144,15 @@ class bgr_replay(C.Structure):
                 ("reserved", C.c_uint32), ("inputs", C.c_void_p)]
 
 
+class bgr_keyframe(C.Structure):
+    _fields_ = [("frame", C.c_int32), ("reserved", C.c_uint32), ("offset", C.c_uint64), ("bytes", C.c_uint64)]
+
+
+class bgr_keyframes(C.Structure):
+    _fields_ = [("interval", C.c_uint32), ("index_cap", C.c_uint32), ("reserved", C.c_uint64), ("dst", C.c_void_p),
+                ("dst_cap", C.c_size_t), ("index", C.POINTER(bgr_keyframe))]
+
+
 class bgr_feed_field(C.Structure):
     _fields_ = [("column", C.c_uint32), ("byte_offset", C.c_uint32), ("byte_len", C.c_uint32)]
 
@@ -239,6 +248,10 @@ PROTOTYPES = {
     "bgr_replay": (C.c_int, [C.c_void_p, C.POINTER(bgr_replay), C.POINTER(bgr_checksum), C.c_uint32, u32p]),
     "bgr_batch_replay": (C.c_int, [C.c_void_p, u32p, C.c_uint32, C.POINTER(bgr_replay), C.POINTER(bgr_checksum), C.c_uint32,
                                    u32p, i32p]),
+    "bgr_replay_keyframes": (C.c_int, [C.c_void_p, C.POINTER(bgr_replay), C.POINTER(bgr_keyframes), C.POINTER(bgr_checksum),
+                                       C.c_uint32, u32p, u32p, C.POINTER(C.c_size_t)]),
+    "bgr_batch_replay_keyframes": (C.c_int, [C.c_void_p, u32p, C.c_uint32, C.POINTER(bgr_replay), C.POINTER(bgr_keyframes),
+                                             C.POINTER(bgr_checksum), C.c_uint32, u32p, u32p, i32p]),
     "bgr_seahash": (C.c_uint64, [C.c_void_p, C.c_uint64]),
     "bgr_ggrs_time_delta_bits": (C.c_uint32, [C.c_uint32, C.c_int32]),
     "bgr_particle_rng_stream": (C.c_int, [C.c_uint64, C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p, C.c_float, C.c_float]),

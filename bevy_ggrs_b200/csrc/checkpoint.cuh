@@ -2,13 +2,16 @@
 // vector (each word plane, then the mask plane read as 128 u32) as CONST, SPARSE or RAW, see include/bevy_ggrs_b200.h
 // "world checkpoints".
 //
-// Save is three launches over the source slot, one 512-thread block per tile and one row per thread:
+// Save is three launches over an image table (frame_digest.cuh ImageEntry: one image for bgr_checkpoint_save, every
+// keyframe of a launch for bgr_replay_keyframes), one 512-thread block per tile of every image and one row per thread:
 //   measure (k_ckpt_measure): reads every plane of the tile once, coalesced, canonicalises in registers (words of rows
 //            that do not exist or lack the column are zero, the mask byte of a row that does not exist is zero), and
 //            decides each vector's kind with block votes: __syncthreads_and against element 0 broadcast through shared
 //            memory, __syncthreads_count for the non-zero elements.  Writes the kinds and the block's byte length.
-//   scan     (k_ckpt_scan, one block): the lengths become the u64 offsets and the total; no ordering depends on atomics.
-//   pack     (k_ckpt_pack): re-reads the tile and writes the kind bytes and the bodies at the block's offset: CONST by
+//   scan     (k_ckpt_scan, one block): the lengths of all blocks become the u64 offsets and the total; an image's own
+//            offsets are differences from its first block's.  No ordering depends on atomics.
+//   pack     (k_ckpt_pack): re-reads the tile and writes the kind bytes and the bodies at the block's offset in its
+//            image's payload (ImageEntry::out_off): CONST by
 //            one thread, the SPARSE bitmap from warp ballots with each non-zero element ranked by a popc prefix plus the
 //            warp totals in shared memory, RAW coalesced.
 // Restore is one launch (k_ckpt_unpack) per uploaded blob: warp 0 validates the kind bytes, the padding and the length
@@ -17,7 +20,7 @@
 // registered absent bits makes the block bad.  A bad block sets the error word and writes nothing.  Otherwise every
 // thread expands its row of every vector into a scratch image, canonical as above.
 #pragma once
-#include "desync_diff.cuh"
+#include "frame_digest.cuh"
 
 namespace bgr {
 
@@ -41,14 +44,16 @@ __host__ __device__ inline uint32_t ckpt_max_block_words(uint32_t words) {
 }
 
 struct CkptParams {
-    const uint8_t* img;                  // save: the source slot's image; restore: the scratch image written
-    uint32_t words, rows;
+    const ImageEntry* images;            // save: the image table
+    uint32_t n_images;
+    const uint8_t* img;                  // restore: the scratch image written
+    uint32_t words, rows;                // rows: restore
     const uint32_t* plane_absent;        // [words] the absent bit of the column each plane belongs to (0: not optional)
     const uint32_t* plane_pad;           // restore: [words] the bits of a plane's word past its column's element bytes
     uint32_t mask_bits;                  // restore: the bits a mask byte may hold (alive and the registered absent bits)
     uint8_t* kinds;                      // save: [tiles][words + 1]
-    unsigned int* lens;                  // save: [tiles] bytes of each block
-    const unsigned long long* offsets;   // [tiles + 1]
+    unsigned int* lens;                  // save: [blocks] bytes of each block
+    const unsigned long long* offsets;   // [blocks + 1]
     uint32_t* payload;
     unsigned int* err;                   // restore: lowest bad block (0xFFFFFFFF: none)
 };
@@ -70,8 +75,10 @@ __global__ void __launch_bounds__(kTileRows) k_ckpt_measure(const __grid_constan
     __shared__ uint32_t s_mask[kCkptMaskWords];
     __shared__ uint32_t s_first;
     const uint32_t tile = blockIdx.x;
-    const uint8_t* tb = p.img + size_t(tile) * tile_bytes_of(p.words);
-    const uint32_t m = diff_mask_tile(tb, p.words, tile * kTileRows + threadIdx.x, p.rows);
+    const ImageEntry& im = image_of(p.images, p.n_images, tile);
+    const uint32_t t = tile - im.first_block;
+    const uint8_t* tb = im.img + size_t(t) * tile_bytes_of(p.words);
+    const uint32_t m = diff_mask_tile(tb, p.words, t * kTileRows + threadIdx.x, im.rows);
     reinterpret_cast<uint8_t*>(s_mask)[threadIdx.x] = uint8_t(m);
     uint32_t len = ckpt_kind_words(p.words);  // thread 0's
     for (uint32_t v = 0; v <= p.words; ++v) {
@@ -125,11 +132,13 @@ __global__ void __launch_bounds__(kTileRows) k_ckpt_pack(const __grid_constant__
     __shared__ uint32_t s_mask[kCkptMaskWords];
     __shared__ uint32_t s_warp[kTileRows / 32u];
     const uint32_t tile = blockIdx.x, lane = threadIdx.x & 31u, warp = threadIdx.x >> 5;
-    const uint8_t* tb = p.img + size_t(tile) * tile_bytes_of(p.words);
-    const uint32_t m = diff_mask_tile(tb, p.words, tile * kTileRows + threadIdx.x, p.rows);
+    const ImageEntry& im = image_of(p.images, p.n_images, tile);
+    const uint32_t t = tile - im.first_block;
+    const uint8_t* tb = im.img + size_t(t) * tile_bytes_of(p.words);
+    const uint32_t m = diff_mask_tile(tb, p.words, t * kTileRows + threadIdx.x, im.rows);
     reinterpret_cast<uint8_t*>(s_mask)[threadIdx.x] = uint8_t(m);
     const uint8_t* kinds = p.kinds + size_t(tile) * (p.words + 1u);
-    uint32_t* out = p.payload + p.offsets[tile] / 4u;
+    uint32_t* out = p.payload + (im.out_off + p.offsets[tile] - p.offsets[im.first_block]) / 4u;
     const uint32_t kw = ckpt_kind_words(p.words);
     for (uint32_t i = threadIdx.x; i < kw; i += blockDim.x) {
         uint32_t k = 0;

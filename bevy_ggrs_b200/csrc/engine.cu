@@ -34,6 +34,7 @@
 #include "change_feed.cuh"
 #include "frame_digest.cuh"
 #include "checkpoint.cuh"
+#include "replay_keyframes.hpp"
 #include "jit.hpp"
 #include "vmm_range.hpp"
 #include "device_memory.hpp"
@@ -72,6 +73,11 @@ constexpr uint32_t kMaxSpawnVals = 1u << 16;  // particles spawned by one reques
 // checksum points one replay launch accumulates (64 MB of accumulators); BGR_TUNE_REPLAY_POINTS lowers it (tests of logs
 // that take several launches)
 constexpr uint32_t kReplayLaunchPoints = 1u << 20;
+
+// bytes of keyframe images one replay launch stages (bgr_replay_keyframes); a launch always holds at least one keyframe
+// of each unfinished world.  256 MB is a choice, not a measurement: a few 1M-row stress frames, or every keyframe of a
+// thousand box_game worlds over a minute.  BGR_TUNE_KEYFRAME_BYTES lowers it (tests of replays that take many launches).
+constexpr uint64_t kKeyframeLaunchBytes = 256ull << 20;
 
 constexpr uint32_t kMaxDeferredOps = 4;  // trailing ADVANCEs a deferred live image replays (SyncTest / P2P ticks: 1)
 
@@ -386,6 +392,7 @@ struct bgr_engine {
     JitKernel replay_jit, replay_jit_small;
     uint32_t tune_replay_points = 0;  // checksum points per replay launch (kReplayLaunchPoints unless BGR_TUNE_REPLAY_POINTS)
     DeviceBuffer<uint8_t> replay_stage;
+    uint64_t tune_keyframe_bytes = 0;  // keyframe images one replay launch stages (kKeyframeLaunchBytes unless BGR_TUNE_KEYFRAME_BYTES)
     DeviceBuffer<unsigned long long> replay_acc;
     const void* jit_chain_kernel = nullptr;  // the signalling launch `tiledep_chain` refers to (its work-item partition must match)
     int tune_jit_item = 0;          // 0 auto (quarter tiles below 3 tiles per SM), 512 / 256 / 128 force the rows per work item
@@ -410,6 +417,7 @@ struct bgr_engine {
     // allocated by their first use
     uint32_t retain_interval = 0, retain_count = 0;
     DeviceBuffer<DigestColumn> digest_cols;
+    DeviceBuffer<ImageEntry> digest_table;          // bgr_frame_digest's one-image table
     DeviceBuffer<unsigned long long> digest_words;  // [tiles][n_cols + 1]
     DeviceBuffer<unsigned int> digest_active;       // [tiles]
     DeviceBuffer<uint8_t> remote;                   // tiles uploaded from a peer's export blob
@@ -2142,6 +2150,7 @@ BGR_API int bgr_engine_create(const bgr_config* cfg, bgr_engine** out) {
     e->tune_jit_rows = env_int("BGR_TUNE_JIT_ROWS", 4);
     e->tune_jit_item = env_int("BGR_TUNE_JIT_ITEM", 0);
     e->tune_replay_points = uint32_t(std::max(1, env_int("BGR_TUNE_REPLAY_POINTS", int(kReplayLaunchPoints))));
+    e->tune_keyframe_bytes = uint64_t(std::max(1, env_int("BGR_TUNE_KEYFRAME_BYTES", int(kKeyframeLaunchBytes))));
     e->tune_jit_tiledep = env_int("BGR_TUNE_JIT_TILEDEP", 0);
     e->tune_passive_early = env_int("BGR_TUNE_PASSIVE_EARLY", -1);
     e->tune_stagger_ns = env_int("BGR_TUNE_STAGGER_NS", 800);
@@ -2797,10 +2806,11 @@ static uint64_t digest_layout(const bgr_engine* e) {
     return bgr_seahash(v.data(), v.size() * sizeof(uint32_t));
 }
 
-// k_frame_digest over the first ceil(rows / 512) tiles of `img`: the block words ([n_blocks][n_columns + 1]), their root
-// and the alive rows
-static int digest_image(bgr_engine* e, const uint8_t* img, uint32_t rows, std::vector<uint64_t>* words, uint64_t* root,
-                        uint64_t* active_rows) {
+// k_frame_digest over the `blocks` blocks of the device image table `d_table` (images of e's registration): the block
+// words ([blocks][n_columns + 1]) to `words` and the alive rows of each block to `active`.  Enqueued; the caller
+// synchronises before reading them.
+static int digest_launch(bgr_engine* e, const ImageEntry* d_table, uint32_t n_images, uint32_t blocks,
+                         std::vector<uint64_t>* words, std::vector<unsigned int>* active) {
     const uint32_t n_cols = uint32_t(e->cols.size()), per = n_cols + 1u;
     // dynamic shared memory: 16 warps x (n_cols + 1) words, next to the kernel's static s_warp[16] (48 KB in all)
     const size_t smem = sizeof(unsigned long long) * (kTileRows / 32u) * per;
@@ -2813,32 +2823,42 @@ static int digest_image(bgr_engine* e, const uint8_t* img, uint32_t rows, std::v
         CUDA_TRY(cudaMemcpyAsync(e->digest_cols.get(), dc.data(), sizeof(DigestColumn) * n_cols, cudaMemcpyHostToDevice, e->stream));
         CUDA_TRY(cudaStreamSynchronize(e->stream));  // `dc` goes out of scope below
     }
+    CUDA_TRY(e->digest_words.ensure(size_t(per) * std::max(e->n_tiles_cap, blocks)));
+    CUDA_TRY(e->digest_active.ensure(std::max(e->n_tiles_cap, blocks)));
+    words->assign(size_t(blocks) * per, 0);
+    active->assign(blocks, 0u);
+    if (!blocks) return BGR_OK;
+    DigestParams p{};
+    p.images = d_table;
+    p.n_images = n_images;
+    p.words = e->words;
+    p.n_cols = n_cols;
+    p.cols = e->digest_cols.get();
+    p.out = e->digest_words.get();
+    p.active = e->digest_active.get();
+    k_frame_digest<<<blocks, kTileRows, smem, e->stream>>>(p);
+    e->launches += 1;
+    CUDA_TRY(cudaGetLastError());
+    CUDA_TRY(cudaMemcpyAsync(words->data(), e->digest_words.get(), sizeof(uint64_t) * words->size(), cudaMemcpyDeviceToHost, e->stream));
+    CUDA_TRY(cudaMemcpyAsync(active->data(), e->digest_active.get(), sizeof(unsigned int) * blocks, cudaMemcpyDeviceToHost, e->stream));
+    return BGR_OK;
+}
+
+// k_frame_digest over the first ceil(rows / 512) tiles of `img`: the block words ([n_blocks][n_columns + 1]), their root
+// and the alive rows
+static int digest_image(bgr_engine* e, const uint8_t* img, uint32_t rows, std::vector<uint64_t>* words, uint64_t* root,
+                        uint64_t* active_rows) {
     const uint32_t n_blocks = e->tiles_for(rows);
-    CUDA_TRY(e->digest_words.ensure(size_t(per) * std::max(e->n_tiles_cap, n_blocks)));
-    CUDA_TRY(e->digest_active.ensure(std::max(e->n_tiles_cap, n_blocks)));
-    std::vector<uint64_t>& w = *words;
-    w.assign(size_t(n_blocks) * per, 0);
-    std::vector<unsigned int> active(n_blocks);
-    if (n_blocks) {
-        DigestParams p{};
-        p.img = img;
-        p.words = e->words;
-        p.n_cols = n_cols;
-        p.n_rows = rows;
-        p.order_base = e->cfg.order_base;
-        p.cols = e->digest_cols.get();
-        p.out = e->digest_words.get();
-        p.active = e->digest_active.get();
-        k_frame_digest<<<n_blocks, kTileRows, smem, e->stream>>>(p);
-        e->launches += 1;
-        CUDA_TRY(cudaGetLastError());
-        CUDA_TRY(cudaMemcpyAsync(w.data(), e->digest_words.get(), sizeof(uint64_t) * w.size(), cudaMemcpyDeviceToHost, e->stream));
-        CUDA_TRY(cudaMemcpyAsync(active.data(), e->digest_active.get(), sizeof(unsigned int) * n_blocks, cudaMemcpyDeviceToHost, e->stream));
-        CUDA_TRY(cudaStreamSynchronize(e->stream));
-    }
+    const ImageEntry t{img, e->cfg.order_base, 0ull, rows, 0u};
+    CUDA_TRY(e->digest_table.ensure(1));
+    CUDA_TRY(cudaMemcpyAsync(e->digest_table.get(), &t, sizeof t, cudaMemcpyHostToDevice, e->stream));
+    std::vector<unsigned int> active;
+    int rc = digest_launch(e, e->digest_table.get(), 1, n_blocks, words, &active);
+    if (rc != BGR_OK) return rc;
+    CUDA_TRY(cudaStreamSynchronize(e->stream));  // also keeps `t` alive until its upload is done
     *active_rows = 0;
     for (unsigned int a : active) *active_rows += a;
-    *root = bgr_seahash(w.data(), w.size() * sizeof(uint64_t));
+    *root = bgr_seahash(words->data(), words->size() * sizeof(uint64_t));
     return BGR_OK;
 }
 
@@ -3048,6 +3068,166 @@ static size_t checkpoint_prefix(uint32_t n_blocks) {
     return sizeof(bgr_checkpoint_header) + sizeof(uint64_t) * (size_t(n_blocks) + 1u);
 }
 
+// ---- the image-table encoder: the checkpoints of many images of one registration in four launches ----
+// k_frame_digest, k_ckpt_measure and k_ckpt_scan run once over every block of every image (one scan: an image's offsets
+// are differences from its first block's), then, with the blob sizes known on the host, k_ckpt_pack writes every payload
+// where its blob lies in host memory relative to the others (runs of blobs that follow each other there, 8-byte aligned,
+// are contiguous on the device too), and all of them come back with one copy.  Headers and offsets are written on the
+// host.
+
+// One image to encode.  The caller sets img, order_base and the header (checkpoint_header); encode_measure adds
+// active, digest_root, payload_bytes and the offsets; encode_pack writes the blob to dst.
+struct EncodeImage {
+    const uint8_t* img = nullptr;
+    unsigned long long order_base = 0;
+    bgr_checkpoint_header h{};
+    std::vector<uint64_t> offsets;
+    uint8_t* dst = nullptr;
+};
+
+static size_t blob_bytes(const EncodeImage& x) { return checkpoint_prefix(x.h.n_blocks) + x.h.payload_bytes; }
+static size_t align8(size_t v) { return (v + 7u) & ~size_t(7); }
+
+// The header of a checkpoint of e's frame `frame` with `rows` rows (active, digest_root and payload_bytes: encode_measure)
+static bgr_checkpoint_header checkpoint_header(const bgr_engine* e, int32_t frame, uint32_t rows, uint64_t elapsed_ns,
+                                               const ParticleRng& rng) {
+    bgr_checkpoint_header h{};
+    h.magic = BGR_CHECKPOINT_MAGIC;
+    h.version = BGR_CHECKPOINT_VERSION;
+    h.layout = digest_layout(e);
+    h.frame = frame;
+    h.rows = rows;
+    h.words = e->words;
+    h.n_blocks = e->tiles_for(rows);
+    h.n_columns = uint32_t(e->cols.size());
+    h.fps = e->cfg.fps;
+    h.elapsed_ns = elapsed_ns;
+    static_assert(sizeof(ParticleRng) == sizeof(h.rng), "ParticleRng is four u64 words");
+    std::memcpy(h.rng, &rng, sizeof h.rng);
+    return h;
+}
+
+// The images of one encoding and the device memory it uses (allocated by the first call that needs it, freed with the
+// encoder).  `e` gives the stream, the word planes and the columns, which every image's engine shares.
+struct ImageEncoder {
+    bgr_engine* e = nullptr;
+    std::vector<EncodeImage> im;
+    std::vector<ImageEntry> table;
+    uint32_t blocks = 0;
+    DeviceBuffer<ImageEntry> d_table;
+    DeviceBuffer<uint32_t> d_absent, d_out;
+    DeviceBuffer<uint8_t> d_kinds;
+    DeviceBuffer<unsigned int> d_lens;
+    DeviceBuffer<unsigned long long> d_offsets;
+    std::vector<unsigned long long> offsets;  // [blocks + 1] over every image
+    std::vector<uint64_t> digest;
+    std::vector<unsigned int> active;
+    CkptParams p{};
+};
+
+// digest, measure and scan: every image's digest root, active rows, offsets and payload size.  Synchronous.
+static int encode_measure(ImageEncoder& x) {
+    bgr_engine* e = x.e;
+    const uint32_t n = uint32_t(x.im.size()), per = uint32_t(e->cols.size()) + 1u;
+    x.table.resize(n);
+    x.blocks = 0;
+    for (uint32_t i = 0; i < n; ++i) {
+        const EncodeImage& m = x.im[i];
+        x.table[i] = ImageEntry{m.img, m.order_base, 0ull, m.h.rows, x.blocks};
+        x.blocks += m.h.n_blocks;
+    }
+    x.offsets.assign(size_t(x.blocks) + 1u, 0ull);
+    if (x.blocks) {
+        const std::vector<uint32_t> absent = plane_absent(e);
+        CUDA_TRY(x.d_table.ensure(n));
+        CUDA_TRY(x.d_absent.ensure(absent.size()));
+        CUDA_TRY(x.d_kinds.ensure(size_t(x.blocks) * (e->words + 1u)));
+        CUDA_TRY(x.d_lens.ensure(x.blocks));
+        CUDA_TRY(x.d_offsets.ensure(size_t(x.blocks) + 1u));
+        CUDA_TRY(cudaMemcpyAsync(x.d_table.get(), x.table.data(), sizeof(ImageEntry) * n, cudaMemcpyHostToDevice, e->stream));
+        CUDA_TRY(cudaMemcpyAsync(x.d_absent.get(), absent.data(), sizeof(uint32_t) * absent.size(), cudaMemcpyHostToDevice, e->stream));
+        int rc = digest_launch(e, x.d_table.get(), n, x.blocks, &x.digest, &x.active);
+        if (rc != BGR_OK) return rc;
+        x.p = CkptParams{};
+        x.p.images = x.d_table.get();
+        x.p.n_images = n;
+        x.p.words = e->words;
+        x.p.plane_absent = x.d_absent.get();
+        x.p.kinds = x.d_kinds.get();
+        x.p.lens = x.d_lens.get();
+        x.p.offsets = x.d_offsets.get();
+        k_ckpt_measure<<<x.blocks, kTileRows, 0, e->stream>>>(x.p);
+        k_ckpt_scan<<<1, kCkptScanBlock, 0, e->stream>>>(x.d_lens.get(), x.blocks, x.d_offsets.get());
+        e->launches += 2;
+        CUDA_TRY(cudaGetLastError());
+        CUDA_TRY(cudaMemcpyAsync(x.offsets.data(), x.d_offsets.get(), sizeof(uint64_t) * x.offsets.size(), cudaMemcpyDeviceToHost, e->stream));
+        CUDA_TRY(cudaStreamSynchronize(e->stream));  // also keeps `absent` and the table alive until their uploads are done
+    } else {
+        x.digest.clear();
+        x.active.clear();
+    }
+    for (EncodeImage& m : x.im) {
+        const ImageEntry& t = x.table[&m - x.im.data()];
+        const size_t nb = m.h.n_blocks;
+        m.h.active = 0;
+        for (size_t b = 0; b < nb; ++b) m.h.active += x.active[t.first_block + b];
+        m.h.digest_root = bgr_seahash(nb ? &x.digest[size_t(t.first_block) * per] : nullptr, nb * per * sizeof(uint64_t));
+        m.offsets.resize(nb + 1u);
+        for (size_t b = 0; b <= nb; ++b) m.offsets[b] = x.offsets[t.first_block + b] - x.offsets[t.first_block];
+        m.h.payload_bytes = m.offsets[nb];
+    }
+    return BGR_OK;
+}
+
+// pack: every image's blob to its dst (after encode_measure).  Synchronous.
+static int encode_pack(ImageEncoder& x) {
+    bgr_engine* e = x.e;
+    const size_t n = x.im.size();
+    // runs of blobs that follow each other in host memory: [first image, end), the device bytes before the run
+    struct Run { size_t first, end, base; };
+    std::vector<Run> runs;
+    size_t out_bytes = 0;
+    auto payload_at = [&](size_t i) { return x.im[i].dst + checkpoint_prefix(x.im[i].h.n_blocks); };
+    for (size_t i = 0; i < n; ++i) {
+        if (i == 0 || x.im[i].dst != x.im[i - 1].dst + align8(blob_bytes(x.im[i - 1]))) {
+            if (!runs.empty()) out_bytes += size_t(x.im[i - 1].dst + blob_bytes(x.im[i - 1]) - payload_at(runs.back().first));
+            runs.push_back(Run{i, i, out_bytes});
+        }
+        runs.back().end = i + 1;
+        x.table[i].out_off = runs.back().base + size_t(payload_at(i) - payload_at(runs.back().first));
+    }
+    if (n) out_bytes += size_t(x.im[n - 1].dst + blob_bytes(x.im[n - 1]) - payload_at(runs.back().first));
+    if (x.blocks) {
+        CUDA_TRY(x.d_out.ensure(std::max<size_t>(1, out_bytes / 4u)));
+        CUDA_TRY(cudaMemcpyAsync(x.d_table.get(), x.table.data(), sizeof(ImageEntry) * n, cudaMemcpyHostToDevice, e->stream));
+        x.p.payload = x.d_out.get();
+        k_ckpt_pack<<<x.blocks, kTileRows, 0, e->stream>>>(x.p);
+        e->launches += 1;
+        CUDA_TRY(cudaGetLastError());
+        // one copy: straight into the caller's memory for one run, else into host staging that is then scattered to the
+        // runs (one small copy per world of a batch cost more device time than the launch's replay kernel)
+        const uint8_t* d_out = reinterpret_cast<const uint8_t*>(x.d_out.get());
+        auto run_len = [&](const Run& r) { return size_t(x.im[r.end - 1].dst + blob_bytes(x.im[r.end - 1]) - payload_at(r.first)); };
+        if (runs.size() == 1) {
+            if (out_bytes) CUDA_TRY(cudaMemcpyAsync(payload_at(0), d_out, out_bytes, cudaMemcpyDeviceToHost, e->stream));
+            CUDA_TRY(cudaStreamSynchronize(e->stream));
+        } else {
+            std::vector<uint8_t> stage(out_bytes);
+            CUDA_TRY(cudaMemcpyAsync(stage.data(), d_out, out_bytes, cudaMemcpyDeviceToHost, e->stream));
+            CUDA_TRY(cudaStreamSynchronize(e->stream));
+            for (const Run& r : runs) std::memcpy(payload_at(r.first), stage.data() + r.base, run_len(r));
+        }
+    }
+    for (size_t i = 0; i < n; ++i) {  // the headers, the offsets and the zero padding between blobs of a run
+        EncodeImage& m = x.im[i];
+        std::memcpy(m.dst, &m.h, sizeof m.h);
+        std::memcpy(m.dst + sizeof m.h, m.offsets.data(), sizeof(uint64_t) * m.offsets.size());
+        if (i + 1 < n && x.im[i + 1].dst == m.dst + align8(blob_bytes(m)))
+            std::memset(m.dst + blob_bytes(m), 0, align8(blob_bytes(m)) - blob_bytes(m));
+    }
+    return BGR_OK;
+}
+
 BGR_API int bgr_checkpoint_save(bgr_engine* e, int32_t frame, void* dst, size_t dst_cap, size_t* bytes, int32_t* found) {
     if (!bytes || !found) return fail(BGR_ERR_INVALID_ARGUMENT, "null argument");
     int rc = checkpoint_args(e);
@@ -3061,65 +3241,20 @@ BGR_API int bgr_checkpoint_save(bgr_engine* e, int32_t frame, void* dst, size_t 
         *bytes = checkpoint_prefix(n_blocks) + size_t(n_blocks) * ckpt_max_block_words(e->words) * 4u;
         return BGR_OK;
     }
-    bgr_checkpoint_header h{};
-    h.magic = BGR_CHECKPOINT_MAGIC;
-    h.version = BGR_CHECKPOINT_VERSION;
-    h.layout = digest_layout(e);
-    h.frame = frame;
-    h.rows = rows;
-    h.words = e->words;
-    h.n_blocks = n_blocks;
-    h.n_columns = uint32_t(e->cols.size());
-    h.fps = e->cfg.fps;
-    h.elapsed_ns = e->st.slot_elapsed_ns[slot];
-    std::memcpy(h.rng, &e->st.slot_rng[slot], sizeof h.rng);
-    std::vector<uint64_t> digest_words;
-    rc = digest_image(e, e->image(slot + 1), rows, &digest_words, &h.digest_root, &h.active);
+    ImageEncoder x;
+    x.e = e;
+    x.im.resize(1);
+    EncodeImage& m = x.im[0];
+    m.img = e->image(slot + 1);
+    m.order_base = e->cfg.order_base;
+    m.h = checkpoint_header(e, frame, rows, e->st.slot_elapsed_ns[slot], e->st.slot_rng[slot]);
+    rc = encode_measure(x);
     if (rc != BGR_OK) return rc;
-    std::vector<uint64_t> offsets(size_t(n_blocks) + 1u, 0);
-    const std::vector<uint32_t> absent = plane_absent(e);
-    DeviceBuffer<uint32_t> d_absent, d_payload;
-    DeviceBuffer<uint8_t> d_kinds;
-    DeviceBuffer<unsigned int> d_lens;
-    DeviceBuffer<unsigned long long> d_offsets;
-    CkptParams p{};
-    if (n_blocks) {
-        CUDA_TRY(d_absent.ensure(absent.size()));
-        CUDA_TRY(d_kinds.ensure(size_t(n_blocks) * (e->words + 1u)));
-        CUDA_TRY(d_lens.ensure(n_blocks));
-        CUDA_TRY(d_offsets.ensure(size_t(n_blocks) + 1u));
-        CUDA_TRY(cudaMemcpyAsync(d_absent.get(), absent.data(), sizeof(uint32_t) * absent.size(), cudaMemcpyHostToDevice, e->stream));
-        p.img = e->image(slot + 1);
-        p.words = e->words;
-        p.rows = rows;
-        p.plane_absent = d_absent.get();
-        p.kinds = d_kinds.get();
-        p.lens = d_lens.get();
-        p.offsets = d_offsets.get();
-        k_ckpt_measure<<<n_blocks, kTileRows, 0, e->stream>>>(p);
-        k_ckpt_scan<<<1, kCkptScanBlock, 0, e->stream>>>(d_lens.get(), n_blocks, d_offsets.get());
-        e->launches += 2;
-        CUDA_TRY(cudaGetLastError());
-        CUDA_TRY(cudaMemcpyAsync(offsets.data(), d_offsets.get(), sizeof(uint64_t) * offsets.size(), cudaMemcpyDeviceToHost, e->stream));
-        CUDA_TRY(cudaStreamSynchronize(e->stream));
-    }
-    h.payload_bytes = offsets[n_blocks];
-    const size_t prefix = checkpoint_prefix(n_blocks), need = prefix + h.payload_bytes;
+    const size_t need = blob_bytes(m);
     *bytes = need;
     if (dst_cap < need) return fail(BGR_ERR_CAPACITY, "the checkpoint needs " + std::to_string(need) + " bytes");
-    uint8_t* out = static_cast<uint8_t*>(dst);
-    if (n_blocks) {
-        CUDA_TRY(d_payload.ensure(h.payload_bytes / 4u));
-        p.payload = d_payload.get();
-        k_ckpt_pack<<<n_blocks, kTileRows, 0, e->stream>>>(p);
-        e->launches += 1;
-        CUDA_TRY(cudaGetLastError());
-        CUDA_TRY(cudaMemcpyAsync(out + prefix, d_payload.get(), h.payload_bytes, cudaMemcpyDeviceToHost, e->stream));
-        CUDA_TRY(cudaStreamSynchronize(e->stream));
-    }
-    std::memcpy(out, &h, sizeof h);
-    std::memcpy(out + sizeof h, offsets.data(), sizeof(uint64_t) * offsets.size());
-    return BGR_OK;
+    m.dst = static_cast<uint8_t*>(dst);
+    return encode_pack(x);
 }
 
 BGR_API int bgr_checkpoint_restore(bgr_engine* e, const void* blob, size_t bytes) {
@@ -3493,6 +3628,12 @@ struct ReplayJob {
     std::vector<bgr_checksum> sums;
     bool bad = false;                // a checksum frame failed its finite assertion; the first is bad_frame
     int32_t bad_frame = 0;
+    // keyframes (bgr_replay_keyframes): frames f0 + j, j in [0, n), with (f0 + j) % kf->interval == 0
+    const struct bgr_keyframes* kf = nullptr;
+    std::vector<KeyframePlan> kfp;   // every keyframe of the log (replay_keyframes.hpp)
+    uint32_t n_kf = 0, kf_done = 0;  // keyframes in the log, and written
+    size_t kf_bound = 0;             // bytes the blobs may take: every vector RAW, alignment included
+    size_t kf_pos = 0, kf_end = 0;   // the next blob's offset in kf->dst, and the end of the last one
 };
 
 uint64_t ggrs_runtime_ns(const bgr_engine* e, int64_t frame) { return uint64_t(frame) * 1000000000ULL / uint64_t(e->cfg.fps); }
@@ -3502,12 +3643,18 @@ uint32_t points_in(const ReplayJob& job, uint32_t a, uint32_t b) { return replay
 // spawn frames before frame j, and RollbackOrdered::len() there
 uint32_t prefix_at(const ReplayJob& job, uint32_t j) { return job.prefix.empty() ? 0u : job.prefix[j]; }
 uint32_t rows_at(const ReplayJob& job, uint32_t j) { return job.c.rows0 + job.c.rate * prefix_at(job, j); }
+// keyframe frames f0 + j with j in [a, b): the first one (~0: none) and how many
+uint64_t first_kf(const ReplayJob& job, uint32_t a, uint32_t b) { return replay_first_point(job.c.f0, job.kf ? job.kf->interval : 0u, a, b); }
+uint32_t kfs_in(const ReplayJob& job, uint32_t a, uint32_t b) { return replay_points_in(job.c.f0, job.kf ? job.kf->interval : 0u, a, b); }
 
-// Validates a replay and computes everything the replay changes on the host, without executing or changing anything
-int replay_plan(bgr_engine* e, const struct bgr_replay* r, ReplayJob& job) {
+// Validates a replay (with keyframes when kf is not null) and computes everything the replay changes on the host,
+// without executing or changing anything
+int replay_plan(bgr_engine* e, const struct bgr_replay* r, ReplayJob& job, const struct bgr_keyframes* kf = nullptr) {
     if (!e) return fail(BGR_ERR_INVALID_ARGUMENT, "null engine");
     if (!e->built) return fail(BGR_ERR_STATE, "bgr_build has not been called");
     if (!r) return fail(BGR_ERR_INVALID_ARGUMENT, "null replay");
+    if (kf && kf->interval == 0) return fail(BGR_ERR_INVALID_ARGUMENT, "bgr_keyframes.interval must be >= 1");
+    if (kf && kf->reserved) return fail(BGR_ERR_INVALID_ARGUMENT, "bgr_keyframes.reserved must be 0");
     if ((e->cfg.flags & BGR_CFG_SHARDED) || e->group) return fail(BGR_ERR_UNSUPPORTED, "replays do not run on sharded engines");
     if (!e->pending.empty()) return fail(BGR_ERR_STATE, "bgr_replay with un-collected bgr_submit_requests pending: call bgr_collect first");
     if (r->reserved) return fail(BGR_ERR_INVALID_ARGUMENT, "bgr_replay.reserved must be 0");
@@ -3522,7 +3669,7 @@ int replay_plan(bgr_engine* e, const struct bgr_replay* r, ReplayJob& job) {
     if (n && ggrs_runtime_ns(e, int64_t(s.frame_count) + 1) < s.elapsed_ns)
         return fail(BGR_ERR_STATE, "tried to move Time<GgrsTime> backwards (RollbackFrameCount went back without LoadWorld)");
     job = ReplayJob{};
-    job.e = e; job.r = r;
+    job.e = e; job.r = r; job.kf = kf;
     uint32_t n_counter = 0;
     for (const SystemReg& sy : e->systems) n_counter += (sy.id == BGR_SYS_U32_STORE_CALL_COUNT);
     const bool spawn = e->spawn_sys >= 0;
@@ -3558,9 +3705,56 @@ int replay_plan(bgr_engine* e, const struct bgr_replay* r, ReplayJob& job) {
                 job.spawn_vals.push_back(v);
             }
     }
+    if (kf) {
+        job.kfp = plan_replay_keyframes(c, n, kf->interval, s.elapsed_ns, job.prefix, s.rng, e->words);
+        job.n_kf = uint32_t(job.kfp.size());
+        for (const KeyframePlan& p : job.kfp) job.kf_bound += p.max_bytes;
+    }
     job.elapsed_end = n ? ggrs_runtime_ns(e, int64_t(c.f0) + n) : s.elapsed_ns;
     job.n_points = points_in(job, 0, n);
     return BGR_OK;
+}
+
+// The output checks of a planned replay with keyframes, made before anything runs (a null dst holds nothing)
+int keyframe_caps(const ReplayJob& job) {
+    const struct bgr_keyframes* kf = job.kf;
+    const size_t cap = kf->dst ? kf->dst_cap : 0u;
+    if (cap < job.kf_bound)
+        return fail(BGR_ERR_CAPACITY, "the keyframes may need " + std::to_string(job.kf_bound) + " bytes, dst_cap is " + std::to_string(cap));
+    if (kf->index_cap < job.n_kf)
+        return fail(BGR_ERR_CAPACITY, "the replay writes " + std::to_string(job.n_kf) + " keyframes, index_cap is " + std::to_string(kf->index_cap));
+    if (job.n_kf && !kf->index) return fail(BGR_ERR_INVALID_ARGUMENT, "null keyframe index");
+    return BGR_OK;
+}
+
+// Encodes the keyframe images of `x` (image i is the next keyframe of owner[i]; a job's images in frame order, one after
+// another) into their jobs' buffers and indices
+int keyframes_write(ImageEncoder& x, const std::vector<ReplayJob*>& owner) {
+    int rc = encode_measure(x);
+    if (rc != BGR_OK) return rc;
+    for (size_t i = 0; i < x.im.size(); ++i) {
+        ReplayJob& job = *owner[i];
+        const size_t bytes = blob_bytes(x.im[i]);
+        x.im[i].dst = static_cast<uint8_t*>(job.kf->dst) + job.kf_pos;
+        bgr_keyframe& k = job.kf->index[job.kf_done++];
+        k.frame = x.im[i].h.frame;
+        k.reserved = 0;
+        k.offset = job.kf_pos;
+        k.bytes = bytes;
+        job.kf_end = job.kf_pos + bytes;
+        job.kf_pos = align8(job.kf_end);
+    }
+    return encode_pack(x);
+}
+
+// The image to encode for keyframe q of `job`, held at `img`
+EncodeImage keyframe_image(const ReplayJob& job, uint32_t q, const uint8_t* img) {
+    const KeyframePlan& p = job.kfp[q];
+    EncodeImage m;
+    m.img = img;
+    m.order_base = job.e->cfg.order_base;
+    m.h = checkpoint_header(job.e, job.c.f0 + int32_t(p.j), p.rows, p.elapsed_ns, p.rng);
+    return m;
 }
 
 // The replay in chunks through the engine's own kernel: each chunk is one request vector of at most kMaxOps ops,
@@ -3573,9 +3767,19 @@ int replay_chunked(ReplayJob& job) {
     std::vector<bgr_request> reqs(kMaxOps);
     Prepared p;
     Program adv;
+    ImageEncoder x;
+    x.e = e;
+    const std::vector<ReplayJob*> owner{&job};
     for (uint32_t j = 0; j < n;) {
+        if (first_kf(job, j, j + 1) == j) {  // a keyframe: image 0 as it stands before frame j, a chunk boundary
+            int rc = materialize_live(e);
+            if (rc != BGR_OK) return rc;
+            x.im.assign(1, keyframe_image(job, job.kf_done, e->image(0)));
+            rc = keyframes_write(x, owner);
+            if (rc != BGR_OK) return rc;
+        }
         uint32_t b = j, ops = 0, saves = 0, spawned = 0;
-        while (b < n) {
+        while (b < n && (b == j || first_kf(job, b, b + 1) != b)) {
             const uint32_t pt = (k && (int64_t(job.c.f0) + b) % k == 0) ? 1u : 0u;
             const uint32_t sp = prefix_at(job, b + 1) != prefix_at(job, b) ? job.c.rate : 0u;
             if (ops + pt + 1 > uint32_t(kMaxOps) || saves + pt > uint32_t(kMaxSaves) || spawned + sp > kMaxSpawnVals) break;
@@ -3666,11 +3870,16 @@ size_t align16(size_t v) { return (v + 15u) & ~size_t(15); }
 // The replays of `jobs` (every one with frames to run) on the replay entry point of `k`: the logs, spawn tables and spawn
 // values go to the device once, then each launch runs every unfinished world through its next frames, as many as keep
 // the launch's checksum points within kReplayLaunchPoints (one launch for everything but very long logs at short
-// intervals), and its checksum points come back with one copy.  Synchronous.
+// intervals), and its checksum points come back with one copy.  Replays with keyframes (every job has them, or none)
+// run k_generic_jit_replay_kf, whose launches also end where the keyframe images staged would pass the keyframe budget
+// (at least one keyframe of each unfinished world per launch); the image-table encoder then turns all of a launch's
+// keyframe images into blobs.  Synchronous.
 int replay_launch(const JitKernel& k, const std::vector<ReplayJob*>& jobs, uint32_t kernel_bits) {
     bgr_engine* e0 = jobs[0]->e;
     cudaStream_t stream = e0->stream;
-    const size_t rec_bytes = align16(sizeof(ReplayWorld) * jobs.size());
+    const bool kf = jobs[0]->kf != nullptr;
+    const size_t world_bytes = align16(sizeof(ReplayWorld) * jobs.size());
+    const size_t rec_bytes = world_bytes + (kf ? align16(sizeof(ReplayKeyframes) * jobs.size()) : 0u);
     std::vector<size_t> in_off(jobs.size()), pre_off(jobs.size()), val_off(jobs.size());
     size_t bytes = rec_bytes;
     for (size_t i = 0; i < jobs.size(); ++i) {
@@ -3699,16 +3908,23 @@ int replay_launch(const JitKernel& k, const std::vector<ReplayJob*>& jobs, uint3
     const uint32_t subs = kTileRows / uint32_t(k.item_rows);
     std::vector<uint32_t> cur(jobs.size(), 0u), seg_end(jobs.size()), seg_points(jobs.size());
     std::vector<ReplayWorld> recs;
+    std::vector<ReplayKeyframes> kf_recs;
     std::vector<size_t> rec_job, acc_off;
     std::vector<unsigned long long> acc;
+    std::vector<uint8_t> h_recs(rec_bytes);
+    ImageEncoder x;
+    x.e = e0;
+    std::vector<ReplayJob*> owner;
+    DeviceBuffer<uint8_t> kf_stage;  // the keyframe images of a launch: up to the keyframe budget, freed with the call
     for (;;) {
-        recs.clear(); rec_job.clear(); acc_off.clear();
+        recs.clear(); kf_recs.clear(); rec_job.clear(); acc_off.clear();
         uint32_t active = 0;
         for (size_t i = 0; i < jobs.size(); ++i) active += cur[i] < jobs[i]->r->n_frames ? 1u : 0u;
         if (!active) break;
         const uint32_t budget = std::max(1u, e0->tune_replay_points / active);
+        const uint64_t kf_budget = std::max<uint64_t>(1, e0->tune_keyframe_bytes / active);
         uint32_t items = 0;
-        size_t points = 0;
+        size_t points = 0, staged = 0;
         for (size_t i = 0; i < jobs.size(); ++i) {
             const ReplayJob& job = *jobs[i];
             bgr_engine* e = job.e;
@@ -3717,6 +3933,12 @@ int replay_launch(const JitKernel& k, const std::vector<ReplayJob*>& jobs, uint3
             uint32_t b = n;
             const uint64_t f = first_point(job, a, n);
             if (f != ~0ULL && f + uint64_t(budget) * kk < n) b = uint32_t(f + uint64_t(budget) * kk);  // `budget` points
+            // keyframe images hold every tile the world has by its end, so that the stride does not depend on b
+            const uint64_t stride = uint64_t(std::max(1u, e->tiles_for(uint32_t(job.rows_end)))) * e->tile_bytes;
+            if (kf) {
+                const uint64_t fk = first_kf(job, a, n), m = std::max<uint64_t>(1, kf_budget / stride), kint = job.kf->interval;
+                if (fk != ~0ULL && fk + m * kint < b) b = uint32_t(fk + m * kint);  // m keyframes
+            }
             seg_end[i] = b;
             seg_points[i] = points_in(job, a, b);
             ReplayWorld w;
@@ -3739,19 +3961,51 @@ int replay_launch(const JitKernel& k, const std::vector<ReplayJob*>& jobs, uint3
             points += seg_points[i];
             recs.push_back(w);
             rec_job.push_back(i);
+            if (kf) {
+                ReplayKeyframes r;
+                std::memset(&r, 0, sizeof r);
+                r.staging = reinterpret_cast<uint8_t*>(staged);  // an offset until the staging is sized (below)
+                r.stride = stride;
+                r.first = first_kf(job, a, b);
+                r.interval = job.kf->interval;
+                staged += size_t(kfs_in(job, a, b)) * stride;
+                kf_recs.push_back(r);
+            }
+        }
+        if (kf) {
+            CUDA_TRY(kf_stage.ensure(std::max<size_t>(1, staged)));
+            for (ReplayKeyframes& r : kf_recs) r.staging = kf_stage.get() + reinterpret_cast<size_t>(r.staging);
         }
         CUDA_TRY(e0->replay_acc.ensure(std::max<size_t>(1, points) * kAccStride));
         for (size_t ri = 0; ri < recs.size(); ++ri) recs[ri].acc = e0->replay_acc.get() + acc_off[ri] * kAccStride;
         if (points) CUDA_TRY(cudaMemsetAsync(e0->replay_acc.get(), 0, points * kAccStride * sizeof(unsigned long long), stream));
-        CUDA_TRY(cudaMemcpyAsync(d, recs.data(), sizeof(ReplayWorld) * recs.size(), cudaMemcpyHostToDevice, stream));
+        std::memcpy(h_recs.data(), recs.data(), sizeof(ReplayWorld) * recs.size());
+        if (kf) std::memcpy(h_recs.data() + world_bytes, kf_recs.data(), sizeof(ReplayKeyframes) * kf_recs.size());
+        CUDA_TRY(cudaMemcpyAsync(d, h_recs.data(), rec_bytes, cudaMemcpyHostToDevice, stream));
         const ReplayWorld* d_recs = reinterpret_cast<const ReplayWorld*>(d);
+        const ReplayKeyframes* d_kfs = reinterpret_cast<const ReplayKeyframes*>(d + world_bytes);
         uint32_t n_recs = uint32_t(recs.size());
-        void* args[] = {&d_recs, &n_recs};
-        CUDA_TRY(cudaLaunchKernel(k.replay_fn, dim3(items), dim3(k.threads), args, 0, stream));
+        void* args[] = {&d_recs, &n_recs, &d_kfs};
+        CUDA_TRY(cudaLaunchKernel(kf ? k.replay_kf_fn : k.replay_fn, dim3(items), dim3(k.threads), args, 0, stream));
         CUDA_TRY(cudaGetLastError());
         acc.resize(points * kAccStride);
         if (points) CUDA_TRY(cudaMemcpyAsync(acc.data(), e0->replay_acc.get(), points * kAccStride * sizeof(unsigned long long), cudaMemcpyDeviceToHost, stream));
         CUDA_TRY(cudaStreamSynchronize(stream));
+        if (kf) {  // the launch's keyframe images, world by world in frame order, to blobs
+            x.im.clear();
+            owner.clear();
+            for (size_t ri = 0; ri < recs.size(); ++ri) {
+                ReplayJob& job = *jobs[rec_job[ri]];
+                const ReplayKeyframes& r = kf_recs[ri];
+                const uint32_t a = cur[rec_job[ri]], b = seg_end[rec_job[ri]], m = kfs_in(job, a, b);
+                for (uint32_t q = 0; q < m; ++q) {
+                    x.im.push_back(keyframe_image(job, job.kf_done + q, r.staging + q * r.stride));
+                    owner.push_back(&job);
+                }
+            }
+            int rc = keyframes_write(x, owner);
+            if (rc != BGR_OK) return rc;
+        }
         // each checksum point through the fold bgr_handle_requests uses
         size_t off = 0;
         for (size_t ri = 0; ri < recs.size(); ++ri) {
@@ -3813,7 +4067,7 @@ int replay_run(ReplayJob& job) {
     int rc = replay_grow(one);
     if (rc != BGR_OK || job.r->n_frames == 0) return rc;
     const JitKernel* k = replay_kernel(job.e, std::max(1u, job.e->tiles_for(uint32_t(job.rows_end))));
-    if (!k) return replay_chunked(job);
+    if (!k || (job.kf && !k->replay_kf_fn)) return replay_chunked(job);
     rc = replay_launch(*k, one, BGR_KERNEL_REPLAY);
     if (rc != BGR_OK) return rc;
     return replay_commit(job);
@@ -3842,13 +4096,46 @@ BGR_API int bgr_replay(bgr_engine* e, const struct bgr_replay* r, bgr_checksum* 
     return replay_results(job, checksums_out, cap, n_out);
 }
 
-BGR_API int bgr_batch_replay(bgr_batch* b, const uint32_t* worlds, uint32_t n_worlds, const struct bgr_replay* replays,
-                             bgr_checksum* checksums_out, uint32_t cap, uint32_t* n_checksums_out, int32_t* status_out) {
+BGR_API int bgr_replay_keyframes(bgr_engine* e, const struct bgr_replay* r, const struct bgr_keyframes* kf,
+                                 bgr_checksum* checksums_out, uint32_t cap, uint32_t* n_out, uint32_t* n_keyframes_out,
+                                 size_t* bytes_out) {
+    if (n_out) *n_out = 0;
+    if (!kf || !n_keyframes_out || !bytes_out) return fail(BGR_ERR_INVALID_ARGUMENT, "null argument");
+    *n_keyframes_out = 0;
+    *bytes_out = 0;
+    NvtxRange span("Replay");
+    ReplayJob job;
+    int rc = replay_plan(e, r, job, kf);
+    if (rc != BGR_OK) return rc;  // nothing executed, nothing changed
+    if (!kf->dst) {               // the query
+        *n_keyframes_out = job.n_kf;
+        *bytes_out = job.kf_bound;
+        return BGR_OK;
+    }
+    rc = keyframe_caps(job);
+    if (rc != BGR_OK) return rc;
+    rc = replay_run(job);
+    *n_keyframes_out = job.kf_done;
+    *bytes_out = job.kf_end;
+    if (rc != BGR_OK) return rc;
+    return replay_results(job, checksums_out, cap, n_out);
+}
+
+namespace {
+
+// bgr_batch_replay, and with kfs (one per world) bgr_batch_replay_keyframes
+int batch_replay(bgr_batch* b, const uint32_t* worlds, uint32_t n_worlds, const struct bgr_replay* replays,
+                 const struct bgr_keyframes* kfs, bgr_checksum* checksums_out, uint32_t cap, uint32_t* n_checksums_out,
+                 uint32_t* n_keyframes_out, int32_t* status_out) {
     if (!b) return fail(BGR_ERR_INVALID_ARGUMENT, "null batch");
     if (n_worlds && (!worlds || !replays || !n_checksums_out || !status_out)) return fail(BGR_ERR_INVALID_ARGUMENT, "null argument");
     NvtxRange span("Replay");
     b->calls += 1;
-    for (uint32_t i = 0; i < n_worlds; ++i) { status_out[i] = BGR_OK; n_checksums_out[i] = 0; }
+    for (uint32_t i = 0; i < n_worlds; ++i) {
+        status_out[i] = BGR_OK;
+        n_checksums_out[i] = 0;
+        if (n_keyframes_out) n_keyframes_out[i] = 0;
+    }
     auto world_fail = [&](uint32_t i, int status) {
         status_out[i] = status;
         g_err = "world " + std::to_string(worlds[i]) + ": " + g_err;
@@ -3862,7 +4149,8 @@ BGR_API int bgr_batch_replay(bgr_batch* b, const uint32_t* worlds, uint32_t n_wo
             return world_fail(i, fail(BGR_ERR_INVALID_ARGUMENT, "no such world in a batch of " + std::to_string(b->engines.size())));
         if (b->listed[w] == b->calls) return world_fail(i, fail(BGR_ERR_INVALID_ARGUMENT, "listed twice in one call"));
         b->listed[w] = b->calls;
-        const int rc = replay_plan(b->engines[w], &replays[i], jobs[i]);
+        int rc = replay_plan(b->engines[w], &replays[i], jobs[i], kfs ? &kfs[i] : nullptr);
+        if (rc == BGR_OK && kfs) rc = keyframe_caps(jobs[i]);
         if (rc != BGR_OK) return world_fail(i, rc);
     }
     int first = BGR_OK;
@@ -3873,13 +4161,14 @@ BGR_API int bgr_batch_replay(bgr_batch* b, const uint32_t* worlds, uint32_t n_wo
         bgr_checksum* out = checksums_out && out_off < cap ? checksums_out + out_off : nullptr;
         if (rc == BGR_OK) rc = replay_results(jobs[i], out, out ? cap - out_off : 0u, &n);
         n_checksums_out[i] = n;
+        if (n_keyframes_out) n_keyframes_out[i] = jobs[i].kf_done;
         out_off += std::min(n, cap - std::min(out_off, cap));
         if (rc != BGR_OK) {
             world_fail(i, rc);
             if (first == BGR_OK) { first = rc; first_err = g_err; }
         }
     };
-    if (!b->k.replay_fn) {  // each world's own replay, in list order
+    if (!b->k.replay_fn || (kfs && !b->k.replay_kf_fn)) {  // each world's own replay, in list order
         for (uint32_t i = 0; i < n_worlds; ++i) results(i, replay_run(jobs[i]));
         if (first != BGR_OK) g_err = first_err;
         return first;
@@ -3895,6 +4184,20 @@ BGR_API int bgr_batch_replay(bgr_batch* b, const uint32_t* worlds, uint32_t n_wo
     for (uint32_t i = 0; i < n_worlds; ++i) results(i, BGR_OK);
     if (first != BGR_OK) g_err = first_err;
     return first;
+}
+
+}  // namespace
+
+BGR_API int bgr_batch_replay(bgr_batch* b, const uint32_t* worlds, uint32_t n_worlds, const struct bgr_replay* replays,
+                             bgr_checksum* checksums_out, uint32_t cap, uint32_t* n_checksums_out, int32_t* status_out) {
+    return batch_replay(b, worlds, n_worlds, replays, nullptr, checksums_out, cap, n_checksums_out, nullptr, status_out);
+}
+
+BGR_API int bgr_batch_replay_keyframes(bgr_batch* b, const uint32_t* worlds, uint32_t n_worlds, const struct bgr_replay* replays,
+                                       const struct bgr_keyframes* kfs, bgr_checksum* checksums_out, uint32_t cap,
+                                       uint32_t* n_checksums_out, uint32_t* n_keyframes_out, int32_t* status_out) {
+    if (n_worlds && (!kfs || !n_keyframes_out)) return fail(BGR_ERR_INVALID_ARGUMENT, "null argument");
+    return batch_replay(b, worlds, n_worlds, replays, kfs, checksums_out, cap, n_checksums_out, n_keyframes_out, status_out);
 }
 
 BGR_API int bgr_save_world(bgr_engine* e, bgr_checksum* checksum_out) {

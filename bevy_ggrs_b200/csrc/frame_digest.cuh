@@ -2,7 +2,7 @@
 // stored frame image, one u64 per registered column and one for existence / presence (see include/bevy_ggrs_b200.h
 // "P2P desync reports").  Two peers exchange these words to find the few blocks whose images differ.
 //
-// One 512-thread block per tile, one row per thread.  Every word plane of the tile is read from HBM once, coalesced (a
+// One 512-thread block per tile of every image of an image table, one row per thread.  Every word plane of the tile is read from HBM once, coalesced (a
 // warp reads 128 contiguous bytes per plane; lanes whose row does not hold the column issue no load), streaming
 // (__ldcs).  The element hash is sea_hash_stream's, fed byte by byte.
 // Each thread's per-column hash is XOR-reduced over the warp (__reduce_xor_sync on both 32-bit halves), then over the
@@ -18,13 +18,33 @@ static_assert(BGR_DIGEST_BLOCK_ROWS == kTileRows, "a digest block is one tile");
 // one registered column: its word planes, its element size (the bytes hashed) and its absent bit (0: not optional)
 struct DigestColumn { uint32_t first_plane, elem_bytes, absent; };
 
-struct DigestParams {
+// An image table: the images one launch of k_frame_digest, k_ckpt_measure or k_ckpt_pack covers, of one registration.
+// Their blocks are numbered in table order: image i holds blocks [first_block, first_block + ceil(rows / 512)).
+struct ImageEntry {
     const uint8_t* img;
-    uint32_t words, n_cols, n_rows;
-    unsigned long long order_base;
+    unsigned long long order_base;  // bgr_config.order_base of the image's engine
+    unsigned long long out_off;     // k_ckpt_pack: byte offset of the image's payload in the output
+    uint32_t rows, first_block;
+};
+static_assert(sizeof(ImageEntry) == 32, "ImageEntry layout");
+
+// the entry of global block `b` (first_block ascends; n >= 1)
+__device__ __forceinline__ const ImageEntry& image_of(const ImageEntry* t, uint32_t n, uint32_t b) {
+    uint32_t lo = 0, hi = n;
+    while (hi - lo > 1u) {
+        const uint32_t mid = (lo + hi) / 2u;
+        if (t[mid].first_block <= b) lo = mid;
+        else hi = mid;
+    }
+    return t[lo];
+}
+
+struct DigestParams {
+    const ImageEntry* images;
+    uint32_t n_images, words, n_cols;
     const DigestColumn* cols;   // [n_cols]
-    unsigned long long* out;    // [tiles][n_cols + 1]
-    unsigned int* active;       // [tiles] alive rows of each tile
+    unsigned long long* out;    // [blocks][n_cols + 1]
+    unsigned int* active;       // [blocks] alive rows of each block
 };
 
 __device__ __forceinline__ uint64_t warp_xor_u64(uint64_t v) {
@@ -38,10 +58,12 @@ __global__ void __launch_bounds__(kTileRows) k_frame_digest(const __grid_constan
     extern __shared__ unsigned long long s_part[];
     __shared__ uint32_t s_warp[kTileRows / 32u];
     const uint32_t lane = threadIdx.x & 31u, warp = threadIdx.x >> 5;
-    const uint8_t* tile = p.img + size_t(blockIdx.x) * tile_bytes_of(p.words);
-    const uint32_t row = blockIdx.x * kTileRows + threadIdx.x;
-    const uint32_t m = diff_mask_tile(tile, p.words, row, p.n_rows);
-    const uint64_t order = p.order_base + row;
+    const ImageEntry& im = image_of(p.images, p.n_images, blockIdx.x);
+    const uint32_t t = blockIdx.x - im.first_block;
+    const uint8_t* tile = im.img + size_t(t) * tile_bytes_of(p.words);
+    const uint32_t row = t * kTileRows + threadIdx.x;
+    const uint32_t m = diff_mask_tile(tile, p.words, row, im.rows);
+    const uint64_t order = im.order_base + row;
     for (uint32_t c = 0; c < p.n_cols; ++c) {
         const DigestColumn col = p.cols[c];
         uint64_t h = 0;

@@ -185,6 +185,17 @@ struct ReplayWorld {
 };
 static_assert(sizeof(ReplayWorld) == 144, "ReplayWorld layout (the engine and the NVRTC module must agree)");
 
+// The keyframes of one world's frames [j0, j1) (bgr_replay_keyframes), parallel to the ReplayWorld array and read only by
+// k_generic_jit_replay_kf: at frame first + q * interval < j1 the block stores its registers, before advancing that
+// frame, into keyframe image q at staging + q * stride.
+struct ReplayKeyframes {
+    uint8_t* staging;
+    unsigned long long stride;     // bytes per keyframe image (>= the world's tiles in this launch)
+    unsigned long long first;      // first keyframe frame >= j0 (>= j1: none)
+    uint32_t interval, reserved;
+};
+static_assert(sizeof(ReplayKeyframes) == 32, "ReplayKeyframes layout (the engine and the NVRTC module must agree)");
+
 // seahash of bytes [off, off+len) of one row's element whose words are `col[w * kTileRows]` (a column of the shared tile)
 // (__noinline__: inlined per checksummed column and per row the interpreter grew to 11k instructions — 176 KB of code,
 // more than the SM's instruction cache — and ran 2.7x slower per frame than the specialised bundle kernel)

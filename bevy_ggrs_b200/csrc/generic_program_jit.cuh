@@ -328,11 +328,14 @@ extern "C" __global__ void __launch_bounds__(BGR_JIT_ITEM_ROWS / BGR_JIT_ROWS, B
 // shared memory kReplayChunk frames at a time.  A checksum frame hashes the registers into a window of kReplayWindow
 // shared accumulators; a full window (and the last one) is folded into the world's acc[point][kAccStride] with one
 // global atomic per non-zero word.  No barrier runs on frames that are neither checksum points nor chunk starts.
+// k_generic_jit_replay_kf also stores the registers at each keyframe frame into the world's keyframe staging (one plain
+// store per row and word, no barrier, no extra read); both entry points are this one body, KF selecting the stores.
 constexpr uint32_t kReplayChunk = 256;  // frames of the log per staging step
 constexpr uint32_t kReplayWindow = 32;  // checksum points per shared window
 
-extern "C" __global__ void __launch_bounds__(BGR_JIT_ITEM_ROWS / BGR_JIT_ROWS, BGR_JIT_MINB)
-    k_generic_jit_replay(const ReplayWorld* __restrict__ worlds, uint32_t n_worlds) {
+template <bool KF>
+__device__ __forceinline__ void jit_replay(const ReplayWorld* __restrict__ worlds, uint32_t n_worlds,
+                                           const ReplayKeyframes* __restrict__ kfs) {
     constexpr int B = kJitItemRows / kJitRows;
     __shared__ unsigned int s_acc[kReplayWindow * kAccStride * 2];
     __shared__ uint8_t s_in[kReplayChunk * 8];
@@ -358,6 +361,9 @@ extern "C" __global__ void __launch_bounds__(BGR_JIT_ITEM_ROWS / BGR_JIT_ROWS, B
 
     unsigned long long next_point = w.next_point;
     uint32_t point = 0, win0 = 0;  // checksum points seen, first point of the shared window
+    unsigned long long next_kf = ~0ULL;
+    uint8_t* kf_img = nullptr;
+    if constexpr (KF) { next_kf = kfs[lo].first; kf_img = kfs[lo].staging; }
     auto flush = [&](uint32_t n) {
         __syncthreads();
         jit_fold_acc(w.acc + size_t(win0) * kAccStride, s_acc, n, tid);
@@ -381,12 +387,30 @@ extern "C" __global__ void __launch_bounds__(BGR_JIT_ITEM_ROWS / BGR_JIT_ROWS, B
             point += 1;
             next_point += interval;
         }
+        if constexpr (KF) {
+            if (j == next_kf) {  // keyframe f0 + j: the registers as they stand before the frame is advanced
+                it.store(r, kf_img);
+                kf_img += kfs[lo].stride;
+                next_kf += kfs[lo].interval;
+            }
+        }
         Op& op = s_op[tid];  // the thread's own copy: box_move indexes its inputs by row, which would put a local one on the stack
         op = replay_op(c, j, &s_in[q * np], s_pre[q]);
         it.advance(r, op, w.spawn_vals, w.spawn_ttl);
     }
     if (point > win0) flush(point - win0);
     it.store(r, w.arena);
+}
+
+extern "C" __global__ void __launch_bounds__(BGR_JIT_ITEM_ROWS / BGR_JIT_ROWS, BGR_JIT_MINB)
+    k_generic_jit_replay(const ReplayWorld* __restrict__ worlds, uint32_t n_worlds) {
+    jit_replay<false>(worlds, n_worlds, nullptr);
+}
+
+// bgr_replay_keyframes, bgr_batch_replay_keyframes: kfs[i] belongs to worlds[i]
+extern "C" __global__ void __launch_bounds__(BGR_JIT_ITEM_ROWS / BGR_JIT_ROWS, BGR_JIT_MINB)
+    k_generic_jit_replay_kf(const ReplayWorld* __restrict__ worlds, uint32_t n_worlds, const ReplayKeyframes* __restrict__ kfs) {
+    jit_replay<true>(worlds, n_worlds, kfs);
 }
 
 }  // namespace bgr

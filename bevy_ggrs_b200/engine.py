@@ -445,6 +445,27 @@ class Engine:
         self._check(self._lib.bgr_replay(self._h, C.byref(r), out, cap, C.byref(n)))
         return _checksum_list(out, 0, n.value)
 
+    def replay_keyframes(self, inputs: np.ndarray, checksum_interval: int,
+                         keyframe_interval: int) -> Tuple[List[Tuple[int, int]], List[Tuple[int, bytes]]]:
+        """``replay`` that also returns a world checkpoint (``checkpoint``'s blob) of every frame f = f0 + j, j < n, with
+        f % keyframe_interval == 0, taken before frame f is advanced: (checksums, [(frame, blob), ...]).  Both intervals
+        are required: every blob is a whole world, so the keyframe interval is the caller's memory budget.  Buffers are
+        sized by the call's query (dst NULL), which runs nothing.  A non-finite value at a checksum frame raises
+        BgrError(BGR_ERR_NON_FINITE) after the whole log ran, with the keyframes written."""
+        log = _replay_log(inputs)
+        r = capi.bgr_replay(log.shape[0], log.shape[1], checksum_interval, 0, log.ctypes.data if log.size else None)
+        kf = capi.bgr_keyframes(keyframe_interval, 0, 0, None, 0, None)
+        n_kf, size = C.c_uint32(), C.c_size_t()
+        n = C.c_uint32()
+        self._check(self._lib.bgr_replay_keyframes(self._h, C.byref(r), C.byref(kf), None, 0, C.byref(n), C.byref(n_kf),
+                                                   C.byref(size)))
+        buf, index = _keyframe_buffers(kf, n_kf.value, size.value)
+        cap = _replay_points(self.rollback_frame_count(), log.shape[0], checksum_interval)
+        out = (capi.bgr_checksum * max(1, cap))()
+        self._check(self._lib.bgr_replay_keyframes(self._h, C.byref(r), C.byref(kf), out, cap, C.byref(n), C.byref(n_kf),
+                                                   C.byref(size)))
+        return _checksum_list(out, 0, n.value), _keyframe_list(buf, index, n_kf.value)
+
     def submit_requests(self, session_info: Sequence[int], requests) -> None:
         reqs = list(requests)
         arr = capi.make_requests(reqs)
@@ -624,6 +645,56 @@ class EngineBatch:
             res.append((status[i], _checksum_list(out, k, k + n_cs[i])))
             k += n_cs[i]
         return res
+
+
+    def replay_keyframes(self, calls) -> List[Tuple[int, List[Tuple[int, int]], List[Tuple[int, bytes]]]]:
+        """``calls`` = [(world, inputs, checksum_interval, keyframe_interval), ...]: Engine.replay_keyframes of every
+        listed world in one synchronous call (one launch per keyframe budget when the batch is specialised).  Returns
+        [(status, checksums, [(frame, blob), ...]), ...] in the same order.  Each world's buffers are sized by its own
+        engine's query; a call refused before anything executed raises BgrError and changes no world."""
+        calls = [(w, _replay_log(x), k, kk) for w, x, k, kk in calls]
+        n = len(calls)
+        worlds = (C.c_uint32 * max(1, n))(*[w for w, _, _, _ in calls])
+        reps = (capi.bgr_replay * max(1, n))(*[capi.bgr_replay(x.shape[0], x.shape[1], k, 0, x.ctypes.data if x.size else None)
+                                               for _, x, k, _ in calls])
+        kfs = (capi.bgr_keyframes * max(1, n))()
+        bufs = []
+        cap = 0
+        for i, (w, x, k, kk) in enumerate(calls):
+            kfs[i].interval = kk
+            buf, index = None, None
+            if 0 <= w < len(self.engines) and kk > 0:
+                q = capi.bgr_keyframes(kk, 0, 0, None, 0, None)
+                n_kf, size, n_cs = C.c_uint32(), C.c_size_t(), C.c_uint32()
+                if self._lib.bgr_replay_keyframes(self.engines[w]._h, C.byref(reps[i]), C.byref(q), None, 0, C.byref(n_cs),
+                                                  C.byref(n_kf), C.byref(size)) == capi.BGR_OK:
+                    buf, index = _keyframe_buffers(kfs[i], n_kf.value, size.value)
+                cap += _replay_points(self.engines[w].rollback_frame_count(), x.shape[0], k)
+            bufs.append((buf, index))
+        out = (capi.bgr_checksum * max(1, cap))()
+        n_cs = (C.c_uint32 * max(1, n))()
+        n_kf = (C.c_uint32 * max(1, n))()
+        status = (C.c_int32 * max(1, n))()
+        rc = self._lib.bgr_batch_replay_keyframes(self._h, worlds, n, reps, kfs, out, cap, n_cs, n_kf, status)
+        if rc not in (capi.BGR_OK, capi.BGR_ERR_NON_FINITE):
+            self._check(rc)
+        res, k = [], 0
+        for i in range(n):
+            res.append((status[i], _checksum_list(out, k, k + n_cs[i]), _keyframe_list(bufs[i][0], bufs[i][1], n_kf[i])))
+            k += n_cs[i]
+        return res
+
+
+def _keyframe_buffers(kf: "capi.bgr_keyframes", n_kf: int, size: int):
+    """A dst of `size` bytes and an index of `n_kf` entries, installed in `kf`; the arrays must outlive the call."""
+    buf = np.empty(max(1, size), np.uint8)
+    index = (capi.bgr_keyframe * max(1, n_kf))()
+    kf.dst, kf.dst_cap, kf.index, kf.index_cap = buf.ctypes.data, size, index, n_kf
+    return buf, index
+
+
+def _keyframe_list(buf, index, n: int) -> List[Tuple[int, bytes]]:
+    return [(index[i].frame, buf[index[i].offset: index[i].offset + index[i].bytes].tobytes()) for i in range(n)]
 
 
 def _replay_log(inputs) -> np.ndarray:

@@ -483,6 +483,48 @@ public:
         return out;
     }
 
+    // replay() that also writes a world checkpoint of every frame f with f % keyframe_interval == 0, before it is
+    // advanced, to `keyframes` as (frame, blob), in order (bgr_replay_keyframes; the engine's world only, as replay()).
+    // The buffers are sized by the call's query, which runs nothing.
+    std::vector<std::pair<ggrs::Frame, unsigned __int128>> replay_keyframes(
+        const std::vector<uint8_t>& inputs, uint32_t n_players, uint32_t checksum_interval, uint32_t keyframe_interval,
+        std::vector<std::pair<ggrs::Frame, std::vector<uint8_t>>>* keyframes) {
+        finish();
+        if (!res_order_.empty() || !host_cols_.empty())
+            throw Panic(BGR_ERR_UNSUPPORTED, "replay runs the engine's world only: the App has rollback resources or host-side components");
+        if (n_players ? inputs.size() % n_players != 0 : !inputs.empty())
+            throw Panic(BGR_ERR_INVALID_ARGUMENT, "the input log is not a whole number of frames of n_players bytes");
+        struct bgr_replay r;
+        std::memset(&r, 0, sizeof r);
+        r.n_players = n_players;
+        r.n_frames = n_players ? uint32_t(inputs.size() / n_players) : 0u;
+        r.checksum_interval = checksum_interval;
+        r.inputs = inputs.data();
+        struct bgr_keyframes kf;
+        std::memset(&kf, 0, sizeof kf);
+        kf.interval = keyframe_interval;
+        uint32_t got = 0, n_kf = 0;
+        size_t bytes = 0;
+        check(bgr_replay_keyframes(engine_, &r, &kf, nullptr, 0, &got, &n_kf, &bytes));  // the query
+        std::vector<uint8_t> dst(std::max<size_t>(bytes, 1));
+        std::vector<bgr_keyframe> index(std::max<uint32_t>(n_kf, 1));
+        kf.dst = dst.data();
+        kf.dst_cap = bytes;
+        kf.index = index.data();
+        kf.index_cap = n_kf;
+        const int64_t f0 = rollback_frame_count(), n = r.n_frames, k = checksum_interval;
+        const size_t cap = k && f0 >= 0 ? size_t((f0 + n + k - 1) / k - (f0 + k - 1) / k) : 0u;
+        std::vector<bgr_checksum> cs(std::max<size_t>(cap, 1));
+        check(bgr_replay_keyframes(engine_, &r, &kf, cs.data(), uint32_t(cap), &got, &n_kf, &bytes));
+        keyframes->clear();
+        for (uint32_t i = 0; i < n_kf && i < kf.index_cap; ++i)
+            keyframes->emplace_back(index[i].frame, std::vector<uint8_t>(dst.begin() + index[i].offset,
+                                                                         dst.begin() + index[i].offset + index[i].bytes));
+        std::vector<std::pair<ggrs::Frame, unsigned __int128>> out;
+        for (uint32_t i = 0; i < got && i < cap; ++i) out.emplace_back(cs[i].frame, (static_cast<unsigned __int128>(cs[i].hi) << 64) | cs[i].lo);
+        return out;
+    }
+
     // Replaces the world and the App's resources with a checkpoint's.  The resource section is checked before the
     // engine restores, so a refused blob changes nothing.
     void restore_checkpoint(const std::vector<uint8_t>& blob) {

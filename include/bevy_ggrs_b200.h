@@ -664,6 +664,55 @@ BGR_API int bgr_replay(bgr_engine* e, const struct bgr_replay* r, bgr_checksum* 
 BGR_API int bgr_batch_replay(bgr_batch* b, const uint32_t* worlds, uint32_t n_worlds, const struct bgr_replay* replays,
                              bgr_checksum* checksums_out, uint32_t cap, uint32_t* n_checksums_out, int32_t* status_out);
 
+/* ---- replay keyframes: a world checkpoint every K frames while a replay runs ---------------------------------------
+ * bgr_replay_keyframes is bgr_replay that also writes a keyframe at each frame f0 + j, j in [0, n), with
+ * (f0 + j) % interval == 0, taken before that frame is advanced (where a checksum point is taken), so keyframes(a) then
+ * keyframes(b) equals keyframes(a ++ b).  Keyframe f is byte for byte the blob bgr_checkpoint_save(f) writes on an
+ * engine that ran the equivalent request stream with a SaveGameState{f} at that frame: the same header (frame, rows,
+ * active, elapsed_ns = Time<GgrsTime> of f, rng = ParticleRng of f, digest_root, layout, fps) and canonical payload.
+ * Everything else (checksums, live world, row count, RollbackFrameCount, Time, ParticleRng, the call counter, the ring,
+ * retained frames, witnesses, change feeds) ends exactly as after bgr_replay of the same log.  Seeking a recorded match:
+ * bgr_checkpoint_restore of the nearest keyframe at or before the target, then bgr_replay of fewer than `interval` frames.
+ *   - Output: the blobs go to dst in frame order, each at a multiple of 8 bytes; index[i] describes blob i.
+ *   - dst == NULL: nothing runs; *n_keyframes_out = the keyframe count and *bytes_out = an upper bound on the bytes
+ *     (every vector RAW, at the row count each keyframe will have, alignment included).
+ *   - Otherwise dst_cap below that bound or index_cap below the count is BGR_ERR_CAPACITY before anything runs; on
+ *     return *n_keyframes_out = the keyframes written and *bytes_out = the end of the last blob.
+ *   - Refusals change nothing: everything bgr_replay refuses, interval == 0 or reserved != 0 (BGR_ERR_INVALID_ARGUMENT)
+ *     and the capacity checks above.  BGR_CFG_SHARDED: BGR_ERR_UNSUPPORTED.
+ *   - A non-finite finite-asserted value at a checksum frame is BGR_ERR_NON_FINITE after the whole log ran; the keyframes
+ *     are written anyway, as bgr_checkpoint_save would write them.
+ * On the generated kernel (k_generic_jit_replay_kf, bgr_last_kernel carries BGR_KERNEL_REPLAY) each launch stores the
+ * registers of its keyframe frames into device staging, whose size ends a launch early (BGR_TUNE_KEYFRAME_BYTES, 256 MB
+ * by default, always at least one keyframe per world), and encodes all of them in four launches and one copy to the host.
+ * The staging and the encoder's device memory are allocated and freed inside the call.
+ * Without a generated kernel the replay runs in chunks that end at each keyframe, which is encoded from the live image:
+ * the same bytes, slower. */
+typedef struct bgr_keyframe {  /* 24 bytes */
+    int32_t frame;
+    uint32_t reserved;         /* 0 */
+    uint64_t offset;           /* of the blob in dst; a multiple of 8 */
+    uint64_t bytes;            /* the blob's exact size */
+} bgr_keyframe;
+struct bgr_keyframes {         /* 40 bytes */
+    uint32_t interval;         /* K >= 1 */
+    uint32_t index_cap;
+    uint64_t reserved;         /* 0 */
+    void* dst;                 /* NULL: query only */
+    size_t dst_cap;
+    bgr_keyframe* index;       /* [index_cap] */
+};
+BGR_API int bgr_replay_keyframes(bgr_engine* e, const struct bgr_replay* r, const struct bgr_keyframes* kf,
+                                 bgr_checksum* checksums_out, uint32_t cap, uint32_t* n_out, uint32_t* n_keyframes_out,
+                                 size_t* bytes_out);
+/* bgr_batch_replay with keyframes: kfs[i] holds world i's interval and buffers, in bgr_replay_keyframes' conventions
+ * (a null dst is refused with BGR_ERR_CAPACITY unless the world writes no keyframe; query a member's sizes with
+ * bgr_replay_keyframes on its engine).  Every listed world is validated, planned and its capacities checked first;
+ * n_keyframes_out[i] is world i's keyframe count. */
+BGR_API int bgr_batch_replay_keyframes(bgr_batch* b, const uint32_t* worlds, uint32_t n_worlds, const struct bgr_replay* replays,
+                                       const struct bgr_keyframes* kfs, bgr_checksum* checksums_out, uint32_t cap,
+                                       uint32_t* n_checksums_out, uint32_t* n_keyframes_out, int32_t* status_out);
+
 /* ---- shard group: the cross-shard step inside the engine (multi-GPU, one process per GPU, one node) -----------------
  * Entity-range shards never exchange state (SURVEY.md §8e: systems read no other entity, box_game.rs:162-169; the
  * checksum is an XOR over entities, component_checksum.rs:88-89).  The only exchange is 64 bytes of partials per

@@ -1,6 +1,7 @@
 //! `#[repr(C)]` mirror of `struct bgr_replay` of `include/bevy_ggrs_b200.h` and safe calls over it (bgr_replay /
 //! bgr_batch_replay): a recorded input log run through a world, checksummed every `checksum_interval` frames, without
-//! pushing snapshots.
+//! pushing snapshots.  With keyframes (bgr_replay_keyframes / bgr_batch_replay_keyframes) the replay also returns a
+//! world checkpoint every `keyframe_interval` frames, the seek points of a recorded match.
 
 use crate::*;
 use core::ptr;
@@ -16,6 +17,29 @@ pub struct bgr_replay {
     pub reserved: u32,
     pub inputs: *const u8,
 }
+
+#[repr(C)]
+#[derive(Clone, Copy, Debug, Default)]
+pub struct bgr_keyframe {
+    pub frame: i32,
+    pub reserved: u32,
+    pub offset: u64,
+    pub bytes: u64,
+}
+
+#[repr(C)]
+#[derive(Clone, Copy, Debug)]
+pub struct bgr_keyframes {
+    pub interval: u32,
+    pub index_cap: u32,
+    pub reserved: u64,
+    pub dst: *mut c_void,
+    pub dst_cap: usize,
+    pub index: *mut bgr_keyframe,
+}
+
+/// A replay's keyframes: `(frame, blob)` in frame order, each blob what `bgr_checkpoint_save` writes.
+pub type Keyframes = Vec<(i32, Vec<u8>)>;
 
 /// An input log: `inputs[j * n_players + h]` is player h's input of frame j.
 pub struct ReplayLog<'a> {
@@ -89,6 +113,93 @@ impl Batch {
             let cs = out[at.min(cap)..end].to_vec();
             at += n as usize;
             (s, cs)
+        }).collect())
+    }
+}
+
+/// Keyframe buffers sized by a query (dst NULL) of `log` on `e`, which runs nothing.
+struct KeyframeBuffers {
+    dst: Vec<u8>,
+    index: Vec<bgr_keyframe>,
+}
+
+impl KeyframeBuffers {
+    fn query(e: *mut bgr_engine, r: &bgr_replay, interval: u32) -> Result<Self, c_int> {
+        let q = bgr_keyframes { interval, index_cap: 0, reserved: 0, dst: ptr::null_mut(), dst_cap: 0, index: ptr::null_mut() };
+        let (mut n_cs, mut n_kf, mut bytes) = (0u32, 0u32, 0usize);
+        let rc = unsafe { bgr_replay_keyframes(e, r, &q, ptr::null_mut(), 0, &mut n_cs, &mut n_kf, &mut bytes) };
+        if rc != BGR_OK { return Err(rc); }
+        Ok(KeyframeBuffers { dst: vec![0u8; bytes.max(1)], index: vec![bgr_keyframe::default(); (n_kf as usize).max(1)] })
+    }
+
+    fn raw(&mut self, interval: u32) -> bgr_keyframes {
+        bgr_keyframes {
+            interval,
+            index_cap: self.index.len() as u32,
+            reserved: 0,
+            dst: self.dst.as_mut_ptr() as *mut c_void,
+            dst_cap: self.dst.len(),
+            index: self.index.as_mut_ptr(),
+        }
+    }
+
+    /// The first `n` blobs, clamped to what the buffers hold.
+    fn blobs(&self, n: u32) -> Keyframes {
+        self.index.iter().take((n as usize).min(self.index.len())).map(|k| {
+            let a = (k.offset as usize).min(self.dst.len());
+            let b = (a + k.bytes as usize).min(self.dst.len());
+            (k.frame, self.dst[a..b].to_vec())
+        }).collect()
+    }
+}
+
+/// `replay` that also returns a keyframe every `keyframe_interval` frames.  Err(status, checksums, keyframes):
+/// BGR_ERR_NON_FINITE after the whole log ran (the keyframes are written), or a refusal that changed nothing.
+pub fn replay_keyframes(e: *mut bgr_engine, log: &ReplayLog, keyframe_interval: u32)
+                        -> Result<(Vec<bgr_checksum>, Keyframes), (c_int, Vec<bgr_checksum>, Keyframes)> {
+    log.check().map_err(|rc| (rc, Vec::new(), Vec::new()))?;
+    let mut f0 = 0i32;
+    unsafe { bgr_rollback_frame_count(e, &mut f0) };
+    let r = log.raw();
+    let mut bufs = KeyframeBuffers::query(e, &r, keyframe_interval).map_err(|rc| (rc, Vec::new(), Vec::new()))?;
+    let kf = bufs.raw(keyframe_interval);
+    let mut out = vec![bgr_checksum::default(); log.points(f0)];
+    let (mut n, mut n_kf, mut bytes) = (0u32, 0u32, 0usize);
+    let rc = unsafe { bgr_replay_keyframes(e, &r, &kf, out.as_mut_ptr(), out.len() as u32, &mut n, &mut n_kf, &mut bytes) };
+    out.truncate((n as usize).min(out.len()));
+    let blobs = bufs.blobs(n_kf);
+    if rc == BGR_OK { Ok((out, blobs)) } else { Err((rc, out, blobs)) }
+}
+
+impl Batch {
+    /// `replay` of `logs[i]` on world `worlds[i]` with keyframes every `keyframe_intervals[i]` frames, in one
+    /// synchronous call.  `engines[i]` is world i's engine: its query sizes the world's buffers.  Err(status) when the
+    /// call was refused before anything executed; otherwise each world's status, checksums and keyframes, in order.
+    pub fn replay_keyframes(&mut self, worlds: &[u32], engines: &[*mut bgr_engine], f0s: &[i32], logs: &[ReplayLog],
+                            keyframe_intervals: &[u32]) -> Result<Vec<(c_int, Vec<bgr_checksum>, Keyframes)>, c_int> {
+        for l in logs { l.check()?; }
+        let reps: Vec<bgr_replay> = logs.iter().map(|l| l.raw()).collect();
+        let mut bufs = Vec::with_capacity(worlds.len());
+        for i in 0..worlds.len() { bufs.push(KeyframeBuffers::query(engines[i], &reps[i], keyframe_intervals[i])?); }
+        let kfs: Vec<bgr_keyframes> = bufs.iter_mut().zip(keyframe_intervals.iter()).map(|(b, &k)| b.raw(k)).collect();
+        let cap: usize = logs.iter().zip(f0s.iter()).map(|(l, &f0)| l.points(f0)).sum();
+        let mut out = vec![bgr_checksum::default(); cap];
+        let mut n_out = vec![0u32; worlds.len()];
+        let mut n_kf = vec![0u32; worlds.len()];
+        let mut status = vec![0i32; worlds.len()];
+        let rc = unsafe {
+            bgr_batch_replay_keyframes(self.raw, worlds.as_ptr(), worlds.len() as u32, reps.as_ptr(), kfs.as_ptr(),
+                                       out.as_mut_ptr(), cap as u32, n_out.as_mut_ptr(), n_kf.as_mut_ptr(), status.as_mut_ptr())
+        };
+        if rc != BGR_OK && rc != BGR_ERR_NON_FINITE {
+            return Err(rc);
+        }
+        let mut at = 0usize;
+        Ok((0..worlds.len()).map(|i| {
+            let end = (at + n_out[i] as usize).min(cap);
+            let cs = out[at.min(cap)..end].to_vec();
+            at += n_out[i] as usize;
+            (status[i], cs, bufs[i].blobs(n_kf[i]))
         }).collect())
     }
 }
