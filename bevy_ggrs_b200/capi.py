@@ -252,6 +252,9 @@ PROTOTYPES = {
                                        C.c_uint32, u32p, u32p, C.POINTER(C.c_size_t)]),
     "bgr_batch_replay_keyframes": (C.c_int, [C.c_void_p, u32p, C.c_uint32, C.POINTER(bgr_replay), C.POINTER(bgr_keyframes),
                                              C.POINTER(bgr_checksum), C.c_uint32, u32p, u32p, i32p]),
+    "bgr_batch_checkpoint_save": (C.c_int, [C.c_void_p, u32p, C.c_uint32, i32p, C.c_void_p, C.c_size_t, C.POINTER(bgr_keyframe),
+                                            C.POINTER(C.c_size_t), i32p]),
+    "bgr_batch_checkpoint_restore": (C.c_int, [C.c_void_p, u32p, C.c_uint32, C.POINTER(C.c_void_p), C.POINTER(C.c_size_t), i32p]),
     "bgr_seahash": (C.c_uint64, [C.c_void_p, C.c_uint64]),
     "bgr_ggrs_time_delta_bits": (C.c_uint32, [C.c_uint32, C.c_int32]),
     "bgr_particle_rng_stream": (C.c_int, [C.c_uint64, C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p, C.c_float, C.c_float]),

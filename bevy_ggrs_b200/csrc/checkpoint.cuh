@@ -14,11 +14,14 @@
 //            image's payload (ImageEntry::out_off): CONST by
 //            one thread, the SPARSE bitmap from warp ballots with each non-zero element ranked by a popc prefix plus the
 //            warp totals in shared memory, RAW coalesced.
-// Restore is one launch (k_ckpt_unpack) per uploaded blob: warp 0 validates the kind bytes, the padding and the length
-// the kinds and bitmaps imply against the block's offsets, reading a bitmap only after checking it lies inside the
-// block; then the mask plane is expanded and an existing row whose mask byte has a bit outside the alive bit and the
-// registered absent bits makes the block bad.  A bad block sets the error word and writes nothing.  Otherwise every
-// thread expands its row of every vector into a scratch image, canonical as above.
+// Restore decodes every uploaded blob in one launch (k_ckpt_unpack) over an image table whose entries are the blobs'
+// scratch images (bgr_checkpoint_restore: one blob; bgr_batch_checkpoint_restore: one per listed world), one 512-thread
+// block per tile of every blob: warp 0 validates the kind bytes, the padding and the length the kinds and bitmaps imply
+// against the block's offsets, reading a bitmap only after checking it lies inside the block; then the mask plane is
+// expanded and an existing row whose mask byte has a bit outside the alive bit and the registered absent bits makes the
+// block bad.  A bad block sets its blob's error word and writes nothing.  Otherwise every thread expands its row of
+// every vector into the scratch image, canonical as above.  Once k_frame_digest has verified every scratch image,
+// k_ckpt_commit copies each to its engine's image 0 and restored ring slot, in one launch over the same table.
 #pragma once
 #include "frame_digest.cuh"
 
@@ -44,18 +47,17 @@ __host__ __device__ inline uint32_t ckpt_max_block_words(uint32_t words) {
 }
 
 struct CkptParams {
-    const ImageEntry* images;            // save: the image table
+    const ImageEntry* images;            // the image table (restore: the scratch images written)
     uint32_t n_images;
-    const uint8_t* img;                  // restore: the scratch image written
-    uint32_t words, rows;                // rows: restore
+    uint32_t words;
     const uint32_t* plane_absent;        // [words] the absent bit of the column each plane belongs to (0: not optional)
     const uint32_t* plane_pad;           // restore: [words] the bits of a plane's word past its column's element bytes
     uint32_t mask_bits;                  // restore: the bits a mask byte may hold (alive and the registered absent bits)
     uint8_t* kinds;                      // save: [tiles][words + 1]
     unsigned int* lens;                  // save: [blocks] bytes of each block
-    const unsigned long long* offsets;   // [blocks + 1]
+    const unsigned long long* offsets;   // [blocks + 1] (restore: bytes into the concatenated payloads of every blob)
     uint32_t* payload;
-    unsigned int* err;                   // restore: lowest bad block (0xFFFFFFFF: none)
+    unsigned int* err;                   // restore: [n_images] each blob's lowest bad block (0xFFFFFFFF: none)
 };
 
 // thread threadIdx.x's canonical word of plane `plane` (m: its canonical mask byte)
@@ -184,6 +186,9 @@ __global__ void __launch_bounds__(kTileRows) k_ckpt_unpack(const __grid_constant
     __shared__ uint32_t s_mask[kCkptMaskWords];
     __shared__ uint32_t s_bad;
     const uint32_t tile = blockIdx.x, lane = threadIdx.x & 31u;
+    const ImageEntry& im = image_of(p.images, p.n_images, tile);
+    const uint32_t t = tile - im.first_block;
+    unsigned int* err = p.err + (&im - p.images);
     const unsigned long long o0 = p.offsets[tile];
     // the host checked: offsets ascend in multiples of 4 inside the upload, and a block is at most ckpt_max_block_words
     const uint32_t len = uint32_t((p.offsets[tile + 1] - o0) / 4u);
@@ -211,7 +216,7 @@ __global__ void __launch_bounds__(kTileRows) k_ckpt_unpack(const __grid_constant
     }
     __syncthreads();
     if (s_bad) {
-        if (threadIdx.x == 0) atomicMin(p.err, tile);
+        if (threadIdx.x == 0) atomicMin(err, t);
         return;
     }
     // this thread's element of vector v (zero past the vector's n)
@@ -226,14 +231,14 @@ __global__ void __launch_bounds__(kTileRows) k_ckpt_unpack(const __grid_constant
         for (uint32_t k = 0; k < j; ++k) rank += __popc(blk[start + k]);
         return blk[start + n / 32u + rank];
     };
-    uint8_t* tb = const_cast<uint8_t*>(p.img) + size_t(tile) * tile_bytes_of(p.words);
+    uint8_t* tb = const_cast<uint8_t*>(im.img) + size_t(t) * tile_bytes_of(p.words);
     const uint32_t mw = element(p.words);
     if (threadIdx.x < kCkptMaskWords) s_mask[threadIdx.x] = mw;
     __syncthreads();
     const uint32_t mb = reinterpret_cast<const uint8_t*>(s_mask)[threadIdx.x];
-    const uint32_t m = (tile * kTileRows + threadIdx.x < p.rows && (mb & 1u)) ? mb : 0u;
+    const uint32_t m = (t * kTileRows + threadIdx.x < im.rows && (mb & 1u)) ? mb : 0u;
     if (__syncthreads_or(m & ~p.mask_bits)) {  // a presence bit of a column this registration does not have
-        if (threadIdx.x == 0) atomicMin(p.err, tile);
+        if (threadIdx.x == 0) atomicMin(err, t);
         return;
     }
     tb[size_t(p.words) * kPlaneBytes + threadIdx.x] = uint8_t(m);
@@ -243,7 +248,23 @@ __global__ void __launch_bounds__(kTileRows) k_ckpt_unpack(const __grid_constant
         stray |= x & p.plane_pad[v];
         *reinterpret_cast<uint32_t*>(tb + size_t(v) * kPlaneBytes + threadIdx.x * 4u) = x;
     }
-    if (__syncthreads_or(stray != 0u) && threadIdx.x == 0) atomicMin(p.err, tile);
+    if (__syncthreads_or(stray != 0u) && threadIdx.x == 0) atomicMin(err, t);
+}
+
+// Block b copies tile b of the table's (verified) scratch images to both destinations of its image, dst[2i] and
+// dst[2i + 1]: the engine's image 0 and its restored ring slot.  16-byte units (tile_bytes is a multiple of 16).
+__global__ void __launch_bounds__(kTileRows) k_ckpt_commit(const ImageEntry* __restrict__ images, uint32_t n_images,
+                                                           uint8_t* const* __restrict__ dst, uint32_t tile_bytes) {
+    const ImageEntry& im = image_of(images, n_images, blockIdx.x);
+    const size_t i = size_t(&im - images), off = size_t(blockIdx.x - im.first_block) * tile_bytes;
+    const uint4* src = reinterpret_cast<const uint4*>(im.img + off);
+    uint4* d0 = reinterpret_cast<uint4*>(dst[2u * i] + off);
+    uint4* d1 = reinterpret_cast<uint4*>(dst[2u * i + 1u] + off);
+    for (uint32_t k = threadIdx.x; k < tile_bytes / 16u; k += blockDim.x) {
+        const uint4 v = __ldcs(src + k);
+        d0[k] = v;
+        d1[k] = v;
+    }
 }
 
 }  // namespace bgr

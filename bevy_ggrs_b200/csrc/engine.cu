@@ -34,6 +34,7 @@
 #include "change_feed.cuh"
 #include "frame_digest.cuh"
 #include "checkpoint.cuh"
+#include "checkpoint_check.hpp"
 #include "replay_keyframes.hpp"
 #include "jit.hpp"
 #include "vmm_range.hpp"
@@ -3063,11 +3064,6 @@ static std::vector<uint32_t> plane_pad(const bgr_engine* e) {
     return a;
 }
 
-// bytes ahead of the payload: the header and the offsets
-static size_t checkpoint_prefix(uint32_t n_blocks) {
-    return sizeof(bgr_checkpoint_header) + sizeof(uint64_t) * (size_t(n_blocks) + 1u);
-}
-
 // ---- the image-table encoder: the checkpoints of many images of one registration in four launches ----
 // k_frame_digest, k_ckpt_measure and k_ckpt_scan run once over every block of every image (one scan: an image's offsets
 // are differences from its first block's), then, with the blob sizes known on the host, k_ckpt_pack writes every payload
@@ -3087,6 +3083,7 @@ struct EncodeImage {
 
 static size_t blob_bytes(const EncodeImage& x) { return checkpoint_prefix(x.h.n_blocks) + x.h.payload_bytes; }
 static size_t align8(size_t v) { return (v + 7u) & ~size_t(7); }
+static size_t align16(size_t v) { return (v + 15u) & ~size_t(15); }
 
 // The header of a checkpoint of e's frame `frame` with `rows` rows (active, digest_root and payload_bytes: encode_measure)
 static bgr_checkpoint_header checkpoint_header(const bgr_engine* e, int32_t frame, uint32_t rows, uint64_t elapsed_ns,
@@ -3257,128 +3254,199 @@ BGR_API int bgr_checkpoint_save(bgr_engine* e, int32_t frame, void* dst, size_t 
     return encode_pack(x);
 }
 
-BGR_API int bgr_checkpoint_restore(bgr_engine* e, const void* blob, size_t bytes) {
+// ---- restore: the blobs checked on the host, decoded and verified in one pass, then committed in one launch ----
+// bgr_checkpoint_restore is the one-blob case of bgr_batch_checkpoint_restore: restore_check, restore_decode and
+// restore_commit serve both.
+
+// One blob to restore into engine e, checked on the host by restore_check
+struct RestoreBlob {
+    bgr_engine* e = nullptr;
+    const uint8_t* payload = nullptr;  // h.payload_bytes bytes inside the caller's blob
+    bgr_checkpoint_header h{};
+    std::vector<uint64_t> offsets;     // [n_blocks + 1]
+    uint32_t slot = 0;                 // restore_commit: the ring slot that holds the restored frame
+};
+
+// The device memory of one restore (every blob's scratch image, the payloads, the tables), freed with it
+struct RestorePass {
+    std::vector<ImageEntry> table;  // one entry per blob, img = its scratch image
+    uint32_t blocks = 0;
+    DeviceBuffer<uint8_t> scratch, meta, payload;
+    size_t dst_off = 0;             // k_ckpt_commit's destinations ([blobs][2] pointers) in `meta`, written by the commit
+};
+
+static CkptTarget ckpt_target(const bgr_engine* e) {
+    return CkptTarget{digest_layout(e), e->words, uint32_t(e->cols.size()), e->cfg.fps, e->ceiling, e->growable()};
+}
+
+// The engine's state checks and the blob's host checks (checkpoint_check.hpp); nothing runs
+static int restore_check(bgr_engine* e, const void* blob, size_t bytes, RestoreBlob* r) {
     int rc = checkpoint_args(e);
     if (rc != BGR_OK) return rc;
     if (!blob) return fail(BGR_ERR_INVALID_ARGUMENT, "null argument");
     if (!e->pending.empty()) return fail(BGR_ERR_STATE, "collect every submitted request vector first");
     if (e->st.ring.depth() == 0 || e->n_slots() == 0)
         return fail(BGR_ERR_STATE, "the snapshot ring has depth 0: it cannot hold the restored frame");
-    // the blob is input from disk or another machine: check every field before using it
-    const uint8_t* in = static_cast<const uint8_t*>(blob);
-    bgr_checkpoint_header h;
-    if (bytes < sizeof h) return fail(BGR_ERR_INVALID_ARGUMENT, "checkpoint truncated: shorter than its header");
-    std::memcpy(&h, in, sizeof h);
-    if (h.magic != BGR_CHECKPOINT_MAGIC) return fail(BGR_ERR_INVALID_ARGUMENT, "not a world checkpoint (bad magic)");
-    if (h.version != BGR_CHECKPOINT_VERSION)
-        return fail(BGR_ERR_INVALID_ARGUMENT, "unsupported checkpoint format version " + std::to_string(h.version));
-    if (h.layout != digest_layout(e) || h.words != e->words || h.n_columns != e->cols.size())
-        return fail(BGR_ERR_INVALID_ARGUMENT, "the checkpoint comes from an engine with a different registration (layout differs)");
-    if (h.fps != e->cfg.fps)
-        return fail(BGR_ERR_INVALID_ARGUMENT, "the checkpoint was taken at " + std::to_string(h.fps) + " fps, this engine runs at " +
-                                                  std::to_string(e->cfg.fps));
-    if (h.n_blocks != e->tiles_for(h.rows))
-        return fail(BGR_ERR_INVALID_ARGUMENT, "checkpoint header: n_blocks does not match rows");
-    if (h.rows > e->ceiling)
-        return fail(BGR_ERR_CAPACITY, "the checkpoint holds " + std::to_string(h.rows) + " rows, more than this engine's " +
-                                          (e->growable() ? "ceiling of " : "capacity of ") + std::to_string(e->ceiling));
-    const uint32_t n_blocks = h.n_blocks;
-    const size_t prefix = checkpoint_prefix(n_blocks);
-    if (bytes < prefix) return fail(BGR_ERR_INVALID_ARGUMENT, "checkpoint truncated: shorter than its block offsets");
-    if (bytes - prefix != h.payload_bytes)
-        return fail(BGR_ERR_INVALID_ARGUMENT, "checkpoint length " + std::to_string(bytes) + " does not match its payload (truncated or overlong)");
-    std::vector<uint64_t> offsets(size_t(n_blocks) + 1u);
-    std::memcpy(offsets.data(), in + sizeof h, sizeof(uint64_t) * offsets.size());
-    // a block is at least its kind bytes and one u32 per vector (every vector CONST) and at most every vector RAW.  The
-    // lower bound also bounds the scratch image the decoding allocates by the blob's size: a tile of the image is at
-    // most tile_bytes / min_block times the smallest block (390x for the stress schema), and only a world that is
-    // constant in every tile gets there.
-    const uint64_t max_block = uint64_t(ckpt_max_block_words(e->words)) * 4u;
-    const uint64_t min_block = uint64_t(ckpt_kind_words(e->words) + e->words + 1u) * 4u;
-    if (offsets[0] != 0 || offsets[n_blocks] != h.payload_bytes)
-        return fail(BGR_ERR_INVALID_ARGUMENT, "checkpoint offsets do not span the payload");
-    for (uint32_t b = 0; b < n_blocks; ++b)
-        if (offsets[b + 1] < offsets[b] + min_block || offsets[b + 1] % 4u || offsets[b + 1] - offsets[b] > max_block)
-            return fail(BGR_ERR_INVALID_ARGUMENT, "checkpoint offset " + std::to_string(b + 1) + " is not ascending, aligned or within a block's size");
-    // decode into a scratch image and verify it with the frame digest before anything is committed
-    DeviceBuffer<uint8_t> scratch;
-    DeviceBuffer<uint32_t> d_payload, d_absent, d_pad;
-    DeviceBuffer<unsigned long long> d_offsets;
-    DeviceBuffer<unsigned int> d_err;
-    const size_t tb = e->tile_bytes, image_bytes = size_t(n_blocks) * tb;
-    if (n_blocks) {
+    std::string err;
+    rc = checkpoint_check(ckpt_target(e), blob, bytes, &r->h, &r->offsets, &err);
+    if (rc != BGR_OK) return fail(rc, err);
+    r->e = e;
+    r->payload = static_cast<const uint8_t*>(blob) + checkpoint_prefix(r->h.n_blocks);
+    return BGR_OK;
+}
+
+// Decodes every blob of `r` (host-checked, into engines of one registration on one stream) into its own scratch image
+// and verifies each with the frame digest, with a fixed number of launches and copies whatever the number of blobs: one
+// upload of the payloads (gathered in `stage`, page-locked, when there are several; one blob is uploaded from the
+// caller's memory), one of the tables and offsets, k_ckpt_unpack and k_frame_digest over every block of every blob, one
+// synchronisation.  Nothing is committed.  A refusal sets *bad to the lowest index of `r` that failed.
+static int restore_decode(std::vector<RestoreBlob>& r, RestorePass& x, MappedHostBuffer<uint8_t>* stage, size_t* bad) {
+    bgr_engine* e = r[0].e;
+    const size_t n = r.size();
+    const uint32_t per = uint32_t(e->cols.size()) + 1u;
+    size_t payload_bytes = 0;
+    x.table.resize(n);
+    x.blocks = 0;
+    for (size_t i = 0; i < n; ++i) {  // scratch images and payloads follow each other in list order
+        x.table[i] = ImageEntry{nullptr, r[i].e->cfg.order_base, payload_bytes, r[i].h.rows, x.blocks};
+        x.blocks += r[i].h.n_blocks;
+        payload_bytes += r[i].h.payload_bytes;
+    }
+    std::vector<uint64_t> digest;
+    std::vector<unsigned int> active, err(n, 0xFFFFFFFFu);
+    if (x.blocks) {
         const size_t smem = sizeof(uint32_t) * (e->words + 1u);
         if (smem + sizeof(uint32_t) * (kCkptMaskWords + 1u) > 48u * 1024u)
             return fail(BGR_ERR_UNSUPPORTED, "bgr_checkpoint_restore supports at most 12000 word planes");
         const std::vector<uint32_t> absent = plane_absent(e), pad = plane_pad(e);
-        CUDA_TRY(scratch.ensure(image_bytes));
-        CUDA_TRY(d_payload.ensure(h.payload_bytes / 4u));
-        CUDA_TRY(d_absent.ensure(absent.size()));
-        CUDA_TRY(d_pad.ensure(pad.size()));
-        CUDA_TRY(d_offsets.ensure(offsets.size()));
-        CUDA_TRY(d_err.ensure(1));
-        CUDA_TRY(cudaMemcpyAsync(d_payload.get(), in + prefix, h.payload_bytes, cudaMemcpyHostToDevice, e->stream));
-        CUDA_TRY(cudaMemcpyAsync(d_absent.get(), absent.data(), sizeof(uint32_t) * absent.size(), cudaMemcpyHostToDevice, e->stream));
-        CUDA_TRY(cudaMemcpyAsync(d_pad.get(), pad.data(), sizeof(uint32_t) * pad.size(), cudaMemcpyHostToDevice, e->stream));
-        CUDA_TRY(cudaMemcpyAsync(d_offsets.get(), offsets.data(), sizeof(uint64_t) * offsets.size(), cudaMemcpyHostToDevice, e->stream));
-        CUDA_TRY(cudaMemsetAsync(d_err.get(), 0xFF, sizeof(unsigned int), e->stream));
+        // the tables in one upload: image table, the offsets rebased onto the concatenated payloads, error words, planes
+        const size_t o_off = align16(sizeof(ImageEntry) * n), o_err = align16(o_off + sizeof(uint64_t) * (x.blocks + 1u));
+        const size_t o_absent = align16(o_err + sizeof(unsigned int) * n), o_pad = align16(o_absent + sizeof(uint32_t) * absent.size());
+        x.dst_off = align16(o_pad + sizeof(uint32_t) * pad.size());
+        const size_t meta_bytes = x.dst_off + sizeof(uint8_t*) * 2u * n;  // every allocation happens before the commit
+        CUDA_TRY(x.scratch.ensure(size_t(x.blocks) * e->tile_bytes));
+        CUDA_TRY(x.meta.ensure(meta_bytes));
+        CUDA_TRY(x.payload.ensure(std::max<size_t>(4, payload_bytes)));
+        for (size_t i = 0; i < n; ++i) x.table[i].img = x.scratch.get() + size_t(x.table[i].first_block) * e->tile_bytes;
+        std::vector<uint8_t> meta(meta_bytes);
+        std::memcpy(meta.data(), x.table.data(), sizeof(ImageEntry) * n);
+        uint64_t* off = reinterpret_cast<uint64_t*>(meta.data() + o_off);
+        for (size_t i = 0; i < n; ++i)
+            for (uint32_t k = 0; k < r[i].h.n_blocks; ++k) off[x.table[i].first_block + k] = x.table[i].out_off + r[i].offsets[k];
+        off[x.blocks] = payload_bytes;
+        std::memcpy(meta.data() + o_err, err.data(), sizeof(unsigned int) * n);
+        std::memcpy(meta.data() + o_absent, absent.data(), sizeof(uint32_t) * absent.size());
+        std::memcpy(meta.data() + o_pad, pad.data(), sizeof(uint32_t) * pad.size());
+        const uint8_t* src = r[0].payload;
+        if (n > 1) {
+            CUDA_TRY(stage->ensure(payload_bytes));
+            for (size_t i = 0; i < n; ++i) std::memcpy(stage->get() + x.table[i].out_off, r[i].payload, r[i].h.payload_bytes);
+            src = stage->get();
+        }
+        CUDA_TRY(cudaMemcpyAsync(x.payload.get(), src, payload_bytes, cudaMemcpyHostToDevice, e->stream));
+        CUDA_TRY(cudaMemcpyAsync(x.meta.get(), meta.data(), meta_bytes, cudaMemcpyHostToDevice, e->stream));
+        uint8_t* d = x.meta.get();
         CkptParams p{};
-        p.img = scratch.get();
+        p.images = reinterpret_cast<const ImageEntry*>(d);
+        p.n_images = uint32_t(n);
         p.words = e->words;
-        p.rows = h.rows;
-        p.plane_absent = d_absent.get();
-        p.plane_pad = d_pad.get();
+        p.plane_absent = reinterpret_cast<const uint32_t*>(d + o_absent);
+        p.plane_pad = reinterpret_cast<const uint32_t*>(d + o_pad);
         p.mask_bits = 1u;
         for (const Column& c : e->cols) p.mask_bits |= c.absent;
-        p.offsets = d_offsets.get();
-        p.payload = d_payload.get();
-        p.err = d_err.get();
-        k_ckpt_unpack<<<n_blocks, kTileRows, smem, e->stream>>>(p);
+        p.offsets = reinterpret_cast<const unsigned long long*>(d + o_off);
+        p.payload = reinterpret_cast<uint32_t*>(x.payload.get());
+        p.err = reinterpret_cast<unsigned int*>(d + o_err);
+        k_ckpt_unpack<<<x.blocks, kTileRows, smem, e->stream>>>(p);
         e->launches += 1;
         CUDA_TRY(cudaGetLastError());
-        unsigned int bad = 0;
-        CUDA_TRY(cudaMemcpyAsync(&bad, d_err.get(), sizeof bad, cudaMemcpyDeviceToHost, e->stream));
-        CUDA_TRY(cudaStreamSynchronize(e->stream));  // `absent` and `offsets` go out of scope or are reused below
-        if (bad != 0xFFFFFFFFu)
-            return fail(BGR_ERR_INVALID_ARGUMENT, "checkpoint block " + std::to_string(bad) +
+        int rc = digest_launch(e, p.images, uint32_t(n), x.blocks, &digest, &active);
+        if (rc != BGR_OK) return rc;
+        CUDA_TRY(cudaMemcpyAsync(err.data(), p.err, sizeof(unsigned int) * n, cudaMemcpyDeviceToHost, e->stream));
+        CUDA_TRY(cudaStreamSynchronize(e->stream));  // `meta` goes out of scope, the staging is reused by the next call
+    }
+    for (size_t i = 0; i < n; ++i) {
+        *bad = i;
+        if (err[i] != 0xFFFFFFFFu)
+            return fail(BGR_ERR_INVALID_ARGUMENT, "checkpoint block " + std::to_string(err[i]) +
                                                       ": a bad kind byte or padding, its kinds and bitmaps imply another length than its "
                                                       "offsets, a row's mask byte has a bit this registration does not use, or a word has "
                                                       "bits past its column's element bytes");
+        const size_t nb = r[i].h.n_blocks, b0 = x.table[i].first_block;
+        uint64_t rows_alive = 0;
+        for (size_t k = 0; k < nb; ++k) rows_alive += active[b0 + k];
+        const uint64_t root = bgr_seahash(nb ? &digest[b0 * per] : nullptr, nb * per * sizeof(uint64_t));
+        if (root != r[i].h.digest_root || rows_alive != r[i].h.active)
+            return fail(BGR_ERR_INVALID_ARGUMENT, "the decoded world's digest or active row count differs from the checkpoint header (corrupt payload)");
     }
-    std::vector<uint64_t> digest_words;
-    uint64_t root = 0, active = 0;
-    rc = digest_image(e, scratch.get(), h.rows, &digest_words, &root, &active);
-    if (rc != BGR_OK) return rc;
-    if (root != h.digest_root || active != h.active)
-        return fail(BGR_ERR_INVALID_ARGUMENT, "the decoded world's digest or active row count differs from the checkpoint header (corrupt payload)");
-    if (e->growable()) rc = grow_to(e, h.rows);
-    if (rc != BGR_OK) return rc;
-    // commit: image 0 and one slot hold the world, which the ring queues alone
-    e->deferred = DeferredLive{};  // image 0 is overwritten: nothing to materialise
-    HostState& s = e->st;
-    const uint32_t slot = s.ring.restart(h.frame);
-    if (n_blocks) {
-        CUDA_TRY(cudaMemcpyAsync(e->image(0), scratch.get(), image_bytes, cudaMemcpyDeviceToDevice, e->stream));
-        CUDA_TRY(cudaMemcpyAsync(e->image(slot + 1), scratch.get(), image_bytes, cudaMemcpyDeviceToDevice, e->stream));
-    }
-    rc = clear_stamps(e, 0);
-    if (rc == BGR_OK) rc = clear_stamps(e, slot + 1);
-    if (rc != BGR_OK) return rc;
-    e->tiledep_chain = false;
-    ParticleRng rng;
-    std::memcpy(&rng, h.rng, sizeof rng);
-    s.frame_count = h.frame;
-    s.elapsed_ns = h.elapsed_ns;
-    s.n_rows = h.rows;
-    s.rng = rng;
-    s.slot_rows[slot] = h.rows;
-    s.slot_elapsed_ns[slot] = h.elapsed_ns;
-    s.slot_rng[slot] = rng;
-    s.cids.live = s.cids.slot[slot] = s.cids.fresh(h.rows);
-    s.live_passive_ver = ++s.ver_counter;  // image 0 holds new content; the restored slot holds the same
-    s.slot_passive_ver[slot] = s.live_passive_ver;
-    CUDA_TRY(cudaStreamSynchronize(e->stream));  // before the scratch image is freed
     return BGR_OK;
+}
+
+// Commits every verified blob of `r` (after restore_decode): growable engines grow to the blob's rows (a failure sets
+// *bad to that blob's index, before any world changed), each ring restarts at the blob's frame, one k_ckpt_commit launch
+// copies every scratch image to its engine's image 0 and restored slot, then each engine's host state becomes the
+// blob's.  Allocates nothing once a world has changed.  Synchronous: the scratch images are freed after it.
+static int restore_commit(std::vector<RestoreBlob>& r, RestorePass& x, size_t* bad) {
+    bgr_engine* e0 = r[0].e;
+    for (size_t i = 0; i < r.size(); ++i)
+        if (r[i].e->growable()) {
+            *bad = i;
+            int rc = grow_to(r[i].e, r[i].h.rows);
+            if (rc != BGR_OK) return rc;
+        }
+    *bad = r.size();
+    // image 0 and one slot hold the world, which the ring queues alone
+    std::vector<uint8_t*> dst(2u * r.size());
+    for (size_t i = 0; i < r.size(); ++i) {
+        bgr_engine* e = r[i].e;
+        e->deferred = DeferredLive{};  // image 0 is overwritten: nothing to materialise
+        r[i].slot = e->st.ring.restart(r[i].h.frame);
+        dst[2u * i] = e->image(0);
+        dst[2u * i + 1u] = e->image(r[i].slot + 1);
+    }
+    if (x.blocks) {
+        uint8_t** d_dst = reinterpret_cast<uint8_t**>(x.meta.get() + x.dst_off);
+        CUDA_TRY(cudaMemcpyAsync(d_dst, dst.data(), sizeof(uint8_t*) * dst.size(), cudaMemcpyHostToDevice, e0->stream));
+        k_ckpt_commit<<<x.blocks, kTileRows, 0, e0->stream>>>(reinterpret_cast<const ImageEntry*>(x.meta.get()), uint32_t(r.size()),
+                                                              d_dst, uint32_t(e0->tile_bytes));
+        e0->launches += 1;
+        CUDA_TRY(cudaGetLastError());
+    }
+    for (RestoreBlob& b : r) {
+        bgr_engine* e = b.e;
+        const bgr_checkpoint_header& h = b.h;
+        const uint32_t slot = b.slot;
+        int rc = clear_stamps(e, 0);
+        if (rc == BGR_OK) rc = clear_stamps(e, slot + 1);
+        if (rc != BGR_OK) return rc;
+        e->tiledep_chain = false;
+        HostState& s = e->st;
+        ParticleRng rng;
+        std::memcpy(&rng, h.rng, sizeof rng);
+        s.frame_count = h.frame;
+        s.elapsed_ns = h.elapsed_ns;
+        s.n_rows = h.rows;
+        s.rng = rng;
+        s.slot_rows[slot] = h.rows;
+        s.slot_elapsed_ns[slot] = h.elapsed_ns;
+        s.slot_rng[slot] = rng;
+        s.cids.live = s.cids.slot[slot] = s.cids.fresh(h.rows);
+        s.live_passive_ver = ++s.ver_counter;  // image 0 holds new content; the restored slot holds the same
+        s.slot_passive_ver[slot] = s.live_passive_ver;
+    }
+    CUDA_TRY(cudaStreamSynchronize(e0->stream));  // before the scratch images and `dst` are freed
+    return BGR_OK;
+}
+
+BGR_API int bgr_checkpoint_restore(bgr_engine* e, const void* blob, size_t bytes) {
+    std::vector<RestoreBlob> r(1);
+    int rc = restore_check(e, blob, bytes, &r[0]);
+    if (rc != BGR_OK) return rc;
+    RestorePass x;
+    size_t bad = 0;
+    rc = restore_decode(r, x, nullptr, &bad);
+    if (rc != BGR_OK) return rc;
+    return restore_commit(r, x, &bad);
 }
 
 BGR_API int bgr_submit_requests(bgr_engine* e, const bgr_session_info* session, const bgr_request* requests,
@@ -3413,6 +3481,7 @@ struct bgr_batch {
     uint32_t calls = 0;
     MappedHostBuffer<uint8_t> h_stage;   // a call's JitWorld records, then the listed worlds' ops
     DeviceBuffer<uint8_t> d_stage;
+    MappedHostBuffer<uint8_t> h_ckpt;    // bgr_batch_checkpoint_restore: the payloads, gathered for one upload
 };
 
 static bool same_specs(const bgr_engine* a, const bgr_engine* b) {
@@ -3865,8 +3934,6 @@ const JitKernel* replay_kernel(bgr_engine* e, uint32_t tiles) {
     return k.replay_fn ? &k : nullptr;
 }
 
-size_t align16(size_t v) { return (v + 15u) & ~size_t(15); }
-
 // The replays of `jobs` (every one with frames to run) on the replay entry point of `k`: the logs, spawn tables and spawn
 // values go to the device once, then each launch runs every unfinished world through its next frames, as many as keep
 // the launch's checksum points within kReplayLaunchPoints (one launch for everything but very long logs at short
@@ -4198,6 +4265,124 @@ BGR_API int bgr_batch_replay_keyframes(bgr_batch* b, const uint32_t* worlds, uin
                                        uint32_t* n_checksums_out, uint32_t* n_keyframes_out, int32_t* status_out) {
     if (n_worlds && (!kfs || !n_keyframes_out)) return fail(BGR_ERR_INVALID_ARGUMENT, "null argument");
     return batch_replay(b, worlds, n_worlds, replays, kfs, checksums_out, cap, n_checksums_out, n_keyframes_out, status_out);
+}
+
+// ---- batched checkpoints: the checkpoints of many worlds saved or restored in one pass ----
+namespace {
+
+// The index checks every batch call makes (in range, listed once), with the "world <index>: " prefix on a refusal
+struct BatchWorlds {
+    bgr_batch* b;
+    const uint32_t* worlds;
+    int32_t* status_out;
+    int fail_at(uint32_t i, int status) {
+        status_out[i] = status;
+        g_err = "world " + std::to_string(worlds[i]) + ": " + g_err;
+        return status;
+    }
+    int check(uint32_t i) {
+        const uint32_t w = worlds[i];
+        if (w >= b->engines.size())
+            return fail_at(i, fail(BGR_ERR_INVALID_ARGUMENT, "no such world in a batch of " + std::to_string(b->engines.size())));
+        if (b->listed[w] == b->calls) return fail_at(i, fail(BGR_ERR_INVALID_ARGUMENT, "listed twice in one call"));
+        b->listed[w] = b->calls;
+        return BGR_OK;
+    }
+};
+
+}  // namespace
+
+BGR_API int bgr_batch_checkpoint_save(bgr_batch* b, const uint32_t* worlds, uint32_t n_worlds, const int32_t* frames,
+                                      void* dst, size_t dst_cap, bgr_keyframe* index, size_t* bytes_out, int32_t* status_out) {
+    if (!b) return fail(BGR_ERR_INVALID_ARGUMENT, "null batch");
+    if (!bytes_out || (n_worlds && (!worlds || !frames || !index || !status_out))) return fail(BGR_ERR_INVALID_ARGUMENT, "null argument");
+    NvtxRange span("CheckpointSave");
+    b->calls += 1;
+    *bytes_out = 0;
+    for (uint32_t i = 0; i < n_worlds; ++i) status_out[i] = BGR_OK;
+    BatchWorlds bw{b, worlds, status_out};
+    for (uint32_t i = 0; i < n_worlds; ++i) {
+        int rc = bw.check(i);
+        if (rc != BGR_OK) return rc;
+    }
+    for (uint32_t i = 0; i < n_worlds; ++i) {  // every member's submitted vectors, their results left queued
+        const int rc = drain(b->engines[worlds[i]]);
+        if (rc != BGR_OK) return bw.fail_at(i, rc);
+    }
+    // one image-table encoder over the held frames of every listed world; its launches count on worlds[0]'s engine
+    ImageEncoder x;
+    x.e = n_worlds ? b->engines[worlds[0]] : nullptr;
+    std::vector<uint32_t> of;  // the list index of each encoded image
+    std::vector<bgr_keyframe> idx(n_worlds);  // copied to `index` when the call succeeds
+    size_t pos = 0;
+    for (uint32_t i = 0; i < n_worlds; ++i) {
+        bgr_engine* e = b->engines[worlds[i]];
+        bgr_keyframe& k = idx[i];
+        k = bgr_keyframe{frames[i], 0u, pos, 0u};
+        uint32_t slot = 0;
+        if (!p2p_slot(e, frames[i], &slot)) continue;  // held neither queued nor retained: bytes 0
+        const uint32_t rows = e->st.slot_rows[slot], n_blocks = e->tiles_for(rows);
+        if (!dst) {
+            k.bytes = checkpoint_prefix(n_blocks) + size_t(n_blocks) * ckpt_max_block_words(e->words) * 4u;
+            pos = align8(pos + k.bytes);
+            continue;
+        }
+        EncodeImage m;
+        m.img = e->image(slot + 1);
+        m.order_base = e->cfg.order_base;
+        m.h = checkpoint_header(e, frames[i], rows, e->st.slot_elapsed_ns[slot], e->st.slot_rng[slot]);
+        x.im.push_back(std::move(m));
+        of.push_back(i);
+    }
+    *bytes_out = pos;
+    if (dst) {
+        int rc = x.e ? encode_measure(x) : BGR_OK;
+        if (rc != BGR_OK) return rc;
+        pos = 0;  // the exact layout: blobs in list order, each at a multiple of 8
+        for (uint32_t i = 0, j = 0; i < n_worlds; ++i) {
+            idx[i].offset = pos;
+            if (j < of.size() && of[j] == i) {
+                idx[i].bytes = blob_bytes(x.im[j]);
+                x.im[j++].dst = static_cast<uint8_t*>(dst) + pos;
+                pos = align8(pos + idx[i].bytes);
+            }
+        }
+        *bytes_out = pos;
+        if (dst_cap < pos)
+            return fail(BGR_ERR_CAPACITY, "the checkpoints need " + std::to_string(pos) + " bytes, dst_cap is " + std::to_string(dst_cap));
+        if (!x.im.empty()) rc = encode_pack(x);
+        if (rc != BGR_OK) return rc;
+        if (!x.im.empty()) {  // encode_pack zeroes the padding between blobs; the last one's is zeroed here
+            const EncodeImage& last = x.im.back();
+            std::memset(last.dst + blob_bytes(last), 0, align8(blob_bytes(last)) - blob_bytes(last));
+        }
+    }
+    std::copy(idx.begin(), idx.end(), index);
+    return BGR_OK;
+}
+
+BGR_API int bgr_batch_checkpoint_restore(bgr_batch* b, const uint32_t* worlds, uint32_t n_worlds, const void* const* blobs,
+                                         const size_t* bytes, int32_t* status_out) {
+    if (!b) return fail(BGR_ERR_INVALID_ARGUMENT, "null batch");
+    if (n_worlds && (!worlds || !blobs || !bytes || !status_out)) return fail(BGR_ERR_INVALID_ARGUMENT, "null argument");
+    NvtxRange span("CheckpointRestore");
+    b->calls += 1;
+    for (uint32_t i = 0; i < n_worlds; ++i) status_out[i] = BGR_OK;
+    BatchWorlds bw{b, worlds, status_out};
+    std::vector<RestoreBlob> r(n_worlds);
+    for (uint32_t i = 0; i < n_worlds; ++i) {  // the host checks, in list order
+        int rc = bw.check(i);
+        if (rc != BGR_OK) return rc;
+        rc = restore_check(b->engines[worlds[i]], blobs[i], bytes[i], &r[i]);
+        if (rc != BGR_OK) return bw.fail_at(i, rc);
+    }
+    if (n_worlds == 0) return BGR_OK;
+    RestorePass x;
+    size_t bad = n_worlds;
+    int rc = restore_decode(r, x, &b->h_ckpt, &bad);
+    if (rc == BGR_OK) rc = restore_commit(r, x, &bad);
+    if (rc != BGR_OK) return bad < n_worlds ? bw.fail_at(uint32_t(bad), rc) : rc;
+    return BGR_OK;
 }
 
 BGR_API int bgr_save_world(bgr_engine* e, bgr_checksum* checksum_out) {

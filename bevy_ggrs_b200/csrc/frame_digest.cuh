@@ -18,12 +18,13 @@ static_assert(BGR_DIGEST_BLOCK_ROWS == kTileRows, "a digest block is one tile");
 // one registered column: its word planes, its element size (the bytes hashed) and its absent bit (0: not optional)
 struct DigestColumn { uint32_t first_plane, elem_bytes, absent; };
 
-// An image table: the images one launch of k_frame_digest, k_ckpt_measure or k_ckpt_pack covers, of one registration.
-// Their blocks are numbered in table order: image i holds blocks [first_block, first_block + ceil(rows / 512)).
+// An image table: the images one launch of k_frame_digest, k_ckpt_measure, k_ckpt_pack, k_ckpt_unpack or k_ckpt_commit
+// covers, of one registration.  Their blocks are numbered in table order: image i holds blocks
+// [first_block, first_block + ceil(rows / 512)).
 struct ImageEntry {
     const uint8_t* img;
     unsigned long long order_base;  // bgr_config.order_base of the image's engine
-    unsigned long long out_off;     // k_ckpt_pack: byte offset of the image's payload in the output
+    unsigned long long out_off;     // byte offset of the image's payload in k_ckpt_pack's output or k_ckpt_unpack's upload
     uint32_t rows, first_block;
 };
 static_assert(sizeof(ImageEntry) == 32, "ImageEntry layout");

@@ -684,6 +684,38 @@ class EngineBatch:
             k += n_cs[i]
         return res
 
+    def checkpoint(self, calls) -> List[Optional[bytes]]:
+        """``calls`` = [(world, frame), ...]: Engine.checkpoint of every listed world in one call (one encoding pass and
+        one copy back).  Returns the blobs in the same order, None where the world holds that frame neither queued
+        nor retained.  The buffer is sized by the call's query (dst NULL), which runs nothing; a refused call raises
+        BgrError naming the world."""
+        calls = list(calls)
+        n = len(calls)
+        worlds = (C.c_uint32 * max(1, n))(*[w for w, _ in calls])
+        frames = (C.c_int32 * max(1, n))(*[f for _, f in calls])
+        index = (capi.bgr_keyframe * max(1, n))()
+        size = C.c_size_t()
+        status = (C.c_int32 * max(1, n))()
+        self._check(self._lib.bgr_batch_checkpoint_save(self._h, worlds, n, frames, None, 0, index, C.byref(size), status))
+        buf = np.empty(max(1, size.value), np.uint8)   # upper bounds: the call reports the exact layout
+        self._check(self._lib.bgr_batch_checkpoint_save(self._h, worlds, n, frames, buf.ctypes.data, size.value, index,
+                                                        C.byref(size), status))
+        return [buf[index[i].offset: index[i].offset + index[i].bytes].tobytes() if index[i].bytes else None
+                for i in range(n)]
+
+    def restore(self, calls) -> None:
+        """``calls`` = [(world, blob), ...]: Engine.restore of every listed world in one call (one decoding pass).  All
+        or nothing: a refused call raises BgrError (its status, and text starting with "world <index>: ") and changes
+        no world."""
+        calls = list(calls)
+        n = len(calls)
+        worlds = (C.c_uint32 * max(1, n))(*[w for w, _ in calls])
+        keep = [C.c_char_p(b if isinstance(b, bytes) else bytes(b)) for _, b in calls]   # no copy of a bytes blob
+        blobs = (C.c_void_p * max(1, n))(*[C.cast(k, C.c_void_p).value for k in keep])
+        sizes = (C.c_size_t * max(1, n))(*[len(b) for _, b in calls])
+        status = (C.c_int32 * max(1, n))()
+        self._check(self._lib.bgr_batch_checkpoint_restore(self._h, worlds, n, blobs, sizes, status))
+
 
 def _keyframe_buffers(kf: "capi.bgr_keyframes", n_kf: int, size: int):
     """A dst of `size` bytes and an index of `n_kf` entries, installed in `kf`; the arrays must outlive the call."""

@@ -713,6 +713,46 @@ BGR_API int bgr_batch_replay_keyframes(bgr_batch* b, const uint32_t* worlds, uin
                                        const struct bgr_keyframes* kfs, bgr_checksum* checksums_out, uint32_t cap,
                                        uint32_t* n_checksums_out, uint32_t* n_keyframes_out, int32_t* status_out);
 
+/* ---- batched checkpoints: the world checkpoints of many batch members saved or restored in one pass ----------------
+ * Both calls follow the conventions of bgr_batch_handle_requests: indices in range and distinct, every listed world
+ * validated before anything executes anywhere, a refusal marks the failing world in status_out with bgr_last_error()
+ * starting with "world <index>: " and the single-world call's message, and worlds not listed are untouched.  Neither
+ * depends on bgr_batch_specialised: the checkpoint kernels are part of the library, so a batch that ticks its worlds one
+ * after another (BGR_TUNE_JIT=0, no NVRTC) saves and restores in one pass too.  The kernels of one call are counted on
+ * worlds[0]'s bgr_launch_count, and their number does not depend on n_worlds: a save is four launches (k_frame_digest,
+ * k_ckpt_measure, k_ckpt_scan, k_ckpt_pack) and a restore three (k_ckpt_unpack, k_frame_digest, k_ckpt_commit); fewer
+ * when no listed world has a row.  Device memory for the encoding or decoding is allocated and freed inside the call.
+ *
+ * bgr_batch_checkpoint_save: blob i is byte for byte what bgr_checkpoint_save(worlds[i], frames[i]) writes (the frame
+ * queued or retained).  The blobs go to dst in list order, each at a multiple of 8 bytes (the padding is zero);
+ * index[i] = {frames[i], 0, offset in dst, bytes}, and bytes == 0 means the world holds that frame neither queued nor
+ * retained (the single call's *found = 0), which is not an error.  dst == NULL: nothing runs; index[i].bytes = world i's
+ * upper bound (every vector RAW), index[i].offset its place under those bounds, and *bytes_out = the total, a multiple
+ * of 8.  Otherwise *bytes_out = the exact total, the end of the last blob rounded up to 8; a dst_cap below it is
+ * BGR_ERR_CAPACITY, and then nothing is written to dst or index.  Waits for each member's submitted vectors and leaves
+ * their results queued.  The payloads of every world come back to dst with one copy (page-locked dst from
+ * bgr_host_alloc copies at the full PCIe rate). */
+BGR_API int bgr_batch_checkpoint_save(bgr_batch* b, const uint32_t* worlds, uint32_t n_worlds, const int32_t* frames,
+                                      void* dst, size_t dst_cap, bgr_keyframe* index, size_t* bytes_out,
+                                      int32_t* status_out);
+/* bgr_batch_checkpoint_restore: each listed world ends exactly as bgr_checkpoint_restore(worlds[i], blobs[i], bytes[i])
+ * would leave it (see there: image 0, one queued ring slot, frame, Time<GgrsTime>, ParticleRng, row count, witnesses and
+ * retained frames released, a deferred live image dropped, change feeds left alone, a growable member grown to the
+ * blob's rows).  All or nothing: if any blob fails any of bgr_checkpoint_restore's checks, no world changes.  The host
+ * checks (header, offsets, capacity, un-collected submits: BGR_ERR_STATE) run first, in list order, and the first
+ * failure is reported; the device checks (kinds, padding, implied lengths, mask bits, stray bits, digest root and active
+ * count) run only if every blob passed the host checks, and the lowest listed index that failed is reported.  One blob
+ * may be listed for several worlds, and a blob may come from another member when its layout (order_base included) and
+ * fps match the target's.  One pass, whatever n_worlds: the payloads are gathered into page-locked staging that the
+ * batch keeps (sized by its largest restore) and uploaded with one copy, the tables and offsets with another, then
+ * k_ckpt_unpack and k_frame_digest run over every block of every blob, three copies bring back the error words, the
+ * digest words and the active counts, and one k_ckpt_commit launch copies every world to its image 0 and restored slot.
+ * Every allocation happens before any world changes: out of device memory is BGR_ERR_CUDA with no world changed.  A
+ * growable member whose growth fails is named (BGR_ERR_CUDA or BGR_ERR_CAPACITY) and nothing is restored; members that
+ * grew before it keep their larger capacity, as in bgr_batch_handle_requests. */
+BGR_API int bgr_batch_checkpoint_restore(bgr_batch* b, const uint32_t* worlds, uint32_t n_worlds,
+                                         const void* const* blobs, const size_t* bytes, int32_t* status_out);
+
 /* ---- shard group: the cross-shard step inside the engine (multi-GPU, one process per GPU, one node) -----------------
  * Entity-range shards never exchange state (SURVEY.md §8e: systems read no other entity, box_game.rs:162-169; the
  * checksum is an XOR over entities, component_checksum.rs:88-89).  The only exchange is 64 bytes of partials per

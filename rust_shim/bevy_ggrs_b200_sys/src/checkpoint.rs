@@ -1,5 +1,9 @@
 //! `#[repr(C)]` mirror of the world checkpoint header of `include/bevy_ggrs_b200.h` (bgr_checkpoint_save /
-//! bgr_checkpoint_restore).
+//! bgr_checkpoint_restore), and the batched calls over a world batch (bgr_batch_checkpoint_save /
+//! bgr_batch_checkpoint_restore).
+
+use crate::*;
+use core::ptr;
 
 pub const BGR_CHECKPOINT_MAGIC: u32 = 0x43524742;
 pub const BGR_CHECKPOINT_VERSION: u32 = 1;
@@ -24,4 +28,52 @@ pub struct bgr_checkpoint_header {
     pub rng: [u64; 4],
     pub digest_root: u64,
     pub payload_bytes: u64,
+}
+
+impl Batch {
+    /// The checkpoints of `frames[i]` on world `worlds[i]` in one call (one encoding pass, one copy back), sized by the
+    /// call's query.  `None` where the world holds that frame neither queued nor retained.  Err(status) when refused.
+    pub fn checkpoint(&mut self, worlds: &[u32], frames: &[i32]) -> Result<Vec<Option<Vec<u8>>>, c_int> {
+        if worlds.len() != frames.len() {
+            return Err(BGR_ERR_INVALID_ARGUMENT);
+        }
+        let n = worlds.len() as u32;
+        let mut index = vec![bgr_keyframe::default(); worlds.len()];
+        let mut status = vec![0i32; worlds.len()];
+        let mut size = 0usize;
+        let rc = unsafe {
+            bgr_batch_checkpoint_save(self.raw, worlds.as_ptr(), n, frames.as_ptr(), ptr::null_mut(), 0, index.as_mut_ptr(),
+                                      &mut size, status.as_mut_ptr())
+        };
+        if rc != BGR_OK {
+            return Err(rc);
+        }
+        let mut dst = vec![0u8; size];
+        let rc = unsafe {
+            bgr_batch_checkpoint_save(self.raw, worlds.as_ptr(), n, frames.as_ptr(), dst.as_mut_ptr() as *mut c_void, dst.len(),
+                                      index.as_mut_ptr(), &mut size, status.as_mut_ptr())
+        };
+        if rc != BGR_OK {
+            return Err(rc);
+        }
+        Ok(index.iter().map(|k| if k.bytes == 0 { None } else {
+            Some(dst[k.offset as usize..(k.offset + k.bytes) as usize].to_vec())
+        }).collect())
+    }
+
+    /// Restores `blobs[i]` into world `worlds[i]` in one call (one decoding pass).  All or nothing: Err(status) (and
+    /// bgr_last_error() naming the world) leaves every world as it was.
+    pub fn restore(&mut self, worlds: &[u32], blobs: &[&[u8]]) -> Result<(), c_int> {
+        if worlds.len() != blobs.len() {
+            return Err(BGR_ERR_INVALID_ARGUMENT);
+        }
+        let ptrs: Vec<*const c_void> = blobs.iter().map(|b| b.as_ptr() as *const c_void).collect();
+        let sizes: Vec<usize> = blobs.iter().map(|b| b.len()).collect();
+        let mut status = vec![0i32; worlds.len()];
+        let rc = unsafe {
+            bgr_batch_checkpoint_restore(self.raw, worlds.as_ptr(), worlds.len() as u32, ptrs.as_ptr(), sizes.as_ptr(),
+                                         status.as_mut_ptr())
+        };
+        if rc == BGR_OK { Ok(()) } else { Err(rc) }
+    }
 }
