@@ -161,6 +161,10 @@ class bgr_feed_info(C.Structure):
     _fields_ = [("n_records", C.c_uint32), ("pending", C.c_uint32), ("rows", C.c_uint32), ("record_bytes", C.c_uint32)]
 
 
+class bgr_batch_feed(C.Structure):
+    _fields_ = [("world", C.c_uint32), ("feed", C.c_uint32), ("records_cap", C.c_uint32)]
+
+
 class bgr_edit(C.Structure):
     _fields_ = [("kind", C.c_uint32), ("column", C.c_uint32), ("row", C.c_uint32), ("count", C.c_uint32),
                 ("byte_offset", C.c_uint32), ("byte_len", C.c_uint32), ("value_offset", C.c_uint32), ("reserved", C.c_uint32)]
@@ -255,6 +259,8 @@ PROTOTYPES = {
     "bgr_batch_checkpoint_save": (C.c_int, [C.c_void_p, u32p, C.c_uint32, i32p, C.c_void_p, C.c_size_t, C.POINTER(bgr_keyframe),
                                             C.POINTER(C.c_size_t), i32p]),
     "bgr_batch_checkpoint_restore": (C.c_int, [C.c_void_p, u32p, C.c_uint32, C.POINTER(C.c_void_p), C.POINTER(C.c_size_t), i32p]),
+    "bgr_batch_feed_begin": (C.c_int, [C.c_void_p, C.POINTER(bgr_batch_feed), C.c_uint32, C.c_void_p, u32p, i32p]),
+    "bgr_batch_feed_wait": (C.c_int, [C.c_void_p, C.c_uint32, C.POINTER(bgr_feed_info)]),
     "bgr_seahash": (C.c_uint64, [C.c_void_p, C.c_uint64]),
     "bgr_ggrs_time_delta_bits": (C.c_uint32, [C.c_uint32, C.c_int32]),
     "bgr_particle_rng_stream": (C.c_int, [C.c_uint64, C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p, C.c_float, C.c_float]),

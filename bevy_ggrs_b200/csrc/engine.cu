@@ -35,6 +35,7 @@
 #include "frame_digest.cuh"
 #include "checkpoint.cuh"
 #include "checkpoint_check.hpp"
+#include "feed_check.hpp"
 #include "replay_keyframes.hpp"
 #include "jit.hpp"
 #include "vmm_range.hpp"
@@ -285,11 +286,11 @@ struct bgr_engine {
     // cross PCIe on copy_stream
     struct Feed {
         bool used = false, busy = false;
-        FeedParams p{};              // fields, rep, keep, rep_words, record_words and views of the buffers below
+        FeedParams p{};              // fields, keep, rep_words, record_words, p.one.rep and views of the buffers below
         uint32_t bound = 0;          // no row at or past it has a reported state other than (0, zeros)
-        uint32_t ticket = 0;         // of the report in flight
-        StridedRange rep, count;     // p.rep, and p.tile_count / tile_off / tile_list one stride each
-        DeviceBuffer<unsigned int> info;
+        uint32_t ticket = 0;         // of the report in flight (single or batched)
+        StridedRange rep, count;     // p.one.rep, and p.tile_count / tile_off / tile_list one stride each
+        DeviceBuffer<unsigned int> info;  // [8]: p.info [4], p.head [2], p.world_scan [2]
         DeviceBuffer<uint32_t> out;  // the records of a report
         MappedHostBuffer<unsigned int> h_info;  // [4]: the info, copied behind the records
         Event packed, done;
@@ -1725,9 +1726,12 @@ int feed_create(bgr_engine* e, const bgr_feed_field* fields, uint32_t n_fields, 
         return fail(BGR_ERR_CUDA, "bgr_feed_create: " + (ok ? std::string(cudaGetErrorString(ce)) : err));
     }
     const size_t count_stride = fd.count.stride / sizeof(unsigned int);  // words between tile_count, tile_off and tile_list
-    fd.p.rep = fd.rep.ptr();
+    fd.p.one.rep = fd.rep.ptr();
+    fd.p.n_worlds = 1;
     fd.p.tile_count = fd.count.ptr<unsigned int>();
     fd.p.info = fd.info.get();
+    fd.p.head = fd.p.info + 4;
+    fd.p.world_scan = fd.p.head + 2;
     fd.p.tile_off = fd.p.tile_count + count_stride;
     fd.p.tile_list = fd.p.tile_off + count_stride;
     fd.used = true;
@@ -1741,27 +1745,74 @@ int feed_reset(bgr_engine* e, uint32_t feed) {
     if (feed >= BGR_MAX_FEEDS || !e->feeds[feed].used) return fail(BGR_ERR_INVALID_ARGUMENT, "unknown feed");
     bgr_engine::Feed& fd = e->feeds[feed];
     // stream-ordered behind a report in flight, whose pass 2 is the last writer of the reported state
-    CUDA_TRY(cudaMemsetAsync(fd.p.rep, 0, size_t(e->tiles_for(fd.bound)) * tile_bytes_of(fd.p.rep_words), e->stream));
+    CUDA_TRY(cudaMemsetAsync(fd.rep.ptr(), 0, size_t(e->tiles_for(fd.bound)) * tile_bytes_of(fd.p.rep_words), e->stream));
     e->tiledep_chain = false;
     fd.bound = 0;
     return BGR_OK;
 }
 
+// The device address of page-locked memory from bgr_host_alloc (mapped into the device address space: unified
+// addressing), or nullptr
+uint32_t* mapped_host(void* host) {
+    cudaPointerAttributes a{};
+    if (cudaPointerGetAttributes(&a, host) != cudaSuccess || a.type != cudaMemoryTypeHost || !a.devicePointer) {
+        cudaGetLastError();
+        return nullptr;
+    }
+    return static_cast<uint32_t*>(a.devicePointer);
+}
+
+// The passes of the report `p` describes (table, scratch and staging set) on e's stream, counted on e; then on `copy`,
+// behind `packed`, the records into page-locked `host_dev` (nullptr: none) and the infos of every listed world into
+// `h_info`, with `done` behind them.  bgr_feed_begin and bgr_batch_feed_begin.
+int feed_report(bgr_engine* e, const FeedParams& p, uint32_t* host_dev, cudaStream_t copy, cudaEvent_t packed, cudaEvent_t done,
+                unsigned int* h_info) {
+    if (p.n_tiles) {
+        if (p.worlds) k_feed_count<true><<<p.n_tiles, kFeedBlock, 0, e->stream>>>(p);
+        else k_feed_count<false><<<p.n_tiles, kFeedBlock, 0, e->stream>>>(p);
+        e->launches += 1;
+        CUDA_TRY(cudaGetLastError());
+    }
+    if (p.worlds) k_feed_scan<<<1, kFeedScanBlock, 0, e->stream>>>(p);
+    else k_feed_scan_one<<<1, kFeedScanBlock, 0, e->stream>>>(p);
+    e->launches += 1;
+    CUDA_TRY(cudaGetLastError());
+    const uint32_t grid2 = std::max(1u, std::min(p.n_tiles, uint32_t(e->num_sms) * 4u));
+    if (p.worlds) k_feed_records<true><<<grid2, kFeedBlock, 0, e->stream>>>(p);
+    else k_feed_records<false><<<grid2, kFeedBlock, 0, e->stream>>>(p);
+    e->launches += 1;
+    CUDA_TRY(cudaGetLastError());
+    e->tiledep_chain = false;
+    CUDA_TRY(cudaEventRecord(packed, e->stream));
+    CUDA_TRY(cudaStreamWaitEvent(copy, packed, 0));
+    if (host_dev) {
+        k_feed_copy<<<std::max(1, e->num_sms), 256, 0, copy>>>(p.out, p.head, p.record_words, host_dev);
+        e->launches += 1;
+        CUDA_TRY(cudaGetLastError());
+    }
+    CUDA_TRY(cudaMemcpyAsync(h_info, p.info, sizeof(bgr_feed_info) * p.n_worlds, cudaMemcpyDeviceToHost, copy));
+    CUDA_TRY(cudaEventRecord(done, copy));
+    return BGR_OK;
+}
+
+// A report of `fd` has started: its rows up to `rows` may now hold a reported state, and it is busy under a fresh ticket
+void feed_started(bgr_engine* e, uint32_t feed, uint32_t rows) {
+    bgr_engine::Feed& fd = e->feeds[feed];
+    fd.bound = std::max(fd.bound, rows);
+    fd.busy = true;
+    e->feed_seq = (e->feed_seq + 1u) & 0x0FFFFFFFu;
+    fd.ticket = feed + BGR_MAX_FEEDS * e->feed_seq;
+}
+
+// bgr_feed_begin: the one-world case of the table-driven passes, its entry in the kernel parameters
 int feed_begin(bgr_engine* e, uint32_t feed, void* host, uint32_t cap, uint32_t* ticket_out) {
     if (!e || !ticket_out || (cap && !host)) return fail(BGR_ERR_INVALID_ARGUMENT, "null argument");
     if (!e->built) return fail(BGR_ERR_STATE, "engine not built");
     if (feed >= BGR_MAX_FEEDS || !e->feeds[feed].used) return fail(BGR_ERR_INVALID_ARGUMENT, "unknown feed");
     bgr_engine::Feed& fd = e->feeds[feed];
     if (fd.busy) return fail(BGR_ERR_STATE, "a report of this feed is in flight");
-    uint32_t* host_dev = nullptr;
-    if (cap) {  // page-locked memory is mapped into the device address space (unified addressing)
-        cudaPointerAttributes a{};
-        if (cudaPointerGetAttributes(&a, host) != cudaSuccess || a.type != cudaMemoryTypeHost || !a.devicePointer) {
-            cudaGetLastError();
-            return fail(BGR_ERR_INVALID_ARGUMENT, "host_dst must come from bgr_host_alloc");
-        }
-        host_dev = static_cast<uint32_t*>(a.devicePointer);
-    }
+    uint32_t* host_dev = cap ? mapped_host(host) : nullptr;
+    if (cap && !host_dev) return fail(BGR_ERR_INVALID_ARGUMENT, "host_dst must come from bgr_host_alloc");
     // no report has more records than the rows it compares
     const uint32_t cap_eff = std::min<uint64_t>(cap, uint64_t(e->n_tiles_cap) * kTileRows);
     CUDA_TRY(fd.out.ensure(size_t(cap_eff) * fd.p.record_words));  // no report of this feed is in flight
@@ -1769,35 +1820,13 @@ int feed_begin(bgr_engine* e, uint32_t feed, void* host, uint32_t cap, uint32_t*
     int rc = touch_live(e);  // stream-ordered behind the queued submits, like the passes below
     if (rc != BGR_OK) return rc;
     FeedParams p = fd.p;
-    p.img = e->image(0);
-    p.rows = e->st.n_rows;
-    p.n_tiles = e->tiles_for(std::max(p.rows, fd.bound));
-    p.cap = cap_eff;
-    if (p.n_tiles) {
-        k_feed_count<<<p.n_tiles, kFeedBlock, 0, e->stream>>>(p);
-        e->launches += 1;
-        CUDA_TRY(cudaGetLastError());
-    }
-    k_feed_scan<<<1, kFeedScanBlock, 0, e->stream>>>(p);
-    e->launches += 1;
-    CUDA_TRY(cudaGetLastError());
-    k_feed_records<<<std::max(1u, std::min(p.n_tiles, uint32_t(e->num_sms) * 4u)), kFeedBlock, 0, e->stream>>>(p);
-    e->launches += 1;
-    CUDA_TRY(cudaGetLastError());
-    e->tiledep_chain = false;
-    fd.bound = std::max(fd.bound, p.rows);
-    CUDA_TRY(cudaEventRecord(fd.packed.get(), e->stream));
-    CUDA_TRY(cudaStreamWaitEvent(e->copy_stream, fd.packed.get(), 0));
-    if (cap) {
-        k_feed_copy<<<std::max(1, e->num_sms), 256, 0, e->copy_stream>>>(p.out, p.info, host_dev);
-        e->launches += 1;
-        CUDA_TRY(cudaGetLastError());
-    }
-    CUDA_TRY(cudaMemcpyAsync(fd.h_info.get(), p.info, 4 * sizeof(unsigned int), cudaMemcpyDeviceToHost, e->copy_stream));
-    CUDA_TRY(cudaEventRecord(fd.done.get(), e->copy_stream));
-    fd.busy = true;
-    e->feed_seq = (e->feed_seq + 1u) & 0x0FFFFFFFu;
-    fd.ticket = feed + BGR_MAX_FEEDS * e->feed_seq;
+    p.one.img = e->image(0);
+    p.one.rows = e->st.n_rows;
+    p.one.n_tiles = p.n_tiles = e->tiles_for(std::max(p.one.rows, fd.bound));
+    p.one.cap = cap_eff;
+    rc = feed_report(e, p, host_dev, e->copy_stream, fd.packed.get(), fd.done.get(), fd.h_info.get());
+    if (rc != BGR_OK) return rc;
+    feed_started(e, feed, p.one.rows);
     *ticket_out = fd.ticket;
     return BGR_OK;
 }
@@ -3482,6 +3511,19 @@ struct bgr_batch {
     MappedHostBuffer<uint8_t> h_stage;   // a call's JitWorld records, then the listed worlds' ops
     DeviceBuffer<uint8_t> d_stage;
     MappedHostBuffer<uint8_t> h_ckpt;    // bgr_batch_checkpoint_restore: the payloads, gathered for one upload
+    // bgr_batch_feed_begin: the scratch of one report in flight, grown to the largest call and never shrunk
+    struct FeedScratch {
+        MappedHostBuffer<FeedWorld> h_table;  // the table, uploaded with one copy
+        DeviceBuffer<FeedWorld> table;
+        DeviceBuffer<unsigned int> counts;    // tile_count, tile_off, tile_list [tiles each], world_scan [2n], info [4n], head [2]
+        DeviceBuffer<uint32_t> out;           // the records, packed
+        MappedHostBuffer<unsigned int> h_info;  // [4n]
+        Event packed, done;
+        cudaStream_t copy = nullptr;          // the records and infos cross PCIe here
+        bool busy = false;
+        uint32_t ticket = 0, seq = 0;
+        std::vector<bgr_batch_feed> listed;   // the entries of the report in flight
+    } feed;
 };
 
 static bool same_specs(const bgr_engine* a, const bgr_engine* b) {
@@ -3549,6 +3591,12 @@ BGR_API int bgr_batch_create(bgr_engine* const* engines, uint32_t n, bgr_batch**
 BGR_API void bgr_batch_destroy(bgr_batch* b) {
     if (!b) return;
     cudaStreamSynchronize(b->stream);
+    if (b->feed.copy) {
+        cudaStreamSynchronize(b->feed.copy);
+        cudaStreamDestroy(b->feed.copy);
+    }
+    if (b->feed.busy)  // a batched report never waited: its feeds take reports again (no single ticket can free them)
+        for (const bgr_batch_feed& r : b->feed.listed) b->engines[r.world]->feeds[r.feed].busy = false;
     delete b;
 }
 
@@ -4382,6 +4430,91 @@ BGR_API int bgr_batch_checkpoint_restore(bgr_batch* b, const uint32_t* worlds, u
     int rc = restore_decode(r, x, &b->h_ckpt, &bad);
     if (rc == BGR_OK) rc = restore_commit(r, x, &bad);
     if (rc != BGR_OK) return bad < n_worlds ? bw.fail_at(uint32_t(bad), rc) : rc;
+    return BGR_OK;
+}
+
+// ---- batched change feed: the feeds of many batch members reported in one pass (change_feed.cuh, feed_check.hpp) ----
+BGR_API int bgr_batch_feed_begin(bgr_batch* b, const bgr_batch_feed* reports, uint32_t n, void* host_dst, uint32_t* ticket_out,
+                                 int32_t* status_out) {
+    if (!b) return fail(BGR_ERR_INVALID_ARGUMENT, "null batch");
+    if (!ticket_out || (n && (!reports || !status_out))) return fail(BGR_ERR_INVALID_ARGUMENT, "null argument");
+    NvtxRange span("FeedReport");
+    for (uint32_t i = 0; i < n; ++i) status_out[i] = BGR_OK;
+    bgr_batch::FeedScratch& x = b->feed;
+    if (x.busy) return fail(BGR_ERR_STATE, "a batched feed report of this batch is in flight: call bgr_batch_feed_wait first");
+    uint32_t bad = 0;
+    std::string why;
+    const int rc = feed_batch_check(uint32_t(b->engines.size()), reports, n, [b](uint32_t w, uint32_t f) {
+        const bgr_engine* e = b->engines[w];
+        return f < BGR_MAX_FEEDS && e->feeds[f].used ? FeedView{&e->feeds[f].p, e->feeds[f].busy} : FeedView{nullptr, false};
+    }, &bad, &why);
+    if (rc != BGR_OK) {
+        status_out[bad] = rc;
+        return fail(rc, "world " + std::to_string(reports[bad].world) + ": " + why);
+    }
+    bool any_cap = false;
+    for (uint32_t i = 0; i < n; ++i) any_cap = any_cap || reports[i].records_cap;
+    uint32_t* host_dev = any_cap ? (host_dst ? mapped_host(host_dst) : nullptr) : nullptr;
+    if (any_cap && !host_dev) return fail(BGR_ERR_INVALID_ARGUMENT, "host_dst must come from bgr_host_alloc");
+    // every allocation before any feed changes: the table, the scratch, the staging, the infos
+    CUDA_TRY(x.h_table.ensure(std::max(1u, n)));
+    FeedWorld* tab = x.h_table.get();
+    for (uint32_t i = 0; i < n; ++i) {
+        bgr_engine* e = b->engines[reports[i].world];
+        const bgr_engine::Feed& fd = e->feeds[reports[i].feed];
+        tab[i] = FeedWorld{e->image(0), fd.rep.ptr(), e->st.n_rows, e->tiles_for(std::max(e->st.n_rows, fd.bound)), 0u, 0u};
+    }
+    uint64_t stage_records = 0;
+    const uint32_t tiles = feed_layout(tab, reports, n, &stage_records);
+    const FeedParams reg = n ? b->engines[reports[0].world]->feeds[reports[0].feed].p : FeedParams{};
+    CUDA_TRY(x.table.ensure(std::max(1u, n)));
+    CUDA_TRY(x.counts.ensure(3ull * tiles + 6ull * n + 2u));
+    CUDA_TRY(x.out.ensure(std::max<uint64_t>(1u, stage_records * reg.record_words)));
+    CUDA_TRY(x.h_info.ensure(4ull * std::max(1u, n)));
+    CUDA_TRY(x.packed.ensure());
+    CUDA_TRY(x.done.ensure());
+    if (!x.copy) CUDA_TRY(cudaStreamCreateWithFlags(&x.copy, cudaStreamNonBlocking));
+    for (uint32_t i = 0; i < n; ++i) {  // stream-ordered behind every queued submit, like the passes below
+        const int r = touch_live(b->engines[reports[i].world]);
+        if (r != BGR_OK) {
+            status_out[i] = r;
+            return fail(r, "world " + std::to_string(reports[i].world) + ": " + g_err);
+        }
+    }
+    if (n) {
+        CUDA_TRY(cudaMemcpyAsync(x.table.get(), tab, sizeof(FeedWorld) * n, cudaMemcpyHostToDevice, b->stream));
+        FeedParams p = reg;
+        p.worlds = x.table.get();
+        p.n_worlds = n;
+        p.n_tiles = tiles;
+        p.tile_count = x.counts.get();
+        p.tile_off = p.tile_count + tiles;
+        p.tile_list = p.tile_off + tiles;
+        p.world_scan = p.tile_list + tiles;
+        p.info = p.world_scan + 2u * n;
+        p.head = p.info + 4u * n;
+        p.out = x.out.get();
+        const int r = feed_report(b->engines[reports[0].world], p, host_dev, x.copy, x.packed.get(), x.done.get(), x.h_info.get());
+        if (r != BGR_OK) return r;
+        for (bgr_engine* e : b->engines) e->tiledep_chain = false;  // the passes ran on the shared stream
+        for (uint32_t i = 0; i < n; ++i) feed_started(b->engines[reports[i].world], reports[i].feed, tab[i].rows);
+    }
+    x.listed.assign(reports, reports + n);
+    x.busy = true;
+    x.seq = (x.seq + 1u) & 0x7FFFFFFFu;
+    x.ticket = x.seq + 1u;
+    *ticket_out = x.ticket;
+    return BGR_OK;
+}
+
+BGR_API int bgr_batch_feed_wait(bgr_batch* b, uint32_t ticket, bgr_feed_info* infos) {
+    if (!b) return fail(BGR_ERR_INVALID_ARGUMENT, "null batch");
+    bgr_batch::FeedScratch& x = b->feed;
+    if (!x.busy || ticket != x.ticket) return fail(BGR_ERR_STATE, "no such batched feed report in flight");
+    if (!x.listed.empty()) CUDA_TRY(cudaEventSynchronize(x.done.get()));
+    x.busy = false;
+    for (const bgr_batch_feed& r : x.listed) b->engines[r.world]->feeds[r.feed].busy = false;
+    if (infos) std::memcpy(infos, x.h_info.get(), sizeof(bgr_feed_info) * x.listed.size());
     return BGR_OK;
 }
 

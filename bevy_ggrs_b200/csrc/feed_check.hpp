@@ -1,0 +1,72 @@
+// Batched change feed (bgr_batch_feed_begin): the host checks of a call's entries, made before anything runs, and the
+// table layout of a report (each world's first global tile and cap, the staging size).  Host only;
+// tests/cpp/test_feed_check.cpp holds it to every refusal and to hand-computed offsets.
+#pragma once
+#include <algorithm>
+#include <cstring>
+#include <string>
+#include <vector>
+
+#include "../../include/bevy_ggrs_b200.h"
+#include "change_feed.cuh"  // FeedParams, FeedWorld
+
+namespace bgr {
+
+// A feed as the checks see it: its registration (the fields, mask bits and record size in `reg`) and whether a report
+// of it is in flight
+struct FeedView {
+    const FeedParams* reg;  // nullptr: no such feed
+    bool busy;
+};
+
+// the same field list (so the same record layout) as another feed of the same registration
+inline bool feed_same_fields(const FeedParams& a, const FeedParams& b) {
+    if (a.n_fields != b.n_fields || a.keep != b.keep || a.record_words != b.record_words) return false;
+    return std::memcmp(a.fields, b.fields, sizeof(FeedField) * a.n_fields) == 0;
+}
+
+// Checks the entries of one call in list order: world in range and listed once, the feed known and idle, its fields
+// those of entry 0's feed.  `view(world, feed)` gives the feed.  BGR_OK, or the status with *bad = the failing entry and
+// *err = why (the single call's message where it has one).
+template <class View>
+int feed_batch_check(uint32_t n_members, const bgr_batch_feed* reports, uint32_t n, View view, uint32_t* bad, std::string* err) {
+    std::vector<bool> seen(n_members, false);
+    const FeedParams* first = nullptr;
+    for (uint32_t i = 0; i < n; ++i) {
+        *bad = i;
+        const bgr_batch_feed& r = reports[i];
+        if (r.world >= n_members) {
+            *err = "no such world in a batch of " + std::to_string(n_members);
+            return BGR_ERR_INVALID_ARGUMENT;
+        }
+        if (seen[r.world]) { *err = "listed twice in one call"; return BGR_ERR_INVALID_ARGUMENT; }
+        seen[r.world] = true;
+        const FeedView f = view(r.world, r.feed);
+        if (!f.reg) { *err = "unknown feed"; return BGR_ERR_INVALID_ARGUMENT; }
+        if (f.busy) { *err = "a report of this feed is in flight"; return BGR_ERR_STATE; }
+        if (!first) first = f.reg;
+        else if (!feed_same_fields(*f.reg, *first)) {
+            *err = "its feed's fields differ from those of entry 0's feed (a call has one record size)";
+            return BGR_ERR_INVALID_ARGUMENT;
+        }
+    }
+    return BGR_OK;
+}
+
+// Fills tile0 and cap of every entry of `tab` (img, rep, rows and n_tiles set) in list order: consecutive global tiles,
+// and a cap of at most every row compared.  Returns the global tile count; *stage_records = the records the staging
+// must hold, the sum of the caps.
+inline uint32_t feed_layout(FeedWorld* tab, const bgr_batch_feed* reports, uint32_t n, uint64_t* stage_records) {
+    uint32_t tiles = 0;
+    uint64_t recs = 0;
+    for (uint32_t i = 0; i < n; ++i) {
+        tab[i].tile0 = tiles;
+        tab[i].cap = uint32_t(std::min<uint64_t>(reports[i].records_cap, uint64_t(tab[i].n_tiles) * kTileRows));
+        tiles += tab[i].n_tiles;
+        recs += tab[i].cap;
+    }
+    *stage_records = recs;
+    return tiles;
+}
+
+}  // namespace bgr

@@ -569,6 +569,8 @@ class EngineBatch:
         self._lib = capi.load_library()
         self._h = None
         self.engines = list(engines)
+        self._pinned: List[C.c_void_p] = []
+        self._feed_tickets: Dict[int, tuple] = {}
         arr = (C.c_void_p * max(1, len(self.engines)))(*[e._h for e in self.engines])
         h = C.c_void_p()
         self._check(self._lib.bgr_batch_create(arr, len(self.engines), C.byref(h)))
@@ -580,8 +582,11 @@ class EngineBatch:
 
     def close(self) -> None:
         if self._h is not None:
-            self._lib.bgr_batch_destroy(self._h)
+            self._lib.bgr_batch_destroy(self._h)   # waits for a report in flight
             self._h = None
+            for p in self._pinned:
+                self._lib.bgr_host_free(p)
+            self._pinned = []
 
     def __del__(self):
         try:
@@ -715,6 +720,62 @@ class EngineBatch:
         sizes = (C.c_size_t * max(1, n))(*[len(b) for _, b in calls])
         status = (C.c_int32 * max(1, n))()
         self._check(self._lib.bgr_batch_checkpoint_restore(self._h, worlds, n, blobs, sizes, status))
+
+    # ---- batched change feed (bgr_batch_feed_*): many members' feeds in one pass ----
+    def _feed_bytes(self, calls) -> Optional[int]:
+        """sum(cap) records of the first call's feed (a call has one record size), or None when the first call names no
+        feed this wrapper knows (the library refuses the call)."""
+        if not calls:
+            return 0
+        w, f, _ = calls[0]
+        dt = self.engines[w]._feed_dtypes.get(f) if 0 <= w < len(self.engines) else None
+        return None if dt is None else sum(cap for _, _, cap in calls) * dt.itemsize
+
+    def feed_alloc(self, calls) -> np.ndarray:
+        """Page-locked buffer for a batched report of ``calls`` = [(world, feed, cap), ...]: sum(cap) records of the
+        first call's feed; freed with the batch."""
+        size = self._feed_bytes(list(calls)) or 0
+        p = C.c_void_p()
+        self._check(self._lib.bgr_host_alloc(max(1, size), C.byref(p)))
+        self._pinned.append(p)
+        return np.frombuffer((C.c_uint8 * max(1, size)).from_address(p.value), dtype=np.uint8)
+
+    def feed_begin(self, calls, buf: Optional[np.ndarray]) -> int:
+        """Starts one report of every ``calls`` entry (world, feed, cap) into ``buf`` (from feed_alloc); returns its
+        ticket.  A refused call raises BgrError (text starting with "world <index>: " for a refused entry) and changes
+        no feed."""
+        calls = [tuple(int(x) for x in c) for c in calls]
+        n = len(calls)
+        need = self._feed_bytes(calls)
+        if need:   # the library cannot check the buffer's size: the records of every entry must fit
+            assert buf is not None and buf.dtype == np.uint8 and buf.flags.c_contiguous and buf.size >= need, \
+                f"feed_begin needs a buffer of {need} bytes (feed_alloc of these calls)"
+        reps = (capi.bgr_batch_feed * max(1, n))(*[capi.bgr_batch_feed(*c) for c in calls])
+        t = C.c_uint32()
+        status = (C.c_int32 * max(1, n))()
+        dst = buf.ctypes.data if buf is not None else None
+        self._check(self._lib.bgr_batch_feed_begin(self._h, reps, n, dst, C.byref(t), status))
+        self._feed_tickets[t.value] = (calls, buf)
+        return t.value
+
+    def feed_wait(self, ticket: int) -> List[Tuple[np.ndarray, FeedInfo]]:
+        """[(records, info), ...] of a batched report, in the order of its calls: structured arrays (row, state, f0,
+        ...) copied out of the buffer, entry i's from behind the earlier entries' records."""
+        calls, buf = self._feed_tickets.get(ticket, ([], None))
+        infos = (capi.bgr_feed_info * max(1, len(calls)))()
+        self._check(self._lib.bgr_batch_feed_wait(self._h, ticket, infos))
+        del self._feed_tickets[ticket]
+        out, at = [], 0
+        for i, (w, f, _) in enumerate(calls):
+            dt = self.engines[w].feed_record_dtype(f)
+            info = infos[i]
+            assert info.record_bytes == dt.itemsize
+            recs = np.empty(info.n_records, dt)
+            if info.n_records:   # buf may be None when every cap is 0
+                C.memmove(recs.ctypes.data, buf.ctypes.data + at, info.n_records * dt.itemsize)
+            at += info.n_records * dt.itemsize
+            out.append((recs, FeedInfo(info.n_records, info.pending, info.rows, info.record_bytes)))
+        return out
 
 
 def _keyframe_buffers(kf: "capi.bgr_keyframes", n_kf: int, size: int):

@@ -753,6 +753,32 @@ BGR_API int bgr_batch_checkpoint_save(bgr_batch* b, const uint32_t* worlds, uint
 BGR_API int bgr_batch_checkpoint_restore(bgr_batch* b, const uint32_t* worlds, uint32_t n_worlds,
                                          const void* const* blobs, const size_t* bytes, int32_t* status_out);
 
+/* ---- batched change feed: the change feeds of many batch members reported in one pass ------------------------------
+ * Entry i reports feed reports[i].feed of member reports[i].world with at most records_cap records.  Its records and
+ * infos[i] are byte for byte what bgr_feed_begin / bgr_feed_wait on that engine would give at that point, and the report
+ * advances the same reported state: batched and single reports of one feed alternate freely, and bgr_feed_reset still
+ * applies.  The records are packed in list order into host_dst: entry i's start at the sum of the earlier entries'
+ * n_records.  host_dst must come from bgr_host_alloc and hold sum(records_cap) records (NULL when every cap is 0); it
+ * must not be read before bgr_batch_feed_wait(ticket) returns.
+ * In the conventions of the other batch calls, every entry is validated before anything runs: indices in range and
+ * distinct, a known feed (BGR_ERR_INVALID_ARGUMENT), no report of that feed in flight, single or batched (BGR_ERR_STATE),
+ * and the same field list as entry 0's feed (BGR_ERR_INVALID_ARGUMENT: a call has one record size).  A refusal marks the
+ * entry in status_out, bgr_last_error() starts with "world <index>: ", and nothing changes: no feed becomes busy and no
+ * reported state moves.  A host_dst not from bgr_host_alloc is BGR_ERR_INVALID_ARGUMENT for the whole call, and a
+ * second bgr_batch_feed_begin before the wait is BGR_ERR_STATE: one batched report per batch is in flight.
+ * The call is ordered behind every vector submitted on the shared stream, un-collected submits of a member included,
+ * materialises a deferred live image only on the listed worlds that have one, and returns without waiting for the GPU.
+ * It does not depend on bgr_batch_specialised.  Whatever n_entries, it is one table upload, four launches counted on
+ * reports[0].world's bgr_launch_count (k_feed_count, k_feed_scan, k_feed_records, and k_feed_copy on a copy stream of
+ * the batch; no k_feed_count when no listed world has a tile, no k_feed_copy when every cap is 0) and one copy of the
+ * infos; the scratch the batch keeps grows to the largest call and is allocated before any feed changes.
+ * bgr_batch_feed_wait waits for the report and writes infos[0 .. n_entries); an unknown or already-waited ticket is
+ * BGR_ERR_STATE. */
+typedef struct bgr_batch_feed { uint32_t world, feed, records_cap; } bgr_batch_feed;
+BGR_API int bgr_batch_feed_begin(bgr_batch* b, const bgr_batch_feed* reports, uint32_t n_entries, void* host_dst,
+                                 uint32_t* ticket_out, int32_t* status_out);
+BGR_API int bgr_batch_feed_wait(bgr_batch* b, uint32_t ticket, bgr_feed_info* infos);
+
 /* ---- shard group: the cross-shard step inside the engine (multi-GPU, one process per GPU, one node) -----------------
  * Entity-range shards never exchange state (SURVEY.md §8e: systems read no other entity, box_game.rs:162-169; the
  * checksum is an XOR over entities, component_checksum.rs:88-89).  The only exchange is 64 bytes of partials per

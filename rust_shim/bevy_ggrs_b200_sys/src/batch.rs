@@ -14,6 +14,8 @@ pub struct BatchCall<'a> {
 /// Owns a `bgr_batch`; the engines it was created from must outlive it (dropping it destroys the batch first).
 pub struct Batch {
     pub(crate) raw: *mut bgr_batch,
+    /// entries of the batched feed report in flight (`feed_begin`): the infos its wait writes
+    pub(crate) feed_entries: usize,
 }
 
 impl Batch {
@@ -21,7 +23,7 @@ impl Batch {
     pub fn new(engines: &[*mut bgr_engine]) -> Result<Batch, c_int> {
         let mut raw = ptr::null_mut();
         let rc = unsafe { bgr_batch_create(engines.as_ptr(), engines.len() as u32, &mut raw) };
-        if rc != BGR_OK { Err(rc) } else { Ok(Batch { raw }) }
+        if rc != BGR_OK { Err(rc) } else { Ok(Batch { raw, feed_entries: 0 }) }
     }
 
     /// True when calls run as one launch; false: each world's own bgr_handle_requests runs in turn.
