@@ -170,6 +170,11 @@ class bgr_edit(C.Structure):
                 ("byte_offset", C.c_uint32), ("byte_len", C.c_uint32), ("value_offset", C.c_uint32), ("reserved", C.c_uint32)]
 
 
+class bgr_batch_edits(C.Structure):
+    _fields_ = [("world", C.c_uint32), ("n_edits", C.c_uint32), ("edits", C.c_void_p), ("values", C.c_void_p),
+                ("values_bytes", C.c_size_t)]
+
+
 u32p = C.POINTER(C.c_uint32)
 i32p = C.POINTER(C.c_int32)
 u64p = C.POINTER(C.c_uint64)
@@ -261,6 +266,7 @@ PROTOTYPES = {
     "bgr_batch_checkpoint_restore": (C.c_int, [C.c_void_p, u32p, C.c_uint32, C.POINTER(C.c_void_p), C.POINTER(C.c_size_t), i32p]),
     "bgr_batch_feed_begin": (C.c_int, [C.c_void_p, C.POINTER(bgr_batch_feed), C.c_uint32, C.c_void_p, u32p, i32p]),
     "bgr_batch_feed_wait": (C.c_int, [C.c_void_p, C.c_uint32, C.POINTER(bgr_feed_info)]),
+    "bgr_batch_apply_edits": (C.c_int, [C.c_void_p, C.POINTER(bgr_batch_edits), C.c_uint32, i32p]),
     "bgr_seahash": (C.c_uint64, [C.c_void_p, C.c_uint64]),
     "bgr_ggrs_time_delta_bits": (C.c_uint32, [C.c_uint32, C.c_int32]),
     "bgr_particle_rng_stream": (C.c_int, [C.c_uint64, C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p, C.c_float, C.c_float]),

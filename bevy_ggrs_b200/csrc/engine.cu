@@ -11,6 +11,7 @@
 
 #include <algorithm>
 #include <array>
+#include <cassert>
 #include <cmath>
 #include <cstdio>
 #include <cstdlib>
@@ -35,6 +36,7 @@
 #include "frame_digest.cuh"
 #include "checkpoint.cuh"
 #include "checkpoint_check.hpp"
+#include "edit_batch.hpp"
 #include "feed_check.hpp"
 #include "replay_keyframes.hpp"
 #include "jit.hpp"
@@ -2007,6 +2009,17 @@ int fold_edits(bgr_engine* e, const bgr_edit* edits, uint32_t n, const uint8_t* 
     return BGR_OK;
 }
 
+// The staging buffer of a patch: the next one of a ring, once the batch that last used it has finished.  It grows to the
+// largest patch and stays (16 B per stored word): freeing the smaller buffer synchronises the device.  Even an empty
+// patch gets a buffer, so that the kernel always has a mapped address to read from.
+int take_edit_stage(bgr_engine::EditStage& sg, size_t bytes) {
+    CUDA_TRY(sg.done.ensure());
+    if (sg.busy) CUDA_TRY(cudaEventSynchronize(sg.done.get()));
+    sg.busy = false;
+    CUDA_TRY(sg.h.ensure(std::max<size_t>(bytes, 64u << 10)));
+    return BGR_OK;
+}
+
 int apply_edits(bgr_engine* e, const bgr_edit* edits, uint32_t n, const void* values, size_t values_bytes) {
     if (!e) return fail(BGR_ERR_INVALID_ARGUMENT, "null engine");
     if (!e->built) return fail(BGR_ERR_STATE, "engine not built");
@@ -2019,16 +2032,11 @@ int apply_edits(bgr_engine* e, const bgr_edit* edits, uint32_t n, const void* va
     f.clear();
     rc = fold_edits(e, edits, n, static_cast<const uint8_t*>(values), f);
     if (rc != BGR_OK) return rc;
-    // the staging buffer: the next one of the ring, once the batch that last used it has finished
     bgr_engine::EditStage& sg = e->edit_stage[e->next_edit];
     const size_t bytes_w = f.words.size() * sizeof(uint4), bytes_m = f.masks.size() * sizeof(uint2);
     const size_t bytes = bytes_w + bytes_m + f.stamps.size() * sizeof(uint32_t);
-    CUDA_TRY(sg.done.ensure());
-    if (sg.busy) CUDA_TRY(cudaEventSynchronize(sg.done.get()));
-    sg.busy = false;
-    // Grows to the largest batch and stays (16 B per stored word): freeing the smaller buffer synchronises the device.
-    // Even an empty patch gets a buffer, so that the kernel always has a mapped address to read from.
-    CUDA_TRY(sg.h.ensure(std::max<size_t>(bytes, 64u << 10)));
+    rc = take_edit_stage(sg, bytes);
+    if (rc != BGR_OK) return rc;
     // nothing fails past the capacity: growing is the last step that can refuse
     if (rows > e->st.n_rows) rc = grow_to(e, rows);
     if (rc == BGR_OK) rc = touch_live(e);  // stream-ordered behind the queued submits, like the launches below
@@ -2040,17 +2048,17 @@ int apply_edits(bgr_engine* e, const bgr_edit* edits, uint32_t n, const void* va
     const uint8_t* dev = sg.h.dev();
     if (rows > e->st.n_rows) {
         const uint32_t count = uint32_t(rows - e->st.n_rows);
-        k_spawn_rows<<<e->grid_for(count, 64), 256, 0, e->stream>>>(e->image(0), e->words, e->st.n_rows, count);
+        k_spawn_rows<false><<<e->grid_for(count, 64), 256, 0, e->stream>>>(e->image(0), e->words, e->st.n_rows, count, nullptr, 0);
         e->launches += 1;
         CUDA_TRY(cudaGetLastError());
     }
-    EditPatch p;
+    EditPatch p{};
     p.words = reinterpret_cast<const uint4*>(dev);
     p.masks = reinterpret_cast<const uint2*>(dev + bytes_w);
     p.stamps = reinterpret_cast<const uint32_t*>(dev + bytes_w + bytes_m);
     p.n_words = uint32_t(f.words.size()); p.n_masks = uint32_t(f.masks.size()); p.n_stamps = uint32_t(f.stamps.size());
     const uint32_t total = p.n_words + p.n_masks + p.n_stamps;
-    k_apply_edits<<<e->grid_for(total, 256), 256, 0, e->stream>>>(e->image(0), e->words, e->stamps.ptr<uint32_t>(), p);
+    k_apply_edits<false><<<e->grid_for(total, 256), 256, 0, e->stream>>>(e->image(0), e->words, e->stamps.ptr<uint32_t>(), p);
     e->launches += 1;
     CUDA_TRY(cudaGetLastError());
     CUDA_TRY(cudaEventRecord(sg.done.get(), e->stream));
@@ -2441,7 +2449,7 @@ BGR_API int bgr_spawn(bgr_engine* e, uint32_t count, uint32_t* first_row_out) {
     if (rc != BGR_OK) return rc;
     uint32_t first = e->st.n_rows;
     if (count) {
-        k_spawn_rows<<<e->grid_for(count, 64), 256, 0, e->stream>>>(e->image(0), e->words, first, count);
+        k_spawn_rows<false><<<e->grid_for(count, 64), 256, 0, e->stream>>>(e->image(0), e->words, first, count, nullptr, 0);
         e->launches += 1;
         CUDA_TRY(cudaGetLastError());
         e->st.n_rows += count;  // before clear_stamps: the fresh content id carries the new row count
@@ -3524,6 +3532,11 @@ struct bgr_batch {
         uint32_t ticket = 0, seq = 0;
         std::vector<bgr_batch_feed> listed;   // the entries of the report in flight
     } feed;
+    // bgr_batch_apply_edits: a ring of page-locked patches read in place (bgr_apply_edits' ring, on the batch's memory),
+    // and the device copy of a call's EditWorld / SpawnWorld tables, grown to the largest call
+    bgr_engine::EditStage edit_stage[bgr_engine::kEditBufs];
+    uint32_t next_edit = 0;
+    DeviceBuffer<uint8_t> edit_tables;
 };
 
 static bool same_specs(const bgr_engine* a, const bgr_engine* b) {
@@ -4515,6 +4528,111 @@ BGR_API int bgr_batch_feed_wait(bgr_batch* b, uint32_t ticket, bgr_feed_info* in
     x.busy = false;
     for (const bgr_batch_feed& r : x.listed) b->engines[r.world]->feeds[r.feed].busy = false;
     if (infos) std::memcpy(infos, x.h_info.get(), sizeof(bgr_feed_info) * x.listed.size());
+    return BGR_OK;
+}
+
+// ---- batched host edits: the bgr_apply_edits batches of many batch members in one call (edit_batch.hpp) ----
+BGR_API int bgr_batch_apply_edits(bgr_batch* b, const bgr_batch_edits* entries, uint32_t n, int32_t* status_out) {
+    if (!b) return fail(BGR_ERR_INVALID_ARGUMENT, "null batch");
+    if (n && (!entries || !status_out)) return fail(BGR_ERR_INVALID_ARGUMENT, "null argument");
+    NvtxRange span("ApplyEdits");
+    for (uint32_t i = 0; i < n; ++i) status_out[i] = BGR_OK;
+    auto world_fail = [&](uint32_t i, int status, const std::string& why) {
+        status_out[i] = status;
+        return fail(status, "world " + std::to_string(entries[i].world) + ": " + why);
+    };
+    // the host checks of every entry, then every fold, before anything runs
+    std::vector<uint64_t> rows(n);
+    uint32_t bad = 0;
+    std::string why;
+    int rc = edit_batch_check(uint32_t(b->engines.size()), entries, n,
+        [b](uint32_t w, const bgr_batch_edits& x, uint64_t* r, std::string* err) {
+            const int s = validate_edits(b->engines[w], x.edits, x.n_edits, x.values_bytes, r);
+            if (s != BGR_OK) *err = g_err;
+            return s;
+        },
+        [b](uint32_t w) { return uint64_t(b->engines[w]->st.n_rows); }, [b](uint32_t w) { return uint64_t(b->engines[w]->ceiling); },
+        rows.data(), &bad, &why);
+    if (rc != BGR_OK) return world_fail(bad, rc, why);
+    std::vector<EditCounts> counts(n);
+    for (uint32_t i = 0; i < n; ++i) {
+        bgr_engine* e = b->engines[entries[i].world];
+        EditFold& f = e->edit_fold;  // each member folds into its own scratch
+        f.clear();
+        if (entries[i].n_edits) {
+            rc = fold_edits(e, entries[i].edits, entries[i].n_edits, static_cast<const uint8_t*>(entries[i].values), f);
+            if (rc != BGR_OK) return world_fail(i, rc, g_err);
+            assert(f.stamps.empty() && "batch members never run the bundle kernel, so they have no content stamps");
+        }
+        counts[i] = EditCounts{f.words.size(), f.masks.size(), e->st.n_rows, uint32_t(rows[i] - e->st.n_rows)};
+    }
+    EditLayout L;
+    rc = edit_layout(counts.data(), n, &L, &bad, &why);
+    if (rc != BGR_OK) return world_fail(bad, rc, why);
+    if (n == 0) return BGR_OK;
+    // every buffer, then growth, then the listed worlds' deferred live images, stream-ordered behind the queued submits
+    bgr_engine::EditStage& sg = b->edit_stage[b->next_edit];
+    rc = take_edit_stage(sg, L.bytes);
+    if (rc != BGR_OK) return rc;
+    const size_t table_bytes = L.bytes - L.off_patch;
+    if (table_bytes) CUDA_TRY(b->edit_tables.ensure(table_bytes));
+    for (uint32_t i = 0; i < n; ++i) {
+        bgr_engine* e = b->engines[entries[i].world];
+        if (rows[i] > e->st.n_rows) rc = grow_to(e, rows[i]);
+        if (rc != BGR_OK) return world_fail(i, rc, g_err);
+    }
+    for (uint32_t i = 0; i < n; ++i) {
+        if (entries[i].n_edits) rc = touch_live(b->engines[entries[i].world]);
+        if (rc != BGR_OK) return world_fail(i, rc, g_err);
+    }
+    // the staging: every world's words and masks at its offsets, then the two tables
+    uint8_t* h = sg.h.get();
+    uint4* hw = reinterpret_cast<uint4*>(h);
+    for (size_t k = 0; k < L.patch.size(); ++k) {
+        EditWorld& w = L.patch[k];
+        const EditFold& f = b->engines[entries[L.patch_entry[k]].world]->edit_fold;
+        w.img = b->engines[entries[L.patch_entry[k]].world]->image(0);
+        for (size_t j = 0; j < f.words.size(); ++j) hw[w.word0 + j] = make_uint4(f.words[j].row, f.words[j].plane, f.words[j].value, 0u);
+        if (!f.masks.empty()) std::memcpy(h + L.off_masks + size_t(w.mask0) * sizeof(uint2), f.masks.data(), f.masks.size() * sizeof(uint2));
+    }
+    for (size_t k = 0; k < L.spawn.size(); ++k) L.spawn[k].img = b->engines[entries[L.spawn_entry[k]].world]->image(0);
+    if (!L.patch.empty()) std::memcpy(h + L.off_patch, L.patch.data(), L.patch.size() * sizeof(EditWorld));
+    if (!L.spawn.empty()) std::memcpy(h + L.off_spawn, L.spawn.data(), L.spawn.size() * sizeof(SpawnWorld));
+    // one table upload and at most two launches, counted on the first listed world
+    bgr_engine* e0 = b->engines[entries[0].world];
+    uint8_t* d_tab = b->edit_tables.get();
+    if (table_bytes) CUDA_TRY(cudaMemcpyAsync(d_tab, h + L.off_patch, table_bytes, cudaMemcpyHostToDevice, b->stream));
+    const uint32_t words = e0->words;  // one registration: one row stride
+    if (L.n_spawned) {
+        const SpawnWorld* d_spawn = reinterpret_cast<const SpawnWorld*>(d_tab + (L.off_spawn - L.off_patch));
+        k_spawn_rows<true><<<e0->grid_for(L.n_spawned, 64), 256, 0, b->stream>>>(nullptr, words, 0u, L.n_spawned, d_spawn,
+                                                                                  uint32_t(L.spawn.size()));
+        e0->launches += 1;
+        CUDA_TRY(cudaGetLastError());
+    }
+    if (L.n_words + L.n_masks) {
+        const uint8_t* dev = sg.h.dev();
+        EditPatch p{};
+        p.words = reinterpret_cast<const uint4*>(dev);
+        p.masks = reinterpret_cast<const uint2*>(dev + L.off_masks);
+        p.n_words = L.n_words; p.n_masks = L.n_masks;
+        p.worlds = reinterpret_cast<const EditWorld*>(d_tab);
+        p.n_worlds = uint32_t(L.patch.size());
+        k_apply_edits<true><<<e0->grid_for(L.n_words + L.n_masks, 256), 256, 0, b->stream>>>(nullptr, words, nullptr, p);
+        e0->launches += 1;
+        CUDA_TRY(cudaGetLastError());
+    }
+    CUDA_TRY(cudaEventRecord(sg.done.get(), b->stream));
+    sg.busy = true;
+    b->next_edit = (b->next_edit + 1) % bgr_engine::kEditBufs;
+    for (bgr_engine* e : b->engines) e->tiledep_chain = false;  // the launches ran on the shared stream
+    for (uint32_t i = 0; i < n; ++i) {  // commit, as apply_edits does
+        if (!entries[i].n_edits) continue;
+        bgr_engine* e = b->engines[entries[i].world];
+        e->st.n_rows = uint32_t(rows[i]);
+        if (e->edit_fold.bump) e->st.live_passive_ver = ++e->st.ver_counter;
+        e->st.cids.live = e->st.cids.fresh(e->st.n_rows);
+    }
     return BGR_OK;
 }
 

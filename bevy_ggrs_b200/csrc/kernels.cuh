@@ -1084,13 +1084,45 @@ __global__ void k_set_absent(uint8_t* img, uint32_t words, uint32_t row, uint32_
     uint8_t* m = img + alive_offset(words, row);
     if (*m & 1u) *m = absent ? uint8_t(*m | bit) : uint8_t(*m & ~bit);
 }
-// `commands.spawn((..., Rollback))`: zeroed components, alive = 1
-__global__ void __launch_bounds__(256) k_spawn_rows(uint8_t* img, uint32_t words, uint32_t first_row, uint32_t count) {
+// The last entry of a table of `n` whose `key` is <= g: the entry global index g belongs to, for tables in ascending key
+// order where an entry owns [its key, the next entry's key).  An entry that owns nothing shares the next one's key and
+// comes before it, so it is never found.
+template <class Entry, class Key>
+__device__ __forceinline__ uint32_t table_entry_of(const Entry* tab, uint32_t n, Key Entry::*key, uint64_t g) {
+    uint32_t lo = 0, hi = n;
+    while (hi - lo > 1u) {
+        const uint32_t mid = (lo + hi) >> 1;
+        if (uint64_t(tab[mid].*key) <= g) lo = mid; else hi = mid;
+    }
+    return lo;
+}
+
+// one spawning world of a batched edit call (bgr_batch_apply_edits): rows [first_row, first_row + count) of its image
+// 0, global spawned rows [row0, row0 + count)
+struct SpawnWorld {
+    uint8_t* img;
+    uint32_t row0, first_row, count, pad;
+};
+static_assert(sizeof(SpawnWorld) == 24, "SpawnWorld layout (the engine and the kernels must agree)");
+
+// `commands.spawn((..., Rollback))`: zeroed components, alive = 1.  kTable: `count` rows over every world of `worlds`
+// (bgr_batch_apply_edits; img and first_row unused), each row's world found by binary search.  Otherwise rows
+// [first_row, first_row + count) of `img`.
+template <bool kTable>
+__global__ void __launch_bounds__(256) k_spawn_rows(uint8_t* img, uint32_t words, uint32_t first_row, uint32_t count,
+                                                    const SpawnWorld* worlds, uint32_t n_worlds) {
     const size_t n = size_t(count) * (words + 1);
     for (size_t t = size_t(blockIdx.x) * blockDim.x + threadIdx.x; t < n; t += size_t(gridDim.x) * blockDim.x) {
         const uint32_t i = uint32_t(t / (words + 1)), w = uint32_t(t % (words + 1));
-        if (w < words) *reinterpret_cast<uint32_t*>(img + word_offset(words, first_row + i, w)) = 0u;
-        else img[alive_offset(words, first_row + i)] = 1;
+        uint8_t* im = img;
+        uint32_t row = first_row + i;
+        if (kTable) {
+            const SpawnWorld s = worlds[table_entry_of(worlds, n_worlds, &SpawnWorld::row0, i)];
+            im = s.img;
+            row = s.first_row + (i - s.row0);
+        }
+        if (w < words) *reinterpret_cast<uint32_t*>(im + word_offset(words, row, w)) = 0u;
+        else im[alive_offset(words, row)] = 1;
     }
 }
 __global__ void k_set_alive(uint8_t* img, uint32_t words, uint32_t row, uint8_t value) { img[alive_offset(words, row)] = value; }
@@ -1103,23 +1135,47 @@ __global__ void k_set_alive(uint8_t* img, uint32_t words, uint32_t row, uint8_t 
 //           clears the byte whatever it held;
 //   stamps: indices into image 0's content-stamp row whose stamps become unknown.
 // The three lists touch disjoint bytes, so one flat index space covers them in any order.
+// bgr_batch_apply_edits patches many worlds in one launch: their words and masks are the concatenation of each world's
+// own lists (in list order), and `worlds` (kTable, below) gives each world its share.  Batch members never run the
+// bundle kernel, so a batched patch has no stamps.
+struct EditWorld {
+    uint8_t* img;            // image 0
+    uint32_t t0;             // its first global index: its words, then its masks, up to the next entry's t0
+    uint32_t n_words;
+    uint32_t word0, mask0;   // its first word in `words`, its first mask in `masks`
+};
+static_assert(sizeof(EditWorld) == 24, "EditWorld layout (the engine and the kernels must agree)");
 struct EditPatch {
     const uint4* words;
     const uint2* masks;
     const uint32_t* stamps;
     uint32_t n_words, n_masks, n_stamps;
+    const EditWorld* worlds;  // kTable: [n_worlds], ascending t0
+    uint32_t n_worlds;
 };
+__device__ __forceinline__ void edit_word(uint8_t* img, uint32_t words, const uint4 w) {
+    *reinterpret_cast<uint32_t*>(img + word_offset(words, w.x, w.y)) = w.z;
+}
+__device__ __forceinline__ void edit_mask(uint8_t* img, uint32_t words, const uint2 m) {
+    uint8_t* a = img + alive_offset(words, m.x);
+    if (m.y >> 16) *a = 0;
+    else if (*a & 1u) *a = uint8_t((*a & m.y) | (m.y >> 8));
+}
+// kTable: the patch of every world of p.worlds (img and stamps unused), each index's world found by binary search.
+// Otherwise the one world `img` with its stamps, as bgr_apply_edits has always run it.
+template <bool kTable>
 __global__ void __launch_bounds__(256) k_apply_edits(uint8_t* img, uint32_t words, uint32_t* stamps, const EditPatch p) {
     const uint32_t n = p.n_words + p.n_masks + p.n_stamps;
     for (uint32_t t = blockIdx.x * blockDim.x + threadIdx.x; t < n; t += gridDim.x * blockDim.x) {
-        if (t < p.n_words) {
-            const uint4 w = p.words[t];
-            *reinterpret_cast<uint32_t*>(img + word_offset(words, w.x, w.y)) = w.z;
+        if (kTable) {
+            const EditWorld w = p.worlds[table_entry_of(p.worlds, p.n_worlds, &EditWorld::t0, t)];
+            const uint32_t k = t - w.t0;
+            if (k < w.n_words) edit_word(w.img, words, p.words[w.word0 + k]);
+            else edit_mask(w.img, words, p.masks[w.mask0 + (k - w.n_words)]);
+        } else if (t < p.n_words) {
+            edit_word(img, words, p.words[t]);
         } else if (t < p.n_words + p.n_masks) {
-            const uint2 m = p.masks[t - p.n_words];
-            uint8_t* a = img + alive_offset(words, m.x);
-            if (m.y >> 16) *a = 0;
-            else if (*a & 1u) *a = uint8_t((*a & m.y) | (m.y >> 8));
+            edit_mask(img, words, p.masks[t - p.n_words]);
         } else {
             stamps[p.stamps[t - p.n_words - p.n_masks]] = 0u;
         }

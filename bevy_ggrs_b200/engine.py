@@ -721,6 +721,20 @@ class EngineBatch:
         status = (C.c_int32 * max(1, n))()
         self._check(self._lib.bgr_batch_checkpoint_restore(self._h, worlds, n, blobs, sizes, status))
 
+    def apply_edits(self, calls) -> None:
+        """``calls`` = [(world, edits, values), ...]: Engine.apply_edits of every listed world in one queued call (at
+        most one spawn launch and one patch launch over all of them).  ``edits`` is an ``EDIT_DTYPE`` array, ``values``
+        the bytes its WRITE / INSERT records point into; both are free on return.  All or nothing: a refused call raises
+        BgrError (its status, and text starting with "world <index>: ") and changes no world."""
+        calls = [(int(w), np.ascontiguousarray(x, dtype=EDIT_DTYPE), np.frombuffer(bytes(v), dtype=np.uint8))
+                 for w, x, v in calls]
+        n = len(calls)
+        entries = (capi.bgr_batch_edits * max(1, n))(*[
+            capi.bgr_batch_edits(w, len(x), x.ctypes.data if len(x) else None, v.ctypes.data if v.size else None, v.size)
+            for w, x, v in calls])
+        status = (C.c_int32 * max(1, n))()
+        self._check(self._lib.bgr_batch_apply_edits(self._h, entries, n, status))
+
     # ---- batched change feed (bgr_batch_feed_*): many members' feeds in one pass ----
     def _feed_bytes(self, calls) -> Optional[int]:
         """sum(cap) records of the first call's feed (a call has one record size), or None when the first call names no

@@ -779,6 +779,37 @@ BGR_API int bgr_batch_feed_begin(bgr_batch* b, const bgr_batch_feed* reports, ui
                                  uint32_t* ticket_out, int32_t* status_out);
 BGR_API int bgr_batch_feed_wait(bgr_batch* b, uint32_t ticket, bgr_feed_info* infos);
 
+/* ---- batched host edits: the bgr_apply_edits batches of many batch members in one call -----------------------------
+ * Entry i leaves member entries[i].world exactly as bgr_apply_edits(that engine, edits, n_edits, values, values_bytes)
+ * would: the live image and row count, presence bytes, the passive version (moved only by spawns, inserts, removes and
+ * passive-plane writes), a fresh live content id, and a deferred live image materialised first.  Worlds not listed are
+ * untouched; an entry with n_edits == 0 changes nothing in its world (it materialises nothing either), but is still
+ * checked for its index.
+ * In the conventions of the other batch calls, every entry is checked in list order before anything runs: indices in
+ * range and distinct, no null pointer, every record by bgr_apply_edits' own checks, spawns past a fixed member's
+ * max_entities or a growable member's ceiling (BGR_ERR_CAPACITY), spawning after the first request vector with
+ * order_base != 0 (BGR_ERR_UNSUPPORTED).  A refusal marks the entry in status_out, bgr_last_error() reads
+ * "world <index>: " and the single call's text ("world 2: edit 3: row out of range"), and nothing changes anywhere: no
+ * member grows, nothing launches.  Then growable members grow; a growth that fails names its world (BGR_ERR_CUDA or
+ * BGR_ERR_CAPACITY) and nothing is edited, and members that grew before it keep their larger capacity, as in
+ * bgr_batch_handle_requests.
+ * The call is ordered on the shared stream behind every queued vector, un-collected bgr_submit_requests of a member
+ * included (they keep their results), and returns without waiting for the GPU.  The caller's buffers are free on
+ * return: the patch goes into one of 4 page-locked staging buffers the batch owns, each grown to the largest call it
+ * has held, and the call waits only when all 4 belong to unfinished calls (bgr_apply_edits' rule, on the batch's
+ * memory).  Whatever n_entries, a call is at most one table upload and two launches, counted on entries[0].world's
+ * bgr_launch_count: k_spawn_rows over every spawning world when one spawns, and k_apply_edits over every patch when
+ * one is non-empty.  A listed world with a deferred live image and n_edits > 0 also gets its own materialisation,
+ * counted on that world.  It does not depend on bgr_batch_specialised: the edit kernels are part of the library. */
+typedef struct bgr_batch_edits {     /* 32 bytes */
+    uint32_t world;                  /* index in the batch */
+    uint32_t n_edits;
+    const bgr_edit* edits;           /* bgr_apply_edits' records, unchanged */
+    const void* values;
+    size_t values_bytes;
+} bgr_batch_edits;
+BGR_API int bgr_batch_apply_edits(bgr_batch* b, const bgr_batch_edits* entries, uint32_t n_entries, int32_t* status_out);
+
 /* ---- shard group: the cross-shard step inside the engine (multi-GPU, one process per GPU, one node) -----------------
  * Entity-range shards never exchange state (SURVEY.md §8e: systems read no other entity, box_game.rs:162-169; the
  * checksum is an XOR over entities, component_checksum.rs:88-89).  The only exchange is 64 bytes of partials per

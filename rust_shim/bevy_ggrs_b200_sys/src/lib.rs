@@ -75,7 +75,7 @@ pub use p2p_desync::*;
 // the change feed structs (bgr_feed_field / bgr_feed_info / bgr_batch_feed) too, and the batched report over a world batch
 mod change_feed;
 pub use change_feed::*;
-
+// the host edit record and the batched edits over a world batch
 mod host_edits;
 pub use host_edits::*;
 // the world checkpoint header too
@@ -215,6 +215,7 @@ extern "C" {
     pub fn bgr_batch_checkpoint_restore(b: *mut bgr_batch, worlds: *const u32, n_worlds: u32, blobs: *const *const c_void, bytes: *const usize, status_out: *mut i32) -> c_int;
     pub fn bgr_batch_feed_begin(b: *mut bgr_batch, reports: *const bgr_batch_feed, n_entries: u32, host_dst: *mut c_void, ticket_out: *mut u32, status_out: *mut i32) -> c_int;
     pub fn bgr_batch_feed_wait(b: *mut bgr_batch, ticket: u32, infos: *mut bgr_feed_info) -> c_int;
+    pub fn bgr_batch_apply_edits(b: *mut bgr_batch, entries: *const bgr_batch_edits, n_entries: u32, status_out: *mut i32) -> c_int;
     pub fn bgr_seahash(bytes: *const c_void, len: u64) -> u64;
     pub fn bgr_ggrs_time_delta_bits(fps: u32, frame: i32) -> u32;
     pub fn bgr_particle_rng_stream(seed: u64, state4_or_null: *const u64, n: u32, next_u64_out: *mut u64, range_out: *mut f32, low: f32, high: f32) -> c_int;
