@@ -157,6 +157,16 @@ class bgr_feed_field(C.Structure):
     _fields_ = [("column", C.c_uint32), ("byte_offset", C.c_uint32), ("byte_len", C.c_uint32)]
 
 
+class bgr_trace_sample(C.Structure):
+    _fields_ = [("frame", C.c_int32), ("rows", C.c_uint32)]
+
+
+class bgr_trace(C.Structure):
+    _fields_ = [("interval", C.c_uint32), ("first_row", C.c_uint32), ("n_rows", C.c_uint32), ("n_fields", C.c_uint32),
+                ("fields", C.POINTER(bgr_feed_field)), ("dst", C.c_void_p), ("dst_cap", C.c_size_t),
+                ("samples", C.POINTER(bgr_trace_sample)), ("samples_cap", C.c_uint32), ("reserved", C.c_uint32)]
+
+
 class bgr_feed_info(C.Structure):
     _fields_ = [("n_records", C.c_uint32), ("pending", C.c_uint32), ("rows", C.c_uint32), ("record_bytes", C.c_uint32)]
 
@@ -261,6 +271,10 @@ PROTOTYPES = {
                                        C.c_uint32, u32p, u32p, C.POINTER(C.c_size_t)]),
     "bgr_batch_replay_keyframes": (C.c_int, [C.c_void_p, u32p, C.c_uint32, C.POINTER(bgr_replay), C.POINTER(bgr_keyframes),
                                              C.POINTER(bgr_checksum), C.c_uint32, u32p, u32p, i32p]),
+    "bgr_replay_trace": (C.c_int, [C.c_void_p, C.POINTER(bgr_replay), C.POINTER(bgr_trace), C.POINTER(bgr_checksum),
+                                   C.c_uint32, u32p, u32p, C.POINTER(C.c_size_t)]),
+    "bgr_batch_replay_trace": (C.c_int, [C.c_void_p, u32p, C.c_uint32, C.POINTER(bgr_replay), C.POINTER(bgr_trace),
+                                         C.POINTER(bgr_checksum), C.c_uint32, u32p, u32p, i32p]),
     "bgr_batch_checkpoint_save": (C.c_int, [C.c_void_p, u32p, C.c_uint32, i32p, C.c_void_p, C.c_size_t, C.POINTER(bgr_keyframe),
                                             C.POINTER(C.c_size_t), i32p]),
     "bgr_batch_checkpoint_restore": (C.c_int, [C.c_void_p, u32p, C.c_uint32, C.POINTER(C.c_void_p), C.POINTER(C.c_size_t), i32p]),

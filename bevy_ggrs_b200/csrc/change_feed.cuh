@@ -26,6 +26,8 @@
 //   copy   (k_feed_copy, copy stream, behind an event after pass 2): moves the records of every listed world from device
 //          memory into page-locked host memory, so PCIe carries n_records * record_bytes; the 16-byte infos follow by
 //          cudaMemcpyAsync.
+// k_trace_gather (below) writes the same records for a row range whether or not they changed: the samples of a replay
+// trace (bgr_replay_trace) taken without a generated kernel.
 #pragma once
 #include "kernels.cuh"
 
@@ -281,6 +283,46 @@ __global__ void __launch_bounds__(kFeedBlock, 4) k_feed_records(const __grid_con
             *reinterpret_cast<uint32_t*>(rt + size_t(rp) * kPlaneBytes + lane_off) = c;
         });
         rt[size_t(p.rep_words) * kPlaneBytes + threadIdx.x] = uint8_t(cm);
+    }
+}
+
+// One listed world of a trace gather: the records of rows [first_row, first_row + n_rows) of image `img` (of `rows`
+// rows) go to out; rec0 is its first record in the launch (a prefix of n_rows in table order)
+struct TraceGather {
+    const uint8_t* img;
+    uint32_t* out;
+    uint32_t rows, first_row, n_rows, rec0;
+};
+
+// The trace records of every listed world's rows (bgr_replay_trace without a generated kernel, at each sample frame):
+// the change feed's record of each row (u32 row, u32 state, the field words, zero where not present), whether or not it
+// changed, and state 0 with zero words for rows that do not exist.  One thread per record.
+__global__ void __launch_bounds__(256) k_trace_gather(const __grid_constant__ FeedParams p, const TraceGather* __restrict__ tab,
+                                                      uint32_t n_worlds, uint32_t n_records) {
+    const uint32_t t = blockIdx.x * blockDim.x + threadIdx.x;
+    if (t >= n_records) return;
+    uint32_t lo = 0, hi = n_worlds;
+    while (hi - lo > 1u) {
+        const uint32_t mid = (lo + hi) >> 1;
+        if (tab[mid].rec0 <= t) lo = mid; else hi = mid;
+    }
+    const TraceGather g = tab[lo];
+    const uint32_t i = t - g.rec0, row = g.first_row + i;
+    const uint8_t* tile = g.img + size_t(row / kTileRows) * tile_bytes_of(p.words);  // read only where the row exists
+    const uint32_t cm = feed_cur_mask(p, tile, g.rows, row);
+    uint32_t* rec = g.out + size_t(i) * p.record_words;
+    uint32_t state = cm ? 1u : 0u;
+    for (uint32_t q = 0; q < p.n_fields; ++q)
+        if (feed_present(cm, p.fields[q].absent)) state |= 2u << q;
+    rec[0] = row;
+    rec[1] = state;
+    uint32_t at = 2;
+    const size_t lane_off = size_t(row % kTileRows) * 4u;
+    for (uint32_t q = 0; q < p.n_fields; ++q) {
+        const FeedField f = p.fields[q];
+        const bool pc = feed_present(cm, f.absent);
+        for (uint32_t w = 0; w < f.words; ++w)
+            rec[at++] = pc ? *reinterpret_cast<const uint32_t*>(tile + size_t(f.plane + w) * kPlaneBytes + lane_off) : 0u;
     }
 }
 

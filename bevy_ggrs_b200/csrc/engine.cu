@@ -39,6 +39,7 @@
 #include "edit_batch.hpp"
 #include "feed_check.hpp"
 #include "replay_keyframes.hpp"
+#include "replay_trace.hpp"
 #include "jit.hpp"
 #include "vmm_range.hpp"
 #include "device_memory.hpp"
@@ -82,6 +83,11 @@ constexpr uint32_t kReplayLaunchPoints = 1u << 20;
 // of each unfinished world.  256 MB is a choice, not a measurement: a few 1M-row stress frames, or every keyframe of a
 // thousand box_game worlds over a minute.  BGR_TUNE_KEYFRAME_BYTES lowers it (tests of replays that take many launches).
 constexpr uint64_t kKeyframeLaunchBytes = 256ull << 20;
+// bytes of trace records one replay launch stages (bgr_replay_trace), split over the unfinished worlds; a launch always
+// holds at least one sample of each.  256 MB is a choice, not a measurement, made like the keyframe budget: every
+// sample of a 3 600-frame match tracing 64 rows of 32-byte records at T = 1 is 7.4 MB, so a thousand such worlds take a
+// few launches.  BGR_TUNE_TRACE_BYTES lowers it (tests of replays that take many launches).
+constexpr uint64_t kTraceLaunchBytes = 256ull << 20;
 
 constexpr uint32_t kMaxDeferredOps = 4;  // trailing ADVANCEs a deferred live image replays (SyncTest / P2P ticks: 1)
 
@@ -397,6 +403,7 @@ struct bgr_engine {
     uint32_t tune_replay_points = 0;  // checksum points per replay launch (kReplayLaunchPoints unless BGR_TUNE_REPLAY_POINTS)
     DeviceBuffer<uint8_t> replay_stage;
     uint64_t tune_keyframe_bytes = 0;  // keyframe images one replay launch stages (kKeyframeLaunchBytes unless BGR_TUNE_KEYFRAME_BYTES)
+    uint64_t tune_trace_bytes = 0;     // trace records one replay launch stages (kTraceLaunchBytes unless BGR_TUNE_TRACE_BYTES)
     DeviceBuffer<unsigned long long> replay_acc;
     const void* jit_chain_kernel = nullptr;  // the signalling launch `tiledep_chain` refers to (its work-item partition must match)
     int tune_jit_item = 0;          // 0 auto (quarter tiles below 3 tiles per SM), 512 / 256 / 128 force the rows per work item
@@ -1683,6 +1690,12 @@ int download_wait(bgr_engine* e, uint32_t ticket) {
 }
 
 // ---- change feed (change_feed.cuh) ----
+// feed_fields (feed_check.hpp) over the engine's registered columns
+int engine_feed_fields(const bgr_engine* e, const bgr_feed_field* fields, uint32_t n_fields, FeedParams& p, std::string* err) {
+    auto col_at = [e](uint32_t c) { return FeedColumn{e->cols[c].first_plane, e->cols[c].words, e->cols[c].absent}; };
+    return feed_fields(uint32_t(e->cols.size()), col_at, e->words, fields, n_fields, p, err);
+}
+
 int feed_create(bgr_engine* e, const bgr_feed_field* fields, uint32_t n_fields, uint32_t* feed_out) {
     if (!e || !feed_out || (n_fields && !fields)) return fail(BGR_ERR_INVALID_ARGUMENT, "null argument");
     if (!e->built) return fail(BGR_ERR_STATE, "bgr_feed_create before bgr_build");
@@ -1692,24 +1705,11 @@ int feed_create(bgr_engine* e, const bgr_feed_field* fields, uint32_t n_fields, 
         if (!e->feeds[i].used) id = i;
     if (id == BGR_MAX_FEEDS) return fail(BGR_ERR_CAPACITY, "too many feeds (BGR_MAX_FEEDS)");
     FeedParams p{};
-    p.keep = 1u;
-    for (uint32_t k = 0; k < n_fields; ++k) {
-        const bgr_feed_field& f = fields[k];
-        if (f.column >= e->cols.size()) return fail(BGR_ERR_INVALID_ARGUMENT, "unknown column");
-        const Column& c = e->cols[f.column];
-        if ((f.byte_offset & 3u) || (f.byte_len & 3u) || f.byte_len == 0 ||
-            uint64_t(f.byte_offset) + f.byte_len > uint64_t(c.words) * 4u)
-            return fail(BGR_ERR_INVALID_ARGUMENT, "field range must be 4-byte aligned and inside the element");
-        p.fields[k] = FeedField{c.first_plane + f.byte_offset / 4u, f.byte_len / 4u, c.absent, p.rep_words};
-        p.rep_words += f.byte_len / 4u;
-        p.keep |= c.absent;
-    }
-    p.n_fields = n_fields;
-    p.words = e->words;
-    p.record_words = 2u + p.rep_words;
+    std::string err;
+    const int rc = engine_feed_fields(e, fields, n_fields, p, &err);
+    if (rc != BGR_OK) return fail(rc, err);
     bgr_engine::Feed& fd = e->feeds[id];
     fd.p = p;
-    std::string err;
     bool ok = true;
     for (const CapacityBuffer& b : feed_buffers(fd))
         ok = ok && create_range(e, b, &err) && b.range->map_to(b.bytes(e->n_tiles_cap), &err);
@@ -2189,6 +2189,7 @@ BGR_API int bgr_engine_create(const bgr_config* cfg, bgr_engine** out) {
     e->tune_jit_item = env_int("BGR_TUNE_JIT_ITEM", 0);
     e->tune_replay_points = uint32_t(std::max(1, env_int("BGR_TUNE_REPLAY_POINTS", int(kReplayLaunchPoints))));
     e->tune_keyframe_bytes = uint64_t(std::max(1, env_int("BGR_TUNE_KEYFRAME_BYTES", int(kKeyframeLaunchBytes))));
+    e->tune_trace_bytes = uint64_t(std::max(1, env_int("BGR_TUNE_TRACE_BYTES", int(kTraceLaunchBytes))));
     e->tune_jit_tiledep = env_int("BGR_TUNE_JIT_TILEDEP", 0);
     e->tune_passive_early = env_int("BGR_TUNE_PASSIVE_EARLY", -1);
     e->tune_stagger_ns = env_int("BGR_TUNE_STAGGER_NS", 800);
@@ -3764,6 +3765,12 @@ struct ReplayJob {
     uint32_t n_kf = 0, kf_done = 0;  // keyframes in the log, and written
     size_t kf_bound = 0;             // bytes the blobs may take: every vector RAW, alignment included
     size_t kf_pos = 0, kf_end = 0;   // the next blob's offset in kf->dst, and the end of the last one
+    // trace (bgr_replay_trace): samples at frames f0 + j, j in [0, n), with (f0 + j) % tr->interval == 0
+    const struct bgr_trace* tr = nullptr;
+    FeedParams tp{};                        // its field list mapped onto the image (feed_fields)
+    std::vector<bgr_trace_sample> samples;  // every sample of the log (replay_trace.hpp)
+    size_t tr_stride = 0;                   // bytes per sample: n_rows records
+    uint32_t tr_done = 0;                   // samples written
 };
 
 uint64_t ggrs_runtime_ns(const bgr_engine* e, int64_t frame) { return uint64_t(frame) * 1000000000ULL / uint64_t(e->cfg.fps); }
@@ -3776,15 +3783,26 @@ uint32_t rows_at(const ReplayJob& job, uint32_t j) { return job.c.rows0 + job.c.
 // keyframe frames f0 + j with j in [a, b): the first one (~0: none) and how many
 uint64_t first_kf(const ReplayJob& job, uint32_t a, uint32_t b) { return replay_first_point(job.c.f0, job.kf ? job.kf->interval : 0u, a, b); }
 uint32_t kfs_in(const ReplayJob& job, uint32_t a, uint32_t b) { return replay_points_in(job.c.f0, job.kf ? job.kf->interval : 0u, a, b); }
+// trace sample frames f0 + j with j in [a, b): the first one (~0: none) and how many
+uint64_t first_tr(const ReplayJob& job, uint32_t a, uint32_t b) { return replay_first_point(job.c.f0, job.tr ? job.tr->interval : 0u, a, b); }
+uint32_t trs_in(const ReplayJob& job, uint32_t a, uint32_t b) { return replay_points_in(job.c.f0, job.tr ? job.tr->interval : 0u, a, b); }
 
-// Validates a replay (with keyframes when kf is not null) and computes everything the replay changes on the host,
-// without executing or changing anything
-int replay_plan(bgr_engine* e, const struct bgr_replay* r, ReplayJob& job, const struct bgr_keyframes* kf = nullptr) {
+// Validates a replay (with keyframes when kf is not null, with a trace when tr is not null) and computes everything the
+// replay changes on the host, without executing or changing anything
+int replay_plan(bgr_engine* e, const struct bgr_replay* r, ReplayJob& job, const struct bgr_keyframes* kf = nullptr,
+                const struct bgr_trace* tr = nullptr) {
     if (!e) return fail(BGR_ERR_INVALID_ARGUMENT, "null engine");
     if (!e->built) return fail(BGR_ERR_STATE, "bgr_build has not been called");
     if (!r) return fail(BGR_ERR_INVALID_ARGUMENT, "null replay");
     if (kf && kf->interval == 0) return fail(BGR_ERR_INVALID_ARGUMENT, "bgr_keyframes.interval must be >= 1");
     if (kf && kf->reserved) return fail(BGR_ERR_INVALID_ARGUMENT, "bgr_keyframes.reserved must be 0");
+    FeedParams tp{};
+    if (tr) {
+        std::string err;
+        int rc = trace_check(*tr, e->growable() ? e->ceiling : e->cfg.max_entities, &err);
+        if (rc == BGR_OK) rc = engine_feed_fields(e, tr->fields, tr->n_fields, tp, &err);
+        if (rc != BGR_OK) return fail(rc, err);
+    }
     if ((e->cfg.flags & BGR_CFG_SHARDED) || e->group) return fail(BGR_ERR_UNSUPPORTED, "replays do not run on sharded engines");
     if (!e->pending.empty()) return fail(BGR_ERR_STATE, "bgr_replay with un-collected bgr_submit_requests pending: call bgr_collect first");
     if (r->reserved) return fail(BGR_ERR_INVALID_ARGUMENT, "bgr_replay.reserved must be 0");
@@ -3799,7 +3817,7 @@ int replay_plan(bgr_engine* e, const struct bgr_replay* r, ReplayJob& job, const
     if (n && ggrs_runtime_ns(e, int64_t(s.frame_count) + 1) < s.elapsed_ns)
         return fail(BGR_ERR_STATE, "tried to move Time<GgrsTime> backwards (RollbackFrameCount went back without LoadWorld)");
     job = ReplayJob{};
-    job.e = e; job.r = r; job.kf = kf;
+    job.e = e; job.r = r; job.kf = kf; job.tr = tr;
     uint32_t n_counter = 0;
     for (const SystemReg& sy : e->systems) n_counter += (sy.id == BGR_SYS_U32_STORE_CALL_COUNT);
     const bool spawn = e->spawn_sys >= 0;
@@ -3840,6 +3858,11 @@ int replay_plan(bgr_engine* e, const struct bgr_replay* r, ReplayJob& job, const
         job.n_kf = uint32_t(job.kfp.size());
         for (const KeyframePlan& p : job.kfp) job.kf_bound += p.max_bytes;
     }
+    if (tr) {
+        job.tp = tp;
+        job.samples = plan_trace_samples(c, n, tr->interval, job.prefix);
+        job.tr_stride = size_t(tr->n_rows) * trace_record_bytes(tp);
+    }
     job.elapsed_end = n ? ggrs_runtime_ns(e, int64_t(c.f0) + n) : s.elapsed_ns;
     job.n_points = points_in(job, 0, n);
     return BGR_OK;
@@ -3854,6 +3877,52 @@ int keyframe_caps(const ReplayJob& job) {
     if (kf->index_cap < job.n_kf)
         return fail(BGR_ERR_CAPACITY, "the replay writes " + std::to_string(job.n_kf) + " keyframes, index_cap is " + std::to_string(kf->index_cap));
     if (job.n_kf && !kf->index) return fail(BGR_ERR_INVALID_ARGUMENT, "null keyframe index");
+    return BGR_OK;
+}
+
+// The output checks of a planned replay with a trace, made before anything runs (a null dst holds nothing)
+int trace_caps(const ReplayJob& job) {
+    const struct bgr_trace* t = job.tr;
+    const size_t need = job.samples.size() * job.tr_stride, cap = t->dst ? t->dst_cap : 0u;
+    if (cap < need) return fail(BGR_ERR_CAPACITY, "the trace writes " + std::to_string(need) + " bytes, dst_cap is " + std::to_string(cap));
+    if (t->samples_cap < job.samples.size())
+        return fail(BGR_ERR_CAPACITY, "the replay takes " + std::to_string(job.samples.size()) + " trace samples, samples_cap is " +
+                                          std::to_string(t->samples_cap));
+    if (!job.samples.empty() && !t->samples) return fail(BGR_ERR_INVALID_ARGUMENT, "null sample index");
+    return BGR_OK;
+}
+
+// Samples [q0, q0 + m) of a launch whose kernel covered the rows below `cover`: the traced rows at or past it exist at none
+// of them, so their records (row, state 0, zero words) are written here
+void trace_fill_rows(const ReplayJob& job, uint32_t q0, uint32_t m, uint32_t cover) {
+    const struct bgr_trace* t = job.tr;
+    const uint32_t end = t->first_row + t->n_rows, rb = trace_record_bytes(job.tp);
+    for (uint32_t q = q0; q < q0 + m; ++q)
+        for (uint32_t row = std::max(t->first_row, cover); row < end; ++row) {
+            uint8_t* rec = static_cast<uint8_t*>(t->dst) + trace_record_offset(q, row - t->first_row, t->n_rows, rb);
+            std::memset(rec, 0, rb);
+            std::memcpy(rec, &row, sizeof row);
+        }
+}
+
+// The records of the job's next sample from image 0 as it stands, straight to dst (the chunked replay, at a sample frame)
+int trace_gather(ReplayJob& job, DeviceBuffer<uint8_t>& stage) {
+    bgr_engine* e = job.e;
+    const struct bgr_trace* t = job.tr;
+    int rc = materialize_live(e);
+    if (rc != BGR_OK) return rc;
+    const size_t tab = align16(sizeof(TraceGather));
+    CUDA_TRY(stage.ensure(tab + job.tr_stride));
+    const TraceGather g{e->image(0), reinterpret_cast<uint32_t*>(stage.get() + tab), e->st.n_rows, t->first_row, t->n_rows, 0u};
+    CUDA_TRY(cudaMemcpyAsync(stage.get(), &g, sizeof g, cudaMemcpyHostToDevice, e->stream));
+    k_trace_gather<<<(t->n_rows + 255u) / 256u, 256, 0, e->stream>>>(job.tp, reinterpret_cast<const TraceGather*>(stage.get()), 1u, t->n_rows);
+    e->launches += 1;
+    CUDA_TRY(cudaGetLastError());
+    e->tiledep_chain = false;
+    uint8_t* dst = static_cast<uint8_t*>(t->dst) + size_t(job.tr_done) * job.tr_stride;
+    CUDA_TRY(cudaMemcpyAsync(dst, stage.get() + tab, job.tr_stride, cudaMemcpyDeviceToHost, e->stream));
+    CUDA_TRY(cudaStreamSynchronize(e->stream));
+    job.tr_done += 1;
     return BGR_OK;
 }
 
@@ -3900,6 +3969,7 @@ int replay_chunked(ReplayJob& job) {
     ImageEncoder x;
     x.e = e;
     const std::vector<ReplayJob*> owner{&job};
+    DeviceBuffer<uint8_t> tr_stage;  // one sample's records: freed with the call
     for (uint32_t j = 0; j < n;) {
         if (first_kf(job, j, j + 1) == j) {  // a keyframe: image 0 as it stands before frame j, a chunk boundary
             int rc = materialize_live(e);
@@ -3908,8 +3978,12 @@ int replay_chunked(ReplayJob& job) {
             rc = keyframes_write(x, owner);
             if (rc != BGR_OK) return rc;
         }
+        if (first_tr(job, j, j + 1) == j) {  // a trace sample: likewise
+            const int rc = trace_gather(job, tr_stage);
+            if (rc != BGR_OK) return rc;
+        }
         uint32_t b = j, ops = 0, saves = 0, spawned = 0;
-        while (b < n && (b == j || first_kf(job, b, b + 1) != b)) {
+        while (b < n && (b == j || (first_kf(job, b, b + 1) != b && first_tr(job, b, b + 1) != b))) {
             const uint32_t pt = (k && (int64_t(job.c.f0) + b) % k == 0) ? 1u : 0u;
             const uint32_t sp = prefix_at(job, b + 1) != prefix_at(job, b) ? job.c.rate : 0u;
             if (ops + pt + 1 > uint32_t(kMaxOps) || saves + pt > uint32_t(kMaxSaves) || spawned + sp > kMaxSpawnVals) break;
@@ -4001,13 +4075,16 @@ const JitKernel* replay_kernel(bgr_engine* e, uint32_t tiles) {
 // intervals), and its checksum points come back with one copy.  Replays with keyframes (every job has them, or none)
 // run k_generic_jit_replay_kf, whose launches also end where the keyframe images staged would pass the keyframe budget
 // (at least one keyframe of each unfinished world per launch); the image-table encoder then turns all of a launch's
-// keyframe images into blobs.  Synchronous.
+// keyframe images into blobs.  Replays with traces (every job has one, with one field list, or none) run
+// k_generic_jit_replay_trace, whose launches likewise end where the records staged would pass the trace budget; a
+// launch's records come back with one copy, straight into dst for one world, else through host memory.  Synchronous.
 int replay_launch(const JitKernel& k, const std::vector<ReplayJob*>& jobs, uint32_t kernel_bits) {
     bgr_engine* e0 = jobs[0]->e;
     cudaStream_t stream = e0->stream;
-    const bool kf = jobs[0]->kf != nullptr;
+    const bool kf = jobs[0]->kf != nullptr, tr = jobs[0]->tr != nullptr;
     const size_t world_bytes = align16(sizeof(ReplayWorld) * jobs.size());
-    const size_t rec_bytes = world_bytes + (kf ? align16(sizeof(ReplayKeyframes) * jobs.size()) : 0u);
+    const size_t rec_bytes = world_bytes + (kf ? align16(sizeof(ReplayKeyframes) * jobs.size()) : 0u) +
+                             (tr ? align16(sizeof(ReplayTrace) * jobs.size()) : 0u);
     std::vector<size_t> in_off(jobs.size()), pre_off(jobs.size()), val_off(jobs.size());
     size_t bytes = rec_bytes;
     for (size_t i = 0; i < jobs.size(); ++i) {
@@ -4037,6 +4114,7 @@ int replay_launch(const JitKernel& k, const std::vector<ReplayJob*>& jobs, uint3
     std::vector<uint32_t> cur(jobs.size(), 0u), seg_end(jobs.size()), seg_points(jobs.size());
     std::vector<ReplayWorld> recs;
     std::vector<ReplayKeyframes> kf_recs;
+    std::vector<ReplayTrace> tr_recs;
     std::vector<size_t> rec_job, acc_off;
     std::vector<unsigned long long> acc;
     std::vector<uint8_t> h_recs(rec_bytes);
@@ -4044,13 +4122,17 @@ int replay_launch(const JitKernel& k, const std::vector<ReplayJob*>& jobs, uint3
     x.e = e0;
     std::vector<ReplayJob*> owner;
     DeviceBuffer<uint8_t> kf_stage;  // the keyframe images of a launch: up to the keyframe budget, freed with the call
+    DeviceBuffer<uint8_t> tr_stage;  // the trace records of a launch: up to the trace budget, freed with the call
+    std::vector<uint8_t> h_tr;       // ... on the host, when they belong to several worlds
+    const TraceMap tr_map = tr ? trace_map(jobs[0]->tp) : TraceMap{};
     for (;;) {
-        recs.clear(); kf_recs.clear(); rec_job.clear(); acc_off.clear();
+        recs.clear(); kf_recs.clear(); tr_recs.clear(); rec_job.clear(); acc_off.clear();
         uint32_t active = 0;
         for (size_t i = 0; i < jobs.size(); ++i) active += cur[i] < jobs[i]->r->n_frames ? 1u : 0u;
         if (!active) break;
         const uint32_t budget = std::max(1u, e0->tune_replay_points / active);
         const uint64_t kf_budget = std::max<uint64_t>(1, e0->tune_keyframe_bytes / active);
+        const uint64_t tr_budget = std::max<uint64_t>(1, e0->tune_trace_bytes / active);
         uint32_t items = 0;
         size_t points = 0, staged = 0;
         for (size_t i = 0; i < jobs.size(); ++i) {
@@ -4067,6 +4149,7 @@ int replay_launch(const JitKernel& k, const std::vector<ReplayJob*>& jobs, uint3
                 const uint64_t fk = first_kf(job, a, n), m = std::max<uint64_t>(1, kf_budget / stride), kint = job.kf->interval;
                 if (fk != ~0ULL && fk + m * kint < b) b = uint32_t(fk + m * kint);  // m keyframes
             }
+            if (tr) b = trace_launch_end(job.c.f0, job.tr->interval, a, b, tr_budget, job.tr_stride);
             seg_end[i] = b;
             seg_points[i] = points_in(job, a, b);
             ReplayWorld w;
@@ -4099,26 +4182,67 @@ int replay_launch(const JitKernel& k, const std::vector<ReplayJob*>& jobs, uint3
                 staged += size_t(kfs_in(job, a, b)) * stride;
                 kf_recs.push_back(r);
             }
+            if (tr) {
+                ReplayTrace r;
+                std::memset(&r, 0, sizeof r);
+                r.staging = reinterpret_cast<uint8_t*>(staged);  // an offset until the staging is sized (below)
+                r.stride = job.tr_stride;
+                r.first = first_tr(job, a, b);
+                r.interval = job.tr->interval;
+                r.first_row = job.tr->first_row;
+                r.n_rows = job.tr->n_rows;
+                staged += size_t(trs_in(job, a, b)) * job.tr_stride;
+                tr_recs.push_back(r);
+            }
         }
         if (kf) {
             CUDA_TRY(kf_stage.ensure(std::max<size_t>(1, staged)));
             for (ReplayKeyframes& r : kf_recs) r.staging = kf_stage.get() + reinterpret_cast<size_t>(r.staging);
+        }
+        if (tr) {
+            CUDA_TRY(tr_stage.ensure(std::max<size_t>(1, staged)));
+            for (ReplayTrace& r : tr_recs) r.staging = tr_stage.get() + reinterpret_cast<size_t>(r.staging);
         }
         CUDA_TRY(e0->replay_acc.ensure(std::max<size_t>(1, points) * kAccStride));
         for (size_t ri = 0; ri < recs.size(); ++ri) recs[ri].acc = e0->replay_acc.get() + acc_off[ri] * kAccStride;
         if (points) CUDA_TRY(cudaMemsetAsync(e0->replay_acc.get(), 0, points * kAccStride * sizeof(unsigned long long), stream));
         std::memcpy(h_recs.data(), recs.data(), sizeof(ReplayWorld) * recs.size());
         if (kf) std::memcpy(h_recs.data() + world_bytes, kf_recs.data(), sizeof(ReplayKeyframes) * kf_recs.size());
+        if (tr) std::memcpy(h_recs.data() + world_bytes, tr_recs.data(), sizeof(ReplayTrace) * tr_recs.size());
         CUDA_TRY(cudaMemcpyAsync(d, h_recs.data(), rec_bytes, cudaMemcpyHostToDevice, stream));
         const ReplayWorld* d_recs = reinterpret_cast<const ReplayWorld*>(d);
         const ReplayKeyframes* d_kfs = reinterpret_cast<const ReplayKeyframes*>(d + world_bytes);
+        const ReplayTrace* d_trs = reinterpret_cast<const ReplayTrace*>(d + world_bytes);
         uint32_t n_recs = uint32_t(recs.size());
         void* args[] = {&d_recs, &n_recs, &d_kfs};
-        CUDA_TRY(cudaLaunchKernel(kf ? k.replay_kf_fn : k.replay_fn, dim3(items), dim3(k.threads), args, 0, stream));
+        void* tr_args[] = {&d_recs, &n_recs, &d_trs, const_cast<TraceMap*>(&tr_map)};
+        CUDA_TRY(cudaLaunchKernel(tr ? k.replay_trace_fn : kf ? k.replay_kf_fn : k.replay_fn, dim3(items), dim3(k.threads),
+                                  tr ? tr_args : args, 0, stream));
         CUDA_TRY(cudaGetLastError());
         acc.resize(points * kAccStride);
         if (points) CUDA_TRY(cudaMemcpyAsync(acc.data(), e0->replay_acc.get(), points * kAccStride * sizeof(unsigned long long), cudaMemcpyDeviceToHost, stream));
+        const bool tr_direct = recs.size() == 1;  // one world's samples are contiguous in its dst
+        if (tr && staged) {
+            const ReplayJob& j0 = *jobs[rec_job[0]];
+            uint8_t* to = tr_direct ? static_cast<uint8_t*>(j0.tr->dst) + size_t(j0.tr_done) * j0.tr_stride : nullptr;
+            if (!tr_direct) {
+                h_tr.resize(staged);
+                to = h_tr.data();
+            }
+            CUDA_TRY(cudaMemcpyAsync(to, tr_stage.get(), staged, cudaMemcpyDeviceToHost, stream));
+        }
         CUDA_TRY(cudaStreamSynchronize(stream));
+        if (tr) {  // each world's samples to its dst, and the records of the rows the launch's tiles did not reach
+            for (size_t ri = 0; ri < recs.size(); ++ri) {
+                ReplayJob& job = *jobs[rec_job[ri]];
+                const uint32_t m = trs_in(job, cur[rec_job[ri]], seg_end[rec_job[ri]]);
+                if (!tr_direct && m)
+                    std::memcpy(static_cast<uint8_t*>(job.tr->dst) + size_t(job.tr_done) * job.tr_stride,
+                                h_tr.data() + size_t(tr_recs[ri].staging - tr_stage.get()), size_t(m) * job.tr_stride);
+                trace_fill_rows(job, job.tr_done, m, uint32_t(std::min<uint64_t>(uint64_t(recs[ri].n_tiles) * kTileRows, UINT32_MAX)));
+                job.tr_done += m;
+            }
+        }
         if (kf) {  // the launch's keyframe images, world by world in frame order, to blobs
             x.im.clear();
             owner.clear();
@@ -4195,7 +4319,7 @@ int replay_run(ReplayJob& job) {
     int rc = replay_grow(one);
     if (rc != BGR_OK || job.r->n_frames == 0) return rc;
     const JitKernel* k = replay_kernel(job.e, std::max(1u, job.e->tiles_for(uint32_t(job.rows_end))));
-    if (!k || (job.kf && !k->replay_kf_fn)) return replay_chunked(job);
+    if (!k || (job.kf && !k->replay_kf_fn) || (job.tr && !k->replay_trace_fn)) return replay_chunked(job);
     rc = replay_launch(*k, one, BGR_KERNEL_REPLAY);
     if (rc != BGR_OK) return rc;
     return replay_commit(job);
@@ -4249,12 +4373,37 @@ BGR_API int bgr_replay_keyframes(bgr_engine* e, const struct bgr_replay* r, cons
     return replay_results(job, checksums_out, cap, n_out);
 }
 
+BGR_API int bgr_replay_trace(bgr_engine* e, const struct bgr_replay* r, const struct bgr_trace* t,
+                             bgr_checksum* checksums_out, uint32_t cap, uint32_t* n_out, uint32_t* n_samples_out, size_t* bytes_out) {
+    if (n_out) *n_out = 0;
+    if (!t || !n_samples_out || !bytes_out) return fail(BGR_ERR_INVALID_ARGUMENT, "null argument");
+    *n_samples_out = 0;
+    *bytes_out = 0;
+    NvtxRange span("Replay");
+    ReplayJob job;
+    int rc = replay_plan(e, r, job, nullptr, t);
+    if (rc != BGR_OK) return rc;  // nothing executed, nothing changed
+    *n_samples_out = uint32_t(job.samples.size());
+    *bytes_out = job.samples.size() * job.tr_stride;
+    if (!t->dst) return BGR_OK;  // the query
+    rc = trace_caps(job);
+    if (rc != BGR_OK) {
+        *n_samples_out = 0;
+        *bytes_out = 0;
+        return rc;
+    }
+    std::copy(job.samples.begin(), job.samples.end(), t->samples);
+    rc = replay_run(job);
+    if (rc != BGR_OK) return rc;
+    return replay_results(job, checksums_out, cap, n_out);
+}
+
 namespace {
 
-// bgr_batch_replay, and with kfs (one per world) bgr_batch_replay_keyframes
+// bgr_batch_replay, with kfs (one per world) bgr_batch_replay_keyframes, with trs (one per world) bgr_batch_replay_trace
 int batch_replay(bgr_batch* b, const uint32_t* worlds, uint32_t n_worlds, const struct bgr_replay* replays,
-                 const struct bgr_keyframes* kfs, bgr_checksum* checksums_out, uint32_t cap, uint32_t* n_checksums_out,
-                 uint32_t* n_keyframes_out, int32_t* status_out) {
+                 const struct bgr_keyframes* kfs, const struct bgr_trace* trs, bgr_checksum* checksums_out, uint32_t cap,
+                 uint32_t* n_checksums_out, uint32_t* n_keyframes_out, uint32_t* n_samples_out, int32_t* status_out) {
     if (!b) return fail(BGR_ERR_INVALID_ARGUMENT, "null batch");
     if (n_worlds && (!worlds || !replays || !n_checksums_out || !status_out)) return fail(BGR_ERR_INVALID_ARGUMENT, "null argument");
     NvtxRange span("Replay");
@@ -4263,6 +4412,7 @@ int batch_replay(bgr_batch* b, const uint32_t* worlds, uint32_t n_worlds, const 
         status_out[i] = BGR_OK;
         n_checksums_out[i] = 0;
         if (n_keyframes_out) n_keyframes_out[i] = 0;
+        if (n_samples_out) n_samples_out[i] = 0;
     }
     auto world_fail = [&](uint32_t i, int status) {
         status_out[i] = status;
@@ -4277,10 +4427,15 @@ int batch_replay(bgr_batch* b, const uint32_t* worlds, uint32_t n_worlds, const 
             return world_fail(i, fail(BGR_ERR_INVALID_ARGUMENT, "no such world in a batch of " + std::to_string(b->engines.size())));
         if (b->listed[w] == b->calls) return world_fail(i, fail(BGR_ERR_INVALID_ARGUMENT, "listed twice in one call"));
         b->listed[w] = b->calls;
-        int rc = replay_plan(b->engines[w], &replays[i], jobs[i], kfs ? &kfs[i] : nullptr);
+        int rc = replay_plan(b->engines[w], &replays[i], jobs[i], kfs ? &kfs[i] : nullptr, trs ? &trs[i] : nullptr);
         if (rc == BGR_OK && kfs) rc = keyframe_caps(jobs[i]);
+        if (rc == BGR_OK && trs && i && !feed_same_fields(jobs[i].tp, jobs[0].tp))
+            rc = fail(BGR_ERR_INVALID_ARGUMENT, "its trace's fields differ from those of entry 0's trace (a call has one record layout)");
+        if (rc == BGR_OK && trs) rc = trace_caps(jobs[i]);
         if (rc != BGR_OK) return world_fail(i, rc);
     }
+    if (trs)  // every world is planned: the sample frames and row counts are known
+        for (uint32_t i = 0; i < n_worlds; ++i) std::copy(jobs[i].samples.begin(), jobs[i].samples.end(), trs[i].samples);
     int first = BGR_OK;
     std::string first_err;
     uint32_t out_off = 0;
@@ -4290,13 +4445,14 @@ int batch_replay(bgr_batch* b, const uint32_t* worlds, uint32_t n_worlds, const 
         if (rc == BGR_OK) rc = replay_results(jobs[i], out, out ? cap - out_off : 0u, &n);
         n_checksums_out[i] = n;
         if (n_keyframes_out) n_keyframes_out[i] = jobs[i].kf_done;
+        if (n_samples_out) n_samples_out[i] = jobs[i].tr_done;
         out_off += std::min(n, cap - std::min(out_off, cap));
         if (rc != BGR_OK) {
             world_fail(i, rc);
             if (first == BGR_OK) { first = rc; first_err = g_err; }
         }
     };
-    if (!b->k.replay_fn || (kfs && !b->k.replay_kf_fn)) {  // each world's own replay, in list order
+    if (!b->k.replay_fn || (kfs && !b->k.replay_kf_fn) || (trs && !b->k.replay_trace_fn)) {  // each world's own replay, in list order
         for (uint32_t i = 0; i < n_worlds; ++i) results(i, replay_run(jobs[i]));
         if (first != BGR_OK) g_err = first_err;
         return first;
@@ -4318,14 +4474,23 @@ int batch_replay(bgr_batch* b, const uint32_t* worlds, uint32_t n_worlds, const 
 
 BGR_API int bgr_batch_replay(bgr_batch* b, const uint32_t* worlds, uint32_t n_worlds, const struct bgr_replay* replays,
                              bgr_checksum* checksums_out, uint32_t cap, uint32_t* n_checksums_out, int32_t* status_out) {
-    return batch_replay(b, worlds, n_worlds, replays, nullptr, checksums_out, cap, n_checksums_out, nullptr, status_out);
+    return batch_replay(b, worlds, n_worlds, replays, nullptr, nullptr, checksums_out, cap, n_checksums_out, nullptr, nullptr, status_out);
 }
 
 BGR_API int bgr_batch_replay_keyframes(bgr_batch* b, const uint32_t* worlds, uint32_t n_worlds, const struct bgr_replay* replays,
                                        const struct bgr_keyframes* kfs, bgr_checksum* checksums_out, uint32_t cap,
                                        uint32_t* n_checksums_out, uint32_t* n_keyframes_out, int32_t* status_out) {
     if (n_worlds && (!kfs || !n_keyframes_out)) return fail(BGR_ERR_INVALID_ARGUMENT, "null argument");
-    return batch_replay(b, worlds, n_worlds, replays, kfs, checksums_out, cap, n_checksums_out, n_keyframes_out, status_out);
+    return batch_replay(b, worlds, n_worlds, replays, kfs, nullptr, checksums_out, cap, n_checksums_out, n_keyframes_out, nullptr,
+                        status_out);
+}
+
+BGR_API int bgr_batch_replay_trace(bgr_batch* b, const uint32_t* worlds, uint32_t n_worlds, const struct bgr_replay* replays,
+                                   const struct bgr_trace* traces, bgr_checksum* checksums_out, uint32_t cap,
+                                   uint32_t* n_checksums_out, uint32_t* n_samples_out, int32_t* status_out) {
+    if (n_worlds && (!traces || !n_samples_out)) return fail(BGR_ERR_INVALID_ARGUMENT, "null argument");
+    return batch_replay(b, worlds, n_worlds, replays, nullptr, traces, checksums_out, cap, n_checksums_out, nullptr, n_samples_out,
+                        status_out);
 }
 
 // ---- batched checkpoints: the checkpoints of many worlds saved or restored in one pass ----

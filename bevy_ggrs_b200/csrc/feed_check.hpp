@@ -12,6 +12,40 @@
 
 namespace bgr {
 
+// A registered column as a change feed's field list sees it: its word planes and its absent bit (0: not optional)
+struct FeedColumn {
+    uint32_t first_plane, words, absent;
+};
+
+// The field list of a change feed (bgr_feed_create) or a replay trace (bgr_replay_trace) checked and mapped onto the
+// image: each field's word plane, words, absent bit and record words, the mask bits its records' state is made of and the
+// record size.  `col_at(c)` gives column c of the n_cols registered.  BGR_OK, or the status with *err = why; p is then
+// unspecified.
+template <class ColAt>
+int feed_fields(uint32_t n_cols, ColAt col_at, uint32_t words, const bgr_feed_field* fields, uint32_t n_fields, FeedParams& p,
+                std::string* err) {
+    if (n_fields > BGR_MAX_FEED_FIELDS) { *err = "too many fields (BGR_MAX_FEED_FIELDS)"; return BGR_ERR_CAPACITY; }
+    if (n_fields && !fields) { *err = "null argument"; return BGR_ERR_INVALID_ARGUMENT; }
+    p.keep = 1u;
+    p.rep_words = 0;
+    for (uint32_t k = 0; k < n_fields; ++k) {
+        const bgr_feed_field& f = fields[k];
+        if (f.column >= n_cols) { *err = "unknown column"; return BGR_ERR_INVALID_ARGUMENT; }
+        const FeedColumn c = col_at(f.column);
+        if ((f.byte_offset & 3u) || (f.byte_len & 3u) || f.byte_len == 0 || uint64_t(f.byte_offset) + f.byte_len > uint64_t(c.words) * 4u) {
+            *err = "field range must be 4-byte aligned and inside the element";
+            return BGR_ERR_INVALID_ARGUMENT;
+        }
+        p.fields[k] = FeedField{c.first_plane + f.byte_offset / 4u, f.byte_len / 4u, c.absent, p.rep_words};
+        p.rep_words += f.byte_len / 4u;
+        p.keep |= c.absent;
+    }
+    p.n_fields = n_fields;
+    p.words = words;
+    p.record_words = 2u + p.rep_words;
+    return BGR_OK;
+}
+
 // A feed as the checks see it: its registration (the fields, mask bits and record size in `reg`) and whether a report
 // of it is in flight
 struct FeedView {

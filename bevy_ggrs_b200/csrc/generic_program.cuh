@@ -196,6 +196,35 @@ struct ReplayKeyframes {
 };
 static_assert(sizeof(ReplayKeyframes) == 32, "ReplayKeyframes layout (the engine and the NVRTC module must agree)");
 
+// The trace samples of one world's frames [j0, j1) (bgr_replay_trace), parallel to the ReplayWorld array and read only by
+// k_generic_jit_replay_trace: at frame first + q * interval < j1, before advancing that frame, the block writes the
+// record of each of its rows in [first_row, first_row + n_rows) to staging + q * stride + (row - first_row) * record bytes.
+struct ReplayTrace {
+    uint8_t* staging;
+    unsigned long long stride;     // bytes per sample: n_rows records
+    unsigned long long first;      // first sample frame >= j0 (>= j1: none)
+    uint32_t interval;
+    uint32_t first_row, n_rows;
+    uint32_t reserved;
+};
+static_assert(sizeof(ReplayTrace) == 40, "ReplayTrace layout (the engine and the NVRTC module must agree)");
+
+// Where a trace record's field words come from, built on the host from the change feed's field list and passed to
+// k_generic_jit_replay_trace by value: record word 2 + slot[s] for s in [word_first[j], word_first[j + 1]) is word plane j
+// (zero unless the row exists and word_absent[j], its column's absent bit, is clear).  A plane listed by several fields
+// has several slots.  The generated kernel takes rows of at most 24 words, so a record holds at most 8 * 24 field words.
+constexpr uint32_t kTraceMaxWords = 24;
+constexpr uint32_t kTraceMaxSlots = 8u * kTraceMaxWords;
+struct TraceMap {
+    uint32_t n_fields, record_words;       // record_words: 2 + the field words
+    uint8_t field_absent[8];               // field k's absent bit: state bit 1 + k
+    uint8_t word_absent[kTraceMaxWords];
+    uint8_t word_first[kTraceMaxWords + 1];
+    uint8_t slot[kTraceMaxSlots];
+    uint8_t pad[3];
+};
+static_assert(sizeof(TraceMap) == 260, "TraceMap layout (the engine and the NVRTC module must agree)");
+
 // seahash of bytes [off, off+len) of one row's element whose words are `col[w * kTileRows]` (a column of the shared tile)
 // (__noinline__: inlined per checksummed column and per row the interpreter grew to 11k instructions — 176 KB of code,
 // more than the SM's instruction cache — and ran 2.7x slower per frame than the specialised bundle kernel)

@@ -102,7 +102,7 @@ __device__ __forceinline__ void jit_hash_columns(const JitRows& r, unsigned int*
 
 // A work item's rows: which tile and which rows of it the thread owns.  load / store move the register copy from / to an
 // image; advance and checksum are the one definition of what an ADVANCE and a SAVE do on the generated kernel, which
-// k_generic_jit, k_generic_jit_batch and k_generic_jit_replay all run.
+// k_generic_jit, k_generic_jit_batch and the replay entry points all run.
 struct JitItem {
     static constexpr int B = kJitItemRows / kJitRows;  // threads per work item
     static constexpr uint32_t kTileBytes = kTileRows * (4u * kJitWords + 1u);
@@ -329,13 +329,42 @@ extern "C" __global__ void __launch_bounds__(BGR_JIT_ITEM_ROWS / BGR_JIT_ROWS, B
 // shared accumulators; a full window (and the last one) is folded into the world's acc[point][kAccStride] with one
 // global atomic per non-zero word.  No barrier runs on frames that are neither checksum points nor chunk starts.
 // k_generic_jit_replay_kf also stores the registers at each keyframe frame into the world's keyframe staging (one plain
-// store per row and word, no barrier, no extra read); both entry points are this one body, KF selecting the stores.
+// store per row and word, no barrier, no extra read); k_generic_jit_replay_trace writes the change-feed record of each
+// traced row at each trace sample frame, from the registers too.  The three entry points are this one body, STORES
+// selecting the stores.
 constexpr uint32_t kReplayChunk = 256;  // frames of the log per staging step
 constexpr uint32_t kReplayWindow = 32;  // checksum points per shared window
+enum ReplayStores : int { kReplayPlain = 0, kReplayKeyframes = 1, kReplayTraces = 2 };
 
-template <bool KF>
+// The trace records of the thread's rows in [first_row, first_row + n_rows) into one sample's staging `img`: u32 row,
+// u32 state (bit 0 the row exists, bit 1 + k field k is present), then the field words, zero where not present.  The
+// words come from the register copy; the plane of each is a literal (the loop over kJitWords is unrolled) and the run-time
+// map only says which record words it goes to, so the rows stay in registers.
+__device__ __forceinline__ void jit_trace_store(const JitRows& r, const JitItem& it, uint8_t* img, uint32_t first_row,
+                                                uint32_t n_rows, const TraceMap& map) {
+#pragma unroll
+    for (int k = 0; k < kJitRows; ++k) {
+        const uint32_t row = it.tile * kTileRows + it.sub_row0 + uint32_t(k * JitItem::B);
+        const uint32_t i = row - first_row;
+        if (i >= n_rows) continue;
+        uint32_t* rec = reinterpret_cast<uint32_t*>(img) + size_t(i) * map.record_words;
+        const uint32_t m = r.m[k];
+        uint32_t state = m & 1u;
+        for (uint32_t f = 0; f < map.n_fields; ++f) state |= row_matches(m, map.field_absent[f]) ? 2u << f : 0u;
+        rec[0] = row;
+        rec[1] = state;
+#pragma unroll
+        for (int j = 0; j < kJitWords; ++j) {
+            const uint32_t v = row_matches(m, map.word_absent[j]) ? r.w[k][j] : 0u;
+            for (uint32_t s = map.word_first[j]; s < map.word_first[j + 1]; ++s) rec[2u + map.slot[s]] = v;
+        }
+    }
+}
+
+template <int STORES>
 __device__ __forceinline__ void jit_replay(const ReplayWorld* __restrict__ worlds, uint32_t n_worlds,
-                                           const ReplayKeyframes* __restrict__ kfs) {
+                                           const ReplayKeyframes* __restrict__ kfs, const ReplayTrace* __restrict__ trs,
+                                           const TraceMap* map) {
     constexpr int B = kJitItemRows / kJitRows;
     __shared__ unsigned int s_acc[kReplayWindow * kAccStride * 2];
     __shared__ uint8_t s_in[kReplayChunk * 8];
@@ -363,7 +392,17 @@ __device__ __forceinline__ void jit_replay(const ReplayWorld* __restrict__ world
     uint32_t point = 0, win0 = 0;  // checksum points seen, first point of the shared window
     unsigned long long next_kf = ~0ULL;
     uint8_t* kf_img = nullptr;
-    if constexpr (KF) { next_kf = kfs[lo].first; kf_img = kfs[lo].staging; }
+    if constexpr (STORES == kReplayKeyframes) { next_kf = kfs[lo].first; kf_img = kfs[lo].staging; }
+    unsigned long long next_tr = ~0ULL;
+    uint8_t* tr_img = nullptr;
+    bool tr_rows = false;  // the work item holds a traced row: uniform over the block
+    if constexpr (STORES == kReplayTraces) {
+        next_tr = trs[lo].first;
+        tr_img = trs[lo].staging;
+        const uint32_t item = blockIdx.x - w.item0;
+        const uint32_t r0 = (item / uint32_t(kJitSubs)) * kTileRows + (item % uint32_t(kJitSubs)) * uint32_t(kJitItemRows);
+        tr_rows = r0 < trs[lo].first_row + trs[lo].n_rows && trs[lo].first_row < r0 + uint32_t(kJitItemRows);
+    }
     auto flush = [&](uint32_t n) {
         __syncthreads();
         jit_fold_acc(w.acc + size_t(win0) * kAccStride, s_acc, n, tid);
@@ -387,11 +426,18 @@ __device__ __forceinline__ void jit_replay(const ReplayWorld* __restrict__ world
             point += 1;
             next_point += interval;
         }
-        if constexpr (KF) {
+        if constexpr (STORES == kReplayKeyframes) {
             if (j == next_kf) {  // keyframe f0 + j: the registers as they stand before the frame is advanced
                 it.store(r, kf_img);
                 kf_img += kfs[lo].stride;
                 next_kf += kfs[lo].interval;
+            }
+        }
+        if constexpr (STORES == kReplayTraces) {
+            if (j == next_tr) {  // trace sample f0 + j: the traced rows as they stand before the frame is advanced
+                if (tr_rows) jit_trace_store(r, it, tr_img, trs[lo].first_row, trs[lo].n_rows, *map);
+                tr_img += trs[lo].stride;
+                next_tr += trs[lo].interval;
             }
         }
         Op& op = s_op[tid];  // the thread's own copy: box_move indexes its inputs by row, which would put a local one on the stack
@@ -404,13 +450,21 @@ __device__ __forceinline__ void jit_replay(const ReplayWorld* __restrict__ world
 
 extern "C" __global__ void __launch_bounds__(BGR_JIT_ITEM_ROWS / BGR_JIT_ROWS, BGR_JIT_MINB)
     k_generic_jit_replay(const ReplayWorld* __restrict__ worlds, uint32_t n_worlds) {
-    jit_replay<false>(worlds, n_worlds, nullptr);
+    jit_replay<kReplayPlain>(worlds, n_worlds, nullptr, nullptr, nullptr);
 }
 
 // bgr_replay_keyframes, bgr_batch_replay_keyframes: kfs[i] belongs to worlds[i]
 extern "C" __global__ void __launch_bounds__(BGR_JIT_ITEM_ROWS / BGR_JIT_ROWS, BGR_JIT_MINB)
     k_generic_jit_replay_kf(const ReplayWorld* __restrict__ worlds, uint32_t n_worlds, const ReplayKeyframes* __restrict__ kfs) {
-    jit_replay<true>(worlds, n_worlds, kfs);
+    jit_replay<kReplayKeyframes>(worlds, n_worlds, kfs, nullptr, nullptr);
+}
+
+// bgr_replay_trace, bgr_batch_replay_trace: trs[i] belongs to worlds[i]; one field map for the launch (a batched call
+// has one field list)
+extern "C" __global__ void __launch_bounds__(BGR_JIT_ITEM_ROWS / BGR_JIT_ROWS, BGR_JIT_MINB)
+    k_generic_jit_replay_trace(const ReplayWorld* __restrict__ worlds, uint32_t n_worlds, const ReplayTrace* __restrict__ trs,
+                               const __grid_constant__ TraceMap map) {
+    jit_replay<kReplayTraces>(worlds, n_worlds, nullptr, trs, &map);
 }
 
 }  // namespace bgr

@@ -29,6 +29,7 @@ struct JitKernel {
     const void* batch_fn = nullptr;  // k_generic_jit_batch of the same module (world batches)
     const void* replay_fn = nullptr; // k_generic_jit_replay of the same module (replays)
     const void* replay_kf_fn = nullptr; // k_generic_jit_replay_kf of the same module (replays with keyframes)
+    const void* replay_trace_fn = nullptr; // k_generic_jit_replay_trace of the same module (replays with traces)
     int threads = 0;
     int item_rows = 0;         // rows per work item (set by the caller)
     int bps = 0;               // resident blocks per SM (occupancy query)
@@ -99,7 +100,7 @@ inline Cache& cache() { static Cache c; return c; }
 }  // namespace jit_detail
 
 // Compile (or fetch) the specialised kernel for `prelude` (the generated #defines): the entry points of the module,
-// k_generic_jit, k_generic_jit_batch, k_generic_jit_replay and k_generic_jit_replay_kf.  Returns false and leaves the reason in *why when the interpreter has to be used.
+// k_generic_jit, k_generic_jit_batch, k_generic_jit_replay, k_generic_jit_replay_kf and k_generic_jit_replay_trace.  Returns false and leaves the reason in *why when the interpreter has to be used.
 inline bool jit_generic_program(const std::string& prelude, int threads, const void* any_symbol_of_this_library, JitKernel* out,
                                 std::string* why) {
     using namespace jit_detail;
@@ -166,6 +167,10 @@ inline bool jit_generic_program(const std::string& prelude, int threads, const v
     else (void)cudaGetLastError();
     cudaKernel_t replay_kf = nullptr;
     if (cudaLibraryGetKernel(&replay_kf, lib, "k_generic_jit_replay_kf") == cudaSuccess) k.replay_kf_fn = reinterpret_cast<const void*>(replay_kf);
+    else (void)cudaGetLastError();
+    cudaKernel_t replay_trace = nullptr;
+    if (cudaLibraryGetKernel(&replay_trace, lib, "k_generic_jit_replay_trace") == cudaSuccess)
+        k.replay_trace_fn = reinterpret_cast<const void*>(replay_trace);
     else (void)cudaGetLastError();
     k.threads = threads;
     int nb = 0;

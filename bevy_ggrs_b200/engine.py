@@ -466,6 +466,28 @@ class Engine:
                                                    C.byref(size)))
         return _checksum_list(out, 0, n.value), _keyframe_list(buf, index, n_kf.value)
 
+    def replay_trace(self, inputs: np.ndarray, checksum_interval: int, trace_interval: int,
+                     fields: Sequence[Tuple[int, int, int]], first_row: int,
+                     n_rows: int) -> Tuple[List[Tuple[int, int]], List[Tuple[int, int]], np.ndarray]:
+        """``replay`` that also samples rows [first_row, first_row + n_rows) at every frame f = f0 + j, j < n, with
+        f % trace_interval == 0, before frame f is advanced: (checksums, [(frame, rows), ...], records).  ``records`` is a
+        uint8 array [n_samples, n_rows, record_bytes] of change-feed records over ``fields`` = [(column, byte_offset,
+        byte_len), ...] (``feed_record_dtype(fields)`` views one); rows that do not exist are state 0 with zero bytes.
+        Buffers are sized by the call's query (dst NULL), which runs nothing.  A non-finite value at a checksum frame
+        raises BgrError(BGR_ERR_NON_FINITE) after the whole log ran, with every sample written."""
+        log = _replay_log(inputs)
+        r = capi.bgr_replay(log.shape[0], log.shape[1], checksum_interval, 0, log.ctypes.data if log.size else None)
+        fa = _feed_fields(fields)
+        t = capi.bgr_trace(trace_interval, first_row, n_rows, len(fields), fa, None, 0, None, 0, 0)
+        n_s, size, n = C.c_uint32(), C.c_size_t(), C.c_uint32()
+        self._check(self._lib.bgr_replay_trace(self._h, C.byref(r), C.byref(t), None, 0, C.byref(n), C.byref(n_s), C.byref(size)))
+        records, samples = _trace_buffers(t, n_s.value, size.value, n_rows, _record_bytes(fields))
+        cap = _replay_points(self.rollback_frame_count(), log.shape[0], checksum_interval)
+        out = (capi.bgr_checksum * max(1, cap))()
+        self._check(self._lib.bgr_replay_trace(self._h, C.byref(r), C.byref(t), out, cap, C.byref(n), C.byref(n_s),
+                                               C.byref(size)))
+        return _checksum_list(out, 0, n.value), _sample_list(samples, n_s.value), records
+
     def submit_requests(self, session_info: Sequence[int], requests) -> None:
         reqs = list(requests)
         arr = capi.make_requests(reqs)
@@ -689,6 +711,45 @@ class EngineBatch:
             k += n_cs[i]
         return res
 
+    def replay_trace(self, calls, fields: Sequence[Tuple[int, int, int]]):
+        """``calls`` = [(world, inputs, checksum_interval, trace_interval, first_row, n_rows), ...]: Engine.replay_trace of
+        every listed world over one field list in one synchronous call (one launch per trace budget when the batch is
+        specialised).  Returns [(status, checksums, [(frame, rows), ...], records), ...] in the same order.  Each world's
+        buffers are sized by its own engine's query; a call refused before anything executed raises BgrError and changes
+        no world."""
+        calls = [(w, _replay_log(x), k, tt, a, nr) for w, x, k, tt, a, nr in calls]
+        n = len(calls)
+        fa = _feed_fields(fields)
+        worlds = (C.c_uint32 * max(1, n))(*[c[0] for c in calls])
+        reps = (capi.bgr_replay * max(1, n))(*[capi.bgr_replay(x.shape[0], x.shape[1], k, 0, x.ctypes.data if x.size else None)
+                                               for _, x, k, _, _, _ in calls])
+        trs = (capi.bgr_trace * max(1, n))()
+        bufs = []
+        cap = 0
+        for i, (w, x, k, tt, a, nr) in enumerate(calls):
+            trs[i] = capi.bgr_trace(tt, a, nr, len(fields), fa, None, 0, None, 0, 0)
+            records, samples = np.zeros((0, nr, _record_bytes(fields)), np.uint8), None
+            if 0 <= w < len(self.engines):
+                q = capi.bgr_trace(tt, a, nr, len(fields), fa, None, 0, None, 0, 0)
+                n_s, size, n_cs = C.c_uint32(), C.c_size_t(), C.c_uint32()
+                if self._lib.bgr_replay_trace(self.engines[w]._h, C.byref(reps[i]), C.byref(q), None, 0, C.byref(n_cs),
+                                              C.byref(n_s), C.byref(size)) == capi.BGR_OK:
+                    records, samples = _trace_buffers(trs[i], n_s.value, size.value, nr, _record_bytes(fields))
+                cap += _replay_points(self.engines[w].rollback_frame_count(), x.shape[0], k)
+            bufs.append((records, samples))
+        out = (capi.bgr_checksum * max(1, cap))()
+        n_cs = (C.c_uint32 * max(1, n))()
+        n_s = (C.c_uint32 * max(1, n))()
+        status = (C.c_int32 * max(1, n))()
+        rc = self._lib.bgr_batch_replay_trace(self._h, worlds, n, reps, trs, out, cap, n_cs, n_s, status)
+        if rc not in (capi.BGR_OK, capi.BGR_ERR_NON_FINITE):
+            self._check(rc)
+        res, k = [], 0
+        for i in range(n):
+            res.append((status[i], _checksum_list(out, k, k + n_cs[i]), _sample_list(bufs[i][1], n_s[i]), bufs[i][0]))
+            k += n_cs[i]
+        return res
+
     def checkpoint(self, calls) -> List[Optional[bytes]]:
         """``calls`` = [(world, frame), ...]: Engine.checkpoint of every listed world in one call (one encoding pass and
         one copy back).  Returns the blobs in the same order, None where the world holds that frame neither queued
@@ -802,6 +863,33 @@ def _keyframe_buffers(kf: "capi.bgr_keyframes", n_kf: int, size: int):
 
 def _keyframe_list(buf, index, n: int) -> List[Tuple[int, bytes]]:
     return [(index[i].frame, buf[index[i].offset: index[i].offset + index[i].bytes].tobytes()) for i in range(n)]
+
+
+def _feed_fields(fields) -> "C.Array[capi.bgr_feed_field]":
+    fields = [tuple(int(x) for x in f) for f in fields]
+    return (capi.bgr_feed_field * max(1, len(fields)))(*[capi.bgr_feed_field(*f) for f in fields])
+
+
+def _trace_buffers(t: "capi.bgr_trace", n_samples: int, size: int, n_rows: int, rb: int):
+    """Records [n_samples, n_rows, rb] (uint8) and a sample index of n_samples entries, installed in `t`; the arrays must
+    outlive the call."""
+    buf = np.zeros(max(1, size), np.uint8)   # never a null dst, which would be a query: a log may take no sample
+    records = buf[:size].reshape(n_samples, n_rows, rb)
+    samples = (capi.bgr_trace_sample * max(1, n_samples))()
+    t.dst, t.dst_cap, t.samples, t.samples_cap = buf.ctypes.data, size, samples, n_samples
+    return records, samples
+
+
+def _record_bytes(fields) -> int:
+    return 8 + sum(int(ln) for _, _, ln in fields)
+
+
+def _sample_list(samples, n: int) -> List[Tuple[int, int]]:
+    """[(frame, rows)] of the first n bgr_trace_sample entries, through numpy: a trace at T = 1 returns thousands."""
+    if not n:
+        return []
+    arr = np.ctypeslib.as_array(samples)[:n]
+    return list(zip(arr["frame"].tolist(), arr["rows"].tolist()))
 
 
 def _replay_log(inputs) -> np.ndarray:

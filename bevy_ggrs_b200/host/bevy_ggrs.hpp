@@ -525,6 +525,52 @@ public:
         return out;
     }
 
+    // replay() that also samples rows [first_row, first_row + n_rows) at every frame f with f % trace_interval == 0,
+    // before it is advanced (bgr_replay_trace; the engine's world only, as replay()).  `samples` gets each sample's
+    // (frame, row count) and `records` n_samples * n_rows change-feed records over `fields`, sample-major.  The buffers are
+    // sized by the call's query, which runs nothing.
+    std::vector<std::pair<ggrs::Frame, unsigned __int128>> replay_trace(
+        const std::vector<uint8_t>& inputs, uint32_t n_players, uint32_t checksum_interval, uint32_t trace_interval,
+        const std::vector<bgr_feed_field>& fields, uint32_t first_row, uint32_t n_rows, std::vector<bgr_trace_sample>* samples,
+        std::vector<uint8_t>* records) {
+        finish();
+        if (!res_order_.empty() || !host_cols_.empty())
+            throw Panic(BGR_ERR_UNSUPPORTED, "replay runs the engine's world only: the App has rollback resources or host-side components");
+        if (n_players ? inputs.size() % n_players != 0 : !inputs.empty())
+            throw Panic(BGR_ERR_INVALID_ARGUMENT, "the input log is not a whole number of frames of n_players bytes");
+        struct bgr_replay r;
+        std::memset(&r, 0, sizeof r);
+        r.n_players = n_players;
+        r.n_frames = n_players ? uint32_t(inputs.size() / n_players) : 0u;
+        r.checksum_interval = checksum_interval;
+        r.inputs = inputs.data();
+        struct bgr_trace t;
+        std::memset(&t, 0, sizeof t);
+        t.interval = trace_interval;
+        t.first_row = first_row;
+        t.n_rows = n_rows;
+        t.n_fields = uint32_t(fields.size());
+        t.fields = fields.data();
+        uint32_t got = 0, n_s = 0;
+        size_t bytes = 0;
+        check(bgr_replay_trace(engine_, &r, &t, nullptr, 0, &got, &n_s, &bytes));  // the query
+        records->assign(std::max<size_t>(bytes, 1), 0);  // never a null dst, which is the query: a log may take no sample
+        samples->assign(std::max<uint32_t>(n_s, 1), bgr_trace_sample{});
+        t.dst = records->data();
+        t.dst_cap = bytes;
+        t.samples = samples->data();
+        t.samples_cap = n_s;
+        const int64_t f0 = rollback_frame_count(), n = r.n_frames, k = checksum_interval;
+        const size_t cap = k && f0 >= 0 ? size_t((f0 + n + k - 1) / k - (f0 + k - 1) / k) : 0u;
+        std::vector<bgr_checksum> cs(std::max<size_t>(cap, 1));
+        check(bgr_replay_trace(engine_, &r, &t, cs.data(), uint32_t(cap), &got, &n_s, &bytes));
+        records->resize(bytes);
+        samples->resize(n_s);
+        std::vector<std::pair<ggrs::Frame, unsigned __int128>> out;
+        for (uint32_t i = 0; i < got && i < cap; ++i) out.emplace_back(cs[i].frame, (static_cast<unsigned __int128>(cs[i].hi) << 64) | cs[i].lo);
+        return out;
+    }
+
     // Replaces the world and the App's resources with a checkpoint's.  The resource section is checked before the
     // engine restores, so a refused blob changes nothing.
     void restore_checkpoint(const std::vector<uint8_t>& blob) {

@@ -713,6 +713,58 @@ BGR_API int bgr_batch_replay_keyframes(bgr_batch* b, const uint32_t* worlds, uin
                                        const struct bgr_keyframes* kfs, bgr_checksum* checksums_out, uint32_t cap,
                                        uint32_t* n_checksums_out, uint32_t* n_keyframes_out, int32_t* status_out);
 
+/* ---- replay traces: chosen fields of a row range every T frames while a replay runs -------------------------------
+ * bgr_replay_trace is bgr_replay that also takes a sample at each frame f0 + j, j in [0, n), with (f0 + j) % interval == 0,
+ * before that frame is advanced (where a checksum point or a keyframe is taken), so trace(a) then trace(b) equals
+ * trace(a ++ b).  Everything else (checksums, live world, row count, RollbackFrameCount, Time, ParticleRng, the call
+ * counter, the ring, retained frames, witnesses, change feeds) ends exactly as after bgr_replay of the same log.  Replay
+ * viewers and match analytics read the entities they draw or mine at every frame without a host round trip per frame.
+ *   - Records: sample s, traced row i (row first_row + i) is one record at dst + (s * n_rows + i) * record_bytes, the change
+ *     feed's record of that row (bgr_feed_create's fields) in the live world at the sample frame: u32 row, u32 state (bit 0
+ *     the row exists, bit 1 + k it exists and field k's column is present), then the fields' bytes, zero where a field is
+ *     not present.  record_bytes = 8 + the sum of byte_len.  Rows that do not exist at the sample (at or past the row
+ *     count, or despawned) are written too, as state 0 with zero bytes, so the layout is dense and fixed.  samples[s] =
+ *     the sample's frame and RollbackOrdered::len() there.
+ *   - dst == NULL: nothing runs; *n_samples_out and *bytes_out = the exact sample count and bytes.  Otherwise a dst_cap or
+ *     samples_cap below them is BGR_ERR_CAPACITY before anything runs.
+ *   - Refusals change nothing: everything bgr_replay refuses; interval == 0, n_rows == 0 or reserved != 0
+ *     (BGR_ERR_INVALID_ARGUMENT); a field list bgr_feed_create would refuse, with its status; first_row + n_rows past the
+ *     engine's max_entities, or past its ceiling for BGR_CFG_GROWABLE (BGR_ERR_INVALID_ARGUMENT).
+ *   - A non-finite finite-asserted value at a checksum frame is BGR_ERR_NON_FINITE after the whole log ran, with every
+ *     sample written.
+ * On the generated kernel (k_generic_jit_replay_trace, bgr_last_kernel carries BGR_KERNEL_REPLAY) each thread writes its
+ * traced rows' records from its registers at each sample frame into device staging, whose size ends a launch early
+ * (BGR_TUNE_TRACE_BYTES, 256 MB by default, split over the unfinished worlds, always at least one sample per world); each
+ * launch's records come back with one copy.  The staging is allocated and freed inside the call.  Without a generated
+ * kernel the replay runs in chunks that end at each sample frame, whose records k_trace_gather writes from the live image:
+ * the same bytes, slower. */
+typedef struct bgr_trace_sample {  /* 8 bytes */
+    int32_t frame;
+    uint32_t rows;                 /* RollbackOrdered::len() at frame */
+} bgr_trace_sample;
+struct bgr_trace {                 /* 56 bytes */
+    uint32_t interval;             /* T >= 1 */
+    uint32_t first_row, n_rows;    /* the traced rows [first_row, first_row + n_rows), n_rows >= 1 */
+    uint32_t n_fields;             /* 0 .. BGR_MAX_FEED_FIELDS */
+    const bgr_feed_field* fields;  /* the change feed's field type and rules */
+    void* dst;                     /* NULL: query only */
+    size_t dst_cap;
+    bgr_trace_sample* samples;     /* [samples_cap] */
+    uint32_t samples_cap;
+    uint32_t reserved;             /* 0 */
+};
+BGR_API int bgr_replay_trace(bgr_engine* e, const struct bgr_replay* r, const struct bgr_trace* t,
+                             bgr_checksum* checksums_out, uint32_t cap, uint32_t* n_out,
+                             uint32_t* n_samples_out, size_t* bytes_out);
+/* bgr_batch_replay with traces: traces[i] holds world i's interval, row range and buffers, in bgr_replay_trace's
+ * conventions (a null dst is refused with BGR_ERR_CAPACITY unless the world takes no sample; query a member's sizes with
+ * bgr_replay_trace on its engine).  Row ranges and intervals may differ between worlds; the field list must equal entry
+ * 0's (BGR_ERR_INVALID_ARGUMENT otherwise), so a launch has one record layout.  Every listed world is validated, planned
+ * and its capacities checked first; n_samples_out[i] is world i's sample count. */
+BGR_API int bgr_batch_replay_trace(bgr_batch* b, const uint32_t* worlds, uint32_t n_worlds, const struct bgr_replay* replays,
+                                   const struct bgr_trace* traces, bgr_checksum* checksums_out, uint32_t cap,
+                                   uint32_t* n_checksums_out, uint32_t* n_samples_out, int32_t* status_out);
+
 /* ---- batched checkpoints: the world checkpoints of many batch members saved or restored in one pass ----------------
  * Both calls follow the conventions of bgr_batch_handle_requests: indices in range and distinct, every listed world
  * validated before anything executes anywhere, a refusal marks the failing world in status_out with bgr_last_error()

@@ -84,7 +84,7 @@ pub use checkpoint::*;
 // world batches: a safe owner of a bgr_batch
 mod batch;
 pub use batch::*;
-// replays: the bgr_replay record and safe calls over an input log, with and without keyframes
+// replays: the bgr_replay record and safe calls over an input log, with and without keyframes or a trace
 mod replay;
 pub use replay::*;
 
@@ -211,6 +211,8 @@ extern "C" {
     pub fn bgr_batch_replay(b: *mut bgr_batch, worlds: *const u32, n_worlds: u32, replays: *const bgr_replay, checksums_out: *mut bgr_checksum, cap: u32, n_checksums_out: *mut u32, status_out: *mut i32) -> c_int;
     pub fn bgr_replay_keyframes(e: *mut bgr_engine, r: *const bgr_replay, kf: *const bgr_keyframes, checksums_out: *mut bgr_checksum, cap: u32, n_out: *mut u32, n_keyframes_out: *mut u32, bytes_out: *mut usize) -> c_int;
     pub fn bgr_batch_replay_keyframes(b: *mut bgr_batch, worlds: *const u32, n_worlds: u32, replays: *const bgr_replay, kfs: *const bgr_keyframes, checksums_out: *mut bgr_checksum, cap: u32, n_checksums_out: *mut u32, n_keyframes_out: *mut u32, status_out: *mut i32) -> c_int;
+    pub fn bgr_replay_trace(e: *mut bgr_engine, r: *const bgr_replay, t: *const bgr_trace, checksums_out: *mut bgr_checksum, cap: u32, n_out: *mut u32, n_samples_out: *mut u32, bytes_out: *mut usize) -> c_int;
+    pub fn bgr_batch_replay_trace(b: *mut bgr_batch, worlds: *const u32, n_worlds: u32, replays: *const bgr_replay, traces: *const bgr_trace, checksums_out: *mut bgr_checksum, cap: u32, n_checksums_out: *mut u32, n_samples_out: *mut u32, status_out: *mut i32) -> c_int;
     pub fn bgr_batch_checkpoint_save(b: *mut bgr_batch, worlds: *const u32, n_worlds: u32, frames: *const i32, dst: *mut c_void, dst_cap: usize, index: *mut bgr_keyframe, bytes_out: *mut usize, status_out: *mut i32) -> c_int;
     pub fn bgr_batch_checkpoint_restore(b: *mut bgr_batch, worlds: *const u32, n_worlds: u32, blobs: *const *const c_void, bytes: *const usize, status_out: *mut i32) -> c_int;
     pub fn bgr_batch_feed_begin(b: *mut bgr_batch, reports: *const bgr_batch_feed, n_entries: u32, host_dst: *mut c_void, ticket_out: *mut u32, status_out: *mut i32) -> c_int;

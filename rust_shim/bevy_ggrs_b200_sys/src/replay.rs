@@ -1,7 +1,9 @@
 //! `#[repr(C)]` mirror of `struct bgr_replay` of `include/bevy_ggrs_b200.h` and safe calls over it (bgr_replay /
 //! bgr_batch_replay): a recorded input log run through a world, checksummed every `checksum_interval` frames, without
 //! pushing snapshots.  With keyframes (bgr_replay_keyframes / bgr_batch_replay_keyframes) the replay also returns a
-//! world checkpoint every `keyframe_interval` frames, the seek points of a recorded match.
+//! world checkpoint every `keyframe_interval` frames, the seek points of a recorded match.  With a trace
+//! (bgr_replay_trace / bgr_batch_replay_trace) it also returns the change-feed records of a row range every
+//! `interval` frames, what a replay viewer draws or a match-analytics job mines.
 
 use crate::*;
 use core::ptr;
@@ -200,6 +202,139 @@ impl Batch {
             let cs = out[at.min(cap)..end].to_vec();
             at += n_out[i] as usize;
             (status[i], cs, bufs[i].blobs(n_kf[i]))
+        }).collect())
+    }
+}
+
+/// One sample of a trace: its frame and RollbackOrdered::len() there.
+#[repr(C)]
+#[derive(Clone, Copy, Debug, Default, PartialEq, Eq)]
+pub struct bgr_trace_sample {
+    pub frame: i32,
+    pub rows: u32,
+}
+
+#[repr(C)]
+#[derive(Clone, Copy, Debug)]
+pub struct bgr_trace {
+    pub interval: u32,
+    pub first_row: u32,
+    pub n_rows: u32,
+    pub n_fields: u32,
+    pub fields: *const bgr_feed_field,
+    pub dst: *mut c_void,
+    pub dst_cap: usize,
+    pub samples: *mut bgr_trace_sample,
+    pub samples_cap: u32,
+    pub reserved: u32,
+}
+
+const _: () = assert!(core::mem::size_of::<bgr_trace_sample>() == 8);
+const _: () = assert!(core::mem::size_of::<bgr_trace>() == 56);
+
+/// What a trace records: every `interval` frames, rows [first_row, first_row + n_rows) as change-feed records over
+/// `fields`.
+pub struct TraceSpec<'a> {
+    pub interval: u32,
+    pub first_row: u32,
+    pub n_rows: u32,
+    pub fields: &'a [bgr_feed_field],
+}
+
+/// A replay's trace: the samples in frame order, and n_samples * n_rows records of `record_bytes` each, sample-major.
+pub struct Trace {
+    pub samples: Vec<bgr_trace_sample>,
+    pub records: Vec<u8>,
+}
+
+impl<'a> TraceSpec<'a> {
+    fn raw(&self, t: Option<&mut Trace>) -> bgr_trace {
+        let (dst, dst_cap, samples, samples_cap) = match t {
+            // never a null dst, which is the query: a log may take no sample
+            Some(t) => (t.records.as_mut_ptr() as *mut c_void, t.records.len() - 1, t.samples.as_mut_ptr(), t.samples.len() as u32 - 1),
+            None => (ptr::null_mut(), 0, ptr::null_mut(), 0),
+        };
+        bgr_trace {
+            interval: self.interval,
+            first_row: self.first_row,
+            n_rows: self.n_rows,
+            n_fields: self.fields.len() as u32,
+            fields: self.fields.as_ptr(),
+            dst,
+            dst_cap,
+            samples,
+            samples_cap,
+            reserved: 0,
+        }
+    }
+
+    /// Buffers sized by a query (dst NULL) of `r` on `e`, which runs nothing (one spare byte and sample each).
+    fn query(&self, e: *mut bgr_engine, r: &bgr_replay) -> Result<Trace, c_int> {
+        let q = self.raw(None);
+        let (mut n_cs, mut n_s, mut bytes) = (0u32, 0u32, 0usize);
+        let rc = unsafe { bgr_replay_trace(e, r, &q, ptr::null_mut(), 0, &mut n_cs, &mut n_s, &mut bytes) };
+        if rc != BGR_OK { return Err(rc); }
+        Ok(Trace { samples: vec![bgr_trace_sample::default(); n_s as usize + 1], records: vec![0u8; bytes + 1] })
+    }
+}
+
+impl Trace {
+    fn finish(mut self, n_samples: u32) -> Trace {
+        let n = (n_samples as usize).min(self.samples.len() - 1);
+        let per = if self.samples.len() > 1 { (self.records.len() - 1) / (self.samples.len() - 1) } else { 0 };
+        self.samples.truncate(n);
+        self.records.truncate(n * per);
+        self
+    }
+}
+
+/// `replay` that also returns a trace.  Err(status, checksums, trace): BGR_ERR_NON_FINITE after the whole log ran
+/// (every sample is written), or a refusal that changed nothing.
+pub fn replay_trace(e: *mut bgr_engine, log: &ReplayLog, spec: &TraceSpec)
+                    -> Result<(Vec<bgr_checksum>, Trace), (c_int, Vec<bgr_checksum>, Option<Trace>)> {
+    log.check().map_err(|rc| (rc, Vec::new(), None))?;
+    let mut f0 = 0i32;
+    unsafe { bgr_rollback_frame_count(e, &mut f0) };
+    let r = log.raw();
+    let mut trace = spec.query(e, &r).map_err(|rc| (rc, Vec::new(), None))?;
+    let t = spec.raw(Some(&mut trace));
+    let mut out = vec![bgr_checksum::default(); log.points(f0)];
+    let (mut n, mut n_s, mut bytes) = (0u32, 0u32, 0usize);
+    let rc = unsafe { bgr_replay_trace(e, &r, &t, out.as_mut_ptr(), out.len() as u32, &mut n, &mut n_s, &mut bytes) };
+    out.truncate((n as usize).min(out.len()));
+    let trace = trace.finish(n_s);
+    if rc == BGR_OK { Ok((out, trace)) } else { Err((rc, out, Some(trace))) }
+}
+
+impl Batch {
+    /// `replay_trace` of `logs[i]` on world `worlds[i]` with `specs[i]` (every spec with the same field list), in one
+    /// synchronous call.  `engines[i]` is world i's engine: its query sizes the world's buffers.  Err(status) when the
+    /// call was refused before anything executed; otherwise each world's status, checksums and trace, in order.
+    pub fn replay_trace(&mut self, worlds: &[u32], engines: &[*mut bgr_engine], f0s: &[i32], logs: &[ReplayLog],
+                        specs: &[TraceSpec]) -> Result<Vec<(c_int, Vec<bgr_checksum>, Trace)>, c_int> {
+        for l in logs { l.check()?; }
+        let reps: Vec<bgr_replay> = logs.iter().map(|l| l.raw()).collect();
+        let mut bufs = Vec::with_capacity(worlds.len());
+        for i in 0..worlds.len() { bufs.push(specs[i].query(engines[i], &reps[i])?); }
+        let trs: Vec<bgr_trace> = bufs.iter_mut().zip(specs.iter()).map(|(b, s)| s.raw(Some(b))).collect();
+        let cap: usize = logs.iter().zip(f0s.iter()).map(|(l, &f0)| l.points(f0)).sum();
+        let mut out = vec![bgr_checksum::default(); cap];
+        let mut n_out = vec![0u32; worlds.len()];
+        let mut n_s = vec![0u32; worlds.len()];
+        let mut status = vec![0i32; worlds.len()];
+        let rc = unsafe {
+            bgr_batch_replay_trace(self.raw, worlds.as_ptr(), worlds.len() as u32, reps.as_ptr(), trs.as_ptr(),
+                                   out.as_mut_ptr(), cap as u32, n_out.as_mut_ptr(), n_s.as_mut_ptr(), status.as_mut_ptr())
+        };
+        if rc != BGR_OK && rc != BGR_ERR_NON_FINITE {
+            return Err(rc);
+        }
+        let mut at = 0usize;
+        Ok(bufs.into_iter().enumerate().map(|(i, b)| {
+            let end = (at + n_out[i] as usize).min(cap);
+            let cs = out[at.min(cap)..end].to_vec();
+            at += n_out[i] as usize;
+            (status[i], cs, b.finish(n_s[i]))
         }).collect())
     }
 }
