@@ -71,6 +71,8 @@ BGR_KERNEL_HELD_SAVES = 1 << 27
 BGR_KERNEL_BATCHED = 1 << 28
 # ... and the last replay ran on the generated kernel's replay entry point (bgr_replay / bgr_batch_replay)
 BGR_KERNEL_REPLAY = 1 << 29
+# ... and the bundle launch reduced each Save's checksum partials over the warp: lane slots would have cost it a block
+BGR_KERNEL_WARP_FOLD = 1 << 30
 # replays
 BGR_MAX_REPLAY_FRAMES = 1 << 24
 # change feed

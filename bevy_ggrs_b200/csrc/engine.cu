@@ -416,7 +416,8 @@ struct bgr_engine {
     int tune_tma = 1;          // stepwise Save/Load through the TMA-staged bulk-copy kernel
     uint32_t tma_stage_tiles = 0;  // one-tile stages of the TMA copy kernel (0: schema too wide for two stages of shared memory)
     DeviceBuffer<unsigned int> tma_ticket;
-    int occ_cache[2][3][2][2] = {};  // [passive TMA][MODE][STAMPS][VERIFY]: blocks per SM of k_particles_program
+    // [WARP_FOLD][passive TMA][MODE][STAMPS][VERIFY][Saves in the vector]: blocks per SM of k_particles_program
+    int occ_cache[2][2][3][2][2][kMaxSaves + 1] = {};
     int snap_fits = -1;              // -1 unknown; 0: the stamp-point snapshot would cost the passive-TMA launches a block per SM
     // desync diff scratch (BGR_CFG_DESYNC_CAPTURE), allocated by the first bgr_desync_diff
     DeviceBuffer<DiffColumn> diff_cols;
@@ -671,22 +672,40 @@ void derive_content_ids(bgr_engine* e, HostState& s, Program& pg) {
 // ---------------------------------------------------------------------------------------------
 // launch: fused bundle kernel
 // ---------------------------------------------------------------------------------------------
-template <int MODE, bool STAMPS, bool VERIFY>
-int launch_particles(bgr_engine* e, const ProgramParams& pp) {
-    auto kern = k_particles_program<MODE, STAMPS, VERIFY>;
+// Every instance opts into the most dynamic shared memory any launch of it can ask for (a 96 KB passive double buffer,
+// the snapshot and 40 Saves' lane slots), so that no engine lowers the limit another engine's launches rely on.
+constexpr size_t kBundleSmemMax = 96u * 1024u + kSnapBytes + fold_bytes(false, kMaxSaves);
+
+// blocks per SM of one k_particles_program instance at `smem` bytes of dynamic shared memory
+template <int MODE, bool STAMPS, bool VERIFY, bool WARP_FOLD>
+int bundle_blocks_per_sm(size_t smem, int& nb) {
+    auto kern = k_particles_program<MODE, STAMPS, VERIFY, WARP_FOLD>;
+    CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, int(kBundleSmemMax)));
+    CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, kern, int(kTileRows) / 2, smem));
+    return BGR_OK;
+}
+
+// A mode runs with and without the passive double buffer (spawns and multi-Load vectors move passive planes per
+// thread), and the checksum partials grow with the vector's Saves: the occupancy is per (fold, buffer, mode, Saves).
+// passive_bytes is fixed at bgr_build, so one entry per setting is exact.  The stamped instances also hold the
+// stamp-point snapshot.
+template <int MODE, bool STAMPS, bool VERIFY, bool WARP_FOLD>
+int bundle_occupancy(bgr_engine* e, size_t base, uint32_t n_saves, int ti, int& nb) {
+    int& occ = e->occ_cache[WARP_FOLD ? 1 : 0][ti][MODE][STAMPS ? 1 : 0][VERIFY ? 1 : 0][n_saves];
+    if (occ == 0) {
+        int n = 0;
+        if (int rc = bundle_blocks_per_sm<MODE, STAMPS, VERIFY, WARP_FOLD>(base + fold_bytes(WARP_FOLD, n_saves), n); rc != BGR_OK) return rc;
+        occ = std::max(1, n);
+    }
+    nb = occ;
+    return BGR_OK;
+}
+
+template <int MODE, bool STAMPS, bool VERIFY, bool WARP_FOLD>
+int launch_bundle(bgr_engine* e, const ProgramParams& pp, size_t smem, int occ) {
+    auto kern = k_particles_program<MODE, STAMPS, VERIFY, WARP_FOLD>;
     constexpr int kBlock = int(kTileRows) / 2;  // two rows per thread
     const int ti = (pp.flags & PF_PASSIVE_TMA) ? 1 : 0;
-    const size_t smem = (ti ? size_t(2) * pp.passive_bytes : 0) + (STAMPS ? kSnapBytes : 0);
-    // A mode runs with and without the passive double buffer (spawns and multi-Load vectors move passive planes per
-    // thread): the shared-memory opt-in and the occupancy are per (mode, buffer).  passive_bytes is fixed at bgr_build,
-    // so one entry per buffer setting is exact.  The stamped instances also hold the stamp-point snapshot.
-    int& occ = e->occ_cache[ti][MODE][STAMPS ? 1 : 0][VERIFY ? 1 : 0];
-    if (occ == 0) {
-        if (smem > 48 * 1024) CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem)));
-        int nb = 0;
-        CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, kern, kBlock, smem));
-        occ = std::max(1, nb);
-    }
     int bps = occ;
     if (e->tune_bps > 0) bps = std::min(e->tune_bps, bps);
     uint32_t grid = std::max(1u, std::min(pp.n_tiles, uint32_t(e->num_sms * bps)));
@@ -705,23 +724,40 @@ int launch_particles(bgr_engine* e, const ProgramParams& pp) {
     const bool passive = pp.n_runs > 0 || pp.n_passive > 0;
     // VEC 2, launch-bounds tier 1 (768 threads per SM), whole-tile work items
     e->last_kernel = BGR_KERNEL_BUNDLE | (2u << 4) | (uint32_t(MODE) << 8) | (1u << 10) | (ti ? 1u << 12 : 0u) |
-                     (passive ? BGR_KERNEL_PASSIVE_PLANES : 0u) | (uint32_t(kTileRows) << 16) | (STAMPS ? BGR_KERNEL_STABLE_PLANES : 0u);
+                     (passive ? BGR_KERNEL_PASSIVE_PLANES : 0u) | (uint32_t(kTileRows) << 16) | (STAMPS ? BGR_KERNEL_STABLE_PLANES : 0u) |
+                     (WARP_FOLD ? BGR_KERNEL_WARP_FOLD : 0u);
     return BGR_OK;
+}
+
+// The lane slots of the checksum fold take 640 bytes of shared memory per Save.  Where they would cost a resident block
+// against the warp fold's 64 bytes per Save (a passive double buffer near a block boundary and many Saves in the
+// vector), the launch runs the warp-fold instance.  The held-Save check (VERIFY) always runs the lane fold.
+template <int MODE, bool STAMPS, bool VERIFY>
+int launch_particles(bgr_engine* e, const ProgramParams& pp) {
+    const int ti = (pp.flags & PF_PASSIVE_TMA) ? 1 : 0;
+    const size_t base = (ti ? size_t(2) * pp.passive_bytes : 0) + (STAMPS ? kSnapBytes : 0);
+    int lane = 0;
+    if (int rc = bundle_occupancy<MODE, STAMPS, VERIFY, false>(e, base, pp.n_saves, ti, lane); rc != BGR_OK) return rc;
+    if constexpr (!VERIFY) {
+        int warp = 0;
+        if (int rc = bundle_occupancy<MODE, STAMPS, false, true>(e, base, pp.n_saves, ti, warp); rc != BGR_OK) return rc;
+        if (lane < warp) return launch_bundle<MODE, STAMPS, false, true>(e, pp, base + fold_bytes(true, pp.n_saves), warp);
+    }
+    return launch_bundle<MODE, STAMPS, VERIFY, false>(e, pp, base + fold_bytes(false, pp.n_saves), lane);
 }
 
 // The stamped instances add the stamp-point snapshot (kSnapBytes) to the passive double buffer.  With more than about
 // 13 passive planes that costs the passive-TMA launches a resident block per SM; such a registration runs the instance
 // without stamps instead.  Launches without the double buffer (17 KB of shared memory) always keep three blocks.
+// The test holds the checksum partials at their least: the warp fold of 40 Saves.
 template <int MODE>
 int snapshot_fits_mode(bgr_engine* e, bool& fits) {
     fits = true;
     if (e->runs.empty() || 2u * e->passive_bytes > 96u * 1024u) return BGR_OK;  // never the passive-TMA configuration
-    auto kern = k_particles_program<MODE, true, false>;
-    const size_t buf = size_t(2) * e->passive_bytes, with = buf + kSnapBytes;
-    if (with > 48 * 1024) CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, int(with)));
+    const size_t buf = size_t(2) * e->passive_bytes + fold_bytes(true, kMaxSaves), with = buf + kSnapBytes;
     int nb_without = 0, nb_with = 0;
-    CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb_without, kern, int(kTileRows) / 2, buf));
-    CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb_with, kern, int(kTileRows) / 2, with));
+    if (int rc = bundle_blocks_per_sm<MODE, true, false, true>(buf, nb_without); rc != BGR_OK) return rc;
+    if (int rc = bundle_blocks_per_sm<MODE, true, false, true>(with, nb_with); rc != BGR_OK) return rc;
     fits = nb_with >= nb_without;
     return BGR_OK;
 }

@@ -139,6 +139,14 @@ constexpr uint32_t kSegsPerTile = kTileRows / kSegRows;
 // The stamped instances keep the active words and alive bytes of the last stamp point in shared memory, one snapshot per
 // thread laid out [word group][thread]: four uint4 groups (two planes of its two rows each) and one alive word.
 constexpr uint32_t kSnapBytes = (4u * 16u + 4u) * (kTileRows / 2u);
+// Checksum partials of the bundle kernel, at the front of its dynamic shared memory.  Lane fold (the default): per Save
+// kLaneWords words per lane, laid out [save][word][lane]: the XOR of the lane's Translation hashes (lo, hi), of its
+// Velocity hashes (lo, hi), and its live rows with bit 31 set once it saw a non-finite value.  Warp fold (launches where
+// those slots would cost a resident block): per Save the kAccStride columns as 32-bit halves, fed by warp reductions.
+constexpr uint32_t kLaneWords = 5;
+__host__ __device__ constexpr uint32_t fold_bytes(bool warp_fold, uint32_t n_saves) {
+    return n_saves * (warp_fold ? uint32_t(kAccStride) * 2u * 4u : kLaneWords * 32u * 4u);
+}
 
 struct ProgramParams {
     uint8_t* arena;
@@ -436,8 +444,9 @@ __device__ __forceinline__ void spawn_row(const SysSpec& sy, Word&& word, int k,
 //       LOAD    : read them from the snapshot image once
 //       ADVANCE : update_particles + despawn_particles in registers (0 bytes)
 //       SAVE    : stream them into the frame's slot and fold the per-entity seahashes of the
-//                 checksummed columns: warp REDUX.XOR -> shared atomics -> one global atomic per
-//                 block per (save, column) -> last block publishes to host-mapped memory.  A warp stores
+//                 checksummed columns: every lane XORs its partials into its own shared-memory slot ->
+//                 after the tiles one warp reduction and one global atomic per block per (save, column)
+//                 -> last block publishes to host-mapped memory.  A warp stores
 //                 only the planes of its 64-row segment whose content stamp the slot does not hold
 //                 already (ProgramParams::stamps): in a 2-D world z, velocity.x, ttl.hi and alive
 //                 keep their bits from frame to frame and are stored once per slot
@@ -461,7 +470,11 @@ __device__ __forceinline__ void spawn_row(const SysSpec& sy, Word&& word, int k,
 // grid is latency-bound, and there the instance without it runs (engine.cu run_fused), which stores every active plane.
 // VERIFY: BGR_TUNE_HELD_SAVES=2, every held Save compares its target with the registers (check_held).  The instances
 // that run by default do not carry that code.
-template <int MODE, bool STAMPS, bool VERIFY>
+// WARP_FOLD: a Save's partials are reduced over the warp (REDUX) and lane 0 adds them to the block's columns, instead of
+// every lane adding its own to its lane slot (fold_bytes).  The lane slots take 640 bytes of shared memory per Save;
+// launch_particles runs this instance only where they would cost a resident block (a wide passive double buffer and
+// many Saves in one vector).
+template <int MODE, bool STAMPS, bool VERIFY, bool WARP_FOLD = false>
 __global__ void __launch_bounds__(256, 3) k_particles_program(const __grid_constant__ ProgramParams p) {  // budget: prologue
     constexpr int VEC = 2, BLOCK = 256;  // rows per thread, threads per block (__launch_bounds__)
     static_assert(VEC * BLOCK == int(kTileRows), "a block iteration covers one tile");
@@ -473,10 +486,11 @@ __global__ void __launch_bounds__(256, 3) k_particles_program(const __grid_const
     const bool CKV = STATIC_CK ? true : (p.flags & PF_CK_V) != 0;
     const bool FINT = STATIC_CK ? true : (p.flags & PF_FIN_T) != 0;
     const bool FINV = STATIC_CK ? true : (p.flags & PF_FIN_V) != 0;
-    extern __shared__ __align__(128) uint8_t s_dyn[];  // STAMPS: the stamp-point snapshot (kSnapBytes); then 2 x passive_bytes (double buffer)
-    uint8_t* const s_passive = s_dyn + (STAMPS ? kSnapBytes : 0u);
-    uint4* const s_snap = reinterpret_cast<uint4*>(s_dyn);
-    __shared__ unsigned int s_acc[kMaxSaves * kAccStride * 2];  // 32-bit halves: native shared atomics, no CAS loop
+    // the checksum partials (fold_bytes); STAMPS: the stamp-point snapshot (kSnapBytes); then 2 x passive_bytes (double buffer)
+    extern __shared__ __align__(128) uint8_t s_dyn[];
+    unsigned int* const s_fold = reinterpret_cast<unsigned int*>(s_dyn);  // 32-bit words: native shared atomics, no CAS loop
+    uint4* const s_snap = reinterpret_cast<uint4*>(s_dyn + fold_bytes(WARP_FOLD, p.n_saves));
+    uint8_t* const s_passive = reinterpret_cast<uint8_t*>(s_snap) + (STAMPS ? kSnapBytes : 0u);
     __shared__ __align__(8) uint64_t s_bar[2];
     __shared__ unsigned int s_last;
     __shared__ unsigned int s_stored;  // bgr_trace_enable: 64-byte units of active planes this block stored
@@ -487,7 +501,7 @@ __global__ void __launch_bounds__(256, 3) k_particles_program(const __grid_const
     // Programmatic dependent launch: let the NEXT request vector's kernel be launched and its blocks scheduled
     // into SM slots as this grid drains (hides launch latency and block ramp-up between back-to-back ticks) ...
     asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
-    for (uint32_t i = tid; i < p.n_saves * kAccStride * 2; i += BLOCK) s_acc[i] = 0u;
+    for (uint32_t i = tid; i < fold_bytes(WARP_FOLD, p.n_saves) / 4u; i += BLOCK) s_fold[i] = 0u;
     const bool use_tma = (p.flags & PF_PASSIVE_TMA) && p.n_runs > 0;
     // the passive planes of a tile as bulk-copy chunks: whole runs of adjacent planes; f(offset inside the tile, bytes)
     auto for_each_passive_chunk = [&](auto&& f) {
@@ -744,12 +758,13 @@ __global__ void __launch_bounds__(256, 3) k_particles_program(const __grid_const
         const bool passive_early = (p.flags & PF_PASSIVE_EARLY) != 0;
         if (use_tma && tid == 0 && passive_early) issue_passive_stores();
 
+        // WARP_FOLD only: the warp's partials of the last Save, added to the block's columns at the next one
         uint32_t pend[5] = {0, 0, 0, 0, 0};
         uint32_t pend_row = 0;
         bool pend_valid = false;
         auto flush_pending = [&]() {
-            if (pend_valid && lane == 0) {
-                unsigned int* a = &s_acc[pend_row * 2];
+            if (WARP_FOLD && pend_valid && lane == 0) {
+                unsigned int* a = &s_fold[pend_row * 2];
                 if (CKT) { atomicXor(&a[2 * p.ck_t_slot], pend[0]); atomicXor(&a[2 * p.ck_t_slot + 1], pend[1]); }
                 if (CKV) { atomicXor(&a[2 * p.ck_v_slot], pend[2]); atomicXor(&a[2 * p.ck_v_slot + 1], pend[3]); }
                 atomicAdd(&a[12], pend[4] & 0xFFFFu);
@@ -853,17 +868,29 @@ __global__ void __launch_bounds__(256, 3) k_particles_program(const __grid_const
                 if ((tz_zero || !CKT) && (vz_zero || !CKV)) hash_rows(BoolConst<true>{});
                 else hash_rows(BoolConst<false>{});
                 const uint32_t n_alive = __popc(alive & 0x01010101u);  // budget: save_fold
-                // warp-level fold (REDUX) now, shared-memory atomics at the NEXT save (or after the op
-                // loop): the REDUX latency is covered by the following ADVANCE instead of stalling lane 0
-                flush_pending();
-                const unsigned full = 0xffffffffu;
-                if (CKT) { pend[0] = __reduce_xor_sync(full, uint32_t(hx_t)); pend[1] = __reduce_xor_sync(full, uint32_t(hx_t >> 32)); }
-                if (CKV) { pend[2] = __reduce_xor_sync(full, uint32_t(hx_v)); pend[3] = __reduce_xor_sync(full, uint32_t(hx_v >> 32)); }
-                // one REDUX for two counts: live rows (at most 32 * VEC) in the low half, lanes that saw a non-finite
-                // value in the high half
-                pend[4] = __reduce_add_sync(full, n_alive | (bad << 16));
-                pend_row = p.ops[i].save_index * kAccStride;
-                pend_valid = true;
+                if (!WARP_FOLD) {
+                    // XOR and + are associative: the lane's slot takes its partials now, the warp and block reductions
+                    // run once, after the tiles.  32 consecutive words per instruction, no bank conflict; the results
+                    // are unused, so nothing waits on them.  A lane's count stays below 2^31: 2 rows x 8 warps x at
+                    // most 2^23 tiles.
+                    unsigned int* a = &s_fold[p.ops[i].save_index * (kLaneWords * 32u) + lane];
+                    if (CKT) { atomicXor(&a[0], uint32_t(hx_t)); atomicXor(&a[32], uint32_t(hx_t >> 32)); }
+                    if (CKV) { atomicXor(&a[64], uint32_t(hx_v)); atomicXor(&a[96], uint32_t(hx_v >> 32)); }
+                    atomicAdd(&a[128], n_alive);
+                    if (bad) atomicOr(&a[128], 0x80000000u);
+                } else {
+                    // warp-level fold (REDUX) now, shared-memory atomics at the NEXT save (or after the op
+                    // loop): the REDUX latency is covered by the following ADVANCE instead of stalling lane 0
+                    flush_pending();
+                    const unsigned full = 0xffffffffu;
+                    if (CKT) { pend[0] = __reduce_xor_sync(full, uint32_t(hx_t)); pend[1] = __reduce_xor_sync(full, uint32_t(hx_t >> 32)); }
+                    if (CKV) { pend[2] = __reduce_xor_sync(full, uint32_t(hx_v)); pend[3] = __reduce_xor_sync(full, uint32_t(hx_v >> 32)); }
+                    // one REDUX for two counts: live rows (at most 32 * VEC) in the low half, lanes that saw a non-finite
+                    // value in the high half
+                    pend[4] = __reduce_add_sync(full, n_alive | (bad << 16));
+                    pend_row = p.ops[i].save_index * kAccStride;
+                    pend_valid = true;
+                }
                 if (store && STAMPS) store_active(img, p.ops[i].call_count, held);  // budget: save_store
             } else {  // OP_LOAD  budget: load
                 load_active(p.arena + (size_t(p.ops[i].image_off256) << 8), p.ops[i].n_rows, p.ops[i].call_count);
@@ -930,13 +957,32 @@ __global__ void __launch_bounds__(256, 3) k_particles_program(const __grid_const
 
     // ---- block partials -> global accumulators -> (last block) host-visible results ----
     __syncthreads();
-    for (uint32_t i = tid; i < p.n_saves * kAccStride; i += BLOCK) {
-        unsigned long long v = (unsigned long long)s_acc[2 * i] | ((unsigned long long)s_acc[2 * i + 1] << 32);
-        uint32_t c = i % kAccStride;
-        if (v) {
-            if (c == 6) atomicAdd(&p.accum[i], v);
-            else if (c == 7) atomicOr(&p.accum[i], v);
-            else atomicXor(&p.accum[i], v);
+    if (WARP_FOLD) {
+        for (uint32_t i = tid; i < p.n_saves * kAccStride; i += BLOCK) {
+            unsigned long long v = (unsigned long long)s_fold[2 * i] | ((unsigned long long)s_fold[2 * i + 1] << 32);
+            uint32_t c = i % kAccStride;
+            if (v) {
+                if (c == 6) atomicAdd(&p.accum[i], v);
+                else if (c == 7) atomicOr(&p.accum[i], v);
+                else atomicXor(&p.accum[i], v);
+            }
+        }
+    } else {
+        // one warp per Save: reduce the 32 lane slots of each word, then the same global atomics as above
+        const unsigned full = 0xffffffffu;
+        for (uint32_t s = tid >> 5; s < p.n_saves; s += BLOCK / 32) {
+            const unsigned int* a = &s_fold[s * (kLaneWords * 32u) + lane];
+            const unsigned long long t = __reduce_xor_sync(full, a[0]) | ((unsigned long long)__reduce_xor_sync(full, a[32]) << 32);
+            const unsigned long long v = __reduce_xor_sync(full, a[64]) | ((unsigned long long)__reduce_xor_sync(full, a[96]) << 32);
+            const uint32_t n = __reduce_add_sync(full, a[128] & 0x7FFFFFFFu);  // at most the world's rows
+            const bool bad = __any_sync(full, a[128] >> 31);
+            if (lane == 0) {
+                unsigned long long* acc = &p.accum[s * kAccStride];
+                if (t) atomicXor(&acc[p.ck_t_slot], t);
+                if (v) atomicXor(&acc[p.ck_v_slot], v);
+                if (n) atomicAdd(&acc[6], (unsigned long long)n);
+                if (bad) atomicOr(&acc[7], 1ULL);
+            }
         }
     }
     if (p.trace && tid == 0 && s_stored) atomicAdd(&p.trace[3], (unsigned long long)s_stored);

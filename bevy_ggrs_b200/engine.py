@@ -50,6 +50,12 @@ class LastKernel(NamedTuple):
         """The last replay ran on the generated kernel's replay entry point (BGR_KERNEL_REPLAY), not in chunks."""
         return bool(self.raw & capi.BGR_KERNEL_REPLAY)
 
+    @property
+    def warp_fold(self) -> bool:
+        """The bundle launch reduced each Save's checksum partials over the warp (BGR_KERNEL_WARP_FOLD): its lane slots
+        would have cost it a resident block per SM."""
+        return bool(self.raw & capi.BGR_KERNEL_WARP_FOLD)
+
     @staticmethod
     def decode(v: int) -> "LastKernel":
         return LastKernel(_KERNEL_KINDS.get(v & 0xF, f"unknown({v & 0xF})"), (v >> 4) & 0xF, (v >> 8) & 0x3,

@@ -931,7 +931,10 @@ BGR_API int bgr_generic_specialised(bgr_engine* e, uint32_t* specialised_out);
  *              (bgr_held_saves; env BGR_TUNE_HELD_SAVES, default 1)
  *   bit 28     BGR_KERNEL_BATCHED, generic NVRTC: the vector ran inside a world batch's launch (bgr_batch_handle_requests)
  *   bit 29     BGR_KERNEL_REPLAY, generic NVRTC: the last bgr_replay / bgr_batch_replay ran on the generated kernel's replay
- *              entry point (k_generic_jit_replay); clear when it ran in chunks through the engine's own kernel */
+ *              entry point (k_generic_jit_replay); clear when it ran in chunks through the engine's own kernel
+ *   bit 30     BGR_KERNEL_WARP_FOLD, bundle: each Save's checksum partials were reduced over the warp as it ran, not
+ *              added to per-lane shared-memory slots and reduced once per block: the slots (640 bytes per Save) would
+ *              have cost the launch a resident block per SM (a wide passive double buffer and many Saves) */
 #define BGR_KERNEL_DEFERRED_LIVE (1u << 13)
 #define BGR_KERNEL_FROM_DEFERRED (1u << 14)
 #define BGR_KERNEL_PASSIVE_PLANES (1u << 15)
@@ -939,6 +942,7 @@ BGR_API int bgr_generic_specialised(bgr_engine* e, uint32_t* specialised_out);
 #define BGR_KERNEL_HELD_SAVES (1u << 27)
 #define BGR_KERNEL_BATCHED (1u << 28)
 #define BGR_KERNEL_REPLAY (1u << 29)
+#define BGR_KERNEL_WARP_FOLD (1u << 30)
 #define BGR_KERNEL_NONE 0u
 #define BGR_KERNEL_STEPWISE_TMA 1u       /* one kernel per request; Save / Load through the TMA-staged copy kernel */
 #define BGR_KERNEL_STEPWISE_FLAT 2u      /* one kernel per request; k_checksum_column + k_copy_image */

@@ -57,6 +57,8 @@ pub const BGR_KERNEL_HELD_SAVES: u32 = 1 << 27;
 pub const BGR_KERNEL_BATCHED: u32 = 1 << 28;
 /// bgr_last_kernel flag: the last replay ran on the generated kernel's replay entry point (bgr_replay / bgr_batch_replay).
 pub const BGR_KERNEL_REPLAY: u32 = 1 << 29;
+/// bgr_last_kernel flag: the bundle launch reduced each Save's checksum partials over the warp (lane slots would have cost a block).
+pub const BGR_KERNEL_WARP_FOLD: u32 = 1 << 30;
 
 pub const BGR_CFG_FORCE_STEPWISE: u32 = 1;
 pub const BGR_CFG_SHARDED: u32 = 2;

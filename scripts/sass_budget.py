@@ -12,7 +12,9 @@ until the next one).  Within each region the count is split by issue pipe:
     fp32   FADD / FMUL / FFMA / FSETP / FMNMX / FSEL ...
     other  memory, control flow, warp votes and reductions, uniform datapath, conversions
 
-It also reports registers, spills and the 256-thread blocks per SM the register count allows (-Xptxas -v).
+It also reports registers, spills and the 256-thread blocks per SM the register count allows (-Xptxas -v), and the
+warp reductions (REDUX) of each region: the default instances reduce a Save's checksum partials in per-lane shared
+memory slots, so their save_fold has none.
 
 A static count is not a timing: predicated-off instructions and code the workload never reaches count like the hot
 path.  It tells where a change can cut instructions, not what the cut is worth.
@@ -119,13 +121,14 @@ _LOC = re.compile(r'"([^"]+)", line (\d+)')
 _INSN = re.compile(r"^\s*/\*[0-9a-f]{4,}\*/\s+(?:@!?U?P[T0-9]+\s+)?([A-Z][A-Z0-9_.]*)")
 
 
-def budget(sass: str, lines_to_region: dict) -> dict:
-    """per-instance {region: {pipe: count}} from nvdisasm -gi output"""
-    out, cur, region = {}, None, "other"
+def budget(sass: str, lines_to_region: dict) -> tuple[dict, dict]:
+    """per-instance {region: {pipe: count}} and {region: REDUX count} from nvdisasm -gi output"""
+    out, redux, cur, red, region = {}, {}, None, None, "other"
     for line in sass.splitlines():
         if line.startswith("//---------------------") and ".text." in line:
             name = line.split(".text.", 1)[1].split()[0]
             cur = out.setdefault(name, {r: dict.fromkeys(PIPES, 0) for r in REGIONS + ["other"]}) if KERNEL in name else None
+            red = redux.setdefault(name, dict.fromkeys(REGIONS + ["other"], 0)) if KERNEL in name else None
             region = "other"
             continue
         if cur is None:
@@ -137,18 +140,21 @@ def budget(sass: str, lines_to_region: dict) -> dict:
         m = _INSN.match(line)
         if m and m.group(1) not in ("NOP",):
             cur[region][pipe_of(m.group(1))] += 1
-    return out
+            red[region] += m.group(1).startswith("REDUX")
+    return out, redux
 
 
 def demangle_params(name: str) -> str:
-    m = re.search(KERNEL + r"ILi(\d)ELb([01])ELb([01])E", name)
-    return f"{KERNEL}<{m.group(1)},{'true' if m.group(2) == '1' else 'false'},{'true' if m.group(3) == '1' else 'false'}>"
+    """<MODE,STAMPS,VERIFY>, with a fourth argument `true` for the warp-fold instances (WARP_FOLD defaults to false)"""
+    m = re.search(KERNEL + r"ILi(\d)ELb([01])ELb([01])E(?:Lb([01])E)?", name)
+    args = [m.group(1)] + ["true" if m.group(i) == "1" else "false" for i in (2, 3)] + (["true"] if m.group(4) == "1" else [])
+    return f"{KERNEL}<{','.join(args)}>"
 
 
 def main():
     ap = argparse.ArgumentParser(description=__doc__.split("\n\n")[0])
     ap.add_argument("--instances", choices=["default", "all"], default="default",
-                    help="default: the six instances without the held-Save check (VERIFY=false)")
+                    help="default: the six instances that run by default (VERIFY=false, lane fold)")
     ap.add_argument("--cubin", help="an engine cubin built already (with --ptxas-log, the -Xptxas -v output)")
     ap.add_argument("--ptxas-log")
     args = ap.parse_args()
@@ -163,7 +169,7 @@ def main():
             raise RuntimeError("nvdisasm failed:\n" + r.stderr)
         sass = r.stdout
     res = ptxas_resources(log)
-    per = budget(sass, region_map())
+    per, redux = budget(sass, region_map())
     instances = {}
     for name in sorted(per):
         label = demangle_params(name)
@@ -177,6 +183,7 @@ def main():
             "blocks_per_sm_by_registers": REGS_PER_SM // (-(-regs // 8) * 8 * BLOCK) if regs else None,
             "total": {p: sum(c[p] for c in per[name].values()) for p in PIPES} | {"all": sum(sum(c.values()) for c in per[name].values())},
             "regions": regions,
+            "redux": {rg: c for rg, c in redux[name].items() if c},
         }
     print(json.dumps({"kernel": KERNEL, "instances": instances}))
 
