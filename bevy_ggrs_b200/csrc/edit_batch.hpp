@@ -7,12 +7,14 @@
 #include <vector>
 
 #include "../../include/bevy_ggrs_b200.h"
+#include "batch_call.hpp"
 #include "kernels.cuh"  // EditWorld, SpawnWorld
 
 namespace bgr {
 
-// Checks the entries of one call in list order: world in range and listed once, no null pointer, every record by the
-// single call's checks, and the row count after the entry's spawns within the member's ceiling.
+// Checks the entries of one call in list order: world admitted to the call's `list` (begun by the caller), no null
+// pointer, every record by the single call's checks, and the row count after the entry's spawns within the member's
+// ceiling.
 //   validate(world, entry, &rows, &err): bgr_apply_edits' own checks of a non-empty entry (status, err = its message,
 //                                        rows = the row count after the entry);
 //   ceiling(world):                      the most rows the member can hold (a growable member's BGR_CFG_GROWABLE
@@ -21,18 +23,12 @@ namespace bgr {
 // BGR_OK with rows[i] = entry i's row count afterwards (its member's rows(world) for an empty entry), or the status with
 // *bad = the failing entry and *err = why.  Nothing is grown here, so a refusal leaves every member as it was.
 template <class Validate, class Rows, class Ceiling>
-int edit_batch_check(uint32_t n_members, const bgr_batch_edits* entries, uint32_t n, Validate validate, Rows rows_of,
+int edit_batch_check(WorldList& list, const bgr_batch_edits* entries, uint32_t n, Validate validate, Rows rows_of,
                      Ceiling ceiling, uint64_t* rows, uint32_t* bad, std::string* err) {
-    std::vector<bool> seen(n_members, false);
     for (uint32_t i = 0; i < n; ++i) {
         *bad = i;
         const bgr_batch_edits& x = entries[i];
-        if (x.world >= n_members) {
-            *err = "no such world in a batch of " + std::to_string(n_members);
-            return BGR_ERR_INVALID_ARGUMENT;
-        }
-        if (seen[x.world]) { *err = "listed twice in one call"; return BGR_ERR_INVALID_ARGUMENT; }
-        seen[x.world] = true;
+        if (const int rc = list.admit(x.world, err); rc != BGR_OK) return rc;
         if ((x.n_edits && !x.edits) || (x.values_bytes && !x.values)) { *err = "null argument"; return BGR_ERR_INVALID_ARGUMENT; }
         rows[i] = rows_of(x.world);
         if (x.n_edits == 0) continue;
@@ -45,6 +41,15 @@ int edit_batch_check(uint32_t n_members, const bgr_batch_edits* entries, uint32_
         }
     }
     return BGR_OK;
+}
+
+// The same checks as one call to a batch of n_members that keeps no listing state between calls
+template <class Validate, class Rows, class Ceiling>
+int edit_batch_check(uint32_t n_members, const bgr_batch_edits* entries, uint32_t n, Validate validate, Rows rows_of,
+                     Ceiling ceiling, uint64_t* rows, uint32_t* bad, std::string* err) {
+    WorldList list(n_members);
+    list.begin();
+    return edit_batch_check(list, entries, n, validate, rows_of, ceiling, rows, bad, err);
 }
 
 // What one entry's folded patch holds: its stored words and presence masks, and the rows it spawns after first_row

@@ -36,6 +36,7 @@
 #include "frame_digest.cuh"
 #include "checkpoint.cuh"
 #include "checkpoint_check.hpp"
+#include "batch_call.hpp"
 #include "edit_batch.hpp"
 #include "feed_check.hpp"
 #include "replay_keyframes.hpp"
@@ -3551,8 +3552,8 @@ struct bgr_batch {
     cudaStream_t stream = nullptr;       // every member's
     JitKernel k;                         // k.batch_fn == nullptr: a call runs its worlds one after another
     std::vector<Prepared> prep;          // per member, reused by every call
-    std::vector<uint32_t> buf, listed;   // per member: its result buffer in this call, the last call that listed it
-    uint32_t calls = 0;
+    std::vector<uint32_t> buf;           // per member: its result buffer in this call
+    WorldList list;                      // the members the current call has listed
     MappedHostBuffer<uint8_t> h_stage;   // a call's JitWorld records, then the listed worlds' ops
     DeviceBuffer<uint8_t> d_stage;
     MappedHostBuffer<uint8_t> h_ckpt;    // bgr_batch_checkpoint_restore: the payloads, gathered for one upload
@@ -3624,7 +3625,7 @@ BGR_API int bgr_batch_create(bgr_engine* const* engines, uint32_t n, bgr_batch**
     b->stream = engines[0]->stream;
     b->prep.resize(n);
     b->buf.assign(n, 0);
-    b->listed.assign(n, 0);
+    b->list = WorldList(n);
     std::string why;
     if (batch_specialise(b, &why)) {
         const size_t bytes = size_t(n) * (sizeof(JitWorld) + sizeof(Op) * kMaxOps);
@@ -3656,59 +3657,103 @@ BGR_API int bgr_batch_specialised(bgr_batch* b, uint32_t* specialised_out) {
     return BGR_OK;
 }
 
+extern "C++" {  // overloads and a template inside the C API's extern "C" block
+namespace {
+
+// entry i's world: worlds[i], or the world of a bgr_batch_feed / bgr_batch_edits entry
+uint32_t world_of(uint32_t w) { return w; }
+uint32_t world_of(const bgr_batch_feed& r) { return r.world; }
+uint32_t world_of(const bgr_batch_edits& x) { return x.world; }
+
+// One bgr_batch_* call over the worlds it lists, in the conventions of include/bevy_ggrs_b200.h's world batches: it
+// begins the call on the batch's WorldList and sets status_out, n_sums and `counts` to 0 for every entry.  Each call keeps
+// its own order of checks, with check() and fail_at() for a refusal.  A call that runs every world reports each one with
+// record(), its checksums written at out() / room(), and returns outcome().
+template <class Entry>
+struct BatchCall {
+    bgr_batch* b;
+    const Entry* entries;
+    int32_t* status_out;
+    bgr_checksum* sums;  // every world's checksums, packed in list order as far as cap reaches
+    uint32_t cap;
+    uint32_t* n_sums;    // per entry: its checksum count
+    uint32_t off = 0;    // the checksums of the entries recorded so far, up to cap
+    int first = BGR_OK;  // the first non-OK status recorded, and its message
+    std::string first_err;
+
+    BatchCall(bgr_batch* b, const Entry* entries, uint32_t n, int32_t* status_out, bgr_checksum* sums = nullptr, uint32_t cap = 0,
+              uint32_t* n_sums = nullptr, std::initializer_list<uint32_t*> counts = {})
+        : b(b), entries(entries), status_out(status_out), sums(sums), cap(cap), n_sums(n_sums) {
+        b->list.begin();
+        std::fill_n(status_out, n, int32_t(BGR_OK));
+        if (n_sums) std::fill_n(n_sums, n, 0u);
+        for (uint32_t* c : counts)
+            if (c) std::fill_n(c, n, 0u);
+    }
+    // entry i's world listed in this call (in range, not listed before), or entry i marked with the refusal
+    int check(uint32_t i) {
+        std::string why;
+        const int rc = b->list.admit(world_of(entries[i]), &why);
+        return rc == BGR_OK ? rc : fail_at(i, fail(rc, why));
+    }
+    // marks entry i with `status` and puts "world <index>: " in front of g_err
+    int fail_at(uint32_t i, int status) {
+        status_out[i] = status;
+        g_err = "world " + std::to_string(world_of(entries[i])) + ": " + g_err;
+        return status;
+    }
+    bgr_checksum* out() const { return sums && off < cap ? sums + off : nullptr; }
+    uint32_t room() const { return sums && off < cap ? cap - off : 0u; }
+    // entry i ran: its status (g_err its message when not OK) and the n checksums it wrote at out()
+    void record(uint32_t i, int rc, uint32_t n) {
+        n_sums[i] = n;
+        off += std::min(n, cap - std::min(off, cap));
+        if (rc != BGR_OK) {
+            fail_at(i, rc);
+            if (first == BGR_OK) { first = rc; first_err = g_err; }
+        }
+    }
+    // the call's status: the first non-OK one recorded, with that world's message
+    int outcome() {
+        if (first != BGR_OK) g_err = first_err;
+        return first;
+    }
+};
+
+}  // namespace
+}  // extern "C++"
+
 BGR_API int bgr_batch_handle_requests(bgr_batch* b, const uint32_t* worlds, uint32_t n_worlds, const bgr_session_info* sessions,
                                       const bgr_request* requests, const uint32_t* n_requests, bgr_checksum* checksums_out,
                                       uint32_t checksums_cap, uint32_t* n_checksums_out, int32_t* status_out) {
     if (!b) return fail(BGR_ERR_INVALID_ARGUMENT, "null batch");
     if (n_worlds && (!worlds || !n_requests || !n_checksums_out || !status_out)) return fail(BGR_ERR_INVALID_ARGUMENT, "null argument");
     NvtxRange span("HandleRequests");
-    b->calls += 1;
-    for (uint32_t i = 0; i < n_worlds; ++i) { status_out[i] = BGR_OK; n_checksums_out[i] = 0; }
-    auto world_fail = [&](uint32_t i, int status) {
-        status_out[i] = status;
-        g_err = "world " + std::to_string(worlds[i]) + ": " + g_err;
-        return status;
-    };
+    BatchCall call(b, worlds, n_worlds, status_out, checksums_out, checksums_cap, n_checksums_out);
     auto session = [&](uint32_t i) { return sessions ? &sessions[i] : nullptr; };
     // every world is validated and compiled before any executes
     std::vector<size_t> req_off(n_worlds + 1, 0);
     for (uint32_t i = 0; i < n_worlds; ++i) {
+        int rc = call.check(i);
+        if (rc != BGR_OK) return rc;
         const uint32_t w = worlds[i];
-        if (w >= b->engines.size())
-            return world_fail(i, fail(BGR_ERR_INVALID_ARGUMENT, "no such world in a batch of " + std::to_string(b->engines.size())));
-        if (b->listed[w] == b->calls) return world_fail(i, fail(BGR_ERR_INVALID_ARGUMENT, "listed twice in one call"));
-        b->listed[w] = b->calls;
-        if (n_requests[i] > BGR_MAX_REQUESTS) return world_fail(i, fail(BGR_ERR_CAPACITY, "too many requests in one handle_requests call"));
+        if (n_requests[i] > BGR_MAX_REQUESTS)
+            return call.fail_at(i, fail(BGR_ERR_CAPACITY, "too many requests in one handle_requests call"));
         bgr_engine* e = b->engines[w];
         if (!e->pending.empty())
-            return world_fail(i, fail(BGR_ERR_STATE, "un-collected bgr_submit_requests pending: call bgr_collect first"));
+            return call.fail_at(i, fail(BGR_ERR_STATE, "un-collected bgr_submit_requests pending: call bgr_collect first"));
         req_off[i + 1] = req_off[i] + n_requests[i];
-        const int rc = prepare(e, session(i), requests ? requests + req_off[i] : nullptr, n_requests[i], b->prep[w]);
-        if (rc != BGR_OK) return world_fail(i, rc);
+        rc = prepare(e, session(i), requests ? requests + req_off[i] : nullptr, n_requests[i], b->prep[w]);
+        if (rc != BGR_OK) return call.fail_at(i, rc);
     }
-    // results: each world's checksums behind the previous worlds', as far as checksums_cap reaches
-    int first = BGR_OK;
-    std::string first_err;
-    uint32_t out_off = 0;
-    auto collect_world = [&](uint32_t i, int rc, uint32_t n) {
-        n_checksums_out[i] = n;
-        out_off += std::min(n, checksums_cap - std::min(out_off, checksums_cap));
-        if (rc != BGR_OK) {
-            world_fail(i, rc);
-            if (first == BGR_OK) { first = rc; first_err = g_err; }
-        }
-    };
-    auto out_at = [&]() { return checksums_out && out_off < checksums_cap ? checksums_out + out_off : nullptr; };
-    auto cap_at = [&]() { return checksums_out && out_off < checksums_cap ? checksums_cap - out_off : 0u; };
     if (!b->k.batch_fn) {  // the worlds' own submit path, in list order
         for (uint32_t i = 0; i < n_worlds; ++i) {
             uint32_t n = 0;
             const int rc = bgr_handle_requests(b->engines[worlds[i]], session(i), requests ? requests + req_off[i] : nullptr, n_requests[i],
-                                               out_at(), cap_at(), &n);
-            collect_world(i, rc, n);
+                                               call.out(), call.room(), &n);
+            call.record(i, rc, n);
         }
-        if (first != BGR_OK) g_err = first_err;
-        return first;
+        return call.outcome();
     }
     if (n_worlds == 0) return BGR_OK;
     // spawning worlds: growable members take the capacity their spawns need (a program does not depend on the capacity,
@@ -3718,8 +3763,8 @@ BGR_API int bgr_batch_handle_requests(bgr_batch* b, const uint32_t* worlds, uint
         const bgr_engine* e = b->engines[worlds[i]];
         const uint64_t rows = b->prep[worlds[i]].pg.rows_needed;
         if (rows > e->ceiling)
-            return world_fail(i, fail(BGR_ERR_CAPACITY, std::to_string(rows) + " rows exceed the engine's ceiling of " +
-                                                            std::to_string(e->ceiling) + " rows (BGR_CFG_GROWABLE)"));
+            return call.fail_at(i, fail(BGR_ERR_CAPACITY, std::to_string(rows) + " rows exceed the engine's ceiling of " +
+                                                              std::to_string(e->ceiling) + " rows (BGR_CFG_GROWABLE)"));
     }
     for (uint32_t i = 0; i < n_worlds; ++i) {
         const uint32_t w = worlds[i];
@@ -3727,7 +3772,7 @@ BGR_API int bgr_batch_handle_requests(bgr_batch* b, const uint32_t* worlds, uint
         const Program& pg = b->prep[w].pg;
         if (pg.rows_needed) {
             const int rc = grow_to(e, pg.rows_needed);
-            if (rc != BGR_OK) return world_fail(i, rc);
+            if (rc != BGR_OK) return call.fail_at(i, rc);
         }
         b->buf[w] = e->next_buf;
         if (!pg.spawn_vals.empty()) std::memcpy(e->spawn[b->buf[w]].get(), pg.spawn_vals.data(), pg.spawn_vals.size() * sizeof(float2));
@@ -3745,7 +3790,7 @@ BGR_API int bgr_batch_handle_requests(bgr_batch* b, const uint32_t* worlds, uint
         p.t_compiled = host_ns();
         e->tiledep_chain = false;
         const int rc = plan(e, p);  // a deferred live image this vector cannot start from is written here, before the launch
-        if (rc != BGR_OK) return world_fail(i, rc);
+        if (rc != BGR_OK) return call.fail_at(i, rc);
         JitWorld r = launch_record(e, p.pg, b->buf[w]);
         r.item0 = items;
         r.ops_off = n_ops;
@@ -3767,15 +3812,14 @@ BGR_API int bgr_batch_handle_requests(bgr_batch* b, const uint32_t* worlds, uint
         e->launches += 1;
         e->last_kernel = BGR_KERNEL_GENERIC_NVRTC | (uint32_t(b->k.item_rows) << 16) | BGR_KERNEL_BATCHED;
         const int rc = commit(e, b->prep[w], b->buf[w]);
-        if (rc != BGR_OK) return world_fail(i, rc);
+        if (rc != BGR_OK) return call.fail_at(i, rc);
     }
     for (uint32_t i = 0; i < n_worlds; ++i) {
         uint32_t n = 0;
-        const int rc = collect(b->engines[worlds[i]], out_at(), cap_at(), &n);
-        collect_world(i, rc, n);
+        const int rc = collect(b->engines[worlds[i]], call.out(), call.room(), &n);
+        call.record(i, rc, n);
     }
-    if (first != BGR_OK) g_err = first_err;
-    return first;
+    return call.outcome();
 }
 
 // ---- replays: a recorded input log run through a world, checksummed at an interval, without snapshots ----
@@ -4443,55 +4487,31 @@ int batch_replay(bgr_batch* b, const uint32_t* worlds, uint32_t n_worlds, const 
     if (!b) return fail(BGR_ERR_INVALID_ARGUMENT, "null batch");
     if (n_worlds && (!worlds || !replays || !n_checksums_out || !status_out)) return fail(BGR_ERR_INVALID_ARGUMENT, "null argument");
     NvtxRange span("Replay");
-    b->calls += 1;
-    for (uint32_t i = 0; i < n_worlds; ++i) {
-        status_out[i] = BGR_OK;
-        n_checksums_out[i] = 0;
-        if (n_keyframes_out) n_keyframes_out[i] = 0;
-        if (n_samples_out) n_samples_out[i] = 0;
-    }
-    auto world_fail = [&](uint32_t i, int status) {
-        status_out[i] = status;
-        g_err = "world " + std::to_string(worlds[i]) + ": " + g_err;
-        return status;
-    };
+    BatchCall call(b, worlds, n_worlds, status_out, checksums_out, cap, n_checksums_out, {n_keyframes_out, n_samples_out});
     // every world is validated and planned before any executes
     std::vector<ReplayJob> jobs(n_worlds);
     for (uint32_t i = 0; i < n_worlds; ++i) {
-        const uint32_t w = worlds[i];
-        if (w >= b->engines.size())
-            return world_fail(i, fail(BGR_ERR_INVALID_ARGUMENT, "no such world in a batch of " + std::to_string(b->engines.size())));
-        if (b->listed[w] == b->calls) return world_fail(i, fail(BGR_ERR_INVALID_ARGUMENT, "listed twice in one call"));
-        b->listed[w] = b->calls;
-        int rc = replay_plan(b->engines[w], &replays[i], jobs[i], kfs ? &kfs[i] : nullptr, trs ? &trs[i] : nullptr);
+        int rc = call.check(i);
+        if (rc != BGR_OK) return rc;
+        rc = replay_plan(b->engines[worlds[i]], &replays[i], jobs[i], kfs ? &kfs[i] : nullptr, trs ? &trs[i] : nullptr);
         if (rc == BGR_OK && kfs) rc = keyframe_caps(jobs[i]);
         if (rc == BGR_OK && trs && i && !feed_same_fields(jobs[i].tp, jobs[0].tp))
             rc = fail(BGR_ERR_INVALID_ARGUMENT, "its trace's fields differ from those of entry 0's trace (a call has one record layout)");
         if (rc == BGR_OK && trs) rc = trace_caps(jobs[i]);
-        if (rc != BGR_OK) return world_fail(i, rc);
+        if (rc != BGR_OK) return call.fail_at(i, rc);
     }
     if (trs)  // every world is planned: the sample frames and row counts are known
         for (uint32_t i = 0; i < n_worlds; ++i) std::copy(jobs[i].samples.begin(), jobs[i].samples.end(), trs[i].samples);
-    int first = BGR_OK;
-    std::string first_err;
-    uint32_t out_off = 0;
     auto results = [&](uint32_t i, int rc) {
         uint32_t n = 0;
-        bgr_checksum* out = checksums_out && out_off < cap ? checksums_out + out_off : nullptr;
-        if (rc == BGR_OK) rc = replay_results(jobs[i], out, out ? cap - out_off : 0u, &n);
-        n_checksums_out[i] = n;
+        if (rc == BGR_OK) rc = replay_results(jobs[i], call.out(), call.room(), &n);
         if (n_keyframes_out) n_keyframes_out[i] = jobs[i].kf_done;
         if (n_samples_out) n_samples_out[i] = jobs[i].tr_done;
-        out_off += std::min(n, cap - std::min(out_off, cap));
-        if (rc != BGR_OK) {
-            world_fail(i, rc);
-            if (first == BGR_OK) { first = rc; first_err = g_err; }
-        }
+        call.record(i, rc, n);
     };
     if (!b->k.replay_fn || (kfs && !b->k.replay_kf_fn) || (trs && !b->k.replay_trace_fn)) {  // each world's own replay, in list order
         for (uint32_t i = 0; i < n_worlds; ++i) results(i, replay_run(jobs[i]));
-        if (first != BGR_OK) g_err = first_err;
-        return first;
+        return call.outcome();
     }
     std::vector<ReplayJob*> run;
     for (ReplayJob& j : jobs)
@@ -4502,8 +4522,7 @@ int batch_replay(bgr_batch* b, const uint32_t* worlds, uint32_t n_worlds, const 
         if (rc == BGR_OK) rc = replay_commit(*j);
     if (rc != BGR_OK) return rc;
     for (uint32_t i = 0; i < n_worlds; ++i) results(i, BGR_OK);
-    if (first != BGR_OK) g_err = first_err;
-    return first;
+    return call.outcome();
 }
 
 }  // namespace
@@ -4530,46 +4549,20 @@ BGR_API int bgr_batch_replay_trace(bgr_batch* b, const uint32_t* worlds, uint32_
 }
 
 // ---- batched checkpoints: the checkpoints of many worlds saved or restored in one pass ----
-namespace {
-
-// The index checks every batch call makes (in range, listed once), with the "world <index>: " prefix on a refusal
-struct BatchWorlds {
-    bgr_batch* b;
-    const uint32_t* worlds;
-    int32_t* status_out;
-    int fail_at(uint32_t i, int status) {
-        status_out[i] = status;
-        g_err = "world " + std::to_string(worlds[i]) + ": " + g_err;
-        return status;
-    }
-    int check(uint32_t i) {
-        const uint32_t w = worlds[i];
-        if (w >= b->engines.size())
-            return fail_at(i, fail(BGR_ERR_INVALID_ARGUMENT, "no such world in a batch of " + std::to_string(b->engines.size())));
-        if (b->listed[w] == b->calls) return fail_at(i, fail(BGR_ERR_INVALID_ARGUMENT, "listed twice in one call"));
-        b->listed[w] = b->calls;
-        return BGR_OK;
-    }
-};
-
-}  // namespace
-
 BGR_API int bgr_batch_checkpoint_save(bgr_batch* b, const uint32_t* worlds, uint32_t n_worlds, const int32_t* frames,
                                       void* dst, size_t dst_cap, bgr_keyframe* index, size_t* bytes_out, int32_t* status_out) {
     if (!b) return fail(BGR_ERR_INVALID_ARGUMENT, "null batch");
     if (!bytes_out || (n_worlds && (!worlds || !frames || !index || !status_out))) return fail(BGR_ERR_INVALID_ARGUMENT, "null argument");
     NvtxRange span("CheckpointSave");
-    b->calls += 1;
     *bytes_out = 0;
-    for (uint32_t i = 0; i < n_worlds; ++i) status_out[i] = BGR_OK;
-    BatchWorlds bw{b, worlds, status_out};
+    BatchCall call(b, worlds, n_worlds, status_out);
     for (uint32_t i = 0; i < n_worlds; ++i) {
-        int rc = bw.check(i);
+        const int rc = call.check(i);
         if (rc != BGR_OK) return rc;
     }
     for (uint32_t i = 0; i < n_worlds; ++i) {  // every member's submitted vectors, their results left queued
         const int rc = drain(b->engines[worlds[i]]);
-        if (rc != BGR_OK) return bw.fail_at(i, rc);
+        if (rc != BGR_OK) return call.fail_at(i, rc);
     }
     // one image-table encoder over the held frames of every listed world; its launches count on worlds[0]'s engine
     ImageEncoder x;
@@ -4628,22 +4621,20 @@ BGR_API int bgr_batch_checkpoint_restore(bgr_batch* b, const uint32_t* worlds, u
     if (!b) return fail(BGR_ERR_INVALID_ARGUMENT, "null batch");
     if (n_worlds && (!worlds || !blobs || !bytes || !status_out)) return fail(BGR_ERR_INVALID_ARGUMENT, "null argument");
     NvtxRange span("CheckpointRestore");
-    b->calls += 1;
-    for (uint32_t i = 0; i < n_worlds; ++i) status_out[i] = BGR_OK;
-    BatchWorlds bw{b, worlds, status_out};
+    BatchCall call(b, worlds, n_worlds, status_out);
     std::vector<RestoreBlob> r(n_worlds);
     for (uint32_t i = 0; i < n_worlds; ++i) {  // the host checks, in list order
-        int rc = bw.check(i);
+        int rc = call.check(i);
         if (rc != BGR_OK) return rc;
         rc = restore_check(b->engines[worlds[i]], blobs[i], bytes[i], &r[i]);
-        if (rc != BGR_OK) return bw.fail_at(i, rc);
+        if (rc != BGR_OK) return call.fail_at(i, rc);
     }
     if (n_worlds == 0) return BGR_OK;
     RestorePass x;
     size_t bad = n_worlds;
     int rc = restore_decode(r, x, &b->h_ckpt, &bad);
     if (rc == BGR_OK) rc = restore_commit(r, x, &bad);
-    if (rc != BGR_OK) return bad < n_worlds ? bw.fail_at(uint32_t(bad), rc) : rc;
+    if (rc != BGR_OK) return bad < n_worlds ? call.fail_at(uint32_t(bad), rc) : rc;
     return BGR_OK;
 }
 
@@ -4653,19 +4644,16 @@ BGR_API int bgr_batch_feed_begin(bgr_batch* b, const bgr_batch_feed* reports, ui
     if (!b) return fail(BGR_ERR_INVALID_ARGUMENT, "null batch");
     if (!ticket_out || (n && (!reports || !status_out))) return fail(BGR_ERR_INVALID_ARGUMENT, "null argument");
     NvtxRange span("FeedReport");
-    for (uint32_t i = 0; i < n; ++i) status_out[i] = BGR_OK;
+    BatchCall call(b, reports, n, status_out);
     bgr_batch::FeedScratch& x = b->feed;
     if (x.busy) return fail(BGR_ERR_STATE, "a batched feed report of this batch is in flight: call bgr_batch_feed_wait first");
     uint32_t bad = 0;
     std::string why;
-    const int rc = feed_batch_check(uint32_t(b->engines.size()), reports, n, [b](uint32_t w, uint32_t f) {
+    const int rc = feed_batch_check(b->list, reports, n, [b](uint32_t w, uint32_t f) {
         const bgr_engine* e = b->engines[w];
         return f < BGR_MAX_FEEDS && e->feeds[f].used ? FeedView{&e->feeds[f].p, e->feeds[f].busy} : FeedView{nullptr, false};
     }, &bad, &why);
-    if (rc != BGR_OK) {
-        status_out[bad] = rc;
-        return fail(rc, "world " + std::to_string(reports[bad].world) + ": " + why);
-    }
+    if (rc != BGR_OK) return call.fail_at(bad, fail(rc, why));
     bool any_cap = false;
     for (uint32_t i = 0; i < n; ++i) any_cap = any_cap || reports[i].records_cap;
     uint32_t* host_dev = any_cap ? (host_dst ? mapped_host(host_dst) : nullptr) : nullptr;
@@ -4690,10 +4678,7 @@ BGR_API int bgr_batch_feed_begin(bgr_batch* b, const bgr_batch_feed* reports, ui
     if (!x.copy) CUDA_TRY(cudaStreamCreateWithFlags(&x.copy, cudaStreamNonBlocking));
     for (uint32_t i = 0; i < n; ++i) {  // stream-ordered behind every queued submit, like the passes below
         const int r = touch_live(b->engines[reports[i].world]);
-        if (r != BGR_OK) {
-            status_out[i] = r;
-            return fail(r, "world " + std::to_string(reports[i].world) + ": " + g_err);
-        }
+        if (r != BGR_OK) return call.fail_at(i, r);
     }
     if (n) {
         CUDA_TRY(cudaMemcpyAsync(x.table.get(), tab, sizeof(FeedWorld) * n, cudaMemcpyHostToDevice, b->stream));
@@ -4737,16 +4722,12 @@ BGR_API int bgr_batch_apply_edits(bgr_batch* b, const bgr_batch_edits* entries, 
     if (!b) return fail(BGR_ERR_INVALID_ARGUMENT, "null batch");
     if (n && (!entries || !status_out)) return fail(BGR_ERR_INVALID_ARGUMENT, "null argument");
     NvtxRange span("ApplyEdits");
-    for (uint32_t i = 0; i < n; ++i) status_out[i] = BGR_OK;
-    auto world_fail = [&](uint32_t i, int status, const std::string& why) {
-        status_out[i] = status;
-        return fail(status, "world " + std::to_string(entries[i].world) + ": " + why);
-    };
+    BatchCall call(b, entries, n, status_out);
     // the host checks of every entry, then every fold, before anything runs
     std::vector<uint64_t> rows(n);
     uint32_t bad = 0;
     std::string why;
-    int rc = edit_batch_check(uint32_t(b->engines.size()), entries, n,
+    int rc = edit_batch_check(b->list, entries, n,
         [b](uint32_t w, const bgr_batch_edits& x, uint64_t* r, std::string* err) {
             const int s = validate_edits(b->engines[w], x.edits, x.n_edits, x.values_bytes, r);
             if (s != BGR_OK) *err = g_err;
@@ -4754,7 +4735,7 @@ BGR_API int bgr_batch_apply_edits(bgr_batch* b, const bgr_batch_edits* entries, 
         },
         [b](uint32_t w) { return uint64_t(b->engines[w]->st.n_rows); }, [b](uint32_t w) { return uint64_t(b->engines[w]->ceiling); },
         rows.data(), &bad, &why);
-    if (rc != BGR_OK) return world_fail(bad, rc, why);
+    if (rc != BGR_OK) return call.fail_at(bad, fail(rc, why));
     std::vector<EditCounts> counts(n);
     for (uint32_t i = 0; i < n; ++i) {
         bgr_engine* e = b->engines[entries[i].world];
@@ -4762,14 +4743,14 @@ BGR_API int bgr_batch_apply_edits(bgr_batch* b, const bgr_batch_edits* entries, 
         f.clear();
         if (entries[i].n_edits) {
             rc = fold_edits(e, entries[i].edits, entries[i].n_edits, static_cast<const uint8_t*>(entries[i].values), f);
-            if (rc != BGR_OK) return world_fail(i, rc, g_err);
+            if (rc != BGR_OK) return call.fail_at(i, rc);
             assert(f.stamps.empty() && "batch members never run the bundle kernel, so they have no content stamps");
         }
         counts[i] = EditCounts{f.words.size(), f.masks.size(), e->st.n_rows, uint32_t(rows[i] - e->st.n_rows)};
     }
     EditLayout L;
     rc = edit_layout(counts.data(), n, &L, &bad, &why);
-    if (rc != BGR_OK) return world_fail(bad, rc, why);
+    if (rc != BGR_OK) return call.fail_at(bad, fail(rc, why));
     if (n == 0) return BGR_OK;
     // every buffer, then growth, then the listed worlds' deferred live images, stream-ordered behind the queued submits
     bgr_engine::EditStage& sg = b->edit_stage[b->next_edit];
@@ -4780,11 +4761,11 @@ BGR_API int bgr_batch_apply_edits(bgr_batch* b, const bgr_batch_edits* entries, 
     for (uint32_t i = 0; i < n; ++i) {
         bgr_engine* e = b->engines[entries[i].world];
         if (rows[i] > e->st.n_rows) rc = grow_to(e, rows[i]);
-        if (rc != BGR_OK) return world_fail(i, rc, g_err);
+        if (rc != BGR_OK) return call.fail_at(i, rc);
     }
     for (uint32_t i = 0; i < n; ++i) {
         if (entries[i].n_edits) rc = touch_live(b->engines[entries[i].world]);
-        if (rc != BGR_OK) return world_fail(i, rc, g_err);
+        if (rc != BGR_OK) return call.fail_at(i, rc);
     }
     // the staging: every world's words and masks at its offsets, then the two tables
     uint8_t* h = sg.h.get();

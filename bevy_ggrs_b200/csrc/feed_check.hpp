@@ -5,9 +5,9 @@
 #include <algorithm>
 #include <cstring>
 #include <string>
-#include <vector>
 
 #include "../../include/bevy_ggrs_b200.h"
+#include "batch_call.hpp"
 #include "change_feed.cuh"  // FeedParams, FeedWorld
 
 namespace bgr {
@@ -59,22 +59,16 @@ inline bool feed_same_fields(const FeedParams& a, const FeedParams& b) {
     return std::memcmp(a.fields, b.fields, sizeof(FeedField) * a.n_fields) == 0;
 }
 
-// Checks the entries of one call in list order: world in range and listed once, the feed known and idle, its fields
-// those of entry 0's feed.  `view(world, feed)` gives the feed.  BGR_OK, or the status with *bad = the failing entry and
-// *err = why (the single call's message where it has one).
+// Checks the entries of one call in list order: world admitted to the call's `list` (begun by the caller), the feed known
+// and idle, its fields those of entry 0's feed.  `view(world, feed)` gives the feed.  BGR_OK, or the status with *bad = the
+// failing entry and *err = why (the single call's message where it has one).
 template <class View>
-int feed_batch_check(uint32_t n_members, const bgr_batch_feed* reports, uint32_t n, View view, uint32_t* bad, std::string* err) {
-    std::vector<bool> seen(n_members, false);
+int feed_batch_check(WorldList& list, const bgr_batch_feed* reports, uint32_t n, View view, uint32_t* bad, std::string* err) {
     const FeedParams* first = nullptr;
     for (uint32_t i = 0; i < n; ++i) {
         *bad = i;
         const bgr_batch_feed& r = reports[i];
-        if (r.world >= n_members) {
-            *err = "no such world in a batch of " + std::to_string(n_members);
-            return BGR_ERR_INVALID_ARGUMENT;
-        }
-        if (seen[r.world]) { *err = "listed twice in one call"; return BGR_ERR_INVALID_ARGUMENT; }
-        seen[r.world] = true;
+        if (const int rc = list.admit(r.world, err); rc != BGR_OK) return rc;
         const FeedView f = view(r.world, r.feed);
         if (!f.reg) { *err = "unknown feed"; return BGR_ERR_INVALID_ARGUMENT; }
         if (f.busy) { *err = "a report of this feed is in flight"; return BGR_ERR_STATE; }
@@ -85,6 +79,14 @@ int feed_batch_check(uint32_t n_members, const bgr_batch_feed* reports, uint32_t
         }
     }
     return BGR_OK;
+}
+
+// The same checks as one call to a batch of n_members that keeps no listing state between calls
+template <class View>
+int feed_batch_check(uint32_t n_members, const bgr_batch_feed* reports, uint32_t n, View view, uint32_t* bad, std::string* err) {
+    WorldList list(n_members);
+    list.begin();
+    return feed_batch_check(list, reports, n, view, bad, err);
 }
 
 // Fills tile0 and cap of every entry of `tab` (img, rep, rows and n_tiles set) in list order: consecutive global tiles,

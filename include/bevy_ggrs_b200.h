@@ -604,7 +604,21 @@ BGR_API int bgr_fold_partials_n(const bgr_partial* combined, uint32_t n, bgr_che
  * may differ, and so may a BGR_SYS_PARTICLES_SPAWN system's rate, ttl and seed (its columns may not).  A spawn past a
  * member's max_entities (or, BGR_CFG_GROWABLE, its ceiling) refuses the whole call; a growable member grows first.
  * bgr_batch_create checks all of this and names the first engine that fails.  Destroy a batch before any of its
- * engines; between calls every per-engine entry point stays usable on the members. */
+ * engines; between calls every per-engine entry point stays usable on the members.
+ * Every bgr_batch_* call below takes a list of entries, entry i naming one world by its index in the batch, and keeps
+ * these conventions (each call's comment adds what its entries are checked for, in which order):
+ *   - Every index is in range and listed at most once per call (BGR_ERR_INVALID_ARGUMENT: "no such world in a batch of
+ *     N", "listed twice in one call").  Worlds not listed are untouched.
+ *   - Every entry is checked, in list order, before anything runs in any world.  The first entry that fails is marked
+ *     in status_out (every other status_out[i] is BGR_OK), the call returns its status, bgr_last_error() reads
+ *     "world <index>: " and the single-world call's message, and no world changes.  A refusal of the call as a whole
+ *     (a null argument) marks no entry.
+ *   - A growable member grows after the checks.  A growth that fails is reported like a refusal of that world
+ *     (BGR_ERR_CUDA or BGR_ERR_CAPACITY) and nothing else runs; members that grew before it keep their larger capacity.
+ *   - A call that runs every world (bgr_batch_handle_requests, the batched replays) sets status_out[i] to what world
+ *     i's own call would have returned and returns the first non-OK one, with that world's message.  World i's
+ *     checksums follow the earlier worlds' in checksums_out, as far as the cap reaches; n_checksums_out[i] is its
+ *     count, and every per-world count is 0 for a world that did not run. */
 typedef struct bgr_batch bgr_batch;
 BGR_API int bgr_batch_create(bgr_engine* const* engines, uint32_t n, bgr_batch** out);
 BGR_API void bgr_batch_destroy(bgr_batch* b);
@@ -615,13 +629,10 @@ BGR_API void bgr_batch_destroy(bgr_batch* b);
 BGR_API int bgr_batch_specialised(bgr_batch* b, uint32_t* specialised_out);
 /* Synchronous: what bgr_handle_requests on worlds[0], worlds[1], ... in that order would do, in one launch.  World
  * worlds[i] runs the n_requests[i] requests that follow the previous worlds' in `requests` under sessions[i] (sessions
- * NULL: no session).  Every world is validated and its vector compiled first (indices in range and distinct,
- * n_requests[i] <= BGR_MAX_REQUESTS, no un-collected bgr_submit_requests): if any fails, nothing executes in any world,
- * the call returns that status, status_out marks that world and bgr_last_error() starts with "world <index>: ".
- * Otherwise every world executes, status_out[i] is what its own call would have returned (BGR_ERR_NON_FINITE ...) and
- * the call returns the first non-OK one.  World i's checksums follow the previous worlds' in checksums_out, as far as
- * checksums_cap reaches; n_checksums_out[i] is its count.  Worlds not listed are untouched.  Each listed world's
- * bgr_launch_count grows by one and its bgr_last_kernel carries BGR_KERNEL_BATCHED. */
+ * NULL: no session).  Each world is checked for its index, n_requests[i] <= BGR_MAX_REQUESTS and no un-collected
+ * bgr_submit_requests, and its vector compiled; then every world's spawns are checked against its ceiling.  Then every
+ * world executes, and status_out[i] is what its own call would have returned (BGR_ERR_NON_FINITE ...).  Each listed
+ * world's bgr_launch_count grows by one and its bgr_last_kernel carries BGR_KERNEL_BATCHED. */
 BGR_API int bgr_batch_handle_requests(bgr_batch* b, const uint32_t* worlds, uint32_t n_worlds, const bgr_session_info* sessions,
                                       const bgr_request* requests, const uint32_t* n_requests, bgr_checksum* checksums_out,
                                       uint32_t checksums_cap, uint32_t* n_checksums_out, int32_t* status_out);
@@ -656,10 +667,8 @@ struct bgr_replay {
     const uint8_t* inputs;       /* n_frames * n_players bytes, frame-major */
 };
 BGR_API int bgr_replay(bgr_engine* e, const struct bgr_replay* r, bgr_checksum* checksums_out, uint32_t cap, uint32_t* n_out);
-/* bgr_replay of replays[i] on worlds[i], in the conventions of bgr_batch_handle_requests: every listed world is validated
- * and planned first, and if any fails nothing executes anywhere (status_out marks it, bgr_last_error() starts with
- * "world <index>: ").  World i's checksums follow the previous worlds' in checksums_out as far as cap reaches;
- * n_checksums_out[i] is its count.  A specialised batch (bgr_batch_specialised) runs every world in one launch of its
+/* bgr_replay of replays[i] on worlds[i].  Each world is checked for its index and everything bgr_replay refuses, and
+ * planned, before any executes.  A specialised batch (bgr_batch_specialised) runs every world in one launch of its
  * generated kernel; otherwise each world's bgr_replay runs in list order. */
 BGR_API int bgr_batch_replay(bgr_batch* b, const uint32_t* worlds, uint32_t n_worlds, const struct bgr_replay* replays,
                              bgr_checksum* checksums_out, uint32_t cap, uint32_t* n_checksums_out, int32_t* status_out);
@@ -707,8 +716,8 @@ BGR_API int bgr_replay_keyframes(bgr_engine* e, const struct bgr_replay* r, cons
                                  size_t* bytes_out);
 /* bgr_batch_replay with keyframes: kfs[i] holds world i's interval and buffers, in bgr_replay_keyframes' conventions
  * (a null dst is refused with BGR_ERR_CAPACITY unless the world writes no keyframe; query a member's sizes with
- * bgr_replay_keyframes on its engine).  Every listed world is validated, planned and its capacities checked first;
- * n_keyframes_out[i] is world i's keyframe count. */
+ * bgr_replay_keyframes on its engine).  Each world's capacities are checked after its plan; n_keyframes_out[i] is world
+ * i's keyframe count. */
 BGR_API int bgr_batch_replay_keyframes(bgr_batch* b, const uint32_t* worlds, uint32_t n_worlds, const struct bgr_replay* replays,
                                        const struct bgr_keyframes* kfs, bgr_checksum* checksums_out, uint32_t cap,
                                        uint32_t* n_checksums_out, uint32_t* n_keyframes_out, int32_t* status_out);
@@ -759,21 +768,19 @@ BGR_API int bgr_replay_trace(bgr_engine* e, const struct bgr_replay* r, const st
 /* bgr_batch_replay with traces: traces[i] holds world i's interval, row range and buffers, in bgr_replay_trace's
  * conventions (a null dst is refused with BGR_ERR_CAPACITY unless the world takes no sample; query a member's sizes with
  * bgr_replay_trace on its engine).  Row ranges and intervals may differ between worlds; the field list must equal entry
- * 0's (BGR_ERR_INVALID_ARGUMENT otherwise), so a launch has one record layout.  Every listed world is validated, planned
- * and its capacities checked first; n_samples_out[i] is world i's sample count. */
+ * 0's (BGR_ERR_INVALID_ARGUMENT otherwise), so a launch has one record layout.  Each world's field list and then its
+ * capacities are checked after its plan; n_samples_out[i] is world i's sample count. */
 BGR_API int bgr_batch_replay_trace(bgr_batch* b, const uint32_t* worlds, uint32_t n_worlds, const struct bgr_replay* replays,
                                    const struct bgr_trace* traces, bgr_checksum* checksums_out, uint32_t cap,
                                    uint32_t* n_checksums_out, uint32_t* n_samples_out, int32_t* status_out);
 
 /* ---- batched checkpoints: the world checkpoints of many batch members saved or restored in one pass ----------------
- * Both calls follow the conventions of bgr_batch_handle_requests: indices in range and distinct, every listed world
- * validated before anything executes anywhere, a refusal marks the failing world in status_out with bgr_last_error()
- * starting with "world <index>: " and the single-world call's message, and worlds not listed are untouched.  Neither
- * depends on bgr_batch_specialised: the checkpoint kernels are part of the library, so a batch that ticks its worlds one
- * after another (BGR_TUNE_JIT=0, no NVRTC) saves and restores in one pass too.  The kernels of one call are counted on
- * worlds[0]'s bgr_launch_count, and their number does not depend on n_worlds: a save is four launches (k_frame_digest,
- * k_ckpt_measure, k_ckpt_scan, k_ckpt_pack) and a restore three (k_ckpt_unpack, k_frame_digest, k_ckpt_commit); fewer
- * when no listed world has a row.  Device memory for the encoding or decoding is allocated and freed inside the call.
+ * Neither depends on bgr_batch_specialised: the checkpoint kernels are part of the library, so a batch that ticks its
+ * worlds one after another (BGR_TUNE_JIT=0, no NVRTC) saves and restores in one pass too.  The kernels of one call are
+ * counted on worlds[0]'s bgr_launch_count, and their number does not depend on n_worlds: a save is four launches
+ * (k_frame_digest, k_ckpt_measure, k_ckpt_scan, k_ckpt_pack) and a restore three (k_ckpt_unpack, k_frame_digest,
+ * k_ckpt_commit); fewer when no listed world has a row.  Device memory for the encoding or decoding is allocated and
+ * freed inside the call.
  *
  * bgr_batch_checkpoint_save: blob i is byte for byte what bgr_checkpoint_save(worlds[i], frames[i]) writes (the frame
  * queued or retained).  The blobs go to dst in list order, each at a multiple of 8 bytes (the padding is zero);
@@ -781,9 +788,9 @@ BGR_API int bgr_batch_replay_trace(bgr_batch* b, const uint32_t* worlds, uint32_
  * retained (the single call's *found = 0), which is not an error.  dst == NULL: nothing runs; index[i].bytes = world i's
  * upper bound (every vector RAW), index[i].offset its place under those bounds, and *bytes_out = the total, a multiple
  * of 8.  Otherwise *bytes_out = the exact total, the end of the last blob rounded up to 8; a dst_cap below it is
- * BGR_ERR_CAPACITY, and then nothing is written to dst or index.  Waits for each member's submitted vectors and leaves
- * their results queued.  The payloads of every world come back to dst with one copy (page-locked dst from
- * bgr_host_alloc copies at the full PCIe rate). */
+ * BGR_ERR_CAPACITY, and then nothing is written to dst or index.  Once every index has passed, waits for each member's
+ * submitted vectors and leaves their results queued.  The payloads of every world come back to dst with one copy
+ * (page-locked dst from bgr_host_alloc copies at the full PCIe rate). */
 BGR_API int bgr_batch_checkpoint_save(bgr_batch* b, const uint32_t* worlds, uint32_t n_worlds, const int32_t* frames,
                                       void* dst, size_t dst_cap, bgr_keyframe* index, size_t* bytes_out,
                                       int32_t* status_out);
@@ -800,8 +807,7 @@ BGR_API int bgr_batch_checkpoint_save(bgr_batch* b, const uint32_t* worlds, uint
  * k_ckpt_unpack and k_frame_digest run over every block of every blob, three copies bring back the error words, the
  * digest words and the active counts, and one k_ckpt_commit launch copies every world to its image 0 and restored slot.
  * Every allocation happens before any world changes: out of device memory is BGR_ERR_CUDA with no world changed.  A
- * growable member whose growth fails is named (BGR_ERR_CUDA or BGR_ERR_CAPACITY) and nothing is restored; members that
- * grew before it keep their larger capacity, as in bgr_batch_handle_requests. */
+ * growable member whose growth fails is named and nothing is restored. */
 BGR_API int bgr_batch_checkpoint_restore(bgr_batch* b, const uint32_t* worlds, uint32_t n_worlds,
                                          const void* const* blobs, const size_t* bytes, int32_t* status_out);
 
@@ -812,12 +818,11 @@ BGR_API int bgr_batch_checkpoint_restore(bgr_batch* b, const uint32_t* worlds, u
  * applies.  The records are packed in list order into host_dst: entry i's start at the sum of the earlier entries'
  * n_records.  host_dst must come from bgr_host_alloc and hold sum(records_cap) records (NULL when every cap is 0); it
  * must not be read before bgr_batch_feed_wait(ticket) returns.
- * In the conventions of the other batch calls, every entry is validated before anything runs: indices in range and
- * distinct, a known feed (BGR_ERR_INVALID_ARGUMENT), no report of that feed in flight, single or batched (BGR_ERR_STATE),
- * and the same field list as entry 0's feed (BGR_ERR_INVALID_ARGUMENT: a call has one record size).  A refusal marks the
- * entry in status_out, bgr_last_error() starts with "world <index>: ", and nothing changes: no feed becomes busy and no
- * reported state moves.  A host_dst not from bgr_host_alloc is BGR_ERR_INVALID_ARGUMENT for the whole call, and a
- * second bgr_batch_feed_begin before the wait is BGR_ERR_STATE: one batched report per batch is in flight.
+ * A second bgr_batch_feed_begin before the wait is BGR_ERR_STATE for the whole call: one batched report per batch is in
+ * flight.  Then each entry is checked for its index, a known feed (BGR_ERR_INVALID_ARGUMENT), no report of that feed in
+ * flight, single or batched (BGR_ERR_STATE), and the same field list as entry 0's feed (BGR_ERR_INVALID_ARGUMENT: a call
+ * has one record size).  A refused call changes nothing: no feed becomes busy and no reported state moves.  A host_dst
+ * not from bgr_host_alloc is BGR_ERR_INVALID_ARGUMENT for the whole call.
  * The call is ordered behind every vector submitted on the shared stream, un-collected submits of a member included,
  * materialises a deferred live image only on the listed worlds that have one, and returns without waiting for the GPU.
  * It does not depend on bgr_batch_specialised.  Whatever n_entries, it is one table upload, four launches counted on
@@ -837,14 +842,10 @@ BGR_API int bgr_batch_feed_wait(bgr_batch* b, uint32_t ticket, bgr_feed_info* in
  * passive-plane writes), a fresh live content id, and a deferred live image materialised first.  Worlds not listed are
  * untouched; an entry with n_edits == 0 changes nothing in its world (it materialises nothing either), but is still
  * checked for its index.
- * In the conventions of the other batch calls, every entry is checked in list order before anything runs: indices in
- * range and distinct, no null pointer, every record by bgr_apply_edits' own checks, spawns past a fixed member's
- * max_entities or a growable member's ceiling (BGR_ERR_CAPACITY), spawning after the first request vector with
- * order_base != 0 (BGR_ERR_UNSUPPORTED).  A refusal marks the entry in status_out, bgr_last_error() reads
- * "world <index>: " and the single call's text ("world 2: edit 3: row out of range"), and nothing changes anywhere: no
- * member grows, nothing launches.  Then growable members grow; a growth that fails names its world (BGR_ERR_CUDA or
- * BGR_ERR_CAPACITY) and nothing is edited, and members that grew before it keep their larger capacity, as in
- * bgr_batch_handle_requests.
+ * Each entry is checked for its index, no null pointer, every record by bgr_apply_edits' own checks (bgr_last_error()
+ * "world 2: edit 3: row out of range"), spawns past a fixed member's max_entities or a growable member's ceiling
+ * (BGR_ERR_CAPACITY), spawning after the first request vector with order_base != 0 (BGR_ERR_UNSUPPORTED).  A refused
+ * call changes nothing anywhere: no member grows, nothing launches.
  * The call is ordered on the shared stream behind every queued vector, un-collected bgr_submit_requests of a member
  * included (they keep their results), and returns without waiting for the GPU.  The caller's buffers are free on
  * return: the patch goes into one of 4 page-locked staging buffers the batch owns, each grown to the largest call it

@@ -1,7 +1,8 @@
 // The host side of a batched change-feed report (csrc/feed_check.hpp, run by bgr_batch_feed_begin before anything
 // runs): every refusal of an entry (world out of range, listed twice, unknown feed, a report in flight, another field
-// list) with its status, message and entry, in list order; and the table layout (first global tile, cap of at most the
-// rows compared, staging size) against offsets computed by hand.  Host only: exit code 0 = passed.
+// list) with its status, message and entry, in list order; a world listed again in a later call of a batch's list; and
+// the table layout (first global tile, cap of at most the rows compared, staging size) against offsets computed by hand.
+// Host only: exit code 0 = passed.
 #include <cstdio>
 #include <cstring>
 #include <string>
@@ -80,6 +81,25 @@ int main() {
     // the first failing entry in list order is the one reported
     check(fl, {{0, 0, 5}, {2, 0, 5}, {9, 0, 5}}, BGR_ERR_STATE, 1, "a report of this feed is in flight");
     check(fl, {{0, 0, 5}, {0, 0, 5}, {2, 0, 5}}, BGR_ERR_INVALID_ARGUMENT, 1, "listed twice in one call");
+
+    // one list kept across calls, as a batch keeps it: a world listed in one call may be listed again in the next,
+    // whether that call passed or was refused, and is still refused when listed twice in one call
+    {
+        WorldList list(4);
+        auto call = [&](const std::vector<bgr_batch_feed>& r, int status, uint32_t entry, const char* text) {
+            uint32_t bad = 12345;
+            std::string err;
+            list.begin();
+            const int rc = feed_batch_check(list, r.data(), uint32_t(r.size()), fl, &bad, &err);
+            EXPECT(rc == status, text);
+            if (status != BGR_OK) EXPECT(bad == entry && err == text, (err + " != " + text).c_str());
+        };
+        call({{0, 0, 5}, {1, 0, 5}}, BGR_OK, 0, "second call");
+        call({{1, 0, 5}, {0, 0, 5}}, BGR_OK, 0, "listed again in the next call");
+        call({{0, 0, 5}, {1, 1, 5}}, BGR_ERR_INVALID_ARGUMENT, 1, "unknown feed");
+        call({{1, 0, 5}, {0, 0, 5}}, BGR_OK, 0, "listed again after a refused call");
+        call({{0, 0, 5}, {1, 0, 5}, {0, 0, 5}}, BGR_ERR_INVALID_ARGUMENT, 2, "listed twice in one call");
+    }
 
     // the layout: tiles compared per world 3, 0, 1, 2048, 0; caps 10, 7, 9999, 2^32-1, 0
     std::vector<FeedWorld> tab(5);
