@@ -54,6 +54,8 @@ BGR_FRAME_BLOB_VERSION = 1
 # world checkpoints
 BGR_CHECKPOINT_MAGIC = 0x43524742
 BGR_CHECKPOINT_VERSION = 1
+BGR_CHECKPOINT_DELTA_MAGIC = 0x44524742
+BGR_CHECKPOINT_DELTA_VERSION = 1
 BGR_CKPT_CONST, BGR_CKPT_SPARSE, BGR_CKPT_RAW = 0, 1, 2
 # bgr_last_kernel: kind in bits 0-3
 BGR_KERNEL_NONE, BGR_KERNEL_STEPWISE_TMA, BGR_KERNEL_STEPWISE_FLAT, BGR_KERNEL_BUNDLE, \
@@ -139,6 +141,14 @@ class bgr_checkpoint_header(C.Structure):
                 ("rows", C.c_uint32), ("words", C.c_uint32), ("n_blocks", C.c_uint32), ("n_columns", C.c_uint32),
                 ("fps", C.c_uint32), ("active", C.c_uint64), ("elapsed_ns", C.c_uint64), ("rng", C.c_uint64 * 4),
                 ("digest_root", C.c_uint64), ("payload_bytes", C.c_uint64)]
+
+
+class bgr_checkpoint_delta_header(C.Structure):
+    _fields_ = [("magic", C.c_uint32), ("version", C.c_uint32), ("layout", C.c_uint64), ("frame", C.c_int32),
+                ("rows", C.c_uint32), ("base_frame", C.c_int32), ("base_rows", C.c_uint32), ("words", C.c_uint32),
+                ("n_blocks", C.c_uint32), ("n_columns", C.c_uint32), ("fps", C.c_uint32), ("active", C.c_uint64),
+                ("elapsed_ns", C.c_uint64), ("rng", C.c_uint64 * 4), ("digest_root", C.c_uint64),
+                ("base_root", C.c_uint64), ("payload_bytes", C.c_uint64)]
 
 
 class bgr_replay(C.Structure):
@@ -250,6 +260,9 @@ PROTOTYPES = {
                                          C.c_uint32, u32p, i32p]),
     "bgr_checkpoint_save": (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p, C.c_size_t, C.POINTER(C.c_size_t), i32p]),
     "bgr_checkpoint_restore": (C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t]),
+    "bgr_checkpoint_save_delta": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_size_t, C.POINTER(C.c_size_t),
+                                            i32p]),
+    "bgr_checkpoint_restore_delta": (C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t]),
     "bgr_save_world": (C.c_int, [C.c_void_p, C.POINTER(bgr_checksum)]),
     "bgr_load_world": (C.c_int, [C.c_void_p]),
     "bgr_advance_world": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint32]),

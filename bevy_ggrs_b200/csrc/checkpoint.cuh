@@ -22,6 +22,15 @@
 // block bad.  A bad block sets its blob's error word and writes nothing.  Otherwise every thread expands its row of
 // every vector into the scratch image, canonical as above.  Once k_frame_digest has verified every scratch image,
 // k_ckpt_commit copies each to its engine's image 0 and restored ring slot, in one launch over the same table.
+//
+// Checkpoint deltas (bgr_checkpoint_save_delta / bgr_checkpoint_restore_delta) are instances of the same kernels:
+//   k_ckpt_measure_delta / k_ckpt_pack_delta read each block's base tile and row count from the parallel per-image
+//            array CkptParams::base, canonicalise both tiles in registers and code canon(target) XOR canon(base);
+//   k_ckpt_unpack_delta expands each block onto the scratch image that already holds the decoded (canonical) base,
+//            zero past the base's blocks, XORs, and refuses a result that is not canonical: a non-zero word of a row that
+//            does not exist or lacks the column, a mask byte of a row that does not exist, a presence bit the
+//            registration lacks, or bits past an element's bytes.
+// The plain kernels are the <false> instances of the same bodies and compile to the code they had before.
 #pragma once
 #include "frame_digest.cuh"
 
@@ -46,6 +55,13 @@ __host__ __device__ inline uint32_t ckpt_max_block_words(uint32_t words) {
     return ckpt_kind_words(words) + words * kTileRows + kCkptMaskWords;
 }
 
+// The base of one image of a delta's table: its image and row count
+struct CkptBase {
+    const uint8_t* img;
+    uint32_t rows, reserved;
+};
+static_assert(sizeof(CkptBase) == 16, "CkptBase layout");
+
 struct CkptParams {
     const ImageEntry* images;            // the image table (restore: the scratch images written)
     uint32_t n_images;
@@ -58,7 +74,24 @@ struct CkptParams {
     const unsigned long long* offsets;   // [blocks + 1] (restore: bytes into the concatenated payloads of every blob)
     uint32_t* payload;
     unsigned int* err;                   // restore: [n_images] each blob's lowest bad block (0xFFFFFFFF: none)
+    const CkptBase* base;                // delta save: [n_images] each image's base
 };
+
+// A delta's base tile of this thread's block, and the thread's canonical base mask byte (both zero without a delta)
+struct CkptBaseTile {
+    const uint8_t* tb;
+    uint32_t m;
+};
+template <bool DELTA>
+__device__ __forceinline__ CkptBaseTile ckpt_base_tile(const CkptParams& p, const ImageEntry& im, uint32_t t) {
+    if constexpr (DELTA) {
+        const CkptBase b = p.base[&im - p.images];
+        const uint8_t* tb = b.img + size_t(t) * tile_bytes_of(p.words);
+        return CkptBaseTile{tb, diff_mask_tile(tb, p.words, t * kTileRows + threadIdx.x, b.rows)};
+    } else {
+        return CkptBaseTile{nullptr, 0u};
+    }
+}
 
 // thread threadIdx.x's canonical word of plane `plane` (m: its canonical mask byte)
 __device__ __forceinline__ uint32_t ckpt_word(const uint8_t* tile, uint32_t plane, uint32_t m, uint32_t absent) {
@@ -67,13 +100,20 @@ __device__ __forceinline__ uint32_t ckpt_word(const uint8_t* tile, uint32_t plan
 }
 
 // Vector v of the tile for this thread: a canonical word, or the mask plane's u32 (s_mask holds the canonical bytes).
-__device__ __forceinline__ uint32_t ckpt_value(const CkptParams& p, const uint8_t* tile, uint32_t v, uint32_t m,
-                                               const uint32_t* s_mask) {
-    if (v < p.words) return ckpt_word(tile, v, m, p.plane_absent[v]);
+// A delta's is the XOR with the base tile's (s_mask then holds the XOR of both canonical mask bytes).
+template <bool DELTA>
+__device__ __forceinline__ uint32_t ckpt_value(const CkptParams& p, const uint8_t* tile, const CkptBaseTile& bt, uint32_t v,
+                                               uint32_t m, const uint32_t* s_mask) {
+    if (v < p.words) {
+        uint32_t x = ckpt_word(tile, v, m, p.plane_absent[v]);
+        if constexpr (DELTA) x ^= ckpt_word(bt.tb, v, bt.m, p.plane_absent[v]);
+        return x;
+    }
     return threadIdx.x < kCkptMaskWords ? s_mask[threadIdx.x] : 0u;
 }
 
-__global__ void __launch_bounds__(kTileRows) k_ckpt_measure(const __grid_constant__ CkptParams p) {
+template <bool DELTA>
+__device__ __forceinline__ void ckpt_measure(const CkptParams& p) {
     __shared__ uint32_t s_mask[kCkptMaskWords];
     __shared__ uint32_t s_first;
     const uint32_t tile = blockIdx.x;
@@ -81,13 +121,14 @@ __global__ void __launch_bounds__(kTileRows) k_ckpt_measure(const __grid_constan
     const uint32_t t = tile - im.first_block;
     const uint8_t* tb = im.img + size_t(t) * tile_bytes_of(p.words);
     const uint32_t m = diff_mask_tile(tb, p.words, t * kTileRows + threadIdx.x, im.rows);
-    reinterpret_cast<uint8_t*>(s_mask)[threadIdx.x] = uint8_t(m);
+    const CkptBaseTile bt = ckpt_base_tile<DELTA>(p, im, t);
+    reinterpret_cast<uint8_t*>(s_mask)[threadIdx.x] = uint8_t(m ^ bt.m);
     uint32_t len = ckpt_kind_words(p.words);  // thread 0's
     for (uint32_t v = 0; v <= p.words; ++v) {
         const uint32_t n = ckpt_elems(v, p.words);
         const bool in = threadIdx.x < n;
         __syncthreads();  // s_mask is complete; s_first of the previous vector has been read
-        const uint32_t x = ckpt_value(p, tb, v, m, s_mask);
+        const uint32_t x = ckpt_value<DELTA>(p, tb, bt, v, m, s_mask);
         if (threadIdx.x == 0) s_first = x;
         __syncthreads();
         const bool eq = __syncthreads_and(!in || x == s_first);
@@ -100,6 +141,9 @@ __global__ void __launch_bounds__(kTileRows) k_ckpt_measure(const __grid_constan
     }
     if (threadIdx.x == 0) p.lens[tile] = len * 4u;
 }
+
+__global__ void __launch_bounds__(kTileRows) k_ckpt_measure(const __grid_constant__ CkptParams p) { ckpt_measure<false>(p); }
+__global__ void __launch_bounds__(kTileRows) k_ckpt_measure_delta(const __grid_constant__ CkptParams p) { ckpt_measure<true>(p); }
 
 // offsets[i] = sum of lens[0 .. i), offsets[n_tiles] = the total, in u64
 __global__ void __launch_bounds__(kCkptScanBlock) k_ckpt_scan(const unsigned int* __restrict__ lens, uint32_t n_tiles,
@@ -130,7 +174,8 @@ __global__ void __launch_bounds__(kCkptScanBlock) k_ckpt_scan(const unsigned int
     if (threadIdx.x == 0) offsets[n_tiles] = carry;
 }
 
-__global__ void __launch_bounds__(kTileRows) k_ckpt_pack(const __grid_constant__ CkptParams p) {
+template <bool DELTA>
+__device__ __forceinline__ void ckpt_pack(const CkptParams& p) {
     __shared__ uint32_t s_mask[kCkptMaskWords];
     __shared__ uint32_t s_warp[kTileRows / 32u];
     const uint32_t tile = blockIdx.x, lane = threadIdx.x & 31u, warp = threadIdx.x >> 5;
@@ -138,7 +183,8 @@ __global__ void __launch_bounds__(kTileRows) k_ckpt_pack(const __grid_constant__
     const uint32_t t = tile - im.first_block;
     const uint8_t* tb = im.img + size_t(t) * tile_bytes_of(p.words);
     const uint32_t m = diff_mask_tile(tb, p.words, t * kTileRows + threadIdx.x, im.rows);
-    reinterpret_cast<uint8_t*>(s_mask)[threadIdx.x] = uint8_t(m);
+    const CkptBaseTile bt = ckpt_base_tile<DELTA>(p, im, t);
+    reinterpret_cast<uint8_t*>(s_mask)[threadIdx.x] = uint8_t(m ^ bt.m);
     const uint8_t* kinds = p.kinds + size_t(tile) * (p.words + 1u);
     uint32_t* out = p.payload + (im.out_off + p.offsets[tile] - p.offsets[im.first_block]) / 4u;
     const uint32_t kw = ckpt_kind_words(p.words);
@@ -153,7 +199,7 @@ __global__ void __launch_bounds__(kTileRows) k_ckpt_pack(const __grid_constant__
         const uint32_t n = ckpt_elems(v, p.words), kind = kinds[v];
         const bool in = threadIdx.x < n;
         __syncthreads();  // s_mask is complete; s_warp of the previous vector has been read
-        const uint32_t x = ckpt_value(p, tb, v, m, s_mask);
+        const uint32_t x = ckpt_value<DELTA>(p, tb, bt, v, m, s_mask);
         if (kind == kCkptConst) {
             if (threadIdx.x == 0) out[pos] = x;
             pos += 1u;
@@ -180,8 +226,12 @@ __global__ void __launch_bounds__(kTileRows) k_ckpt_pack(const __grid_constant__
     }
 }
 
+__global__ void __launch_bounds__(kTileRows) k_ckpt_pack(const __grid_constant__ CkptParams p) { ckpt_pack<false>(p); }
+__global__ void __launch_bounds__(kTileRows) k_ckpt_pack_delta(const __grid_constant__ CkptParams p) { ckpt_pack<true>(p); }
+
 // dynamic shared memory: (words + 1) u32, the first body word of each vector
-__global__ void __launch_bounds__(kTileRows) k_ckpt_unpack(const __grid_constant__ CkptParams p) {
+template <bool DELTA>
+__device__ __forceinline__ void ckpt_unpack(const CkptParams& p) {
     extern __shared__ uint32_t s_start[];
     __shared__ uint32_t s_mask[kCkptMaskWords];
     __shared__ uint32_t s_bad;
@@ -232,24 +282,37 @@ __global__ void __launch_bounds__(kTileRows) k_ckpt_unpack(const __grid_constant
         return blk[start + n / 32u + rank];
     };
     uint8_t* tb = const_cast<uint8_t*>(im.img) + size_t(t) * tile_bytes_of(p.words);
-    const uint32_t mw = element(p.words);
+    uint32_t mw = element(p.words);
+    if constexpr (DELTA)  // the base's canonical mask bytes, read before any thread writes its row's
+        if (threadIdx.x < kCkptMaskWords) mw ^= reinterpret_cast<const uint32_t*>(tb + size_t(p.words) * kPlaneBytes)[threadIdx.x];
     if (threadIdx.x < kCkptMaskWords) s_mask[threadIdx.x] = mw;
     __syncthreads();
     const uint32_t mb = reinterpret_cast<const uint8_t*>(s_mask)[threadIdx.x];
-    const uint32_t m = (t * kTileRows + threadIdx.x < im.rows && (mb & 1u)) ? mb : 0u;
-    if (__syncthreads_or(m & ~p.mask_bits)) {  // a presence bit of a column this registration does not have
+    const bool exists = t * kTileRows + threadIdx.x < im.rows && (mb & 1u);
+    const uint32_t m = exists ? mb : 0u;
+    // a presence bit of a column this registration does not have (a delta: also a mask byte of a row that does not exist)
+    if (__syncthreads_or((m & ~p.mask_bits) | (DELTA && !exists ? mb : 0u))) {
         if (threadIdx.x == 0) atomicMin(err, t);
         return;
     }
     tb[size_t(p.words) * kPlaneBytes + threadIdx.x] = uint8_t(m);
     uint32_t stray = 0;   // bits past a sub-word element's end: no digest covers them, so they are refused here
     for (uint32_t v = 0; v < p.words; ++v) {
-        const uint32_t x = (m && !(m & p.plane_absent[v])) ? element(v) : 0u;
-        stray |= x & p.plane_pad[v];
+        uint32_t x;
+        if constexpr (DELTA) {  // the base word XOR the delta's; a non-zero word of a row that lacks the column is refused
+            x = element(v) ^ *reinterpret_cast<const uint32_t*>(tb + size_t(v) * kPlaneBytes + threadIdx.x * 4u);
+            stray |= (m && !(m & p.plane_absent[v])) ? x & p.plane_pad[v] : x;
+        } else {
+            x = (m && !(m & p.plane_absent[v])) ? element(v) : 0u;
+            stray |= x & p.plane_pad[v];
+        }
         *reinterpret_cast<uint32_t*>(tb + size_t(v) * kPlaneBytes + threadIdx.x * 4u) = x;
     }
     if (__syncthreads_or(stray != 0u) && threadIdx.x == 0) atomicMin(err, t);
 }
+
+__global__ void __launch_bounds__(kTileRows) k_ckpt_unpack(const __grid_constant__ CkptParams p) { ckpt_unpack<false>(p); }
+__global__ void __launch_bounds__(kTileRows) k_ckpt_unpack_delta(const __grid_constant__ CkptParams p) { ckpt_unpack<true>(p); }
 
 // Block b copies tile b of the table's (verified) scratch images to both destinations of its image, dst[2i] and
 // dst[2i + 1]: the engine's image 0 and its restored ring slot.  16-byte units (tile_bytes is a multiple of 16).

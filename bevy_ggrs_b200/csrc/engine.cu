@@ -3147,16 +3147,24 @@ static std::vector<uint32_t> plane_pad(const bgr_engine* e) {
 // host.
 
 // One image to encode.  The caller sets img, order_base and the header (checkpoint_header); encode_measure adds
-// active, digest_root, payload_bytes and the offsets; encode_pack writes the blob to dst.
+// active, digest_root, payload_bytes and the offsets; encode_pack writes the blob to dst.  A checkpoint delta also sets
+// base and base_rows (the image it is coded against; h.n_blocks then covers both frames' rows) and `delta`, the header
+// encode_pack writes in place of h, which the caller completes from h after encode_measure.
 struct EncodeImage {
     const uint8_t* img = nullptr;
     unsigned long long order_base = 0;
     bgr_checkpoint_header h{};
     std::vector<uint64_t> offsets;
     uint8_t* dst = nullptr;
+    const uint8_t* base = nullptr;
+    uint32_t base_rows = 0;
+    const bgr_checkpoint_delta_header* delta = nullptr;
 };
 
-static size_t blob_bytes(const EncodeImage& x) { return checkpoint_prefix(x.h.n_blocks) + x.h.payload_bytes; }
+static size_t blob_prefix(const EncodeImage& x) {
+    return x.delta ? checkpoint_delta_prefix(x.h.n_blocks) : checkpoint_prefix(x.h.n_blocks);
+}
+static size_t blob_bytes(const EncodeImage& x) { return blob_prefix(x) + x.h.payload_bytes; }
 static size_t align8(size_t v) { return (v + 7u) & ~size_t(7); }
 static size_t align16(size_t v) { return (v + 15u) & ~size_t(15); }
 
@@ -3180,13 +3188,17 @@ static bgr_checkpoint_header checkpoint_header(const bgr_engine* e, int32_t fram
 }
 
 // The images of one encoding and the device memory it uses (allocated by the first call that needs it, freed with the
-// encoder).  `e` gives the stream, the word planes and the columns, which every image's engine shares.
+// encoder).  `e` gives the stream, the word planes and the columns, which every image's engine shares.  `delta`: every
+// image is a checkpoint delta (k_ckpt_measure_delta / k_ckpt_pack_delta over the parallel array of bases).
 struct ImageEncoder {
     bgr_engine* e = nullptr;
+    bool delta = false;
     std::vector<EncodeImage> im;
     std::vector<ImageEntry> table;
     uint32_t blocks = 0;
     DeviceBuffer<ImageEntry> d_table;
+    std::vector<CkptBase> bases;  // delta: [images] each image's base
+    DeviceBuffer<CkptBase> d_base;
     DeviceBuffer<uint32_t> d_absent, d_out;
     DeviceBuffer<uint8_t> d_kinds;
     DeviceBuffer<unsigned int> d_lens;
@@ -3228,7 +3240,16 @@ static int encode_measure(ImageEncoder& x) {
         x.p.kinds = x.d_kinds.get();
         x.p.lens = x.d_lens.get();
         x.p.offsets = x.d_offsets.get();
-        k_ckpt_measure<<<x.blocks, kTileRows, 0, e->stream>>>(x.p);
+        if (x.delta) {
+            x.bases.resize(n);
+            for (uint32_t i = 0; i < n; ++i) x.bases[i] = CkptBase{x.im[i].base, x.im[i].base_rows, 0u};
+            CUDA_TRY(x.d_base.ensure(n));
+            CUDA_TRY(cudaMemcpyAsync(x.d_base.get(), x.bases.data(), sizeof(CkptBase) * n, cudaMemcpyHostToDevice, e->stream));
+            x.p.base = x.d_base.get();
+            k_ckpt_measure_delta<<<x.blocks, kTileRows, 0, e->stream>>>(x.p);
+        } else {
+            k_ckpt_measure<<<x.blocks, kTileRows, 0, e->stream>>>(x.p);
+        }
         k_ckpt_scan<<<1, kCkptScanBlock, 0, e->stream>>>(x.d_lens.get(), x.blocks, x.d_offsets.get());
         e->launches += 2;
         CUDA_TRY(cudaGetLastError());
@@ -3243,7 +3264,9 @@ static int encode_measure(ImageEncoder& x) {
         const size_t nb = m.h.n_blocks;
         m.h.active = 0;
         for (size_t b = 0; b < nb; ++b) m.h.active += x.active[t.first_block + b];
-        m.h.digest_root = bgr_seahash(nb ? &x.digest[size_t(t.first_block) * per] : nullptr, nb * per * sizeof(uint64_t));
+        // over the image's own blocks (a delta's blocks past its rows digest to zero words and are not part of its root)
+        const size_t own = e->tiles_for(m.h.rows);
+        m.h.digest_root = bgr_seahash(own ? &x.digest[size_t(t.first_block) * per] : nullptr, own * per * sizeof(uint64_t));
         m.offsets.resize(nb + 1u);
         for (size_t b = 0; b <= nb; ++b) m.offsets[b] = x.offsets[t.first_block + b] - x.offsets[t.first_block];
         m.h.payload_bytes = m.offsets[nb];
@@ -3259,7 +3282,7 @@ static int encode_pack(ImageEncoder& x) {
     struct Run { size_t first, end, base; };
     std::vector<Run> runs;
     size_t out_bytes = 0;
-    auto payload_at = [&](size_t i) { return x.im[i].dst + checkpoint_prefix(x.im[i].h.n_blocks); };
+    auto payload_at = [&](size_t i) { return x.im[i].dst + blob_prefix(x.im[i]); };
     for (size_t i = 0; i < n; ++i) {
         if (i == 0 || x.im[i].dst != x.im[i - 1].dst + align8(blob_bytes(x.im[i - 1]))) {
             if (!runs.empty()) out_bytes += size_t(x.im[i - 1].dst + blob_bytes(x.im[i - 1]) - payload_at(runs.back().first));
@@ -3273,7 +3296,8 @@ static int encode_pack(ImageEncoder& x) {
         CUDA_TRY(x.d_out.ensure(std::max<size_t>(1, out_bytes / 4u)));
         CUDA_TRY(cudaMemcpyAsync(x.d_table.get(), x.table.data(), sizeof(ImageEntry) * n, cudaMemcpyHostToDevice, e->stream));
         x.p.payload = x.d_out.get();
-        k_ckpt_pack<<<x.blocks, kTileRows, 0, e->stream>>>(x.p);
+        if (x.delta) k_ckpt_pack_delta<<<x.blocks, kTileRows, 0, e->stream>>>(x.p);
+        else k_ckpt_pack<<<x.blocks, kTileRows, 0, e->stream>>>(x.p);
         e->launches += 1;
         CUDA_TRY(cudaGetLastError());
         // one copy: straight into the caller's memory for one run, else into host staging that is then scattered to the
@@ -3292,8 +3316,9 @@ static int encode_pack(ImageEncoder& x) {
     }
     for (size_t i = 0; i < n; ++i) {  // the headers, the offsets and the zero padding between blobs of a run
         EncodeImage& m = x.im[i];
-        std::memcpy(m.dst, &m.h, sizeof m.h);
-        std::memcpy(m.dst + sizeof m.h, m.offsets.data(), sizeof(uint64_t) * m.offsets.size());
+        const size_t head = m.delta ? sizeof *m.delta : sizeof m.h;
+        std::memcpy(m.dst, m.delta ? static_cast<const void*>(m.delta) : static_cast<const void*>(&m.h), head);
+        std::memcpy(m.dst + head, m.offsets.data(), sizeof(uint64_t) * m.offsets.size());
         if (i + 1 < n && x.im[i + 1].dst == m.dst + align8(blob_bytes(m)))
             std::memset(m.dst + blob_bytes(m), 0, align8(blob_bytes(m)) - blob_bytes(m));
     }
@@ -3325,6 +3350,67 @@ BGR_API int bgr_checkpoint_save(bgr_engine* e, int32_t frame, void* dst, size_t 
     const size_t need = blob_bytes(m);
     *bytes = need;
     if (dst_cap < need) return fail(BGR_ERR_CAPACITY, "the checkpoint needs " + std::to_string(need) + " bytes");
+    m.dst = static_cast<uint8_t*>(dst);
+    return encode_pack(x);
+}
+
+// A delta of `frame` against `base_frame`: the encoder's delta instances over the target's slot image, each block coded
+// against the base slot image's (the blocks past one frame's rows against zeros), and the base's root from its own
+// frame digest.
+BGR_API int bgr_checkpoint_save_delta(bgr_engine* e, int32_t frame, int32_t base_frame, void* dst, size_t dst_cap,
+                                      size_t* bytes, int32_t* found) {
+    if (!bytes || !found) return fail(BGR_ERR_INVALID_ARGUMENT, "null argument");
+    int rc = checkpoint_args(e);
+    if (rc == BGR_OK) rc = drain(e);
+    if (rc != BGR_OK) return rc;
+    uint32_t slot = 0, base_slot = 0;
+    if (!p2p_slot(e, frame, &slot) || !p2p_slot(e, base_frame, &base_slot)) { *found = 0; return BGR_OK; }
+    *found = 1;
+    const uint32_t rows = e->st.slot_rows[slot], base_rows = e->st.slot_rows[base_slot];
+    const uint32_t n_blocks = e->tiles_for(std::max(rows, base_rows));
+    if (!dst) {
+        *bytes = checkpoint_delta_prefix(n_blocks) + size_t(n_blocks) * ckpt_max_block_words(e->words) * 4u;
+        return BGR_OK;
+    }
+    std::vector<uint64_t> base_words;
+    uint64_t base_root = 0, base_active = 0;
+    rc = digest_image(e, e->image(base_slot + 1), base_rows, &base_words, &base_root, &base_active);
+    if (rc != BGR_OK) return rc;
+    bgr_checkpoint_delta_header dh{};
+    ImageEncoder x;
+    x.e = e;
+    x.delta = true;
+    x.im.resize(1);
+    EncodeImage& m = x.im[0];
+    m.img = e->image(slot + 1);
+    m.order_base = e->cfg.order_base;
+    m.h = checkpoint_header(e, frame, rows, e->st.slot_elapsed_ns[slot], e->st.slot_rng[slot]);
+    m.h.n_blocks = n_blocks;
+    m.base = e->image(base_slot + 1);
+    m.base_rows = base_rows;
+    m.delta = &dh;
+    rc = encode_measure(x);
+    if (rc != BGR_OK) return rc;
+    dh.magic = BGR_CHECKPOINT_DELTA_MAGIC;
+    dh.version = BGR_CHECKPOINT_DELTA_VERSION;
+    dh.layout = m.h.layout;
+    dh.frame = frame;
+    dh.rows = rows;
+    dh.base_frame = base_frame;
+    dh.base_rows = base_rows;
+    dh.words = m.h.words;
+    dh.n_blocks = n_blocks;
+    dh.n_columns = m.h.n_columns;
+    dh.fps = m.h.fps;
+    dh.active = m.h.active;
+    dh.elapsed_ns = m.h.elapsed_ns;
+    std::memcpy(dh.rng, m.h.rng, sizeof dh.rng);
+    dh.digest_root = m.h.digest_root;
+    dh.base_root = base_root;
+    dh.payload_bytes = m.h.payload_bytes;
+    const size_t need = blob_bytes(m);
+    *bytes = need;
+    if (dst_cap < need) return fail(BGR_ERR_CAPACITY, "the checkpoint delta needs " + std::to_string(need) + " bytes");
     m.dst = static_cast<uint8_t*>(dst);
     return encode_pack(x);
 }
@@ -3521,6 +3607,112 @@ BGR_API int bgr_checkpoint_restore(bgr_engine* e, const void* blob, size_t bytes
     size_t bad = 0;
     rc = restore_decode(r, x, nullptr, &bad);
     if (rc != BGR_OK) return rc;
+    return restore_commit(r, x, &bad);
+}
+
+// ---- restore of a delta: the base decoded and verified as bgr_checkpoint_restore does, the delta applied onto its
+// scratch image (k_ckpt_unpack_delta) and the target verified, then committed as a checkpoint of the target ----
+
+// Applies the host-checked delta `dh` (offsets `off`, payload at `payload`) onto x's scratch image, which restore_decode
+// filled with the verified base, and verifies the target's digest root and active rows.  On success x describes the
+// target for restore_commit: its table (in a new `meta`) holds the scratch image with the target's rows.
+static int restore_delta_decode(bgr_engine* e, const bgr_checkpoint_delta_header& dh, const std::vector<uint64_t>& off,
+                                const uint8_t* payload, uint32_t base_blocks, RestorePass& x) {
+    const uint32_t per = uint32_t(e->cols.size()) + 1u, own = e->tiles_for(dh.rows);
+    unsigned int err = 0xFFFFFFFFu;
+    std::vector<uint64_t> digest;
+    std::vector<unsigned int> active;
+    x.table.assign(1, ImageEntry{x.scratch.get(), e->cfg.order_base, 0ull, dh.rows, 0u});
+    if (dh.n_blocks) {
+        const size_t smem = sizeof(uint32_t) * (e->words + 1u);
+        if (smem + sizeof(uint32_t) * (kCkptMaskWords + 1u) > 48u * 1024u)
+            return fail(BGR_ERR_UNSUPPORTED, "bgr_checkpoint_restore supports at most 12000 word planes");
+        const std::vector<uint32_t> absent = plane_absent(e), pad = plane_pad(e);
+        // one upload, laid out as restore_decode's: image table, offsets, error word, planes, then the commit's pointers
+        const size_t o_off = align16(sizeof(ImageEntry)), o_err = align16(o_off + sizeof(uint64_t) * off.size());
+        const size_t o_absent = align16(o_err + sizeof(unsigned int)), o_pad = align16(o_absent + sizeof(uint32_t) * absent.size());
+        const size_t dst_off = align16(o_pad + sizeof(uint32_t) * pad.size()), meta_bytes = dst_off + sizeof(uint8_t*) * 2u;
+        DeviceBuffer<uint8_t> meta, d_payload;
+        CUDA_TRY(meta.ensure(meta_bytes));
+        CUDA_TRY(d_payload.ensure(std::max<uint64_t>(4, dh.payload_bytes)));
+        std::vector<uint8_t> h(meta_bytes);
+        std::memcpy(h.data(), x.table.data(), sizeof(ImageEntry));
+        std::memcpy(h.data() + o_off, off.data(), sizeof(uint64_t) * off.size());
+        std::memcpy(h.data() + o_err, &err, sizeof err);
+        std::memcpy(h.data() + o_absent, absent.data(), sizeof(uint32_t) * absent.size());
+        std::memcpy(h.data() + o_pad, pad.data(), sizeof(uint32_t) * pad.size());
+        // the blocks past the base's XOR against zeros
+        if (dh.n_blocks > base_blocks)
+            CUDA_TRY(cudaMemsetAsync(x.scratch.get() + size_t(base_blocks) * e->tile_bytes, 0,
+                                     size_t(dh.n_blocks - base_blocks) * e->tile_bytes, e->stream));
+        CUDA_TRY(cudaMemcpyAsync(d_payload.get(), payload, dh.payload_bytes, cudaMemcpyHostToDevice, e->stream));
+        CUDA_TRY(cudaMemcpyAsync(meta.get(), h.data(), meta_bytes, cudaMemcpyHostToDevice, e->stream));
+        uint8_t* d = meta.get();
+        CkptParams p{};
+        p.images = reinterpret_cast<const ImageEntry*>(d);
+        p.n_images = 1;
+        p.words = e->words;
+        p.plane_absent = reinterpret_cast<const uint32_t*>(d + o_absent);
+        p.plane_pad = reinterpret_cast<const uint32_t*>(d + o_pad);
+        p.mask_bits = 1u;
+        for (const Column& c : e->cols) p.mask_bits |= c.absent;
+        p.offsets = reinterpret_cast<const unsigned long long*>(d + o_off);
+        p.payload = reinterpret_cast<uint32_t*>(d_payload.get());
+        p.err = reinterpret_cast<unsigned int*>(d + o_err);
+        k_ckpt_unpack_delta<<<dh.n_blocks, kTileRows, smem, e->stream>>>(p);
+        e->launches += 1;
+        CUDA_TRY(cudaGetLastError());
+        int rc = digest_launch(e, p.images, 1u, own, &digest, &active);
+        if (rc != BGR_OK) return rc;
+        CUDA_TRY(cudaMemcpyAsync(&err, p.err, sizeof err, cudaMemcpyDeviceToHost, e->stream));
+        CUDA_TRY(cudaStreamSynchronize(e->stream));  // `h` and the payload are freed below
+        x.meta = std::move(meta);
+        x.dst_off = dst_off;
+    }
+    x.blocks = own;
+    if (err != 0xFFFFFFFFu)
+        return fail(BGR_ERR_INVALID_ARGUMENT, "checkpoint delta block " + std::to_string(err) +
+                                                  ": a bad kind byte or padding, its kinds and bitmaps imply another length than its "
+                                                  "offsets, or the target is not canonical (a non-zero word or mask byte of a row that "
+                                                  "does not exist or lacks the column, a mask bit this registration does not use, or "
+                                                  "bits past a column's element bytes)");
+    uint64_t rows_alive = 0;
+    for (uint32_t k = 0; k < own; ++k) rows_alive += active[k];
+    const uint64_t root = bgr_seahash(own ? digest.data() : nullptr, size_t(own) * per * sizeof(uint64_t));
+    if (root != dh.digest_root || rows_alive != dh.active)
+        return fail(BGR_ERR_INVALID_ARGUMENT, "the decoded target's digest or active row count differs from the checkpoint delta "
+                                              "header (corrupt payload)");
+    return BGR_OK;
+}
+
+BGR_API int bgr_checkpoint_restore_delta(bgr_engine* e, const void* base, size_t base_bytes, const void* delta,
+                                         size_t delta_bytes) {
+    std::vector<RestoreBlob> r(1);
+    int rc = restore_check(e, base, base_bytes, &r[0]);
+    if (rc != BGR_OK) return rc;
+    if (!delta) return fail(BGR_ERR_INVALID_ARGUMENT, "null argument");
+    bgr_checkpoint_delta_header dh;
+    std::vector<uint64_t> off;
+    std::string err;
+    rc = checkpoint_delta_check(ckpt_target(e), r[0].h, delta, delta_bytes, &dh, &off, &err);
+    if (rc != BGR_OK) return fail(rc, err);
+    RestorePass x;
+    CUDA_TRY(x.scratch.ensure(std::max<size_t>(1, size_t(dh.n_blocks) * e->tile_bytes)));  // both frames' blocks
+    size_t bad = 0;
+    rc = restore_decode(r, x, nullptr, &bad);
+    if (rc != BGR_OK) return rc;
+    rc = restore_delta_decode(e, dh, off, static_cast<const uint8_t*>(delta) + checkpoint_delta_prefix(dh.n_blocks),
+                              r[0].h.n_blocks, x);
+    if (rc != BGR_OK) return rc;
+    // commit the target as bgr_checkpoint_restore commits a checkpoint of it
+    bgr_checkpoint_header& h = r[0].h;
+    h.frame = dh.frame;
+    h.rows = dh.rows;
+    h.n_blocks = e->tiles_for(dh.rows);
+    h.active = dh.active;
+    h.elapsed_ns = dh.elapsed_ns;
+    std::memcpy(h.rng, dh.rng, sizeof h.rng);
+    h.digest_root = dh.digest_root;
     return restore_commit(r, x, &bad);
 }
 

@@ -412,6 +412,24 @@ class Engine:
         """Replace the world with a checkpoint's; the ring then holds the checkpoint's frame alone."""
         self._check(self._lib.bgr_checkpoint_restore(self._h, blob, len(blob)))
 
+    def checkpoint_delta(self, frame: int, base_frame: int) -> Optional[bytes]:
+        """The checkpoint delta of ``frame`` against ``base_frame`` (include/bevy_ggrs_b200.h "checkpoint deltas"): the
+        blocks of the two frames' canonical images XORed and coded as a checkpoint's.  Both frames queued or retained;
+        None if either is not.  ``restore_delta(checkpoint(base_frame), delta)`` restores ``frame``."""
+        size, found = C.c_size_t(), C.c_int32()
+        self._check(self._lib.bgr_checkpoint_save_delta(self._h, frame, base_frame, None, 0, C.byref(size), C.byref(found)))
+        if not found.value:
+            return None
+        out = np.empty(size.value, np.uint8)   # an upper bound: the call reports the exact size
+        self._check(self._lib.bgr_checkpoint_save_delta(self._h, frame, base_frame, out.ctypes.data, out.size, C.byref(size),
+                                                        C.byref(found)))
+        return out[: size.value].tobytes()
+
+    def restore_delta(self, base: bytes, delta: bytes) -> None:
+        """Replace the world with a delta's target frame, given the full checkpoint the delta was written against; the
+        engine ends exactly as ``restore`` of the target's full checkpoint leaves it."""
+        self._check(self._lib.bgr_checkpoint_restore_delta(self._h, base, len(base), delta, len(delta)))
+
     # ---- schedules ----
     def save_world(self) -> Tuple[int, int]:
         cs = capi.bgr_checksum()

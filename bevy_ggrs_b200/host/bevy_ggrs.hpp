@@ -432,9 +432,7 @@ public:
     // holds neither a queued nor a retained snapshot of the frame.
     std::vector<uint8_t> checkpoint(ggrs::Frame frame) {
         checkpoint_args();
-        auto rs = res_store_.find(frame);
-        if (!res_order_.empty() && rs == res_store_.end())
-            throw Panic(BGR_ERR_NO_SNAPSHOT, "the App holds no resource snapshot of frame " + std::to_string(frame));
+        auto rs = resource_snapshot(frame);
         size_t bytes = 0;
         int32_t found = 0;
         check(bgr_checkpoint_save(engine_, frame, nullptr, 0, &bytes, &found));
@@ -442,17 +440,23 @@ public:
         std::vector<uint8_t> blob(bytes);  // an upper bound; the call reports the exact size
         check(bgr_checkpoint_save(engine_, frame, blob.data(), blob.size(), &bytes, &found));
         blob.resize(bytes);
-        auto put = [&blob](uint32_t v) { const uint8_t* p = reinterpret_cast<const uint8_t*>(&v); blob.insert(blob.end(), p, p + 4); };
-        put(uint32_t(res_order_.size()));
-        for (const auto& r : res_order_) {
-            auto it = rs->second.find(r.first);
-            const bool present = it != rs->second.end();
-            put(present ? 1u : 0u);
-            put(present ? uint32_t(it->second.size()) : 0u);
-            if (!present) continue;
-            blob.insert(blob.end(), it->second.begin(), it->second.end());
-            blob.resize(blob.size() + (4 - it->second.size() % 4) % 4, 0);
-        }
+        put_resources(rs, &blob);
+        return blob;
+    }
+    // The engine's checkpoint delta of `frame` against `base_frame` (bgr_checkpoint_save_delta) followed by the App's
+    // resources of `frame`, in checkpoint()'s section.  Refused where checkpoint(frame) is; empty: the engine holds either
+    // frame neither queued nor retained.
+    std::vector<uint8_t> checkpoint_delta(ggrs::Frame frame, ggrs::Frame base_frame) {
+        checkpoint_args();
+        auto rs = resource_snapshot(frame);
+        size_t bytes = 0;
+        int32_t found = 0;
+        check(bgr_checkpoint_save_delta(engine_, frame, base_frame, nullptr, 0, &bytes, &found));
+        if (!found) return {};
+        std::vector<uint8_t> blob(bytes);  // an upper bound; the call reports the exact size
+        check(bgr_checkpoint_save_delta(engine_, frame, base_frame, blob.data(), blob.size(), &bytes, &found));
+        blob.resize(bytes);
+        put_resources(rs, &blob);
         return blob;
     }
     // ---- replays (bgr_replay; INTEGRATION.md "Replays") ----
@@ -578,18 +582,76 @@ public:
         bgr_checkpoint_header h;
         if (blob.size() < sizeof h) throw Panic(BGR_ERR_INVALID_ARGUMENT, "checkpoint truncated: shorter than its header");
         std::memcpy(&h, blob.data(), sizeof h);
-        const uint64_t prefix = sizeof h + 8ull * (uint64_t(h.n_blocks) + 1);
-        if (h.payload_bytes > blob.size() || prefix + h.payload_bytes > blob.size())
-            throw Panic(BGR_ERR_INVALID_ARGUMENT, "checkpoint truncated: no resource section");
-        const size_t engine_bytes = size_t(prefix + h.payload_bytes);
-        size_t at = engine_bytes;
+        const size_t engine_bytes = engine_part(blob, sizeof h, h.n_blocks, h.payload_bytes, "checkpoint");
+        ResourceMap res = take_resources(blob, engine_bytes, "checkpoint");
+        check(bgr_checkpoint_restore(engine_, blob.data(), engine_bytes));
+        set_restored_resources(h.frame, res);
+    }
+
+    // Replaces the world and the App's resources with the target frame of `delta` (from checkpoint_delta()), given the
+    // App checkpoint `base` it was written against.  Both resource sections are checked before the engine restores, so
+    // a refused pair changes nothing.
+    void restore_checkpoint_delta(const std::vector<uint8_t>& base, const std::vector<uint8_t>& delta) {
+        checkpoint_args();
+        bgr_checkpoint_header bh;
+        bgr_checkpoint_delta_header dh;
+        if (base.size() < sizeof bh) throw Panic(BGR_ERR_INVALID_ARGUMENT, "checkpoint truncated: shorter than its header");
+        if (delta.size() < sizeof dh) throw Panic(BGR_ERR_INVALID_ARGUMENT, "checkpoint delta truncated: shorter than its header");
+        std::memcpy(&bh, base.data(), sizeof bh);
+        std::memcpy(&dh, delta.data(), sizeof dh);
+        const size_t base_bytes = engine_part(base, sizeof bh, bh.n_blocks, bh.payload_bytes, "checkpoint");
+        const size_t delta_bytes = engine_part(delta, sizeof dh, dh.n_blocks, dh.payload_bytes, "checkpoint delta");
+        take_resources(base, base_bytes, "checkpoint");
+        ResourceMap res = take_resources(delta, delta_bytes, "checkpoint delta");
+        check(bgr_checkpoint_restore_delta(engine_, base.data(), base_bytes, delta.data(), delta_bytes));
+        set_restored_resources(dh.frame, res);
+    }
+
+private:
+    void checkpoint_args() {
+        finish();
+        if (!host_cols_.empty())
+            throw Panic(BGR_ERR_UNSUPPORTED, "an App with host-side component tables cannot be checkpointed: their values are not plain bytes");
+    }
+    using Resources = std::map<std::type_index, std::vector<uint8_t>>;  // ResourceMap, declared below
+    // the App's resource snapshot of `frame` (end(): none, and none is needed without registered resources)
+    std::map<ggrs::Frame, Resources>::const_iterator resource_snapshot(ggrs::Frame frame) const {
+        auto rs = res_store_.find(frame);
+        if (!res_order_.empty() && rs == res_store_.end())
+            throw Panic(BGR_ERR_NO_SNAPSHOT, "the App holds no resource snapshot of frame " + std::to_string(frame));
+        return rs;
+    }
+    // appends the resource section of snapshot `rs` to `blob`
+    void put_resources(std::map<ggrs::Frame, Resources>::const_iterator rs, std::vector<uint8_t>* blob) const {
+        auto put = [blob](uint32_t v) { const uint8_t* p = reinterpret_cast<const uint8_t*>(&v); blob->insert(blob->end(), p, p + 4); };
+        put(uint32_t(res_order_.size()));
+        for (const auto& r : res_order_) {
+            auto it = rs->second.find(r.first);
+            const bool present = it != rs->second.end();
+            put(present ? 1u : 0u);
+            put(present ? uint32_t(it->second.size()) : 0u);
+            if (!present) continue;
+            blob->insert(blob->end(), it->second.begin(), it->second.end());
+            blob->resize(blob->size() + (4 - it->second.size() % 4) % 4, 0);
+        }
+    }
+    // the bytes of the engine blob at the start of `blob` (`head`: its header's size), which a resource section follows
+    static size_t engine_part(const std::vector<uint8_t>& blob, size_t head, uint32_t n_blocks, uint64_t payload_bytes,
+                              const char* what) {
+        const uint64_t prefix = head + 8ull * (uint64_t(n_blocks) + 1);
+        if (payload_bytes > blob.size() || prefix + payload_bytes > blob.size())
+            throw Panic(BGR_ERR_INVALID_ARGUMENT, std::string(what) + " truncated: no resource section");
+        return size_t(prefix + payload_bytes);
+    }
+    // the resource section of `blob` from byte `at` to its end, checked against the App's registration
+    Resources take_resources(const std::vector<uint8_t>& blob, size_t at, const char* what) const {
         auto take = [&](size_t n) {
-            if (n > blob.size() - at) throw Panic(BGR_ERR_INVALID_ARGUMENT, "checkpoint truncated: its resource section is incomplete");
+            if (n > blob.size() - at) throw Panic(BGR_ERR_INVALID_ARGUMENT, std::string(what) + " truncated: its resource section is incomplete");
             at += n;
             return blob.data() + at - n;
         };
         auto get = [&]() { uint32_t v; std::memcpy(&v, take(4), 4); return v; };
-        if (get() != res_order_.size()) throw Panic(BGR_ERR_INVALID_ARGUMENT, "the checkpoint's resources are not the App's");
+        if (get() != res_order_.size()) throw Panic(BGR_ERR_INVALID_ARGUMENT, std::string("the ") + what + "'s resources are not the App's");
         ResourceMap res;
         for (const auto& r : res_order_) {
             const uint32_t present = get(), n = get();
@@ -602,19 +664,14 @@ public:
             for (uint32_t i = 0; i < (4 - n % 4) % 4; ++i)
                 if (pad[i]) throw Panic(BGR_ERR_INVALID_ARGUMENT, std::string("resource ") + r.first.name() + ": non-zero padding");
         }
-        if (at != blob.size()) throw Panic(BGR_ERR_INVALID_ARGUMENT, "checkpoint overlong: bytes follow its resource section");
-        check(bgr_checkpoint_restore(engine_, blob.data(), engine_bytes));
+        if (at != blob.size()) throw Panic(BGR_ERR_INVALID_ARGUMENT, std::string(what) + " overlong: bytes follow its resource section");
+        return res;
+    }
+    void set_restored_resources(ggrs::Frame frame, const Resources& res) {
         resources_ = res;
         res_store_.clear();
-        if (!res_order_.empty()) res_store_[h.frame] = res;
-        res_frame_ = h.frame;
-    }
-
-private:
-    void checkpoint_args() {
-        finish();
-        if (!host_cols_.empty())
-            throw Panic(BGR_ERR_UNSUPPORTED, "an App with host-side component tables cannot be checkpointed: their values are not plain bytes");
+        if (!res_order_.empty()) res_store_[frame] = res;
+        res_frame_ = frame;
     }
     template <class T> App& register_component(uint32_t strategy) {
         static_assert(std::is_trivially_copyable<T>::value, "only POD components cross the C ABI");

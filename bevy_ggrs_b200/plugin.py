@@ -283,13 +283,30 @@ class App:
         """The checkpoint of a queued or retained frame with the App's resources of that frame; None if the engine
         holds neither.  Refused when the App no longer holds the frame's resource snapshot."""
         self._checkpoint_args()
-        if self._res_registered and frame not in self._res_store:
-            raise capi.BgrError(capi.BGR_ERR_NO_SNAPSHOT, f"the App holds no resource snapshot of frame {frame}")
+        self._check_resource_snapshot(frame)
         blob = self.world.checkpoint(frame)
         if blob is None:
             return None
+        return blob + self._resource_section(frame)
+
+    def checkpoint_delta(self, frame: int, base_frame: int) -> Optional[bytes]:
+        """The engine's checkpoint delta of ``frame`` against ``base_frame`` followed by the App's resources of
+        ``frame``, in the section ``checkpoint`` writes; None if the engine holds either frame neither queued nor
+        retained.  Refused where ``checkpoint(frame)`` is refused."""
+        self._checkpoint_args()
+        self._check_resource_snapshot(frame)
+        delta = self.world.checkpoint_delta(frame, base_frame)
+        if delta is None:
+            return None
+        return delta + self._resource_section(frame)
+
+    def _check_resource_snapshot(self, frame: int) -> None:
+        if self._res_registered and frame not in self._res_store:
+            raise capi.BgrError(capi.BGR_ERR_NO_SNAPSHOT, f"the App holds no resource snapshot of frame {frame}")
+
+    def _resource_section(self, frame: int) -> bytes:
         snap = self._res_store.get(frame, {})
-        out = [blob, struct.pack("<I", len(self._res_registered))]
+        out = [struct.pack("<I", len(self._res_registered))]
         for name in self._res_registered:
             v = snap.get(name)
             out.append(struct.pack("<II", 0 if v is None else 1, 0 if v is None else len(v)))
@@ -297,25 +314,20 @@ class App:
                 out.append(bytes(v) + bytes(-len(v) % 4))
         return b"".join(out)
 
-    def restore_checkpoint(self, blob: bytes) -> None:
-        """Replaces the world and the App's resources with a checkpoint's.  The resource section is checked before the
-        engine restores, so a refused blob changes nothing."""
-        self._checkpoint_args()
-        if len(blob) < capi.C.sizeof(capi.bgr_checkpoint_header):
-            raise capi.BgrError(capi.BGR_ERR_INVALID_ARGUMENT, "checkpoint truncated: shorter than its header")
-        h = capi.bgr_checkpoint_header.from_buffer_copy(blob)
-        at = capi.C.sizeof(h) + 8 * (h.n_blocks + 1) + h.payload_bytes
+    def _parse_resources(self, blob: bytes, at: int, what: str) -> Dict[str, Optional[bytes]]:
+        """The resource section of ``blob`` from byte ``at`` to its end (``what``: "checkpoint" or "checkpoint
+        delta"), checked against the App's registration."""
         res: Dict[str, Optional[bytes]] = {}
 
         def take(n: int) -> bytes:
             nonlocal at
             if at + n > len(blob):
-                raise capi.BgrError(capi.BGR_ERR_INVALID_ARGUMENT, "checkpoint truncated: its resource section is incomplete")
+                raise capi.BgrError(capi.BGR_ERR_INVALID_ARGUMENT, f"{what} truncated: its resource section is incomplete")
             at += n
             return blob[at - n:at]
         (count,) = struct.unpack("<I", take(4))
         if count != len(self._res_registered):
-            raise capi.BgrError(capi.BGR_ERR_INVALID_ARGUMENT, f"the checkpoint holds {count} resources, the App registers "
+            raise capi.BgrError(capi.BGR_ERR_INVALID_ARGUMENT, f"the {what} holds {count} resources, the App registers "
                                                                f"{len(self._res_registered)}")
         for name in self._res_registered:
             present, n = struct.unpack("<II", take(8))
@@ -325,11 +337,43 @@ class App:
             if any(take(-n % 4)):
                 raise capi.BgrError(capi.BGR_ERR_INVALID_ARGUMENT, f"resource {name}: non-zero padding")
         if at != len(blob):
-            raise capi.BgrError(capi.BGR_ERR_INVALID_ARGUMENT, "checkpoint overlong: bytes follow its resource section")
-        self.world.restore(blob[: capi.C.sizeof(h) + 8 * (h.n_blocks + 1) + h.payload_bytes])
+            raise capi.BgrError(capi.BGR_ERR_INVALID_ARGUMENT, f"{what} overlong: bytes follow its resource section")
+        return res
+
+    def restore_checkpoint(self, blob: bytes) -> None:
+        """Replaces the world and the App's resources with a checkpoint's.  The resource section is checked before the
+        engine restores, so a refused blob changes nothing."""
+        self._checkpoint_args()
+        if len(blob) < capi.C.sizeof(capi.bgr_checkpoint_header):
+            raise capi.BgrError(capi.BGR_ERR_INVALID_ARGUMENT, "checkpoint truncated: shorter than its header")
+        h = capi.bgr_checkpoint_header.from_buffer_copy(blob)
+        at = capi.C.sizeof(h) + 8 * (h.n_blocks + 1) + h.payload_bytes
+        res = self._parse_resources(blob, at, "checkpoint")
+        self.world.restore(blob[:at])
+        self._set_restored_resources(h.frame, res)
+
+    def restore_checkpoint_delta(self, base: bytes, delta: bytes) -> None:
+        """Replaces the world and the App's resources with the target frame of ``delta`` (from ``checkpoint_delta``),
+        given the App checkpoint ``base`` it was written against.  Both resource sections are checked before the engine
+        restores, so a refused pair changes nothing."""
+        self._checkpoint_args()
+        if len(base) < capi.C.sizeof(capi.bgr_checkpoint_header):
+            raise capi.BgrError(capi.BGR_ERR_INVALID_ARGUMENT, "checkpoint truncated: shorter than its header")
+        if len(delta) < capi.C.sizeof(capi.bgr_checkpoint_delta_header):
+            raise capi.BgrError(capi.BGR_ERR_INVALID_ARGUMENT, "checkpoint delta truncated: shorter than its header")
+        bh = capi.bgr_checkpoint_header.from_buffer_copy(base)
+        dh = capi.bgr_checkpoint_delta_header.from_buffer_copy(delta)
+        b_at = capi.C.sizeof(bh) + 8 * (bh.n_blocks + 1) + bh.payload_bytes
+        d_at = capi.C.sizeof(dh) + 8 * (dh.n_blocks + 1) + dh.payload_bytes
+        self._parse_resources(base, b_at, "checkpoint")
+        res = self._parse_resources(delta, d_at, "checkpoint delta")
+        self.world.restore_delta(base[:b_at], delta[:d_at])
+        self._set_restored_resources(dh.frame, res)
+
+    def _set_restored_resources(self, frame: int, res: Dict[str, Optional[bytes]]) -> None:
         self.resources = {n: bytearray(v) for n, v in res.items() if v is not None}
-        self._res_store = {h.frame: res} if self._res_registered else {}
-        self._res_frame = h.frame
+        self._res_store = {frame: res} if self._res_registered else {}
+        self._res_frame = frame
 
     # ---- frame resources ----
     def rollback_frame_count(self) -> int:

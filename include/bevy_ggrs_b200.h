@@ -562,6 +562,52 @@ BGR_API int bgr_checkpoint_save(bgr_engine* e, int32_t frame, void* dst, size_t 
  * Device memory for the decoding (a scratch image of the blob's rows) is allocated and freed inside the call. */
 BGR_API int bgr_checkpoint_restore(bgr_engine* e, const void* blob, size_t bytes);
 
+/* ---- checkpoint deltas: a frame encoded against an earlier (or later) frame's checkpoint ----------------------------
+ * Blob: this header, then u64 offsets[n_blocks + 1], then payload_bytes of payload, with the offsets and the block
+ * coding of a checkpoint.  Vector v of block b is canon(target) XOR canon(base) of that block (the mask plane too), with
+ * canon the checkpoint's canonical form; the blocks past one frame's rows XOR against zeros.  An unchanged block codes
+ * as every vector CONST zero.  Kinds follow the checkpoint's rule, so the delta is a pure function of the two frames'
+ * contents: two engines whose digests agree on both frames write byte-identical deltas.  A delta applies to exactly
+ * one base checkpoint (base_frame, base_rows, base_root). */
+#define BGR_CHECKPOINT_DELTA_MAGIC 0x44524742u /* "BGRD" */
+#define BGR_CHECKPOINT_DELTA_VERSION 1u
+typedef struct bgr_checkpoint_delta_header {  /* 120 bytes, no padding */
+    uint32_t magic;          /* BGR_CHECKPOINT_DELTA_MAGIC */
+    uint32_t version;        /* BGR_CHECKPOINT_DELTA_VERSION */
+    uint64_t layout;         /* bgr_frame_digest_header.layout */
+    int32_t frame;           /* the target frame */
+    uint32_t rows;           /* the target's row count */
+    int32_t base_frame;
+    uint32_t base_rows;
+    uint32_t words;
+    uint32_t n_blocks;       /* ceil(max(rows, base_rows) / 512) */
+    uint32_t n_columns;
+    uint32_t fps;
+    uint64_t active;         /* the target's, as in bgr_checkpoint_header */
+    uint64_t elapsed_ns;
+    uint64_t rng[4];
+    uint64_t digest_root;    /* the target's root */
+    uint64_t base_root;      /* the base's root: the checkpoint this delta applies to */
+    uint64_t payload_bytes;
+} bgr_checkpoint_delta_header;
+/* Encodes `frame` against `base_frame` (both queued or retained; *found = 0 if either is not, and nothing runs).
+ * base_frame may be earlier than, later than or equal to frame.  dst == NULL: *bytes = an upper bound (every vector
+ * RAW), nothing runs.  Otherwise BGR_ERR_CAPACITY with *bytes = the exact size if dst_cap is smaller.  Waits for
+ * submitted vectors and leaves their results queued, like bgr_checkpoint_save. */
+BGR_API int bgr_checkpoint_save_delta(bgr_engine* e, int32_t frame, int32_t base_frame, void* dst, size_t dst_cap,
+                                      size_t* bytes, int32_t* found);
+/* Replaces the engine's world with the delta's target frame, given the full checkpoint `base` it was written against.
+ * Both blobs are untrusted and checked in full before anything changes: the base exactly as bgr_checkpoint_restore
+ * checks it (its decoded world must reproduce its root); the delta's magic and version, its layout, fps and words
+ * against the engine's and the base's, base_frame, base_rows and base_root against the base header's, n_blocks, its
+ * length, offsets, kinds and padding.  The target must be canonical (a non-zero word in a row that does not exist or
+ * lacks the column, a presence bit the registration lacks, or bits past an element's bytes are refused) and reproduce
+ * digest_root and active.  Failures return BGR_ERR_INVALID_ARGUMENT, or what bgr_checkpoint_restore returns for
+ * capacity (either frame's rows), un-collected submits or a sharded engine.  A refused call changes nothing observable.
+ * On success the engine is exactly as bgr_checkpoint_restore of the target's full checkpoint leaves it. */
+BGR_API int bgr_checkpoint_restore_delta(bgr_engine* e, const void* base, size_t base_bytes, const void* delta,
+                                         size_t delta_bytes);
+
 /* ---- the three schedules, one at a time (SnapshotPlugin-only users: benches/bench.rs:18-27,
  *      mod.rs:510-535 save_world / advance_frame / load_world helpers) -------------------- */
 BGR_API int bgr_save_world(bgr_engine* e, bgr_checksum* checksum_out);         /* world.run_schedule(SaveWorld) */

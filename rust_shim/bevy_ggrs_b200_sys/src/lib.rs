@@ -80,7 +80,7 @@ pub use change_feed::*;
 // the host edit record and the batched edits over a world batch
 mod host_edits;
 pub use host_edits::*;
-// the world checkpoint header too
+// the world checkpoint and checkpoint delta headers too
 mod checkpoint;
 pub use checkpoint::*;
 // world batches: a safe owner of a bgr_batch
@@ -195,6 +195,8 @@ extern "C" {
     pub fn bgr_desync_diff_remote(e: *mut bgr_engine, frame: i32, blob: *const c_void, bytes: usize, summary: *mut bgr_desync_summary, cols: *mut bgr_desync_column, cols_cap: u32, records: *mut bgr_desync_record, records_cap: u32, n_records: *mut u32, found: *mut i32) -> c_int;
     pub fn bgr_checkpoint_save(e: *mut bgr_engine, frame: i32, dst: *mut c_void, dst_cap: usize, bytes: *mut usize, found: *mut i32) -> c_int;
     pub fn bgr_checkpoint_restore(e: *mut bgr_engine, blob: *const c_void, bytes: usize) -> c_int;
+    pub fn bgr_checkpoint_save_delta(e: *mut bgr_engine, frame: i32, base_frame: i32, dst: *mut c_void, dst_cap: usize, bytes: *mut usize, found: *mut i32) -> c_int;
+    pub fn bgr_checkpoint_restore_delta(e: *mut bgr_engine, base: *const c_void, base_bytes: usize, delta: *const c_void, delta_bytes: usize) -> c_int;
     pub fn bgr_save_world(e: *mut bgr_engine, checksum_out: *mut bgr_checksum) -> c_int;
     pub fn bgr_load_world(e: *mut bgr_engine) -> c_int;
     pub fn bgr_advance_world(e: *mut bgr_engine, inputs: *const u8, status: *const u8, n_players: u32) -> c_int;
