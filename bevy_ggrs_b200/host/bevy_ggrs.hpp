@@ -440,7 +440,7 @@ public:
         std::vector<uint8_t> blob(bytes);  // an upper bound; the call reports the exact size
         check(bgr_checkpoint_save(engine_, frame, blob.data(), blob.size(), &bytes, &found));
         blob.resize(bytes);
-        put_resources(rs, &blob);
+        put_resources(rs == res_store_.end() ? Resources{} : rs->second, &blob);
         return blob;
     }
     // The engine's checkpoint delta of `frame` against `base_frame` (bgr_checkpoint_save_delta) followed by the App's
@@ -456,54 +456,37 @@ public:
         std::vector<uint8_t> blob(bytes);  // an upper bound; the call reports the exact size
         check(bgr_checkpoint_save_delta(engine_, frame, base_frame, blob.data(), blob.size(), &bytes, &found));
         blob.resize(bytes);
-        put_resources(rs, &blob);
+        put_resources(rs == res_store_.end() ? Resources{} : rs->second, &blob);
         return blob;
     }
     // ---- replays (bgr_replay; INTEGRATION.md "Replays") ----
-    // A recorded input log (inputs[j * n_players + h], n_players per frame) run from the current frame in one call; the
-    // checksums of the frames f with f % checksum_interval == 0, before they are advanced, in order.  The engine's
-    // world only: refused while rollback resources or host-side component tables are registered, whose per-frame
-    // schedules the engine does not run.
+    // A recorded input log (inputs[j * n_players + h], n_players per frame) run from the current frame f0 in one call.  It
+    // leaves the App as handle_requests of the stream [Save(f) if f % checksum_interval == 0, Advance(inputs[j])],
+    // f = f0 + j, would leave it, except that no snapshot is pushed: the engine re-simulates the world, and the App steps
+    // its rollback resources through the same frames on the host and XORs their checksum parts in.  The engine's ring is
+    // not touched, so neither is the App's resource store.  Resource systems run at frames the world is not at: they must
+    // not read the world.  Returns the checksums of the frames f with f % checksum_interval == 0, before they are
+    // advanced, in order.  Refused while host-side component tables are registered.  A refused replay changes nothing; a
+    // non-finite value at a checksum frame throws BGR_ERR_NON_FINITE after the whole log ran and the resources were
+    // committed.
     std::vector<std::pair<ggrs::Frame, unsigned __int128>> replay(const std::vector<uint8_t>& inputs, uint32_t n_players,
                                                                   uint32_t checksum_interval) {
-        finish();
-        if (!res_order_.empty() || !host_cols_.empty())
-            throw Panic(BGR_ERR_UNSUPPORTED, "replay runs the engine's world only: the App has rollback resources or host-side components");
-        if (n_players ? inputs.size() % n_players != 0 : !inputs.empty())
-            throw Panic(BGR_ERR_INVALID_ARGUMENT, "the input log is not a whole number of frames of n_players bytes");
-        struct bgr_replay r;
-        std::memset(&r, 0, sizeof r);
-        r.n_players = n_players;
-        r.n_frames = n_players ? uint32_t(inputs.size() / n_players) : 0u;
-        r.checksum_interval = checksum_interval;
-        r.inputs = inputs.data();
-        const int64_t f0 = rollback_frame_count(), n = r.n_frames, k = checksum_interval;
-        const size_t cap = k && f0 >= 0 ? size_t((f0 + n + k - 1) / k - (f0 + k - 1) / k) : 0u;
-        std::vector<bgr_checksum> cs(std::max<size_t>(cap, 1));
+        const struct bgr_replay r = replay_args(inputs, n_players, checksum_interval);
+        std::vector<bgr_checksum> cs(checksum_cap(r) + 1);
         uint32_t got = 0;
-        check(bgr_replay(engine_, &r, cs.data(), uint32_t(cap), &got));
-        std::vector<std::pair<ggrs::Frame, unsigned __int128>> out;
-        for (uint32_t i = 0; i < got && i < cap; ++i) out.emplace_back(cs[i].frame, (static_cast<unsigned __int128>(cs[i].hi) << 64) | cs[i].lo);
-        return out;
+        ResourceSteps steps = step_resources(r.n_frames, checksum_interval, 0);
+        commit_replay(steps, bgr_replay(engine_, &r, cs.data(), uint32_t(cs.size() - 1), &got));
+        return fold_checksums(cs, got, steps);
     }
 
-    // replay() that also writes a world checkpoint of every frame f with f % keyframe_interval == 0, before it is
-    // advanced, to `keyframes` as (frame, blob), in order (bgr_replay_keyframes; the engine's world only, as replay()).
-    // The buffers are sized by the call's query, which runs nothing.
+    // replay() that also writes an App checkpoint of every frame f with f % keyframe_interval == 0, before it is advanced,
+    // to `keyframes` as (frame, blob), in order (bgr_replay_keyframes): the engine's keyframe followed by the App's
+    // resources of the frame, byte for byte what checkpoint(f) writes on an App that ticked to f and saved it.  The
+    // buffers are sized by the call's query, which runs nothing.
     std::vector<std::pair<ggrs::Frame, unsigned __int128>> replay_keyframes(
         const std::vector<uint8_t>& inputs, uint32_t n_players, uint32_t checksum_interval, uint32_t keyframe_interval,
         std::vector<std::pair<ggrs::Frame, std::vector<uint8_t>>>* keyframes) {
-        finish();
-        if (!res_order_.empty() || !host_cols_.empty())
-            throw Panic(BGR_ERR_UNSUPPORTED, "replay runs the engine's world only: the App has rollback resources or host-side components");
-        if (n_players ? inputs.size() % n_players != 0 : !inputs.empty())
-            throw Panic(BGR_ERR_INVALID_ARGUMENT, "the input log is not a whole number of frames of n_players bytes");
-        struct bgr_replay r;
-        std::memset(&r, 0, sizeof r);
-        r.n_players = n_players;
-        r.n_frames = n_players ? uint32_t(inputs.size() / n_players) : 0u;
-        r.checksum_interval = checksum_interval;
-        r.inputs = inputs.data();
+        const struct bgr_replay r = replay_args(inputs, n_players, checksum_interval);
         struct bgr_keyframes kf;
         std::memset(&kf, 0, sizeof kf);
         kf.interval = keyframe_interval;
@@ -516,38 +499,28 @@ public:
         kf.dst_cap = bytes;
         kf.index = index.data();
         kf.index_cap = n_kf;
-        const int64_t f0 = rollback_frame_count(), n = r.n_frames, k = checksum_interval;
-        const size_t cap = k && f0 >= 0 ? size_t((f0 + n + k - 1) / k - (f0 + k - 1) / k) : 0u;
-        std::vector<bgr_checksum> cs(std::max<size_t>(cap, 1));
-        check(bgr_replay_keyframes(engine_, &r, &kf, cs.data(), uint32_t(cap), &got, &n_kf, &bytes));
+        std::vector<bgr_checksum> cs(checksum_cap(r) + 1);
+        ResourceSteps steps = step_resources(r.n_frames, checksum_interval, keyframe_interval);
+        commit_replay(steps, bgr_replay_keyframes(engine_, &r, &kf, cs.data(), uint32_t(cs.size() - 1), &got, &n_kf, &bytes));
         keyframes->clear();
-        for (uint32_t i = 0; i < n_kf && i < kf.index_cap; ++i)
+        for (uint32_t i = 0; i < n_kf && i < kf.index_cap; ++i) {
             keyframes->emplace_back(index[i].frame, std::vector<uint8_t>(dst.begin() + index[i].offset,
                                                                          dst.begin() + index[i].offset + index[i].bytes));
-        std::vector<std::pair<ggrs::Frame, unsigned __int128>> out;
-        for (uint32_t i = 0; i < got && i < cap; ++i) out.emplace_back(cs[i].frame, (static_cast<unsigned __int128>(cs[i].hi) << 64) | cs[i].lo);
-        return out;
+            auto snap = steps.snapshots.find(index[i].frame);
+            put_resources(snap == steps.snapshots.end() ? Resources{} : snap->second, &keyframes->back().second);
+        }
+        return fold_checksums(cs, got, steps);
     }
 
     // replay() that also samples rows [first_row, first_row + n_rows) at every frame f with f % trace_interval == 0,
-    // before it is advanced (bgr_replay_trace; the engine's world only, as replay()).  `samples` gets each sample's
-    // (frame, row count) and `records` n_samples * n_rows change-feed records over `fields`, sample-major.  The buffers are
-    // sized by the call's query, which runs nothing.
+    // before it is advanced (bgr_replay_trace).  `samples` gets each sample's (frame, row count) and `records`
+    // n_samples * n_rows change-feed records over `fields`, sample-major: engine fields only, while the checksums include
+    // the resources' parts.  The buffers are sized by the call's query, which runs nothing.
     std::vector<std::pair<ggrs::Frame, unsigned __int128>> replay_trace(
         const std::vector<uint8_t>& inputs, uint32_t n_players, uint32_t checksum_interval, uint32_t trace_interval,
         const std::vector<bgr_feed_field>& fields, uint32_t first_row, uint32_t n_rows, std::vector<bgr_trace_sample>* samples,
         std::vector<uint8_t>* records) {
-        finish();
-        if (!res_order_.empty() || !host_cols_.empty())
-            throw Panic(BGR_ERR_UNSUPPORTED, "replay runs the engine's world only: the App has rollback resources or host-side components");
-        if (n_players ? inputs.size() % n_players != 0 : !inputs.empty())
-            throw Panic(BGR_ERR_INVALID_ARGUMENT, "the input log is not a whole number of frames of n_players bytes");
-        struct bgr_replay r;
-        std::memset(&r, 0, sizeof r);
-        r.n_players = n_players;
-        r.n_frames = n_players ? uint32_t(inputs.size() / n_players) : 0u;
-        r.checksum_interval = checksum_interval;
-        r.inputs = inputs.data();
+        const struct bgr_replay r = replay_args(inputs, n_players, checksum_interval);
         struct bgr_trace t;
         std::memset(&t, 0, sizeof t);
         t.interval = trace_interval;
@@ -564,15 +537,12 @@ public:
         t.dst_cap = bytes;
         t.samples = samples->data();
         t.samples_cap = n_s;
-        const int64_t f0 = rollback_frame_count(), n = r.n_frames, k = checksum_interval;
-        const size_t cap = k && f0 >= 0 ? size_t((f0 + n + k - 1) / k - (f0 + k - 1) / k) : 0u;
-        std::vector<bgr_checksum> cs(std::max<size_t>(cap, 1));
-        check(bgr_replay_trace(engine_, &r, &t, cs.data(), uint32_t(cap), &got, &n_s, &bytes));
+        std::vector<bgr_checksum> cs(checksum_cap(r) + 1);
+        ResourceSteps steps = step_resources(r.n_frames, checksum_interval, 0);
+        commit_replay(steps, bgr_replay_trace(engine_, &r, &t, cs.data(), uint32_t(cs.size() - 1), &got, &n_s, &bytes));
         records->resize(bytes);
         samples->resize(n_s);
-        std::vector<std::pair<ggrs::Frame, unsigned __int128>> out;
-        for (uint32_t i = 0; i < got && i < cap; ++i) out.emplace_back(cs[i].frame, (static_cast<unsigned __int128>(cs[i].hi) << 64) | cs[i].lo);
-        return out;
+        return fold_checksums(cs, got, steps);
     }
 
     // Replaces the world and the App's resources with a checkpoint's.  The resource section is checked before the
@@ -614,6 +584,87 @@ private:
             throw Panic(BGR_ERR_UNSUPPORTED, "an App with host-side component tables cannot be checkpointed: their values are not plain bytes");
     }
     using Resources = std::map<std::type_index, std::vector<uint8_t>>;  // ResourceMap, declared below
+
+    // checks that the App can replay `inputs` from its current frame and describes the log
+    struct bgr_replay replay_args(const std::vector<uint8_t>& inputs, uint32_t n_players, uint32_t checksum_interval) {
+        finish();
+        if (!host_cols_.empty())
+            throw Panic(BGR_ERR_UNSUPPORTED, "an App with host-side component tables cannot replay: their rows follow spawns and "
+                                             "despawns a replay does not report frame by frame");
+        if (n_players ? inputs.size() % n_players != 0 : !inputs.empty())
+            throw Panic(BGR_ERR_INVALID_ARGUMENT, "the input log is not a whole number of frames of n_players bytes");
+        if (!res_order_.empty() && res_frame_ != rollback_frame_count())
+            throw Panic(BGR_ERR_STATE, "the App's resources are at frame " + std::to_string(res_frame_) + ", its world at frame " +
+                                           std::to_string(rollback_frame_count()));
+        struct bgr_replay r;
+        std::memset(&r, 0, sizeof r);
+        r.n_players = n_players;
+        r.n_frames = n_players ? uint32_t(inputs.size() / n_players) : 0u;
+        r.checksum_interval = checksum_interval;
+        r.inputs = inputs.data();
+        return r;
+    }
+    // the number of checksum frames of replay `r` from the current frame
+    size_t checksum_cap(const struct bgr_replay& r) {
+        const int64_t f0 = rollback_frame_count(), n = r.n_frames, k = r.checksum_interval;
+        return k && f0 >= 0 ? size_t((f0 + n + k - 1) / k - (f0 + k - 1) / k) : 0u;
+    }
+    // The resources of a replay stepped through its frames: the resources and frame before it, the resource parts of the
+    // checksum frames in order, and the resource snapshots of the keyframe frames.
+    struct ResourceSteps {
+        Resources before;
+        ggrs::Frame frame_before = 0;
+        std::vector<uint64_t> parts;
+        std::map<ggrs::Frame, Resources> snapshots;
+    };
+    // The request-free counterpart of handle_resource_requests: steps resources_ and res_frame_ through the n_frames of a
+    // replay as its Saves and Advances would, before the engine runs it.  At a checksum frame the resource part, at a
+    // keyframe frame the resource snapshot, then the resource systems.  A throw (an absent checksummed resource, a
+    // resource system) restores the resources first.
+    ResourceSteps step_resources(uint32_t n_frames, uint32_t checksum_interval, uint32_t keyframe_interval) {
+        ResourceSteps st;
+        if (res_order_.empty()) return st;
+        st.before = resources_;
+        st.frame_before = res_frame_;
+        try {
+            for (uint32_t j = 0; j < n_frames; ++j) {
+                if (checksum_interval && int64_t(res_frame_) % checksum_interval == 0) st.parts.push_back(resource_part());
+                if (keyframe_interval && int64_t(res_frame_) % keyframe_interval == 0) st.snapshots[res_frame_] = resources_;
+                res_frame_ += 1;
+                for (auto& f : res_systems_) f(*this);
+            }
+        } catch (...) {
+            resources_ = st.before;
+            res_frame_ = st.frame_before;
+            throw;
+        }
+        return st;
+    }
+    // Once the engine's replay call returned `rc`: BGR_OK or BGR_ERR_NON_FINITE (the log ran; thrown after this) keep the
+    // stepped resources, any other status restores them and throws.
+    void commit_replay(const ResourceSteps& st, int rc) {
+        if (rc != BGR_OK && rc != BGR_ERR_NON_FINITE && !res_order_.empty()) {
+            resources_ = st.before;
+            res_frame_ = st.frame_before;
+        }
+        check(rc);
+    }
+    // the first `got` checksums of a replay with the resource parts XORed in
+    static std::vector<std::pair<ggrs::Frame, unsigned __int128>> fold_checksums(std::vector<bgr_checksum>& cs, uint32_t got,
+                                                                                const ResourceSteps& st) {
+        std::vector<std::pair<ggrs::Frame, unsigned __int128>> out;
+        for (uint32_t i = 0; i < got && i + 1 < cs.size(); ++i) {
+            if (i < st.parts.size()) cs[i].lo ^= st.parts[i];
+            out.emplace_back(cs[i].frame, (static_cast<unsigned __int128>(cs[i].hi) << 64) | cs[i].lo);
+        }
+        return out;
+    }
+    // the XOR of the checksummed resources' seahashes (resource_checksum.rs:63-82: the resource must exist)
+    uint64_t resource_part() const {
+        uint64_t part = 0;
+        for (auto& t : res_checksummed_) { auto& b = resources_.at(t); part ^= bgr_seahash(b.data(), b.size()); }
+        return part;
+    }
     // the App's resource snapshot of `frame` (end(): none, and none is needed without registered resources)
     std::map<ggrs::Frame, Resources>::const_iterator resource_snapshot(ggrs::Frame frame) const {
         auto rs = res_store_.find(frame);
@@ -621,13 +672,13 @@ private:
             throw Panic(BGR_ERR_NO_SNAPSHOT, "the App holds no resource snapshot of frame " + std::to_string(frame));
         return rs;
     }
-    // appends the resource section of snapshot `rs` to `blob`
-    void put_resources(std::map<ggrs::Frame, Resources>::const_iterator rs, std::vector<uint8_t>* blob) const {
+    // appends the resource section of a resource snapshot to `blob`
+    void put_resources(const Resources& snap, std::vector<uint8_t>* blob) const {
         auto put = [blob](uint32_t v) { const uint8_t* p = reinterpret_cast<const uint8_t*>(&v); blob->insert(blob->end(), p, p + 4); };
         put(uint32_t(res_order_.size()));
         for (const auto& r : res_order_) {
-            auto it = rs->second.find(r.first);
-            const bool present = it != rs->second.end();
+            auto it = snap.find(r.first);
+            const bool present = it != snap.end();
             put(present ? 1u : 0u);
             put(present ? uint32_t(it->second.size()) : 0u);
             if (!present) continue;
@@ -776,8 +827,7 @@ private:
         for (const auto& r : requests) {
             if (r.kind == ggrs::GgrsRequest::SaveGameState) {
                 res_store_[res_frame_] = resources_;
-                uint64_t part = 0;
-                for (auto& t : res_checksummed_) { auto& b = resources_.at(t); part ^= bgr_seahash(b.data(), b.size()); }
+                const uint64_t part = resource_part();
                 if (k < last_checksums_.size()) last_checksums_[k].lo ^= part;
                 ++k;
             } else if (r.kind == ggrs::GgrsRequest::LoadGameState) {

@@ -27,7 +27,7 @@ from __future__ import annotations
 
 import struct
 from dataclasses import dataclass, field
-from typing import Callable, Dict, List, Optional, Sequence
+from typing import Callable, Dict, List, Optional, Sequence, Tuple
 
 from . import capi
 from .host_components import HostComponents
@@ -287,7 +287,7 @@ class App:
         blob = self.world.checkpoint(frame)
         if blob is None:
             return None
-        return blob + self._resource_section(frame)
+        return blob + self._resource_section(self._res_store.get(frame, {}))
 
     def checkpoint_delta(self, frame: int, base_frame: int) -> Optional[bytes]:
         """The engine's checkpoint delta of ``frame`` against ``base_frame`` followed by the App's resources of
@@ -298,14 +298,13 @@ class App:
         delta = self.world.checkpoint_delta(frame, base_frame)
         if delta is None:
             return None
-        return delta + self._resource_section(frame)
+        return delta + self._resource_section(self._res_store.get(frame, {}))
 
     def _check_resource_snapshot(self, frame: int) -> None:
         if self._res_registered and frame not in self._res_store:
             raise capi.BgrError(capi.BGR_ERR_NO_SNAPSHOT, f"the App holds no resource snapshot of frame {frame}")
 
-    def _resource_section(self, frame: int) -> bytes:
-        snap = self._res_store.get(frame, {})
+    def _resource_section(self, snap: Dict[str, Optional[bytes]]) -> bytes:
         out = [struct.pack("<I", len(self._res_registered))]
         for name in self._res_registered:
             v = snap.get(name)
@@ -374,6 +373,77 @@ class App:
         self.resources = {n: bytearray(v) for n, v in res.items() if v is not None}
         self._res_store = {frame: res} if self._res_registered else {}
         self._res_frame = frame
+
+    # ---- replays (INTEGRATION.md "Replays") ----
+    # App.replay(inputs, k) leaves the App as handle_requests of the stream [Save(f) if f % k == 0, Advance(inputs[j])],
+    # f = f0 + j, would leave it, except that no snapshot is pushed: the engine re-simulates the world, and the App steps
+    # its resources through the same frames on the host and XORs their checksum parts in.  The engine's ring is not
+    # touched, so neither is the App's resource store.  Resource systems run at frames the world is not at: they must not
+    # read the world.
+    def replay(self, inputs, checksum_interval: int = 0) -> List[tuple]:
+        """``Engine.replay`` of the App: [(frame, checksum), ...] of the checksum frames, with the resources' parts.  A
+        non-finite value at a checksum frame raises BgrError(BGR_ERR_NON_FINITE) after the whole log ran and the
+        resources were committed."""
+        steps = self._replay_steps(len(inputs), checksum_interval, 0)
+        checksums = self._replay_run(steps, lambda: self.world.replay(inputs, checksum_interval))
+        return steps.fold(checksums)
+
+    def replay_keyframes(self, inputs, checksum_interval: int, keyframe_interval: int) -> Tuple[List[tuple], List[tuple]]:
+        """``Engine.replay_keyframes`` of the App: (checksums, [(frame, blob), ...]), each blob the App checkpoint
+        ``checkpoint(frame)`` writes on an App that ticked to the frame and saved it."""
+        steps = self._replay_steps(len(inputs), checksum_interval, keyframe_interval)
+        checksums, kfs = self._replay_run(steps, lambda: self.world.replay_keyframes(inputs, checksum_interval,
+                                                                                        keyframe_interval))
+        return steps.fold(checksums), [(f, blob + self._resource_section(steps.snapshots.get(f, {}))) for f, blob in kfs]
+
+    def replay_trace(self, inputs, checksum_interval: int, trace_interval: int, fields, first_row: int, n_rows: int):
+        """``Engine.replay_trace`` of the App: (checksums, samples, records).  The records hold engine fields only; the
+        checksums include the resources' parts."""
+        steps = self._replay_steps(len(inputs), checksum_interval, 0)
+        checksums, samples, records = self._replay_run(steps, lambda: self.world.replay_trace(
+            inputs, checksum_interval, trace_interval, fields, first_row, n_rows))
+        return steps.fold(checksums), samples, records
+
+    def _replay_steps(self, n_frames: int, checksum_interval: int, keyframe_interval: int) -> "_ResourceSteps":
+        """The App's half of a replay of ``n_frames``, before the engine runs it.  Checks that the App can replay, then
+        steps the resources through the frames on a copy, as the tick's host half does for Saves and Advances: at a
+        checksum frame the resource part, at a keyframe frame the resource snapshot, then the resource systems."""
+        self._finish()
+        if self.host_components.columns:
+            raise capi.BgrError(capi.BGR_ERR_UNSUPPORTED, "an App with host-side component tables cannot replay: their rows "
+                                                          "follow spawns and despawns a replay does not report frame by frame")
+        steps = _ResourceSteps(n_frames, {}, [], {})
+        if not self._res_registered:
+            return steps
+        f0 = self.world.rollback_frame_count()
+        if self._res_frame != f0:
+            raise capi.BgrError(capi.BGR_ERR_STATE, f"the App's resources are at frame {self._res_frame}, its world at "
+                                                    f"frame {f0}")
+        res = steps.resources = {n: bytearray(v) for n, v in self.resources.items()}
+        for f in range(f0, f0 + n_frames):
+            if checksum_interval and f % checksum_interval == 0:
+                steps.parts.append(self._resource_part(res))
+            if keyframe_interval and f % keyframe_interval == 0:
+                steps.snapshots[f] = self._resource_snapshot(res)
+            self._run_resource_systems(res, f + 1)
+        return steps
+
+    def _replay_run(self, steps: "_ResourceSteps", run: Callable):
+        """``run()`` (the engine's replay) and then the commit of ``steps``.  BGR_ERR_NON_FINITE means the log ran: the
+        resources are committed before it is raised.  Any other refusal commits nothing."""
+        try:
+            out = run()
+        except capi.BgrError as e:
+            if e.status == capi.BGR_ERR_NON_FINITE:
+                self._replay_commit(steps)
+            raise
+        self._replay_commit(steps)
+        return out
+
+    def _replay_commit(self, steps: "_ResourceSteps") -> None:
+        if self._res_registered:
+            self.resources = steps.resources
+            self._res_frame += steps.n_frames
 
     # ---- frame resources ----
     def rollback_frame_count(self) -> int:
@@ -477,19 +547,12 @@ class App:
     # the same request vector, replayed on a few bytes of host state; parts are XORed into the engine's
     # checksum exactly like ChecksumPlugin::update folds every ChecksumPart (checksum.rs:88-99).
     def _handle_resource_requests(self, requests, checksums):
-        import ctypes as C
-        lib = capi.load_library()
         out, k = [], 0
         for r in requests:
-            if r.kind == SAVE:  # resource_snapshot.rs:65-73: Some(clone) or None
-                self._res_store[self._res_frame] = {n: (bytes(self.resources[n]) if n in self.resources else None)
-                                                    for n in self._res_registered}
-                part = 0
-                for name in self._res_checksummed:  # resource_checksum.rs:63-82 (the resource must exist)
-                    b = bytes(self.resources[name])
-                    part ^= lib.bgr_seahash(C.create_string_buffer(b, len(b)), len(b))
+            if r.kind == SAVE:
+                self._res_store[self._res_frame] = self._resource_snapshot(self.resources)
                 frame, cs = checksums[k]
-                out.append((frame, cs ^ part))
+                out.append((frame, cs ^ self._resource_part(self.resources)))
                 k += 1
             elif r.kind == LOAD:  # resource_snapshot.rs:77-93: update / insert / remove
                 self._res_frame = r.frame
@@ -500,14 +563,45 @@ class App:
                         self.resources[n] = bytearray(v)
             else:
                 self._res_frame += 1
-                for fn in self._res_systems:
-                    if fn.__code__.co_argcount >= 2:
-                        fn(self.resources, self._res_frame)   # (resources, RollbackFrameCount)
-                    else:
-                        fn(self.resources)
+                self._run_resource_systems(self.resources, self._res_frame)
         alive = set(self.world.snapshot_frames())
         self._res_store = {f: v for f, v in self._res_store.items() if f in alive}
         return out
+
+    def _resource_snapshot(self, resources) -> Dict[str, Optional[bytes]]:  # resource_snapshot.rs:65-73: Some(clone) or None
+        return {n: (bytes(resources[n]) if n in resources else None) for n in self._res_registered}
+
+    def _resource_part(self, resources) -> int:  # resource_checksum.rs:63-82 (the resource must exist)
+        import ctypes as C
+        lib = capi.load_library()
+        part = 0
+        for name in self._res_checksummed:
+            b = bytes(resources[name])
+            part ^= lib.bgr_seahash(C.create_string_buffer(b, len(b)), len(b))
+        return part
+
+    def _run_resource_systems(self, resources, frame: int) -> None:
+        for fn in self._res_systems:
+            if fn.__code__.co_argcount >= 2:
+                fn(resources, frame)   # (resources, RollbackFrameCount)
+            else:
+                fn(resources)
+
+
+@dataclass
+class _ResourceSteps:
+    """An App's resources stepped through the frames of a replay, on a copy: the resources after the last frame, the
+    resource parts of the checksum frames in order, and the resource snapshots of the keyframe frames."""
+    n_frames: int
+    resources: Dict[str, bytearray]
+    parts: List[int]
+    snapshots: Dict[int, Dict[str, Optional[bytes]]]
+
+    def fold(self, checksums: List[tuple]) -> List[tuple]:
+        """The engine's checksums of the replay with the resource parts XORed in (checksum.rs:88-99)."""
+        if not self.parts:
+            return checksums
+        return [(f, cs ^ p) for (f, cs), p in zip(checksums, self.parts)]
 
 
 def step_batch(apps: Sequence[App], batch) -> None:
@@ -534,3 +628,51 @@ def step_batch(apps: Sequence[App], batch) -> None:
         app.ticks += 1
     if failed is not None:
         raise failed
+
+
+# ---- world batches of replays: EngineBatch.replay* over many Apps, each App's resources stepped as App.replay* does ----
+def replay_batch(calls, batch) -> List[List[tuple]]:
+    """``App.replay`` of every listed App with ONE engine call: ``calls`` = [(app, inputs, checksum_interval), ...] over
+    Apps whose built engines are in ``batch`` (an ``EngineBatch``).  Returns each App's checksums in the same order."""
+    return [steps.fold(cs) for _, steps, (_, cs) in _replay_batch(calls, batch, batch.replay, 0)]
+
+
+def replay_keyframes_batch(calls, batch) -> List[Tuple[List[tuple], List[tuple]]]:
+    """``App.replay_keyframes`` of every listed App with ONE engine call: ``calls`` = [(app, inputs, checksum_interval,
+    keyframe_interval), ...].  Returns each App's (checksums, [(frame, App checkpoint), ...]) in the same order."""
+    return [(steps.fold(cs), [(f, blob + app._resource_section(steps.snapshots.get(f, {}))) for f, blob in kfs])
+            for app, steps, (_, cs, kfs) in _replay_batch(calls, batch, batch.replay_keyframes, 3)]
+
+
+def replay_trace_batch(calls, batch, fields):
+    """``App.replay_trace`` of every listed App over one field list with ONE engine call: ``calls`` = [(app, inputs,
+    checksum_interval, trace_interval, first_row, n_rows), ...].  Returns each App's (checksums, samples, records) in the
+    same order."""
+    return [(steps.fold(cs), samples, records)
+            for _, steps, (_, cs, samples, records) in _replay_batch(calls, batch, lambda c: batch.replay_trace(c, fields), 0)]
+
+
+def _replay_batch(calls, batch, run: Callable, keyframe_at: int):
+    """Steps the resources of every App in ``calls`` (entries (app, inputs, checksum_interval, ...); the keyframe interval
+    at index ``keyframe_at``, 0: none) on copies, runs ``run`` (the EngineBatch call, on the same entries with each App
+    replaced by its world's index) and commits every App whose world ran.  A refused call commits nothing.  A world that
+    reported BGR_ERR_NON_FINITE raises once every App has committed.  Returns [(app, steps, the world's result), ...]."""
+    calls = [tuple(c) for c in calls]
+    index = {id(e): i for i, e in enumerate(batch.engines)}
+    worlds = []
+    for c in calls:
+        if id(c[0].world) not in index:
+            raise capi.BgrError(capi.BGR_ERR_INVALID_ARGUMENT, "an App's engine is not a member of the batch")
+        worlds.append(index[id(c[0].world)])
+    steps = [c[0]._replay_steps(len(c[1]), c[2], c[keyframe_at] if keyframe_at else 0) for c in calls]
+    results = run([(w,) + c[1:] for w, c in zip(worlds, calls)])
+    failed = None
+    for w, c, st, res in zip(worlds, calls, steps, results):
+        if res[0] in (capi.BGR_OK, capi.BGR_ERR_NON_FINITE):
+            c[0]._replay_commit(st)
+        if res[0] != capi.BGR_OK:
+            failed = failed or capi.BgrError(res[0], f"world {w}: " + ("Hashing is not stable for NaN f32 values."
+                                                                       if res[0] == capi.BGR_ERR_NON_FINITE else f"status {res[0]}"))
+    if failed is not None:
+        raise failed
+    return [(c[0], st, res) for c, st, res in zip(calls, steps, results)]
